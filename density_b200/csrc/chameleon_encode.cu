@@ -410,8 +410,8 @@ cham_flag_pass(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles_
 //      successor stores the bucket's final fingerprint. First touches of a bucket inside the run go to the unresolved list.  (barrier)
 // Clean buckets are never written and every dirty bucket is written once in D, so the dictionary after D is the sequential one.
 // Phases A-D do the same work in every warp whatever the data; an overflow mailbox that would need a 17th entry (~20 dirty
-// members of one bucket inside one tile that are not one run) sends the tile to f6_replay: the in-order replay of the dirty members
-// by one warp (exact for any input, slow; 1 % of the tiles of the bench text).
+// members of one bucket inside one tile that are not one run) sends the tile to f6_replay: the in-order replay of the dirty members,
+// one bucket class per warp (exact for any input; on text, the first three tiles of every run, whose dictionary starts empty).
 // ------------------------------------------------------------------------------------------------------
 constexpr int F6_THREADS = 512, F6_QPT = 8;           // 16 warps, 8 quads per thread: one tile = TILE_Q quads
 constexpr int F6_NW = F6_THREADS / 32, F6_WQ = 32 * F6_QPT;   // warps; quads (= record region size) per warp
@@ -433,7 +433,7 @@ struct Flag6Smem {
     uint2 rec[TILE_Q];            // warp w: records [128 w, 128 w + cnt[w]) in stream order. x = hash | fp << 16, y see above
     union {
         uint16_t mb[F6_MB_SLOTS][F6_MB_CAP];
-        uint2 dense[TILE_Q];      // fallback only (the mailboxes are void then): the same records, dense
+        uint2 stage[F6_NW][64];   // fallback only (the mailboxes are void then): per-warp staging of the replayed records
     };
     uint32_t mbcnt[2][F6_MB_SLOTS / 4];   // entry counts, 8 bits per slot; double buffered (the idle half is cleared during the tile)
     __align__(16) uint32_t sec[F6_SEC_SLOTS][F6_SEC_CAP];
@@ -458,57 +458,78 @@ __device__ __forceinline__ void f6_append_unres(bool pred, uint32_t qidx_in_run,
     }
 }
 
-// Fallback: in-order replay of the tile's dirty members by one warp. Copies the regions into one dense, stream-ordered list and
-// restores the pre-tile value of every dirty bucket (each record carries it), then walks the list 32 records per step
-// (match_any for records of the same bucket inside a step).
-__device__ __noinline__ void f6_replay(Flag6Smem& S, uint32_t buf, uint32_t run_q0, uint2* __restrict__ unres_run) {
+// Fallback: in-order replay of the tile's dirty members, exact for any input. Buckets of different classes (hash >> 12) never interact,
+// so warp w replays the members of class w: every warp first restores the pre-tile value of the dirty buckets of its own region (each
+// record carries it); then each warp reads all regions in stream order, stages the records of its class (ballot + popc) and walks them
+// 32 per step (match_any for members of the same bucket inside a step). All threads of the CTA call.
+static_assert(F6_NW == 16, "one warp per bucket class hash >> 12");
+__device__ __forceinline__ void f6_replay_step(Flag6Smem& S, const uint2* stage, uint32_t n, uint32_t buf, uint32_t run_q0,
+                                               uint2* __restrict__ unres_run) {
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t c = lane < (uint32_t)F6_NW ? S.cnt[lane] : 0u;
-    uint32_t incl = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
-    const uint32_t excl = incl - c;
-    const uint32_t n = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    #pragma unroll 1
-    for (uint32_t i0 = 0; i0 < n; i0 += 32) {
-        const uint32_t i = i0 + lane;
-        uint32_t w = 0;     // number of regions that end at or before i == the region that holds dense index i
-#pragma unroll
-        for (int b = 16; b >= 1; b >>= 1) { const uint32_t t = __shfl_sync(0xFFFFFFFFu, incl, (w + b - 1) & 31); if (t <= i) w += b; }
-        const uint32_t e = __shfl_sync(0xFFFFFFFFu, excl, w & 31);
-        if (i < n) {
-            const uint2 r = S.rec[w * F6_WQ + (i - e)];
-            S.dense[i] = r;
+    const bool valid = lane < n;
+    uint2 r = make_uint2(0, 0);
+    if (valid) r = stage[lane];
+    const uint32_t hh = r.x & 0xFFFFu, ff = r.x >> 16, pos = r.y & 0xFFFu;
+    uint32_t cur = 0;
+    if (valid) cur = S.tab[hh];
+    const uint32_t grp = __match_any_sync(0xFFFFFFFFu, valid ? hh : 0x10000u + lane);
+    const uint32_t lower = grp & lanemask_lt();
+    const uint32_t fprev = __shfl_sync(0xFFFFFFFFu, ff, lower ? 31 - __clz(lower) : 0);
+    bool touched = true, hit;
+    if (lower) hit = fprev == ff;
+    else {
+        if (cur == 0) touched = bit_test(S.vbit, hh);
+        hit = touched && cur == ff;
+    }
+    if (valid && (grp & lanemask_gt()) == 0) {
+        S.tab[hh] = (uint16_t)ff;
+        if (ff == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
+    }
+    if (valid && hit) atomicOr(&S.sigw[buf][pos >> 5], 1u << (pos & 31));
+    f6_append_unres(valid && !touched, run_q0 + pos, r.x, &S.unres_count, unres_run);
+    __syncwarp();
+}
+
+__device__ __noinline__ void f6_replay(Flag6Smem& S, uint32_t buf, uint32_t run_q0, uint2* __restrict__ unres_run) {
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    {
+        const uint32_t n = S.cnt[warp];
+        const uint2* __restrict__ myrec = S.rec + warp * F6_WQ;
+        #pragma unroll 1
+        for (uint32_t i = lane; i < n; i += 32) {
+            const uint2 r = myrec[i];
             S.tab[r.x & 0xFFFFu] = (uint16_t)(r.y >> 16);
         }
     }
-    __syncwarp();
+    __syncthreads();   // every dirty bucket holds its pre-tile value
+    uint2* __restrict__ stage = S.stage[warp];   // < 32 staged records carried between steps + one region step
+    uint32_t ns = 0;
     #pragma unroll 1
-    for (uint32_t i0 = 0; i0 < n; i0 += 32) {
-        const uint32_t i = i0 + lane;
-        const bool valid = i < n;
-        uint2 r = make_uint2(0, 0);
-        if (valid) r = S.dense[i];
-        const uint32_t hh = r.x & 0xFFFFu, ff = r.x >> 16, pos = r.y & 0xFFFu;
-        uint32_t cur = 0;
-        if (valid) cur = S.tab[hh];
-        const uint32_t grp = __match_any_sync(0xFFFFFFFFu, valid ? hh : 0x10000u + lane);
-        const uint32_t lower = grp & lanemask_lt();
-        const uint32_t fprev = __shfl_sync(0xFFFFFFFFu, ff, lower ? 31 - __clz(lower) : 0);
-        bool touched = true, hit;
-        if (lower) hit = fprev == ff;
-        else {
-            if (cur == 0) touched = bit_test(S.vbit, hh);
-            hit = touched && cur == ff;
+    for (uint32_t w = 0; w < (uint32_t)F6_NW; ++w) {
+        const uint32_t n = S.cnt[w];
+        const uint2* __restrict__ rg = S.rec + w * F6_WQ;
+        #pragma unroll 1
+        for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+            const uint32_t i = i0 + lane;
+            uint2 r = make_uint2(0, 0);
+            if (i < n) r = rg[i];
+            const bool mine = i < n && ((r.x & 0xFFFFu) >> 12) == warp;
+            const uint32_t m = __ballot_sync(0xFFFFFFFFu, mine);
+            if (mine) stage[ns + __popc(m & lanemask_lt())] = r;
+            ns += __popc(m);
+            if (ns >= 32) {
+                __syncwarp();
+                f6_replay_step(S, stage, 32, buf, run_q0, unres_run);
+                const uint2 rest = stage[32 + lane];
+                __syncwarp();
+                if (lane < ns - 32) stage[lane] = rest;
+                ns -= 32;
+                __syncwarp();
+            }
         }
-        if (valid && (grp & lanemask_gt()) == 0) {
-            S.tab[hh] = (uint16_t)ff;
-            if (ff == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
-        }
-        if (valid && hit) atomicOr(&S.sigw[buf][pos >> 5], 1u << (pos & 31));
-        f6_append_unres(valid && !touched, run_q0 + pos, r.x, &S.unres_count, unres_run);
-        __syncwarp();
     }
+    __syncwarp();
+    if (ns) f6_replay_step(S, stage, ns, buf, run_q0, unres_run);
 }
 
 // One tile. GENERIC: the tile is partial or has copy-mode blocks (`validmask` bit j: my sub-row j quad takes part).
@@ -579,7 +600,7 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
     uint2 r0 = make_uint2(0, 0);
     bool drop0 = false;
     {
-        uint32_t carry_x = 0xFFFFFFFFu, carry_pos = 0xFFFFFFFFu;   // record before lane 0's (previous step's lane 31)
+        uint32_t carry_x = 0, carry_pos = 0;   // record before lane 0's (previous step's lane 31); record 0 has none
         #pragma unroll 1
         for (uint32_t i0 = 0; i0 < base; i0 += 32) {
             const uint32_t i = i0 + lane;
@@ -592,7 +613,7 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
             }
             uint32_t px = __shfl_up_sync(0xFFFFFFFFu, r.x, 1), ppos = __shfl_up_sync(0xFFFFFFFFu, r.y & 0xFFFu, 1);
             if (lane == 0) { px = carry_x; ppos = carry_pos; }
-            const bool drop = valid && px == r.x && ppos + 1 == (r.y & 0xFFFu);
+            const bool drop = valid && i != 0 && px == r.x && ppos + 1 == (r.y & 0xFFFu);
             carry_x = __shfl_sync(0xFFFFFFFFu, r.x, 31); carry_pos = __shfl_sync(0xFFFFFFFFu, r.y & 0xFFFu, 31);
             if (i0 == 0) { r0 = r; drop0 = drop; }
             if (drop) {
@@ -616,10 +637,10 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
     __syncthreads();   // S3: records, counts, clean flags and mailboxes complete; nobody reads the published values any more
     F6_PH(2)
 #ifdef DNS_PHASE_TIMING
-    if (threadIdx.x == 0 && blockIdx.x == 77) { g_f6_ph[6] += S.overflow; uint32_t tot = 0; for (int w = 0; w < 32; ++w) tot += S.cnt[w]; g_f6_ph[7] += tot; }
+    if (threadIdx.x == 0 && blockIdx.x == 77) { g_f6_ph[6] += S.overflow; uint32_t tot = 0; for (int w = 0; w < F6_NW; ++w) tot += S.cnt[w]; g_f6_ph[7] += tot; }
 #endif
     if (S.overflow) {
-        if (warp == 0) f6_replay(S, buf, run_q0, unres_run);
+        f6_replay(S, buf, run_q0, unres_run);
     } else {
         // ---- D
         #pragma unroll 1

@@ -5,9 +5,10 @@ unresolved list). Checked against the in-order dictionary walk of chameleon.rs:8
   A  every quad reads old = tab[h]; misser <=> old != f (fingerprint 0 on a never-touched bucket: misser too)
   B  missers store f — racy: ANY one of the missers of a bucket may win (the model picks a pseudo-random one)
   C  hit members read again: unchanged -> flag 1. Dirty members = missers + hit members whose bucket changed; records in stream
-     order; a record equal to the record before it whose quad is also right before it in the stream is dropped (flag 1);
-     the others go to the mailbox of their slot (low 12 hash bits, 4 entries) or, from the fifth on, to one of 64 overflow
-     mailboxes (16 entries); a 17th entry => the whole tile is replayed in order instead (`replay`)
+     order; a record equal to the record before it whose quad is also right before it in the stream, in the same 256-quad
+     region (the records of one warp), is dropped (flag 1); the others go to the mailbox of their slot (low 12 hash bits,
+     4 entries) or, from the fifth on, to one of 64 overflow mailboxes (16 entries); a 17th entry => the whole tile is replayed
+     in order instead (`replay`)
   D  per record: predecessor = entry of my bucket with the largest smaller record index -> flag = its fingerprint == mine; none ->
      touched ? pre-tile fingerprint == mine : unresolved; the member without a successor stores the bucket's final fingerprint
 """
@@ -16,6 +17,7 @@ import numpy as np
 M = 0x9D6EF916
 TILE = 4096
 MB_SLOTS, MB_CAP, SEC_SLOTS, SEC_CAP = 4096, 4, 64, 16
+REGION = 256                                   # quads per warp: a warp compacts and deposits its own records
 
 
 def hf(q):
@@ -62,7 +64,7 @@ def flag_pass(q, seed=1, stats=None):
         dropped = np.zeros(rec.size, bool)
         for k in range(1, rec.size):
             i, j = rec[k], rec[k - 1]
-            if i == j + 1 and hs[i] == hs[j] and fs[i] == fs[j]:
+            if i == j + 1 and i // REGION == j // REGION and hs[i] == hs[j] and fs[i] == fs[j]:
                 dropped[k] = True
                 flags[i] = 1
         mb, sec, overflow = {}, {}, False

@@ -85,6 +85,7 @@ def flag_pass(q, seed=1, stats=None):
             stats["tiles"] = stats.get("tiles", 0) + 1
             stats["overflow"] = stats.get("overflow", 0) + int(overflow)
             stats["dirty"] = stats.get("dirty", 0) + int(rec.size)
+            stats.setdefault("tile_overflow", []).append(overflow)   # per tile, in stream order
         if overflow:
             # replay: restore the pre-tile values of the dirty buckets, walk the dirty members in stream order
             cur, cur_t = tab, touched
@@ -190,6 +191,7 @@ def decode_pass(is_plain, payload, seed=1, stats=None):
         if stats is not None:
             stats["overflow"] = stats.get("overflow", 0) + int(overflow)
             stats["suspects"] = stats.get("suspects", 0) + len(suspects)
+            stats.setdefault("tile_overflow", []).append(overflow)
         if overflow:                                                # d7_replay: records in order, "written so far in this tile" bitmap
             seen = {}
             for i in recs:

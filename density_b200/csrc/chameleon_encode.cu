@@ -734,9 +734,14 @@ cham_flag_pass6(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles
         if (tid == 0) { S.unres_count = 0; S.overflow = 0; }
     }
     __syncthreads();
-    uint32_t nxt[F6_QPT];   // register double buffer of the tile's quads
+    // Register ring of the next two tiles' quads: a tile's loads are issued two tiles before it runs, so they have two tiles' time to
+    // arrive (every warp of the CTA issues its loads in the same burst, right after the tile's last barrier).
+    uint32_t nxt[F6_QPT], nxt2[F6_QPT];
 #pragma unroll
-    for (int j = 0; j < F6_QPT; ++j) nxt[j] = (pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + pos0 + 32 * j) : 0u;
+    for (int j = 0; j < F6_QPT; ++j) {
+        nxt[j] = (pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + pos0 + 32 * j) : 0u;
+        nxt2[j] = (TILE_Q + pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + TILE_Q + pos0 + 32 * j) : 0u;
+    }
     #pragma unroll 1
     for (uint32_t lt = 0; lt < ntile_run; ++lt) {
         uint32_t q[F6_QPT];
@@ -744,16 +749,16 @@ cham_flag_pass6(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles
         const uint32_t left = run_q0 < run_quads ? run_quads - run_q0 : 0u;
         const uint32_t buf = lt & 1u;
 #pragma unroll
-        for (int j = 0; j < F6_QPT; ++j) q[j] = nxt[j];
+        for (int j = 0; j < F6_QPT; ++j) { q[j] = nxt[j]; nxt[j] = nxt2[j]; }
         {
-            const uint32_t nleft = left > (uint32_t)TILE_Q ? left - TILE_Q : 0u;
-            const uint32_t* __restrict__ np = rin + run_q0 + TILE_Q + pos0;
+            const uint32_t nleft = left > 2u * TILE_Q ? left - 2u * TILE_Q : 0u;
+            const uint32_t* __restrict__ np = rin + run_q0 + 2 * TILE_Q + pos0;
             if (nleft >= (uint32_t)TILE_Q) {
 #pragma unroll
-                for (int j = 0; j < F6_QPT; ++j) nxt[j] = ld_stream_u32(np + 32 * j);
+                for (int j = 0; j < F6_QPT; ++j) nxt2[j] = ld_stream_u32(np + 32 * j);
             } else {
 #pragma unroll
-                for (int j = 0; j < F6_QPT; ++j) nxt[j] = (pos0 + 32 * j < nleft) ? ld_stream_u32(np + 32 * j) : 0u;
+                for (int j = 0; j < F6_QPT; ++j) nxt2[j] = (pos0 + 32 * j < nleft) ? ld_stream_u32(np + 32 * j) : 0u;
             }
         }
         if (left >= (uint32_t)TILE_Q && !rcm) {

@@ -11,6 +11,15 @@ unresolved list). Checked against the in-order dictionary walk of chameleon.rs:8
      in order instead (`replay`)
   D  per record: predecessor = entry of my bucket with the largest smaller record index -> flag = its fingerprint == mine; none ->
      touched ? pre-tile fingerprint == mine : unresolved; the member without a successor stores the bucket's final fingerprint
+
+`overlap=True` models a three-barrier tile that was built and measured slower (DESIGN.md section 9): when the tile before this
+one exists and did not overflow, phase A of this tile runs during that tile's phase D, while D writes the dictionary. A bucket with an
+entry in the previous tile's mailboxes is *stale*: D is writing it. Its value after D is the fingerprint of the bucket's entry with
+the largest record index (D writes exactly that), so a stale member takes its pre-tile value, touched, from the mailbox and the
+record; both are read-only during D. Every other bucket is written neither by B nor by D of the previous tile, so the dictionary
+read during D is its pre-tile value. The model gives the other buckets the dictionary as it stood when D began: a bucket that D did
+write would read a wrong value there. After the first tile of the run and after an overflow tile, A runs after the barrier. The
+dirty members, the mailboxes and the overflow tiles are those of the four-barrier tile (`overlap=False`, the kernel).
 """
 import numpy as np
 
@@ -40,17 +49,42 @@ def reference_flags(q):
     return out, tab
 
 
-def flag_pass(q, seed=1, stats=None):
+def _mailbox_last(mb, sec, rec, hs, b):
+    """Record index of the last member of bucket b in a tile's mailboxes (the one D lets write the bucket), or None."""
+    slot = b & (MB_SLOTS - 1)
+    cand = list(mb.get(slot, []))
+    if len(cand) >= MB_CAP:
+        cand += sec.get(slot & (SEC_SLOTS - 1), [])
+    same = [c for c in cand if int(hs[rec[c]]) == b]
+    return max(same) if same else None
+
+
+def flag_pass(q, seed=1, stats=None, overlap=False):
     rng = np.random.default_rng(seed)
     h, f = hf(q)
     tab = np.zeros(65536, np.int64)            # fingerprints
     touched = np.zeros(65536, bool)            # tab != 0 or the touched bit
     out = np.zeros(q.size, np.uint8)
+    early = None                               # A of this tile ran during the previous tile's D: what it could read there
     for t0 in range(0, q.size, TILE):
         hs, fs = h[t0:t0 + TILE], f[t0:t0 + TILE]
         n = hs.size
-        old = tab[hs].copy()
-        old_t = touched[hs].copy()
+        if early is None:
+            old = tab[hs].copy()
+            old_t = touched[hs].copy()
+            nstale = 0
+        else:
+            tab_d, touched_d, pmb, psec, prec, phs, pfs = early
+            old = tab_d[hs].copy()
+            old_t = touched_d[hs].copy()
+            nstale = 0
+            for b in np.unique(hs):
+                k = _mailbox_last(pmb, psec, prec, phs, int(b))
+                if k is not None:                  # stale: the previous D writes this bucket; its last record says with what
+                    sel = hs == b
+                    old[sel] = pfs[prec[k]]
+                    old_t[sel] = True
+                    nstale += int(sel.sum())
         miss = (old != fs) | ((fs == 0) & (old == 0) & ~old_t)
         # B: racy publish
         pub = tab.copy()
@@ -85,7 +119,10 @@ def flag_pass(q, seed=1, stats=None):
             stats["tiles"] = stats.get("tiles", 0) + 1
             stats["overflow"] = stats.get("overflow", 0) + int(overflow)
             stats["dirty"] = stats.get("dirty", 0) + int(rec.size)
+            stats["early"] = stats.get("early", 0) + int(early is not None)
+            stats["stale"] = stats.get("stale", 0) + nstale
             stats.setdefault("tile_overflow", []).append(overflow)   # per tile, in stream order
+        early = None
         if overflow:
             # replay: restore the pre-tile values of the dirty buckets, walk the dirty members in stream order
             cur, cur_t = tab, touched
@@ -101,6 +138,8 @@ def flag_pass(q, seed=1, stats=None):
                 cur[b] = v
                 cur_t[b] = True
         else:
+            if overlap:                         # the next tile's A sees the dictionary as D begins, and these mailboxes
+                early = (pub.copy(), touched.copy(), mb, sec, rec, hs, fs)
             newtab = pub                        # clean buckets: unchanged; dirty buckets: written once below
             for k in range(rec.size):
                 if dropped[k]:
@@ -218,3 +257,24 @@ def decode_pass(is_plain, payload, seed=1, stats=None):
                     res[i] = int(pay[recs[max(lower)]]) if lower else (pre[i] if pre[i] is not None else 0)
         out[t0:t0 + n] = res
     return out, dic
+
+
+if __name__ == "__main__":
+    # Records per tile and overflow tiles per run of the flag pass on the bench text (1 GiB of synth_text, the runs of an H100),
+    # with the four-barrier tile and with the three-barrier one: `python -m tools.proto_tile_protocol_v6 [runs...]`
+    import sys
+    from density_b200 import synth
+    nbytes, nsm = 1 << 30, 132
+    ntiles = nbytes // (TILE * 4)
+    nruns = min(max(ntiles // 16, 1), nsm)
+    for r in [int(a) for a in sys.argv[1:]] or [0, 77]:
+        t0, t1 = r * ntiles // nruns, (r + 1) * ntiles // nruns
+        data = synth.synth_text(t1 * TILE * 4).numpy()[t0 * TILE * 4:]
+        q = data.view(np.uint32)
+        want, _ = reference_flags(q)
+        for overlap in (False, True):
+            st = {}
+            got, _, _ = flag_pass(q, seed=1, stats=st, overlap=overlap)
+            assert (got == want).all()
+            print(f"run {r} ({st['tiles']} tiles) {'three' if overlap else 'four'} barriers: records/tile {st['dirty'] / st['tiles']:.1f}, "
+                  f"stale members/tile {st['stale'] / st['tiles']:.1f}, tiles with an early A {st['early']}, overflow tiles {st['overflow']}", flush=True)

@@ -29,6 +29,13 @@ _SIGS = {
     "density_b200_encode_sharded": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p,
                                                    ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, ctypes.c_void_p]),
     "density_b200_sharded_profile": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float)]),
+    "density_b200_decode_shard_create": (ctypes.c_void_p, []),
+    "density_b200_decode_shard_destroy": (None, [ctypes.c_void_p]),
+    "density_b200_decode_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
+                                                        ctypes.c_void_p]),
+    "density_b200_decode_shard_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_u8p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_codec_create": (ctypes.c_void_p, [ctypes.c_int]),
     "density_b200_codec_destroy": (None, [ctypes.c_void_p]),
     "density_b200_codec_clear_state": (ctypes.c_int, [ctypes.c_void_p]),

@@ -666,6 +666,69 @@ int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in,
     return DENSITY_B200_OK;
 }
 
+// ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
+struct density_b200_decode_shard {
+    DevBuf ws;
+    const uint8_t* d_in = nullptr;
+    size_t n = 0, cap = 0;
+    int is_last = 1;
+    int num_sms = 0;
+    bool phase1_done = false;
+};
+
+density_b200_decode_shard* density_b200_decode_shard_create(void) {
+    g_last_error.clear();
+    DeviceCtx* c = current_ctx();
+    if (!c) return nullptr;
+    density_b200_decode_shard* s = new density_b200_decode_shard();
+    s->num_sms = c->num_sms;
+    return s;
+}
+void density_b200_decode_shard_destroy(density_b200_decode_shard* s) {
+    if (!s) return;
+    s->ws.release();
+    delete s;
+}
+int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                     uint32_t* d_table_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_in) & 1) { set_error("d_in must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase1_done = false;
+    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    uint64_t launches = 0;
+    if (n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
+    else e = cham_decode_phase1(d_in, n, cap, s->ws.p, s->num_sms, d_table_out, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("decode shard phase1", e); return DENSITY_B200_ECUDA; }
+    s->phase1_done = true;
+    return DENSITY_B200_OK;
+}
+int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
+                                     uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s || !s->phase1_done) { set_error("decode_shard_phase2: phase1 not done"); return DENSITY_B200_EARG; }
+    if ((!d_out && s->cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_out) & 3) { set_error("d_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    cudaError_t e;
+    if (s->n == 0) {
+        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
+    } else {
+        e = cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches);
+        if (e == cudaSuccess) e = cham_decode_seam_words(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, s->is_last, d_out_size, d_seam8, st, &launches);
+    }
+    g_launches += launches;
+    s->phase1_done = false;     // the decode pass overwrites the run tables: one phase 2 per phase 1
+    if (e != cudaSuccess) { set_error("decode shard phase2", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon encode across the GPUs of one box (SURVEY §8e): one process per GPU, NCCL over NVLink ---------------------
 // NCCL is resolved at run time from the library that is already in the process (torch loads its bundled libnccl.so.2), else the
 // system one: no link-time dependency, one NCCL per process.
@@ -719,6 +782,7 @@ struct density_b200_sharded {
     int rank = 0, world = 1, num_sms = 0;
     nccl_comm_t comm = nullptr;
     DevBuf ws, aux;                 // aux: gathered tables [world][65536] + carry [65536] + seam words [world][8] + offsets [world + 1] + size
+    DevBuf dws;                     // decode workspace (density_b200_decode_sharded), apart from the encoder's
     ChamLayout L{};
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     cudaEvent_t ev[6] = {};         // stage timing of the last call: start, flag pass, exchange, phase 2 up to emit, emit, gather
@@ -756,10 +820,23 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-    h->ws.release(); h->aux.release();
+    h->ws.release(); h->aux.release(); h->dws.release();
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
     delete h;
+}
+
+// the exchange buffers of a handle, shared by encode and decode
+struct ShardedAux { uint32_t *tables, *carry, *words; uint64_t* offsets; };
+static cudaError_t sharded_aux(density_b200_sharded* h, cudaStream_t st, ShardedAux* x) {
+    const size_t W = (size_t)h->world;
+    const size_t aux_tables = W * 65536 * sizeof(uint32_t), aux_carry = 65536 * sizeof(uint32_t), aux_words = W * 8 * sizeof(uint32_t);
+    const cudaError_t e = h->aux.ensure(aux_tables + aux_carry + aux_words + (W + 2) * sizeof(uint64_t) + 256, st);
+    x->tables = reinterpret_cast<uint32_t*>(h->aux.p);
+    x->carry = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables);
+    x->words = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables + aux_carry);
+    x->offsets = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words);
+    return e;
 }
 
 // One bit-exact stream cut across `world` GPUs; this rank's shard is d_in[0 .. n) (n % 256 == 0 except on the last rank).
@@ -776,14 +853,14 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
     NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
     const size_t W = (size_t)h->world;
-    const size_t aux_tables = W * 65536 * sizeof(uint32_t), aux_carry = 65536 * sizeof(uint32_t), aux_words = W * 8 * sizeof(uint32_t);
     cudaError_t e = h->ws.ensure(cham_workspace_bytes(n, h->num_sms, &h->L), st);
-    if (e == cudaSuccess) e = h->aux.ensure(aux_tables + aux_carry + aux_words + (W + 2) * sizeof(uint64_t) + 256, st);
+    ShardedAux x;
+    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* d_tables = reinterpret_cast<uint32_t*>(h->aux.p);
-    uint32_t* d_carry = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables);
-    uint32_t* d_words = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables + aux_carry);
-    uint64_t* d_offsets = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words);
+    uint32_t* d_tables = x.tables;
+    uint32_t* d_carry = x.carry;
+    uint32_t* d_words = x.words;
+    uint64_t* d_offsets = x.offsets;
     const uint32_t nruns = cham_pick_runs(n, h->num_sms);
     uint64_t launches = 0;
     cudaEventRecord(h->ev[0], st);
@@ -837,6 +914,42 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     cudaEventRecord(h->ev[5], st);
     h->timed = true;
     g_launches += launches;
+    return DENSITY_B200_OK;
+}
+
+// The inverse of density_b200_encode_sharded without a gather: this rank's piece d_in[0 .. n) decodes to the shard it was encoded from.
+// Everything is enqueued on `stream`; nothing blocks.
+int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    ShardedAux x;
+    cudaError_t e = h->dws.ensure(cham_decode_workspace_bytes(n, cap, h->num_sms), st);
+    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint32_t* my_table = x.tables + (size_t)h->rank * 65536;
+    uint32_t* my_words = x.words + 8 * h->rank;
+    uint64_t launches = 0;
+    // phase 1: boundaries and writer pass need no carry-in; the piece's table (runs + tail) lands in my slot of the gather buffer
+    if (n) e = cham_decode_phase1(d_in, n, cap, h->dws.p, h->num_sms, my_table, st, &launches);
+    else e = cudaMemsetAsync(my_table, 0, 65536 * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("sharded decode phase 1", e); return DENSITY_B200_ECUDA; }
+    if (h->world > 1 && !nccl_check(a->AllGather(my_table, x.tables, 65536, NCCL_UINT32, h->comm, st), "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+    e = cham_rank_fold(x.tables, (uint32_t)h->rank, x.carry, st, &launches);
+    // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
+    if (e == cudaSuccess && n) e = cham_decode_phase2(d_in, n, d_out, cap, h->dws.p, h->num_sms, x.carry, d_out_size, st, &launches);
+    if (e == cudaSuccess && n) e = cham_decode_seam_words(d_in, n, cap, h->dws.p, h->num_sms, h->rank == h->world - 1, d_out_size, my_words, st, &launches);
+    if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
+    if (e == cudaSuccess && !n) e = cudaMemsetAsync(my_words, 0, 8 * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("sharded decode phase 2", e); return DENSITY_B200_ECUDA; }
+    if (h->world > 1 && !nccl_check(a->AllGather(my_words, x.words, 8, NCCL_UINT32, h->comm, st), "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
+    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
     return DENSITY_B200_OK;
 }
 

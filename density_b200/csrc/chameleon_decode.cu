@@ -28,6 +28,9 @@
 //     and patched afterwards from the per-run carry-in tables (same machinery as the encoder).
 //  4. Tail.  The last < 264 bytes of the stream (codec.rs:102-123: per-unit bounds checks, partial units, 1-3 raw bytes) are
 //     decoded by one thread with the reference's literal control flow, starting from the folded dictionary.
+//  5. Sharded decode (DESIGN §5).  One piece of a sharded stream in two phases: phase 1 (boundaries, writer pass) needs no carry-in
+//     and exports the piece's last-writer table, tail included; phase 2 folds the carry-in from the pieces before it into every
+//     run's dictionary, decodes, and writes the piece's seam words for the cross-piece quiet check.
 #include "common.cuh"
 #include "encode_internal.cuh"
 #include "decode_bounds.cuh"
@@ -685,11 +688,14 @@ cham_decode_pass7(const uint8_t* __restrict__ in, const uint64_t* __restrict__ b
     }
 }
 
-// carry-in fold for decode: initial dictionary is all zero values (chameleon.rs:41): nothing touched.
-__global__ void dec_carry_scan(const uint32_t* __restrict__ final_tab, uint32_t nruns, uint32_t* __restrict__ carry, uint32_t* __restrict__ dict_out) {
+// carry-in fold for decode, starting from `carry_in` (the dictionary before this piece of a sharded stream, shard format) or, when it
+// is null, from the stream start: all zero values (chameleon.rs:41), nothing touched. The encoder's stream-start table (bucket 0
+// touched with fingerprint 0) is the same dictionary: quad_from_hf(0, 0) == 0.
+__global__ void dec_carry_scan(const uint32_t* __restrict__ final_tab, uint32_t nruns, uint32_t* __restrict__ carry, uint32_t* __restrict__ dict_out,
+                               const uint32_t* __restrict__ carry_in) {
     uint32_t hb = blockIdx.x * blockDim.x + threadIdx.x;
     if (hb >= 65536) return;
-    uint32_t c = 0;
+    uint32_t c = carry_in ? carry_in[hb] : 0u;
     for (uint32_t r = 0; r < nruns; ++r) {
         carry[(size_t)r * 65536 + hb] = c;
         uint32_t v = final_tab[(size_t)r * 65536 + hb];
@@ -767,6 +773,103 @@ __global__ void dec_tail(const uint8_t* __restrict__ in, uint64_t n, uint8_t* __
     if (d_out_size) *d_out_size = res;
 }
 
+// ---- 5. sharded decode: a piece's exported table and its seam words ----------------------------------------------------------
+// The tail's blocks as dec_tail goes through them, without output: plain(q) sees every PLAIN quad in stream order. The control flow
+// does not depend on the dictionary, so this runs before the carry-in is known.
+struct TailWalk {
+    uint64_t blocks;        // blocks the tail loop entered (copy-mode, encoded, partial)
+    uint32_t first_inc;     // the first tail block is a complete incompressible block
+    uint32_t copied, bad;   // a copy-mode block; a malformed block
+    Protection ps;          // protection state when the tail loop stops
+};
+template <class F>
+__device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
+    TailWalk w; w.blocks = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
+    Protection& ps = w.ps;
+    ps.init();
+    ps.counter = st->main_blocks;
+    ps.previous_incompressible = st->last_main_inc;
+    if (st->seq) { ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev; }
+    uint64_t idx = st->tail_off;
+    while (n - idx > 0) {
+        ++w.blocks;
+        if (ps.revert_to_copy()) {
+            w.copied = 1;
+            const uint64_t rem = n - idx;
+            idx += rem > 256 ? 256 : rem;
+            if (rem <= 256) break;
+            ps.decay();
+            continue;
+        }
+        const uint64_t mark = idx;
+        if (n - idx < 8) { w.bad = 1; break; }
+        uint64_t sig = 0;
+        for (int i = 0; i < 8; ++i) sig |= (uint64_t)in[idx + i] << (8 * i);
+        idx += 8;
+        bool end = false;
+        for (int u = 0; u < 32 && !end && !w.bad; ++u) {
+            const bool checked = (n - idx) < 8;
+            for (int k = 0; k < 2 && !end; ++k) {
+                const uint32_t fl = (uint32_t)(sig & 1); sig >>= 1;
+                if (checked && fl == 0) {
+                    const uint64_t rem = n - idx;
+                    if (rem == 0) { end = true; break; }
+                    if (rem < 4) { idx = n; end = true; break; }
+                }
+                if (fl) {
+                    if (n - idx < 2) { w.bad = 1; break; }
+                    idx += 2;
+                } else {
+                    if (n - idx < 4) { w.bad = 1; break; }
+                    plain(in[idx] | (in[idx + 1] << 8) | (in[idx + 2] << 16) | ((uint32_t)in[idx + 3] << 24));
+                    idx += 4;
+                }
+            }
+        }
+        if (end || w.bad) break;
+        const bool inc = idx - mark >= 256;
+        if (w.blocks == 1) w.first_inc = inc ? 1u : 0u;
+        ps.update(inc);
+    }
+    return w;
+}
+
+// The piece's exported table: the left fold of its run tables (writer pass) ...
+__global__ void dec_export_fold(const uint32_t* __restrict__ final_tab, uint32_t nruns, uint32_t* __restrict__ table_out) {
+    const uint32_t hb = blockIdx.x * blockDim.x + threadIdx.x;
+    if (hb >= 65536) return;
+    uint32_t c = 0;
+    for (uint32_t r = 0; r < nruns; ++r) { const uint32_t v = final_tab[(size_t)r * 65536 + hb]; if (v & 0x10000u) c = v; }
+    table_out[hb] = c;
+}
+// ... then the PLAIN quads of the tail on top: in a non-final piece the tail is usually its last block, and a MAP quad of the next
+// piece may read what it wrote
+__global__ void dec_export_tail(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, uint32_t* __restrict__ table_out) {
+    if (threadIdx.x || blockIdx.x) return;
+    if (st->nonquiet || st->error) return;     // dec_tail will not run; the piece is refused
+    tail_walk(in, n, st, [&](uint32_t q) { const uint32_t p = hash_prod(q); table_out[prod_hash(p)] = 0x10000u | prod_fp(p, q); });
+}
+
+// What a decoded piece tells the others, in the layout of cham_seam_words_k: {first block incompressible, last block incompressible,
+// not quiet or error, has blocks, decoded size lo, hi, 0, 0}. Runs after dec_tail. Not quiet: copy-mode blocks in the main loop
+// (dec_seq_walk ran) or in the tail, two incompressible blocks at the end (the next piece's first block would be copied: penalty > 0),
+// an error (malformed, output beyond cap), or a non-final piece that does not decode to whole 256-byte blocks.
+__global__ void dec_seam_words_k(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, int is_last,
+                                 const uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
+    if (threadIdx.x || blockIdx.x) return;
+    const uint64_t sz = *d_out_size;
+    uint32_t first = 0, last = 0, bad = (st->nonquiet || st->error || st->seq) ? 1u : 0u;
+    if (!bad) {
+        const TailWalk w = tail_walk(in, n, st, [](uint32_t) {});
+        first = st->main_blocks ? (T::consumed(bounds::ldsig(in)) >= 256u ? 1u : 0u) : w.first_inc;
+        last = w.ps.previous_incompressible;
+        if (w.bad || w.copied || w.ps.copy_penalty) bad = 1;
+    }
+    if (!is_last && (sz % 256)) bad = 1;
+    words[0] = first; words[1] = last; words[2] = bad; words[3] = 1;
+    words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
+}
+
 }  // namespace chamdec
 
 using namespace chamdec;
@@ -787,10 +890,17 @@ static size_t dec_layout(size_t nbytes, size_t cap, int nruns_max, ChamDecLayout
 
 size_t cham_decode_workspace_bytes(size_t nbytes, size_t cap, int nruns_max) { ChamDecLayout L; return dec_layout(nbytes, cap, nruns_max, &L); }
 
-// Enqueues the parallel decode. On return (after the stream drains) *d_nonquiet != 0 means the caller must run the exact
-// in-order kernel instead (copy-mode blocks present, or a pathological tile); d_out_size is only written when it is 0.
-cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms,
-                                 uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches) {
+// run count from an upper bound of the block count (the kernels read the real one from the status block)
+static uint32_t dec_pick_runs(const ChamDecLayout& L, int num_sms) {
+    const uint64_t tiles_ub = (L.B.maxblocks + 63) / 64;
+    uint32_t nruns = (uint32_t)(tiles_ub / 16); if (nruns < 1) nruns = 1; if (nruns > (uint32_t)num_sms) nruns = num_sms;
+    return nruns;
+}
+
+// Phase 1 of the parallel decode, which needs no carry-in: boundaries, then the writer pass (each run's last-writer table). With
+// d_table_out it also exports the piece's table (shard format) for the pieces after it.
+cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
+                               cudaStream_t stream, uint64_t* launches) {
     static bool attr_done = false;
     if (!attr_done) {
         cudaError_t e0 = cudaFuncSetAttribute(cham_decode_pass<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DecSmem));
@@ -805,21 +915,55 @@ cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
     uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
     cudaError_t e = bounds::bounds_launch<T>(d_in, nbytes, cap, ws, L.B, stream, launches);
     if (e != cudaSuccess) return e;
-    const uint64_t maxblocks = L.B.maxblocks;
-    // run count from an upper bound of the block count (the kernel reads the real one from the status block)
-    uint64_t tiles_ub = (maxblocks + 63) / 64;
-    uint32_t nruns = (uint32_t)(tiles_ub / 16); if (nruns < 1) nruns = 1; if (nruns > (uint32_t)num_sms) nruns = num_sms;
+    const uint32_t nruns = dec_pick_runs(L, num_sms);
     uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
-    uint32_t* carry = reinterpret_cast<uint32_t*>(ws + L.carry);
     if (g_cham_decode_impl == 1) cham_decode_pass<true><<<nruns, DP_THREADS, sizeof(DecSmem), stream>>>(d_in, blk_off, st, nruns, nullptr, nullptr, final_tab);
     else cham_decode_pass7<true><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, nullptr, nullptr, final_tab);
     ++*launches;
-    dec_carry_scan<<<65536 / 256, 256, 0, stream>>>(final_tab, nruns, carry, reinterpret_cast<uint32_t*>(ws + L.dict)); ++*launches;
+    if (d_table_out) {
+        dec_export_fold<<<65536 / 256, 256, 0, stream>>>(final_tab, nruns, d_table_out);
+        dec_export_tail<<<1, 32, 0, stream>>>(d_in, nbytes, st, d_table_out);
+        *launches += 2;
+    }
+    return cudaGetLastError();
+}
+
+// Phase 2: the carry-in of every run folded from d_carry_in (NULL: stream start), the decode pass and the tail. The workspace is the one
+// phase 1 filled for the same (d_in, nbytes, cap, num_sms).
+cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms, const uint32_t* d_carry_in,
+                               uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches) {
+    ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
+    DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.B.status);
+    uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
+    const uint32_t nruns = dec_pick_runs(L, num_sms);
+    uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
+    uint32_t* carry = reinterpret_cast<uint32_t*>(ws + L.carry);
+    dec_carry_scan<<<65536 / 256, 256, 0, stream>>>(final_tab, nruns, carry, reinterpret_cast<uint32_t*>(ws + L.dict), d_carry_in); ++*launches;
     if (g_cham_decode_impl == 1) cham_decode_pass<false><<<nruns, DP_THREADS, sizeof(DecSmem), stream>>>(d_in, blk_off, st, nruns, reinterpret_cast<uint32_t*>(d_out), carry, final_tab);
     else cham_decode_pass7<false><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, reinterpret_cast<uint32_t*>(d_out), carry, final_tab);
     ++*launches;
     dec_tail<<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, reinterpret_cast<uint32_t*>(ws + L.dict), st, d_out_size); ++*launches;
-    e = cudaMemcpyAsync(d_nonquiet, &st->nonquiet, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream);
+    return cudaGetLastError();
+}
+
+// The 8 seam words of a decoded piece (after phase 2; d_out_size as phase 2 wrote it).
+cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint64_t* d_out_size,
+                                   uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
+    ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
+    dec_seam_words_k<<<1, 32, 0, stream>>>(d_in, nbytes, reinterpret_cast<const DecStatus*>(ws + L.B.status), is_last, d_out_size, d_words);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// Enqueues the parallel decode. On return (after the stream drains) *d_nonquiet != 0 means the caller must run the exact
+// in-order kernel instead (copy-mode blocks present, or a pathological tile); d_out_size is only written when it is 0.
+cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms,
+                                 uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches) {
+    cudaError_t e = cham_decode_phase1(d_in, nbytes, cap, ws, num_sms, nullptr, stream, launches);
+    if (e == cudaSuccess) e = cham_decode_phase2(d_in, nbytes, d_out, cap, ws, num_sms, nullptr, d_out_size, stream, launches);
+    if (e != cudaSuccess) return e;
+    ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
+    e = cudaMemcpyAsync(d_nonquiet, &reinterpret_cast<DecStatus*>(ws + L.B.status)->nonquiet, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }

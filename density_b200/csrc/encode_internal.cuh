@@ -57,6 +57,14 @@ cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, ui
 size_t cham_decode_workspace_bytes(size_t nbytes, size_t cap, int nruns_max);
 cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms,
                                  uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches);
+// the same as two phases, for one piece of a sharded stream: phase 1 needs no carry-in and exports the piece's last-writer table
+// (shard format) when d_table_out is set; phase 2 decodes from d_carry_in (NULL: stream start); then the piece's 8 seam words
+cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
+                               cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms, const uint32_t* d_carry_in,
+                               uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint64_t* d_out_size,
+                                   uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 
 // cl_decode.cu (run-parallel Cheetah decode)
 size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);

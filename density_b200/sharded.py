@@ -8,6 +8,10 @@ Rank r owns bytes [r*S, (r+1)*S) of the stream (S a multiple of 256 so block gri
 The concatenation of the per-rank outputs is byte-identical to one chameleon_encode call over the whole buffer as long as
 the protection automaton stays quiet (flags bit 0 reports otherwise). Outputs stay where they were produced; a caller
 that wants them on one rank gathers them with the sizes returned here.
+
+Decode is the mirror image: rank r decodes its piece back into its shard with the same table exchange and fold. The decode
+phase 1 (boundaries, writer pass) needs no carry-in and exports the piece's table; phase 2 decodes from the folded carry-in
+and writes 8 seam words, which every rank gathers and judges with `seam_verdict`.
 """
 import ctypes
 
@@ -43,6 +47,35 @@ def exchange_tables(table, group=None):
     gathered = torch.empty((world, TABLE_ENTRIES), dtype=torch.int32, device=table.device)
     dist.all_gather_into_tensor(gathered.view(-1), table.contiguous(), group=group)
     return gathered
+
+
+SEAM_WORDS = 8
+
+
+def exchange_seam_words(words, group=None):
+    """all_gather of every rank's 8 seam words: int32 [world, 8]."""
+    world = dist.get_world_size(group)
+    gathered = torch.empty((world, SEAM_WORDS), dtype=torch.int32, device=words.device)
+    dist.all_gather_into_tensor(gathered.view(-1), words.contiguous(), group=group)
+    return gathered
+
+
+def seam_verdict(words):
+    """The Python twin of cham_seam_verdict_k. words: int32 [world, 8], one row per piece in stream order:
+    {first block incompressible, last block incompressible, not quiet or error, has blocks, size lo, size hi, 0, 0}.
+    Returns (flags, total, offsets): flags 1 when a piece is not quiet or a seam joins two incompressible blocks (the
+    protection automaton would fire across the cut, protection_state.rs:38-43), else 0; total = the summed sizes;
+    offsets = int64 [world + 1], the prefix sums of the sizes. Pieces without blocks are skipped at the seams."""
+    w = words.to("cpu", torch.int64) & 0xFFFFFFFF
+    sizes = w[:, 4] | (w[:, 5] << 32)
+    offsets = torch.zeros(w.shape[0] + 1, dtype=torch.int64)
+    offsets[1:] = torch.cumsum(sizes, 0)
+    bad, prev_inc = bool((w[:, 2] != 0).any()), False
+    for r in range(w.shape[0]):
+        if w[r, 3]:
+            bad |= prev_inc and bool(w[r, 0])
+            prev_inc = bool(w[r, 1])
+    return int(bad), int(offsets[-1]), offsets
 
 
 class ShardedChameleonEncoder:
@@ -86,11 +119,54 @@ class ShardedChameleonEncoder:
             raise _lib.DensityB200Error(f"shard_phase2 rc={rc}: {_lib.last_error()}")
 
 
-class ShardedEncoder:
-    """The C++ multi-GPU path (`density_b200_encode_sharded`, include/density_b200.h): one process per GPU; the library owns its NCCL
-    communicator (the 128-byte id travels once through torch.distributed), the table all-gather, the single fold kernel, the exact
-    seam verdict and the optional variable-length gather of the pieces to one rank. torch.distributed is only used to hand out the id.
-    """
+class ShardedChameleonDecoder:
+    """Decode of this rank's piece through the shard phases, with torch.distributed for the exchanges (the mirror of
+    ShardedChameleonEncoder)."""
+
+    def __init__(self):
+        self._lib = _lib.load()
+        self._h = self._lib.density_b200_decode_shard_create()
+        if not self._h:
+            raise _lib.DensityB200Error(_lib.last_error())
+
+    def close(self):
+        if self._h:
+            self._lib.density_b200_decode_shard_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def decode(self, d_in, d_out, d_size, group=None):
+        """d_in: CUDA uint8 tensor, this rank's piece (2-byte aligned); d_out: uint8 tensor of capacity d_out.numel() (4-byte aligned);
+        d_size: int64[1]. Returns seam_verdict's (flags, total, offsets) over all ranks; flags != 0: the pieces are void."""
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=d_in.device)
+        rc = self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(rank == world - 1),
+                                                        table.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"decode_shard_phase1 rc={rc}: {_lib.last_error()}")
+        carry_ptr = None
+        if world > 1:
+            gathered = exchange_tables(table, group)
+            if rank > 0:
+                self._carry = fold_tables(gathered, rank)
+                carry_ptr = self._carry.data_ptr()
+        words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=d_in.device)
+        rc = self._lib.density_b200_decode_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"decode_shard_phase2 rc={rc}: {_lib.last_error()}")
+        return seam_verdict(exchange_seam_words(words, group) if world > 1 else words.view(1, SEAM_WORDS))
+
+
+class _ShardedHandle:
+    """A `density_b200_sharded` handle: one process per GPU; the library owns its NCCL communicator (the 128-byte id travels once
+    through torch.distributed). torch.distributed is only used to hand out the id."""
 
     def __init__(self, device, group=None):
         self._lib = _lib.load()
@@ -124,6 +200,12 @@ class ShardedEncoder:
         except Exception:
             pass
 
+
+class ShardedEncoder(_ShardedHandle):
+    """The C++ multi-GPU path (`density_b200_encode_sharded`, include/density_b200.h): the table all-gather, the single fold kernel,
+    the exact seam verdict and the optional variable-length gather of the pieces to one rank, over the library's NCCL communicator.
+    """
+
     def encode(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None):
         """Enqueue on torch's current stream. d_size int64[1]: this rank's piece; d_flags int32[1]: != 0 -> the stream is not quiet and
         the pieces are void; self.d_total int64[1]: stream length. gather_root >= 0: pieces gathered into d_gather on that rank (blocks)."""
@@ -142,3 +224,18 @@ class ShardedEncoder:
         if rc:
             raise _lib.DensityB200Error(f"sharded_profile rc={rc}: {_lib.last_error()}")
         return [float(x) for x in out]
+
+
+class ShardedDecoder(_ShardedHandle):
+    """The C++ multi-GPU decode (`density_b200_decode_sharded`): the inverse of ShardedEncoder.encode without a gather. Each rank
+    decodes its piece back into the shard it was encoded from; the exchanges run over the library's NCCL communicator."""
+
+    def decode(self, d_in, d_out, d_size, d_flags):
+        """Enqueue on torch's current stream; nothing blocks. d_in: this rank's piece (2-byte aligned); d_out: capacity d_out.numel()
+        (4-byte aligned); d_size int64[1]: the decoded size; d_flags int32[1]: != 0 -> the pieces are void and the caller decodes the
+        gathered stream on one device; self.d_total int64[1]: the original length."""
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rc = self._lib.density_b200_decode_sharded(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(),
+                                                   d_flags.data_ptr(), self.d_total.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"decode_sharded rc={rc}: {_lib.last_error()}")

@@ -156,6 +156,35 @@ DENSITY_B200_API int density_b200_encode_sharded(density_b200_sharded*, const ui
 DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* out_ms5);
 
 /*
+ * Sharded Chameleon decode: the inverse of the sharded encode. Piece r is what shard r of a sharded encode produced (rank r's
+ * d_out[0 .. d_out_size)), or equally the slice of a single-call stream at the prefix sums of those sizes. Decoding piece r with the
+ * dictionary carried in from pieces < r gives back shard r byte for byte, so the concatenation equals chameleon_decode of the whole
+ * stream. Quiet streams only, as for encode: the verdict is non-zero when a piece holds a copy-mode block, a seam joins two
+ * incompressible blocks, a non-final piece does not decode to whole 256-byte blocks, or a piece is malformed or its output exceeds
+ * `cap`. The decoded pieces are then void and the caller decodes the gathered stream on one device. Nothing is written past `cap`.
+ * d_in must be 2-byte and d_out 4-byte aligned (there is no in-order fallback on this path); otherwise DENSITY_B200_EARG.
+ */
+typedef struct density_b200_decode_shard density_b200_decode_shard; /* opaque */
+DENSITY_B200_API density_b200_decode_shard* density_b200_decode_shard_create(void);
+DENSITY_B200_API void density_b200_decode_shard_destroy(density_b200_decode_shard*);
+/* phase 1: boundaries and writer pass; exports the piece's last-writer table (shard format, as density_b200_shard_phase1) to
+   d_table_out, including the PLAIN quads of the tail. cap = output capacity (sizes the boundary layout). */
+DENSITY_B200_API int density_b200_decode_shard_phase1(density_b200_decode_shard*, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                     uint32_t* d_table_out, void* stream);
+/* phase 2: d_carry_in = dictionary before this piece (the left fold of the earlier pieces' tables over density_b200_table_init's
+   state; NULL = stream start). Decodes into d_out, writes the decoded size to *d_out_size and the piece's 8 seam words to d_seam8:
+   {first block incompressible, last block incompressible, not quiet or error, has blocks, decoded size lo, hi, 0, 0}, the layout
+   of the encoder's seam words. One phase 2 per phase 1. */
+DENSITY_B200_API int density_b200_decode_shard_phase2(density_b200_decode_shard*, const uint32_t* d_carry_in, uint8_t* d_out,
+                                     uint64_t* d_out_size, uint32_t* d_seam8, void* stream);
+/* End to end over NCCL on the communicator of a density_b200_sharded handle: phase 1 -> ncclAllGather(tables) -> fold kernel -> phase 2
+   -> ncclAllGather(seam words) -> seam verdict. *d_flags != 0: the pieces are void. *d_total_size = the original length, on every
+   rank (may be NULL). Never blocks; each rank gets back the shard it started with, so there is no gather. Uses its own workspace in
+   the handle: encode_sharded and decode_sharded may alternate on one handle. */
+DENSITY_B200_API int density_b200_decode_sharded(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
  * A reused Codec INSTANCE (streaming continuation). In the reference `encode` / `decode` are methods of an instance
  * (/root/reference/src/codec/codec.rs:16,72,82) whose dictionary survives from call to call until clear_state()
  * (chameleon.rs:148-150, cheetah.rs:198-202, lion.rs:327-331), while the protection state is created inside every call

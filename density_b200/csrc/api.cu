@@ -782,9 +782,10 @@ struct density_b200_sharded {
     int rank = 0, world = 1, num_sms = 0;
     nccl_comm_t comm = nullptr;
     DevBuf ws, aux;                 // aux: gathered tables [world][65536] + carry [65536] + seam words [world][8] + offsets [world + 1] + size
-    DevBuf dws;                     // decode workspace (density_b200_decode_sharded), apart from the encoder's
+    DevBuf dws;                     // decode workspace (density_b200_decode_sharded[_stream]), apart from the encoder's
     ChamLayout L{};
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
+    uint64_t* h_maps = nullptr;     // pinned, world range maps (density_b200_decode_sharded_stream)
     cudaEvent_t ev[6] = {};         // stage timing of the last call: start, flag pass, exchange, phase 2 up to emit, emit, gather
     bool timed = false;
 };
@@ -812,7 +813,14 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
         nccl_unique_id id; memcpy(id.internal, nccl_unique_id_128, 128);
         if (!nccl_check(a->CommInitRank(&h->comm, world, id, rank), "ncclCommInitRank")) { delete h; return nullptr; }
     }
-    if (cudaMallocHost(&h->h_offsets, sizeof(uint64_t) * (world + 2)) != cudaSuccess) { set_error("cudaMallocHost"); delete h; return nullptr; }
+    if (cudaMallocHost(&h->h_offsets, sizeof(uint64_t) * (world + 2)) != cudaSuccess ||
+        cudaMallocHost(&h->h_maps, sizeof(uint64_t) * DENSITY_B200_LOCATE_MAP_WORDS * world) != cudaSuccess) {
+        set_error("cudaMallocHost");
+        if (h->h_offsets) cudaFreeHost(h->h_offsets);
+        if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
+        delete h;
+        return nullptr;
+    }
     for (auto& e : h->ev) cudaEventCreate(&e);
     return h;
 }
@@ -822,20 +830,23 @@ void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
     h->ws.release(); h->aux.release(); h->dws.release();
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
+    if (h->h_maps) cudaFreeHost(h->h_maps);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
     delete h;
 }
 
 // the exchange buffers of a handle, shared by encode and decode
-struct ShardedAux { uint32_t *tables, *carry, *words; uint64_t* offsets; };
+struct ShardedAux { uint32_t *tables, *carry, *words; uint64_t *offsets, *maps; };
 static cudaError_t sharded_aux(density_b200_sharded* h, cudaStream_t st, ShardedAux* x) {
     const size_t W = (size_t)h->world;
     const size_t aux_tables = W * 65536 * sizeof(uint32_t), aux_carry = 65536 * sizeof(uint32_t), aux_words = W * 8 * sizeof(uint32_t);
-    const cudaError_t e = h->aux.ensure(aux_tables + aux_carry + aux_words + (W + 2) * sizeof(uint64_t) + 256, st);
+    const size_t aux_offsets = (W + 2) * sizeof(uint64_t), aux_maps = W * DENSITY_B200_LOCATE_MAP_WORDS * sizeof(uint64_t);
+    const cudaError_t e = h->aux.ensure(aux_tables + aux_carry + aux_words + aux_offsets + aux_maps + 256, st);
     x->tables = reinterpret_cast<uint32_t*>(h->aux.p);
     x->carry = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables);
     x->words = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables + aux_carry);
     x->offsets = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words);
+    x->maps = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words + aux_offsets);
     return e;
 }
 
@@ -917,14 +928,11 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     return DENSITY_B200_OK;
 }
 
-// The inverse of density_b200_encode_sharded without a gather: this rank's piece d_in[0 .. n) decodes to the shard it was encoded from.
-// Everything is enqueued on `stream`; nothing blocks.
-int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                                uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+// The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it, over the handle's communicator:
+// phase 1 -> table exchange -> fold -> phase 2 -> seam words -> verdict. is_last: the piece ends the stream (a non-final piece must decode
+// to whole 256-byte blocks). d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
+static int decode_sharded_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, int is_last, uint8_t* d_out, size_t cap,
+                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, cudaStream_t st) {
     NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
     if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
     ShardedAux x;
@@ -942,15 +950,107 @@ int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     e = cham_rank_fold(x.tables, (uint32_t)h->rank, x.carry, st, &launches);
     // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
     if (e == cudaSuccess && n) e = cham_decode_phase2(d_in, n, d_out, cap, h->dws.p, h->num_sms, x.carry, d_out_size, st, &launches);
-    if (e == cudaSuccess && n) e = cham_decode_seam_words(d_in, n, cap, h->dws.p, h->num_sms, h->rank == h->world - 1, d_out_size, my_words, st, &launches);
+    if (e == cudaSuccess && n) e = cham_decode_seam_words(d_in, n, cap, h->dws.p, h->num_sms, is_last, d_out_size, my_words, st, &launches);
     if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
     if (e == cudaSuccess && !n) e = cudaMemsetAsync(my_words, 0, 8 * sizeof(uint32_t), st);
     if (e != cudaSuccess) { set_error("sharded decode phase 2", e); return DENSITY_B200_ECUDA; }
     if (h->world > 1 && !nccl_check(a->AllGather(my_words, x.words, 8, NCCL_UINT32, h->comm, st), "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
     e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
     g_launches += launches;
+    if (e == cudaSuccess && d_out_offset) e = cudaMemcpyAsync(d_out_offset, x.offsets + h->rank, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
     return DENSITY_B200_OK;
+}
+
+// The inverse of density_b200_encode_sharded without a gather: this rank's piece d_in[0 .. n) decodes to the shard it was encoded from.
+// Everything is enqueued on `stream`; nothing blocks.
+int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    return decode_sharded_piece(h, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
+                                reinterpret_cast<cudaStream_t>(stream_v));
+}
+
+int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_map) & 7)) { set_error("d_in must be 2-byte, d_map 8-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase1_done = false;     // the scratch is phase 1's
+    cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t launches = 0;
+    e = cham_decode_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("decode locate", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
+int density_b200_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out4[4]) {
+    g_last_error.clear();
+    constexpr uint64_t W = DENSITY_B200_LOCATE_MAP_WORDS, TERM = ~0ull, CH = 16384, HALO = 264, NCAND = 132;
+    if (!h_maps || !out4 || world < 1 || rank < 0 || rank >= world) { set_error("locate_piece: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+    uint64_t later = 0;                 // stream bytes behind range r
+    for (int r = world - 1; r >= 0; --r) {
+        const uint64_t* m = h_maps + (size_t)r * W;
+        if (r < world - 1 && m[0] % CH) { set_error("locate_piece: a non-last range is not a multiple of 16384 bytes"); return DENSITY_B200_EARG; }
+        if (m[1] != (later < HALO ? later : HALO)) { set_error("locate_piece: a halo is not min(264, the bytes of the later ranges)"); return DENSITY_B200_EARG; }
+        for (uint64_t c = 0; c < NCAND; ++c)
+            if (m[2 + 2 * c] != TERM && m[2 + 2 * c] >= NCAND) { set_error("locate_piece: bad exit index in a range map"); return DENSITY_B200_EARG; }
+        if (m[0] > ~later) { set_error("locate_piece: ranges overflow"); return DENSITY_B200_EARG; }
+        later += m[0];
+    }
+    uint64_t idx = 0, blocks = 0;       // walk from the stream start; an empty range passes the entry on unchanged
+    for (int r = 0; r < rank; ++r) {
+        const uint64_t* m = h_maps + (size_t)r * W;
+        if (m[0] == 0) continue;
+        blocks += m[3 + 2 * idx];
+        idx = m[2 + 2 * idx];
+        if (idx == TERM) { out4[0] = 0; out4[1] = 0; out4[2] = blocks; out4[3] = 1; return DENSITY_B200_OK; }   // behind the stream end
+    }
+    const uint64_t* m = h_maps + (size_t)rank * W;
+    const uint64_t n_range = m[0], n_halo = m[1];
+    if (n_range == 0) { out4[0] = 0; out4[1] = 0; out4[2] = blocks; out4[3] = n_halo == 0; return DENSITY_B200_OK; }
+    const uint64_t ex = m[2 + 2 * idx];
+    const uint64_t start = 2 * idx, end = ex == TERM ? n_range + n_halo : n_range + 2 * ex;
+    if (start > end || end > n_range + n_halo) { set_error("locate_piece: inconsistent range maps"); return DENSITY_B200_EARG; }
+    out4[0] = start; out4[1] = end; out4[2] = blocks; out4[3] = end == n_range + n_halo;
+    return DENSITY_B200_OK;
+}
+
+// Sharded decode of a stream without known cuts: this rank holds its range + halo (include/density_b200.h). Locates the piece (one
+// host synchronisation), then decodes it as density_b200_decode_sharded does.
+int density_b200_decode_sharded_stream(density_b200_sharded* h, const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* d_out, size_t cap,
+                                       uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n_range + n_halo) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    const size_t W = (size_t)h->world;
+    ShardedAux x;
+    // sized for the whole range + halo: covers the locate scratch and the phases on any piece of it
+    cudaError_t e = h->dws.ensure(cham_decode_workspace_bytes(n_range + n_halo, cap, h->num_sms), st);
+    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t* my_map = x.maps + (size_t)h->rank * DENSITY_B200_LOCATE_MAP_WORDS;
+    uint64_t launches = 0;
+    e = cham_decode_locate(d_in, n_range, n_halo, h->dws.p, my_map, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("decode locate", e); return DENSITY_B200_ECUDA; }
+    if (h->world > 1 && !nccl_check(a->AllGather(my_map, x.maps, DENSITY_B200_LOCATE_MAP_WORDS * 8, NCCL_UINT8, h->comm, st), "ncclAllGather(maps)"))
+        return DENSITY_B200_ECUDA;
+    e = cudaMemcpyAsync(h->h_maps, x.maps, W * DENSITY_B200_LOCATE_MAP_WORDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("range maps to host", e); return DENSITY_B200_ECUDA; }
+    uint64_t piece[4];
+    const int rc = density_b200_locate_piece(h->h_maps, h->world, h->rank, piece);
+    if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
+    return decode_sharded_piece(h, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[3], d_out, cap, d_out_size, d_flags,
+                                d_total_size, d_out_offset, st);
 }
 
 /* stage times of the last density_b200_encode_sharded call (waits for it): out_ms[0] flag pass, [1] table exchange + fold,

@@ -955,6 +955,28 @@ cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t ca
     return cudaGetLastError();
 }
 
+// The range map of d_in[0 .. n_range + n_halo) (sharded decode of a stream without known cuts): the candidate walks over the range's
+// chunks, with the halo visible to the walks of its last chunk, their composition per group, then over the whole range. The scratch is
+// the res / gres arrays of the boundary layout of n_range + n_halo bytes, where phase 1 puts them too.
+size_t cham_locate_workspace_bytes(size_t nbytes) { bounds::BoundsLayout B; return bounds::bounds_layout<T>(nbytes, 0, &B); }
+
+cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint64_t* d_map, cudaStream_t stream,
+                               uint64_t* launches) {
+    bounds::BoundsLayout B; bounds::bounds_layout<T>(n_range + n_halo, 0, &B);
+    uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
+    uint4* gres = reinterpret_cast<uint4*>(ws + B.gres);
+    const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
+    const uint32_t ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
+    if (nchunks) {
+        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
+        bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
+        *launches += 2;
+    }
+    bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(gres, ngroups, n_range, n_halo, reinterpret_cast<unsigned long long*>(d_map));
+    ++*launches;
+    return cudaGetLastError();
+}
+
 // Enqueues the parallel decode. On return (after the stream drains) *d_nonquiet != 0 means the caller must run the exact
 // in-order kernel instead (copy-mode blocks present, or a pathological tile); d_out_size is only written when it is 0.
 cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms,

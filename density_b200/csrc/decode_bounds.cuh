@@ -337,6 +337,44 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
     }
 }
 
+// ---- 3. the map of a whole byte range (sharded decode of a stream whose cuts are not known) ----------------------------------------
+// Folds the group rows of dec_group_compose over all `ngroups` groups of a range, for every candidate entry at once, and writes the
+// range map (DENSITY_B200_LOCATE_MAP_WORDS u64): {n_range, n_halo}, then per candidate {exit index into the next range or ~0 (the walk
+// reached the stream end), blocks}. With no groups (an empty range) every row is the identity. Each thread follows one candidate's
+// chain of dependent rows; the whole CTA stages RC_BATCH groups of rows in shared memory at a time, so a link costs a shared load.
+constexpr int RC_BATCH = 32;
+constexpr int RC_THREADS = 256;
+template <class T>
+__global__ void __launch_bounds__(RC_THREADS) dec_range_compose(const uint4* __restrict__ gres, uint32_t ngroups, uint64_t n_range,
+                                                                uint64_t n_halo, unsigned long long* __restrict__ map) {
+    __shared__ uint2 rows[RC_BATCH * T::NCAND];     // {exit, blocks} of the staged groups
+    const uint32_t tid = threadIdx.x;
+    uint32_t idx = tid;
+    unsigned long long blocks = 0;
+    for (uint32_t g0 = 0; g0 < ngroups; g0 += RC_BATCH) {
+        const uint32_t nb = min(ngroups - g0, (uint32_t)RC_BATCH);
+        __syncthreads();
+        for (uint32_t i = tid; i < nb * T::NCAND; i += RC_THREADS) {
+            const uint4 r = gres[(size_t)g0 * T::NCAND + i];
+            rows[i] = make_uint2(r.x, r.y);
+        }
+        __syncthreads();
+        if (tid < T::NCAND && idx != TERM) {
+            for (uint32_t g = 0; g < nb; ++g) {
+                const uint2 r = rows[g * T::NCAND + idx];
+                blocks += r.y;
+                idx = r.x;
+                if (idx == TERM) break;
+            }
+        }
+    }
+    if (tid < T::NCAND) {
+        map[2 + 2 * tid] = idx == TERM ? ~0ull : (unsigned long long)idx;
+        map[3 + 2 * tid] = blocks;
+    }
+    if (tid == 0) { map[0] = n_range; map[1] = n_halo; }
+}
+
 // ---- host side: workspace layout + launch sequence ---------------------------------------------------------------------------------
 struct BoundsLayout { size_t status, res, gres, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, total; uint64_t maxblocks; };
 

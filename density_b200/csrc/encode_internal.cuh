@@ -65,6 +65,11 @@ cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_ou
                                uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint64_t* d_out_size,
                                    uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+// the range map of a piece of a stream without known cuts (DENSITY_B200_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`, at least
+// cham_locate_workspace_bytes(n_range + n_halo), which cham_decode_workspace_bytes of the same length covers
+size_t cham_locate_workspace_bytes(size_t nbytes);
+cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint64_t* d_map, cudaStream_t stream,
+                               uint64_t* launches);
 
 // cl_decode.cu (run-parallel Cheetah decode)
 size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);

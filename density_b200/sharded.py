@@ -12,9 +12,15 @@ that wants them on one rank gathers them with the sizes returned here.
 Decode is the mirror image: rank r decodes its piece back into its shard with the same table exchange and fold. The decode
 phase 1 (boundaries, writer pass) needs no carry-in and exports the piece's table; phase 2 decodes from the folded carry-in
 and writes 8 seam words, which every rank gathers and judges with `seam_verdict`.
+
+A stream whose cuts are not known (one chameleon_encode call, the reference library, a file) is cut at byte ranges instead
+(`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
+(density_b200_decode_locate), and after an all_gather of the maps `locate_piece` gives every rank the exact offset where its
+first block starts. The located piece then decodes as above.
 """
 import ctypes
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -76,6 +82,34 @@ def seam_verdict(words):
             bad |= prev_inc and bool(w[r, 0])
             prev_inc = bool(w[r, 1])
     return int(bad), int(offsets[-1]), offsets
+
+
+LOCATE_MAP_WORDS = 266     # DENSITY_B200_LOCATE_MAP_WORDS
+CHUNK = 16384              # non-last ranges are multiples of the boundary walk's chunk
+HALO = 264                 # the largest Chameleon block: every byte a block starting inside a range can reach
+
+
+def stream_ranges(total, world):
+    """[(offset, n_range, n_halo)] per rank for a stream of `total` bytes: equal ranges rounded down to 16 KiB, the last rank takes
+    the rest; each halo is the next min(264, bytes after the range) stream bytes."""
+    per = total // world // CHUNK * CHUNK
+    out = []
+    for r in range(world):
+        off = r * per
+        n = per if r < world - 1 else total - off
+        out.append((off, n, min(HALO, total - off - n)))
+    return out
+
+
+def locate_piece(maps, rank):
+    """density_b200_locate_piece (host only) on the gathered range maps, uint64-compatible [world, 266] in rank order. Returns
+    (start, end, blocks_before, is_final): this rank's piece is its buffer's bytes [start, end)."""
+    m = np.ascontiguousarray(np.asarray(maps).astype(np.uint64, copy=False).reshape(-1, LOCATE_MAP_WORDS))
+    out = (ctypes.c_uint64 * 4)()
+    rc = _lib.load().density_b200_locate_piece(m.ctypes.data, m.shape[0], rank, out)
+    if rc:
+        raise _lib.DensityB200Error(f"locate_piece rc={rc}: {_lib.last_error()}")
+    return tuple(int(v) for v in out)
 
 
 class ShardedChameleonEncoder:
@@ -145,9 +179,38 @@ class ShardedChameleonDecoder:
         d_size: int64[1]. Returns seam_verdict's (flags, total, offsets) over all ranks; flags != 0: the pieces are void."""
         rank = dist.get_rank(group) if dist.is_initialized() else 0
         world = dist.get_world_size(group) if dist.is_initialized() else 1
+        return self._decode_piece(d_in, d_out, d_size, rank == world - 1, group)
+
+    def decode_stream(self, d_in, n_range, d_out, d_size, group=None):
+        """Decode of a stream without known cuts. d_in: CUDA uint8 tensor (2-byte aligned), this rank's range (its first n_range bytes)
+        followed by its halo (stream_ranges gives the layout); d_out, d_size as in decode. Locates the piece (one host synchronisation
+        for the maps) and decodes it. Returns (flags, total, offsets, my_offset): seam_verdict's result and where this rank's output
+        starts in the original bytes; flags != 0: the pieces are void and the caller decodes the whole stream on one device."""
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        n_halo = d_in.numel() - n_range
+        if n_halo < 0:
+            raise ValueError("d_in is shorter than its range")
+        m = torch.empty(LOCATE_MAP_WORDS, dtype=torch.int64, device=d_in.device)
+        rc = self._lib.density_b200_decode_locate(self._h, d_in.data_ptr(), n_range, n_halo, m.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"decode_locate rc={rc}: {_lib.last_error()}")
+        if world > 1:
+            maps = torch.empty((world, LOCATE_MAP_WORDS), dtype=torch.int64, device=d_in.device)
+            dist.all_gather_into_tensor(maps.view(-1), m, group=group)
+        else:
+            maps = m.view(1, LOCATE_MAP_WORDS)
+        start, end, _, is_final = locate_piece(maps.cpu().numpy().view(np.uint64), rank)
+        flags, total, offsets = self._decode_piece(d_in[start:end], d_out, d_size, bool(is_final), group)
+        return flags, total, offsets, int(offsets[rank])
+
+    def _decode_piece(self, d_in, d_out, d_size, is_last, group):
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=d_in.device)
-        rc = self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(rank == world - 1),
+        rc = self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last),
                                                         table.data_ptr(), stream)
         if rc:
             raise _lib.DensityB200Error(f"decode_shard_phase1 rc={rc}: {_lib.last_error()}")
@@ -188,6 +251,7 @@ class _ShardedHandle:
         if not self._h:
             raise _lib.DensityB200Error(_lib.last_error())
         self.d_total = torch.zeros(1, dtype=torch.int64, device=device)
+        self.d_offset = torch.zeros(1, dtype=torch.int64, device=device)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -239,3 +303,14 @@ class ShardedDecoder(_ShardedHandle):
                                                    d_flags.data_ptr(), self.d_total.data_ptr(), stream)
         if rc:
             raise _lib.DensityB200Error(f"decode_sharded rc={rc}: {_lib.last_error()}")
+
+    def decode_stream(self, d_in, n_range, d_out, d_size, d_flags):
+        """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range
+        bytes) followed by its halo (stream_ranges gives the layout); the rest as in decode. Blocks once, on the range maps.
+        self.d_offset int64[1]: where this rank's output starts in the original bytes."""
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rc = self._lib.density_b200_decode_sharded_stream(self._h, d_in.data_ptr(), n_range, d_in.numel() - n_range, d_out.data_ptr(),
+                                                          d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(), d_flags.data_ptr(),
+                                                          self.d_total.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"decode_sharded_stream rc={rc}: {_lib.last_error()}")

@@ -185,6 +185,41 @@ DENSITY_B200_API int density_b200_decode_sharded(density_b200_sharded*, const ui
                                 uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
+ * Sharded decode of a stream whose cuts are not known: a stream written by one chameleon_encode call, by the reference library,
+ * read from a file, or a gathered sharded stream without its piece sizes. The stream is cut at byte ranges; each rank finds
+ * where its piece starts from the stream itself.
+ *
+ * Input layout. Rank r holds one contiguous device buffer (2-byte aligned): its RANGE, stream bytes [o_r, o_r + n_range_r), followed
+ * by its HALO, the next n_halo_r = min(264, total - o_r - n_range_r) stream bytes (every byte a block starting inside the range can
+ * reach). o_r is the sum of the n_range of the ranks before r; every non-last n_range is a multiple of 16384 (zero is allowed); the
+ * last rank's n_range is any length and its halo is empty. Scattering a stream held by one rank is the caller's job.
+ *
+ * The range map (DENSITY_B200_LOCATE_MAP_WORDS u64): {n_range, n_halo}, then for each of the 132 possible even entry offsets e (2e
+ * bytes into the range) {exit index x: the walk leaves the range at offset n_range + 2x and enters the next range at 2x; or ~0: the
+ * walk reached the end of the stream; number of blocks it walked}.
+ */
+#define DENSITY_B200_LOCATE_MAP_WORDS 266
+/* Enqueues the range map of d_in[0 .. n_range + n_halo) into d_map (device, 8-byte aligned). The scratch lives in the handle's
+   workspace, which the next phase 1 overwrites. The layout is not checked here but by density_b200_locate_piece, which every rank
+   runs on the same gathered maps. */
+DENSITY_B200_API int density_b200_decode_locate(density_b200_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                uint64_t* d_map, void* stream);
+/* Host only, needs no device. h_maps: the range maps of all `world` ranks in rank order. Checks the layout (non-last ranges multiples
+   of 16384, each halo min(264, the bytes of the later ranges); DENSITY_B200_EARG otherwise, on every rank alike) and walks the maps
+   from the stream start to `rank`. out4 = {start, end, blocks_before, is_final}: this rank's piece is d_in[start .. end), it begins
+   after blocks_before blocks, and is_final = 1 when no stream byte follows it. A piece behind the end of the stream is empty. */
+DENSITY_B200_API int density_b200_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out4[4]);
+/* End to end over NCCL on a density_b200_sharded handle: range map -> ncclAllGather(maps) -> one device-to-host copy and ONE host
+   synchronisation (phase 1's launch grid depends on the piece length) -> density_b200_locate_piece -> the path of
+   density_b200_decode_sharded on the located piece. *d_out_offset = where this piece's output starts in the original bytes;
+   *d_flags, *d_total_size as density_b200_decode_sharded (d_out_offset and d_total_size may be NULL). Quiet streams only: a zero
+   verdict proves every cut is a true block boundary (DESIGN.md section 5). For a quiet stream cap >= 2 * (n_range + n_halo) is always
+   enough; a piece whose output does not fit is refused. Uses the handle's decode workspace. */
+DENSITY_B200_API int density_b200_decode_sharded_stream(density_b200_sharded*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                       uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset,
+                                       uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
  * A reused Codec INSTANCE (streaming continuation). In the reference `encode` / `decode` are methods of an instance
  * (/root/reference/src/codec/codec.rs:16,72,82) whose dictionary survives from call to call until clear_state()
  * (chameleon.rs:148-150, cheetah.rs:198-202, lion.rs:327-331), while the protection state is created inside every call

@@ -56,8 +56,6 @@ _SIGS = {
     "density_b200_cheetah_decode_rounds": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint32)]),
     "density_b200_encode_status": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_test_set_stage_rounds": (None, [ctypes.c_int]),
-    "density_b200_test_set_flag_impl": (None, [ctypes.c_int]),
-    "density_b200_test_set_decode_impl": (None, [ctypes.c_int]),
     "density_b200_prot_debug": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_shutdown": (None, []),
     "density_b200_version": (ctypes.c_char_p, []),

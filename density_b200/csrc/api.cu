@@ -1284,10 +1284,6 @@ int density_b200_cheetah_decode_rounds(uint32_t* out4) {
 /* test hook: rounds per stage of the Cheetah / Lion copy-map iteration (1..7; 7 = default) */
 void density_b200_test_set_stage_rounds(int k) { g_chee_stage_rounds = (k >= 1 && k <= 7) ? k : 7; }
 
-/* test / timing hook: which Chameleon flag pass kernel runs (1 = round-1 class protocol, 6 = write / verify / replay, the default) */
-void density_b200_test_set_flag_impl(int k) { g_cham_flag_impl = (k == 1) ? 1 : 6; }
-void density_b200_test_set_decode_impl(int k) { g_cham_decode_impl = (k == 1) ? 1 : 7; }
-
 /* diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed (~0: none),
    number of such blocks}; 16 rounds x 2 values (synchronises) */
 int density_b200_prot_debug(uint64_t* out32) {

@@ -19,13 +19,11 @@
 //     candidate table, the others are walked block by block from shared memory and their copy-mode blocks marked; the
 //     dictionary passes below then run unchanged (a copy-mode block is 64 raw quads that neither read nor write the
 //     dictionary, codec.rs:89-92).
-//  3. Dictionary.  `cham_decode_pass`: one persistent CTA per contiguous run of blocks, the run's dictionary in shared
-//     memory as 16-bit fingerprints (common.cuh). Per tile of 4096 quads: PLAIN quads (~8 %) are the writers, MAP quads the
-//     readers; barrier-phased optimistic protocol — A readers read / B writers publish / C readers re-read; unchanged means
-//     no writer touched the bucket in this tile / D the few readers whose bucket was written resolve exactly (all writers
-//     later than me -> pre-tile value; writers agree and one precedes me -> that value; else search the tile's writer list).
-//     A reader whose bucket has not been written in this run yet cannot know the carried-in dictionary: it is recorded
-//     and patched afterwards from the per-run carry-in tables (same machinery as the encoder).
+//  3. Dictionary.  `cham_decode_pass7`: one persistent CTA per contiguous run of blocks, the run's dictionary in shared
+//     memory as 16-bit fingerprints (common.cuh). PLAIN quads (~7 %) are the writers, MAP quads the readers. A first launch, the
+//     writer pass, looks at the writers only and leaves each run's last-writer table; `dec_carry_scan` folds those tables into the
+//     dictionary each run starts from; a second launch decodes every run from it. Inside a run, tiles of 4096 quads go through a
+//     write / verify / mailbox protocol (see the section comment above the kernel).
 //  4. Tail.  The last < 264 bytes of the stream (codec.rs:102-123: per-unit bounds checks, partial units, 1-3 raw bytes) are
 //     decoded by one thread with the reference's literal control flow, starting from the folded dictionary.
 //  5. Sharded decode (DESIGN §5).  One piece of a sharded stream in two phases: phase 1 (boundaries, writer pass) needs no carry-in
@@ -44,308 +42,21 @@ using bounds::ldu16;
 using T = bounds::ChamT;     // boundaries: decode_bounds.cuh (shared with the Cheetah decoder)
 
 // ---- 3. decode pass ---------------------------------------------------------------------------------------------------------
-constexpr int DP_THREADS = 1024;
-constexpr int DP_QPT = 4;
-constexpr int TILE_Q = DP_THREADS * DP_QPT;   // 4096 quads = 64 blocks
-constexpr int SIDE_N = 4096;
-constexpr uint32_t SIDE_EMPTY = 0xFFFFFFFFu;
-
-// writer record: x = hash | fp << 16, y = pos(12) | agree-flag etc.   suspect reader record: x = hash | w << 16, y = pos | touched << 12 | fa << 16
-constexpr uint32_t W_CONF = 1u << 12;
-constexpr uint32_t S_TOUCHED = 1u << 12;
-
-struct DecSmem {
-    uint16_t tab[65536];
-    uint32_t vbit[2048];
-    uint32_t conf[2048];          // per-tile: writers of the bucket disagree
-    uint32_t wbit[2048];          // per-tile: bucket has a writer in this tile
-    uint32_t side[SIDE_N];        // per-tile min over writers of (pos << 16 | hash)
-    uint2 wrec[TILE_Q];           // writers (plain quads) of the tile from the front; suspect readers (readers whose bucket is written in
-                                  // this tile) from the back: a quad is one or the other, so the two lists never meet
-    unsigned long long boff[2][64];  // stream offset of each block of the tile (double buffered: next tile staged early)
-    uint32_t bsig[2][128];           // signature halves
-    uint32_t bcopy[2][2];            // copy-mode blocks of the tile (bit per block)
-    uint32_t nw, ns;
-};
-static_assert(sizeof(DecSmem) <= 227 * 1024, "decode pass shared memory");
+constexpr int TILE_Q = 4096;   // quads per tile = 64 blocks
 
 __device__ __forceinline__ bool bit_test(const uint32_t* bm, uint32_t i) { return (bm[i >> 5] >> (i & 31)) & 1u; }
 
-// WONLY = true: "writer pass" — only the PLAIN quads are looked at; produces each run's last-writer table so that the
-// carry-in dictionary of every run is known before the real decode pass starts (a MAP quad cannot tell what its bucket
-// held at the start of the run). WONLY = false: the decode pass proper, dictionary preloaded from `carry`.
-// Stage block offsets + signatures of the tile starting at block b0 into buffer `buf` (first 64 threads).
-__device__ __forceinline__ void stage_tile(DecSmem& S, int buf, const uint8_t* __restrict__ in, const uint64_t* __restrict__ blk_off,
-                                           uint64_t b0, uint64_t nblocks) {
-    const uint32_t tid = threadIdx.x;
-    if (tid < 64) {     // warps 0 and 1, whole warps
-        unsigned long long o = 0; uint32_t lo = 0, hi = 0; bool copied = false;
-        if (b0 + tid < nblocks) {
-            o = blk_off[b0 + tid];
-            copied = (o & BLK_COPY) != 0;
-            o &= ~BLK_COPY;
-            if (!copied) {
-                const uint8_t* p = in + o;
-                lo = ldu16(p) | (ldu16(p + 2) << 16); hi = ldu16(p + 4) | (ldu16(p + 6) << 16);
-                o += 8;                       // payload starts behind the signature
-            }                                 // copy-mode block: 64 raw quads = "all PLAIN" payload right at the block start
-        }
-        S.boff[buf][tid] = o; S.bsig[buf][2 * tid] = lo; S.bsig[buf][2 * tid + 1] = hi;
-        const uint32_t cmask = __ballot_sync(0xFFFFFFFFu, copied);
-        if ((tid & 31) == 0) S.bcopy[buf][tid >> 5] = cmask;
-    }
-}
-// Issue the payload loads of my DP_QPT quads of the tile staged in `buf`: MAP -> 16-bit hash, PLAIN -> the quad.
-template <bool WONLY>
-__device__ __forceinline__ void fetch_payload(const DecSmem& S, int buf, const uint8_t* __restrict__ in, uint32_t nb_tile, uint32_t (&v)[DP_QPT]) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int j = 0; j < DP_QPT; ++j) {
-        const uint32_t bl = warp * 2 + (j >> 1);
-        const uint32_t k = (j & 1) * 32 + lane;
-        v[j] = 0;
-        if (bl < nb_tile) {
-            const uint32_t lo = S.bsig[buf][2 * bl], hi = S.bsig[buf][2 * bl + 1];
-            const uint32_t flag = (((j & 1) ? hi : lo) >> lane) & 1u;
-            const uint32_t before = (j & 1) ? (__popc(lo) + __popc(hi & lanemask_lt())) : __popc(lo & lanemask_lt());
-            const uint8_t* p = in + S.boff[buf][bl] + 4 * k - 2 * before;
-            if (flag) { if (!WONLY) v[j] = ldu16(p); }                       // decode_map reads the 16-bit hash (chameleon.rs:64)
-            else v[j] = ldu16(p) | (ldu16(p + 2) << 16);                     // decode_plain reads the quad (chameleon.rs:56)
-        }
-    }
-}
-
-template <bool WONLY>
-__global__ void __launch_bounds__(DP_THREADS, 1)
-cham_decode_pass(const uint8_t* __restrict__ in, const uint64_t* __restrict__ blk_off, DecStatus* st,
-                 uint32_t nruns, uint32_t* __restrict__ out /* quads */, const uint32_t* __restrict__ carry,
-                 uint32_t* __restrict__ final_tab) {
-    if (st->nonquiet || st->error) return;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    DecSmem& S = *reinterpret_cast<DecSmem*>(smem_raw);
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t run = blockIdx.x;
-    const uint64_t nblocks = st->main_blocks;
-    const uint64_t ntiles = (nblocks + 63) / 64;
-    const uint64_t t_begin = (uint64_t)run * ntiles / nruns, t_end = (uint64_t)(run + 1) * ntiles / nruns;
-
-    {
-        uint4 z = make_uint4(0, 0, 0, 0);
-        uint4* t4 = reinterpret_cast<uint4*>(S.tab);
-        for (uint32_t i = tid; i < 65536 * 2 / 16; i += DP_THREADS) t4[i] = z;
-        for (uint32_t i = tid; i < 2048; i += DP_THREADS) { S.vbit[i] = 0; S.conf[i] = 0; S.wbit[i] = 0; }
-        if (!WONLY) {
-            __syncthreads();
-            const uint32_t* __restrict__ cr = carry + (size_t)run * 65536;   // dictionary before this run
-            for (uint32_t i = tid; i < 65536; i += DP_THREADS) {
-                const uint32_t c = cr[i];
-                if (c & 0x10000u) {
-                    S.tab[i] = (uint16_t)c;
-                    if ((c & 0xFFFFu) == 0) atomicOr(&S.vbit[i >> 5], 1u << (i & 31));
-                }
-            }
-        }
-        for (uint32_t i = tid; i < SIDE_N; i += DP_THREADS) S.side[i] = SIDE_EMPTY;
-        if (tid == 0) { S.nw = 0; S.ns = 0; }
-    }
-    __syncthreads();
-
-    // prologue: stage the first tile and issue its payload loads
-    uint32_t nval[DP_QPT];
-    if (t_begin < t_end) stage_tile(S, 0, in, blk_off, t_begin * 64, nblocks);
-    __syncthreads();
-    if (t_begin < t_end) fetch_payload<WONLY>(S, 0, in, (uint32_t)((nblocks - t_begin * 64 < 64) ? (nblocks - t_begin * 64) : 64), nval);
-
-    for (uint64_t t = t_begin; t < t_end; ++t) {
-        const uint64_t b0 = t * 64;
-        const uint32_t nb_tile = (uint32_t)((nblocks - b0 < 64) ? (nblocks - b0) : 64);
-        const int cur = (int)((t - t_begin) & 1);
-        // stage the NEXT tile's offsets + signatures now; they become visible at S1 and feed the payload prefetch
-        if (t + 1 < t_end) stage_tile(S, cur ^ 1, in, blk_off, b0 + 64, nblocks);
-
-        // ---- phase A: my quads (prefetched); writers compact themselves; readers read the pre-tile dictionary ----------
-        uint32_t val[DP_QPT];       // PLAIN: the quad; MAP: hash from the stream
-        uint32_t fa[DP_QPT];        // readers: pre-tile fingerprint
-        uint32_t kind = 0;          // per sub-row: bit j = active, bit 4+j = writer, bit 8+j = reader bucket touched pre-tile, bit 12+j = raw (copy mode)
-        uint32_t wb[DP_QPT], wtot = 0;
-#pragma unroll
-        for (int j = 0; j < DP_QPT; ++j) {
-            const uint32_t bl = warp * 2 + (j >> 1);
-            bool active = bl < nb_tile, writer = false;
-            val[j] = nval[j]; fa[j] = 0;
-            if (active) {
-                const uint32_t flag = (S.bsig[cur][2 * bl + (j & 1)] >> lane) & 1u;
-                if ((S.bcopy[cur][bl >> 5] >> (bl & 31)) & 1u) {
-                    kind |= 1u << (12 + j);             // raw quad of a copy-mode block: no dictionary access at all
-                } else if (flag) {
-                    if (!WONLY) {
-                        fa[j] = S.tab[val[j]];
-                        if (fa[j] != 0 || bit_test(S.vbit, val[j])) kind |= 1u << (8 + j);
-                    }
-                } else {
-                    writer = true;
-                }
-                kind |= 1u << j;
-            }
-            if (writer) kind |= 1u << (4 + j);
-            wb[j] = __ballot_sync(0xFFFFFFFFu, writer);
-            wtot += __popc(wb[j]);
-        }
-        if (wtot) {
-            uint32_t base = 0;
-            if (lane == 0) base = atomicAdd(&S.nw, wtot);
-            base = __shfl_sync(0xFFFFFFFFu, base, 0);
-#pragma unroll
-            for (int j = 0; j < DP_QPT; ++j) {
-                if (kind & (1u << (4 + j))) {
-                    const uint32_t p = hash_prod(val[j]);
-                    S.wrec[base + __popc(wb[j] & lanemask_lt())] = make_uint2(prod_hash(p) | (prod_fp(p, val[j]) << 16), warp * 128 + j * 32 + lane);
-                }
-                base += __popc(wb[j]);
-            }
-        }
-        __syncthreads();  // S1: readers have read tab; writer list complete; next tile's signatures staged
-        const uint32_t nw = S.nw;
-        if (t + 1 < t_end)   // payload of the next tile: in flight during phases B-D
-            fetch_payload<WONLY>(S, cur ^ 1, in, (uint32_t)((nblocks - (b0 + 64) < 64) ? (nblocks - (b0 + 64)) : 64), nval);
-
-        // ---- phase B: writers publish ----------------------------------------------------------------------------------
-#pragma unroll 1
-        for (uint32_t i = tid; i < nw; i += DP_THREADS) {
-            const uint2 r = S.wrec[i];
-            const uint32_t hh = r.x & 0xFFFFu;
-            S.tab[hh] = (uint16_t)(r.x >> 16);
-            atomicMin(&S.side[hh & (SIDE_N - 1)], ((r.y & 0xFFFu) << 16) | hh);
-            atomicOr(&S.wbit[hh >> 5], 1u << (hh & 31));
-        }
-        __syncthreads();  // S2
-
-        // ---- phase C: readers re-read; writers check agreement ---------------------------------------------------------
-        const uint64_t q0 = b0 * 64;   // first output quad of the tile
-        if (!WONLY) {
-#pragma unroll
-            for (int j = 0; j < DP_QPT; ++j) {
-                const uint32_t pos = warp * 128 + j * 32 + lane;
-                const bool active = kind & (1u << j), writer = kind & (1u << (4 + j));
-                const bool touched = kind & (1u << (8 + j));
-                bool suspect = false;
-                if (active) {
-                    if (writer || (kind & (1u << (12 + j)))) {
-                        out[q0 + pos] = val[j];
-                    } else if (!bit_test(S.wbit, val[j])) {
-                        // no PLAIN quad of this tile falls into my bucket: the pre-tile dictionary decides (empty -> 0, chameleon.rs:41)
-                        out[q0 + pos] = touched ? quad_from_hf(val[j], fa[j]) : 0u;
-                    } else {
-                        suspect = true;
-                    }
-                }
-                const uint32_t sm = __ballot_sync(0xFFFFFFFFu, suspect);
-                if (sm) {
-                    uint32_t base = 0;
-                    if (lane == 0) base = atomicAdd(&S.ns, (uint32_t)__popc(sm));
-                    base = __shfl_sync(0xFFFFFFFFu, base, 0);
-                    if (suspect) {
-                        const uint32_t e = base + __popc(sm & lanemask_lt());
-                        S.wrec[TILE_Q - 1 - e] = make_uint2(val[j], pos | (touched ? S_TOUCHED : 0u) | (fa[j] << 16));
-                    }
-                }
-            }
-        }
-#pragma unroll 1
-        for (uint32_t i = tid; i < nw; i += DP_THREADS) {
-            const uint2 r = S.wrec[i];
-            const uint32_t hh = r.x & 0xFFFFu;
-            const uint32_t slot = S.side[hh & (SIDE_N - 1)];
-            if ((slot & 0xFFFFu) != hh || S.tab[hh] != (r.x >> 16)) {   // foreign slot owner, or the writers of my bucket disagree
-                S.wrec[i].y = r.y | W_CONF;
-                atomicOr(&S.conf[hh >> 5], 1u << (hh & 31));
-            }
-        }
-        __syncthreads();  // S3
-        const uint32_t ns = S.ns;
-
-        // ---- phase D: suspect readers resolve; writers of disagreeing buckets leave the last value ----------------------
-        if (!WONLY) {
-#pragma unroll 1
-            for (uint32_t base = warp * 32; base < ns; base += DP_THREADS) {
-                const uint32_t i = base + lane;
-                uint32_t hs = 0, pos = 0, fval = 0; bool have = false, search = false;
-                if (i < ns) {
-                    const uint2 r = S.wrec[TILE_Q - 1 - i];
-                    hs = r.x & 0xFFFFu; pos = r.y & 0xFFFu;
-                    fval = r.y >> 16; have = (r.y & S_TOUCHED) != 0;             // pre-tile value
-                    const uint32_t slot = S.side[hs & (SIDE_N - 1)];
-                    if ((slot & 0xFFFFu) == hs && pos < (slot >> 16)) {
-                        // every writer of my bucket comes after me: pre-tile value
-                    } else if ((slot & 0xFFFFu) == hs && !bit_test(S.conf, hs)) {
-                        fval = S.tab[hs]; have = true;                           // the writers agree and the first one precedes me
-                    } else {
-                        search = true;                                           // disagreeing writers, or the side slot belongs to another bucket
-                    }
-                }
-                // warp-cooperative search of the tile's writer list for the predecessor of each lane that needs it
-                uint32_t todo = __ballot_sync(0xFFFFFFFFu, search);
-                while (todo) {
-                    const int src = __ffs(todo) - 1; todo &= todo - 1;
-                    const uint32_t shs = __shfl_sync(0xFFFFFFFFu, hs, src), spos = __shfl_sync(0xFFFFFFFFu, pos, src);
-                    uint32_t key = 0;
-                    for (uint32_t k = lane; k < nw; k += 32) {
-                        const uint2 d = S.wrec[k];
-                        const uint32_t pk = d.y & 0xFFFu;
-                        if ((d.x & 0xFFFFu) == shs && pk < spos) key = max(key, ((pk + 1) << 16) | (d.x >> 16));
-                    }
-                    key = __reduce_max_sync(0xFFFFFFFFu, key);
-                    if ((int)lane == src && key) { fval = key & 0xFFFFu; have = true; }
-                }
-                if (i < ns) out[q0 + pos] = have ? quad_from_hf(hs, fval) : 0u;
-            }
-        }
-#pragma unroll 1
-        for (uint32_t base = warp * 32; base < nw; base += DP_THREADS) {
-            const uint32_t i = base + lane;
-            uint32_t hh = 0x10000u, ff = 0, pos = 0; bool confw = false;
-            if (i < nw) {
-                const uint2 r = S.wrec[i];
-                hh = r.x & 0xFFFFu; ff = r.x >> 16; pos = r.y & 0xFFFu; confw = (r.y & W_CONF) != 0;
-                if (ff == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
-            }
-            // writers of disagreeing buckets: the last one (largest position) leaves its value (chameleon.rs:59)
-            uint32_t todo = __ballot_sync(0xFFFFFFFFu, confw);
-            while (todo) {
-                const int src = __ffs(todo) - 1; todo &= todo - 1;
-                const uint32_t shh = __shfl_sync(0xFFFFFFFFu, hh, src), spos = __shfl_sync(0xFFFFFFFFu, pos, src);
-                bool later = false;
-                for (uint32_t k = lane; k < nw; k += 32) {
-                    const uint2 d = S.wrec[k];
-                    later |= (d.x & 0xFFFFu) == shh && (d.y & 0xFFFu) > spos;
-                }
-                later = __any_sync(0xFFFFFFFFu, later);
-                if ((int)lane == src && !later) S.tab[hh] = (uint16_t)ff;
-            }
-        }
-        __syncthreads();  // S4: all readers of conf/side/lists done
-#pragma unroll 1
-        for (uint32_t i = tid; i < nw; i += DP_THREADS) {
-            const uint2 r = S.wrec[i];
-            if (r.y & W_CONF) atomicAnd(&S.conf[(r.x & 0xFFFFu) >> 5], ~(1u << (r.x & 31)));
-            atomicAnd(&S.wbit[(r.x & 0xFFFFu) >> 5], ~(1u << (r.x & 31)));
-            S.side[(r.x & 0xFFFFu) & (SIDE_N - 1)] = SIDE_EMPTY;
-        }
-        if (tid == 0) { S.nw = 0; S.ns = 0; }
-        __syncthreads();  // S5: counters reset before the next tile's phase A
-    }
-
-    for (uint32_t i = tid; i < 65536; i += DP_THREADS) {
-        uint32_t v = S.tab[i];
-        uint32_t tch = (v != 0 || bit_test(S.vbit, i)) ? 0x10000u : 0u;
-        final_tab[(size_t)run * 65536 + i] = v | tch;
-    }
-}
-
 // ------------------------------------------------------------------------------------------------------------------------------
-// Decode pass, second formulation (same contract as cham_decode_pass; the structure of the round-2 encoder flag pass,
-// chameleon_encode.cu cham_flag_pass6: nothing but loads, compares and ballots on the per-quad path; atomics and searches only on
-// the few "dirty" quads, one record per lane).  512 threads, 8 quads per thread, tile = 4096 quads = 64 blocks:
+// Decode pass: the structure of the encoder's flag pass (chameleon_encode.cu cham_flag_pass6): nothing but loads, compares and ballots
+// on the per-quad path; atomics and searches only on the few "dirty" quads, one record per lane.
+// One persistent CTA per run: run r owns tiles [r * ntiles / nruns, (r + 1) * ntiles / nruns) of the st->main_blocks blocks (blk_off:
+// each block's stream offset and copy-mode bit) and keeps the run's dictionary in shared memory as 16-bit fingerprints. Nothing runs
+// when st reports a non-quiet stream or an error. Both instances leave the run's last-writer table in final_tab (65536 x
+// touched << 16 | fp per run).
+// WONLY = true: "writer pass" — only the PLAIN quads are looked at; produces each run's last-writer table so that the carry-in
+// dictionary of every run is known before the real decode pass starts (a MAP quad cannot tell what its bucket held at the start of
+// the run). WONLY = false: the decode pass proper, dictionary preloaded from `carry`, every quad of the run written to `out`.
+// 512 threads, 8 quads per thread, tile = 4096 quads = 64 blocks:
 //   A  readers (MAP quads) read the pre-tile dictionary; writers (PLAIN quads, ~7 %) compute hash and fingerprint.        (barrier)
 //   B  writers store their fingerprint (racy on purpose) and raise the bucket's byte in a hashed per-tile mark map.        (barrier)
 //   C  raw and PLAIN quads go out as they are; a reader whose mark byte is clear saw no writer of its bucket in this tile: the
@@ -353,7 +64,7 @@ cham_decode_pass(const uint8_t* __restrict__ in, const uint64_t* __restrict__ bl
 //      the warp's record region; writers drop their record index into the mailbox of their bucket (4096 slots x 4 + overflow).  (barrier)
 //   D  one record per lane: a suspect takes the fingerprint of the writer with the largest smaller index in its bucket, or its own
 //      pre-tile value; the writer without a successor leaves the bucket's final fingerprint and clears the mark.            (barrier)
-// WONLY (writer pass: the run's last-writer table only) needs A, the deposit and D.
+// The writer pass needs A, the deposit and D.
 // A mailbox overflow (more than ~20 PLAIN quads of one bucket in one tile) sends the tile to d7_replay (one warp, in order).
 // ------------------------------------------------------------------------------------------------------------------------------
 constexpr int D7_THREADS = 512, D7_QPT = 8, D7_NW = D7_THREADS / 32, D7_WQ = 32 * D7_QPT;
@@ -874,8 +585,6 @@ __global__ void dec_seam_words_k(const uint8_t* __restrict__ in, uint64_t n, con
 
 using namespace chamdec;
 
-int g_cham_decode_impl = 7;   // 1: round-1 decode pass, 7: write / verify / mailbox (timing comparisons and tests)
-
 struct ChamDecLayout { bounds::BoundsLayout B; size_t final_tab, carry, dict, total; };
 
 static size_t dec_layout(size_t nbytes, size_t cap, int nruns_max, ChamDecLayout* L) {
@@ -903,9 +612,7 @@ cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, u
                                cudaStream_t stream, uint64_t* launches) {
     static bool attr_done = false;
     if (!attr_done) {
-        cudaError_t e0 = cudaFuncSetAttribute(cham_decode_pass<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DecSmem));
-        if (e0 == cudaSuccess) e0 = cudaFuncSetAttribute(cham_decode_pass<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DecSmem));
-        if (e0 == cudaSuccess) e0 = cudaFuncSetAttribute(cham_decode_pass7<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Dec7Smem));
+        cudaError_t e0 = cudaFuncSetAttribute(cham_decode_pass7<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Dec7Smem));
         if (e0 == cudaSuccess) e0 = cudaFuncSetAttribute(cham_decode_pass7<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Dec7Smem));
         if (e0 != cudaSuccess) return e0;
         attr_done = true;
@@ -917,8 +624,7 @@ cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, u
     if (e != cudaSuccess) return e;
     const uint32_t nruns = dec_pick_runs(L, num_sms);
     uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
-    if (g_cham_decode_impl == 1) cham_decode_pass<true><<<nruns, DP_THREADS, sizeof(DecSmem), stream>>>(d_in, blk_off, st, nruns, nullptr, nullptr, final_tab);
-    else cham_decode_pass7<true><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, nullptr, nullptr, final_tab);
+    cham_decode_pass7<true><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, nullptr, nullptr, final_tab);
     ++*launches;
     if (d_table_out) {
         dec_export_fold<<<65536 / 256, 256, 0, stream>>>(final_tab, nruns, d_table_out);
@@ -939,8 +645,7 @@ cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_ou
     uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
     uint32_t* carry = reinterpret_cast<uint32_t*>(ws + L.carry);
     dec_carry_scan<<<65536 / 256, 256, 0, stream>>>(final_tab, nruns, carry, reinterpret_cast<uint32_t*>(ws + L.dict), d_carry_in); ++*launches;
-    if (g_cham_decode_impl == 1) cham_decode_pass<false><<<nruns, DP_THREADS, sizeof(DecSmem), stream>>>(d_in, blk_off, st, nruns, reinterpret_cast<uint32_t*>(d_out), carry, final_tab);
-    else cham_decode_pass7<false><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, reinterpret_cast<uint32_t*>(d_out), carry, final_tab);
+    cham_decode_pass7<false><<<nruns, D7_THREADS, sizeof(Dec7Smem), stream>>>(d_in, blk_off, st, nruns, reinterpret_cast<uint32_t*>(d_out), carry, final_tab);
     ++*launches;
     dec_tail<<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, reinterpret_cast<uint32_t*>(ws + L.dict), st, d_out_size); ++*launches;
     return cudaGetLastError();

@@ -10,14 +10,11 @@
 //   flag_i = 1  <=>  the previous quad in the same hash bucket (in stream order, skipping copy-mode blocks)
 //                    equals quad_i; an empty bucket behaves as "holds quad 0".
 //
-// Pass 1  cham_flag_pass      one persistent CTA per SM; CTA r owns the contiguous run r of the stream and
-//                             keeps the run's dictionary in shared memory as 16-bit fingerprints (128 KiB,
-//                             see common.cuh). It walks the run in tiles of 4096 quads; inside a tile the
-//                             "previous in bucket" relation is resolved with a barrier-phased optimistic
-//                             protocol (A read / B racy publish / C read back / D classify) and a small
-//                             in-order slow path for buckets that really interleave different values.
-//                             First touches of a bucket inside a run cannot know the dictionary carried in
-//                             from earlier runs; they are recorded in an "unresolved" list.
+// Pass 1  cham_flag_pass6     one persistent CTA per SM; CTA r owns the contiguous run r of the stream, keeps the run's
+//                             dictionary in shared memory as 16-bit fingerprints and walks the run in tiles of 4096 quads
+//                             (write / verify / mailbox; see the section comment above the kernel). First touches of a bucket
+//                             inside a run cannot know the dictionary carried in from earlier runs; they are recorded in an
+//                             "unresolved" list.
 //         cham_carry_scan     per-bucket left fold of the runs' last-writer tables -> carry-in table per run.
 //         cham_resolve        patches the unresolved flags from the carry-in tables.
 //         cham_tile_sizes     per-block output sizes -> per-tile byte counts; detects whether the reference's
@@ -36,366 +33,17 @@ namespace dns {
 namespace cham {
 
 // ------------------------------------------------------------------------------------------------------
-// Pass 1: flag pass
-// ------------------------------------------------------------------------------------------------------
-constexpr int FP_THREADS = 1024;
-constexpr int FP_QPT = 4;                          // quads per thread per tile
-constexpr int TILE_Q = FP_THREADS * FP_QPT;        // 4096 quads = 16 KiB = 64 blocks
-constexpr int SIDE_N = 8192;                       // first-misser table (u32), indexed by hash & (SIDE_N-1)
-constexpr uint32_t SIDE_EMPTY = 0xFFFFFFFFu;
-
-constexpr int CLS_N = 32;                          // slow-path classes: class = hash >> 11, one warp each
-constexpr int CLS_CAP = 128;                       // entries per class list; overflow -> in-order tile fallback
-
-// Compacted per-tile record of a misser (or of a hit member that turned out to need the slow path):
-//   x = hash | fp << 16
-//   y = pos(12) | touched << 12 | slow << 13 | first << 14 | setter << 15 | old_fp << 16
-constexpr uint32_t R_TOUCHED = 1u << 12, R_SLOW = 1u << 13, R_FIRST = 1u << 14;
-
-struct FlagSmem {
-    uint16_t tab[65536];          // fingerprint of the last quad seen in each bucket
-    uint32_t vbit[2048];          // "bucket touched" for the one case tab cannot express (fingerprint 0)
-    uint32_t conf[2048];          // per-tile conflict bits (bucket interleaves different values)
-    uint32_t side[SIDE_N];        // per-tile min over missers of (pos << 16 | hash)
-    uint2 rec[TILE_Q];            // records: missers (phase A) then slow hit members (phase C); quad staging in the fallback
-    uint16_t cls_list[CLS_N][CLS_CAP];  // record indices of the slow members of each class (unordered)
-    uint32_t cls_count[CLS_N];
-    uint32_t sigw[TILE_Q / 32];   // flag bits of the tile: word (w*4+j) = sub-row j of warp w
-    uint32_t nrec;
-    uint32_t unres_count;
-    uint32_t cls_overflow;
-};
-static_assert(sizeof(FlagSmem) <= 227 * 1024, "flag pass shared memory");
-
-__device__ __forceinline__ bool bit_test(const uint32_t* bm, uint32_t i) { return (bm[i >> 5] >> (i & 31)) & 1u; }
-
-// Append the lanes with `pred` set to the run's unresolved list (warp-aggregated). Must be called by all 32 lanes.
-__device__ __forceinline__ void append_unres(bool pred, uint32_t qidx_in_run, uint32_t h, uint32_t f,
-                                             uint32_t* s_count, uint2* __restrict__ unres_run) {
-    uint32_t m = __ballot_sync(0xFFFFFFFFu, pred);
-    if (m == 0) return;
-    uint32_t base = 0;
-    const uint32_t lane = threadIdx.x & 31;
-    if (lane == 0) base = atomicAdd(s_count, (uint32_t)__popc(m));
-    base = __shfl_sync(0xFFFFFFFFu, base, 0);
-    if (pred) {
-        uint32_t idx = base + __popc(m & lanemask_lt());
-        if (idx < 65536u) unres_run[idx] = make_uint2(qidx_in_run, h | (f << 16));
-    }
-}
-
-// In-order walk of one whole tile by one warp, from the (restored) pre-tile dictionary. Fallback for tiles whose
-// class lists overflow (adversarial inputs: hundreds of interleaving quads in a handful of buckets).
-__device__ __noinline__ void tile_in_order(FlagSmem& S, const uint32_t* qs, uint32_t rem, uint32_t run_q0,
-                                           uint2* __restrict__ unres_run, const uint8_t* __restrict__ cm_tile) {
-    const uint32_t lane = threadIdx.x & 31;
-    for (uint32_t c = 0; c < TILE_Q / 32; ++c) {
-        const uint32_t pos = c * 32 + lane;
-        const bool valid = pos < rem && !(cm_tile && cm_tile[pos >> 6]);   // copy-mode blocks never touch the dictionary (codec.rs:35-37)
-        const uint32_t q = qs[pos];
-        const uint32_t p = hash_prod(q);
-        const uint32_t hh = valid ? prod_hash(p) : 0x10000u + lane;
-        const uint32_t ff = prod_fp(p, q);
-        uint32_t cur = 0; bool touched = false;
-        if (valid) { cur = S.tab[hh]; touched = cur != 0 || bit_test(S.vbit, hh); }
-        const uint32_t grp = __match_any_sync(0xFFFFFFFFu, hh);
-        const uint32_t lower = grp & lanemask_lt();
-        const int pl = lower ? 31 - __clz(lower) : 0;
-        const uint32_t fprev = __shfl_sync(0xFFFFFFFFu, ff, pl);
-        const bool hit = valid && (lower ? (fprev == ff) : (touched && cur == ff));
-        const bool is_last = (grp & lanemask_gt()) == 0;
-        if (valid && is_last && (lower || !hit)) {
-            S.tab[hh] = (uint16_t)ff;
-            if (ff == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
-        }
-        const uint32_t fb = __ballot_sync(0xFFFFFFFFu, hit);
-        if (lane == 0) S.sigw[c] = fb;
-        append_unres(valid && !lower && !touched, run_q0 + pos, hh, ff, &S.unres_count, unres_run);
-        __syncwarp();
-    }
-}
-
-__global__ void __launch_bounds__(FP_THREADS, 1)
-cham_flag_pass(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles_total, uint32_t nruns,
-               uint32_t* __restrict__ sigw_g,        // 2 x u32 per block (low half first)
-               uint2* __restrict__ unres,            // nruns x 65536
-               uint32_t* __restrict__ unres_count,   // nruns
-               uint32_t* __restrict__ final_tab,     // nruns x 65536: touched << 16 | fp
-               const uint8_t* __restrict__ copymap,  // optional: 1 byte per block, non-zero = copy-mode block (skipped)
-               const Status* __restrict__ gate)      // optional: run only while the protection iteration is still open
-{
-    if (gate && !(gate->nonquiet && !gate->converged)) return;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    FlagSmem& S = *reinterpret_cast<FlagSmem*>(smem_raw);
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t run = blockIdx.x;
-    const uint64_t t_begin = (uint64_t)run * tiles_total / nruns;
-    const uint64_t t_end = (uint64_t)(run + 1) * tiles_total / nruns;
-    uint2* __restrict__ unres_run = unres + (size_t)run * 65536;
-    const uint32_t pos0 = warp * 128 + lane;  // position of my sub-row 0 quad inside a tile; sub-row j adds 32*j
-    // run-relative 32-bit geometry (a run is < 2^32 quads): keeps 64-bit compares out of the tile loop
-    const uint32_t ntile_run = (uint32_t)(t_end - t_begin);
-    const uint64_t q_begin = t_begin * TILE_Q;
-    const uint64_t q_end64 = (t_end * TILE_Q < nquads) ? t_end * TILE_Q : nquads;
-    const uint32_t run_quads = q_begin < q_end64 ? (uint32_t)(q_end64 - q_begin) : 0u;
-    const uint32_t* __restrict__ rin = in + q_begin;
-    uint32_t* __restrict__ rsig = sigw_g + t_begin * (TILE_Q / 32);
-    const uint8_t* __restrict__ rcm = copymap ? copymap + t_begin * 64 : nullptr;
-
-    // ---- init shared state -------------------------------------------------------------------------
-    {
-        uint4 z = make_uint4(0, 0, 0, 0);
-        uint4* t4 = reinterpret_cast<uint4*>(S.tab);
-        #pragma unroll 1
-        for (uint32_t i = tid; i < 65536 * 2 / 16; i += FP_THREADS) t4[i] = z;
-        #pragma unroll 1
-        for (uint32_t i = tid; i < 2048; i += FP_THREADS) { S.vbit[i] = 0; S.conf[i] = 0; }
-        #pragma unroll 1
-        for (uint32_t i = tid; i < SIDE_N; i += FP_THREADS) S.side[i] = SIDE_EMPTY;
-        if (tid < CLS_N) S.cls_count[tid] = 0;
-        if (tid == 0) { S.unres_count = 0; S.cls_overflow = 0; S.nrec = 0; }
-    }
-    __syncthreads();
-
-    // ---- prefetch the first tile --------------------------------------------------------------------
-    uint32_t nxt[FP_QPT];
-#pragma unroll
-    for (int j = 0; j < FP_QPT; ++j) nxt[j] = (pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + pos0 + 32 * j) : 0u;
-
-#ifdef DNS_PHASE_TIMING
-    long long ph[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tprev = clock64();
-#define DNS_PH(k) { long long tn = clock64(); ph[k] += tn - tprev; tprev = tn; }
-#else
-#define DNS_PH(k)
-#endif
-    #pragma unroll 1
-    for (uint32_t lt = 0; lt < ntile_run; ++lt) {
-        uint32_t q[FP_QPT], h[FP_QPT], f[FP_QPT];
-        const uint32_t run_q0 = lt * TILE_Q;                                  // first quad of the tile, relative to the run
-        const uint32_t left = run_q0 < run_quads ? run_quads - run_q0 : 0u;   // quads left in the run from here
-        const uint32_t rem = left < (uint32_t)TILE_Q ? left : (uint32_t)TILE_Q;
-#pragma unroll
-        for (int j = 0; j < FP_QPT; ++j) q[j] = nxt[j];
-        {   // prefetch next tile (register double buffer; consumed one full tile later)
-            const uint32_t nleft = left > (uint32_t)TILE_Q ? left - TILE_Q : 0u;
-            const uint32_t* __restrict__ np = rin + run_q0 + TILE_Q + pos0;
-#pragma unroll
-            for (int j = 0; j < FP_QPT; ++j) nxt[j] = (pos0 + 32 * j < nleft) ? ld_stream_u32(np + 32 * j) : 0u;
-        }
-
-        uint32_t actmask = 0;     // bit j: my sub-row j quad exists and its block is not in copy mode
-        {
-            uint32_t cp = 0;      // bit 0/1: block 2*warp / 2*warp+1 of this tile is a copy-mode block
-            if (rcm) cp = (rcm[lt * 64 + warp * 2] ? 1u : 0u) | (rcm[lt * 64 + warp * 2 + 1] ? 2u : 0u);
-#pragma unroll
-            for (int j = 0; j < FP_QPT; ++j)
-                if (pos0 + 32 * j < rem && !((cp >> (j >> 1)) & 1u)) actmask |= 1u << j;
-        }
-        // ---- phase A: read the pre-tile dictionary; compact the missers into S.rec --------------------
-        uint32_t missmask = 0;    // bit j: my sub-row j quad missed
-        {
-            uint32_t old[FP_QPT], tch = 0;
-#pragma unroll
-            for (int j = 0; j < FP_QPT; ++j) {
-                const uint32_t p = hash_prod(q[j]);
-                h[j] = prod_hash(p);
-                f[j] = prod_fp(p, q[j]);
-                old[j] = S.tab[h[j]];
-            }
-            uint32_t mb[FP_QPT], tot = 0;
-#pragma unroll
-            for (int j = 0; j < FP_QPT; ++j) {
-                bool touched = old[j] != 0;
-                if (!touched) touched = bit_test(S.vbit, h[j]);
-                if (touched) tch |= 1u << j;
-                const bool miss = ((actmask >> j) & 1u) && !(touched && old[j] == f[j]);
-                if (miss) missmask |= 1u << j;
-                mb[j] = __ballot_sync(0xFFFFFFFFu, miss);
-                tot += __popc(mb[j]);
-            }
-            if (tot) {
-                uint32_t base = 0;
-                if (lane == 0) base = atomicAdd(&S.nrec, tot);
-                base = __shfl_sync(0xFFFFFFFFu, base, 0);
-#pragma unroll
-                for (int j = 0; j < FP_QPT; ++j) {
-                    if (missmask & (1u << j))
-                        S.rec[base + __popc(mb[j] & lanemask_lt())] =
-                            make_uint2(h[j] | (f[j] << 16), (pos0 + 32 * j) | ((tch >> j) & 1u ? R_TOUCHED : 0u) | (old[j] << 16));
-                    base += __popc(mb[j]);
-                }
-            }
-        }
-        __syncthreads();  // S1: all reads of tab/vbit precede the publishes; S.nrec = number of missers
-        DNS_PH(0)
-        const uint32_t nmiss = S.nrec;  // stable until phase C appends behind it
-
-        // ---- phase B: missers publish ---------------------------------------------------------------
-        #pragma unroll 1
-        for (uint32_t i = tid; i < nmiss; i += FP_THREADS) {
-            const uint2 r = S.rec[i];
-            const uint32_t hh = r.x & 0xFFFFu;
-            S.tab[hh] = (uint16_t)(r.x >> 16);  // racy between different values on purpose
-            atomicMin(&S.side[hh & (SIDE_N - 1)], ((r.y & 0xFFFu) << 16) | hh);
-        }
-        __syncthreads();  // S2
-        DNS_PH(1)
-
-        // ---- phase C: read back ----------------------------------------------------------------------
-        // hit members: the bucket still holds my value unless some misser published (its value differs from mine)
-#pragma unroll
-        for (int j = 0; j < FP_QPT; ++j) {
-            const uint32_t pos = pos0 + 32 * j;
-            bool ok = false;
-            if (((actmask >> j) & 1u) && !(missmask & (1u << j))) {
-                ok = S.tab[h[j]] == f[j];
-                if (!ok) {
-                    const uint32_t slot = S.side[h[j] & (SIDE_N - 1)];
-                    if ((slot & 0xFFFFu) == h[j] && pos < (slot >> 16)) {
-                        ok = true;  // every misser of my bucket comes after me
-                    } else {
-                        // slow hit member: join the records and my class list, raise the conflict bit
-                        const uint32_t idx = atomicAdd(&S.nrec, 1u);
-                        S.rec[idx] = make_uint2(h[j] | (f[j] << 16), pos | R_TOUCHED | (f[j] << 16));
-                        const uint32_t c = h[j] >> 11;
-                        const uint32_t k = atomicAdd(&S.cls_count[c], 1u);
-                        if (k < CLS_CAP) S.cls_list[c][k] = (uint16_t)idx; else S.cls_overflow = 1;
-                        atomicOr(&S.conf[h[j] >> 5], 1u << (h[j] & 31));
-                    }
-                }
-            }
-            const uint32_t fb = __ballot_sync(0xFFFFFFFFu, ok);
-            if (lane == 0) S.sigw[warp * 4 + j] = fb;
-        }
-        // missers: do all missers of my bucket agree, and who is first?
-        #pragma unroll 1
-        for (uint32_t i = tid; i < nmiss; i += FP_THREADS) {
-            const uint2 r = S.rec[i];
-            const uint32_t hh = r.x & 0xFFFFu;
-            const uint32_t slot = S.side[hh & (SIDE_N - 1)];
-            const uint32_t w = S.tab[hh];
-            uint32_t y = r.y;
-            if ((slot & 0xFFFFu) != hh || w != (r.x >> 16)) {   // foreign slot owner, or missers disagree
-                y |= R_SLOW;
-                atomicOr(&S.conf[hh >> 5], 1u << (hh & 31));
-            } else if (slot == (((r.y & 0xFFFu) << 16) | hh)) {
-                y |= R_FIRST;
-            }
-            if (y != r.y) S.rec[i].y = y;
-        }
-        __syncthreads();  // S3
-        DNS_PH(2)
-
-        // ---- phase D: missers classify ----------------------------------------------------------------
-        #pragma unroll 1
-        for (uint32_t i = tid; i < nmiss; i += FP_THREADS) {
-            const uint2 r = S.rec[i];
-            const uint32_t hh = r.x & 0xFFFFu;
-            uint32_t y = r.y;
-            if (!(y & R_SLOW) && bit_test(S.conf, hh)) { y |= R_SLOW; S.rec[i].y = y; }
-            if (y & R_SLOW) {
-                const uint32_t c = hh >> 11;
-                const uint32_t k = atomicAdd(&S.cls_count[c], 1u);
-                if (k < CLS_CAP) S.cls_list[c][k] = (uint16_t)i; else S.cls_overflow = 1;
-            } else if (!(y & R_FIRST)) {
-                const uint32_t pos = y & 0xFFFu;
-                atomicOr(&S.sigw[pos >> 5], 1u << (pos & 31));  // predecessor in the bucket is a misser with my value
-            }
-            S.side[hh & (SIDE_N - 1)] = SIDE_EMPTY;
-        }
-        __syncthreads();  // S4
-        DNS_PH(3)
-
-        // ---- phase F ------------------------------------------------------------------------------------
-        S.conf[tid] = 0; S.conf[tid + FP_THREADS] = 0;   // all readers of the conflict bits are behind S4; next set in the next tile's phase C
-        if (S.cls_overflow) {
-            // restore the pre-tile dictionary (only missers wrote), clear the per-tile state, walk the tile in order
-            #pragma unroll 1
-            for (uint32_t i = tid; i < nmiss; i += FP_THREADS) {
-                const uint2 r = S.rec[i];
-                S.tab[r.x & 0xFFFFu] = (uint16_t)(r.y >> 16);
-            }
-            if (tid < CLS_N) S.cls_count[tid] = 0;
-            __syncthreads();
-            uint32_t* qs = reinterpret_cast<uint32_t*>(S.rec);
-#pragma unroll
-            for (int j = 0; j < FP_QPT; ++j) qs[pos0 + 32 * j] = q[j];
-            if (tid == 0) { S.nrec = 0; S.cls_overflow = 0; }
-            __syncthreads();
-            if (warp == 0) tile_in_order(S, qs, rem, run_q0, unres_run, rcm ? rcm + lt * 64 : nullptr);
-        } else {
-            // first missers of agreeing buckets: genuine miss or unresolved first touch; deferred vbit; conflict-bit cleanup
-            #pragma unroll 1
-            for (uint32_t base = warp * 32; base < nmiss; base += FP_THREADS) {
-                const uint32_t i = base + lane;
-                uint2 r = make_uint2(0, 0);
-                if (i < nmiss) r = S.rec[i];
-                const uint32_t hh = r.x & 0xFFFFu;
-                const bool first = (i < nmiss) && (r.y & (R_FIRST | R_SLOW)) == R_FIRST;
-                if (first && (r.x >> 16) == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
-                append_unres(first && !(r.y & R_TOUCHED), run_q0 + (r.y & 0xFFFu), hh, r.x >> 16, &S.unres_count, unres_run);
-            }
-            // slow members, warp w <- class w. In-order semantics per bucket: my predecessor is the member of my bucket
-            // with the largest smaller position; without one the pre-tile value decides. The last member's value stays.
-            const uint32_t n = S.cls_count[warp];
-            const uint16_t* __restrict__ lst = S.cls_list[warp];
-            #pragma unroll 1
-            for (uint32_t base = 0; base < n; base += 32) {
-                const uint32_t i = base + lane;
-                const bool valid = i < n;
-                uint32_t pos = 0, hh = 0xFFFFFFFFu, ff = 0, oldv = 0; bool touched = false;
-                if (valid) {
-                    const uint2 d = S.rec[lst[i]];
-                    hh = d.x & 0xFFFFu; ff = d.x >> 16; pos = d.y & 0xFFFu; touched = (d.y & R_TOUCHED) != 0; oldv = d.y >> 16;
-                }
-                int best = -1; uint32_t bestf = 0; bool later = false;
-                #pragma unroll 1
-                for (uint32_t k = 0; k < n; ++k) {
-                    const uint2 dk = S.rec[lst[k]];      // broadcast reads
-                    const uint32_t pk = dk.y & 0xFFFu;
-                    if ((dk.x & 0xFFFFu) == hh) {
-                        if (pk < pos && (int)pk > best) { best = (int)pk; bestf = dk.x >> 16; }
-                        later |= pk > pos;
-                    }
-                }
-                const bool hit = valid && (best >= 0 ? (bestf == ff) : (touched && oldv == ff));
-                if (hit) atomicOr(&S.sigw[pos >> 5], 1u << (pos & 31));
-                if (valid && !later) {
-                    S.tab[hh] = (uint16_t)ff;
-                    if (ff == 0) atomicOr(&S.vbit[hh >> 5], 1u << (hh & 31));
-                }
-                append_unres(valid && best < 0 && !touched, run_q0 + pos, hh, ff, &S.unres_count, unres_run);
-            }
-            __syncwarp();
-            if (lane == 0) S.cls_count[warp] = 0;
-            if (tid == 0) S.nrec = 0;
-        }
-        __syncthreads();  // S5: dictionary final for this tile, sigw final
-        DNS_PH(4)
-
-        if (tid < TILE_Q / 32) rsig[lt * (TILE_Q / 32) + tid] = S.sigw[tid];  // workspace is sized in whole tiles
-        // (the next iteration rewrites S.sigw only after two more barriers)
-    }
-
-#ifdef DNS_PHASE_TIMING
-    if (tid == 0 && run == 77) { const long long nt = (long long)ntile_run;
-        printf("run %u tiles %lld cycles/tile: A %lld B %lld C %lld D %lld F %lld  total %lld\n", run, nt,
-               ph[0] / nt, ph[1] / nt, ph[2] / nt, ph[3] / nt, ph[4] / nt, (ph[0] + ph[1] + ph[2] + ph[3] + ph[4]) / nt); }
-#endif
-    // ---- export the run's last-writer table ---------------------------------------------------------
-    #pragma unroll 1
-    for (uint32_t i = tid; i < 65536; i += FP_THREADS) {
-        uint32_t v = S.tab[i];
-        uint32_t tch = (v != 0 || bit_test(S.vbit, i)) ? 0x10000u : 0u;
-        final_tab[(size_t)run * 65536 + i] = v | tch;
-    }
-    if (tid == 0) unres_count[run] = S.unres_count < 65536u ? S.unres_count : 65536u;
-}
-
-// ------------------------------------------------------------------------------------------------------
-// Pass 1, second formulation: write -> verify -> resolve the dirty members through a per-tile mailbox.
+// Pass 1: flag pass. Write -> verify -> resolve the dirty members through a per-tile mailbox.
 //
-// Same contract as cham_flag_pass (inputs, outputs, unresolved list, last-writer table). Per 4096-quad tile:
+// One persistent CTA per run: run r owns tiles [r * tiles_total / nruns, (r + 1) * tiles_total / nruns) of the stream and keeps the
+// run's dictionary in shared memory as 16-bit fingerprints (128 KiB, see common.cuh), starting empty. Outputs:
+//   sigw_g       the flag bits of every block of the run, 2 x u32 per block (low half first);
+//   unres        per run, up to 65536 (quad index in the run, hash | fp << 16): the quads whose bucket the run had not touched yet.
+//                They cannot know the dictionary carried in from earlier runs, so their flag is left 0 for cham_resolve to patch;
+//   unres_count  per run, the length of that list;
+//   final_tab    per run, 65536 x (touched << 16 | fp): the run's last-writer table, folded by cham_carry_scan.
+// With `copymap`, the quads of copy-mode blocks neither read nor write the dictionary (codec.rs:35-37); with `gate`, the kernel runs
+// only while the protection iteration is still open. Per 4096-quad tile:
 //   A  every quad reads the pre-tile dictionary: old != f => misser.                                                    (barrier)
 //   B  missers store their fingerprint (racy on purpose).                                                              (barrier)
 //   C  hit members read again: unchanged => no misser in my bucket => flag 1, final. Everything else -- the missers and the hit
@@ -413,6 +61,9 @@ cham_flag_pass(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles_
 // members of one bucket inside one tile that are not one run) sends the tile to f6_replay: the in-order replay of the dirty members,
 // one bucket class per warp (exact for any input; on text, the first three tiles of every run, whose dictionary starts empty).
 // ------------------------------------------------------------------------------------------------------
+constexpr int TILE_Q = 4096;                           // quads per tile = 16 KiB = 64 blocks
+__device__ __forceinline__ bool bit_test(const uint32_t* bm, uint32_t i) { return (bm[i >> 5] >> (i & 31)) & 1u; }
+
 constexpr int F6_THREADS = 512, F6_QPT = 8;           // 16 warps, 8 quads per thread: one tile = TILE_Q quads
 constexpr int F6_NW = F6_THREADS / 32, F6_WQ = 32 * F6_QPT;   // warps; quads (= record region size) per warp
 static_assert(F6_THREADS * F6_QPT == TILE_Q, "tile geometry");
@@ -1544,9 +1195,7 @@ static cudaError_t set_smem_attrs_once() {
     static bool done = false;
     static cudaError_t err = cudaSuccess;
     if (!done) {
-        err = cudaFuncSetAttribute(cham_flag_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FlagSmem));
-        if (err == cudaSuccess)
-            err = cudaFuncSetAttribute(cham_flag_pass6, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Flag6Smem));
+        err = cudaFuncSetAttribute(cham_flag_pass6, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Flag6Smem));
         if (err == cudaSuccess)
             err = cudaFuncSetAttribute(cham_protected_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ProtSmem));
         done = true;
@@ -1554,13 +1203,9 @@ static cudaError_t set_smem_attrs_once() {
     return err;
 }
 
-int g_cham_flag_impl = 6;   // 1: barrier-phased class protocol (round 1), 6: write / verify / replay
 static void launch_flag_pass(uint32_t nruns, cudaStream_t stream, const uint32_t* in, uint64_t nquads, uint32_t ntiles, uint32_t* sigw,
                              uint2* unres, uint32_t* unres_count, uint32_t* final_tab, const uint8_t* copymap, const Status* gate) {
-    if (g_cham_flag_impl == 1)
-        cham_flag_pass<<<nruns, FP_THREADS, sizeof(FlagSmem), stream>>>(in, nquads, ntiles, nruns, sigw, unres, unres_count, final_tab, copymap, gate);
-    else
-        cham_flag_pass6<<<nruns, F6_THREADS, sizeof(Flag6Smem), stream>>>(in, nquads, ntiles, nruns, sigw, unres, unres_count, final_tab, copymap, gate);
+    cham_flag_pass6<<<nruns, F6_THREADS, sizeof(Flag6Smem), stream>>>(in, nquads, ntiles, nruns, sigw, unres, unres_count, final_tab, copymap, gate);
 }
 
 static cudaError_t prot_iterate_coop(int ctas, cudaStream_t stream, const uint32_t* sigw, uint64_t nbytes, uint64_t nblocks, uint32_t nseg, Status* st, int it,

@@ -13,8 +13,6 @@ struct ChamLayout {
 
 size_t cham_workspace_bytes(size_t nbytes, int nruns_max, ChamLayout* L);
 uint32_t cham_pick_runs(size_t nbytes, int num_sms);
-extern int g_cham_decode_impl;  // which Chameleon decode pass kernel runs (chameleon_decode.cu)
-extern int g_cham_flag_impl;   // which flag pass kernel runs (chameleon_encode.cu; timing comparisons and tests)
 cudaError_t cham_encode_phase1(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns,
                                uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev = nullptr);
 cudaError_t cham_encode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns,

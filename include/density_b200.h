@@ -258,10 +258,6 @@ DENSITY_B200_API void density_b200_shutdown(void);
 /* Test hook: cut every stage of the Cheetah / Lion copy-map iteration to k rounds (1..7, default 7) so that the host-resumed
    iteration of path 4 can be exercised on ordinary inputs. */
 DENSITY_B200_API void density_b200_test_set_stage_rounds(int k);
-/* Test / timing hook: which Chameleon flag pass kernel runs (1 = round-1 class protocol, 6 = write / verify / replay; default 6). */
-DENSITY_B200_API void density_b200_test_set_flag_impl(int k);
-/* Same for the Chameleon decode pass (1 = round-1 kernel, 7 = write / verify / mailbox; default 7). */
-DENSITY_B200_API void density_b200_test_set_decode_impl(int k);
 /* Diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed
    (~0: none), number of such blocks}: 16 rounds x 2 values. Synchronises the device. */
 DENSITY_B200_API int density_b200_prot_debug(uint64_t* out32);

@@ -130,12 +130,11 @@ def _same_bucket_pair():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("impl", [6, 1])
-def test_chameleon_runs_of_equal_quads_and_mailbox_overflow(torch_cuda, codecs, impl):
-    """Round-2 flag pass (write / verify / mailbox): runs of equal quads of every length up to several tiles (one mailbox entry per run:
-    the run is dropped at deposit time), runs cut by a different quad of the same bucket, 5 - 40 quads of one bucket that are NOT a run
-    (main mailbox -> overflow mailboxes -> in-order replay of the tile), all inside text so that most blocks stay compressible; the
-    round-1 kernel must agree (impl 1)."""
+def test_chameleon_runs_of_equal_quads_and_mailbox_overflow(torch_cuda, codecs):
+    """Flag pass (write / verify / mailbox): runs of equal quads of every length up to several tiles (one mailbox entry per run: the
+    run is dropped at deposit time), runs cut by a different quad of the same bucket, 5 - 40 quads of one bucket that are NOT a run
+    (main mailbox -> overflow mailboxes -> in-order replay of the tile), all inside text so that most blocks stay compressible. Both
+    encode paths must match the oracle, and the stream must decode back."""
     torch = torch_cuda
     import density_b200
     from density_b200 import synth
@@ -163,30 +162,22 @@ def test_chameleon_runs_of_equal_quads_and_mailbox_overflow(torch_cuda, codecs, 
         k += 1
     data = np.concatenate(pieces).view(np.uint8)[:-1]
     want = oracle.encode("chameleon", data)
-    lib = density_b200.load()
-    lib.density_b200_test_set_flag_impl(impl)
-    try:
-        for path in (0, 1):
-            d_in = torch.from_numpy(data.copy()).cuda()
-            d_out = torch.zeros(codecs["chameleon"].safe_encode_buffer_size(data.size) + 64, dtype=torch.uint8, device="cuda")
-            d_sz = torch.zeros(1, dtype=torch.int64, device="cuda")
-            density_b200.encode_device("chameleon", d_in, d_out, d_sz, path=path)
-            torch.cuda.synchronize()
-            n = int(d_sz.item())
-            if path == 1 and n == 0:
-                continue          # path 1 = parallel only: gives up (size 0) when the copy map does not settle; path 0 must still be exact
-            assert n == want.size and (d_out[:n].cpu().numpy() == want).all(), (impl, path)
-        # and back through the decoder (both decode pass kernels)
-        for dimpl in (7, 1):
-            lib.density_b200_test_set_decode_impl(dimpl)
-            d_enc = torch.from_numpy(want.copy()).cuda()
-            d_dec = torch.zeros(data.size + 64, dtype=torch.uint8, device="cuda")
-            density_b200.decode_device("chameleon", d_enc, want.size, d_dec, d_sz, path=0)
-            torch.cuda.synchronize()
-            assert int(d_sz.item()) == data.size and (d_dec[:data.size].cpu().numpy() == data).all(), dimpl
-    finally:
-        lib.density_b200_test_set_flag_impl(6)
-        lib.density_b200_test_set_decode_impl(7)
+    for path in (0, 1):
+        d_in = torch.from_numpy(data.copy()).cuda()
+        d_out = torch.zeros(codecs["chameleon"].safe_encode_buffer_size(data.size) + 64, dtype=torch.uint8, device="cuda")
+        d_sz = torch.zeros(1, dtype=torch.int64, device="cuda")
+        density_b200.encode_device("chameleon", d_in, d_out, d_sz, path=path)
+        torch.cuda.synchronize()
+        n = int(d_sz.item())
+        if path == 1 and n == 0:
+            continue          # path 1 = parallel only: gives up (size 0) when the copy map does not settle; path 0 must still be exact
+        assert n == want.size and (d_out[:n].cpu().numpy() == want).all(), path
+    # and back through the decoder
+    d_enc = torch.from_numpy(want.copy()).cuda()
+    d_dec = torch.zeros(data.size + 64, dtype=torch.uint8, device="cuda")
+    density_b200.decode_device("chameleon", d_enc, want.size, d_dec, d_sz, path=0)
+    torch.cuda.synchronize()
+    assert int(d_sz.item()) == data.size and (d_dec[:data.size].cpu().numpy() == data).all()
 
 
 @pytest.mark.parametrize("path", [0, 1, 2])

@@ -84,22 +84,17 @@ def want_stream(alg, name):
 
 
 # ---- Chameleon encode -------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("impl", [6, 1])
 @pytest.mark.parametrize("name,path", [("cham33", 0), ("cham33", 1), ("cham5", 2), ("copy3", 0), ("copy3", 2)])
-def test_chameleon_encode_device_paths(torch_cuda, lib, impl, name, path):
-    """encode_device paths 0 (auto), 1 (fast path only: quiet corpora) and 2 (protection-aware walk), with the write / verify /
-    replay flag pass (6) and the round-1 class protocol (1). The GPU stream decodes back with the oracle and on the GPU."""
+def test_chameleon_encode_device_paths(torch_cuda, lib, name, path):
+    """encode_device paths 0 (auto), 1 (fast path only: quiet corpora) and 2 (protection-aware walk). The GPU stream decodes back
+    with the oracle and on the GPU."""
     torch = torch_cuda
     data, _ = corpus(name)
     want = want_stream("chameleon", name)
-    lib.density_b200_test_set_flag_impl(impl)
-    try:
-        rc, n, got, tail = dev_encode(torch, lib, "chameleon", data, path)
-        if path == 1:
-            assert lib.density_b200_last_encode_was_fast() == 1
-    finally:
-        lib.density_b200_test_set_flag_impl(6)
-    assert_stream(rc, n, got, want, f"{name} path {path} flag impl {impl}")
+    rc, n, got, tail = dev_encode(torch, lib, "chameleon", data, path)
+    if path == 1:
+        assert lib.density_b200_last_encode_was_fast() == 1
+    assert_stream(rc, n, got, want, f"{name} path {path}")
     assert (tail == CANARY).all()
     assert (oracle.decode("chameleon", got, data.size) == data).all()
     rc, m, back, _ = dev_decode(torch, lib, "chameleon", got, data.size, 0)
@@ -126,20 +121,15 @@ def test_chameleon_encode_through_reference_symbols(torch_cuda, lib):
 
 
 # ---- Chameleon decode -------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("impl", [7, 1])
 @pytest.mark.parametrize("name,path", [("cham33", 0), ("cham33", 1), ("cham5", 3), ("copy3", 0), ("copy3", 1), ("copy3", 3)])
-def test_chameleon_decode_device_paths(torch_cuda, lib, impl, name, path):
-    """decode_device paths 0, 1 and 3 on oracle streams, with the write / verify / mailbox decode pass (7) and the round-1 kernel (1);
-    the output buffer is exactly n bytes, followed by a canary that must stay intact."""
+def test_chameleon_decode_device_paths(torch_cuda, lib, name, path):
+    """decode_device paths 0, 1 and 3 on oracle streams; the output buffer is exactly n bytes, followed by a canary that must stay
+    intact."""
     torch = torch_cuda
     data, _ = corpus(name)
     enc = want_stream("chameleon", name)
-    lib.density_b200_test_set_decode_impl(impl)
-    try:
-        rc, m, got, tail = dev_decode(torch, lib, "chameleon", enc, data.size, path)
-    finally:
-        lib.density_b200_test_set_decode_impl(7)
-    assert rc == 0 and m == data.size, (name, path, impl, m)
+    rc, m, got, tail = dev_decode(torch, lib, "chameleon", enc, data.size, path)
+    assert rc == 0 and m == data.size, (name, path, m)
     assert (got == data).all(), f"first differing byte {first_diff(got, data)}"
     assert (tail == CANARY).all(), "wrote past the output capacity"
 

@@ -1,4 +1,4 @@
-"""Per-phase cycle counts of cham_flag_pass (needs a lib built with -DDNS_PHASE_TIMING: tools/build_variant.sh timing "-DDNS_PHASE_TIMING";
+"""Per-phase cycle counts of cham_flag_pass6 (needs a lib built with -DDNS_PHASE_TIMING: tools/build_variant.sh timing "-DDNS_PHASE_TIMING";
 run with DENSITY_B200_SO=density_b200/_variants/lib_timing.so)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -40,6 +40,18 @@ _SIGS = {
     "density_b200_locate_piece": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_decode_sharded_stream": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
                                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_shard_create": (ctypes.c_void_p, [ctypes.c_int]),
+    "density_b200_cl_shard_destroy": (None, [ctypes.c_void_p]),
+    "density_b200_cl_table_words": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int]),
+    "density_b200_cl_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                                    ctypes.c_void_p]),
+    "density_b200_cl_shard_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_shard_phase3": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p,
+                                                    ctypes.c_void_p]),
+    "density_b200_cl_table_init": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_table_fold": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_encode_sharded_cl": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                      ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, ctypes.c_void_p]),
     "density_b200_codec_create": (ctypes.c_void_p, [ctypes.c_int]),
     "density_b200_codec_destroy": (None, [ctypes.c_void_p]),
     "density_b200_codec_clear_state": (ctypes.c_int, [ctypes.c_void_p]),

@@ -666,6 +666,132 @@ int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in,
     return DENSITY_B200_OK;
 }
 
+// ---- sharded Cheetah / Lion encode: one shard of a longer stream in three phases around two table exchanges ---------------------------
+struct density_b200_cl_shard {
+    int alg = ALG_CHEETAH, num_sms = 0;
+    DevBuf ws, tables[3];           // workspace; the epoch-tagged run tables (zero at allocation, one entry format each)
+    uint32_t epoch = 0, epoch_base = 0;
+    const uint8_t* d_in = nullptr;
+    size_t n = 0;
+    bool first = true, is_last = true;
+    int phase = 0;                  // the last phase done on the current shard
+};
+
+static bool cl_alg_ok(int alg) { return alg == ALG_CHEETAH || alg == ALG_LION; }
+
+density_b200_cl_shard* density_b200_cl_shard_create(int alg) {
+    g_last_error.clear();
+    if (!cl_alg_ok(alg)) { set_error("cl_shard_create: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return nullptr; }
+    DeviceCtx* c = current_ctx();
+    if (!c) return nullptr;
+    density_b200_cl_shard* s = new density_b200_cl_shard();
+    s->alg = alg; s->num_sms = c->num_sms;
+    return s;
+}
+void density_b200_cl_shard_destroy(density_b200_cl_shard* s) {
+    if (!s) return;
+    s->ws.release(); for (auto& t : s->tables) t.release();
+    delete s;
+}
+size_t density_b200_cl_table_words(int alg, int kind) {
+    if (!cl_alg_ok(alg) || (kind != DENSITY_B200_CL_TABLE_P && kind != DENSITY_B200_CL_TABLE_C)) return 0;
+    return (size_t)cl_table_planes(alg, kind) * 65536;
+}
+
+static int cl_phase1_impl(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last, const uint32_t* d_prev_quad, uint32_t* d_tab_p,
+                          cudaStream_t st) {
+    if ((!d_in && n) || !d_tab_p) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!is_last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_prev_quad) & 3)) { set_error("d_in and d_prev_quad must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    s->phase = 0;
+    cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
+    for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    if (s->epoch > 0x0FFFFF00u) {                      // epochs exhausted: start over on cleared tables
+        for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = cudaMemsetAsync(s->tables[rg].p, 0, s->tables[rg].bytes, st);
+        if (e != cudaSuccess) { set_error("cudaMemsetAsync", e); return DENSITY_B200_ECUDA; }
+        s->epoch = 0;
+    }
+    s->epoch_base = s->epoch + 1; s->epoch += cl_shard_epochs();
+    s->d_in = d_in; s->n = n; s->first = d_prev_quad == nullptr; s->is_last = is_last != 0;
+    uint64_t launches = 0;
+    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
+    if (n == 0) e = cudaMemsetAsync(d_tab_p, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_P) * sizeof(uint32_t), st);   // identity
+    else e = cl_shard_phase1(s->alg, d_in, n, d_prev_quad, s->ws.p, tabs, s->epoch_base, s->num_sms, d_tab_p, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cl shard phase1", e); return DENSITY_B200_ECUDA; }
+    s->phase = 1;
+    return DENSITY_B200_OK;
+}
+static int cl_phase2_impl(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t st) {
+    if (s->phase != 1) { set_error("cl_shard_phase2: phase 1 not done"); return DENSITY_B200_EARG; }
+    if (!d_tab_c) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
+    cudaError_t e;
+    if (s->n == 0) e = cudaMemsetAsync(d_tab_c, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_C) * sizeof(uint32_t), st);
+    else e = cl_shard_phase2(s->alg, s->d_in, s->n, s->first, d_carry_p, s->ws.p, tabs, s->epoch_base, s->num_sms, d_tab_c, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cl shard phase2", e); return DENSITY_B200_ECUDA; }
+    s->phase = 2;
+    return DENSITY_B200_OK;
+}
+static int cl_phase3_impl(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
+                          cudaStream_t st) {
+    if (s->phase != 2) { set_error("cl_shard_phase3: phase 2 not done"); return DENSITY_B200_EARG; }
+    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
+    cudaError_t e;
+    if (s->n == 0) {
+        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
+    } else {
+        e = cl_shard_phase3(s->alg, s->d_in, s->n, s->first, s->is_last, d_carry_c, s->ws.p, tabs, s->epoch_base, s->num_sms, d_out, cap, d_out_size,
+                            d_seam8, st, &launches);
+    }
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cl shard phase3", e); return DENSITY_B200_ECUDA; }
+    s->phase = 3;
+    return DENSITY_B200_OK;
+}
+int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, const uint32_t* d_prev_quad,
+                                 uint32_t* d_table_p_out, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cl_phase1_impl(s, d_in, n, is_last_shard, d_prev_quad, d_table_p_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cl_shard_phase2(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cl_phase2_impl(s, d_carry_p, d_table_c_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cl_shard_phase3(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                 uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cl_phase3_impl(s, d_carry_c, d_out, cap, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* stream) {
+    g_last_error.clear();
+    if (!density_b200_cl_table_words(alg, kind) || !d_table) { set_error("cl_table_init: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
+    uint64_t l = 0;
+    cudaError_t e = cl_table_init(alg, kind, d_table, reinterpret_cast<cudaStream_t>(stream), &l);
+    g_launches += l;
+    if (e != cudaSuccess) { set_error("cl_table_init", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, void* stream) {
+    g_last_error.clear();
+    if (!density_b200_cl_table_words(alg, kind) || !d_acc || !d_next) { set_error("cl_table_fold: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
+    uint64_t l = 0;
+    cudaError_t e = cl_table_fold(alg, kind, d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
+    g_launches += l;
+    if (e != cudaSuccess) { set_error("cl_table_fold", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
 struct density_b200_decode_shard {
     DevBuf ws;
@@ -783,6 +909,8 @@ struct density_b200_sharded {
     nccl_comm_t comm = nullptr;
     DevBuf ws, aux;                 // aux: gathered tables [world][65536] + carry [65536] + seam words [world][8] + offsets [world + 1] + size
     DevBuf dws;                     // decode workspace (density_b200_decode_sharded[_stream]), apart from the encoder's
+    density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion shard state of density_b200_encode_sharded_cl
+    DevBuf cl_aux;                  // its exchange buffers: gathered P and C tables, the carries, the last quads
     ChamLayout L{};
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     uint64_t* h_maps = nullptr;     // pinned, world range maps (density_b200_decode_sharded_stream)
@@ -828,7 +956,8 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-    h->ws.release(); h->aux.release(); h->dws.release();
+    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release();
+    for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     if (h->h_maps) cudaFreeHost(h->h_maps);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
@@ -850,6 +979,36 @@ static cudaError_t sharded_aux(density_b200_sharded* h, cudaStream_t st, Sharded
     return e;
 }
 
+// variable-length gather of the pieces to `gather_root` at their stream offsets (d_offsets: world + 1 prefix sums, on the device); blocks
+static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_offsets, const uint8_t* d_out, int gather_root, uint8_t* d_gather,
+                         size_t gather_cap, cudaStream_t st) {
+    const size_t W = (size_t)h->world;
+    cudaError_t e;
+    // variable-length gather of the pieces at their stream offsets (SURVEY §8e step 5): sizes -> host -> grouped send / recv
+    e = cudaMemcpyAsync(h->h_offsets, d_offsets, (W + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("gather: sizes to host", e); return DENSITY_B200_ECUDA; }
+    const uint64_t total = h->h_offsets[W];
+    const uint64_t my_off = h->h_offsets[h->rank], my_size = h->h_offsets[h->rank + 1] - my_off;
+    if (h->rank == gather_root) {
+        if (!d_gather || gather_cap < total) { set_error("gather buffer too small"); return DENSITY_B200_ECAPACITY; }
+        if (my_size) e = cudaMemcpyAsync(d_gather + my_off, d_out, my_size, cudaMemcpyDeviceToDevice, st);
+        if (e != cudaSuccess) { set_error("gather: local piece", e); return DENSITY_B200_ECUDA; }
+    }
+    if (h->world > 1) {
+        if (!nccl_check(a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
+        bool ok = true;
+        if (h->rank == gather_root) {
+            for (int r = 0; r < h->world && ok; ++r) {
+                const uint64_t sz = h->h_offsets[r + 1] - h->h_offsets[r];
+                if (r != h->rank && sz) ok = nccl_check(a->Recv(d_gather + h->h_offsets[r], sz, NCCL_UINT8, r, h->comm, st), "ncclRecv");
+            }
+        } else if (my_size) ok = nccl_check(a->Send(d_out, my_size, NCCL_UINT8, gather_root, h->comm, st), "ncclSend");
+        if (!nccl_check(a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
+    }
+    return DENSITY_B200_OK;
+}
+
 // One bit-exact stream cut across `world` GPUs; this rank's shard is d_in[0 .. n) (n % 256 == 0 except on the last rank).
 // All work is enqueued on `stream`. With gather_root >= 0 the call BLOCKS on the stream once (the piece sizes must reach the host before
 // the variable-length ncclSend / ncclRecv can be posted) and the pieces land in d_gather on rank gather_root at their stream offsets.
@@ -863,7 +1022,6 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
     NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    const size_t W = (size_t)h->world;
     cudaError_t e = h->ws.ensure(cham_workspace_bytes(n, h->num_sms, &h->L), st);
     ShardedAux x;
     if (e == cudaSuccess) e = sharded_aux(h, st, &x);
@@ -899,32 +1057,85 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     e = cham_seam_verdict(d_words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, d_offsets, st, &launches);
     if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
     if (gather_root >= 0) {
-        // variable-length gather of the pieces at their stream offsets (SURVEY §8e step 5): sizes -> host -> grouped send / recv
-        e = cudaMemcpyAsync(h->h_offsets, d_offsets, (W + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("gather: sizes to host", e); return DENSITY_B200_ECUDA; }
-        const uint64_t total = h->h_offsets[W];
-        const uint64_t my_off = h->h_offsets[h->rank], my_size = h->h_offsets[h->rank + 1] - my_off;
-        if (h->rank == gather_root) {
-            if (!d_gather || gather_cap < total) { set_error("gather buffer too small"); return DENSITY_B200_ECAPACITY; }
-            if (my_size) e = cudaMemcpyAsync(d_gather + my_off, d_out, my_size, cudaMemcpyDeviceToDevice, st);
-            if (e != cudaSuccess) { set_error("gather: local piece", e); return DENSITY_B200_ECUDA; }
-        }
-        if (h->world > 1) {
-            if (!nccl_check(a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
-            bool ok = true;
-            if (h->rank == gather_root) {
-                for (int r = 0; r < h->world && ok; ++r) {
-                    const uint64_t sz = h->h_offsets[r + 1] - h->h_offsets[r];
-                    if (r != h->rank && sz) ok = nccl_check(a->Recv(d_gather + h->h_offsets[r], sz, NCCL_UINT8, r, h->comm, st), "ncclRecv");
-                }
-            } else if (my_size) ok = nccl_check(a->Send(d_out, my_size, NCCL_UINT8, gather_root, h->comm, st), "ncclSend");
-            if (!nccl_check(a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
-        }
+        const int rc = gather_pieces(h, a, d_offsets, d_out, gather_root, d_gather, gather_cap, st);
+        if (rc != DENSITY_B200_OK) return rc;
     }
     cudaEventRecord(h->ev[5], st);
     h->timed = true;
     g_launches += launches;
+    return DENSITY_B200_OK;
+}
+
+// Sharded Cheetah / Lion encode over the handle's communicator: last quads -> phase 1 -> P tables -> fold -> phase 2 -> C tables -> fold
+// -> phase 3 -> seam words -> verdict -> optional gather, as density_b200_encode_sharded. The exchanges are ncclAllGathers on `stream`.
+int density_b200_encode_sharded_cl(density_b200_sharded* h, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                   uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
+    const bool last = h->rank == h->world - 1;
+    if (!last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    density_b200_cl_shard*& s = h->cl[alg - ALG_CHEETAH];
+    if (!s) { s = new density_b200_cl_shard(); s->alg = alg; s->num_sms = h->num_sms; }
+    const size_t W = (size_t)h->world, R = (size_t)h->rank;
+    const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
+    ShardedAux x;
+    cudaError_t e = sharded_aux(h, st, &x);
+    if (e == cudaSuccess) e = h->cl_aux.ensure(((W + 1) * (wp + wc) + 2 * W + 64) * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint32_t* tab_p = reinterpret_cast<uint32_t*>(h->cl_aux.p);          // [world][wp]
+    uint32_t* carry_p = tab_p + W * wp;
+    uint32_t* tab_c = carry_p + wp;                                       // [world][wc]
+    uint32_t* carry_c = tab_c + W * wc;
+    uint32_t* quads = carry_c + wc;                                       // [world] {has a quad, last quad}
+    uint32_t* prev_quad = quads + 2 * W;
+    uint64_t launches = 0;
+    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
+        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
+    };
+    // 0. the context of my first quad: the last quad of the nearest earlier shard that has one
+    e = cl_last_quad(d_in, n, quads + 2 * R, st, &launches);
+    if (e == cudaSuccess && !gather(quads, 2, "ncclAllGather(last quads)")) return DENSITY_B200_ECUDA;
+    if (e == cudaSuccess) e = cl_prev_quad(quads, (uint32_t)R, prev_quad, st, &launches);
+    g_launches += launches; launches = 0;
+    if (e != cudaSuccess) { set_error("sharded cl: last quads", e); return DENSITY_B200_ECUDA; }
+    // 1-2. predictions, exchange, fold
+    cudaEventRecord(h->ev[0], st);
+    int rc = cl_phase1_impl(s, d_in, n, last, R ? prev_quad : nullptr, tab_p + R * wp, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[1], st);
+    if (!gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
+    e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
+    g_launches += launches; launches = 0;
+    if (e != cudaSuccess) { set_error("sharded cl: P fold", e); return DENSITY_B200_ECUDA; }
+    cudaEventRecord(h->ev[2], st);
+    // 3-4. chunk map, exchange, fold
+    rc = cl_phase2_impl(s, carry_p, tab_c + R * wc, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
+    e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_C, tab_c, (uint32_t)R, carry_c, st, &launches);
+    g_launches += launches; launches = 0;
+    if (e != cudaSuccess) { set_error("sharded cl: C fold", e); return DENSITY_B200_ECUDA; }
+    cudaEventRecord(h->ev[3], st);
+    // 5. emit and seam words, the verdict over all shards, the optional gather
+    rc = cl_phase3_impl(s, carry_c, d_out, cap, d_out_size, x.words + 8 * R, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[4], st);
+    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
+    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
+    if (gather_root >= 0) {
+        rc = gather_pieces(h, a, x.offsets, d_out, gather_root, d_gather, gather_cap, st);
+        if (rc != DENSITY_B200_OK) return rc;
+    }
+    cudaEventRecord(h->ev[5], st);
+    h->timed = true;
     return DENSITY_B200_OK;
 }
 
@@ -1053,8 +1264,9 @@ int density_b200_decode_sharded_stream(density_b200_sharded* h, const uint8_t* d
                                 d_total_size, d_out_offset, st);
 }
 
-/* stage times of the last density_b200_encode_sharded call (waits for it): out_ms[0] flag pass, [1] table exchange + fold,
-   [2] carry / resolve / sizes / scan, [3] emit, [4] seam exchange + gather. */
+/* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag
+   pass, [1] table exchange + fold, [2] carry / resolve / sizes / scan, [3] emit, [4] seam exchange + gather. Cheetah / Lion: [0] phase 1
+   (after the last-quad exchange), [1] P exchange + fold, [2] phase 2 + C exchange + fold, [3] phase 3, [4] seam exchange + gather. */
 int density_b200_sharded_profile(density_b200_sharded* h, float* out_ms) {
     if (!h || !out_ms || !h->timed) return DENSITY_B200_EARG;
     cudaError_t e = cudaEventSynchronize(h->ev[5]);

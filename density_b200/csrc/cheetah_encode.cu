@@ -33,14 +33,18 @@ constexpr uint32_t FP_INVALID = 0x10000u;   // a fingerprint value that matches 
 
 __device__ __forceinline__ uint64_t run_block_begin(uint32_t r, uint32_t nruns, uint64_t ntiles) { return ((uint64_t)r * ntiles / nruns) * TILE_B; }
 
-// context of the first encoded quad of every run: hash of the last quad of the last encoded block before the run (0 if none)
+// context of the first encoded quad of every run: hash of the last quad of the last encoded block before the run (0 if none; a
+// shard of a longer stream passes the last quad of the shard before it in `prev_quad`). ctx0 opens every round that runs, so
+// `epoch_out` (may be nullptr) ends up holding the epoch of the last one: the settled round once the copy map has converged.
 __global__ void chee_ctx0(const uint32_t* __restrict__ in, uint64_t nquads, const uint8_t* __restrict__ copymap, uint32_t nruns, uint64_t ntiles,
-                          const Status* __restrict__ gate, uint32_t* __restrict__ ctx0) {
+                          const Status* __restrict__ gate, const uint32_t* __restrict__ prev_quad, uint32_t epoch, uint32_t* __restrict__ epoch_out,
+                          uint32_t* __restrict__ ctx0) {
     if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (epoch_out && r == 0) *epoch_out = epoch;
     if (r >= nruns) return;
     uint64_t b = run_block_begin(r, nruns, ntiles);
-    uint32_t c = 0;
+    uint32_t c = prev_quad ? prod_hash(hash_prod(*prev_quad)) : 0u;
     while (b > 0) {
         --b;
         if (copymap && copymap[b]) continue;
@@ -104,13 +108,14 @@ chee_pass_p(const uint32_t* __restrict__ in, uint64_t nquads, uint64_t nblocks, 
     }
 }
 
-// walk the runs in order per context: resolve each run's first access from the carried-in value, carry the run's last value on
+// walk the runs in order per context: resolve each run's first access from the carried-in value, carry the run's last value on.
+// `carry` (nullptr: the stream start) = the value per context before the first run, for a shard of a longer stream.
 __global__ void chee_fold_p(const uint32_t* __restrict__ in, uint32_t nruns, const Status* __restrict__ gate, const uint4* __restrict__ entP_all,
-                            uint32_t epoch, uint32_t* __restrict__ Pbits) {
+                            uint32_t epoch, const uint32_t* __restrict__ carry, uint32_t* __restrict__ Pbits) {
     if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
     if (ctx >= 65536) return;
-    uint32_t c = 0;                                                   // prediction table starts as 0 everywhere (cheetah.rs:53)
+    uint32_t c = carry ? carry[ctx] : 0u;                             // prediction table starts as 0 everywhere (cheetah.rs:53)
     for (uint32_t r0 = 0; r0 < nruns; r0 += 8) {
         uint4 e[8];
 #pragma unroll
@@ -204,14 +209,16 @@ chee_pass_c(const uint32_t* __restrict__ in, uint64_t nquads, uint64_t nblocks, 
     }
 }
 
-// walk the runs in order per bucket: resolve the (at most two) undecided accesses of each run, carry (a, b) on
+// walk the runs in order per bucket: resolve the (at most two) undecided accesses of each run, carry (a, b) on.
+// `carry` (nullptr: the stream start) = planes a, b (65536 words apart) before the first run, for a shard of a longer stream.
 __global__ void chee_fold_c(const uint32_t* __restrict__ in, uint32_t nruns, const Status* __restrict__ gate, const uint4* __restrict__ entC_all,
-                            uint32_t epoch, uint32_t* __restrict__ Abits, uint32_t* __restrict__ Bbits) {
+                            uint32_t epoch, const uint32_t* __restrict__ carry, uint32_t* __restrict__ Abits, uint32_t* __restrict__ Bbits) {
     if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= 65536) return;
     // chunk map starts as (quad 0, quad 0) (cheetah.rs:52): only bucket 0 can ever match that
     uint32_t a0 = h ? FP_INVALID : 0u, b0 = a0;
+    if (carry) { a0 = carry[h]; b0 = carry[65536 + h]; }
     for (uint32_t r0 = 0; r0 < nruns; r0 += 8) {
         uint4 e[8];
 #pragma unroll
@@ -355,12 +362,14 @@ chee_emit(const uint32_t* __restrict__ in, uint64_t nbytes, uint64_t nblocks, co
 // Tables per (run, context): hot 32 B {p0..p4, epoch << 3 | m, -, -}; cold 32 B {1 + quad index of the k-th undecided access, k < 5}.
 // =====================================================================================================================================
 __global__ void lion_ctx0(const uint32_t* __restrict__ in, uint64_t nquads, const uint8_t* __restrict__ copymap, uint32_t nruns, uint64_t ntiles,
-                          const Status* __restrict__ gate, uint32_t* __restrict__ ctx0) {
+                          const Status* __restrict__ gate, const uint32_t* __restrict__ prev_quad, uint32_t epoch, uint32_t* __restrict__ epoch_out,
+                          uint32_t* __restrict__ ctx0) {
     if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (epoch_out && r == 0) *epoch_out = epoch;
     if (r >= nruns) return;
     uint64_t b = run_block_begin(r, nruns, ntiles) * 2;       // in 64-byte blocks
-    uint32_t c = 0;
+    uint32_t c = prev_quad ? prod_hash(hash_prod(*prev_quad)) : 0u;
     while (b > 0) {
         --b;
         if (copymap && copymap[b]) continue;
@@ -440,13 +449,15 @@ lion_pass_p(const uint32_t* __restrict__ in, uint64_t nquads, uint64_t nsteps, u
     }
 }
 
+// `carry` (nullptr: the stream start) = the five list planes (65536 words apart) before the first run, for a shard of a longer stream
 __global__ void lion_fold_p(const uint32_t* __restrict__ in, uint32_t nruns, const Status* __restrict__ gate, const uint4* __restrict__ hot_all,
-                            const uint32_t* __restrict__ cold_all, uint32_t epoch, uint32_t* __restrict__ F0, uint32_t* __restrict__ F1,
-                            uint32_t* __restrict__ F2, uint32_t* __restrict__ Pany) {
+                            const uint32_t* __restrict__ cold_all, uint32_t epoch, const uint32_t* __restrict__ carry, uint32_t* __restrict__ F0,
+                            uint32_t* __restrict__ F1, uint32_t* __restrict__ F2, uint32_t* __restrict__ Pany) {
     if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
     if (ctx >= 65536) return;
     uint32_t c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0;                 // the carried list: five zeros at the stream start (lion.rs:64-72)
+    if (carry) { c0 = carry[ctx]; c1 = carry[65536 + ctx]; c2 = carry[2 * 65536 + ctx]; c3 = carry[3 * 65536 + ctx]; c4 = carry[4 * 65536 + ctx]; }
     for (uint32_t r0 = 0; r0 < nruns; r0 += 4) {
         uint4 ea[4], eb[4];
 #pragma unroll
@@ -623,6 +634,193 @@ __global__ void chee_finish(const Status* __restrict__ st, uint32_t* __restrict_
 // open the gate of a stage of up to 8 rounds; a continuation stage inherits "already settled" from the stage before it
 __global__ void chee_chain_gate(Status* __restrict__ st, const Status* __restrict__ prev) { st->nonquiet = 1; st->converged = prev ? prev->converged : 0u; }   // Cheetah always runs the copy-map iteration
 
+
+// =====================================================================================================================================
+// Sharded encode (one stream cut across GPUs / calls): what a shard tells the shards after it, as TRANSFERS per context / bucket.
+// Every table is a stack of u32 planes of 65536 entries (word w of key i at [w * 65536 + i]); all-zero = the identity transfer.
+//   P, Cheetah (2 planes)  {touched, last quad}: pred[ctx] always ends as the last quad seen in the context, so the fold overwrites.
+//   P, Lion (12 planes)    {m, nu, l0..l4, v0..v4}: the shard leaves its m local values l in front of what is left of the carried-in
+//                          list; its nu undecided accesses (values v, the k-th made with k local entries in front) each remove one
+//                          matching carried entry, as lion_fold_p replays them. A concrete list is {5, 0, list, -}.
+//   C, both (3 planes)     {T, a, b}: T0 untouched, T1 v = the bucket was accessed with one value v, T2 = it ends as (a, b).
+// compose(x, y) = "x, then y" keeps each form closed; the stream-start states (cl_table_init) are concrete, and a left fold of shard
+// transfers over them gives the concrete state the in-order encoder has at the cut.
+// =====================================================================================================================================
+constexpr uint32_t PL = 65536;
+
+struct LionT { uint32_t m, nu, l[5], v[5]; };
+__device__ __forceinline__ void lion_t_load(const uint32_t* __restrict__ t, uint32_t i, LionT& x) {
+    x.m = t[i]; x.nu = t[PL + i];
+#pragma unroll
+    for (int s = 0; s < 5; ++s) { x.l[s] = t[(2 + s) * PL + i]; x.v[s] = t[(7 + s) * PL + i]; }
+}
+__device__ __forceinline__ void lion_t_store(uint32_t* __restrict__ t, uint32_t i, const LionT& x) {
+    t[i] = x.m; t[PL + i] = x.nu;
+#pragma unroll
+    for (int s = 0; s < 5; ++s) { t[(2 + s) * PL + i] = x.l[s]; t[(7 + s) * PL + i] = x.v[s]; }
+}
+// x <- x then y. y's k-th undecided access sees the first 5 - k entries of what x leaves: x's literals first (a match there decides it
+// and removes the literal), then x's unknown carried-in remainder (no literal match while that remainder is visible: the access stays
+// undecided in the composition)
+__device__ __forceinline__ void lion_t_compose(LionT& x, const LionT& y) {
+    uint32_t lit[5], nl = x.m, nu = x.nu;
+#pragma unroll
+    for (int s = 0; s < 5; ++s) lit[s] = x.l[s];
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        if ((uint32_t)k >= y.nu) break;
+        const uint32_t vis = 5 - k, lim = nl < vis ? nl : vis;
+        uint32_t j = 5;
+#pragma unroll
+        for (int s = 4; s >= 0; --s) if ((uint32_t)s < lim && lit[s] == y.v[k]) j = s;
+        if (j < 5) {
+#pragma unroll
+            for (int s = 0; s < 4; ++s) if ((uint32_t)s >= j) lit[s] = lit[s + 1];
+            --nl;
+        } else if (nl < vis && nu < 5) {
+#pragma unroll
+            for (int s = 0; s < 5; ++s) if ((uint32_t)s == nu) x.v[s] = y.v[k];
+            ++nu;
+        }
+    }
+    const uint32_t keep = nl < 5 - y.m ? nl : 5 - y.m;
+#pragma unroll
+    for (int s = 0; s < 5; ++s) {
+        uint32_t w = 0;
+#pragma unroll
+        for (int t = 0; t < 5; ++t) if ((uint32_t)s >= y.m && (uint32_t)(s - t) == y.m && (uint32_t)t < keep) w = lit[t];
+        x.l[s] = (uint32_t)s < y.m ? y.l[s] : w;
+    }
+    x.m = y.m + keep; x.nu = nu;
+}
+__device__ __forceinline__ void chunk_t_compose(uint32_t& T, uint32_t& a, uint32_t& b, uint32_t T2, uint32_t a2, uint32_t b2) {
+    if (T2 == 0) return;
+    if (T2 == 2) { T = 2; a = a2; b = b2; return; }
+    if (T == 0) { T = 1; a = a2; }                                     // T1 v after nothing
+    else if (a2 != a) { b = a; a = a2; T = 2; }                        // T1 v after T1 w (v != w) or over (a, b) (v != a): (v, a)
+}
+
+// the shard's transfer, composed over its runs in order (the run tables of the round whose tag is *epoch_p)
+__global__ void cl_export_p_chee(const uint4* __restrict__ entP_all, uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+    const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ctx >= PL) return;
+    const uint32_t epoch = *epoch_p;
+    uint32_t touched = 0, q = 0;
+    for (uint32_t r = 0; r < nruns; ++r) {
+        const uint4 e = entP_all[(size_t)r * PL + ctx];
+        if (e.y == epoch) { touched = 1; q = e.x; }
+    }
+    out[ctx] = touched; out[PL + ctx] = q;
+}
+__global__ void cl_export_p_lion(const uint32_t* __restrict__ in, const uint4* __restrict__ hot_all, const uint32_t* __restrict__ cold_all,
+                                 uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+    const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ctx >= PL) return;
+    const uint32_t epoch = *epoch_p;
+    LionT x = {};
+    for (uint32_t r = 0; r < nruns; ++r) {
+        const size_t i = (size_t)r * PL + ctx;
+        const uint4 e1 = hot_all[2 * i + 1];
+        if ((e1.y >> 3) != epoch) continue;
+        const uint4 e0 = hot_all[2 * i];
+        LionT y;
+        y.m = y.nu = e1.y & 7u;
+        y.l[0] = e0.x; y.l[1] = e0.y; y.l[2] = e0.z; y.l[3] = e0.w; y.l[4] = e1.x;
+#pragma unroll
+        for (int k = 0; k < 5; ++k) y.v[k] = (uint32_t)k < y.nu ? in[cold_all[i * 8 + k] - 1] : 0u;
+        lion_t_compose(x, y);
+    }
+    lion_t_store(out, ctx, x);
+}
+__global__ void cl_export_c(const uint4* __restrict__ entC_all, uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= PL) return;
+    const uint32_t epoch = *epoch_p;
+    uint32_t T = 0, a = 0, b = 0;
+    for (uint32_t r = 0; r < nruns; ++r) {
+        const uint4 e = entC_all[(size_t)r * PL + h];
+        if ((e.y >> 2) == epoch) chunk_t_compose(T, a, b, e.y & 3u, e.x & 0xFFFFu, e.x >> 16);
+    }
+    out[h] = T; out[PL + h] = a; out[2 * PL + h] = b;
+}
+
+// kind 0 = P, 1 = C. The stream-start states: pred 0 everywhere; Lion lists of five zeros; chunk map (0, 0) in bucket 0, else nothing.
+__device__ __forceinline__ void cl_t_init(int alg, int kind, uint32_t* __restrict__ t, uint32_t i) {
+    if (kind == 1) { t[i] = 2; t[PL + i] = i ? FP_INVALID : 0u; t[2 * PL + i] = i ? FP_INVALID : 0u; }
+    else if (alg == ALG_LION) { LionT x = {}; x.m = 5; lion_t_store(t, i, x); }
+    else { t[i] = 1; t[PL + i] = 0; }
+}
+// acc[i] <- acc[i] then next[i]
+__device__ __forceinline__ void cl_t_fold(int alg, int kind, uint32_t* __restrict__ acc, const uint32_t* __restrict__ next, uint32_t i) {
+    if (kind == 1) {
+        uint32_t T = acc[i], a = acc[PL + i], b = acc[2 * PL + i];
+        chunk_t_compose(T, a, b, next[i], next[PL + i], next[2 * PL + i]);
+        acc[i] = T; acc[PL + i] = a; acc[2 * PL + i] = b;
+    } else if (alg == ALG_LION) {
+        LionT x, y; lion_t_load(acc, i, x); lion_t_load(next, i, y);
+        lion_t_compose(x, y);
+        lion_t_store(acc, i, x);
+    } else if (next[i]) {
+        acc[i] = 1; acc[PL + i] = next[PL + i];
+    }
+}
+__global__ void cl_table_init_k(int alg, int kind, uint32_t* __restrict__ t) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < PL) cl_t_init(alg, kind, t, i);
+}
+__global__ void cl_table_fold_k(int alg, int kind, uint32_t* __restrict__ acc, const uint32_t* __restrict__ next) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < PL) cl_t_fold(alg, kind, acc, next, i);
+}
+// carry-in of shard `rank` = the stream-start state, then the transfers of shards 0 .. rank - 1 (`tables` = [world][planes][65536])
+__global__ void cl_rank_fold_k(int alg, int kind, const uint32_t* __restrict__ tables, uint32_t planes, uint32_t rank, uint32_t* __restrict__ carry) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= PL) return;
+    cl_t_init(alg, kind, carry, i);
+    for (uint32_t r = 0; r < rank; ++r) cl_t_fold(alg, kind, carry, tables + (size_t)r * planes * PL, i);
+}
+// the context of a shard's first quad comes from the last quad of the nearest earlier shard that has one (words: [world] {has, quad})
+__global__ void cl_prev_quad_k(const uint32_t* __restrict__ words, uint32_t rank, uint32_t* __restrict__ out) {
+    uint32_t q = 0;
+    for (uint32_t r = 0; r < rank; ++r) if (words[2 * r]) q = words[2 * r + 1];
+    *out = q;
+}
+__global__ void cl_last_quad_k(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t* __restrict__ out) {
+    out[0] = nquads ? 1u : 0u; out[1] = nquads ? in[nquads - 1] : 0u;
+}
+
+// shard gates: the passes of a later shard run under `gate` (open); emit runs under `emit`, settled when the copy-map iteration of the
+// first shard settled (later shards have no copy map). A later shard's round uses `own_epoch`; the first shard's iteration has left
+// the epoch of its settled round in *epoch_word already.
+__global__ void cl_shard_gates(Status* __restrict__ gate, Status* __restrict__ emit, const Status* __restrict__ iter, uint32_t* __restrict__ pair_flag,
+                               uint32_t* __restrict__ epoch_word, uint32_t own_epoch) {
+    gate->nonquiet = 1; gate->converged = 0; gate->error = 0;
+    if (!iter) *epoch_word = own_epoch;
+    emit->nonquiet = 0; emit->error = 0; emit->out_bytes = 0; emit->converged = iter ? iter->converged : 1u;
+    *pair_flag = 0;
+}
+// later shards: two consecutive incompressible blocks would start copy mode (protection_state.rs:38-43)
+__global__ void cl_inc_pairs(const uint8_t* __restrict__ inc, uint64_t nblocks, uint32_t* __restrict__ flag) {
+    for (uint64_t b = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; b + 1 < nblocks; b += (uint64_t)gridDim.x * blockDim.x)
+        if (inc[b] && inc[b + 1]) *flag = 1;
+}
+// the shard's 8 seam words in the layout of the Chameleon encoder's: {first block incompressible, previous_incompressible at the end,
+// refused, has blocks, size lo, size hi, 0, 0}. The first shard of a longer stream is refused when it ends inside a copy run or with a
+// copy penalty pending (its last block incompressible after an incompressible or copied block)
+__global__ void cl_seam_words_k(const uint8_t* __restrict__ inc, const uint8_t* __restrict__ copymap, uint64_t nblocks, int first, int is_last,
+                                const Status* __restrict__ emit, const uint32_t* __restrict__ pair_flag, const uint64_t* __restrict__ d_out_size,
+                                uint32_t* __restrict__ words) {
+    const uint64_t lb = nblocks - 1;
+    auto cp = [&](uint64_t b) { return copymap && copymap[b]; };
+    uint32_t bad = (emit->error || !emit->converged || (pair_flag && *pair_flag)) ? 1u : 0u;
+    if (first && !is_last && (cp(lb) || (inc[lb] && lb > 0 && (cp(lb - 1) || inc[lb - 1])))) bad = 1;
+    words[0] = (!cp(0) && inc[0]) ? 1u : 0u;
+    words[1] = (cp(lb) || inc[lb]) ? 1u : 0u;
+    words[2] = bad; words[3] = 1;
+    const uint64_t sz = *d_out_size;
+    words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
+}
+
 }  // namespace chee
 
 using namespace chee;
@@ -687,32 +885,39 @@ size_t chee_tables_bytes(int alg, int region, size_t nbytes, int num_sms) {
     return (size_t)chee_pick_runs(nbytes, num_sms) * 65536 * per;
 }
 
-// Enqueue the parallel Cheetah / Lion encode. *d_converged (device u32) != 0 afterwards means d_out / d_out_size hold the result;
-// otherwise the caller's in-order kernel (queued behind, gated on that flag) produces it. `epoch_base`: the caller hands out 32 fresh
-// epochs (values in 1 .. 2^28) per call and clears `tables` if it ever has to reuse one.
-// `resume`: continue an iteration that a previous call on the same input and workspace left unsettled (callers that may block read
-// *d_converged and call again): the stages on the prefix are skipped and the whole-input stages start from the last committed map.
-cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* const tables[3],
-                                 uint32_t epoch_base, int num_sms, uint64_t* d_out_size, uint32_t* d_converged, bool resume,
-                                 cudaStream_t stream, uint64_t* launches) {
+// pointers into one workspace (chee_layout) and the three run-table regions
+struct CheeBufs {
+    Status* stages; uint32_t *Pb, *Ab, *Bb, *F0, *F1, *F2; uint8_t *cm, *cm2, *incb; uint32_t *seg, *ctx0, *tile_bytes, *tile_local;
+    uint64_t *group_total, *group_off; uint4* entP; uint32_t* coldP; uint4* entC;
+    CheeBufs(uint8_t* ws, const CheeLayout& L, uint8_t* const tables[3]) {
+        stages = reinterpret_cast<Status*>(ws + L.status);
+        Pb = reinterpret_cast<uint32_t*>(ws + L.Pbits); Ab = reinterpret_cast<uint32_t*>(ws + L.Abits); Bb = reinterpret_cast<uint32_t*>(ws + L.Bbits);
+        F0 = reinterpret_cast<uint32_t*>(ws + L.F0); F1 = reinterpret_cast<uint32_t*>(ws + L.F1); F2 = reinterpret_cast<uint32_t*>(ws + L.F2);
+        cm = ws + L.copymap; cm2 = ws + L.copymap2; incb = ws + L.incb;
+        seg = reinterpret_cast<uint32_t*>(ws + L.seg_state);
+        ctx0 = reinterpret_cast<uint32_t*>(ws + L.ctx0);
+        tile_bytes = reinterpret_cast<uint32_t*>(ws + L.tile_bytes); tile_local = reinterpret_cast<uint32_t*>(ws + L.tile_local);
+        group_total = reinterpret_cast<uint64_t*>(ws + L.group_total); group_off = reinterpret_cast<uint64_t*>(ws + L.group_off);
+        entP = reinterpret_cast<uint4*>(tables[0]); coldP = reinterpret_cast<uint32_t*>(tables[1]); entC = reinterpret_cast<uint4*>(tables[2]);
+    }
+};
+
+// The staged copy-map iteration (epochs epoch_base .. epoch_base + 31). *st_out = the Status block of the last stage: converged != 0
+// means the committed copy map (cm) and the flags and run tables of the last round that ran are final; *d_epoch_out (device, may be
+// nullptr) receives that round's epoch.
+static cudaError_t chee_iterate(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* ws, const CheeLayout& L, uint32_t nruns, uint8_t* const tables[3],
+                                uint32_t epoch_base, int num_sms, bool resume, uint32_t* d_epoch_out, cudaStream_t stream, uint64_t* launches,
+                                Status** st_out) {
     const bool lion = alg == ALG_LION;
     const uint32_t bbytes = lion ? 64 : 128;
-    const uint32_t nruns = chee_pick_runs(nbytes, num_sms);
-    CheeLayout L; chee_layout(nbytes, nruns, &L);
-    const uint64_t nblocks = (nbytes + bbytes - 1) / bbytes;
     const uint32_t ntiles = (uint32_t)(((nbytes + 127) / 128 + TILE_B - 1) / TILE_B);
-    const uint32_t ngroups = (ntiles + 4095) / 4096;
-    Status* const stages = reinterpret_cast<Status*>(ws + L.status);
+    const CheeBufs B(ws, L, tables);
+    Status* const stages = B.stages;
     const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    uint32_t* Pb = reinterpret_cast<uint32_t*>(ws + L.Pbits); uint32_t* Ab = reinterpret_cast<uint32_t*>(ws + L.Abits); uint32_t* Bb = reinterpret_cast<uint32_t*>(ws + L.Bbits);
-    uint32_t* F0 = reinterpret_cast<uint32_t*>(ws + L.F0); uint32_t* F1 = reinterpret_cast<uint32_t*>(ws + L.F1); uint32_t* F2 = reinterpret_cast<uint32_t*>(ws + L.F2);
-    uint8_t* cm = ws + L.copymap; uint8_t* cm2 = ws + L.copymap2; uint8_t* incb = ws + L.incb;
-    uint32_t* seg = reinterpret_cast<uint32_t*>(ws + L.seg_state);
-    uint32_t* ctx0 = reinterpret_cast<uint32_t*>(ws + L.ctx0);
-    uint32_t* tile_bytes = reinterpret_cast<uint32_t*>(ws + L.tile_bytes);
-    uint4* entP = reinterpret_cast<uint4*>(tables[0]);
-    uint32_t* coldP = reinterpret_cast<uint32_t*>(tables[1]);
-    uint4* entC = reinterpret_cast<uint4*>(tables[2]);
+    uint32_t* Pb = B.Pb; uint32_t* Ab = B.Ab; uint32_t* Bb = B.Bb; uint32_t* F0 = B.F0; uint32_t* F1 = B.F1; uint32_t* F2 = B.F2;
+    uint8_t* cm = B.cm; uint8_t* cm2 = B.cm2; uint8_t* incb = B.incb;
+    uint32_t* seg = B.seg; uint32_t* ctx0 = B.ctx0; uint32_t* tile_bytes = B.tile_bytes;
+    uint4* entP = B.entP; uint32_t* coldP = B.coldP; uint4* entC = B.entC;
     cudaError_t e = cudaMemsetAsync(ws + L.status, 0, L.Pbits - L.status, stream);     // both status blocks
     if (e != cudaSuccess) return e;
 
@@ -724,18 +929,18 @@ cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, ui
         const uint32_t run_ctas = (runs + RP_WARPS - 1) / RP_WARPS;
         const uint8_t* mask = it ? cm : nullptr;
         if (lion) {
-            lion_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, ctx0);
+            lion_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, nullptr, epoch, d_epoch_out, ctx0);
             lion_pass_p<<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, ctx0, entP, coldP, epoch, F0, F1, F2, Pb);
-            lion_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, coldP, epoch, F0, F1, F2, Pb);
+            lion_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, coldP, epoch, nullptr, F0, F1, F2, Pb);
             chee_pass_c<2><<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, Pb, entC, epoch, Ab, Bb);
-            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, Ab, Bb);
+            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, nullptr, Ab, Bb);
             lion_tile_sizes<<<(nt + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, mask, nb, nblk, nt, 0, st, incb, tile_bytes);
         } else {
-            chee_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, ctx0);
+            chee_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, nullptr, epoch, d_epoch_out, ctx0);
             chee_pass_p<<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, mask, runs, nt, st, ctx0, entP, epoch, Pb);
-            chee_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, epoch, Pb);
+            chee_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, epoch, nullptr, Pb);
             chee_pass_c<1><<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, Pb, entC, epoch, Ab, Bb);
-            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, Ab, Bb);
+            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, nullptr, Ab, Bb);
             chee_tile_sizes<<<(nt + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, mask, nb, nblk, nt, 0, st, incb, tile_bytes);
         }
         *launches += 7;
@@ -774,6 +979,31 @@ cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, ui
         if (e == cudaSuccess) e = stage(&stages[1], &stages[0], 1, nbytes, nruns, epoch_base + 8);
         st = &stages[1];
     }
+    *st_out = st;
+    return e;
+}
+
+// Enqueue the parallel Cheetah / Lion encode. *d_converged (device u32) != 0 afterwards means d_out / d_out_size hold the result;
+// otherwise the caller's in-order kernel (queued behind, gated on that flag) produces it. `epoch_base`: the caller hands out 32 fresh
+// epochs (values in 1 .. 2^28) per call and clears `tables` if it ever has to reuse one.
+// `resume`: continue an iteration that a previous call on the same input and workspace left unsettled (callers that may block read
+// *d_converged and call again): the stages on the prefix are skipped and the whole-input stages start from the last committed map.
+cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* const tables[3],
+                                 uint32_t epoch_base, int num_sms, uint64_t* d_out_size, uint32_t* d_converged, bool resume,
+                                 cudaStream_t stream, uint64_t* launches) {
+    const bool lion = alg == ALG_LION;
+    const uint32_t bbytes = lion ? 64 : 128;
+    const uint32_t nruns = chee_pick_runs(nbytes, num_sms);
+    CheeLayout L; chee_layout(nbytes, nruns, &L);
+    const uint64_t nblocks = (nbytes + bbytes - 1) / bbytes;
+    const uint32_t ntiles = (uint32_t)(((nbytes + 127) / 128 + TILE_B - 1) / TILE_B);
+    const uint32_t ngroups = (ntiles + 4095) / 4096;
+    const CheeBufs B(ws, L, tables);
+    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
+    uint32_t* Pb = B.Pb; uint32_t* Ab = B.Ab; uint32_t* Bb = B.Bb; uint32_t* F0 = B.F0; uint32_t* F1 = B.F1; uint32_t* F2 = B.F2;
+    uint8_t* cm = B.cm; uint8_t* incb = B.incb; uint32_t* tile_bytes = B.tile_bytes;
+    Status* st = nullptr;
+    cudaError_t e = chee_iterate(alg, d_in, nbytes, ws, L, nruns, tables, epoch_base, num_sms, resume, nullptr, stream, launches, &st);
     if (e != cudaSuccess) return e;
     // final sizes under the committed copy map (valid only if converged), scan, emit
     if (lion) lion_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, cm, nbytes, nblocks, ntiles, 1, st, incb, tile_bytes);
@@ -787,6 +1017,147 @@ cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, ui
                                                reinterpret_cast<uint64_t*>(ws + L.group_off), 4096, d_out);
     chee_finish<<<1, 1, 0, stream>>>(st, d_converged, d_out_size);
     *launches += 5;
+    return cudaGetLastError();
+}
+
+// ---- sharded encode: one shard of a longer stream, in three phases around the two table exchanges ----------------------------------
+// The shard's workspace = chee_layout of its length, then the shard's own status area (gate, emit gate, pair flag, the epoch of the
+// round the shard exports). Every call takes CL_SHARD_EPOCHS fresh epochs: the first 32 for the copy-map iteration of the first shard,
+// epoch_base + 32 for the one round of a later shard, which all three phases share.
+//
+// The first shard has no carry-in: when its iteration has settled, the flags and run tables of its settled round are final, so it
+// only exports them (the epoch comes from ctx0, on the device) and, in phase 3, sizes, scans and emits under the committed map as
+// chee_encode_parallel does. A later shard runs ctx0 and pass P, fold P and pass C, fold C, without a copy map.
+constexpr uint32_t CL_SHARD_EPOCHS = 40;
+uint32_t cl_shard_epochs() { return CL_SHARD_EPOCHS; }
+uint32_t cl_table_planes(int alg, int kind) { return kind == 1 ? 3u : alg == ALG_LION ? 12u : 2u; }
+size_t cl_shard_workspace_bytes(size_t nbytes, int num_sms) { return ((chee_workspace_bytes(nbytes, num_sms) + 255) & ~(size_t)255) + 1024; }
+
+namespace {
+struct ClShardGeo {
+    bool lion; uint32_t bbytes, nruns, ntiles, ngroups, run_ctas; uint64_t nq, nstep, nblk; CheeLayout L;
+    Status *gate, *emit; uint32_t *pair_flag, *epoch_word;
+    ClShardGeo(int alg, size_t n, int num_sms, uint8_t* ws) {
+        lion = alg == ALG_LION; bbytes = lion ? 64 : 128;
+        nruns = chee_pick_runs(n, num_sms); chee_layout(n, nruns, &L);
+        nq = n / 4; nstep = (n + 127) / 128; nblk = (n + bbytes - 1) / bbytes;
+        ntiles = (uint32_t)((nstep + TILE_B - 1) / TILE_B); ngroups = (ntiles + 4095) / 4096; run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
+        gate = reinterpret_cast<Status*>(ws + ((L.total + 255) & ~(size_t)255)); emit = gate + 1; pair_flag = reinterpret_cast<uint32_t*>(emit + 1);
+        epoch_word = pair_flag + 1;
+    }
+};
+}  // namespace
+
+// Phase 1: the first shard (d_prev_quad == nullptr) runs the copy-map iteration to the end; a later shard runs ctx0 and pass P. Both
+// export their P transfer.
+cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32_t* d_prev_quad, uint8_t* ws, uint8_t* const tables[3],
+                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches) {
+    const ClShardGeo G(alg, n, num_sms, ws);
+    const CheeBufs B(ws, G.L, tables);
+    const bool first = d_prev_quad == nullptr;
+    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
+    const uint32_t ep = epoch_base + 32;
+    Status* iter = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (first) e = chee_iterate(alg, d_in, n, ws, G.L, G.nruns, tables, epoch_base, num_sms, false, G.epoch_word, stream, launches, &iter);
+    if (e != cudaSuccess) return e;
+    cl_shard_gates<<<1, 1, 0, stream>>>(G.gate, G.emit, iter, G.pair_flag, G.epoch_word, ep);
+    ++*launches;
+    if (!first) {
+        if (G.lion) {
+            lion_ctx0<<<(G.nruns + 127) / 128, 128, 0, stream>>>(in32, G.nq, nullptr, G.nruns, G.ntiles, G.gate, d_prev_quad, ep, nullptr, B.ctx0);
+            lion_pass_p<<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.ctx0, B.entP, B.coldP,
+                                                                  ep, B.F0, B.F1, B.F2, B.Pb);
+        } else {
+            chee_ctx0<<<(G.nruns + 127) / 128, 128, 0, stream>>>(in32, G.nq, nullptr, G.nruns, G.ntiles, G.gate, d_prev_quad, ep, nullptr, B.ctx0);
+            chee_pass_p<<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, nullptr, G.nruns, G.ntiles, G.gate, B.ctx0, B.entP, ep, B.Pb);
+        }
+        *launches += 2;
+    }
+    if (G.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(in32, B.entP, B.coldP, G.nruns, G.epoch_word, d_tab_p);
+    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(B.entP, G.nruns, G.epoch_word, d_tab_p);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// Phase 2: a later shard makes its predictions final from the carried-in P state (planes as cl_table_init / cl_rank_fold leave them;
+// nullptr = stream start) and runs pass C; every shard exports its C transfer. The first shard ignores d_carry_p (its state is the
+// stream start, and its flags are final already).
+cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, const uint32_t* d_carry_p, uint8_t* ws, uint8_t* const tables[3],
+                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
+    const ClShardGeo G(alg, n, num_sms, ws);
+    const CheeBufs B(ws, G.L, tables);
+    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
+    const uint32_t ep = epoch_base + 32;
+    if (!first && G.lion) {
+        lion_fold_p<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entP, B.coldP, ep, d_carry_p ? d_carry_p + 2 * PL : nullptr, B.F0, B.F1, B.F2, B.Pb);
+        chee_pass_c<2><<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.Pb, B.entC, ep, B.Ab, B.Bb);
+        *launches += 2;
+    } else if (!first) {
+        chee_fold_p<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entP, ep, d_carry_p ? d_carry_p + PL : nullptr, B.Pb);
+        chee_pass_c<1><<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.Pb, B.entC, ep, B.Ab, B.Bb);
+        *launches += 2;
+    }
+    cl_export_c<<<PL / 128, 128, 0, stream>>>(B.entC, G.nruns, G.epoch_word, d_tab_c);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// Phase 3: a later shard makes its chunk-map flags final from the carried-in C state (the first shard ignores d_carry_c); then sizes
+// and incompressible bits, scan, emit, the shard's 8 seam words.
+cudaError_t cl_shard_phase3(int alg, const uint8_t* d_in, size_t n, bool first, bool is_last, const uint32_t* d_carry_c, uint8_t* ws,
+                            uint8_t* const tables[3], uint32_t epoch_base, int num_sms, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                            uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
+    const ClShardGeo G(alg, n, num_sms, ws);
+    const CheeBufs B(ws, G.L, tables);
+    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
+    const uint32_t ep = epoch_base + 32;
+    const uint8_t* mask = first ? B.cm : nullptr;
+    if (!first) {
+        chee_fold_c<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entC, ep, d_carry_c ? d_carry_c + PL : nullptr, B.Ab, B.Bb);
+        ++*launches;
+    }
+    if (G.lion) lion_tile_sizes<<<(G.ntiles + 7) / 8, 256, 0, stream>>>(B.Pb, B.Ab, B.Bb, mask, n, G.nblk, G.ntiles, 0, G.gate, B.incb, B.tile_bytes);
+    else chee_tile_sizes<<<(G.ntiles + 7) / 8, 256, 0, stream>>>(B.Pb, B.Ab, B.Bb, mask, n, G.nblk, G.ntiles, 0, G.gate, B.incb, B.tile_bytes);
+    ++*launches;
+    if (!first) {
+        const uint64_t want = (G.nblk + 255) / 256;
+        const uint32_t grid = (uint32_t)(want < (uint64_t)num_sms * 8 ? (want ? want : 1) : (uint64_t)num_sms * 8);
+        cl_inc_pairs<<<grid, 256, 0, stream>>>(B.incb, G.nblk, G.pair_flag);
+        ++*launches;
+    }
+    cudaError_t e = scan_tiles_launch(B.tile_bytes, G.ntiles, B.tile_local, B.group_total, B.group_off, G.ngroups, G.emit, cap, d_out_size, stream);
+    if (e != cudaSuccess) return e;
+    if (G.lion) lion_emit<<<G.ntiles, 256, 0, stream>>>(in32, n, G.nblk, B.F0, B.F1, B.F2, B.Pb, B.Ab, B.Bb, mask, G.emit, B.tile_local, B.group_off, 4096, d_out);
+    else chee_emit<<<G.ntiles, 256, 0, stream>>>(in32, n, G.nblk, B.Pb, B.Ab, B.Bb, mask, G.emit, B.tile_local, B.group_off, 4096, d_out);
+    cl_seam_words_k<<<1, 1, 0, stream>>>(B.incb, mask, G.nblk, first, is_last, G.emit, first ? nullptr : G.pair_flag, d_out_size, d_seam8);
+    *launches += 4;
+    return cudaGetLastError();
+}
+
+cudaError_t cl_table_init(int alg, int kind, uint32_t* d_table, cudaStream_t stream, uint64_t* launches) {
+    cl_table_init_k<<<PL / 256, 256, 0, stream>>>(alg, kind, d_table);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches) {
+    cl_table_fold_k<<<PL / 256, 256, 0, stream>>>(alg, kind, d_acc, d_next);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cl_rank_fold(int alg, int kind, const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches) {
+    cl_rank_fold_k<<<PL / 128, 128, 0, stream>>>(alg, kind, d_tables, cl_table_planes(alg, kind), rank, d_carry);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cl_last_quad(const uint8_t* d_in, size_t n, uint32_t* d_out2, cudaStream_t stream, uint64_t* launches) {
+    cl_last_quad_k<<<1, 1, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_in), n / 4, d_out2);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cl_prev_quad(const uint32_t* d_words, uint32_t rank, uint32_t* d_out, cudaStream_t stream, uint64_t* launches) {
+    cl_prev_quad_k<<<1, 1, 0, stream>>>(d_words, rank, d_out);
+    ++*launches;
     return cudaGetLastError();
 }
 

@@ -50,6 +50,25 @@ size_t chee_tables_bytes(int alg, int region, size_t nbytes, int num_sms);
 cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* const tables[3],
                                  uint32_t epoch_base, int num_sms, uint64_t* d_out_size, uint32_t* d_converged, bool resume,
                                  cudaStream_t stream, uint64_t* launches);
+// sharded Cheetah / Lion encode: one shard of a longer stream (non-final shards whole 256-byte multiples). Tables are stacks of
+// cl_table_planes(alg, kind) planes of 65536 u32 (kind 0 = predictions, 1 = chunk map). Each call of phase 1 takes cl_shard_epochs()
+// fresh epochs starting at epoch_base; phases 2 and 3 get the same epoch_base. d_prev_quad: the last quad of the stream before the shard
+// (nullptr = the first shard, which alone may use copy mode); d_carry_*: the carried-in state (nullptr = stream start).
+uint32_t cl_shard_epochs();
+uint32_t cl_table_planes(int alg, int kind);
+size_t cl_shard_workspace_bytes(size_t nbytes, int num_sms);
+cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32_t* d_prev_quad, uint8_t* ws, uint8_t* const tables[3],
+                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, const uint32_t* d_carry_p, uint8_t* ws, uint8_t* const tables[3],
+                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_shard_phase3(int alg, const uint8_t* d_in, size_t n, bool first, bool is_last, const uint32_t* d_carry_c, uint8_t* ws,
+                            uint8_t* const tables[3], uint32_t epoch_base, int num_sms, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                            uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_table_init(int alg, int kind, uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_rank_fold(int alg, int kind, const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_last_quad(const uint8_t* d_in, size_t n, uint32_t* d_out2, cudaStream_t stream, uint64_t* launches);   // {has a quad, last quad}
+cudaError_t cl_prev_quad(const uint32_t* d_words, uint32_t rank, uint32_t* d_out, cudaStream_t stream, uint64_t* launches);
 
 // chameleon_decode.cu
 size_t cham_decode_workspace_bytes(size_t nbytes, size_t cap, int nruns_max);

@@ -13,6 +13,12 @@ Decode is the mirror image: rank r decodes its piece back into its shard with th
 phase 1 (boundaries, writer pass) needs no carry-in and exports the piece's table; phase 2 decodes from the folded carry-in
 and writes 8 seam words, which every rank gathers and judges with `seam_verdict`.
 
+Cheetah and Lion shard the same way with three phases around two exchanges (ShardedCLEncoder): the last quad of every shard (the
+context of the next shard's first quad), then the shard's prediction transfer (P table), then its chunk-map transfer (C table). A
+transfer says what the shard does to the state carried into it; the carry-in of rank r is the stream-start state folded with the
+transfers of ranks < r (density_b200_cl_table_init / _fold, on the device). Only rank 0 may use copy mode; the seam verdict refuses
+what would need it elsewhere.
+
 A stream whose cuts are not known (one chameleon_encode call, the reference library, a file) is cut at byte ranges instead
 (`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
 (density_b200_decode_locate), and after an all_gather of the maps `locate_piece` gives every rank the exact offset where its
@@ -153,6 +159,118 @@ class ShardedChameleonEncoder:
             raise _lib.DensityB200Error(f"shard_phase2 rc={rc}: {_lib.last_error()}")
 
 
+ALGS = {"chameleon": 0, "cheetah": 1, "lion": 2}
+CL_TABLE_P, CL_TABLE_C = 0, 1
+
+
+def _alg_id(alg):
+    return ALGS[alg] if isinstance(alg, str) else int(alg)
+
+
+def fold_cl_tables(alg, kind, gathered, rank):
+    """carry-in of `rank` for the Cheetah / Lion sharded encode: the stream-start state (density_b200_cl_table_init) folded with the
+    tables of ranks < rank in order (density_b200_cl_table_fold). gathered: CUDA int32 [world, words]. Enqueued on torch's current
+    stream."""
+    lib = _lib.load()
+    alg = _alg_id(alg)
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    carry = torch.empty(gathered.shape[1], dtype=torch.int32, device=gathered.device)
+    rc = lib.density_b200_cl_table_init(alg, kind, carry.data_ptr(), stream)
+    for r in range(rank):
+        if rc == 0:
+            rc = lib.density_b200_cl_table_fold(alg, kind, carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
+    if rc:
+        raise _lib.DensityB200Error(f"cl_table_init / fold rc={rc}: {_lib.last_error()}")
+    return carry
+
+
+class ShardedCLEncoder:
+    """Sharded Cheetah / Lion encode through the shard phases, with torch.distributed for the exchanges (the phase-level twin of
+    ShardedEncoder.encode(..., alg=...)). Rank r's d_in is bytes [o_r, o_r + n_r) of one input; non-final shards are multiples of 256
+    bytes. The concatenation of the pieces equals one cheetah_encode / lion_encode call over the whole input when flags == 0."""
+
+    def __init__(self, alg):
+        self._lib = _lib.load()
+        self.alg = _alg_id(alg)
+        self._h = self._lib.density_b200_cl_shard_create(self.alg)
+        if not self._h:
+            raise _lib.DensityB200Error(_lib.last_error())
+        self.words_p = self._lib.density_b200_cl_table_words(self.alg, CL_TABLE_P)
+        self.words_c = self._lib.density_b200_cl_table_words(self.alg, CL_TABLE_C)
+        self.events = None
+
+    def close(self):
+        if self._h:
+            self._lib.density_b200_cl_shard_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _gather(self, t, world, group):
+        if world == 1:
+            return t.view(1, -1)
+        out = torch.empty((world, t.numel()), dtype=t.dtype, device=t.device)
+        dist.all_gather_into_tensor(out.view(-1), t.contiguous(), group=group)
+        return out
+
+    def encode(self, d_in, d_out, d_size, group=None, timing=False):
+        """d_in: CUDA uint8 tensor (4-byte aligned), this rank's shard; d_out: its output buffer (2-byte aligned); d_size: int64[1].
+        Returns seam_verdict's (flags, total, offsets) over all ranks; flags != 0: the pieces are void and the caller encodes on one
+        device. timing: record CUDA events around the phases in self.events (phase 1, P exchange + fold, phase 2, C exchange + fold,
+        phase 3 + seams)."""
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        dev = d_in.device
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)] if timing else None
+        mark = (lambda k: ev[k].record()) if timing else (lambda k: None)
+        n = d_in.numel()
+        last = torch.zeros(2, dtype=torch.int32, device=dev)        # {has a quad, last quad}: the next shard's first context
+        if n >= 4:
+            last[0] = 1
+            last[1:] = d_in[n // 4 * 4 - 4:n // 4 * 4].clone().view(torch.int32)
+        quads = self._gather(last, world, group)
+        prev = None
+        if rank > 0:
+            prev = torch.zeros(1, dtype=torch.int32, device=dev)
+            for r in range(rank):
+                prev = torch.where(quads[r, 0] != 0, quads[r, 1:2], prev)
+        mark(0)
+        tp = torch.empty(self.words_p, dtype=torch.int32, device=dev)
+        rc = self._lib.density_b200_cl_shard_phase1(self._h, d_in.data_ptr(), n, int(rank == world - 1),
+                                                    prev.data_ptr() if prev is not None else None, tp.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"cl_shard_phase1 rc={rc}: {_lib.last_error()}")
+        mark(1)
+        carry_p = fold_cl_tables(self.alg, CL_TABLE_P, self._gather(tp, world, group), rank) if rank > 0 else None
+        mark(2)
+        tc = torch.empty(self.words_c, dtype=torch.int32, device=dev)
+        rc = self._lib.density_b200_cl_shard_phase2(self._h, carry_p.data_ptr() if carry_p is not None else None, tc.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"cl_shard_phase2 rc={rc}: {_lib.last_error()}")
+        mark(3)
+        carry_c = fold_cl_tables(self.alg, CL_TABLE_C, self._gather(tc, world, group), rank) if rank > 0 else None
+        mark(4)
+        words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
+        rc = self._lib.density_b200_cl_shard_phase3(self._h, carry_c.data_ptr() if carry_c is not None else None, d_out.data_ptr(),
+                                                    d_out.numel(), d_size.data_ptr(), words.data_ptr(), stream)
+        if rc:
+            raise _lib.DensityB200Error(f"cl_shard_phase3 rc={rc}: {_lib.last_error()}")
+        verdict = seam_verdict(self._gather(words, world, group))
+        mark(5)
+        self.events = ev
+        return verdict
+
+    def phase_ms(self):
+        """[phase 1, P exchange + fold, phase 2, C exchange + fold, phase 3 + seams] in ms, of the last encode(timing=True)"""
+        torch.cuda.synchronize()
+        return [self.events[k].elapsed_time(self.events[k + 1]) for k in range(5)]
+
+
 class ShardedChameleonDecoder:
     """Decode of this rank's piece through the shard phases, with torch.distributed for the exchanges (the mirror of
     ShardedChameleonEncoder)."""
@@ -270,19 +388,24 @@ class ShardedEncoder(_ShardedHandle):
     the exact seam verdict and the optional variable-length gather of the pieces to one rank, over the library's NCCL communicator.
     """
 
-    def encode(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None):
+    def encode(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None, alg="chameleon"):
         """Enqueue on torch's current stream. d_size int64[1]: this rank's piece; d_flags int32[1]: != 0 -> the stream is not quiet and
-        the pieces are void; self.d_total int64[1]: stream length. gather_root >= 0: pieces gathered into d_gather on that rank (blocks)."""
+        the pieces are void; self.d_total int64[1]: stream length. gather_root >= 0: pieces gathered into d_gather on that rank (blocks).
+        alg "cheetah" / "lion" (or their ids): density_b200_encode_sharded_cl, the same contract for those algorithms."""
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self._lib.density_b200_encode_sharded(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(),
-                                                   d_flags.data_ptr(), self.d_total.data_ptr(), int(gather_root),
-                                                   d_gather.data_ptr() if d_gather is not None else None,
-                                                   d_gather.numel() if d_gather is not None else 0, stream)
+        args = (d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(),
+                int(gather_root), d_gather.data_ptr() if d_gather is not None else None, d_gather.numel() if d_gather is not None else 0, stream)
+        alg = _alg_id(alg)
+        if alg == 0:
+            rc = self._lib.density_b200_encode_sharded(self._h, *args)
+        else:
+            rc = self._lib.density_b200_encode_sharded_cl(self._h, alg, *args)
         if rc:
-            raise _lib.DensityB200Error(f"encode_sharded rc={rc}: {_lib.last_error()}")
+            raise _lib.DensityB200Error(f"encode_sharded{'' if alg == 0 else '_cl'} rc={rc}: {_lib.last_error()}")
 
     def profile(self):
-        """stage times (ms) of the last call: flag pass, table exchange + fold, carry / resolve / sizes / scan, emit, seams + gather"""
+        """stage times (ms) of the last encode: Chameleon flag pass, table exchange + fold, carry / resolve / sizes / scan, emit, seams +
+        gather; Cheetah / Lion phase 1, P exchange + fold, phase 2 + C exchange + fold, phase 3, seams + gather"""
         out = (ctypes.c_float * 5)()
         rc = self._lib.density_b200_sharded_profile(self._h, out)
         if rc:

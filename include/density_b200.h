@@ -152,8 +152,59 @@ DENSITY_B200_API density_b200_sharded* density_b200_sharded_create(const uint8_t
 DENSITY_B200_API void density_b200_sharded_destroy(density_b200_sharded*);
 DENSITY_B200_API int density_b200_encode_sharded(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream);
-/* stage times (ms) of the last call: [0] flag pass, [1] table exchange + fold, [2] carry / resolve / sizes / scan, [3] emit, [4] seams + gather */
+/* stage times (ms) of the last encode_sharded or encode_sharded_cl call. Chameleon: [0] flag pass, [1] table exchange + fold, [2] carry /
+   resolve / sizes / scan, [3] emit, [4] seams + gather. Cheetah / Lion: [0] phase 1, [1] P exchange + fold, [2] phase 2 + C exchange +
+   fold, [3] phase 3, [4] seams + gather. */
 DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* out_ms5);
+
+/*
+ * Sharded Cheetah / Lion encode (one bit-exact stream cut across several GPUs / calls; DESIGN.md section 5). Shard r holds bytes
+ * [o_r, o_r + n_r) of one input; every non-final shard is a multiple of 256 bytes. The concatenation of the shard outputs equals one
+ * cheetah_encode / lion_encode call over the whole input, byte for byte, whenever the verdict is 0. The verdict is non-zero (the pieces
+ * are void and the caller encodes on one device) when the first shard's copy-map iteration did not settle; when the first shard is not
+ * the last one and ends inside a copy run or with a copy penalty pending; when a later shard has two consecutive incompressible blocks
+ * (it would need copy mode, which only the first shard may use); when a seam joins two incompressible blocks; or on an error (capacity).
+ * The stream start belongs to the first shard: with that shard empty, the next one meets the cold-dictionary start without a copy map
+ * and is normally refused.
+ * Three phases around two table exchanges. Tables are stacks of u32 planes of 65536 entries (density_b200_cl_table_words u32 in all):
+ *   P, Cheetah  {touched, last quad} per context
+ *   P, Lion     {m, nu, l0..l4, v0..v4} per context: the shard's m local values, and the nu values of its undecided accesses, each of
+ *               which removes one matching entry of the list carried into the shard
+ *   C, both     {T, a, b} per bucket: T 0 untouched, 1 accessed with one value a, 2 ends as (a, b); 16-bit in-bucket fingerprints
+ * A table describes what a shard does to the state carried into it; density_b200_cl_table_init gives the stream-start state and
+ * density_b200_cl_table_fold(acc, next) makes acc "acc, then next", so the carry-in of shard r is init folded with the tables of
+ * shards 0 .. r - 1 in order. All-zero tables are the identity (an empty shard).
+ */
+#define DENSITY_B200_CL_TABLE_P 0
+#define DENSITY_B200_CL_TABLE_C 1
+typedef struct density_b200_cl_shard density_b200_cl_shard; /* opaque */
+/* alg: DENSITY_B200_CHEETAH or DENSITY_B200_LION (otherwise NULL, see density_b200_last_error) */
+DENSITY_B200_API density_b200_cl_shard* density_b200_cl_shard_create(int alg);
+DENSITY_B200_API void density_b200_cl_shard_destroy(density_b200_cl_shard*);
+/* u32 words of one table of `kind` (DENSITY_B200_CL_TABLE_P / _C); 0 for a bad algorithm or kind */
+DENSITY_B200_API size_t density_b200_cl_table_words(int alg, int kind);
+/* phase 1: d_in 4-byte aligned. d_prev_quad: device pointer to the last quad (4 bytes) of the stream before this shard, NULL for the
+   first shard, which alone runs the copy-map iteration (as the single-device encoder) and exports straight from its settled round.
+   Exports the shard's P table. Phases 2 and 3 read d_in again: it must stay valid and unchanged until phase 3 has been enqueued. */
+DENSITY_B200_API int density_b200_cl_shard_phase1(density_b200_cl_shard*, const uint8_t* d_in, size_t n, int is_last_shard,
+                                 const uint32_t* d_prev_quad, uint32_t* d_table_p_out, void* stream);
+/* phase 2: d_carry_p = the P state before this shard (NULL = stream start; the first shard ignores it). Exports the shard's C table. */
+DENSITY_B200_API int density_b200_cl_shard_phase2(density_b200_cl_shard*, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream);
+/* phase 3: d_carry_c = the C state before this shard (NULL = stream start; the first shard ignores it). Writes the shard's piece to d_out (2-byte aligned), its size
+   to *d_out_size and its 8 seam words to d_seam8 in the layout of density_b200_decode_shard_phase2 ("last block incompressible" =
+   previous_incompressible at the shard end; word 2 = this shard is refused). The verdict over all shards is that of the Chameleon
+   sharded paths: non-zero when a word 2 is set or a seam joins two incompressible blocks. One phase 3 per phase 1. */
+DENSITY_B200_API int density_b200_cl_shard_phase3(density_b200_cl_shard*, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap,
+                                 uint64_t* d_out_size, uint32_t* d_seam8, void* stream);
+DENSITY_B200_API int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* stream);
+DENSITY_B200_API int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, void* stream);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments and gather semantics of density_b200_encode_sharded:
+   ncclAllGather of the last quads -> phase 1 -> ncclAllGather(P tables, 0.5 MiB per rank for Cheetah, 3 MiB for Lion) -> one fold
+   kernel -> phase 2 -> ncclAllGather(C tables, 0.75 MiB) -> one fold kernel -> phase 3 -> seam words -> verdict -> optional gather.
+   Uses its own workspace in the handle. */
+DENSITY_B200_API int density_b200_encode_sharded_cl(density_b200_sharded*, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                   uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather,
+                                   size_t gather_cap, void* stream);
 
 /*
  * Sharded Chameleon decode: the inverse of the sharded encode. Piece r is what shard r of a sharded encode produced (rank r's

@@ -52,6 +52,22 @@ _SIGS = {
     "density_b200_cl_table_fold": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_encode_sharded_cl": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
                                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_create": (ctypes.c_void_p, []),
+    "density_b200_cheetah_decode_shard_destroy": (None, [ctypes.c_void_p]),
+    "density_b200_cheetah_decode_round_budget": (ctypes.c_int, []),
+    "density_b200_cheetah_cmap_words": (ctypes.c_size_t, []),
+    "density_b200_cheetah_decode_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_int,
+                                                                ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_round_walk": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_round_fold": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                                    ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_phase3": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_status": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32)]),
+    "density_b200_cheetah_cmap_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_cmap_fold": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded_cheetah": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_codec_create": (ctypes.c_void_p, [ctypes.c_int]),
     "density_b200_codec_destroy": (None, [ctypes.c_void_p]),
     "density_b200_codec_clear_state": (ctypes.c_int, [ctypes.c_void_p]),
@@ -68,6 +84,7 @@ _SIGS = {
     "density_b200_cheetah_decode_rounds": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint32)]),
     "density_b200_encode_status": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_test_set_stage_rounds": (None, [ctypes.c_int]),
+    "density_b200_test_set_decode_rounds": (None, [ctypes.c_int]),
     "density_b200_prot_debug": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_shutdown": (None, []),
     "density_b200_version": (ctypes.c_char_p, []),

@@ -855,6 +855,165 @@ int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_
     return DENSITY_B200_OK;
 }
 
+// ---- sharded Cheetah decode: one piece, its chunk map carried in and its prediction rounds run over all pieces ------------------------
+static int g_chee_dec_rounds = 40;    // round budget of the sharded Cheetah decode (density_b200_test_set_decode_rounds)
+
+struct density_b200_cheetah_decode_shard {
+    DevBuf ws, tables;
+    CheeShardArgs a{};
+    int num_sms = 0;
+    // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2 or a round's fold, 3 a round's walk, 4 phase 3
+    int phase = 0;
+    uint32_t round = 0;
+};
+
+density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void) {
+    g_last_error.clear();
+    DeviceCtx* c = current_ctx();
+    if (!c) return nullptr;
+    density_b200_cheetah_decode_shard* s = new density_b200_cheetah_decode_shard();
+    s->num_sms = c->num_sms;
+    return s;
+}
+void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard* s) {
+    if (!s) return;
+    s->ws.release(); s->tables.release();
+    delete s;
+}
+int density_b200_cheetah_decode_round_budget(void) { return g_chee_dec_rounds; }
+size_t density_b200_cheetah_cmap_words(void) { return 3 * 65536; }
+
+static int cd_phase1_impl(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
+                          uint32_t* d_cmap_out, cudaStream_t st) {
+    if ((!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    s->phase = 0; s->round = 0;
+    CheeShardArgs& a = s->a;
+    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
+    cudaError_t e = cudaSuccess;
+    if (n) {
+        e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
+        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
+        if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    }
+    a.ws = s->ws.p; a.tables = s->tables.p;
+    uint64_t launches = 0;
+    if (n) e = chee_shard_phase1(a, d_cmap_out, st, &launches);
+    else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode shard phase1", e); return DENSITY_B200_ECUDA; }
+    s->phase = 1;
+    return DENSITY_B200_OK;
+}
+static int cd_phase2_impl(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, cudaStream_t st) {
+    if (s->phase != 1) { set_error("cheetah_decode_shard_phase2: phase 1 not done"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e = s->a.n ? chee_shard_phase2(s->a, d_cmap_carry, st, &launches) : cudaSuccess;
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode shard phase2", e); return DENSITY_B200_ECUDA; }
+    s->phase = 2;
+    return DENSITY_B200_OK;
+}
+static int cd_round_walk_impl(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, cudaStream_t st) {
+    if (s->phase != 2) { set_error("cheetah_decode_shard_round_walk: phase 2 or the previous round's fold not done"); return DENSITY_B200_EARG; }
+    if (!d_words4) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->round >= (uint32_t)g_chee_dec_rounds) { set_error("cheetah_decode_shard_round_walk: round budget used up"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e;
+    if (s->a.n) e = chee_shard_round_walk(s->a, s->round, d_pred_out, d_words4, st, &launches);
+    else {   // an empty piece: the identity transfer, no exit context, nothing walked
+        e = cudaMemsetAsync(d_words4, 0, 4 * sizeof(uint32_t), st);
+        if (e == cudaSuccess && d_pred_out) e = cudaMemsetAsync(d_pred_out, 0, 2 * 65536 * sizeof(uint32_t), st);
+    }
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode shard round walk", e); return DENSITY_B200_ECUDA; }
+    s->phase = 3;
+    return DENSITY_B200_OK;
+}
+static int cd_round_fold_impl(density_b200_cheetah_decode_shard* s, const uint32_t* d_pred_carry, const uint32_t* d_all_words, int world, int rank,
+                              cudaStream_t st) {
+    if (s->phase != 3) { set_error("cheetah_decode_shard_round_fold: the round's walk not done"); return DENSITY_B200_EARG; }
+    if (!d_all_words || world < 1 || rank < 0 || rank >= world) { set_error("cheetah_decode_shard_round_fold: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e = s->a.n ? chee_shard_round_fold(s->a, s->round, d_pred_carry, d_all_words, (uint32_t)world, (uint32_t)rank, st, &launches) : cudaSuccess;
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode shard round fold", e); return DENSITY_B200_ECUDA; }
+    s->phase = 2; ++s->round;
+    return DENSITY_B200_OK;
+}
+static int cd_phase3_impl(density_b200_cheetah_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st) {
+    if (s->phase != 2) { set_error("cheetah_decode_shard_phase3: phase 2 or the last round's fold not done"); return DENSITY_B200_EARG; }
+    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e;
+    if (s->a.n) e = chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches);
+    else {
+        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
+    }
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode shard phase3", e); return DENSITY_B200_ECUDA; }
+    s->phase = 4;
+    return DENSITY_B200_OK;
+}
+int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                             int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cd_phase1_impl(s, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cd_phase2_impl(s, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cd_round_walk_impl(s, d_pred_out, d_words4, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cheetah_decode_shard_round_fold(density_b200_cheetah_decode_shard* s, const uint32_t* d_pred_carry, const uint32_t* d_all_words,
+                                                 int world, int rank, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cd_round_fold_impl(s, d_pred_carry, d_all_words, world, rank, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cheetah_decode_shard_phase3(density_b200_cheetah_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    return cd_phase3_impl(s, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard* s, uint32_t* out4) {
+    g_last_error.clear();
+    if (!s || !out4 || s->phase != 4) { set_error("cheetah_decode_shard_status: null pointer / phase 3 not done"); return DENSITY_B200_EARG; }
+    unsigned int raw[8] = {0};
+    if (s->a.n) {
+        cudaError_t e = cudaDeviceSynchronize();
+        if (e == cudaSuccess) e = cudaMemcpy(raw, chee_shard_status_ptr(s->a), sizeof raw, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { set_error("cheetah_decode_shard_status", e); return DENSITY_B200_ECUDA; }
+    } else raw[2] = 1;
+    out4[0] = raw[3]; out4[1] = raw[2] && !raw[5]; out4[2] = raw[6]; out4[3] = s->round;
+    return DENSITY_B200_OK;
+}
+int density_b200_cheetah_cmap_init(uint32_t* d_table, void* stream) {
+    g_last_error.clear();
+    if (!d_table) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    uint64_t l = 0;
+    cudaError_t e = chee_cmap_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
+    g_launches += l;
+    if (e != cudaSuccess) { set_error("cheetah_cmap_init", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+int density_b200_cheetah_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, void* stream) {
+    g_last_error.clear();
+    if (!d_acc || !d_next) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    uint64_t l = 0;
+    cudaError_t e = chee_cmap_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
+    g_launches += l;
+    if (e != cudaSuccess) { set_error("cheetah_cmap_fold", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon encode across the GPUs of one box (SURVEY §8e): one process per GPU, NCCL over NVLink ---------------------
 // NCCL is resolved at run time from the library that is already in the process (torch loads its bundled libnccl.so.2), else the
 // system one: no link-time dependency, one NCCL per process.
@@ -911,6 +1070,8 @@ struct density_b200_sharded {
     DevBuf dws;                     // decode workspace (density_b200_decode_sharded[_stream]), apart from the encoder's
     density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion shard state of density_b200_encode_sharded_cl
     DevBuf cl_aux;                  // its exchange buffers: gathered P and C tables, the carries, the last quads
+    density_b200_cheetah_decode_shard* cdec = nullptr;   // piece state of density_b200_decode_sharded_cheetah
+    DevBuf cd_aux;                  // its exchange buffers: gathered chunk-map and prediction transfers, the carries, the round words
     ChamLayout L{};
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     uint64_t* h_maps = nullptr;     // pinned, world range maps (density_b200_decode_sharded_stream)
@@ -956,8 +1117,9 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release();
+    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release(); h->cd_aux.release();
     for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
+    density_b200_cheetah_decode_shard_destroy(h->cdec);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     if (h->h_maps) cudaFreeHost(h->h_maps);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
@@ -1182,6 +1344,64 @@ int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
     return decode_sharded_piece(h, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
                                 reinterpret_cast<cudaStream_t>(stream_v));
+}
+
+// Sharded Cheetah decode over the handle's communicator: phase 1 -> chunk-map transfers -> fold -> phase 2 -> every round of the budget
+// (walk -> prediction transfers + round words -> fold) -> phase 3 -> seam words -> verdict. Every rank issues the same collectives in the
+// same order whatever its piece holds: an empty piece sends identity transfers and zero words, a refused one keeps exchanging until the
+// verdict. The rounds after the settled one are gated off on the device; their all-gathers still run.
+int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                        uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    if (!h->cdec) { h->cdec = new density_b200_cheetah_decode_shard(); h->cdec->num_sms = h->num_sms; }
+    density_b200_cheetah_decode_shard* s = h->cdec;
+    const size_t W = (size_t)h->world, R = (size_t)h->rank;
+    const size_t wc = density_b200_cheetah_cmap_words(), wp = 2 * 65536;
+    const bool first = R == 0, last = R == W - 1;
+    ShardedAux x;
+    cudaError_t e = sharded_aux(h, st, &x);
+    if (e == cudaSuccess) e = h->cd_aux.ensure(((W + 1) * (wc + wp) + 4 * W + 64) * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint32_t* tab_c = reinterpret_cast<uint32_t*>(h->cd_aux.p);         // [world][wc]
+    uint32_t* carry_c = tab_c + W * wc;
+    uint32_t* tab_p = carry_c + wc;                                       // [world][wp]
+    uint32_t* carry_p = tab_p + W * wp;
+    uint32_t* rwords = carry_p + wp;                                      // [world][4]
+    uint64_t launches = 0;
+    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
+        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
+    };
+    // the last piece's transfers are never read: it sends what its slot holds
+    int rc = cd_phase1_impl(s, d_in, n, d_out, cap, first, last, last ? nullptr : tab_c + R * wc, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
+    if (!first) e = chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
+    g_launches += launches; launches = 0;
+    if (e != cudaSuccess) { set_error("sharded cheetah decode: chunk-map fold", e); return DENSITY_B200_ECUDA; }
+    rc = cd_phase2_impl(s, first ? nullptr : carry_c, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    for (int k = 0; k < g_chee_dec_rounds; ++k) {
+        rc = cd_round_walk_impl(s, last ? nullptr : tab_p + R * wp, rwords + 4 * R, st);
+        if (rc != DENSITY_B200_OK) return rc;
+        if (!gather(tab_p, wp, "ncclAllGather(prediction transfers)") || !gather(rwords, 4, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        if (!first) e = cl_rank_fold(ALG_CHEETAH, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
+        g_launches += launches; launches = 0;
+        if (e != cudaSuccess) { set_error("sharded cheetah decode: prediction fold", e); return DENSITY_B200_ECUDA; }
+        rc = cd_round_fold_impl(s, first ? nullptr : carry_p, rwords, (int)W, (int)R, st);
+        if (rc != DENSITY_B200_OK) return rc;
+    }
+    rc = cd_phase3_impl(s, d_out_size, x.words + 8 * R, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
+    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
@@ -1495,6 +1715,7 @@ int density_b200_cheetah_decode_rounds(uint32_t* out4) {
 
 /* test hook: rounds per stage of the Cheetah / Lion copy-map iteration (1..7; 7 = default) */
 void density_b200_test_set_stage_rounds(int k) { g_chee_stage_rounds = (k >= 1 && k <= 7) ? k : 7; }
+void density_b200_test_set_decode_rounds(int k) { g_chee_dec_rounds = (k >= 1 && k <= 40) ? k : 40; }
 
 /* diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed (~0: none),
    number of such blocks}; 16 rounds x 2 values (synchronises) */

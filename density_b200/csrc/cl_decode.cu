@@ -20,6 +20,11 @@
 //                       contexts. When nothing changed and nothing was unknown the round's values are the reference's (induction
 //                       over the runs). Text settles in 5-8 rounds for any run count (tests/test_cl_model_cpu.py).
 //  4. Tail              (codec.rs:102-123) the last < 136 stream bytes in order by one thread from the folded tables (scalar_codec.cu).
+//  5. Sharded decode    one piece of a longer stream is more runs of the same scheme (DESIGN.md section 5): the blocks a non-final piece
+//                       leaves to the tail are appended to its block list (cd_piece_end), its chunk-map lists compose into one transfer
+//                       (cd_cmap_export) that the later pieces fold into their cd_cmap_fold, and every prediction round exchanges each
+//                       piece's table transfer (cd_pred_export, into cd_pred_fold) and exit context (cd_round_words, into
+//                       cd_shard_round_end); the rounds stop for all pieces at once when none of them walked a run.
 //
 // Lion is NOT decoded here: its 5-deep move-to-front lists make the same iteration advance one run per round (a misplaced
 // operation desynchronises a whole list; measured in tests/cl_model.cpp), so lion_decode stays on the in-order kernel.
@@ -130,13 +135,15 @@ cd_cmap_walk(const DecStatus* __restrict__ st, uint32_t nruns, const uint4* __re
     }
 }
 
-// one thread per bucket: the list carried into every run, and the chunk map after the main loop (for the tail)
+// one thread per bucket: the list carried into every run, and the chunk map after the main loop (for the tail).
+// carry (sharded decode, nullptr otherwise): the chunk map in front of this piece, concrete planes {tags 0, a, b} (cd_cmap_export).
 __global__ void cd_cmap_fold(const DecStatus* __restrict__ st, uint32_t nruns, const uint4* __restrict__ entC_all, uint2* __restrict__ cin,
-                             uint32_t* __restrict__ chunk_a, uint32_t* __restrict__ chunk_b) {
+                             uint32_t* __restrict__ chunk_a, uint32_t* __restrict__ chunk_b, const uint32_t* __restrict__ carry) {
     if (st->error) return;
     const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= 65536) return;
     uint32_t c[2] = {0u, 0u};                                      // chunk map starts as (0, 0) (cheetah.rs:52)
+    if (carry) { c[0] = carry[65536 + h]; c[1] = carry[2 * 65536 + h]; }
     for (uint32_t r0 = 0; r0 < nruns; r0 += 8) {
         uint4 e[8];
 #pragma unroll
@@ -204,7 +211,7 @@ __global__ void __launch_bounds__(RP_WARPS * 32)
 cd_pred_walk(const DecStatus* __restrict__ st, ClStatus* __restrict__ cs, uint32_t nruns, uint32_t round, const uint4* __restrict__ flags,
              const uint16_t* __restrict__ K, uint2* __restrict__ entP_all, const uint32_t* __restrict__ snap_all, const uint32_t* __restrict__ ctx_in,
              uint32_t* __restrict__ ctx_out, const uint32_t* __restrict__ dirty_cur, uint32_t* __restrict__ dirty_next, uint32_t* __restrict__ run_epoch,
-             uint32_t* __restrict__ rbits_all, uint32_t* __restrict__ out) {
+             uint32_t* __restrict__ rbits_all, uint32_t* __restrict__ out, uint32_t run0_snap) {
     if (cs->done) return;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t r = blockIdx.x * RP_WARPS + (threadIdx.x >> 5);
@@ -217,7 +224,7 @@ cd_pred_walk(const DecStatus* __restrict__ st, ClStatus* __restrict__ cs, uint32
     for (uint32_t i = lane; i < 2048; i += 32) rbits[i] = 0;
     __syncwarp();
     const uint32_t epoch = round + 1;
-    const bool has_snap = round > 0 || r == 0;
+    const bool has_snap = round > 0 || (r == 0 && run0_snap);     // run0_snap: run 0 starts at the stream start (its snapshot is the zero table)
     const uint64_t nsteps = st->main_blocks;
     const uint64_t s0 = run_step_begin(r, nruns, nsteps), s1 = run_step_begin(r + 1, nruns, nsteps);
     uint2* __restrict__ entP = entP_all + (size_t)r * 65536;
@@ -297,13 +304,14 @@ cd_pred_walk(const DecStatus* __restrict__ st, ClStatus* __restrict__ cs, uint32
 
 // one thread per context: snapshot of the table in front of every run (in place), and the table after the main loop (for the tail).
 // A run whose snapshot changed at a context it read has to be walked again.
+// carry (sharded decode, nullptr otherwise): the table in front of this piece as of this round, planes {touched, value} (cl_rank_fold P).
 __global__ void cd_pred_fold(const DecStatus* __restrict__ st, ClStatus* __restrict__ cs, uint32_t nruns, uint32_t round, const uint2* __restrict__ entP_all,
                              uint32_t* __restrict__ snap, const uint32_t* __restrict__ run_epoch, const uint32_t* __restrict__ rbits_all,
-                             uint32_t* __restrict__ dirty_next, uint32_t* __restrict__ pred_final) {
+                             uint32_t* __restrict__ dirty_next, uint32_t* __restrict__ pred_final, const uint32_t* __restrict__ carry) {
     if (cs->done) return;
     const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
     if (ctx >= 65536) return;
-    uint32_t c = 0;                                                // prediction table starts as 0 everywhere (cheetah.rs:53)
+    uint32_t c = carry ? carry[65536 + ctx] : 0u;                  // prediction table starts as 0 everywhere (cheetah.rs:53)
     for (uint32_t r0 = 0; r0 < nruns; r0 += 8) {
         uint2 e[8]; uint32_t so[8], ep[8];
 #pragma unroll
@@ -353,6 +361,216 @@ __global__ void cd_finish(const DecStatus* __restrict__ st, ClStatus* __restrict
     if (!ok && !st->error) cs->gave_up = 1;
     *d_fallback = ok ? 0u : 1u;
     if (!ok && d_out_size) *d_out_size = 0;
+}
+
+// ---- 5. sharded decode: one piece of a longer stream --------------------------------------------------------------------------------
+// A piece is more runs of the same scheme: the chunk-map lists and the prediction table come in from the pieces before it as transfers,
+// the context of its first quad from their exit contexts (DESIGN.md section 5).
+constexpr uint32_t PL = 65536;
+constexpr uint32_t CM_IDENTITY = 1u | (2u << 3);          // chunk-map transfer tags: slot j = carried-in slot j
+
+struct PieceStatus { unsigned int refuse, first_inc, last_inc, tail_blocks, pad[4]; };
+
+// The end of the piece, right after the boundary walk. A non-final piece is followed by more stream bytes, so the reference decodes all of
+// its blocks in the main loop (codec.rs:88-100); the blocks the boundary walk left to the tail (those starting in the last 136 bytes) are
+// appended to the block list. Their control flow does not depend on the tables. The final piece keeps its in-order tail; its control flow
+// is walked here for the seam words. Refused (pst->refuse): a piece > 0 that is not quiet (copy mode, two consecutive incompressible
+// blocks); a non-final piece that meets copy mode at its end, ends with a copy penalty pending or inside a copy run, or whose blocks do
+// not end exactly at its last byte.
+__global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, int first, int last, DecStatus* __restrict__ st,
+                             uint64_t* __restrict__ blk_off, uint64_t maxblocks, PieceStatus* __restrict__ pst) {
+    if (threadIdx.x || blockIdx.x) return;
+    auto sig_at = [&](uint64_t o) { uint64_t s = 0; for (int i = 0; i < 8; ++i) s |= (uint64_t)in[o + i] << (8 * i); return s; };
+    if (st->error) { pst->refuse = 1; pst->first_inc = 0; pst->last_inc = 0; pst->tail_blocks = 0; return; }
+    uint32_t refuse = (!first && st->seq) ? 1u : 0u;             // dec_seq_walk ran: two consecutive incompressible blocks in the main loop
+    Protection ps; ps.init();
+    ps.counter = st->main_blocks; ps.previous_incompressible = st->last_main_inc;
+    if (st->seq) { ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev; }
+    uint64_t idx = st->tail_off, b = st->main_blocks;
+    uint32_t tail_first = 0, tail_blocks = 0;
+    if (!last) {
+        bool bad = false, ends_copy = b > 0 && (blk_off[b - 1] & BLK_COPY);
+        while (idx < n) {
+            if (ps.revert_to_copy()) { bad = true; break; }       // copy mode at the end of a non-final piece
+            if (n - idx < 8) { bad = true; break; }
+            const uint32_t consumed = cld::cheetah_block_bytes(sig_at(idx));
+            if (consumed > n - idx) { bad = true; break; }         // the block runs past the piece
+            if (b < maxblocks) blk_off[b] = idx; else st->error = 2;
+            ++b; ++tail_blocks; idx += consumed; ends_copy = false;
+            ps.update(consumed >= 128);                            // codec.rs:94-98
+        }
+        if (bad || ends_copy || ps.copy_penalty) refuse = 1;
+        if (!bad) {
+            st->main_blocks = b; st->tail_off = idx; st->last_main_inc = ps.previous_incompressible;
+            if (st->seq) { st->ps_penalty = ps.copy_penalty; st->ps_start = ps.copy_penalty_start; st->ps_prev = ps.previous_incompressible; }
+        }
+        if (b * 128 > cap) st->error = 2;
+    } else {
+        // the tail loop's control flow (codec.rs:102-123, scalar_codec.cu decode_loops): copy mode or a new incompressible pair there
+        // is refused in a piece > 0; malformed input is left to the tail kernel, which reports it
+        uint32_t copied = 0, pair = 0;
+        while (n - idx > 0) {
+            ++tail_blocks;
+            if (ps.revert_to_copy()) {
+                copied = 1;
+                if (n - idx > 128) { idx += 128; ps.decay(); continue; }
+                break;
+            }
+            const uint64_t mark = idx;
+            if (n - idx < 8) break;
+            uint64_t sig = sig_at(idx);
+            idx += 8;
+            bool end = false;
+            for (int u = 0; u < 32 && !end; ++u) {
+                const uint32_t fl = (uint32_t)(sig & 3u); sig >>= 2;
+                const uint64_t rem = n - idx;
+                if (fl == 0 && rem < 4) end = true;                 // decode_partial_unit: the stream ends inside this quad
+                else if (fl == 0) idx += 4;
+                else if (fl != 3) { if (rem < 2) end = true; else idx += 2; }
+            }
+            if (end) break;
+            const uint32_t inc = idx - mark >= 128 ? 1u : 0u;
+            if (tail_blocks == 1) tail_first = inc;
+            pair |= inc & ps.previous_incompressible;
+            ps.update(inc);
+        }
+        if (!first && (copied || pair)) refuse = 1;
+    }
+    const uint64_t b0 = blk_off[0];
+    pst->first_inc = st->main_blocks ? ((!(b0 & BLK_COPY) && cld::cheetah_block_bytes(sig_at(b0)) >= 128) ? 1u : 0u) : tail_first;
+    pst->last_inc = ps.previous_incompressible;
+    pst->refuse = refuse;
+    pst->tail_blocks = tail_blocks;
+}
+
+// chunk-map transfer of a piece, planes {tags, a, b} per bucket: slot s of the list the piece leaves is the literal v[s] (tag 0) or
+// slot t - 1 of the list carried into the piece (tag t, 3 bits per slot as in List<2>). "x, then y" applies y's tags to x's slots.
+__device__ __forceinline__ void cm_compose(uint32_t (&v)[2], uint32_t& tag, const uint32_t (&yv)[2], uint32_t ytag) {
+    uint32_t nv[2], nt = 0;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        const uint32_t t = (ytag >> (3 * s)) & 7u;
+        if (t == TAG_LIT || t > 2) nv[s] = yv[s];
+        else { nv[s] = v[t - 1]; nt |= ((tag >> (3 * (t - 1))) & 7u) << (3 * s); }
+    }
+    v[0] = nv[0]; v[1] = nv[1]; tag = nt;
+}
+// the composition over the piece's runs (nruns 0 or st == nullptr: the identity, an empty piece)
+__global__ void cd_cmap_export(const DecStatus* __restrict__ st, uint32_t nruns, const uint4* __restrict__ entC_all, uint32_t* __restrict__ out) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= PL) return;
+    uint32_t v[2] = {0u, 0u}, tag = CM_IDENTITY;
+    if (st && !st->error) {
+        for (uint32_t r = 0; r < nruns; ++r) {
+            const uint4 e = entC_all[(size_t)r * PL + h];
+            if (meta_epoch(e.z) != 1u) continue;
+            const uint32_t yv[2] = {e.x, e.y};
+            cm_compose(v, tag, yv, e.z & 0x3Fu);
+        }
+    }
+    out[h] = tag; out[PL + h] = v[0]; out[2 * PL + h] = v[1];
+}
+// the stream-start chunk map (0, 0) in every bucket (cheetah.rs:52); acc <- acc, then next; the carry-in of piece `rank`
+__global__ void cd_cmap_init_k(uint32_t* __restrict__ t) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h < PL) { t[h] = 0; t[PL + h] = 0; t[2 * PL + h] = 0; }
+}
+__global__ void cd_cmap_fold_k(uint32_t* __restrict__ acc, const uint32_t* __restrict__ next) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= PL) return;
+    uint32_t v[2] = {acc[PL + h], acc[2 * PL + h]}, tag = acc[h];
+    const uint32_t yv[2] = {next[PL + h], next[2 * PL + h]};
+    cm_compose(v, tag, yv, next[h]);
+    acc[h] = tag; acc[PL + h] = v[0]; acc[2 * PL + h] = v[1];
+}
+__global__ void cd_cmap_rank_fold_k(const uint32_t* __restrict__ tables, uint32_t rank, uint32_t* __restrict__ carry) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= PL) return;
+    uint32_t v[2] = {0u, 0u}, tag = 0;
+    for (uint32_t r = 0; r < rank; ++r) {
+        const uint32_t* t = tables + (size_t)r * 3 * PL;
+        const uint32_t yv[2] = {t[PL + h], t[2 * PL + h]};
+        cm_compose(v, tag, yv, t[h]);
+    }
+    carry[h] = tag; carry[PL + h] = v[0]; carry[2 * PL + h] = v[1];
+}
+
+// prediction transfer of this round, planes {touched, last value} per context: the entries cd_pred_fold counts (the epoch of their run's
+// last walk), in run order. The format of the Cheetah encoder's P table, so cl_rank_fold / cl_table_fold compose it.
+__global__ void cd_pred_export(const ClStatus* __restrict__ cs, uint32_t nruns, const uint2* __restrict__ entP_all, const uint32_t* __restrict__ run_epoch,
+                               uint32_t* __restrict__ out) {
+    if (cs->done) return;
+    const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ctx >= PL) return;
+    uint32_t touched = 0, v = 0;
+    for (uint32_t r = 0; r < nruns; ++r) {
+        const uint32_t ep = run_epoch[r];
+        const uint2 e = entP_all[(size_t)r * PL + ctx];
+        if (ep != 0 && meta_epoch(e.y) == ep) { touched = 1; v = e.x; }
+    }
+    out[ctx] = touched; out[PL + ctx] = v;
+}
+// the piece's 4 round words after its walk: {has an exit context, exit context (the last run's with encoded quads; may be H_UNKNOWN),
+// runs walked in this round, a run met an unknown}. A settled or failed piece walks nothing.
+__global__ void cd_round_words(const DecStatus* __restrict__ st, const ClStatus* __restrict__ cs, uint32_t nruns, const uint32_t* __restrict__ ctx_out,
+                               const uint32_t* __restrict__ dirty_cur, const uint32_t* __restrict__ dirty_next, uint32_t* __restrict__ words) {
+    __shared__ int s_last;
+    __shared__ uint32_t s_walked, s_unknown;
+    if (threadIdx.x == 0) { s_last = -1; s_walked = 0; s_unknown = 0; }
+    __syncthreads();
+    const bool live = !st->error;
+    const bool walking = live && !cs->done;
+    int last = -1; uint32_t walked = 0, unknown = 0;
+    for (uint32_t r = threadIdx.x; live && r < nruns; r += blockDim.x) {
+        if (ctx_out[r] != CTX_PASS) last = (int)r;
+        if (walking) { walked += dirty_cur[r]; unknown |= dirty_next[r]; }
+    }
+    if (last >= 0) atomicMax(&s_last, last);
+    if (walked) atomicAdd(&s_walked, walked);
+    if (unknown) atomicOr(&s_unknown, 1u);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        words[0] = s_last >= 0 ? 1u : 0u; words[1] = s_last >= 0 ? ctx_out[s_last] : 0u;
+        words[2] = s_walked; words[3] = s_unknown;
+    }
+}
+// context sweep of a piece: run 0's entry context is the exit context of the nearest earlier piece that has one (0 if none,
+// cheetah.rs:54). Round 0: only the run at the stream start had a snapshot. The rounds have settled when no piece walked a run in this
+// round, which every piece reads off the same gathered words, so all pieces stop together.
+__global__ void cd_shard_round_end(ClStatus* __restrict__ cs, uint32_t nruns, uint32_t round, uint32_t first, uint32_t rank, uint32_t world,
+                                   const uint32_t* __restrict__ all_words, uint32_t* __restrict__ ctx_in, const uint32_t* __restrict__ ctx_out,
+                                   uint32_t* __restrict__ dirty_cur, uint32_t* __restrict__ dirty_next) {
+    if (threadIdx.x || blockIdx.x || cs->done) return;
+    uint32_t c = 0, walked = 0, ndirty = 0;
+    for (uint32_t q = 0; q < world; ++q) {
+        const uint32_t* w = all_words + 4 * q;
+        if (q < rank && w[0]) c = w[1];
+        walked += w[2];
+    }
+    for (uint32_t r = 0; r < nruns; ++r) {
+        uint32_t d = dirty_next[r];
+        if (round == 0 && (r > 0 || !first)) d = 1;
+        if (ctx_in[r] != c) { d = 1; ctx_in[r] = c; }
+        dirty_cur[r] = d; dirty_next[r] = 0;
+        ndirty += d;
+        const uint32_t o = ctx_out[r];
+        if (o != CTX_PASS) c = o;
+    }
+    cs->final_ctx = c;
+    cs->rounds = round + 1;
+    cs->pad0 += ndirty;
+    if (walked == 0) cs->done = 1;
+}
+// the piece's 8 seam words in the layout of the Chameleon decoder's (after the tail): {first block incompressible, previous_incompressible
+// at the end, refused, has blocks, decoded size lo, hi, 0, 0}
+__global__ void cd_seam_words(const PieceStatus* __restrict__ pst, const uint32_t* __restrict__ fallback, const Status* __restrict__ tail_status,
+                              int is_last, const uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
+    if (threadIdx.x || blockIdx.x) return;
+    const uint64_t sz = *d_out_size;
+    uint32_t bad = (pst->refuse || *fallback || tail_status->error) ? 1u : 0u;
+    if (!is_last && (sz % 128)) bad = 1;
+    words[0] = pst->first_inc; words[1] = pst->last_inc; words[2] = bad; words[3] = 1;
+    words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
 }
 
 }  // namespace cheedec
@@ -433,13 +651,13 @@ cudaError_t chee_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
     const uint32_t run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
     cd_unpack<<<wide, 256, 0, stream>>>(d_in, blk_off, st, flags, K, out32);
     cd_cmap_walk<<<run_ctas, RP_WARPS * 32, 0, stream>>>(st, nruns, flags, K, entC, out32, usym);
-    cd_cmap_fold<<<65536 / 128, 128, 0, stream>>>(st, nruns, entC, cin, chunk_a, chunk_b);
+    cd_cmap_fold<<<65536 / 128, 128, 0, stream>>>(st, nruns, entC, cin, chunk_a, chunk_b, nullptr);
     cd_cmap_resolve<<<wide, 256, 0, stream>>>(st, nruns, usym, K, cin, out32);
     cd_ctx_init<<<(nruns + 127) / 128, 128, 0, stream>>>(st, nruns, flags, K, ctx_in, dirty_cur, dirty_next, run_epoch, cs);
     *launches += 5;
     for (int round = 0; round < MAX_ROUNDS; ++round) {
-        cd_pred_walk<<<run_ctas, RP_WARPS * 32, 0, stream>>>(st, cs, nruns, (uint32_t)round, flags, K, entP, snap, ctx_in, ctx_out, dirty_cur, dirty_next, run_epoch, rbits, out32);
-        cd_pred_fold<<<65536 / 128, 128, 0, stream>>>(st, cs, nruns, (uint32_t)round, entP, snap, run_epoch, rbits, dirty_next, pred_final);
+        cd_pred_walk<<<run_ctas, RP_WARPS * 32, 0, stream>>>(st, cs, nruns, (uint32_t)round, flags, K, entP, snap, ctx_in, ctx_out, dirty_cur, dirty_next, run_epoch, rbits, out32, 1u);
+        cd_pred_fold<<<65536 / 128, 128, 0, stream>>>(st, cs, nruns, (uint32_t)round, entP, snap, run_epoch, rbits, dirty_next, pred_final, nullptr);
         cd_round_end<<<1, 32, 0, stream>>>(cs, nruns, (uint32_t)round, ctx_in, ctx_out, dirty_cur, dirty_next);
         *launches += 3;
     }
@@ -454,5 +672,141 @@ const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int n
     if (cl_status) *cl_status = ws + L.cs;
     return ws + L.B.status;
 }
+
+// ---- sharded decode: one piece, in phases around the exchanges (include/density_b200.h, DESIGN.md section 5) --------------------------
+// Workspace: the layout of the single-device decoder, then the fallback word and the PieceStatus (256 B), then the tail's tables
+// (the scalar_codec.cu layout: Status (256 B) + chunk_a + chunk_b + pred).
+struct CheeShardPtrs {
+    uint32_t nruns, run_ctas;
+    DecStatus* st; ClStatus* cs; uint64_t* blk_off; uint4* flags; uint16_t* K; uint2* usym;
+    uint32_t *ctx_in, *ctx_out, *dirty_cur, *dirty_next, *run_epoch, *rbits, *snap, *fallback, *chunk_a, *chunk_b, *pred_final;
+    uint2* cin; uint4* entC; uint2* entP; PieceStatus* pst; uint8_t* tail_ws;
+};
+static size_t chee_shard_layout(const CheeShardArgs& a, CheeDecLayout* L) {
+    const size_t off = (cd_layout(a.n, a.cap, cd_pick_runs(a.n, a.num_sms), L) + 255) & ~(size_t)255;
+    return off + 256 + scalar_workspace_bytes(ALG_CHEETAH);
+}
+static CheeShardPtrs chee_shard_ptrs(const CheeShardArgs& a) {
+    CheeShardPtrs p;
+    CheeDecLayout L;
+    chee_shard_layout(a, &L);
+    uint8_t* ws = a.ws;
+    const size_t off = (L.total + 255) & ~(size_t)255;
+    p.nruns = cd_pick_runs(a.n, a.num_sms);
+    p.run_ctas = (p.nruns + RP_WARPS - 1) / RP_WARPS;
+    p.st = reinterpret_cast<DecStatus*>(ws + L.B.status);
+    p.cs = reinterpret_cast<ClStatus*>(ws + L.cs);
+    p.blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
+    p.flags = reinterpret_cast<uint4*>(ws + L.flags);
+    p.K = reinterpret_cast<uint16_t*>(ws + L.K);
+    p.usym = reinterpret_cast<uint2*>(ws + L.usym);
+    p.ctx_in = reinterpret_cast<uint32_t*>(ws + L.ctx_in);
+    p.ctx_out = reinterpret_cast<uint32_t*>(ws + L.ctx_out);
+    p.dirty_cur = reinterpret_cast<uint32_t*>(ws + L.dirty);
+    p.dirty_next = p.dirty_cur + p.nruns;
+    p.run_epoch = reinterpret_cast<uint32_t*>(ws + L.run_epoch);
+    p.rbits = reinterpret_cast<uint32_t*>(ws + L.rbits);
+    p.cin = reinterpret_cast<uint2*>(ws + L.cin);
+    p.snap = reinterpret_cast<uint32_t*>(ws + L.snap0);
+    p.fallback = reinterpret_cast<uint32_t*>(ws + off);
+    p.pst = reinterpret_cast<PieceStatus*>(ws + off + 128);
+    p.tail_ws = ws + off + 256;
+    p.chunk_a = reinterpret_cast<uint32_t*>(p.tail_ws + 256);
+    p.chunk_b = p.chunk_a + PL;
+    p.pred_final = p.chunk_a + 2 * PL;
+    p.entC = reinterpret_cast<uint4*>(a.tables);
+    p.entP = reinterpret_cast<uint2*>(a.tables + (size_t)p.nruns * PL * sizeof(uint4));
+    return p;
+}
+
+size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
+    CheeShardArgs a{}; a.n = n; a.cap = cap; a.num_sms = num_sms;
+    CheeDecLayout L;
+    return chee_shard_layout(a, &L);
+}
+
+// Phase 1: boundaries (piece 0 may use copy mode: dec_seq_walk from the fresh automaton), the end of the piece, unpack (literals and
+// copy-mode blocks go straight to d_out), the symbolic chunk-map walk and the piece's chunk-map transfer (d_cmap_out, may be null).
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches) {
+    const CheeShardPtrs p = chee_shard_ptrs(a);
+    CheeDecLayout L; chee_shard_layout(a, &L);
+    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, L.B, stream, launches);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.tables, 0, chee_decode_tables_bytes(a.n, a.num_sms), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.snap, 0, (size_t)p.nruns * PL * sizeof(uint32_t), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
+    if (e != cudaSuccess) return e;
+    const int wide = a.num_sms * 8;
+    uint32_t* out32 = reinterpret_cast<uint32_t*>(a.d_out);
+    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, p.st, p.blk_off, L.B.maxblocks, p.pst);
+    cd_unpack<<<wide, 256, 0, stream>>>(a.d_in, p.blk_off, p.st, p.flags, p.K, out32);
+    cd_cmap_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.entC, out32, p.usym);
+    *launches += 3;
+    if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
+    return cudaGetLastError();
+}
+
+// Phase 2: the chunk map carried in (d_cmap_carry: concrete, the left fold of the earlier pieces' transfers over cd_cmap_init_k's state;
+// nullptr = the stream start), the reads of carried-in slots, the context init.
+cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
+    const CheeShardPtrs p = chee_shard_ptrs(a);
+    uint32_t* out32 = reinterpret_cast<uint32_t*>(a.d_out);
+    cd_cmap_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.nruns, p.entC, p.cin, p.chunk_a, p.chunk_b, d_cmap_carry);
+    cd_cmap_resolve<<<a.num_sms * 8, 256, 0, stream>>>(p.st, p.nruns, p.usym, p.K, p.cin, out32);
+    cd_ctx_init<<<(p.nruns + 127) / 128, 128, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.ctx_in, p.dirty_cur, p.dirty_next, p.run_epoch, p.cs);
+    *launches += 3;
+    return cudaGetLastError();
+}
+
+// A prediction round, first half: walk the dirty runs, export this round's transfer (d_pred_out, may be null) and the 4 round words.
+cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
+    const CheeShardPtrs p = chee_shard_ptrs(a);
+    cd_pred_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.cs, p.nruns, round, p.flags, p.K, p.entP, p.snap, p.ctx_in, p.ctx_out, p.dirty_cur,
+                                                           p.dirty_next, p.run_epoch, p.rbits, reinterpret_cast<uint32_t*>(a.d_out), a.first ? 1u : 0u);
+    if (d_pred_out) { cd_pred_export<<<PL / 128, 128, 0, stream>>>(p.cs, p.nruns, p.entP, p.run_epoch, d_pred_out); ++*launches; }
+    cd_round_words<<<1, 256, 0, stream>>>(p.st, p.cs, p.nruns, p.ctx_out, p.dirty_cur, p.dirty_next, d_words);
+    *launches += 2;
+    return cudaGetLastError();
+}
+
+// Second half: the snapshots from the carried-in table of this round (d_pred_carry, nullptr = the stream start's zeros) and the
+// context sweep from the gathered round words of all `world` pieces.
+cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
+                                  uint32_t rank, cudaStream_t stream, uint64_t* launches) {
+    const CheeShardPtrs p = chee_shard_ptrs(a);
+    cd_pred_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.cs, p.nruns, round, p.entP, p.snap, p.run_epoch, p.rbits, p.dirty_next, p.pred_final, d_pred_carry);
+    cd_shard_round_end<<<1, 32, 0, stream>>>(p.cs, p.nruns, round, a.first ? 1u : 0u, rank, world, d_all_words, p.ctx_in, p.ctx_out, p.dirty_cur, p.dirty_next);
+    *launches += 2;
+    return cudaGetLastError();
+}
+
+// Phase 3: the verdict of the rounds, the final piece's tail from the folded tables (the tail of a non-final piece is empty), the size
+// and the seam words.
+cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
+    const CheeShardPtrs p = chee_shard_ptrs(a);
+    cd_finish<<<1, 1, 0, stream>>>(p.st, p.cs, p.fallback, d_out_size);
+    ++*launches;
+    cudaError_t e = scalar_decode_tail(ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
+    if (e != cudaSuccess) return e;
+    cd_seam_words<<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_out_size, d_seam8);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// the diagnostic words of the piece's iteration (ClStatus, 8 x u32)
+const void* chee_shard_status_ptr(const CheeShardArgs& a) { return chee_shard_ptrs(a).cs; }
+
+cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches) {
+    cd_cmap_export<<<PL / 256, 256, 0, stream>>>(nullptr, 0, nullptr, d_table); ++*launches; return cudaGetLastError();
+}
+cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches) {
+    cd_cmap_init_k<<<PL / 256, 256, 0, stream>>>(d_table); ++*launches; return cudaGetLastError();
+}
+cudaError_t chee_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches) {
+    cd_cmap_fold_k<<<PL / 256, 256, 0, stream>>>(d_acc, d_next); ++*launches; return cudaGetLastError();
+}
+cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches) {
+    cd_cmap_rank_fold_k<<<PL / 128, 128, 0, stream>>>(d_tables, rank, d_carry); ++*launches; return cudaGetLastError();
+}
+uint32_t chee_shard_max_rounds() { return MAX_ROUNDS; }
 
 }  // namespace dns

@@ -94,6 +94,23 @@ size_t chee_decode_tables_bytes(size_t nbytes, int num_sms);
 cudaError_t chee_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
                                  int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches);
 const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** cl_status);
+// sharded Cheetah decode: one piece of a longer stream (first: it holds the stream start; last: no stream byte follows it). ws holds
+// chee_shard_workspace_bytes, tables chee_decode_tables_bytes of the piece. Phase 1, phase 2, then any number of rounds (walk, exchange,
+// fold), then phase 3; every call of one piece gets the same arguments. Chunk-map tables: 3 planes {tags, a, b} of 65536 u32.
+struct CheeShardArgs { const uint8_t* d_in; size_t n; uint8_t* d_out; size_t cap; bool first, last; uint8_t* ws; uint8_t* tables; int num_sms; };
+size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
+uint32_t chee_shard_max_rounds();
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
+                                  uint32_t rank, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches);
+const void* chee_shard_status_ptr(const CheeShardArgs& a);
+cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
 
 // scalar_codec.cu (Cheetah / Lion, in-order)
 size_t scalar_workspace_bytes(int alg);

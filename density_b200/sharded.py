@@ -19,6 +19,10 @@ transfer says what the shard does to the state carried into it; the carry-in of 
 transfers of ranks < r (density_b200_cl_table_init / _fold, on the device). Only rank 0 may use copy mode; the seam verdict refuses
 what would need it elsewhere.
 
+A sharded Cheetah stream decodes the same way in pieces (ShardedDecoder.decode(..., alg="cheetah"), or the piece phases
+density_b200_cheetah_decode_shard_* with fold_cheetah_cmap and fold_cl_tables for the exchanges): the chunk-map transfers are
+exchanged once, then every prediction round exchanges each piece's prediction transfer and 4 round words, for a fixed budget of rounds.
+
 A stream whose cuts are not known (one chameleon_encode call, the reference library, a file) is cut at byte ranges instead
 (`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
 (density_b200_decode_locate), and after an all_gather of the maps `locate_piece` gives every rank the exact offset where its
@@ -181,6 +185,22 @@ def fold_cl_tables(alg, kind, gathered, rank):
             rc = lib.density_b200_cl_table_fold(alg, kind, carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
     if rc:
         raise _lib.DensityB200Error(f"cl_table_init / fold rc={rc}: {_lib.last_error()}")
+    return carry
+
+
+def fold_cheetah_cmap(gathered, rank):
+    """carry-in of piece `rank` for the sharded Cheetah decode: the stream-start chunk map (density_b200_cheetah_cmap_init) folded with
+    the chunk-map transfers of pieces < rank in order (density_b200_cheetah_cmap_fold). gathered: CUDA int32 [world, 3 * 65536].
+    Enqueued on torch's current stream."""
+    lib = _lib.load()
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    carry = torch.empty(gathered.shape[1], dtype=torch.int32, device=gathered.device)
+    rc = lib.density_b200_cheetah_cmap_init(carry.data_ptr(), stream)
+    for r in range(rank):
+        if rc == 0:
+            rc = lib.density_b200_cheetah_cmap_fold(carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
+    if rc:
+        raise _lib.DensityB200Error(f"cheetah_cmap_init / fold rc={rc}: {_lib.last_error()}")
     return carry
 
 
@@ -417,15 +437,20 @@ class ShardedDecoder(_ShardedHandle):
     """The C++ multi-GPU decode (`density_b200_decode_sharded`): the inverse of ShardedEncoder.encode without a gather. Each rank
     decodes its piece back into the shard it was encoded from; the exchanges run over the library's NCCL communicator."""
 
-    def decode(self, d_in, d_out, d_size, d_flags):
+    def decode(self, d_in, d_out, d_size, d_flags, alg="chameleon"):
         """Enqueue on torch's current stream; nothing blocks. d_in: this rank's piece (2-byte aligned); d_out: capacity d_out.numel()
         (4-byte aligned); d_size int64[1]: the decoded size; d_flags int32[1]: != 0 -> the pieces are void and the caller decodes the
-        gathered stream on one device; self.d_total int64[1]: the original length."""
+        gathered stream on one device; self.d_total int64[1]: the original length. alg "cheetah" (or its id): the pieces of a sharded
+        Cheetah stream (density_b200_decode_sharded_cheetah); Lion has no parallel decoder to shard."""
+        alg = _alg_id(alg)
+        if alg not in (0, 1):
+            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self._lib.density_b200_decode_sharded(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(),
-                                                   d_flags.data_ptr(), self.d_total.data_ptr(), stream)
+        fn = self._lib.density_b200_decode_sharded if alg == 0 else self._lib.density_b200_decode_sharded_cheetah
+        rc = fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
+                self.d_total.data_ptr(), stream)
         if rc:
-            raise _lib.DensityB200Error(f"decode_sharded rc={rc}: {_lib.last_error()}")
+            raise _lib.DensityB200Error(f"decode_sharded{'' if alg == 0 else '_cheetah'} rc={rc}: {_lib.last_error()}")
 
     def decode_stream(self, d_in, n_range, d_out, d_size, d_flags):
         """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range

@@ -236,6 +236,69 @@ DENSITY_B200_API int density_b200_decode_sharded(density_b200_sharded*, const ui
                                 uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
+ * Sharded Cheetah decode (DESIGN.md section 5). Piece r is what rank r of a sharded Cheetah encode produced (density_b200_cl_shard_phase3
+ * or density_b200_encode_sharded_cl), or equally the slice of a single-call cheetah_encode stream at the prefix sums of those sizes.
+ * Decoding every piece gives back its shard byte for byte whenever the verdict is 0, so the concatenation equals cheetah_decode of the
+ * whole stream. The verdict is non-zero (the pieces are void and the caller decodes the gathered stream on one device) when:
+ *   - the first piece, not being the last, ends inside a copy run or with a copy penalty pending;
+ *   - a later piece is not quiet (a copy-mode block, two consecutive incompressible blocks) or a seam joins two incompressible blocks;
+ *   - a non-final piece's blocks do not end exactly at its last byte, or meet copy mode there;
+ *   - the prediction rounds did not settle within the round budget (density_b200_cheetah_decode_round_budget);
+ *   - a piece is malformed, its output exceeds `cap`, or a non-final piece does not decode to whole 128-byte blocks.
+ * Only the first piece may use copy mode: it holds the stream start, where every Cheetah stream has copy-mode blocks. Lion streams and
+ * streams without known cuts are not decoded this way. d_in must be 2-byte and d_out 4-byte aligned; nothing is written past `cap`.
+ *
+ * Phase API of one piece (any transport; W pieces may run on one GPU): phase 1 -> exchange of the chunk-map transfers -> phase 2 -> rounds
+ * (round_walk -> exchange of the prediction transfers and the round words -> round_fold), as many as the round budget -> phase 3 -> seam
+ * words -> verdict (the rule of density_b200_decode_shard_phase2's words). Every piece runs the same number of rounds.
+ * Tables are stacks of u32 planes of 65536 entries:
+ *   chunk map (density_b200_cheetah_cmap_words() u32)  {tags, a, b} per bucket: slot s of the list the piece leaves is the literal in
+ *                                                      plane 1 + s (tag bits 3s..3s+2 = 0) or slot t - 1 of the list carried in (tag t)
+ *   predictions (density_b200_cl_table_words(DENSITY_B200_CHEETAH, DENSITY_B200_CL_TABLE_P) u32)  {touched, last value} per context: the
+ *                                                      format of the Cheetah encoder's P table; fold it with density_b200_cl_table_init /
+ *                                                      _fold(DENSITY_B200_CHEETAH, DENSITY_B200_CL_TABLE_P)
+ *   round words (4 u32 per piece)                      {has an exit context, exit context, runs walked this round, an unknown was met}
+ * The carry-in of piece r is the stream-start state (density_b200_cheetah_cmap_init, density_b200_cl_table_init) folded with the tables
+ * of pieces 0 .. r - 1 in order; the round words are gathered from all pieces in rank order.
+ */
+typedef struct density_b200_cheetah_decode_shard density_b200_cheetah_decode_shard; /* opaque */
+DENSITY_B200_API density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void);
+DENSITY_B200_API void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard*);
+/* rounds every piece runs (40; density_b200_test_set_decode_rounds lowers it) */
+DENSITY_B200_API int density_b200_cheetah_decode_round_budget(void);
+/* u32 words of a chunk-map table (3 x 65536) */
+DENSITY_B200_API size_t density_b200_cheetah_cmap_words(void);
+/* phase 1: boundaries (the first piece from the fresh protection automaton, copy mode allowed), the end of the piece, unpack (literals and
+   copy-mode blocks go to d_out at once), the symbolic chunk-map walk, and the piece's chunk-map transfer to d_cmap_out (may be NULL: no
+   export). is_first: the piece holds the stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n, uint8_t* d_out,
+                                             size_t cap, int is_first, int is_last, uint32_t* d_cmap_out, void* stream);
+/* phase 2: d_cmap_carry = the chunk map before this piece (NULL = stream start). Resolves the chunk-map reads, initialises the contexts. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard*, const uint32_t* d_cmap_carry, void* stream);
+/* one round, first half: walks the runs that need it, exports this round's prediction transfer (d_pred_out, may be NULL) and the piece's 4
+   round words (d_words4). DENSITY_B200_EARG once the round budget is used up. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_shard*, uint32_t* d_pred_out, uint32_t* d_words4, void* stream);
+/* second half: d_pred_carry = this round's prediction table before the piece (NULL = stream start), d_all_words = the round words of all
+   `world` pieces in rank order, this piece being `rank`. Once no piece walked a run in a round, the rounds have settled and the kernels of
+   the later rounds return at once. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_round_fold(density_b200_cheetah_decode_shard*, const uint32_t* d_pred_carry,
+                                                 const uint32_t* d_all_words, int world, int rank, void* stream);
+/* phase 3: the tail of the final piece, the decoded size to *d_out_size (0 when the piece is refused) and the 8 seam words to d_seam8:
+   {first block incompressible, previous_incompressible at the end, refused, has blocks, size lo, size hi, 0, 0}. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_phase3(density_b200_cheetah_decode_shard*, uint64_t* d_out_size, uint32_t* d_seam8, void* stream);
+/* Diagnostic, after phase 3 (synchronises the device): out4 = {rounds until settled, settled, run walks after round 0, rounds run}. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard*, uint32_t* out4);
+/* the stream-start chunk map ((0, 0) in every bucket), and d_acc <- d_acc, then d_next */
+DENSITY_B200_API int density_b200_cheetah_cmap_init(uint32_t* d_table, void* stream);
+DENSITY_B200_API int density_b200_cheetah_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, void* stream);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments and semantics of density_b200_decode_sharded: phase 1 ->
+   ncclAllGather(chunk-map transfers, 0.75 MiB per rank) -> one fold kernel -> phase 2 -> per round ncclAllGather(prediction transfers,
+   0.5 MiB per rank) + ncclAllGather(round words) -> one fold kernel -> round fold, for every round of the budget -> phase 3 ->
+   ncclAllGather(seam words) -> verdict. Never blocks, has no gather, uses its own workspace in the handle. */
+DENSITY_B200_API int density_b200_decode_sharded_cheetah(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
  * Sharded decode of a stream whose cuts are not known: a stream written by one chameleon_encode call, by the reference library,
  * read from a file, or a gathered sharded stream without its piece sizes. The stream is cut at byte ranges; each rank finds
  * where its piece starts from the stream itself.
@@ -309,6 +372,9 @@ DENSITY_B200_API void density_b200_shutdown(void);
 /* Test hook: cut every stage of the Cheetah / Lion copy-map iteration to k rounds (1..7, default 7) so that the host-resumed
    iteration of path 4 can be exercised on ordinary inputs. */
 DENSITY_B200_API void density_b200_test_set_stage_rounds(int k);
+/* Test hook: cut the round budget of the sharded Cheetah decode to k rounds (1..40, default 40) so that its "did not settle" refusal
+   can be exercised. density_b200_decode_device does not read it. */
+DENSITY_B200_API void density_b200_test_set_decode_rounds(int k);
 /* Diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed
    (~0: none), number of such blocks}: 16 rounds x 2 values. Synchronises the device. */
 DENSITY_B200_API int density_b200_prot_debug(uint64_t* out32);

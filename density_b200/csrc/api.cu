@@ -1346,23 +1346,24 @@ int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
                                 reinterpret_cast<cudaStream_t>(stream_v));
 }
 
-// Sharded Cheetah decode over the handle's communicator: phase 1 -> chunk-map transfers -> fold -> phase 2 -> every round of the budget
-// (walk -> prediction transfers + round words -> fold) -> phase 3 -> seam words -> verdict. Every rank issues the same collectives in the
-// same order whatever its piece holds: an empty piece sends identity transfers and zero words, a refused one keeps exchanging until the
-// verdict. The rounds after the settled one are gated off on the device; their all-gathers still run.
-int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                                        uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+static density_b200_cheetah_decode_shard* sharded_cdec(density_b200_sharded* h) {
+    if (!h->cdec) { h->cdec = new density_b200_cheetah_decode_shard(); h->cdec->num_sms = h->num_sms; }
+    return h->cdec;
+}
+
+// Sharded Cheetah decode of this rank's piece d_in[0 .. n) over the handle's communicator: phase 1 -> chunk-map transfers -> fold ->
+// phase 2 -> every round of the budget (walk -> prediction transfers + round words -> fold) -> phase 3 -> seam words -> verdict. Every
+// rank issues the same collectives in the same order whatever its piece holds: an empty piece sends identity transfers and zero words, a
+// refused one keeps exchanging until the verdict. The rounds after the settled one are gated off on the device; their all-gathers still
+// run. first: the piece holds the stream start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output
+// starts, from the verdict's prefix offsets.
+static int decode_sharded_cheetah_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
+                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, cudaStream_t st) {
     NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
     if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    if (!h->cdec) { h->cdec = new density_b200_cheetah_decode_shard(); h->cdec->num_sms = h->num_sms; }
-    density_b200_cheetah_decode_shard* s = h->cdec;
+    density_b200_cheetah_decode_shard* s = sharded_cdec(h);
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wc = density_b200_cheetah_cmap_words(), wp = 2 * 65536;
-    const bool first = R == 0, last = R == W - 1;
     ShardedAux x;
     cudaError_t e = sharded_aux(h, st, &x);
     if (e == cudaSuccess) e = h->cd_aux.ensure(((W + 1) * (wc + wp) + 4 * W + 64) * sizeof(uint32_t), st);
@@ -1400,8 +1401,19 @@ int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* 
     if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
     e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
     g_launches += launches;
+    if (e == cudaSuccess && d_out_offset) e = cudaMemcpyAsync(d_out_offset, x.offsets + h->rank, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
     return DENSITY_B200_OK;
+}
+
+// The pieces of a sharded Cheetah encode: rank 0 holds the stream start, the last rank its end.
+int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                        uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    return decode_sharded_cheetah_piece(h, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
+                                        reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
@@ -1419,35 +1431,91 @@ int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in
     return DENSITY_B200_OK;
 }
 
-int density_b200_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out4[4]) {
-    g_last_error.clear();
-    constexpr uint64_t W = DENSITY_B200_LOCATE_MAP_WORDS, TERM = ~0ull, CH = 16384, HALO = 264, NCAND = 132;
-    if (!h_maps || !out4 || world < 1 || rank < 0 || rank >= world) { set_error("locate_piece: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+// The layout checks and the walk from the stream start shared by density_b200_locate_piece (Chameleon) and
+// density_b200_cheetah_locate_piece. A map is {n_range, n_halo}, NCAND candidate rows {exit index or ~0, blocks}, and with START the
+// four words {range_offset, has_start_row, start exit, start blocks}: the first non-empty range then takes its exit from its start row
+// rather than from candidate 0. out5 = {start, end, blocks_before, is_final, is_first}.
+extern "C++" { namespace {
+template <uint64_t W, uint64_t NCAND, bool START>
+int locate_piece_walk(const uint64_t* h_maps, int world, int rank, uint64_t out5[5]) {
+    constexpr uint64_t TERM = ~0ull, CH = 16384, HALO = 264;
+    if (!h_maps || world < 1 || rank < 0 || rank >= world) { set_error("locate_piece: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
     uint64_t later = 0;                 // stream bytes behind range r
     for (int r = world - 1; r >= 0; --r) {
         const uint64_t* m = h_maps + (size_t)r * W;
         if (r < world - 1 && m[0] % CH) { set_error("locate_piece: a non-last range is not a multiple of 16384 bytes"); return DENSITY_B200_EARG; }
         if (m[1] != (later < HALO ? later : HALO)) { set_error("locate_piece: a halo is not min(264, the bytes of the later ranges)"); return DENSITY_B200_EARG; }
-        for (uint64_t c = 0; c < NCAND; ++c)
-            if (m[2 + 2 * c] != TERM && m[2 + 2 * c] >= NCAND) { set_error("locate_piece: bad exit index in a range map"); return DENSITY_B200_EARG; }
+        for (uint64_t c = 0; c < NCAND + (START ? 1 : 0); ++c) {    // + the start row's exit
+            const uint64_t x = c < NCAND ? m[2 + 2 * c] : m[4 + 2 * NCAND];
+            if (x != TERM && x >= NCAND) { set_error("locate_piece: bad exit index in a range map"); return DENSITY_B200_EARG; }
+        }
         if (m[0] > ~later) { set_error("locate_piece: ranges overflow"); return DENSITY_B200_EARG; }
         later += m[0];
     }
-    uint64_t idx = 0, blocks = 0;       // walk from the stream start; an empty range passes the entry on unchanged
+    if (START) {
+        uint64_t off = 0;
+        bool seen = false;              // a non-empty range before r
+        for (int r = 0; r < world; ++r) {
+            const uint64_t* m = h_maps + (size_t)r * W;
+            const uint64_t* s = m + 2 + 2 * NCAND;
+            if (s[0] != off) { set_error("locate_piece: a range offset is not the sum of the earlier ranges"); return DENSITY_B200_EARG; }
+            const bool holds_start = !seen && m[0] > 0;
+            if (s[1] != (holds_start ? 1u : 0u)) { set_error("locate_piece: the start row is not on exactly the first non-empty range"); return DENSITY_B200_EARG; }
+            seen |= m[0] > 0;
+            off += m[0];
+        }
+    }
+    // walk from the stream start; an empty range passes the entry on unchanged
+    uint64_t idx = 0, blocks = 0;
+    bool started = !START;              // START: the first non-empty range has not been passed yet
     for (int r = 0; r < rank; ++r) {
         const uint64_t* m = h_maps + (size_t)r * W;
         if (m[0] == 0) continue;
-        blocks += m[3 + 2 * idx];
-        idx = m[2 + 2 * idx];
-        if (idx == TERM) { out4[0] = 0; out4[1] = 0; out4[2] = blocks; out4[3] = 1; return DENSITY_B200_OK; }   // behind the stream end
+        const uint64_t* row = started ? m + 2 + 2 * idx : m + 4 + 2 * NCAND;
+        started = true;
+        blocks += row[1];
+        idx = row[0];
+        if (idx == TERM) { out5[0] = 0; out5[1] = 0; out5[2] = blocks; out5[3] = 1; out5[4] = 0; return DENSITY_B200_OK; }   // behind the stream end
     }
     const uint64_t* m = h_maps + (size_t)rank * W;
     const uint64_t n_range = m[0], n_halo = m[1];
-    if (n_range == 0) { out4[0] = 0; out4[1] = 0; out4[2] = blocks; out4[3] = n_halo == 0; return DENSITY_B200_OK; }
-    const uint64_t ex = m[2 + 2 * idx];
+    if (n_range == 0) { out5[0] = 0; out5[1] = 0; out5[2] = blocks; out5[3] = n_halo == 0; out5[4] = 0; return DENSITY_B200_OK; }
+    const uint64_t ex = started ? m[2 + 2 * idx] : m[4 + 2 * NCAND];
     const uint64_t start = 2 * idx, end = ex == TERM ? n_range + n_halo : n_range + 2 * ex;
     if (start > end || end > n_range + n_halo) { set_error("locate_piece: inconsistent range maps"); return DENSITY_B200_EARG; }
-    out4[0] = start; out4[1] = end; out4[2] = blocks; out4[3] = end == n_range + n_halo;
+    out5[0] = start; out5[1] = end; out5[2] = blocks; out5[3] = end == n_range + n_halo; out5[4] = started ? 0 : 1;
+    return DENSITY_B200_OK;
+}
+} }  // namespace, extern "C++"
+
+int density_b200_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out4[4]) {
+    g_last_error.clear();
+    if (!out4) { set_error("locate_piece: null pointer"); return DENSITY_B200_EARG; }
+    uint64_t out5[5];
+    const int rc = locate_piece_walk<DENSITY_B200_LOCATE_MAP_WORDS, 132, false>(h_maps, world, rank, out5);
+    if (rc == DENSITY_B200_OK) memcpy(out4, out5, 4 * sizeof(uint64_t));
+    return rc;
+}
+
+int density_b200_cheetah_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out5[5]) {
+    g_last_error.clear();
+    if (!out5) { set_error("locate_piece: null pointer"); return DENSITY_B200_EARG; }
+    return locate_piece_walk<DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS, 68, true>(h_maps, world, rank, out5);
+}
+
+int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset,
+                                       uint64_t* d_map, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_map) & 7)) { set_error("d_in must be 2-byte, d_map 8-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase = 0;               // the scratch is phase 1's
+    cudaError_t e = s->ws.ensure(chee_locate_workspace_bytes(n_range, n_halo, range_offset), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t launches = 0;
+    e = chee_decode_locate(d_in, n_range, n_halo, range_offset, s->ws.p, d_map, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode locate", e); return DENSITY_B200_ECUDA; }
     return DENSITY_B200_OK;
 }
 
@@ -1482,6 +1550,43 @@ int density_b200_decode_sharded_stream(density_b200_sharded* h, const uint8_t* d
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
     return decode_sharded_piece(h, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[3], d_out, cap, d_out_size, d_flags,
                                 d_total_size, d_out_offset, st);
+}
+
+// Sharded decode of a Cheetah stream without known cuts: this rank holds its range + halo at range_offset (include/density_b200.h).
+// Locates the piece (one host synchronisation), then decodes it as density_b200_decode_sharded_cheetah does, with the piece's own
+// "holds the stream start" and "ends the stream" rather than the rank's.
+int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset,
+                                               uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags,
+                                               uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n_range + n_halo) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    constexpr size_t MW = DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS;
+    density_b200_cheetah_decode_shard* s = sharded_cdec(h);
+    ShardedAux x;
+    // sized for the locate scratch and for the phases on any piece of range + halo, so that phase 1 does not reallocate
+    const size_t locate_bytes = chee_locate_workspace_bytes(n_range, n_halo, range_offset);
+    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms);
+    cudaError_t e = s->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, st);
+    if (e == cudaSuccess) e = sharded_aux(h, st, &x);    // its map slots hold DENSITY_B200_LOCATE_MAP_WORDS >= MW words per rank
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t* my_map = x.maps + (size_t)h->rank * MW;
+    uint64_t launches = 0;
+    e = chee_decode_locate(d_in, n_range, n_halo, range_offset, s->ws.p, my_map, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("cheetah decode locate", e); return DENSITY_B200_ECUDA; }
+    if (h->world > 1 && !nccl_check(a->AllGather(my_map, x.maps, MW * 8, NCCL_UINT8, h->comm, st), "ncclAllGather(maps)")) return DENSITY_B200_ECUDA;
+    e = cudaMemcpyAsync(h->h_maps, x.maps, (size_t)h->world * MW * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("range maps to host", e); return DENSITY_B200_ECUDA; }
+    uint64_t piece[5];
+    const int rc = density_b200_cheetah_locate_piece(h->h_maps, h->world, h->rank, piece);
+    if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
+    return decode_sharded_cheetah_piece(h, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
+                                        d_flags, d_total_size, d_out_offset, st);
 }
 
 /* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag

@@ -809,4 +809,44 @@ cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_
 }
 uint32_t chee_shard_max_rounds() { return MAX_ROUNDS; }
 
+// ---- the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64) ---------------------
+// Any range: the candidate walks over its chunks (the halo visible to its last chunk's walks), their composition per group and over the
+// whole range, as cham_decode_locate does, then {range_offset, 0, 0, 0}. The range that holds the stream start (range_offset 0, n_range
+// > 0) instead runs the exact boundary walk over range + halo and reads its start row off it (dec_start_row); its candidate rows are the
+// identity. Its scratch is the whole boundary layout with one offset per possible block.
+static bool chee_locate_has_start(size_t n_range, uint64_t range_offset) { return range_offset == 0 && n_range > 0; }
+
+size_t chee_locate_workspace_bytes(size_t n_range, size_t n_halo, uint64_t range_offset) {
+    bounds::BoundsLayout B;
+    return bounds::bounds_layout<T>(n_range + n_halo, chee_locate_has_start(n_range, range_offset) ? ~(size_t)0 : 0, &B);
+}
+
+cudaError_t chee_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset, uint8_t* ws, uint64_t* d_map,
+                               cudaStream_t stream, uint64_t* launches) {
+    const bool start = chee_locate_has_start(n_range, range_offset);
+    bounds::BoundsLayout B; bounds::bounds_layout<T>(n_range + n_halo, start ? ~(size_t)0 : 0, &B);
+    const uint4* gres = reinterpret_cast<const uint4*>(ws + B.gres);
+    unsigned long long* map = reinterpret_cast<unsigned long long*>(d_map);
+    uint32_t ngroups = 0;
+    if (start) {
+        const cudaError_t e = bounds::bounds_launch<T>(d_in, n_range + n_halo, ~(size_t)0, ws, B, stream, launches);
+        if (e != cudaSuccess) return e;
+    } else {
+        uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
+        const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
+        ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
+        if (nchunks) {
+            bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
+            bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, reinterpret_cast<uint4*>(ws + B.gres));
+            *launches += 2;
+        }
+    }
+    bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(gres, ngroups, n_range, n_halo, map);
+    bounds::dec_start_row<T><<<1, 32, 0, stream>>>(start ? reinterpret_cast<const DecStatus*>(ws + B.status) : nullptr,
+                                                   reinterpret_cast<const uint64_t*>(ws + B.blk_off), n_range, range_offset,
+                                                   map + 2 + 2 * T::NCAND);
+    *launches += 2;
+    return cudaGetLastError();
+}
+
 }  // namespace dns

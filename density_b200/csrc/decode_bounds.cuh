@@ -375,6 +375,33 @@ __global__ void __launch_bounds__(RC_THREADS) dec_range_compose(const uint4* __r
     if (tid == 0) { map[0] = n_range; map[1] = n_halo; }
 }
 
+// ---- 3b. the start row of the range that holds the stream start (sharded Cheetah decode without known cuts) -------------------------
+// The stream start's copy-mode blocks void the candidate walks of its range, so that range's exit comes from the exact boundary walk
+// (bounds_launch over range + halo from the fresh automaton, copy-mode blocks included): the first block start >= n_range, found in
+// blk_off, or the tail offset when the main loop ended behind n_range without another block start; ~0 when it ended (fewer than MAXBLK
+// bytes left) in front of n_range, i.e. the stream ends inside this range or its halo. The exit is an index into the next range as in a
+// candidate row, the block count includes the copy-mode blocks. Writes {range_offset, has_start_row, exit, blocks} to out4; st ==
+// nullptr (a range without the stream start): {range_offset, 0, 0, 0}.
+template <class T>
+__global__ void dec_start_row(const DecStatus* __restrict__ st, const uint64_t* __restrict__ blk_off, uint64_t n_range, uint64_t range_offset,
+                              unsigned long long* __restrict__ out4) {
+    if (threadIdx.x || blockIdx.x) return;
+    unsigned long long ex = 0, nb = 0;
+    if (st) {
+        const uint64_t mb = st->main_blocks;       // every block has its offset: the workspace holds one per T::SIG bytes
+        uint64_t lo = 0, hi = mb;
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if ((blk_off[mid] & ~BLK_COPY) < n_range) lo = mid + 1; else hi = mid;
+        }
+        nb = lo;
+        if (lo < mb) ex = ((blk_off[lo] & ~BLK_COPY) - n_range) >> 1;
+        else if (st->tail_off >= n_range) ex = (st->tail_off - n_range) >> 1;
+        else ex = ~0ull;
+    }
+    out4[0] = range_offset; out4[1] = st ? 1ull : 0ull; out4[2] = ex; out4[3] = nb;
+}
+
 // ---- host side: workspace layout + launch sequence ---------------------------------------------------------------------------------
 struct BoundsLayout { size_t status, res, gres, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, total; uint64_t maxblocks; };
 

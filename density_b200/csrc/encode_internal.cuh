@@ -111,6 +111,11 @@ cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t*
 cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
+// the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`,
+// at least chee_locate_workspace_bytes of the same arguments
+size_t chee_locate_workspace_bytes(size_t n_range, size_t n_halo, uint64_t range_offset);
+cudaError_t chee_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset, uint8_t* ws, uint64_t* d_map,
+                               cudaStream_t stream, uint64_t* launches);
 
 // scalar_codec.cu (Cheetah / Lion, in-order)
 size_t scalar_workspace_bytes(int alg);

@@ -27,6 +27,11 @@ A stream whose cuts are not known (one chameleon_encode call, the reference libr
 (`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
 (density_b200_decode_locate), and after an all_gather of the maps `locate_piece` gives every rank the exact offset where its
 first block starts. The located piece then decodes as above.
+
+A Cheetah stream without known cuts takes the same layout (ShardedDecoder.decode_stream(..., alg="cheetah", range_offset=o_r), or
+density_b200_cheetah_decode_locate with `locate_piece(maps, rank, alg="cheetah")` and the piece phases). Its stream start has
+copy-mode blocks, so the range that holds it (range_offset 0) finds its exit with the exact boundary walk; every later range uses
+its candidate rows.
 """
 import ctypes
 
@@ -95,6 +100,7 @@ def seam_verdict(words):
 
 
 LOCATE_MAP_WORDS = 266     # DENSITY_B200_LOCATE_MAP_WORDS
+CHEETAH_LOCATE_MAP_WORDS = 142   # DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS
 CHUNK = 16384              # non-last ranges are multiples of the boundary walk's chunk
 HALO = 264                 # the largest Chameleon block: every byte a block starting inside a range can reach
 
@@ -111,12 +117,17 @@ def stream_ranges(total, world):
     return out
 
 
-def locate_piece(maps, rank):
+def locate_piece(maps, rank, alg="chameleon"):
     """density_b200_locate_piece (host only) on the gathered range maps, uint64-compatible [world, 266] in rank order. Returns
-    (start, end, blocks_before, is_final): this rank's piece is its buffer's bytes [start, end)."""
-    m = np.ascontiguousarray(np.asarray(maps).astype(np.uint64, copy=False).reshape(-1, LOCATE_MAP_WORDS))
-    out = (ctypes.c_uint64 * 4)()
-    rc = _lib.load().density_b200_locate_piece(m.ctypes.data, m.shape[0], rank, out)
+    (start, end, blocks_before, is_final): this rank's piece is its buffer's bytes [start, end). alg "cheetah": the Cheetah maps
+    [world, 142] (density_b200_cheetah_locate_piece), and the tuple ends with is_first (the piece holds the stream start)."""
+    cheetah = _alg_id(alg) == 1
+    words, nout = (CHEETAH_LOCATE_MAP_WORDS, 5) if cheetah else (LOCATE_MAP_WORDS, 4)
+    m = np.ascontiguousarray(np.asarray(maps).astype(np.uint64, copy=False).reshape(-1, words))
+    out = (ctypes.c_uint64 * nout)()
+    lib = _lib.load()
+    fn = lib.density_b200_cheetah_locate_piece if cheetah else lib.density_b200_locate_piece
+    rc = fn(m.ctypes.data, m.shape[0], rank, out)
     if rc:
         raise _lib.DensityB200Error(f"locate_piece rc={rc}: {_lib.last_error()}")
     return tuple(int(v) for v in out)
@@ -452,13 +463,22 @@ class ShardedDecoder(_ShardedHandle):
         if rc:
             raise _lib.DensityB200Error(f"decode_sharded{'' if alg == 0 else '_cheetah'} rc={rc}: {_lib.last_error()}")
 
-    def decode_stream(self, d_in, n_range, d_out, d_size, d_flags):
+    def decode_stream(self, d_in, n_range, d_out, d_size, d_flags, alg="chameleon", range_offset=None):
         """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range
         bytes) followed by its halo (stream_ranges gives the layout); the rest as in decode. Blocks once, on the range maps.
-        self.d_offset int64[1]: where this rank's output starts in the original bytes."""
+        self.d_offset int64[1]: where this rank's output starts in the original bytes. alg "cheetah" (or its id): a Cheetah stream
+        (density_b200_decode_sharded_cheetah_stream); range_offset, where this rank's range starts in the stream, is then required."""
+        alg = _alg_id(alg)
+        if alg not in (0, 1):
+            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+        if alg == 1 and range_offset is None:
+            raise ValueError("sharded Cheetah stream decode: range_offset is required")
+        n_halo = d_in.numel() - n_range
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self._lib.density_b200_decode_sharded_stream(self._h, d_in.data_ptr(), n_range, d_in.numel() - n_range, d_out.data_ptr(),
-                                                          d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(), d_flags.data_ptr(),
-                                                          self.d_total.data_ptr(), stream)
+        tail = (d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), stream)
+        if alg == 0:
+            rc = self._lib.density_b200_decode_sharded_stream(self._h, d_in.data_ptr(), n_range, n_halo, *tail)
+        else:
+            rc = self._lib.density_b200_decode_sharded_cheetah_stream(self._h, d_in.data_ptr(), n_range, n_halo, int(range_offset), *tail)
         if rc:
-            raise _lib.DensityB200Error(f"decode_sharded_stream rc={rc}: {_lib.last_error()}")
+            raise _lib.DensityB200Error(f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream rc={rc}: {_lib.last_error()}")

@@ -246,7 +246,8 @@ DENSITY_B200_API int density_b200_decode_sharded(density_b200_sharded*, const ui
  *   - the prediction rounds did not settle within the round budget (density_b200_cheetah_decode_round_budget);
  *   - a piece is malformed, its output exceeds `cap`, or a non-final piece does not decode to whole 128-byte blocks.
  * Only the first piece may use copy mode: it holds the stream start, where every Cheetah stream has copy-mode blocks. Lion streams and
- * streams without known cuts are not decoded this way. d_in must be 2-byte and d_out 4-byte aligned; nothing is written past `cap`.
+ * streams without known cuts are not decoded this way (density_b200_decode_sharded_cheetah_stream locates their pieces first). d_in must
+ * be 2-byte and d_out 4-byte aligned; nothing is written past `cap`.
  *
  * Phase API of one piece (any transport; W pieces may run on one GPU): phase 1 -> exchange of the chunk-map transfers -> phase 2 -> rounds
  * (round_walk -> exchange of the prediction transfers and the round words -> round_fold), as many as the round budget -> phase 3 -> seam
@@ -332,6 +333,43 @@ DENSITY_B200_API int density_b200_locate_piece(const uint64_t* h_maps, int world
 DENSITY_B200_API int density_b200_decode_sharded_stream(density_b200_sharded*, const uint8_t* d_in, size_t n_range, size_t n_halo,
                                        uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset,
                                        uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
+ * Sharded decode of a Cheetah stream whose cuts are not known (one cheetah_encode call, the reference library, a file, a gathered
+ * sharded stream without its piece sizes), with the input layout of density_b200_decode_sharded_stream: range + halo of min(264, the
+ * bytes of the later ranges), non-last ranges multiples of 16384 bytes. Each rank also passes its range_offset o_r (the sum of the
+ * earlier n_range): the range with range_offset 0 and n_range > 0 holds the stream start.
+ *
+ * The range map (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64): {n_range, n_halo}, then for each of the 68 possible even entry offsets
+ * {exit index or ~0, blocks} as in the Chameleon map (blocks taken as encoded blocks), then {range_offset, has_start_row, start exit,
+ * start blocks}. Every Cheetah stream has copy-mode blocks near its start, which void the candidate walks there, so the range that
+ * holds the stream start has a START ROW instead (its candidate rows are the identity): the exit and block count of the exact boundary
+ * walk (codec.rs's main loop with the protection automaton, copy-mode blocks counted) from the stream start, the exit being the first
+ * block start at or after n_range, or ~0 when the walk ends (fewer than 136 bytes left) in front of n_range.
+ */
+#define DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS 142
+/* Enqueues the range map of d_in[0 .. n_range + n_halo) into d_map (device, 8-byte aligned). Kernels: 4 on a range without the stream
+   start (2 when it is empty), 11 on the range with it (the 9 boundary kernels of the exact walk, the identity rows, the start row).
+   The scratch lives in the handle's workspace, which the next phase 1 overwrites; on the start range it holds one offset per 8 stream
+   bytes. The layout is checked by density_b200_cheetah_locate_piece. */
+DENSITY_B200_API int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                        uint64_t range_offset, uint64_t* d_map, void* stream);
+/* Host only, needs no device. h_maps: the Cheetah range maps of all `world` ranks in rank order. Checks the layout as
+   density_b200_locate_piece does, and that every range_offset is the sum of the earlier n_range and the start row is set on exactly
+   the first non-empty range (DENSITY_B200_EARG otherwise, on every rank alike). Walks the maps from the start row: empty ranges pass
+   the entry on, later ranges follow their candidate rows. out5 = {start, end, blocks_before, is_final, is_first}: this rank's piece is
+   d_in[start .. end), it begins after blocks_before blocks, is_final = 1 when no stream byte follows it, is_first = 1 when it holds the
+   stream start. A piece behind the end of the stream is empty. */
+DENSITY_B200_API int density_b200_cheetah_locate_piece(const uint64_t* h_maps, int world, int rank, uint64_t out5[5]);
+/* End to end over NCCL on a density_b200_sharded handle: Cheetah range map -> ncclAllGather(maps) -> one device-to-host copy and ONE
+   host synchronisation -> density_b200_cheetah_locate_piece -> the path of density_b200_decode_sharded_cheetah on the located piece,
+   with is_first / is_last of the located piece. *d_out_offset = where this piece's output starts in the original bytes; the other
+   outputs as density_b200_decode_sharded_cheetah (d_out_offset and d_total_size may be NULL). Only the piece that holds the stream
+   start may use copy mode; a zero verdict proves every cut is a true block boundary (DESIGN.md section 5). For a quiet piece
+   cap >= 16 * (n_range + n_halo) is always enough; a piece whose output does not fit is refused, and nothing is written past cap. */
+DENSITY_B200_API int density_b200_decode_sharded_cheetah_stream(density_b200_sharded*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                               uint64_t range_offset, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                               uint64_t* d_out_offset, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
  * A reused Codec INSTANCE (streaming continuation). In the reference `encode` / `decode` are methods of an instance

@@ -1814,7 +1814,7 @@ int density_b200_cheetah_decode_rounds(uint32_t* out4) {
     std::lock_guard<std::mutex> lk(c->mu);
     unsigned int raw[8] = {0};
     if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(raw, c->last_cl_status, sizeof raw, cudaMemcpyDeviceToHost) != cudaSuccess) return DENSITY_B200_ECUDA;
-    out4[0] = raw[3]; out4[1] = raw[2] && !raw[5]; out4[2] = raw[6]; out4[3] = 40;
+    out4[0] = raw[3]; out4[1] = raw[2] && !raw[5]; out4[2] = raw[6]; out4[3] = chee_shard_max_rounds();   // cl_decode.cu MAX_ROUNDS
     return DENSITY_B200_OK;
 }
 

@@ -29,7 +29,7 @@ inline uint32_t rd16(const uint8_t* p) { return p[0] | (p[1] << 8); }
 inline uint32_t rd32(const uint8_t* p) { return rd16(p) | (rd16(p + 2) << 16); }
 
 template <int NP /* prediction slots: 1 cheetah, 5 lion */>
-size_t decode_impl(const uint8_t* in, size_t n, uint8_t* out, size_t cap, uint32_t nruns, uint32_t max_rounds, uint32_t* stats) {
+size_t decode_impl(const uint8_t* in, size_t n, uint8_t* out, size_t cap, uint32_t nruns, uint32_t max_rounds, uint32_t* stats, uint32_t nstats = 4) {
     constexpr bool LION = NP == 5;
     constexpr uint32_t BS = LION ? 64 : 128, SB = LION ? 6 : 8, QPB = BS / 4, FB = LION ? 3 : 2;
     // ---- 0. boundaries (codec.rs:88-100) ------------------------------------------------------------------------------
@@ -120,7 +120,8 @@ size_t decode_impl(const uint8_t* in, size_t n, uint8_t* out, size_t cap, uint32
     std::vector<uint8_t> dirty(nruns, 1), dirty_next(nruns, 0);
     std::vector<uint32_t> run_epoch(nruns, 0);
     std::vector<std::vector<uint8_t>> rset(nruns, std::vector<uint8_t>(65536, 0));
-    uint64_t walks = 0;
+    uint64_t walks = 0, queued = 0;                        // queued: run walks the context sweeps ask for (cd_round_end's counter)
+    uint32_t last_queued = 0;
     for (uint32_t round = 0; round < max_rounds && !converged; ++round) {
         ++rounds;
         const uint32_t epoch = round + 1;
@@ -178,17 +179,22 @@ size_t decode_impl(const uint8_t* in, size_t n, uint8_t* out, size_t cap, uint32
         uint32_t c = 0, ndirty = 0;
         for (uint32_t r = 0; r < nruns; ++r) {
             uint8_t d = dirty_next[r];
-            if (round == 0 && r > 0) d = 1;                // runs > 0 had no snapshot in round 0
+            // runs > 0 had no snapshot in round 0. This changes no value: such a run that read carried-in state met an unknown and is
+            // dirty anyway (list_init without a snapshot); one that did not is walked again when its entry context changes, and was exact
+            // otherwise. The rule only adds walks, as in cd_round_end, whose walk counts the GPU tests compare with these.
+            if (round == 0 && r > 0) d = 1;
             if (ctx_in[r] != c) { d = 1; ctx_in[r] = c; }
             dirty[r] = d; dirty_next[r] = 0; ndirty += d;
             if (ctx_out[r] != 0xFFFFFFFEu) c = ctx_out[r];
         }
         final_ctx = c;
         converged = ndirty == 0;
+        queued += ndirty; last_queued = ndirty;
         if (getenv("CL_MODEL_TRUTH")) fprintf(stderr, "round %u: dirty runs for the next round %u\n", round, ndirty);
     }
     if (stats) stats[3] = (uint32_t)walks;
     if (stats) { stats[0] = rounds; stats[1] = converged; stats[2] = (uint32_t)nb; }
+    if (stats && nstats >= 7) { stats[4] = (uint32_t)queued; stats[5] = last_queued; stats[6] = nruns; }
     if (!converged) return 0;
     // ---- write the main part --------------------------------------------------------------------------------------------------------
     for (uint64_t i = 0; i < nq; ++i) { out[4 * i] = (uint8_t)val[i]; out[4 * i + 1] = (uint8_t)(val[i] >> 8); out[4 * i + 2] = (uint8_t)(val[i] >> 16); out[4 * i + 3] = (uint8_t)(val[i] >> 24); }
@@ -245,4 +251,10 @@ extern "C" size_t cl_model_decode(int alg, const uint8_t* in, size_t n, uint8_t*
     if (alg == 1) return decode_impl<1>(in, n, out, cap, nruns, max_rounds, stats);
     if (alg == 2) return decode_impl<5>(in, n, out, cap, nruns, max_rounds, stats);
     return 0;
+}
+
+// Cheetah only, stats7 = {rounds, settled, main blocks, run walks, run walks queued by the context sweeps of all rounds (the GPU's counter:
+// the walks after round 0, plus those the last round queued when it did not settle), walks queued by the last round, run count used}
+extern "C" size_t cl_model_decode_stats(const uint8_t* in, size_t n, uint8_t* out, size_t cap, uint32_t nruns, uint32_t max_rounds, uint32_t* stats7) {
+    return decode_impl<1>(in, n, out, cap, nruns, max_rounds, stats7, 7);
 }

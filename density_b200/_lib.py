@@ -29,6 +29,17 @@ _SIGS = {
     "density_b200_encode_sharded": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p,
                                                    ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, ctypes.c_void_p]),
     "density_b200_sharded_profile": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float)]),
+    "density_b200_prot_round_budget": (ctypes.c_int, []),
+    "density_b200_shard_prot_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_uint64, ctypes.c_int, ctypes.c_void_p,
+                                                      ctypes.c_void_p]),
+    "density_b200_shard_prot_transfer": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_shard_prot_settle": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_shard_prot_next": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_shard_prot_finish": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_shard_prot_status": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32)]),
+    "density_b200_encode_sharded_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t,
+                                                             ctypes.c_void_p]),
     "density_b200_decode_shard_create": (ctypes.c_void_p, []),
     "density_b200_decode_shard_destroy": (None, [ctypes.c_void_p]),
     "density_b200_decode_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
@@ -91,6 +102,7 @@ _SIGS = {
     "density_b200_encode_status": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_test_set_stage_rounds": (None, [ctypes.c_int]),
     "density_b200_test_set_decode_rounds": (None, [ctypes.c_int]),
+    "density_b200_test_set_prot_rounds": (None, [ctypes.c_int]),
     "density_b200_prot_debug": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_shutdown": (None, []),
     "density_b200_version": (ctypes.c_char_p, []),

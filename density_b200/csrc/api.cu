@@ -612,6 +612,10 @@ struct density_b200_shard {
     int is_last = 1;
     int num_sms = 0;
     bool phase1_done = false;
+    // the copy-map iteration of density_b200_shard_prot_*: the shard's device record and where the phases stand
+    DevBuf prot;
+    int prot_phase = 0;             // 0 none, 1 flags ready (phase 1 / next with a table), 2 transfer, 3 settle, 4 committed, 5 finished
+    int round = 0;
 };
 
 density_b200_shard* density_b200_shard_create(void) {
@@ -625,6 +629,7 @@ density_b200_shard* density_b200_shard_create(void) {
 void density_b200_shard_destroy(density_b200_shard* s) {
     if (!s) return;
     s->ws.release();
+    s->prot.release();
     delete s;
 }
 int density_b200_shard_phase1(density_b200_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, uint32_t* d_table_out, void* stream) {
@@ -632,6 +637,7 @@ int density_b200_shard_phase1(density_b200_shard* s, const uint8_t* d_in, size_t
     if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
     if (reinterpret_cast<uintptr_t>(d_in) & 3) { set_error("d_in must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    s->prot_phase = 0;              // the workspace is this phase's now: the copy-map phases start over with prot_phase1
     size_t need = cham_workspace_bytes(n, s->num_sms, &s->L);
     cudaError_t e = s->ws.ensure(need);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
@@ -663,6 +669,123 @@ int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in,
     }
     g_launches += launches;
     if (e != cudaSuccess) { set_error("shard phase2", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
+// ---- sharded Chameleon encode with copy mode: the copy-map iteration carried over the cuts ---------------------------------------------
+static int g_prot_rounds = (int)PROT_MAX_ROUNDS;   // round budget (density_b200_test_set_prot_rounds)
+static bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+static ProtShard* prot_rec(density_b200_shard* s) { return reinterpret_cast<ProtShard*>(s->prot.p); }
+
+int density_b200_prot_round_budget(void) { return g_prot_rounds; }
+void density_b200_test_set_prot_rounds(int k) { g_prot_rounds = (k >= 1 && k <= (int)PROT_MAX_ROUNDS) ? k : (int)PROT_MAX_ROUNDS; }
+
+// first_block = ~0: taken from d_lengths (the gathered shard lengths) on the device instead
+static int prot_phase1_impl(density_b200_shard* s, const uint8_t* d_in, size_t n, uint64_t first_block, const uint64_t* d_lengths, int rank,
+                            int is_last_shard, uint32_t* d_table_out, cudaStream_t st) {
+    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if (!al4(d_in) || !al4(d_table_out)) { set_error("d_in and d_table_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);
+    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->is_last = is_last_shard; s->nruns = cham_pick_runs(n, s->num_sms);
+    s->phase1_done = false; s->prot_phase = 0; s->round = 0;
+    uint64_t launches = 0;
+    e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, n ? d_table_out : nullptr, st, &launches);
+    if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);   // nothing touched
+    if (e == cudaSuccess) e = cham_prot_start(s->ws.p, s->L, prot_rec(s), d_lengths ? 0 : first_block, d_lengths, (uint32_t)rank, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("shard prot phase1", e); return DENSITY_B200_ECUDA; }
+    s->prot_phase = 1;
+    return DENSITY_B200_OK;
+}
+static int prot_transfer_impl(density_b200_shard* s, const uint32_t* d_carry_in, uint32_t* d_transfer_out, cudaStream_t st) {
+    if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 1) { set_error("shard_prot_transfer: call it after prot_phase1 or prot_next with a table"); return DENSITY_B200_EARG; }
+    if (!al4(d_carry_in) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e = cham_prot_transfer(s->n, s->ws.p, s->L, s->nruns, d_carry_in, prot_rec(s), s->round, d_transfer_out, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("shard prot transfer", e); return DENSITY_B200_ECUDA; }
+    s->prot_phase = 2;
+    return DENSITY_B200_OK;
+}
+static int prot_settle_impl(density_b200_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out, cudaStream_t st) {
+    if (!s || !d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 2) { set_error("shard_prot_settle: call it after prot_transfer"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e = cham_prot_settle(s->n, s->ws.p, s->L, prot_rec(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("shard prot settle", e); return DENSITY_B200_ECUDA; }
+    s->prot_phase = 3;
+    return DENSITY_B200_OK;
+}
+static int prot_next_impl(density_b200_shard* s, const uint32_t* d_all_words, int world, uint32_t* d_table_out, cudaStream_t st) {
+    if (!s || !d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 3) { set_error("shard_prot_next: call it after prot_settle"); return DENSITY_B200_EARG; }
+    if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_words) || !al4(d_table_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (d_table_out && s->round + 1 >= g_prot_rounds) { set_error("shard_prot_next: the round budget is used up"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    cudaError_t e = cham_prot_next(s->d_in, s->n, s->ws.p, s->L, s->nruns, prot_rec(s), s->round, d_all_words, (uint32_t)world, d_table_out, st,
+                                   &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("shard prot next", e); return DENSITY_B200_ECUDA; }
+    if (d_table_out) { ++s->round; s->prot_phase = 1; }
+    else s->prot_phase = 4;
+    return DENSITY_B200_OK;
+}
+static int prot_finish_impl(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st,
+                            cudaEvent_t* ev) {
+    if (!s || (!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 4) { set_error("shard_prot_finish: call it after prot_next without a table"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_out) & 1) || (reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) {
+        set_error("d_out must be 2-byte, d_out_size 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    uint64_t launches = 0;
+    cudaError_t e = cham_prot_finish(s->d_in, s->n, s->ws.p, s->L, prot_rec(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("shard prot finish", e); return DENSITY_B200_ECUDA; }
+    s->prot_phase = 5;
+    return DENSITY_B200_OK;
+}
+
+int density_b200_shard_prot_phase1(density_b200_shard* s, const uint8_t* d_in, size_t n, uint64_t first_block, int is_last_shard,
+                                   uint32_t* d_table_out, void* stream) {
+    g_last_error.clear();
+    if (first_block == ~0ull) { set_error("bad first_block"); return DENSITY_B200_EARG; }
+    return prot_phase1_impl(s, d_in, n, first_block, nullptr, 0, is_last_shard, d_table_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_shard_prot_transfer(density_b200_shard* s, const uint32_t* d_carry_in, uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    return prot_transfer_impl(s, d_carry_in, d_transfer_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_shard_prot_settle(density_b200_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out, void* stream) {
+    g_last_error.clear();
+    return prot_settle_impl(s, d_all_transfers, world, rank, d_words_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_shard_prot_next(density_b200_shard* s, const uint32_t* d_all_words, int world, uint32_t* d_table_out, void* stream) {
+    g_last_error.clear();
+    return prot_next_impl(s, d_all_words, world, d_table_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int density_b200_shard_prot_finish(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    return prot_finish_impl(s, d_out, cap, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream), nullptr);
+}
+int density_b200_shard_prot_status(density_b200_shard* s, uint32_t* out) {
+    g_last_error.clear();
+    if (!s || !out || s->prot_phase < 4) { set_error("shard_prot_status: null pointer / rounds not committed"); return DENSITY_B200_EARG; }
+    ProtShard h{};
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(&h, s->prot.p, sizeof h, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error("shard_prot_status", e); return DENSITY_B200_ECUDA; }
+    out[0] = h.rounds; out[1] = h.settled; out[3] = h.esc;
+    const uint32_t c = h.in_state;   // pc_encode candidate -> penalty | start << 8 | previous_incompressible << 16
+    out[2] = c >= PROT_TRANSFER_WORDS ? 0xFFFFFFFFu : (c % 10) | (((c / 10) % 10 + 1) << 8) | ((c / 100) << 16);
+    for (int k = 0; k < 16; ++k) out[4 + k] = h.changed[k];
     return DENSITY_B200_OK;
 }
 
@@ -1072,6 +1195,8 @@ struct density_b200_sharded {
     DevBuf cl_aux;                  // its exchange buffers: gathered P and C tables, the carries, the last quads
     density_b200_cheetah_decode_shard* cdec = nullptr;   // piece state of density_b200_decode_sharded_cheetah
     DevBuf cd_aux;                  // its exchange buffers: gathered chunk-map and prediction transfers, the carries, the round words
+    density_b200_shard* prot = nullptr;   // shard state of density_b200_encode_sharded_protected
+    DevBuf prot_aux;                // its exchange buffers: gathered shard lengths, transfers and round words
     ChamLayout L{};
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     uint64_t* h_maps = nullptr;     // pinned, world range maps (density_b200_decode_sharded_stream)
@@ -1117,7 +1242,8 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release(); h->cd_aux.release();
+    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release(); h->cd_aux.release(); h->prot_aux.release();
+    density_b200_shard_destroy(h->prot);
     for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
     density_b200_cheetah_decode_shard_destroy(h->cdec);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
@@ -1288,6 +1414,83 @@ int density_b200_encode_sharded_cl(density_b200_sharded* h, int alg, const uint8
     rc = cl_phase3_impl(s, carry_c, d_out, cap, d_out_size, x.words + 8 * R, st);
     if (rc != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[4], st);
+    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
+    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
+    if (gather_root >= 0) {
+        rc = gather_pieces(h, a, x.offsets, d_out, gather_root, d_gather, gather_cap, st);
+        if (rc != DENSITY_B200_OK) return rc;
+    }
+    cudaEventRecord(h->ev[5], st);
+    h->timed = true;
+    return DENSITY_B200_OK;
+}
+
+// Sharded Chameleon encode with copy mode over the handle's communicator: the shard lengths -> phase 1 -> the round budget of
+// {tables -> fold -> transfer -> transfers -> settle -> round words -> commit (+ next round's flags)} -> finish -> seam words -> verdict
+// -> optional gather. Every rank runs the same rounds, so the collectives match; the gates keep the settled rounds cheap.
+int density_b200_encode_sharded_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                          uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap,
+                                          void* stream_v) {
+    g_last_error.clear();
+    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    const bool last = h->rank == h->world - 1;
+    if (!last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+    // every argument the later phases check is checked here, before the first collective: a rank that returned EARG half way through
+    // would leave the others waiting in an all-gather
+    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || (reinterpret_cast<uintptr_t>(d_total_size) & 7) || !al4(d_flags)) {
+        set_error("d_out_size and d_total_size must be 8-byte, d_flags 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
+    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+    if (!h->prot) {
+        h->prot = new density_b200_shard();
+        h->prot->num_sms = h->num_sms;
+    }
+    density_b200_shard* s = h->prot;
+    const size_t W = (size_t)h->world, R = (size_t)h->rank;
+    ShardedAux x;
+    cudaError_t e = sharded_aux(h, st, &x);
+    if (e == cudaSuccess) e = h->prot_aux.ensure(W * (2 * sizeof(uint64_t) + (PROT_TRANSFER_WORDS + PROT_ROUND_WORDS) * sizeof(uint32_t)) + 256, st);
+    if (e == cudaSuccess) e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);      // phase 1 finds them in place
+    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t* lengths = reinterpret_cast<uint64_t*>(h->prot_aux.p);                   // [world]
+    uint32_t* transfers = reinterpret_cast<uint32_t*>(lengths + W);                   // [world][PROT_TRANSFER_WORDS]
+    uint32_t* rwords = transfers + W * PROT_TRANSFER_WORDS;                          // [world][PROT_ROUND_WORDS]
+    uint32_t* my_table = x.tables + R * 65536;
+    uint64_t launches = 0;
+    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
+        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
+    };
+    cudaEventRecord(h->ev[0], st);
+    e = cham_put_u64(lengths + R, (uint64_t)n, st, &launches);
+    g_launches += launches; launches = 0;
+    if (e != cudaSuccess) { set_error("sharded protected: length", e); return DENSITY_B200_ECUDA; }
+    if (!gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
+    int rc = prot_phase1_impl(s, d_in, n, 0, lengths, (int)R, last, my_table, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[1], st);
+    for (int k = 0; k < g_prot_rounds; ++k) {
+        if (k > 0 && (rc = prot_next_impl(s, rwords, (int)W, my_table, st)) != DENSITY_B200_OK) return rc;
+        if (!gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+        e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, st, &launches);
+        g_launches += launches; launches = 0;
+        if (e != cudaSuccess) { set_error("sharded protected: fold", e); return DENSITY_B200_ECUDA; }
+        if (k == 0) cudaEventRecord(h->ev[2], st);
+        if ((rc = prot_transfer_impl(s, x.carry, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        if ((rc = prot_settle_impl(s, transfers, (int)W, (int)R, rwords + R * PROT_ROUND_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!gather(rwords, PROT_ROUND_WORDS, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+    }
+    if ((rc = prot_next_impl(s, rwords, (int)W, nullptr, st)) != DENSITY_B200_OK) return rc;
+    cudaEvent_t pev[4] = {nullptr, nullptr, h->ev[3], h->ev[4]};
+    if ((rc = prot_finish_impl(s, d_out, cap, d_out_size, x.words + 8 * R, st, n ? pev : nullptr)) != DENSITY_B200_OK) return rc;
+    if (!n) { cudaEventRecord(h->ev[3], st); cudaEventRecord(h->ev[4], st); }
     if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
     e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
     g_launches += launches;

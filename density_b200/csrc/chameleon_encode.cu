@@ -1160,6 +1160,177 @@ __global__ void cham_seam_verdict_k(const uint32_t* __restrict__ all_words, uint
     (void)rank;
 }
 
+// ------------------------------------------------------------------------------------------------------
+// Sharded copy-map iteration (include/density_b200.h density_b200_shard_prot_*, DESIGN.md section 5). Each shard runs the rounds of
+// prot_iterate's fixed point on its own blocks, with the automaton state carried over the cuts: per round it exports its TRANSFER
+// (candidate state at the shard start -> candidate state at the shard end, or PC_ESC; the candidates of pc_encode), every shard composes
+// the transfers of the shards before it from the canonical state, walks its blocks from that true incoming state and reports round words
+// {blocks whose copy status changed, met PC_ESC, the iteration had settled before this round, 0}. The verdict over all shards' words is
+// the same on every shard: settled when no block changed anywhere and no path met PC_ESC. ps->first_block makes `counter` global:
+// revert_to_copy halves the start on every 16th block of the STREAM, and shards start at any block.
+// ------------------------------------------------------------------------------------------------------
+constexpr uint32_t PROT_REFUSED = 16;   // Status::error of a shard whose iteration did not settle (or met PC_ESC): nothing is emitted
+
+__global__ void cham_put_u64_k(uint64_t* __restrict__ p, uint64_t v) { if (threadIdx.x == 0 && blockIdx.x == 0) *p = v; }
+__global__ void cham_prot_start_k(Status* __restrict__ st, ProtShard* __restrict__ ps, uint64_t first_block, const uint64_t* __restrict__ lengths,
+                                  uint32_t rank) {
+    if (threadIdx.x || blockIdx.x) return;
+    if (lengths) { uint64_t o = 0; for (uint32_t r = 0; r < rank; ++r) o += lengths[r]; first_block = o / 256; }
+    *ps = ProtShard{};
+    ps->first_block = first_block;
+    st->nonquiet = 1;        // the copy map is always in force on this path: every round's kernels run until the global verdict closes them
+    st->converged = 0;
+}
+
+// segment s: refresh the incompressible bits of its blocks (prot_iterate step 1), then walk it from every candidate state at once, one
+// candidate per thread; the paths merge quickly (the start halves every 16 blocks, a penalty decays), and once they all agree one thread
+// walks the rest of the segment.
+__global__ void __launch_bounds__(PSEG)
+cham_prot_seg_k(const uint32_t* __restrict__ sigw_g, uint64_t nbytes, uint64_t nblocks, uint32_t nseg, const Status* __restrict__ st, int it,
+                uint8_t* __restrict__ inc, const uint8_t* __restrict__ cm_old, const ProtShard* __restrict__ ps, uint16_t* __restrict__ T) {
+    if (!gate_open(st)) return;
+    __shared__ uint8_t s_inc[PSEG];
+    __shared__ uint32_t s_ref;
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t seg = blockIdx.x; seg < nseg; seg += gridDim.x) {   // a bounded grid: the settled rounds launch it for nothing
+    const uint64_t b0 = (uint64_t)seg * PSEG;
+    const uint32_t nb = (uint32_t)((nblocks - b0 < (uint64_t)PSEG) ? (nblocks - b0) : PSEG);
+    if (tid < nb) {
+        const uint64_t b = b0 + tid;
+        if (!(it && cm_old[b])) inc[b] = (nbytes - b * 256 >= 256) && (__popc(sigw_g[2 * b]) + __popc(sigw_g[2 * b + 1]) <= 4);
+        s_inc[tid] = inc[b];
+    }
+    __syncthreads();
+    Protection p; pc_decode(tid < PC_NC ? tid : 0u, p);
+    p.counter = ps->first_block + b0;
+    uint32_t k = 0;
+    while (k < nb) {                                               // CTA-uniform
+        const uint32_t k1 = (k + 16 < nb) ? k + 16 : nb;
+        for (; k < k1; ++k) { if (p.revert_to_copy()) p.decay(); else p.update(s_inc[k] != 0); }
+        if (tid == 0) s_ref = prot_pack(p);
+        __syncthreads();
+        if (__syncthreads_and(prot_pack(p) == s_ref)) break;
+    }
+    if (k < nb) {
+        if (tid == 0) {
+            for (; k < nb; ++k) { if (p.revert_to_copy()) p.decay(); else p.update(s_inc[k] != 0); }
+            s_ref = pc_encode(p);
+        }
+        __syncthreads();
+        if (tid < PC_NC) T[(size_t)seg * PC_NC + tid] = (uint16_t)s_ref;
+    } else if (tid < PC_NC) {
+        T[(size_t)seg * PC_NC + tid] = (uint16_t)pc_encode(p);
+    }
+    __syncthreads();                                               // s_inc and s_ref are reused by the next segment
+    }
+}
+
+// group tables (as prot_iterate's GT) and the shard's transfer: the group tables composed in order for every candidate
+__global__ void cham_prot_groups_k(uint32_t nseg, const Status* __restrict__ st, const uint16_t* __restrict__ T, uint16_t* __restrict__ GT) {
+    if (!gate_open(st)) return;
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    const uint64_t idx = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (uint64_t)ngrp * PC_NC) return;
+    const uint32_t g = (uint32_t)(idx / PC_NC);
+    uint32_t x = (uint32_t)(idx % PC_NC);
+    const uint32_t s1 = ((g + 1) * PC_GROUP < nseg) ? (g + 1) * PC_GROUP : nseg;
+    for (uint32_t s = g * PC_GROUP; s < s1 && x != PC_ESC; ++s) x = T[(size_t)s * PC_NC + x];
+    GT[idx] = (uint16_t)x;
+}
+__global__ void cham_prot_transfer_k(uint32_t nseg, const Status* __restrict__ st, const uint16_t* __restrict__ GT, uint32_t* __restrict__ out) {
+    if (!gate_open(st)) return;
+    const uint32_t c = threadIdx.x;
+    if (c >= PC_NC) return;
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    uint32_t x = c;                                                // an empty shard is the identity
+    for (uint32_t g = 0; g < ngrp && x != PC_ESC; ++g) x = GT[(size_t)g * PC_NC + x];
+    out[c] = x;
+}
+
+// settle, 1: the true incoming state (the transfers of the shards before `rank` composed from the canonical state), the incoming state
+// of every group, and this round's words (written whether or not the gate is open, so that every gathered word is this round's)
+__global__ void cham_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t nseg, const Status* __restrict__ st,
+                                  const uint16_t* __restrict__ GT, uint32_t* __restrict__ gin, ProtShard* __restrict__ ps,
+                                  uint32_t* __restrict__ words) {
+    if (threadIdx.x || blockIdx.x) return;
+    const bool open = gate_open(st);
+    words[0] = 0; words[1] = 0; words[2] = open ? 0u : 1u; words[3] = 0;
+    if (!open) return;
+    uint32_t x = 0;                                                // canonical state: penalty 0, start 1, not incompressible
+    for (uint32_t r = 0; r < rank && x != PC_ESC; ++r) x = all_transfers[(size_t)r * PC_NC + x];
+    ps->in_state = x;
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    for (uint32_t g = 0; g < ngrp; ++g) { gin[g] = x; if (x != PC_ESC) x = GT[(size_t)g * PC_NC + x]; }
+    gin[ngrp] = x;
+    if (x == PC_ESC) words[1] = 1;
+}
+// settle, 2: the incoming state of every segment
+__global__ void cham_prot_seams_k(uint32_t nseg, const Status* __restrict__ st, const uint16_t* __restrict__ T, const uint32_t* __restrict__ gin,
+                                  uint32_t* __restrict__ in_state) {
+    if (!gate_open(st)) return;
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= ngrp || gin[ngrp] == PC_ESC) return;
+    uint32_t x = gin[g];
+    const uint32_t s1 = ((g + 1) * PC_GROUP < nseg) ? (g + 1) * PC_GROUP : nseg;
+    for (uint32_t s = g * PC_GROUP; s < s1; ++s) { in_state[s] = x; x = T[(size_t)s * PC_NC + x]; }
+}
+// settle, 3: every segment walked from its true incoming state writes the new copy map; the blocks whose status changed are counted
+__global__ void cham_prot_walk_k(uint64_t nblocks, uint32_t nseg, const Status* __restrict__ st, int it, const uint8_t* __restrict__ inc,
+                                 const uint8_t* __restrict__ cm_old, uint8_t* __restrict__ cm_new, const uint32_t* __restrict__ in_state,
+                                 const uint32_t* __restrict__ gin, ProtShard* __restrict__ ps, uint32_t* __restrict__ words) {
+    if (!gate_open(st)) return;
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nseg || gin[ngrp] == PC_ESC) return;
+    Protection p; pc_decode(in_state[s], p);
+    const uint64_t b0 = (uint64_t)s * PSEG, b1 = (b0 + PSEG < nblocks) ? b0 + PSEG : nblocks;
+    p.counter = ps->first_block + b0;
+    prot_walk(p, inc, b0, b1, cm_new);
+    uint32_t nd = 0;
+    for (uint64_t b = b0; b < b1; ++b) nd += cm_new[b] != (it ? cm_old[b] : 0);
+    if (nd) {
+        atomicAdd(&words[0], nd);
+        if (it < 16) atomicAdd(&ps->changed[it], nd);
+    }
+}
+
+__device__ __forceinline__ void prot_round_verdict(const uint32_t* all_words, uint32_t world, bool& changed, bool& esc) {
+    changed = false; esc = false;
+    for (uint32_t r = 0; r < world; ++r) { changed |= all_words[4 * r] != 0; esc |= all_words[4 * r + 1] != 0; }
+}
+// the global commit of a round, 1: cm_old <- cm_new unless the map settled (as prot_iterate step 4; round 0 always commits)
+__global__ void cham_prot_commit_k(const uint32_t* __restrict__ all_words, uint32_t world, uint64_t nblocks, const Status* __restrict__ st, int it,
+                                   uint8_t* __restrict__ cm_old, const uint8_t* __restrict__ cm_new) {
+    if (!gate_open(st)) return;
+    bool changed, esc;
+    prot_round_verdict(all_words, world, changed, esc);
+    if (esc || !(changed || it == 0)) return;
+    for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nblocks; b += (uint64_t)gridDim.x * blockDim.x) cm_old[b] = cm_new[b];
+}
+// 2: the verdict closes the gate of every later kernel when the map has settled, or when a path met PC_ESC (the shard is then refused)
+__global__ void cham_prot_verdict_k(const uint32_t* __restrict__ all_words, uint32_t world, Status* __restrict__ st, int it, ProtShard* __restrict__ ps) {
+    if (threadIdx.x || blockIdx.x || !gate_open(st)) return;
+    bool changed, esc;
+    prot_round_verdict(all_words, world, changed, esc);
+    if (esc) { ps->esc = 1; st->converged = 1; }
+    else if (!changed) { ps->settled = 1; ps->rounds = (uint32_t)it + 1; st->converged = 1; }
+}
+// finish: a shard whose iteration did not settle is refused (nothing is emitted: cham_emit returns on an error)
+__global__ void cham_prot_finish_k(Status* __restrict__ st, const ProtShard* __restrict__ ps) {
+    if (threadIdx.x || blockIdx.x) return;
+    if (!ps->settled) st->error = PROT_REFUSED;
+}
+// the seam words of the layout of cham_seam_words_k: incompressible blocks may meet at a cut here, so words 0 and 1 stay 0; word 2 = refused
+// or error (the size is then 0)
+__global__ void cham_prot_seam_words_k(uint64_t nblocks, const Status* __restrict__ st, uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
+    if (threadIdx.x || blockIdx.x) return;
+    const uint64_t sz = (nblocks && !st->error) ? *d_out_size : 0;
+    *d_out_size = sz;
+    words[0] = 0; words[1] = 0; words[2] = st->error ? 1u : 0u; words[3] = nblocks ? 1u : 0u;
+    words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
+}
+
 }  // namespace cham
 
 // ------------------------------------------------------------------------------------------------------
@@ -1521,6 +1692,117 @@ cudaError_t cham_encode_protected_only(const uint8_t* d_in, size_t nbytes, uint8
     cham_emit<false><<<ntiles, EM_THREADS, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, nblocks, sigw, copymap, 0, st,
                                                         reinterpret_cast<uint32_t*>(ws + L.tile_local),
                                                         reinterpret_cast<uint64_t*>(ws + L.group_off), d_out);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// ---- sharded copy-map iteration (see cham_prot_start_k) --------------------------------------------------------------------------------
+// The segment states and candidate tables sit in the seg_state region, in prot_iterate's layout: in_state [nseg + 1], out_state [nseg + 1]
+// (unused here), then gin [ngrp + 2] (as u32), T [nseg][PC_NC], GT [ngrp][PC_NC] (u16).
+struct ProtPtrs { uint32_t* in_state; uint32_t* gin; uint16_t* T; uint16_t* GT; };
+static ProtPtrs prot_ptrs(uint8_t* ws, const ChamLayout& L, uint32_t nseg) {
+    uint32_t* seg_state = reinterpret_cast<uint32_t*>(ws + L.seg_state);
+    uint16_t* ptab = reinterpret_cast<uint16_t*>(seg_state + 2 * (nseg + 1));
+    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    ProtPtrs p;
+    p.in_state = seg_state;
+    p.gin = reinterpret_cast<uint32_t*>(ptab);
+    p.T = ptab + 2 * (ngrp + 2);
+    p.GT = p.T + (size_t)nseg * PC_NC;
+    return p;
+}
+
+cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
+                            cudaStream_t stream, uint64_t* launches) {
+    cham_prot_start_k<<<1, 32, 0, stream>>>(reinterpret_cast<Status*>(ws + L.status), ps, first_block, d_lengths, rank);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t* launches) {
+    cham_put_u64_k<<<1, 32, 0, stream>>>(d, v);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
+                               int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches) {
+    const uint64_t nblocks = (nbytes + 255) / 256;
+    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
+    const uint32_t nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG), ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    const Status* st = reinterpret_cast<const Status*>(ws + L.status);
+    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
+    const ProtPtrs p = prot_ptrs(ws, L, nseg);
+    if (nblocks) {
+        cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), d_carry_in, 0, nruns,
+                                                        reinterpret_cast<uint32_t*>(ws + L.carry), nullptr, st);
+        cham_resolve<<<dim3(32, nruns), 256, 0, stream>>>(reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
+                                                         reinterpret_cast<uint32_t*>(ws + L.carry), ntiles, nruns, sigw, st);
+        cham_prot_seg_k<<<nseg < 2048u ? nseg : 2048u, PSEG, 0, stream>>>(sigw, nbytes, nblocks, nseg, st, it, ws + L.incb, ws + L.copymap, ps, p.T);
+        cham_prot_groups_k<<<(ngrp * PC_NC + 255) / 256, 256, 0, stream>>>(nseg, st, p.T, p.GT);
+        *launches += 4;
+    }
+    cham_prot_transfer_k<<<1, 256, 0, stream>>>(nseg, st, p.GT, d_transfer_out);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
+                             uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
+    const uint64_t nblocks = (nbytes + 255) / 256;
+    const uint32_t nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG), ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+    const Status* st = reinterpret_cast<const Status*>(ws + L.status);
+    const ProtPtrs p = prot_ptrs(ws, L, nseg);
+    cham_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, nseg, st, p.GT, p.gin, ps, d_words);
+    ++*launches;
+    if (nseg) {
+        cham_prot_seams_k<<<(ngrp + 127) / 128, 128, 0, stream>>>(nseg, st, p.T, p.gin, p.in_state);
+        cham_prot_walk_k<<<(nseg + 127) / 128, 128, 0, stream>>>(nblocks, nseg, st, it, ws + L.incb, ws + L.copymap, ws + L.copymap2, p.in_state,
+                                                                 p.gin, ps, d_words);
+        *launches += 2;
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
+                           const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches) {
+    const uint64_t nblocks = (nbytes + 255) / 256;
+    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
+    Status* st = reinterpret_cast<Status*>(ws + L.status);
+    if (nblocks) {
+        cham_prot_commit_k<<<(uint32_t)((nblocks + 1023) / 1024 < 1024 ? (nblocks + 1023) / 1024 : 1024), 256, 0, stream>>>(
+            d_all_words, world, nblocks, st, it, ws + L.copymap, ws + L.copymap2);
+        ++*launches;
+    }
+    cham_prot_verdict_k<<<1, 32, 0, stream>>>(d_all_words, world, st, it, ps);
+    ++*launches;
+    if (d_table_out) {
+        if (nblocks) {   // round it + 1: flags under the new map (copy-mode blocks hidden from the dictionary) and the shard's table
+            cudaError_t e = set_smem_attrs_once();
+            if (e != cudaSuccess) return e;
+            launch_flag_pass(nruns, stream, reinterpret_cast<const uint32_t*>(d_in), nbytes / 4, ntiles, reinterpret_cast<uint32_t*>(ws + L.sigw),
+                             reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
+                             reinterpret_cast<uint32_t*>(ws + L.final_tab), ws + L.copymap, st);
+            cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), nullptr, 1, nruns, nullptr,
+                                                            d_table_out, st);
+            *launches += 2;
+        } else {
+            cudaError_t e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), stream);   // nothing touched
+            if (e != cudaSuccess) return e;
+        }
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
+                             uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
+    const uint64_t nblocks = (nbytes + 255) / 256;
+    Status* st = reinterpret_cast<Status*>(ws + L.status);
+    cham_prot_finish_k<<<1, 32, 0, stream>>>(st, ps);
+    ++*launches;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && nblocks) e = cham_phase2_finish(d_in, nbytes, ws, L, d_out, cap, d_out_size, true, stream, launches, ev, false);
+    if (e != cudaSuccess) return e;
+    cham_prot_seam_words_k<<<1, 32, 0, stream>>>(nblocks, st, d_out_size, d_seam8);
     ++*launches;
     return cudaGetLastError();
 }

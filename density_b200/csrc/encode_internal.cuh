@@ -138,4 +138,29 @@ cudaError_t cham_seam_verdict(const uint32_t* d_all_words, uint32_t world, uint3
                               cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_table_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 
+// sharded copy-map iteration (density_b200_shard_prot_*): one shard of a longer stream. The shard's record lives in device memory.
+struct ProtShard {
+    unsigned long long first_block;   // global index of the shard's first block
+    uint32_t rounds;                  // rounds run until the map settled (0: not settled)
+    uint32_t settled, in_state, esc;  // in_state: pc_encode candidate of the true incoming state of the last round (0xFFFF: PC_ESC)
+    uint32_t changed[16];             // blocks of this shard whose copy status changed, per round
+};
+constexpr uint32_t PROT_TRANSFER_WORDS = 200, PROT_ROUND_WORDS = 4, PROT_MAX_ROUNDS = 16;
+// start: after cham_encode_phase1 (round 0's flags); first_block, or the sum of lengths[0 .. rank) / 256 when d_lengths is set
+cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
+                            cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t* launches);   // *d = v in stream order
+// round `it`: resolve the flags against the carry-in (NULL = stream start), export the transfer (PROT_TRANSFER_WORDS u32)
+cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
+                               int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches);
+// compose the gathered transfers of the shards before `rank`, walk, compare: PROT_ROUND_WORDS u32 to d_words
+cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
+                             uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+// the global commit of round `it` from the gathered round words; with d_table_out, round it + 1's flags under the new map and its table
+cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
+                           const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches);
+// sizes under the copy map, scan, emit, 8 seam words (word 2: refused or error); ev as cham_encode_phase2
+cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
+                             uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev = nullptr);
+
 }  // namespace dns

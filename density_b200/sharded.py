@@ -9,6 +9,10 @@ The concatenation of the per-rank outputs is byte-identical to one chameleon_enc
 the protection automaton stays quiet (flags bit 0 reports otherwise). Outputs stay where they were produced; a caller
 that wants them on one rank gathers them with the sizes returned here.
 
+Input on which the protection automaton fires (copy mode) goes through ShardedChameleonEncoder.encode_protected or
+ShardedEncoder.encode_protected instead: the copy-map iteration runs over all ranks, every round exchanging the tables, each rank's
+automaton transfer (compose_prot_transfers is its numpy twin) and 4 round words, for a fixed budget of rounds.
+
 Decode is the mirror image: rank r decodes its piece back into its shard with the same table exchange and fold. The decode
 phase 1 (boundaries, writer pass) needs no carry-in and exports the piece's table; phase 2 decodes from the folded carry-in
 and writes 8 seam words, which every rank gathers and judges with `seam_verdict`.
@@ -99,6 +103,41 @@ def seam_verdict(words):
     return int(bad), int(offsets[-1]), offsets
 
 
+PROT_TRANSFER_WORDS = 200  # DENSITY_B200_PROT_TRANSFER_WORDS: candidate states of the protection automaton
+PROT_ROUND_WORDS = 4       # DENSITY_B200_PROT_ROUND_WORDS
+PROT_STATUS_WORDS = 20     # DENSITY_B200_PROT_STATUS_WORDS
+PROT_ESC = 0xFFFF          # a path that left the candidate states
+_PC_NS, _PC_NP = 10, 10    # candidate starts 1..10, penalties 0..9 (chameleon_encode.cu: PC_NS, PC_NP)
+
+
+def prot_candidate(state):
+    """(penalty, start, previous_incompressible) -> the candidate index of a transfer entry (pc_encode), PROT_ESC outside the set."""
+    p, s, prev = state
+    if p >= _PC_NP or s < 1 or s > _PC_NS:
+        return PROT_ESC
+    return (int(prev) * _PC_NS + (s - 1)) * _PC_NP + p
+
+
+def prot_state(c):
+    """The inverse of prot_candidate (pc_decode); None for PROT_ESC."""
+    if c == PROT_ESC:
+        return None
+    return (c % _PC_NP, (c // _PC_NP) % _PC_NS + 1, c // (_PC_NP * _PC_NS))
+
+
+def compose_prot_transfers(transfers, rank):
+    """The numpy twin of cham_prot_enter_k's composition: the candidate state entering shard `rank`, the transfers of shards < rank
+    (int [world, PROT_TRANSFER_WORDS], entry c = candidate at the shard end when entered in candidate c, or PROT_ESC) applied in order
+    to the stream-start state (candidate 0). PROT_ESC once a path leaves the candidates."""
+    t = np.asarray(transfers).astype(np.int64) & 0xFFFFFFFF
+    x = 0
+    for r in range(rank):
+        if x == PROT_ESC:
+            break
+        x = int(t[r, x])
+    return x
+
+
 LOCATE_MAP_WORDS = 266     # DENSITY_B200_LOCATE_MAP_WORDS
 CHEETAH_LOCATE_MAP_WORDS = 142   # DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS
 CHUNK = 16384              # non-last ranges are multiples of the boundary walk's chunk
@@ -150,6 +189,62 @@ class ShardedChameleonEncoder:
             self.close()
         except Exception:
             pass
+
+    def encode_protected(self, d_in, d_out, d_size, group=None):
+        """The copy-mode path (density_b200_shard_prot_*): d_in / d_out / d_size as in encode, any input. Runs the round budget of the
+        copy-map iteration with torch.distributed exchanges (tables, transfers, round words) and the device folds. Returns
+        seam_verdict's (flags, total, offsets) over all ranks; flags != 0 only when the map did not settle, the automaton left the
+        candidate states, or on an error: the pieces are then void."""
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        dev = d_in.device
+        lib = self._lib
+
+        def gather(t):
+            if world == 1:
+                return t.view(1, -1)
+            out = torch.empty((world, t.numel()), dtype=t.dtype, device=dev)
+            dist.all_gather_into_tensor(out.view(-1), t.contiguous(), group=group)
+            return out
+
+        def check(rc, what):
+            if rc:
+                raise _lib.DensityB200Error(f"shard_prot_{what} rc={rc}: {_lib.last_error()}")
+
+        n = d_in.numel()
+        first_block = int(gather(torch.tensor([n], dtype=torch.int64, device=dev))[:rank].sum()) // 256
+        table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=dev)
+        transfer = torch.empty(PROT_TRANSFER_WORDS, dtype=torch.int32, device=dev)
+        words = torch.empty(PROT_ROUND_WORDS, dtype=torch.int32, device=dev)
+        check(lib.density_b200_shard_prot_phase1(self._h, d_in.data_ptr(), n, first_block, int(rank == world - 1), table.data_ptr(),
+                                                 stream), "phase1")
+        all_words = None
+        for k in range(lib.density_b200_prot_round_budget()):
+            if k:
+                check(lib.density_b200_shard_prot_next(self._h, all_words.data_ptr(), world, table.data_ptr(), stream), "next")
+            carry = fold_tables(gather(table), rank).contiguous()
+            check(lib.density_b200_shard_prot_transfer(self._h, carry.data_ptr(), transfer.data_ptr(), stream), "transfer")
+            all_transfers = gather(transfer).contiguous()
+            check(lib.density_b200_shard_prot_settle(self._h, all_transfers.data_ptr(), world, rank, words.data_ptr(), stream), "settle")
+            all_words = gather(words).contiguous()
+        check(lib.density_b200_shard_prot_next(self._h, all_words.data_ptr(), world, None, stream), "next")
+        seam = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
+        check(lib.density_b200_shard_prot_finish(self._h, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), seam.data_ptr(), stream),
+              "finish")
+        return seam_verdict(gather(seam))
+
+    def prot_status(self):
+        """density_b200_shard_prot_status after encode_protected (waits for the device): dict with rounds (until settled, 0: not
+        settled), settled, in_state ((penalty, start, previous_incompressible) entering the shard, None: left the candidates), esc and
+        changed (this shard's blocks whose copy status changed, per round, 16 values)."""
+        out = (ctypes.c_uint32 * PROT_STATUS_WORDS)()
+        rc = self._lib.density_b200_shard_prot_status(self._h, out)
+        if rc:
+            raise _lib.DensityB200Error(f"shard_prot_status rc={rc}: {_lib.last_error()}")
+        v = list(out)
+        ins = None if v[2] == 0xFFFFFFFF else (v[2] & 0xFF, (v[2] >> 8) & 0xFF, v[2] >> 16)
+        return {"rounds": v[0], "settled": v[1], "in_state": ins, "esc": v[3], "changed": v[4:20]}
 
     def encode(self, d_in, d_out, d_size, d_flags, group=None):
         """d_in / d_out: CUDA uint8 tensors (this rank's shard / its output buffer); d_size: int64[1]; d_flags: int32[1].
@@ -433,6 +528,17 @@ class ShardedEncoder(_ShardedHandle):
             rc = self._lib.density_b200_encode_sharded_cl(self._h, alg, *args)
         if rc:
             raise _lib.DensityB200Error(f"encode_sharded{'' if alg == 0 else '_cl'} rc={rc}: {_lib.last_error()}")
+
+    def encode_protected(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None):
+        """density_b200_encode_sharded_protected: Chameleon with copy mode, the arguments of encode. d_flags != 0 only when the copy map
+        did not settle within the round budget, the automaton left the candidate states, or on an error: the pieces are then void."""
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rc = self._lib.density_b200_encode_sharded_protected(
+            self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
+            self.d_total.data_ptr(), int(gather_root), d_gather.data_ptr() if d_gather is not None else None,
+            d_gather.numel() if d_gather is not None else 0, stream)
+        if rc:
+            raise _lib.DensityB200Error(f"encode_sharded_protected rc={rc}: {_lib.last_error()}")
 
     def profile(self):
         """stage times (ms) of the last encode: Chameleon flag pass, table exchange + fold, carry / resolve / sizes / scan, emit, seams +

@@ -143,7 +143,8 @@ DENSITY_B200_API int density_b200_table_fold(uint32_t* d_acc, const uint32_t* d_
  *                                    (ncclAllGather of 32 bytes per rank: first / last block incompressible, quiet, size) -> optional
  *                                    variable-length gather of the pieces to `gather_root` (grouped ncclSend / ncclRecv at prefix-sum
  *                                    offsets). *d_flags != 0: the stream is not quiet (a copy-mode block somewhere, or two incompressible
- *                                    blocks across a cut): the pieces are void and the caller encodes on one device instead.
+ *                                    blocks across a cut): the pieces are void and the caller encodes on one device instead, or
+ *                                    with density_b200_encode_sharded_protected below, which accepts such input.
  *                                    *d_total_size = length of the whole stream, on every rank. gather_root < 0: no gather, nothing blocks.
  */
 typedef struct density_b200_sharded density_b200_sharded; /* opaque */
@@ -154,8 +155,71 @@ DENSITY_B200_API int density_b200_encode_sharded(density_b200_sharded*, const ui
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream);
 /* stage times (ms) of the last encode_sharded or encode_sharded_cl call. Chameleon: [0] flag pass, [1] table exchange + fold, [2] carry /
    resolve / sizes / scan, [3] emit, [4] seams + gather. Cheetah / Lion: [0] phase 1, [1] P exchange + fold, [2] phase 2 + C exchange +
-   fold, [3] phase 3, [4] seams + gather. */
+   fold, [3] phase 3, [4] seams + gather. encode_sharded_protected: [0] phase 1, [1] the first table exchange + fold, [2] the rounds, sizes
+   and scan, [3] emit, [4] seams + gather. */
 DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* out_ms5);
+
+/*
+ * Sharded Chameleon encode with copy mode (DESIGN.md section 5): the quiet-only paths above refuse any input on which the protection
+ * automaton fires (two incompressible blocks in a row anywhere: 512 bytes of compressed or random data). This path accepts it. The copy
+ * map is the fixed point the single-device encoder iterates (flags under the map -> incompressible bits -> automaton -> new map); here
+ * every round runs on all shards at once, with the dictionary and the automaton state carried over the cuts, so the shards compute the
+ * single-device sequence of maps exactly. Shard r holds bytes [o_r, o_r + n_r) of one input, every non-final shard a multiple of 256
+ * bytes; its first global block is o_r / 256. The concatenation of the pieces equals one chameleon_encode call over the whole input,
+ * byte for byte, whenever the verdict is 0. Copy-mode blocks, penalties pending at a cut and incompressible pairs across a cut are all
+ * accepted. The verdict is non-zero (the pieces are void; nothing is written past `cap`) only when the map did not settle within the
+ * round budget, when the automaton's true path left the candidate states (penalty < 10, start 1..10: never seen on real data), or on an
+ * error (capacity).
+ *
+ * Phase API on a density_b200_shard handle (any transport; W shards may run on one GPU). Per round k = 0, 1, ...:
+ *   flags      k = 0: prot_phase1; k > 0: prot_next with a table. Exports the shard's last-writer table under the round's map.
+ *   exchange   the tables of all shards; the carry-in of shard r is density_b200_table_init folded with the tables of shards < r.
+ *   transfer   prot_transfer: DENSITY_B200_PROT_TRANSFER_WORDS u32, entry c = the automaton state at the shard end when the shard is
+ *              entered in candidate state c (c = (previous_incompressible * 10 + start - 1) * 10 + penalty), or 0xFFFF.
+ *   exchange   the transfers of all shards, in rank order.
+ *   settle     prot_settle: the true incoming state (the transfers of shards < rank composed from c = 0, the stream start), the new
+ *              copy map of the shard, and DENSITY_B200_PROT_ROUND_WORDS round words {blocks whose copy status changed, met 0xFFFF,
+ *              settled before this round, 0}.
+ *   exchange   the round words of all shards, in rank order; then prot_next: the global commit (settled when no shard changed and
+ *              none met 0xFFFF: every later kernel returns at once), and with a table the next round's flags.
+ * After the last round prot_next without a table commits it, and prot_finish emits. Every shard runs the same number of rounds; at
+ * most density_b200_prot_round_budget() (prot_next with a table returns DENSITY_B200_EARG beyond it). Phases called out of order,
+ * misaligned pointers (d_in and tables 4-byte, d_out 2-byte) and a non-final shard that is not a multiple of 256 bytes return
+ * DENSITY_B200_EARG without enqueuing anything.
+ */
+#define DENSITY_B200_PROT_TRANSFER_WORDS 200
+#define DENSITY_B200_PROT_ROUND_WORDS 4
+#define DENSITY_B200_PROT_STATUS_WORDS 20
+/* rounds of the iteration (16; density_b200_test_set_prot_rounds lowers it) */
+DENSITY_B200_API int density_b200_prot_round_budget(void);
+/* round 0: flags with unknown carry-in, the last-writer table (as density_b200_shard_phase1) to d_table_out. d_in must stay valid and
+   unchanged until prot_finish has been enqueued. */
+DENSITY_B200_API int density_b200_shard_prot_phase1(density_b200_shard*, const uint8_t* d_in, size_t n, uint64_t first_block, int is_last_shard,
+                                   uint32_t* d_table_out, void* stream);
+/* d_carry_in: the dictionary before this shard under the round's map (NULL = stream start) */
+DENSITY_B200_API int density_b200_shard_prot_transfer(density_b200_shard*, const uint32_t* d_carry_in, uint32_t* d_transfer_out, void* stream);
+DENSITY_B200_API int density_b200_shard_prot_settle(density_b200_shard*, const uint32_t* d_all_transfers, int world, int rank,
+                                   uint32_t* d_words_out, void* stream);
+/* d_table_out NULL: commit the last round (then prot_finish) */
+DENSITY_B200_API int density_b200_shard_prot_next(density_b200_shard*, const uint32_t* d_all_words, int world, uint32_t* d_table_out, void* stream);
+/* sizes under the copy map, scan, emit: the piece to d_out, its size to *d_out_size (0 when refused) and 8 seam words to d_seam8 in the
+   layout of density_b200_decode_shard_phase2 (words 0 and 1 are 0: incompressible blocks may meet at a cut; word 2 = refused or error).
+   The verdict over all shards is cham_seam_verdict's rule: non-zero when any word 2 is set. */
+DENSITY_B200_API int density_b200_shard_prot_finish(density_b200_shard*, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
+                                   void* stream);
+/* after the last commit (waits for the device): out[0] rounds until the map settled (0: not settled), [1] settled, [2] the incoming state
+   of the last round run, penalty | start << 8 | previous_incompressible << 16 (~0: left the candidates), [3] met 0xFFFF, [4 + k] this
+   shard's blocks whose copy status changed in round k (k < 16) */
+DENSITY_B200_API int density_b200_shard_prot_status(density_b200_shard*, uint32_t* out20);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments and gather semantics of density_b200_encode_sharded: an
+   ncclAllGather of the shard lengths (the first global block) -> phase 1 -> the round budget of {ncclAllGather(tables) -> fold kernel ->
+   transfer -> ncclAllGather(transfers, 800 bytes per rank) -> settle -> ncclAllGather(round words, 16 bytes) -> commit} -> finish ->
+   seam verdict -> optional gather. Uses its own shard state in the handle; nothing blocks unless gather_root >= 0. Bad arguments
+   (d_in 4-byte, d_out 2-byte, d_out_size and d_total_size 8-byte, d_flags 4-byte aligned; a non-final shard a multiple of 256 bytes)
+   return DENSITY_B200_EARG before any collective is enqueued. */
+DENSITY_B200_API int density_b200_encode_sharded_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                          uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
+                                          uint8_t* d_gather, size_t gather_cap, void* stream);
 
 /*
  * Sharded Cheetah / Lion encode (one bit-exact stream cut across several GPUs / calls; DESIGN.md section 5). Shard r holds bytes
@@ -413,6 +477,9 @@ DENSITY_B200_API void density_b200_test_set_stage_rounds(int k);
 /* Test hook: cut the round budget of the sharded Cheetah decode to k rounds (1..40, default 40) so that its "did not settle" refusal
    can be exercised. density_b200_decode_device does not read it. */
 DENSITY_B200_API void density_b200_test_set_decode_rounds(int k);
+/* Test hook: cut the round budget of the sharded copy-map iteration (density_b200_shard_prot_*, density_b200_encode_sharded_protected)
+   to k rounds (1..16, default 16) so that its "did not settle" refusal can be exercised. The single-device encoder does not read it. */
+DENSITY_B200_API void density_b200_test_set_prot_rounds(int k);
 /* Diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed
    (~0: none), number of such blocks}: 16 rounds x 2 values. Synchronises the device. */
 DENSITY_B200_API int density_b200_prot_debug(uint64_t* out32);

@@ -33,6 +33,17 @@ static void set_error(const char* what, cudaError_t e) {
     g_last_error = buf;
 }
 static void set_error(const char* what) { g_last_error = what; }
+// the end of an enqueued step: its kernel launches are counted, and a CUDA error becomes DENSITY_B200_ECUDA with `what` as the message
+static int step_result(cudaError_t e, uint64_t launches, const char* what) {
+    g_launches += launches;
+    if (e != cudaSuccess) { set_error(what, e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+// the outputs of an empty piece of a sharded stream: size 0, and seam words that say it has no blocks
+static cudaError_t empty_piece_outputs(uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st) {
+    const cudaError_t e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
+    return e == cudaSuccess ? cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st) : e;
+}
 
 // grow-only device buffer
 struct DevBuf {
@@ -341,9 +352,7 @@ static int encode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
         e = scalar_encode(alg, d_in, n, d_out, cap, c->ws.p, d_out_size, stream, &launches);
         c->last_was_chameleon_fastpath_capable = 0;
     }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("encode launch", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    return step_result(e, launches, "encode launch");
 }
 
 // path: 0 auto (parallel decoder with exact in-order fallback), 1 parallel only, 3 in-order kernel only
@@ -370,9 +379,7 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
         e = cham_decode_parallel(d_in, n, d_out, cap, c->ws.p, c->num_sms, d_out_size, d_nonquiet, stream, &launches);
         if (e == cudaSuccess && path != 1)
             e = scalar_decode(alg, d_in, n, d_out, cap, c->ws.p + pw + 256, d_out_size, stream, &launches, d_nonquiet);
-        g_launches += launches;
-        if (e != cudaSuccess) { set_error("decode launch", e); return DENSITY_B200_ECUDA; }
-        return DENSITY_B200_OK;
+        return step_result(e, launches, "decode launch");
     }
     if (alg == ALG_CHEETAH && path != 3 && !(reinterpret_cast<uintptr_t>(d_in) & 1) && !(reinterpret_cast<uintptr_t>(d_out) & 3)) {
         // run-parallel Cheetah decoder (cl_decode.cu) + in-order tail; the exact in-order kernel is queued behind it and only runs if
@@ -394,16 +401,12 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
         }
         if (e == cudaSuccess && path != 1)
             e = scalar_decode(alg, d_in, n, d_out, cap, scalar_ws, d_out_size, stream, &launches, d_fallback);
-        g_launches += launches;
-        if (e != cudaSuccess) { set_error("decode launch", e); return DENSITY_B200_ECUDA; }
-        return DENSITY_B200_OK;
+        return step_result(e, launches, "decode launch");
     }
     e = c->ws.ensure(scalar_workspace_bytes(alg), stream);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     e = scalar_decode(alg, d_in, n, d_out, cap, c->ws.p, d_out_size, stream, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("decode launch", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    return step_result(e, launches, "decode launch");
 }
 
 // Host-pointer Chameleon encode, pipelined over PCIe: the input is cut into chunks that are treated as shards of one
@@ -609,7 +612,6 @@ struct density_b200_shard {
     const uint8_t* d_in = nullptr;
     size_t n = 0;
     uint32_t nruns = 0;
-    int is_last = 1;
     int num_sms = 0;
     bool phase1_done = false;
     // the copy-map iteration of density_b200_shard_prot_*: the shard's device record and where the phases stand
@@ -618,14 +620,18 @@ struct density_b200_shard {
     int round = 0;
 };
 
-density_b200_shard* density_b200_shard_create(void) {
+// a phase object of the sharded API for the current device (NULL, with the error set, without one)
+extern "C++" {
+template <class S> static S* new_shard() {
     g_last_error.clear();
     DeviceCtx* c = current_ctx();
     if (!c) return nullptr;
-    density_b200_shard* s = new density_b200_shard();
+    S* s = new S();
     s->num_sms = c->num_sms;
     return s;
 }
+}
+density_b200_shard* density_b200_shard_create(void) { return new_shard<density_b200_shard>(); }
 void density_b200_shard_destroy(density_b200_shard* s) {
     if (!s) return;
     s->ws.release();
@@ -637,39 +643,43 @@ int density_b200_shard_phase1(density_b200_shard* s, const uint8_t* d_in, size_t
     if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
     if (reinterpret_cast<uintptr_t>(d_in) & 3) { set_error("d_in must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->prot_phase = 0;              // the workspace is this phase's now: the copy-map phases start over with prot_phase1
     size_t need = cham_workspace_bytes(n, s->num_sms, &s->L);
-    cudaError_t e = s->ws.ensure(need);
+    cudaError_t e = s->ws.ensure(need, st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->is_last = is_last_shard; s->nruns = cham_pick_runs(n, s->num_sms);
+    s->d_in = d_in; s->n = n; s->nruns = cham_pick_runs(n, s->num_sms);
     uint64_t launches = 0;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (n == 0) {
         e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
     } else {
         e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, d_table_out, st, &launches);
     }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard phase1", e); return DENSITY_B200_ECUDA; }
-    s->phase1_done = true;
-    return DENSITY_B200_OK;
+    const int rc = step_result(e, launches, "shard phase1");
+    if (rc == DENSITY_B200_OK) s->phase1_done = true;
+    return rc;
+}
+// phase 2 on the shard's workspace: carry-in, first-touch flags, sizes, scan, emit. assume_prev_inc: the block before the shard counts
+// as incompressible; ev (may be NULL): the stage events of cham_encode_phase2.
+static int shard_phase2_impl(density_b200_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                             bool assume_prev_inc, cudaEvent_t* ev, cudaStream_t st) {
+    uint64_t launches = 0;
+    const cudaError_t e = cham_encode_phase2(s->d_in, s->n, s->ws.p, s->L, s->nruns, d_carry_in, d_out, cap, d_out_size, false,
+                                             assume_prev_inc, st, &launches, ev);
+    return step_result(e, launches, "shard phase2");
 }
 int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                               uint32_t* d_flags, void* stream) {
     g_last_error.clear();
     if (!s || !s->phase1_done || !d_out_size) { set_error("shard_phase2: phase1 not done / null pointer"); return DENSITY_B200_EARG; }
     if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    cudaError_t e = cham_encode_phase2(s->d_in, s->n, s->ws.p, s->L, s->nruns, d_carry_in, d_out, cap, d_out_size, false,
-                                       d_carry_in != nullptr, st, &launches, nullptr);
-    if (e == cudaSuccess && d_flags) {
-        if (s->n) e = cudaMemcpyAsync(d_flags, s->ws.p + s->L.status + offsetof(Status, nonquiet), sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
-        else e = cudaMemsetAsync(d_flags, 0, sizeof(uint32_t), st);
-    }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard phase2", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const int rc = shard_phase2_impl(s, d_carry_in, d_out, cap, d_out_size, d_carry_in != nullptr, nullptr, st);
+    if (rc != DENSITY_B200_OK || !d_flags) return rc;
+    const cudaError_t e = s->n ? cudaMemcpyAsync(d_flags, s->ws.p + s->L.status + offsetof(Status, nonquiet), sizeof(uint32_t),
+                                                 cudaMemcpyDeviceToDevice, st)
+                               : cudaMemsetAsync(d_flags, 0, sizeof(uint32_t), st);
+    return step_result(e, 0, "shard phase2");
 }
 
 // ---- sharded Chameleon encode with copy mode: the copy-map iteration carried over the cuts ---------------------------------------------
@@ -689,55 +699,17 @@ static int prot_phase1_impl(density_b200_shard* s, const uint8_t* d_in, size_t n
     cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);
     if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->is_last = is_last_shard; s->nruns = cham_pick_runs(n, s->num_sms);
+    s->d_in = d_in; s->n = n; s->nruns = cham_pick_runs(n, s->num_sms);
     s->phase1_done = false; s->prot_phase = 0; s->round = 0;
     uint64_t launches = 0;
     e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, n ? d_table_out : nullptr, st, &launches);
     if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);   // nothing touched
     if (e == cudaSuccess) e = cham_prot_start(s->ws.p, s->L, prot_rec(s), d_lengths ? 0 : first_block, d_lengths, (uint32_t)rank, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard prot phase1", e); return DENSITY_B200_ECUDA; }
-    s->prot_phase = 1;
-    return DENSITY_B200_OK;
+    const int rc = step_result(e, launches, "shard prot phase1");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 1;
+    return rc;
 }
-static int prot_transfer_impl(density_b200_shard* s, const uint32_t* d_carry_in, uint32_t* d_transfer_out, cudaStream_t st) {
-    if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 1) { set_error("shard_prot_transfer: call it after prot_phase1 or prot_next with a table"); return DENSITY_B200_EARG; }
-    if (!al4(d_carry_in) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    cudaError_t e = cham_prot_transfer(s->n, s->ws.p, s->L, s->nruns, d_carry_in, prot_rec(s), s->round, d_transfer_out, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard prot transfer", e); return DENSITY_B200_ECUDA; }
-    s->prot_phase = 2;
-    return DENSITY_B200_OK;
-}
-static int prot_settle_impl(density_b200_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out, cudaStream_t st) {
-    if (!s || !d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 2) { set_error("shard_prot_settle: call it after prot_transfer"); return DENSITY_B200_EARG; }
-    if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    cudaError_t e = cham_prot_settle(s->n, s->ws.p, s->L, prot_rec(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard prot settle", e); return DENSITY_B200_ECUDA; }
-    s->prot_phase = 3;
-    return DENSITY_B200_OK;
-}
-static int prot_next_impl(density_b200_shard* s, const uint32_t* d_all_words, int world, uint32_t* d_table_out, cudaStream_t st) {
-    if (!s || !d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 3) { set_error("shard_prot_next: call it after prot_settle"); return DENSITY_B200_EARG; }
-    if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_words) || !al4(d_table_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    if (d_table_out && s->round + 1 >= g_prot_rounds) { set_error("shard_prot_next: the round budget is used up"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    cudaError_t e = cham_prot_next(s->d_in, s->n, s->ws.p, s->L, s->nruns, prot_rec(s), s->round, d_all_words, (uint32_t)world, d_table_out, st,
-                                   &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard prot next", e); return DENSITY_B200_ECUDA; }
-    if (d_table_out) { ++s->round; s->prot_phase = 1; }
-    else s->prot_phase = 4;
-    return DENSITY_B200_OK;
-}
+// ev (may be NULL): the stage events of cham_encode_phase2
 static int prot_finish_impl(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st,
                             cudaEvent_t* ev) {
     if (!s || (!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
@@ -746,11 +718,10 @@ static int prot_finish_impl(density_b200_shard* s, uint8_t* d_out, size_t cap, u
         set_error("d_out must be 2-byte, d_out_size 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG;
     }
     uint64_t launches = 0;
-    cudaError_t e = cham_prot_finish(s->d_in, s->n, s->ws.p, s->L, prot_rec(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("shard prot finish", e); return DENSITY_B200_ECUDA; }
-    s->prot_phase = 5;
-    return DENSITY_B200_OK;
+    const cudaError_t e = cham_prot_finish(s->d_in, s->n, s->ws.p, s->L, prot_rec(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev);
+    const int rc = step_result(e, launches, "shard prot finish");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 5;
+    return rc;
 }
 
 int density_b200_shard_prot_phase1(density_b200_shard* s, const uint8_t* d_in, size_t n, uint64_t first_block, int is_last_shard,
@@ -761,15 +732,44 @@ int density_b200_shard_prot_phase1(density_b200_shard* s, const uint8_t* d_in, s
 }
 int density_b200_shard_prot_transfer(density_b200_shard* s, const uint32_t* d_carry_in, uint32_t* d_transfer_out, void* stream) {
     g_last_error.clear();
-    return prot_transfer_impl(s, d_carry_in, d_transfer_out, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 1) { set_error("shard_prot_transfer: call it after prot_phase1 or prot_next with a table"); return DENSITY_B200_EARG; }
+    if (!al4(d_carry_in) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cham_prot_transfer(s->n, s->ws.p, s->L, s->nruns, d_carry_in, prot_rec(s), s->round, d_transfer_out,
+                                             reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 2;
+    return rc;
 }
 int density_b200_shard_prot_settle(density_b200_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out, void* stream) {
     g_last_error.clear();
-    return prot_settle_impl(s, d_all_transfers, world, rank, d_words_out, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || !d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 2) { set_error("shard_prot_settle: call it after prot_transfer"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cham_prot_settle(s->n, s->ws.p, s->L, prot_rec(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out,
+                                           reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "shard prot settle");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 3;
+    return rc;
 }
 int density_b200_shard_prot_next(density_b200_shard* s, const uint32_t* d_all_words, int world, uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
-    return prot_next_impl(s, d_all_words, world, d_table_out, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || !d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (s->prot_phase != 3) { set_error("shard_prot_next: call it after prot_settle"); return DENSITY_B200_EARG; }
+    if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_words) || !al4(d_table_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (d_table_out && s->round + 1 >= g_prot_rounds) { set_error("shard_prot_next: the round budget is used up"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cham_prot_next(s->d_in, s->n, s->ws.p, s->L, s->nruns, prot_rec(s), s->round, d_all_words, (uint32_t)world,
+                                         d_table_out, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "shard prot next");
+    if (rc != DENSITY_B200_OK) return rc;
+    if (d_table_out) { ++s->round; s->prot_phase = 1; }
+    else s->prot_phase = 4;
+    return DENSITY_B200_OK;
 }
 int density_b200_shard_prot_finish(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
@@ -803,12 +803,9 @@ struct density_b200_cl_shard {
 static bool cl_alg_ok(int alg) { return alg == ALG_CHEETAH || alg == ALG_LION; }
 
 density_b200_cl_shard* density_b200_cl_shard_create(int alg) {
-    g_last_error.clear();
     if (!cl_alg_ok(alg)) { set_error("cl_shard_create: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return nullptr; }
-    DeviceCtx* c = current_ctx();
-    if (!c) return nullptr;
-    density_b200_cl_shard* s = new density_b200_cl_shard();
-    s->alg = alg; s->num_sms = c->num_sms;
+    density_b200_cl_shard* s = new_shard<density_b200_cl_shard>();
+    if (s) s->alg = alg;
     return s;
 }
 void density_b200_cl_shard_destroy(density_b200_cl_shard* s) {
@@ -821,11 +818,13 @@ size_t density_b200_cl_table_words(int alg, int kind) {
     return (size_t)cl_table_planes(alg, kind) * 65536;
 }
 
-static int cl_phase1_impl(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last, const uint32_t* d_prev_quad, uint32_t* d_tab_p,
-                          cudaStream_t st) {
-    if ((!d_in && n) || !d_tab_p) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!is_last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, const uint32_t* d_prev_quad,
+                                 uint32_t* d_table_p_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || !d_table_p_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
     if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_prev_quad) & 3)) { set_error("d_in and d_prev_quad must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase = 0;
     cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
     for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
@@ -836,83 +835,58 @@ static int cl_phase1_impl(density_b200_cl_shard* s, const uint8_t* d_in, size_t 
         s->epoch = 0;
     }
     s->epoch_base = s->epoch + 1; s->epoch += cl_shard_epochs();
-    s->d_in = d_in; s->n = n; s->first = d_prev_quad == nullptr; s->is_last = is_last != 0;
+    s->d_in = d_in; s->n = n; s->first = d_prev_quad == nullptr; s->is_last = is_last_shard != 0;
     uint64_t launches = 0;
     uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    if (n == 0) e = cudaMemsetAsync(d_tab_p, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_P) * sizeof(uint32_t), st);   // identity
-    else e = cl_shard_phase1(s->alg, d_in, n, d_prev_quad, s->ws.p, tabs, s->epoch_base, s->num_sms, d_tab_p, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cl shard phase1", e); return DENSITY_B200_ECUDA; }
-    s->phase = 1;
-    return DENSITY_B200_OK;
-}
-static int cl_phase2_impl(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t st) {
-    if (s->phase != 1) { set_error("cl_shard_phase2: phase 1 not done"); return DENSITY_B200_EARG; }
-    if (!d_tab_c) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    cudaError_t e;
-    if (s->n == 0) e = cudaMemsetAsync(d_tab_c, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_C) * sizeof(uint32_t), st);
-    else e = cl_shard_phase2(s->alg, s->d_in, s->n, s->first, d_carry_p, s->ws.p, tabs, s->epoch_base, s->num_sms, d_tab_c, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cl shard phase2", e); return DENSITY_B200_ECUDA; }
-    s->phase = 2;
-    return DENSITY_B200_OK;
-}
-static int cl_phase3_impl(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
-                          cudaStream_t st) {
-    if (s->phase != 2) { set_error("cl_shard_phase3: phase 2 not done"); return DENSITY_B200_EARG; }
-    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    cudaError_t e;
-    if (s->n == 0) {
-        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
-    } else {
-        e = cl_shard_phase3(s->alg, s->d_in, s->n, s->first, s->is_last, d_carry_c, s->ws.p, tabs, s->epoch_base, s->num_sms, d_out, cap, d_out_size,
-                            d_seam8, st, &launches);
-    }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cl shard phase3", e); return DENSITY_B200_ECUDA; }
-    s->phase = 3;
-    return DENSITY_B200_OK;
-}
-int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, const uint32_t* d_prev_quad,
-                                 uint32_t* d_table_p_out, void* stream) {
-    g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cl_phase1_impl(s, d_in, n, is_last_shard, d_prev_quad, d_table_p_out, reinterpret_cast<cudaStream_t>(stream));
+    if (n == 0) e = cudaMemsetAsync(d_table_p_out, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_P) * sizeof(uint32_t), st);   // identity
+    else e = cl_shard_phase1(s->alg, d_in, n, d_prev_quad, s->ws.p, tabs, s->epoch_base, s->num_sms, d_table_p_out, st, &launches);
+    const int rc = step_result(e, launches, "cl shard phase1");
+    if (rc == DENSITY_B200_OK) s->phase = 1;
+    return rc;
 }
 int density_b200_cl_shard_phase2(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream) {
     g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cl_phase2_impl(s, d_carry_p, d_table_c_out, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || s->phase != 1) { set_error("cl_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
+    if (!d_table_c_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
+    cudaError_t e;
+    if (s->n == 0) e = cudaMemsetAsync(d_table_c_out, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_C) * sizeof(uint32_t), st);
+    else e = cl_shard_phase2(s->alg, s->d_in, s->n, s->first, d_carry_p, s->ws.p, tabs, s->epoch_base, s->num_sms, d_table_c_out, st, &launches);
+    const int rc = step_result(e, launches, "cl shard phase2");
+    if (rc == DENSITY_B200_OK) s->phase = 2;
+    return rc;
 }
 int density_b200_cl_shard_phase3(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                  uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cl_phase3_impl(s, d_carry_c, d_out, cap, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || s->phase != 2) { set_error("cl_shard_phase3: null pointer / phase 2 not done"); return DENSITY_B200_EARG; }
+    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
+    const cudaError_t e = s->n ? cl_shard_phase3(s->alg, s->d_in, s->n, s->first, s->is_last, d_carry_c, s->ws.p, tabs, s->epoch_base, s->num_sms, d_out,
+                                                 cap, d_out_size, d_seam8, st, &launches)
+                               : empty_piece_outputs(d_out_size, d_seam8, st);
+    const int rc = step_result(e, launches, "cl shard phase3");
+    if (rc == DENSITY_B200_OK) s->phase = 3;
+    return rc;
 }
 int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* stream) {
     g_last_error.clear();
     if (!density_b200_cl_table_words(alg, kind) || !d_table) { set_error("cl_table_init: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
     uint64_t l = 0;
-    cudaError_t e = cl_table_init(alg, kind, d_table, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("cl_table_init", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = cl_table_init(alg, kind, d_table, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "cl_table_init");
 }
 int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, void* stream) {
     g_last_error.clear();
     if (!density_b200_cl_table_words(alg, kind) || !d_acc || !d_next) { set_error("cl_table_fold: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
     uint64_t l = 0;
-    cudaError_t e = cl_table_fold(alg, kind, d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("cl_table_fold", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = cl_table_fold(alg, kind, d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "cl_table_fold");
 }
 
 // ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
@@ -925,14 +899,7 @@ struct density_b200_decode_shard {
     bool phase1_done = false;
 };
 
-density_b200_decode_shard* density_b200_decode_shard_create(void) {
-    g_last_error.clear();
-    DeviceCtx* c = current_ctx();
-    if (!c) return nullptr;
-    density_b200_decode_shard* s = new density_b200_decode_shard();
-    s->num_sms = c->num_sms;
-    return s;
-}
+density_b200_decode_shard* density_b200_decode_shard_create(void) { return new_shard<density_b200_decode_shard>(); }
 void density_b200_decode_shard_destroy(density_b200_decode_shard* s) {
     if (!s) return;
     s->ws.release();
@@ -951,10 +918,9 @@ int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t
     uint64_t launches = 0;
     if (n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
     else e = cham_decode_phase1(d_in, n, cap, s->ws.p, s->num_sms, d_table_out, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("decode shard phase1", e); return DENSITY_B200_ECUDA; }
-    s->phase1_done = true;
-    return DENSITY_B200_OK;
+    const int rc = step_result(e, launches, "decode shard phase1");
+    if (rc == DENSITY_B200_OK) s->phase1_done = true;
+    return rc;
 }
 int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
                                      uint32_t* d_seam8, void* stream) {
@@ -964,18 +930,11 @@ int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_
     if (reinterpret_cast<uintptr_t>(d_out) & 3) { set_error("d_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
-    cudaError_t e;
-    if (s->n == 0) {
-        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
-    } else {
-        e = cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches);
-        if (e == cudaSuccess) e = cham_decode_seam_words(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, s->is_last, d_out_size, d_seam8, st, &launches);
-    }
-    g_launches += launches;
+    cudaError_t e = s->n ? cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches)
+                         : empty_piece_outputs(d_out_size, d_seam8, st);
+    if (e == cudaSuccess && s->n) e = cham_decode_seam_words(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, s->is_last, d_out_size, d_seam8, st, &launches);
     s->phase1_done = false;     // the decode pass overwrites the run tables: one phase 2 per phase 1
-    if (e != cudaSuccess) { set_error("decode shard phase2", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    return step_result(e, launches, "decode shard phase2");
 }
 
 // ---- sharded Cheetah decode: one piece, its chunk map carried in and its prediction rounds run over all pieces ------------------------
@@ -990,14 +949,7 @@ struct density_b200_cheetah_decode_shard {
     uint32_t round = 0;
 };
 
-density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void) {
-    g_last_error.clear();
-    DeviceCtx* c = current_ctx();
-    if (!c) return nullptr;
-    density_b200_cheetah_decode_shard* s = new density_b200_cheetah_decode_shard();
-    s->num_sms = c->num_sms;
-    return s;
-}
+density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void) { return new_shard<density_b200_cheetah_decode_shard>(); }
 void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard* s) {
     if (!s) return;
     s->ws.release(); s->tables.release();
@@ -1006,10 +958,12 @@ void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard
 int density_b200_cheetah_decode_round_budget(void) { return g_chee_dec_rounds; }
 size_t density_b200_cheetah_cmap_words(void) { return 3 * 65536; }
 
-static int cd_phase1_impl(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
-                          uint32_t* d_cmap_out, cudaStream_t st) {
-    if ((!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                             int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase = 0; s->round = 0;
     CheeShardArgs& a = s->a;
     a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
@@ -1023,24 +977,25 @@ static int cd_phase1_impl(density_b200_cheetah_decode_shard* s, const uint8_t* d
     uint64_t launches = 0;
     if (n) e = chee_shard_phase1(a, d_cmap_out, st, &launches);
     else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode shard phase1", e); return DENSITY_B200_ECUDA; }
-    s->phase = 1;
-    return DENSITY_B200_OK;
+    const int rc = step_result(e, launches, "cheetah decode shard phase1");
+    if (rc == DENSITY_B200_OK) s->phase = 1;
+    return rc;
 }
-static int cd_phase2_impl(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, cudaStream_t st) {
-    if (s->phase != 1) { set_error("cheetah_decode_shard_phase2: phase 1 not done"); return DENSITY_B200_EARG; }
+int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
+    g_last_error.clear();
+    if (!s || s->phase != 1) { set_error("cheetah_decode_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
     uint64_t launches = 0;
-    cudaError_t e = s->a.n ? chee_shard_phase2(s->a, d_cmap_carry, st, &launches) : cudaSuccess;
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode shard phase2", e); return DENSITY_B200_ECUDA; }
-    s->phase = 2;
-    return DENSITY_B200_OK;
+    const cudaError_t e = s->a.n ? chee_shard_phase2(s->a, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;
+    const int rc = step_result(e, launches, "cheetah decode shard phase2");
+    if (rc == DENSITY_B200_OK) s->phase = 2;
+    return rc;
 }
-static int cd_round_walk_impl(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, cudaStream_t st) {
-    if (s->phase != 2) { set_error("cheetah_decode_shard_round_walk: phase 2 or the previous round's fold not done"); return DENSITY_B200_EARG; }
+int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, void* stream) {
+    g_last_error.clear();
+    if (!s || s->phase != 2) { set_error("cheetah_decode_shard_round_walk: null pointer / phase 2 or the previous round's fold not done"); return DENSITY_B200_EARG; }
     if (!d_words4) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (s->round >= (uint32_t)g_chee_dec_rounds) { set_error("cheetah_decode_shard_round_walk: round budget used up"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
     cudaError_t e;
     if (s->a.n) e = chee_shard_round_walk(s->a, s->round, d_pred_out, d_words4, st, &launches);
@@ -1048,63 +1003,33 @@ static int cd_round_walk_impl(density_b200_cheetah_decode_shard* s, uint32_t* d_
         e = cudaMemsetAsync(d_words4, 0, 4 * sizeof(uint32_t), st);
         if (e == cudaSuccess && d_pred_out) e = cudaMemsetAsync(d_pred_out, 0, 2 * 65536 * sizeof(uint32_t), st);
     }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode shard round walk", e); return DENSITY_B200_ECUDA; }
-    s->phase = 3;
-    return DENSITY_B200_OK;
-}
-static int cd_round_fold_impl(density_b200_cheetah_decode_shard* s, const uint32_t* d_pred_carry, const uint32_t* d_all_words, int world, int rank,
-                              cudaStream_t st) {
-    if (s->phase != 3) { set_error("cheetah_decode_shard_round_fold: the round's walk not done"); return DENSITY_B200_EARG; }
-    if (!d_all_words || world < 1 || rank < 0 || rank >= world) { set_error("cheetah_decode_shard_round_fold: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    cudaError_t e = s->a.n ? chee_shard_round_fold(s->a, s->round, d_pred_carry, d_all_words, (uint32_t)world, (uint32_t)rank, st, &launches) : cudaSuccess;
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode shard round fold", e); return DENSITY_B200_ECUDA; }
-    s->phase = 2; ++s->round;
-    return DENSITY_B200_OK;
-}
-static int cd_phase3_impl(density_b200_cheetah_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st) {
-    if (s->phase != 2) { set_error("cheetah_decode_shard_phase3: phase 2 or the last round's fold not done"); return DENSITY_B200_EARG; }
-    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    cudaError_t e;
-    if (s->a.n) e = chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches);
-    else {
-        e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(d_seam8, 0, 8 * sizeof(uint32_t), st);
-    }
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode shard phase3", e); return DENSITY_B200_ECUDA; }
-    s->phase = 4;
-    return DENSITY_B200_OK;
-}
-int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                             int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
-    g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cd_phase1_impl(s, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, reinterpret_cast<cudaStream_t>(stream));
-}
-int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
-    g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cd_phase2_impl(s, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream));
-}
-int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, void* stream) {
-    g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cd_round_walk_impl(s, d_pred_out, d_words4, reinterpret_cast<cudaStream_t>(stream));
+    const int rc = step_result(e, launches, "cheetah decode shard round walk");
+    if (rc == DENSITY_B200_OK) s->phase = 3;
+    return rc;
 }
 int density_b200_cheetah_decode_shard_round_fold(density_b200_cheetah_decode_shard* s, const uint32_t* d_pred_carry, const uint32_t* d_all_words,
                                                  int world, int rank, void* stream) {
     g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cd_round_fold_impl(s, d_pred_carry, d_all_words, world, rank, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || s->phase != 3) { set_error("cheetah_decode_shard_round_fold: null pointer / the round's walk not done"); return DENSITY_B200_EARG; }
+    if (!d_all_words || world < 1 || rank < 0 || rank >= world) { set_error("cheetah_decode_shard_round_fold: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = s->a.n ? chee_shard_round_fold(s->a, s->round, d_pred_carry, d_all_words, (uint32_t)world, (uint32_t)rank,
+                                                         reinterpret_cast<cudaStream_t>(stream), &launches)
+                                 : cudaSuccess;
+    const int rc = step_result(e, launches, "cheetah decode shard round fold");
+    if (rc == DENSITY_B200_OK) { s->phase = 2; ++s->round; }
+    return rc;
 }
 int density_b200_cheetah_decode_shard_phase3(density_b200_cheetah_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
-    if (!s) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    return cd_phase3_impl(s, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream));
+    if (!s || s->phase != 2) { set_error("cheetah_decode_shard_phase3: null pointer / phase 2 or the last round's fold not done"); return DENSITY_B200_EARG; }
+    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    const cudaError_t e = s->a.n ? chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches) : empty_piece_outputs(d_out_size, d_seam8, st);
+    const int rc = step_result(e, launches, "cheetah decode shard phase3");
+    if (rc == DENSITY_B200_OK) s->phase = 4;
+    return rc;
 }
 int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard* s, uint32_t* out4) {
     g_last_error.clear();
@@ -1122,19 +1047,15 @@ int density_b200_cheetah_cmap_init(uint32_t* d_table, void* stream) {
     g_last_error.clear();
     if (!d_table) { set_error("null pointer"); return DENSITY_B200_EARG; }
     uint64_t l = 0;
-    cudaError_t e = chee_cmap_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("cheetah_cmap_init", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = chee_cmap_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "cheetah_cmap_init");
 }
 int density_b200_cheetah_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, void* stream) {
     g_last_error.clear();
     if (!d_acc || !d_next) { set_error("null pointer"); return DENSITY_B200_EARG; }
     uint64_t l = 0;
-    cudaError_t e = chee_cmap_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("cheetah_cmap_fold", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = chee_cmap_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "cheetah_cmap_fold");
 }
 
 // ---- sharded Chameleon encode across the GPUs of one box (SURVEY §8e): one process per GPU, NCCL over NVLink ---------------------
@@ -1189,17 +1110,15 @@ bool nccl_check(int rc, const char* what) {
 struct density_b200_sharded {
     int rank = 0, world = 1, num_sms = 0;
     nccl_comm_t comm = nullptr;
-    DevBuf ws, aux;                 // aux: gathered tables [world][65536] + carry [65536] + seam words [world][8] + offsets [world + 1] + size
-    DevBuf dws;                     // decode workspace (density_b200_decode_sharded[_stream]), apart from the encoder's
-    density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion shard state of density_b200_encode_sharded_cl
-    DevBuf cl_aux;                  // its exchange buffers: gathered P and C tables, the carries, the last quads
-    density_b200_cheetah_decode_shard* cdec = nullptr;   // piece state of density_b200_decode_sharded_cheetah
-    DevBuf cd_aux;                  // its exchange buffers: gathered chunk-map and prediction transfers, the carries, the round words
-    density_b200_shard* prot = nullptr;   // shard state of density_b200_encode_sharded_protected
-    DevBuf prot_aux;                // its exchange buffers: gathered shard lengths, transfers and round words
-    ChamLayout L{};
+    DevBuf aux;                     // the exchange buffers of the drivers (Exchange)
+    // the phase state of each driver, apart from the others', so that the drivers may alternate on one handle
+    density_b200_shard* enc = nullptr;                   // density_b200_encode_sharded
+    density_b200_shard* prot = nullptr;                  // density_b200_encode_sharded_protected
+    density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion of density_b200_encode_sharded_cl
+    density_b200_decode_shard* dec = nullptr;            // density_b200_decode_sharded[_stream]
+    density_b200_cheetah_decode_shard* cdec = nullptr;   // density_b200_decode_sharded_cheetah[_stream]
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
-    uint64_t* h_maps = nullptr;     // pinned, world range maps (density_b200_decode_sharded_stream)
+    uint64_t* h_maps = nullptr;     // pinned, world range maps (the stream decodes)
     cudaEvent_t ev[6] = {};         // stage timing of the last call: start, flag pass, exchange, phase 2 up to emit, emit, gather
     bool timed = false;
 };
@@ -1230,11 +1149,12 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
     if (cudaMallocHost(&h->h_offsets, sizeof(uint64_t) * (world + 2)) != cudaSuccess ||
         cudaMallocHost(&h->h_maps, sizeof(uint64_t) * DENSITY_B200_LOCATE_MAP_WORDS * world) != cudaSuccess) {
         set_error("cudaMallocHost");
-        if (h->h_offsets) cudaFreeHost(h->h_offsets);
-        if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-        delete h;
+        density_b200_sharded_destroy(h);
         return nullptr;
     }
+    h->enc = density_b200_shard_create(); h->prot = density_b200_shard_create();
+    h->cl[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->cl[1] = density_b200_cl_shard_create(ALG_LION);
+    h->dec = density_b200_decode_shard_create(); h->cdec = density_b200_cheetah_decode_shard_create();
     for (auto& e : h->ev) cudaEventCreate(&e);
     return h;
 }
@@ -1242,9 +1162,11 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
     if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
-    h->ws.release(); h->aux.release(); h->dws.release(); h->cl_aux.release(); h->cd_aux.release(); h->prot_aux.release();
+    h->aux.release();
+    density_b200_shard_destroy(h->enc);
     density_b200_shard_destroy(h->prot);
     for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
+    density_b200_decode_shard_destroy(h->dec);
     density_b200_cheetah_decode_shard_destroy(h->cdec);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     if (h->h_maps) cudaFreeHost(h->h_maps);
@@ -1252,20 +1174,59 @@ void density_b200_sharded_destroy(density_b200_sharded* h) {
     delete h;
 }
 
-// the exchange buffers of a handle, shared by encode and decode
-struct ShardedAux { uint32_t *tables, *carry, *words; uint64_t *offsets, *maps; };
-static cudaError_t sharded_aux(density_b200_sharded* h, cudaStream_t st, ShardedAux* x) {
-    const size_t W = (size_t)h->world;
-    const size_t aux_tables = W * 65536 * sizeof(uint32_t), aux_carry = 65536 * sizeof(uint32_t), aux_words = W * 8 * sizeof(uint32_t);
-    const size_t aux_offsets = (W + 2) * sizeof(uint64_t), aux_maps = W * DENSITY_B200_LOCATE_MAP_WORDS * sizeof(uint64_t);
-    const cudaError_t e = h->aux.ensure(aux_tables + aux_carry + aux_words + aux_offsets + aux_maps + 256, st);
-    x->tables = reinterpret_cast<uint32_t*>(h->aux.p);
-    x->carry = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables);
-    x->words = reinterpret_cast<uint32_t*>(h->aux.p + aux_tables + aux_carry);
-    x->offsets = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words);
-    x->maps = reinterpret_cast<uint64_t*>(h->aux.p + aux_tables + aux_carry + aux_words + aux_offsets);
-    return e;
-}
+// The collectives of one driver call on the handle's communicator, enqueued on `st`, and the exchange buffers they share. Every rank
+// issues the same collectives in the same order (include/density_b200.h lists them per driver); all of them are all-gathers but the
+// grouped send / recv of gather_pieces.
+struct Exchange {
+    density_b200_sharded* h = nullptr;
+    cudaStream_t st = nullptr;
+    NcclApi* a = nullptr;               // NULL with world == 1
+    uint32_t *tables = nullptr, *carry = nullptr, *words = nullptr;   // [world][65536] tables, [65536] carry-in, [world][8] seam words
+    uint64_t *offsets = nullptr, *maps = nullptr;                     // [world + 2] piece offsets, [world][LOCATE_MAP_WORDS] range maps
+    uint8_t* extra = nullptr;           // the driver's own exchange buffers
+
+    // NCCL (world > 1) and the buffers, extra_bytes of them the driver's; DENSITY_B200_ECUDA with the error set when either is missing
+    int open(density_b200_sharded* handle, void* stream, size_t extra_bytes = 0) {
+        h = handle; st = reinterpret_cast<cudaStream_t>(stream);
+        a = h->world > 1 ? nccl_api() : nullptr;
+        if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
+        const size_t W = (size_t)h->world;
+        const size_t n_tables = W * 65536, n_carry = 65536, n_words = W * 8, n_offsets = W + 2;
+        size_t bytes = (n_tables + n_carry + n_words) * sizeof(uint32_t) + (n_offsets + W * DENSITY_B200_LOCATE_MAP_WORDS) * sizeof(uint64_t);
+        bytes = (bytes + 255) & ~(size_t)255;
+        const cudaError_t e = h->aux.ensure(bytes + extra_bytes + 256, st);
+        if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        tables = reinterpret_cast<uint32_t*>(h->aux.p);
+        carry = tables + n_tables;
+        words = carry + n_carry;
+        offsets = reinterpret_cast<uint64_t*>(words + n_words);
+        maps = offsets + n_offsets;
+        extra = h->aux.p + bytes;
+        return DENSITY_B200_OK;
+    }
+    // this rank's slot of buf ([world][n] u32) to every rank
+    bool gather(uint32_t* buf, size_t n, const char* what) const {
+        return h->world == 1 || nccl_check(a->AllGather(buf + (size_t)h->rank * n, buf, n, NCCL_UINT32, h->comm, st), what);
+    }
+    uint32_t* my_words() const { return words + 8 * (size_t)h->rank; }
+    // this rank's seam words (my_words) to every rank -> the verdict over all pieces; *d_out_offset (may be NULL) = where this rank's
+    // output starts
+    int verdict(uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) const {
+        if (!gather(words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
+        uint64_t launches = 0;
+        cudaError_t e = cham_seam_verdict(words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, offsets, st, &launches);
+        if (e == cudaSuccess && d_out_offset) e = cudaMemcpyAsync(d_out_offset, offsets + h->rank, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st);
+        return step_result(e, launches, "seam verdict");
+    }
+    // this rank's range map (map_words u64 in its slot of `maps`) to every rank, then all of them to h->h_maps: the call's one host
+    // synchronisation
+    int maps_to_host(size_t map_words) const {
+        if (!gather(reinterpret_cast<uint32_t*>(maps), 2 * map_words, "ncclAllGather(maps)")) return DENSITY_B200_ECUDA;
+        cudaError_t e = cudaMemcpyAsync(h->h_maps, maps, (size_t)h->world * map_words * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        return step_result(e, 0, "range maps to host");
+    }
+};
 
 // variable-length gather of the pieces to `gather_root` at their stream offsets (d_offsets: world + 1 prefix sums, on the device); blocks
 static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_offsets, const uint8_t* d_out, int gather_root, uint8_t* d_gather,
@@ -1297,61 +1258,57 @@ static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_
     return DENSITY_B200_OK;
 }
 
+// the argument checks of the sharded encoders
+static int encode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, size_t n, const uint8_t* d_out, const uint64_t* d_out_size,
+                               int gather_root) {
+    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (h->rank != h->world - 1 && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+
+// the end of every sharded encode: the verdict, the optional gather of the pieces to gather_root, the last stage event
+static int encode_sharded_end(const Exchange& x, const uint8_t* d_out, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
+                              uint8_t* d_gather, size_t gather_cap) {
+    int rc = x.verdict(d_flags, d_total_size, nullptr);
+    if (rc == DENSITY_B200_OK && gather_root >= 0) rc = gather_pieces(x.h, x.a, x.offsets, d_out, gather_root, d_gather, gather_cap, x.st);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaEventRecord(x.h->ev[5], x.st);
+    x.h->timed = true;
+    return DENSITY_B200_OK;
+}
+
 // One bit-exact stream cut across `world` GPUs; this rank's shard is d_in[0 .. n) (n % 256 == 0 except on the last rank).
 // All work is enqueued on `stream`. With gather_root >= 0 the call BLOCKS on the stream once (the piece sizes must reach the host before
 // the variable-length ncclSend / ncclRecv can be posted) and the pieces land in d_gather on rank gather_root at their stream offsets.
 int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    const bool last = h->rank == h->world - 1;
-    if (!last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
-    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    cudaError_t e = h->ws.ensure(cham_workspace_bytes(n, h->num_sms, &h->L), st);
-    ShardedAux x;
-    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* d_tables = x.tables;
-    uint32_t* d_carry = x.carry;
-    uint32_t* d_words = x.words;
-    uint64_t* d_offsets = x.offsets;
-    const uint32_t nruns = cham_pick_runs(n, h->num_sms);
-    uint64_t launches = 0;
-    cudaEventRecord(h->ev[0], st);
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
+    density_b200_shard* s = h->enc;
+    cudaEventRecord(h->ev[0], x.st);
     // phase 1: flags with unknown carry-in; my last-writer table lands in my slot of the gather buffer
-    cudaEvent_t pev[4] = {nullptr, nullptr, nullptr, nullptr};
-    if (n) e = cham_encode_phase1(d_in, n, h->ws.p, h->L, nruns, d_tables + (size_t)h->rank * 65536, st, &launches);
-    else e = cudaMemsetAsync(d_tables + (size_t)h->rank * 65536, 0, 65536 * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("sharded phase 1", e); return DENSITY_B200_ECUDA; }
-    cudaEventRecord(h->ev[1], st);
+    rc = density_b200_shard_phase1(s, d_in, n, h->rank == h->world - 1, x.tables + (size_t)h->rank * 65536, x.st);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[1], x.st);
     // the one exchange step of the path: 256 KiB per rank over NVLink, then ONE fold kernel
-    if (h->world > 1) {
-        if (!a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-        if (!nccl_check(a->AllGather(d_tables + (size_t)h->rank * 65536, d_tables, 65536, NCCL_UINT32, h->comm, st), "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-    }
-    e = cham_rank_fold(d_tables, (uint32_t)h->rank, d_carry, st, &launches);
-    cudaEventRecord(h->ev[2], st);
+    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    cudaError_t e = cham_rank_fold(x.tables, (uint32_t)h->rank, x.carry, x.st, &launches);
+    if ((rc = step_result(e, launches, "sharded fold")) != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[2], x.st);
     // phase 2: carry-in, first-touch flags, sizes, scan, emit (seams are judged below, exactly, once every shard knows its flags)
-    pev[2] = h->ev[3]; pev[3] = h->ev[4];
-    if (e == cudaSuccess) e = cham_encode_phase2(d_in, n, h->ws.p, h->L, nruns, d_carry, d_out, cap, d_out_size, false, false, st, &launches, n ? pev : nullptr);
-    if (!n) { cudaEventRecord(h->ev[3], st); cudaEventRecord(h->ev[4], st); }
-    if (e == cudaSuccess && n) e = cham_seam_words(h->ws.p, h->L, n, d_out_size, d_words + 8 * h->rank, st, &launches);
-    else if (e == cudaSuccess) e = cudaMemsetAsync(d_words + 8 * h->rank, 0, 8 * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("sharded phase 2", e); return DENSITY_B200_ECUDA; }
-    if (h->world > 1 && !nccl_check(a->AllGather(d_words + 8 * h->rank, d_words, 8, NCCL_UINT32, h->comm, st), "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
-    e = cham_seam_verdict(d_words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, d_offsets, st, &launches);
-    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
-    if (gather_root >= 0) {
-        const int rc = gather_pieces(h, a, d_offsets, d_out, gather_root, d_gather, gather_cap, st);
-        if (rc != DENSITY_B200_OK) return rc;
-    }
-    cudaEventRecord(h->ev[5], st);
-    h->timed = true;
-    g_launches += launches;
-    return DENSITY_B200_OK;
+    cudaEvent_t pev[4] = {nullptr, nullptr, h->ev[3], h->ev[4]};
+    if ((rc = shard_phase2_impl(s, x.carry, d_out, cap, d_out_size, false, n ? pev : nullptr, x.st)) != DENSITY_B200_OK) return rc;
+    if (!n) { cudaEventRecord(h->ev[3], x.st); cudaEventRecord(h->ev[4], x.st); }
+    launches = 0;
+    if (n) e = cham_seam_words(s->ws.p, s->L, n, d_out_size, x.my_words(), x.st, &launches);
+    else e = cudaMemsetAsync(x.my_words(), 0, 8 * sizeof(uint32_t), x.st);
+    if ((rc = step_result(e, launches, "sharded seam words")) != DENSITY_B200_OK) return rc;
+    return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
 }
 
 // Sharded Cheetah / Lion encode over the handle's communicator: last quads -> phase 1 -> P tables -> fold -> phase 2 -> C tables -> fold
@@ -1359,72 +1316,47 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
 int density_b200_encode_sharded_cl(density_b200_sharded* h, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                    uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    if (rc != DENSITY_B200_OK) return rc;
     if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
-    const bool last = h->rank == h->world - 1;
-    if (!last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
-    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    density_b200_cl_shard*& s = h->cl[alg - ALG_CHEETAH];
-    if (!s) { s = new density_b200_cl_shard(); s->alg = alg; s->num_sms = h->num_sms; }
+    density_b200_cl_shard* s = h->cl[alg - ALG_CHEETAH];
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
-    ShardedAux x;
-    cudaError_t e = sharded_aux(h, st, &x);
-    if (e == cudaSuccess) e = h->cl_aux.ensure(((W + 1) * (wp + wc) + 2 * W + 64) * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* tab_p = reinterpret_cast<uint32_t*>(h->cl_aux.p);          // [world][wp]
+    Exchange x;
+    if ((rc = x.open(h, stream_v, ((W + 1) * (wp + wc) + 2 * W + 64) * sizeof(uint32_t))) != DENSITY_B200_OK) return rc;
+    cudaStream_t st = x.st;
+    uint32_t* tab_p = reinterpret_cast<uint32_t*>(x.extra);              // [world][wp]
     uint32_t* carry_p = tab_p + W * wp;
     uint32_t* tab_c = carry_p + wp;                                       // [world][wc]
     uint32_t* carry_c = tab_c + W * wc;
     uint32_t* quads = carry_c + wc;                                       // [world] {has a quad, last quad}
     uint32_t* prev_quad = quads + 2 * W;
     uint64_t launches = 0;
-    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
-        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
-    };
     // 0. the context of my first quad: the last quad of the nearest earlier shard that has one
-    e = cl_last_quad(d_in, n, quads + 2 * R, st, &launches);
-    if (e == cudaSuccess && !gather(quads, 2, "ncclAllGather(last quads)")) return DENSITY_B200_ECUDA;
+    cudaError_t e = cl_last_quad(d_in, n, quads + 2 * R, st, &launches);
+    if (e == cudaSuccess && !x.gather(quads, 2, "ncclAllGather(last quads)")) return DENSITY_B200_ECUDA;
     if (e == cudaSuccess) e = cl_prev_quad(quads, (uint32_t)R, prev_quad, st, &launches);
-    g_launches += launches; launches = 0;
-    if (e != cudaSuccess) { set_error("sharded cl: last quads", e); return DENSITY_B200_ECUDA; }
+    if ((rc = step_result(e, launches, "sharded cl: last quads")) != DENSITY_B200_OK) return rc;
     // 1-2. predictions, exchange, fold
     cudaEventRecord(h->ev[0], st);
-    int rc = cl_phase1_impl(s, d_in, n, last, R ? prev_quad : nullptr, tab_p + R * wp, st);
-    if (rc != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cl_shard_phase1(s, d_in, n, R == W - 1, R ? prev_quad : nullptr, tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[1], st);
-    if (!gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
+    if (!x.gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
+    launches = 0;
     e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
-    g_launches += launches; launches = 0;
-    if (e != cudaSuccess) { set_error("sharded cl: P fold", e); return DENSITY_B200_ECUDA; }
+    if ((rc = step_result(e, launches, "sharded cl: P fold")) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[2], st);
     // 3-4. chunk map, exchange, fold
-    rc = cl_phase2_impl(s, carry_p, tab_c + R * wc, st);
-    if (rc != DENSITY_B200_OK) return rc;
-    if (!gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
+    if ((rc = density_b200_cl_shard_phase2(s, carry_p, tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
+    if (!x.gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
+    launches = 0;
     e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_C, tab_c, (uint32_t)R, carry_c, st, &launches);
-    g_launches += launches; launches = 0;
-    if (e != cudaSuccess) { set_error("sharded cl: C fold", e); return DENSITY_B200_ECUDA; }
+    if ((rc = step_result(e, launches, "sharded cl: C fold")) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[3], st);
     // 5. emit and seam words, the verdict over all shards, the optional gather
-    rc = cl_phase3_impl(s, carry_c, d_out, cap, d_out_size, x.words + 8 * R, st);
-    if (rc != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cl_shard_phase3(s, carry_c, d_out, cap, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[4], st);
-    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
-    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
-    if (gather_root >= 0) {
-        rc = gather_pieces(h, a, x.offsets, d_out, gather_root, d_gather, gather_cap, st);
-        if (rc != DENSITY_B200_OK) return rc;
-    }
-    cudaEventRecord(h->ev[5], st);
-    h->timed = true;
-    return DENSITY_B200_OK;
+    return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
 }
 
 // Sharded Chameleon encode with copy mode over the handle's communicator: the shard lengths -> phase 1 -> the round budget of
@@ -1434,108 +1366,75 @@ int density_b200_encode_sharded_protected(density_b200_sharded* h, const uint8_t
                                           uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap,
                                           void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    const bool last = h->rank == h->world - 1;
-    if (!last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    if (rc != DENSITY_B200_OK) return rc;
     // every argument the later phases check is checked here, before the first collective: a rank that returned EARG half way through
     // would leave the others waiting in an all-gather
     if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || (reinterpret_cast<uintptr_t>(d_total_size) & 7) || !al4(d_flags)) {
         set_error("d_out_size and d_total_size must be 8-byte, d_flags 4-byte aligned"); return DENSITY_B200_EARG;
     }
-    if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    if (!h->prot) {
-        h->prot = new density_b200_shard();
-        h->prot->num_sms = h->num_sms;
-    }
     density_b200_shard* s = h->prot;
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
-    ShardedAux x;
-    cudaError_t e = sharded_aux(h, st, &x);
-    if (e == cudaSuccess) e = h->prot_aux.ensure(W * (2 * sizeof(uint64_t) + (PROT_TRANSFER_WORDS + PROT_ROUND_WORDS) * sizeof(uint32_t)) + 256, st);
-    if (e == cudaSuccess) e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);      // phase 1 finds them in place
+    Exchange x;
+    if ((rc = x.open(h, stream_v, W * (2 * sizeof(uint64_t) + (PROT_TRANSFER_WORDS + PROT_ROUND_WORDS) * sizeof(uint32_t)))) != DENSITY_B200_OK) return rc;
+    cudaStream_t st = x.st;
+    cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);      // phase 1 finds them in place
     if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t* lengths = reinterpret_cast<uint64_t*>(h->prot_aux.p);                   // [world]
+    uint64_t* lengths = reinterpret_cast<uint64_t*>(x.extra);                         // [world]
     uint32_t* transfers = reinterpret_cast<uint32_t*>(lengths + W);                   // [world][PROT_TRANSFER_WORDS]
     uint32_t* rwords = transfers + W * PROT_TRANSFER_WORDS;                          // [world][PROT_ROUND_WORDS]
     uint32_t* my_table = x.tables + R * 65536;
     uint64_t launches = 0;
-    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
-        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
-    };
     cudaEventRecord(h->ev[0], st);
     e = cham_put_u64(lengths + R, (uint64_t)n, st, &launches);
-    g_launches += launches; launches = 0;
-    if (e != cudaSuccess) { set_error("sharded protected: length", e); return DENSITY_B200_ECUDA; }
-    if (!gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
-    int rc = prot_phase1_impl(s, d_in, n, 0, lengths, (int)R, last, my_table, st);
-    if (rc != DENSITY_B200_OK) return rc;
+    if ((rc = step_result(e, launches, "sharded protected: length")) != DENSITY_B200_OK) return rc;
+    if (!x.gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
+    if ((rc = prot_phase1_impl(s, d_in, n, 0, lengths, (int)R, R == W - 1, my_table, st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[1], st);
     for (int k = 0; k < g_prot_rounds; ++k) {
-        if (k > 0 && (rc = prot_next_impl(s, rwords, (int)W, my_table, st)) != DENSITY_B200_OK) return rc;
-        if (!gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+        if (k > 0 && (rc = density_b200_shard_prot_next(s, rwords, (int)W, my_table, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+        launches = 0;
         e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, st, &launches);
-        g_launches += launches; launches = 0;
-        if (e != cudaSuccess) { set_error("sharded protected: fold", e); return DENSITY_B200_ECUDA; }
+        if ((rc = step_result(e, launches, "sharded protected: fold")) != DENSITY_B200_OK) return rc;
         if (k == 0) cudaEventRecord(h->ev[2], st);
-        if ((rc = prot_transfer_impl(s, x.carry, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
-        if (!gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
-        if ((rc = prot_settle_impl(s, transfers, (int)W, (int)R, rwords + R * PROT_ROUND_WORDS, st)) != DENSITY_B200_OK) return rc;
-        if (!gather(rwords, PROT_ROUND_WORDS, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_shard_prot_transfer(s, x.carry, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_shard_prot_settle(s, transfers, (int)W, (int)R, rwords + R * PROT_ROUND_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(rwords, PROT_ROUND_WORDS, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
     }
-    if ((rc = prot_next_impl(s, rwords, (int)W, nullptr, st)) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_shard_prot_next(s, rwords, (int)W, nullptr, st)) != DENSITY_B200_OK) return rc;
     cudaEvent_t pev[4] = {nullptr, nullptr, h->ev[3], h->ev[4]};
-    if ((rc = prot_finish_impl(s, d_out, cap, d_out_size, x.words + 8 * R, st, n ? pev : nullptr)) != DENSITY_B200_OK) return rc;
+    if ((rc = prot_finish_impl(s, d_out, cap, d_out_size, x.my_words(), st, n ? pev : nullptr)) != DENSITY_B200_OK) return rc;
     if (!n) { cudaEventRecord(h->ev[3], st); cudaEventRecord(h->ev[4], st); }
-    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
-    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
-    if (gather_root >= 0) {
-        rc = gather_pieces(h, a, x.offsets, d_out, gather_root, d_gather, gather_cap, st);
-        if (rc != DENSITY_B200_OK) return rc;
-    }
-    cudaEventRecord(h->ev[5], st);
-    h->timed = true;
+    return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
+}
+
+// the argument checks of the sharded decoders; n: the bytes of d_in
+static int decode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap, const uint64_t* d_out_size,
+                               const uint32_t* d_flags) {
+    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
     return DENSITY_B200_OK;
 }
 
-// The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it, over the handle's communicator:
-// phase 1 -> table exchange -> fold -> phase 2 -> seam words -> verdict. is_last: the piece ends the stream (a non-final piece must decode
-// to whole 256-byte blocks). d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
-static int decode_sharded_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, int is_last, uint8_t* d_out, size_t cap,
-                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, cudaStream_t st) {
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    ShardedAux x;
-    cudaError_t e = h->dws.ensure(cham_decode_workspace_bytes(n, cap, h->num_sms), st);
-    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* my_table = x.tables + (size_t)h->rank * 65536;
-    uint32_t* my_words = x.words + 8 * h->rank;
-    uint64_t launches = 0;
+// The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it: phase 1 -> table exchange ->
+// fold -> phase 2 -> seam words -> verdict. is_last: the piece ends the stream (a non-final piece must decode to whole 256-byte blocks).
+// d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
+static int decode_sharded_piece(const Exchange& x, const uint8_t* d_in, size_t n, int is_last, uint8_t* d_out, size_t cap,
+                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) {
+    density_b200_decode_shard* s = x.h->dec;
     // phase 1: boundaries and writer pass need no carry-in; the piece's table (runs + tail) lands in my slot of the gather buffer
-    if (n) e = cham_decode_phase1(d_in, n, cap, h->dws.p, h->num_sms, my_table, st, &launches);
-    else e = cudaMemsetAsync(my_table, 0, 65536 * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("sharded decode phase 1", e); return DENSITY_B200_ECUDA; }
-    if (h->world > 1 && !nccl_check(a->AllGather(my_table, x.tables, 65536, NCCL_UINT32, h->comm, st), "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-    e = cham_rank_fold(x.tables, (uint32_t)h->rank, x.carry, st, &launches);
+    int rc = density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, x.tables + (size_t)x.h->rank * 65536, x.st);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)x.h->rank, x.carry, x.st, &launches);
+    if ((rc = step_result(e, launches, "sharded decode fold")) != DENSITY_B200_OK) return rc;
     // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
-    if (e == cudaSuccess && n) e = cham_decode_phase2(d_in, n, d_out, cap, h->dws.p, h->num_sms, x.carry, d_out_size, st, &launches);
-    if (e == cudaSuccess && n) e = cham_decode_seam_words(d_in, n, cap, h->dws.p, h->num_sms, is_last, d_out_size, my_words, st, &launches);
-    if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), st);
-    if (e == cudaSuccess && !n) e = cudaMemsetAsync(my_words, 0, 8 * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("sharded decode phase 2", e); return DENSITY_B200_ECUDA; }
-    if (h->world > 1 && !nccl_check(a->AllGather(my_words, x.words, 8, NCCL_UINT32, h->comm, st), "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
-    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
-    g_launches += launches;
-    if (e == cudaSuccess && d_out_offset) e = cudaMemcpyAsync(d_out_offset, x.offsets + h->rank, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    if ((rc = density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)) != DENSITY_B200_OK) return rc;
+    return x.verdict(d_flags, d_total_size, d_out_offset);
 }
 
 // The inverse of density_b200_encode_sharded without a gather: this rank's piece d_in[0 .. n) decodes to the shard it was encoded from.
@@ -1543,15 +1442,15 @@ static int decode_sharded_piece(density_b200_sharded* h, const uint8_t* d_in, si
 int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                 uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    return decode_sharded_piece(h, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
-                                reinterpret_cast<cudaStream_t>(stream_v));
+    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
+    return decode_sharded_piece(x, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr);
 }
 
-static density_b200_cheetah_decode_shard* sharded_cdec(density_b200_sharded* h) {
-    if (!h->cdec) { h->cdec = new density_b200_cheetah_decode_shard(); h->cdec->num_sms = h->num_sms; }
-    return h->cdec;
+// the exchange buffers of decode_sharded_cheetah_piece: gathered chunk-map and prediction transfers, the carries, the round words
+static size_t cheetah_piece_extra_bytes(const density_b200_sharded* h) {
+    return (((size_t)h->world + 1) * (density_b200_cheetah_cmap_words() + 2 * 65536) + 4 * (size_t)h->world + 64) * sizeof(uint32_t);
 }
 
 // Sharded Cheetah decode of this rank's piece d_in[0 .. n) over the handle's communicator: phase 1 -> chunk-map transfers -> fold ->
@@ -1559,64 +1458,49 @@ static density_b200_cheetah_decode_shard* sharded_cdec(density_b200_sharded* h) 
 // rank issues the same collectives in the same order whatever its piece holds: an empty piece sends identity transfers and zero words, a
 // refused one keeps exchanging until the verdict. The rounds after the settled one are gated off on the device; their all-gathers still
 // run. first: the piece holds the stream start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output
-// starts, from the verdict's prefix offsets.
-static int decode_sharded_cheetah_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
-                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, cudaStream_t st) {
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    density_b200_cheetah_decode_shard* s = sharded_cdec(h);
+// starts, from the verdict's prefix offsets. x is opened with cheetah_piece_extra_bytes.
+static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
+                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) {
+    density_b200_sharded* h = x.h;
+    cudaStream_t st = x.st;
+    density_b200_cheetah_decode_shard* s = h->cdec;
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wc = density_b200_cheetah_cmap_words(), wp = 2 * 65536;
-    ShardedAux x;
-    cudaError_t e = sharded_aux(h, st, &x);
-    if (e == cudaSuccess) e = h->cd_aux.ensure(((W + 1) * (wc + wp) + 4 * W + 64) * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* tab_c = reinterpret_cast<uint32_t*>(h->cd_aux.p);         // [world][wc]
+    uint32_t* tab_c = reinterpret_cast<uint32_t*>(x.extra);              // [world][wc]
     uint32_t* carry_c = tab_c + W * wc;
     uint32_t* tab_p = carry_c + wc;                                       // [world][wp]
     uint32_t* carry_p = tab_p + W * wp;
     uint32_t* rwords = carry_p + wp;                                      // [world][4]
     uint64_t launches = 0;
-    auto gather = [&](uint32_t* buf, size_t words, const char* what) {
-        return h->world == 1 || nccl_check(a->AllGather(buf + R * words, buf, words, NCCL_UINT32, h->comm, st), what);
-    };
     // the last piece's transfers are never read: it sends what its slot holds
-    int rc = cd_phase1_impl(s, d_in, n, d_out, cap, first, last, last ? nullptr : tab_c + R * wc, st);
+    int rc = density_b200_cheetah_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, last ? nullptr : tab_c + R * wc, st);
     if (rc != DENSITY_B200_OK) return rc;
-    if (!gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
-    if (!first) e = chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
-    g_launches += launches; launches = 0;
-    if (e != cudaSuccess) { set_error("sharded cheetah decode: chunk-map fold", e); return DENSITY_B200_ECUDA; }
-    rc = cd_phase2_impl(s, first ? nullptr : carry_c, st);
-    if (rc != DENSITY_B200_OK) return rc;
+    if (!x.gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
+    cudaError_t e = first ? cudaSuccess : chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
+    if ((rc = step_result(e, launches, "sharded cheetah decode: chunk-map fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cheetah_decode_shard_phase2(s, first ? nullptr : carry_c, st)) != DENSITY_B200_OK) return rc;
     for (int k = 0; k < g_chee_dec_rounds; ++k) {
-        rc = cd_round_walk_impl(s, last ? nullptr : tab_p + R * wp, rwords + 4 * R, st);
+        rc = density_b200_cheetah_decode_shard_round_walk(s, last ? nullptr : tab_p + R * wp, rwords + 4 * R, st);
         if (rc != DENSITY_B200_OK) return rc;
-        if (!gather(tab_p, wp, "ncclAllGather(prediction transfers)") || !gather(rwords, 4, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        if (!x.gather(tab_p, wp, "ncclAllGather(prediction transfers)") || !x.gather(rwords, 4, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        launches = 0;
         if (!first) e = cl_rank_fold(ALG_CHEETAH, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
-        g_launches += launches; launches = 0;
-        if (e != cudaSuccess) { set_error("sharded cheetah decode: prediction fold", e); return DENSITY_B200_ECUDA; }
-        rc = cd_round_fold_impl(s, first ? nullptr : carry_p, rwords, (int)W, (int)R, st);
+        if ((rc = step_result(e, launches, "sharded cheetah decode: prediction fold")) != DENSITY_B200_OK) return rc;
+        rc = density_b200_cheetah_decode_shard_round_fold(s, first ? nullptr : carry_p, rwords, (int)W, (int)R, st);
         if (rc != DENSITY_B200_OK) return rc;
     }
-    rc = cd_phase3_impl(s, d_out_size, x.words + 8 * R, st);
-    if (rc != DENSITY_B200_OK) return rc;
-    if (!gather(x.words, 8, "ncclAllGather(seams)")) return DENSITY_B200_ECUDA;
-    e = cham_seam_verdict(x.words, (uint32_t)h->world, (uint32_t)h->rank, d_flags, d_total_size, x.offsets, st, &launches);
-    g_launches += launches;
-    if (e == cudaSuccess && d_out_offset) e = cudaMemcpyAsync(d_out_offset, x.offsets + h->rank, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) { set_error("seam verdict", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    if ((rc = density_b200_cheetah_decode_shard_phase3(s, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
+    return x.verdict(d_flags, d_total_size, d_out_offset);
 }
 
 // The pieces of a sharded Cheetah encode: rank 0 holds the stream start, the last rank its end.
 int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                         uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    return decode_sharded_cheetah_piece(h, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
-                                        reinterpret_cast<cudaStream_t>(stream_v));
+    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h))) != DENSITY_B200_OK) return rc;
+    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr);
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
@@ -1629,9 +1513,7 @@ int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     uint64_t launches = 0;
     e = cham_decode_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("decode locate", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    return step_result(e, launches, "decode locate");
 }
 
 // The layout checks and the walk from the stream start shared by density_b200_locate_piece (Chameleon) and
@@ -1717,9 +1599,7 @@ int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard* s, con
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     uint64_t launches = 0;
     e = chee_decode_locate(d_in, n_range, n_halo, range_offset, s->ws.p, d_map, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode locate", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    return step_result(e, launches, "cheetah decode locate");
 }
 
 // Sharded decode of a stream without known cuts: this rank holds its range + halo (include/density_b200.h). Locates the piece (one
@@ -1727,32 +1607,21 @@ int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard* s, con
 int density_b200_decode_sharded_stream(density_b200_sharded* h, const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* d_out, size_t cap,
                                        uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n_range + n_halo) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    const size_t W = (size_t)h->world;
-    ShardedAux x;
-    // sized for the whole range + halo: covers the locate scratch and the phases on any piece of it
-    cudaError_t e = h->dws.ensure(cham_decode_workspace_bytes(n_range + n_halo, cap, h->num_sms), st);
-    if (e == cudaSuccess) e = sharded_aux(h, st, &x);
+    int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
+    // sized for the whole range + halo: covers the locate scratch and the phases on any piece of it, so that phase 1 does not reallocate
+    const cudaError_t e = h->dec->ws.ensure(cham_decode_workspace_bytes(n_range + n_halo, cap, h->num_sms), x.st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t* my_map = x.maps + (size_t)h->rank * DENSITY_B200_LOCATE_MAP_WORDS;
-    uint64_t launches = 0;
-    e = cham_decode_locate(d_in, n_range, n_halo, h->dws.p, my_map, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("decode locate", e); return DENSITY_B200_ECUDA; }
-    if (h->world > 1 && !nccl_check(a->AllGather(my_map, x.maps, DENSITY_B200_LOCATE_MAP_WORDS * 8, NCCL_UINT8, h->comm, st), "ncclAllGather(maps)"))
-        return DENSITY_B200_ECUDA;
-    e = cudaMemcpyAsync(h->h_maps, x.maps, W * DENSITY_B200_LOCATE_MAP_WORDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("range maps to host", e); return DENSITY_B200_ECUDA; }
+    constexpr size_t MW = DENSITY_B200_LOCATE_MAP_WORDS;
+    if ((rc = density_b200_decode_locate(h->dec, d_in, n_range, n_halo, x.maps + (size_t)h->rank * MW, x.st)) != DENSITY_B200_OK ||
+        (rc = x.maps_to_host(MW)) != DENSITY_B200_OK)
+        return rc;
     uint64_t piece[4];
-    const int rc = density_b200_locate_piece(h->h_maps, h->world, h->rank, piece);
+    rc = density_b200_locate_piece(h->h_maps, h->world, h->rank, piece);
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
-    return decode_sharded_piece(h, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[3], d_out, cap, d_out_size, d_flags,
-                                d_total_size, d_out_offset, st);
+    return decode_sharded_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[3], d_out, cap, d_out_size, d_flags,
+                                d_total_size, d_out_offset);
 }
 
 // Sharded decode of a Cheetah stream without known cuts: this rank holds its range + halo at range_offset (include/density_b200.h).
@@ -1762,34 +1631,23 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
                                                uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags,
                                                uint64_t* d_total_size, void* stream_v) {
     g_last_error.clear();
-    if (!h || (!d_in && n_range + n_halo) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-    NcclApi* a = h->world > 1 ? nccl_api() : nullptr;
-    if (h->world > 1 && !a) { set_error("NCCL is not available"); return DENSITY_B200_ECUDA; }
-    constexpr size_t MW = DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS;
-    density_b200_cheetah_decode_shard* s = sharded_cdec(h);
-    ShardedAux x;
+    int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h))) != DENSITY_B200_OK) return rc;
     // sized for the locate scratch and for the phases on any piece of range + halo, so that phase 1 does not reallocate
     const size_t locate_bytes = chee_locate_workspace_bytes(n_range, n_halo, range_offset);
     const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms);
-    cudaError_t e = s->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, st);
-    if (e == cudaSuccess) e = sharded_aux(h, st, &x);    // its map slots hold DENSITY_B200_LOCATE_MAP_WORDS >= MW words per rank
+    const cudaError_t e = h->cdec->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, x.st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t* my_map = x.maps + (size_t)h->rank * MW;
-    uint64_t launches = 0;
-    e = chee_decode_locate(d_in, n_range, n_halo, range_offset, s->ws.p, my_map, st, &launches);
-    g_launches += launches;
-    if (e != cudaSuccess) { set_error("cheetah decode locate", e); return DENSITY_B200_ECUDA; }
-    if (h->world > 1 && !nccl_check(a->AllGather(my_map, x.maps, MW * 8, NCCL_UINT8, h->comm, st), "ncclAllGather(maps)")) return DENSITY_B200_ECUDA;
-    e = cudaMemcpyAsync(h->h_maps, x.maps, (size_t)h->world * MW * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("range maps to host", e); return DENSITY_B200_ECUDA; }
+    constexpr size_t MW = DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS;    // the map slots hold DENSITY_B200_LOCATE_MAP_WORDS >= MW words per rank
+    if ((rc = density_b200_cheetah_decode_locate(h->cdec, d_in, n_range, n_halo, range_offset, x.maps + (size_t)h->rank * MW, x.st)) != DENSITY_B200_OK ||
+        (rc = x.maps_to_host(MW)) != DENSITY_B200_OK)
+        return rc;
     uint64_t piece[5];
-    const int rc = density_b200_cheetah_locate_piece(h->h_maps, h->world, h->rank, piece);
+    rc = density_b200_cheetah_locate_piece(h->h_maps, h->world, h->rank, piece);
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
-    return decode_sharded_cheetah_piece(h, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
-                                        d_flags, d_total_size, d_out_offset, st);
+    return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
+                                        d_flags, d_total_size, d_out_offset);
 }
 
 /* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag
@@ -1913,17 +1771,13 @@ size_t density_b200_codec_decode(density_b200_codec* h, const uint8_t* in, size_
 
 int density_b200_table_init(uint32_t* d_table, void* stream) {
     uint64_t l = 0;
-    cudaError_t e = cham_table_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("table_init", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = cham_table_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "table_init");
 }
 int density_b200_table_fold(uint32_t* d_acc, const uint32_t* d_next, void* stream) {
     uint64_t l = 0;
-    cudaError_t e = cham_table_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
-    g_launches += l;
-    if (e != cudaSuccess) { set_error("table_fold", e); return DENSITY_B200_ECUDA; }
-    return DENSITY_B200_OK;
+    const cudaError_t e = cham_table_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
+    return step_result(e, l, "table_fold");
 }
 
 // ---- per-stage device timing of the last Chameleon encode (bench.py's roofline) -----------------------------

@@ -49,6 +49,33 @@ TABLE_ENTRIES = 65536
 TOUCHED = 0x10000
 
 
+def _rank_world(group=None):
+    """(rank, world) of this process in `group`; (0, 1) without torch.distributed"""
+    if not dist.is_initialized():
+        return 0, 1
+    return dist.get_rank(group), dist.get_world_size(group)
+
+
+def _stream():
+    """torch's current CUDA stream, as the library takes it"""
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _check(rc, what):
+    if rc:
+        raise _lib.DensityB200Error(f"{what} rc={rc}: {_lib.last_error()}")
+
+
+def gather_rows(t, group=None):
+    """all_gather of every rank's `t`: [world, t.numel()] in rank order (world 1: a view of t)"""
+    world = _rank_world(group)[1]
+    if world == 1:
+        return t.view(1, -1)
+    out = torch.empty((world, t.numel()), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out.view(-1), t.contiguous(), group=group)
+    return out
+
+
 def initial_table(device):
     """Dictionary state at the stream start: only bucket 0 'holds quad 0' (chameleon.rs:41,89-91)."""
     t = torch.zeros(TABLE_ENTRIES, dtype=torch.int32, device=device)
@@ -67,22 +94,7 @@ def fold_tables(gathered, rank):
     return carry
 
 
-def exchange_tables(table, group=None):
-    world = dist.get_world_size(group)
-    gathered = torch.empty((world, TABLE_ENTRIES), dtype=torch.int32, device=table.device)
-    dist.all_gather_into_tensor(gathered.view(-1), table.contiguous(), group=group)
-    return gathered
-
-
 SEAM_WORDS = 8
-
-
-def exchange_seam_words(words, group=None):
-    """all_gather of every rank's 8 seam words: int32 [world, 8]."""
-    world = dist.get_world_size(group)
-    gathered = torch.empty((world, SEAM_WORDS), dtype=torch.int32, device=words.device)
-    dist.all_gather_into_tensor(gathered.view(-1), words.contiguous(), group=group)
-    return gathered
 
 
 def seam_verdict(words):
@@ -166,22 +178,23 @@ def locate_piece(maps, rank, alg="chameleon"):
     out = (ctypes.c_uint64 * nout)()
     lib = _lib.load()
     fn = lib.density_b200_cheetah_locate_piece if cheetah else lib.density_b200_locate_piece
-    rc = fn(m.ctypes.data, m.shape[0], rank, out)
-    if rc:
-        raise _lib.DensityB200Error(f"locate_piece rc={rc}: {_lib.last_error()}")
+    _check(fn(m.ctypes.data, m.shape[0], rank, out), "locate_piece")
     return tuple(int(v) for v in out)
 
 
-class ShardedChameleonEncoder:
-    def __init__(self):
+class _Handle:
+    """Owns one library handle: made by `create`, freed by `destroy` on close() or when the object is collected."""
+
+    def _open(self, create, destroy, *args):
         self._lib = _lib.load()
-        self._h = self._lib.density_b200_shard_create()
+        self._destroy = getattr(self._lib, destroy)
+        self._h = getattr(self._lib, create)(*args)
         if not self._h:
             raise _lib.DensityB200Error(_lib.last_error())
 
     def close(self):
-        if self._h:
-            self._lib.density_b200_shard_destroy(self._h)
+        if getattr(self, "_h", None):
+            self._destroy(self._h)
             self._h = None
 
     def __del__(self):
@@ -190,30 +203,26 @@ class ShardedChameleonEncoder:
         except Exception:
             pass
 
+
+class ShardedChameleonEncoder(_Handle):
+    def __init__(self):
+        self._open("density_b200_shard_create", "density_b200_shard_destroy")
+
     def encode_protected(self, d_in, d_out, d_size, group=None):
         """The copy-mode path (density_b200_shard_prot_*): d_in / d_out / d_size as in encode, any input. Runs the round budget of the
         copy-map iteration with torch.distributed exchanges (tables, transfers, round words) and the device folds. Returns
         seam_verdict's (flags, total, offsets) over all ranks; flags != 0 only when the map did not settle, the automaton left the
         candidate states, or on an error: the pieces are then void."""
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rank, world = _rank_world(group)
+        stream = _stream()
         dev = d_in.device
         lib = self._lib
 
-        def gather(t):
-            if world == 1:
-                return t.view(1, -1)
-            out = torch.empty((world, t.numel()), dtype=t.dtype, device=dev)
-            dist.all_gather_into_tensor(out.view(-1), t.contiguous(), group=group)
-            return out
-
         def check(rc, what):
-            if rc:
-                raise _lib.DensityB200Error(f"shard_prot_{what} rc={rc}: {_lib.last_error()}")
+            _check(rc, f"shard_prot_{what}")
 
         n = d_in.numel()
-        first_block = int(gather(torch.tensor([n], dtype=torch.int64, device=dev))[:rank].sum()) // 256
+        first_block = int(gather_rows(torch.tensor([n], dtype=torch.int64, device=dev), group)[:rank].sum()) // 256
         table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=dev)
         transfer = torch.empty(PROT_TRANSFER_WORDS, dtype=torch.int32, device=dev)
         words = torch.empty(PROT_ROUND_WORDS, dtype=torch.int32, device=dev)
@@ -223,25 +232,23 @@ class ShardedChameleonEncoder:
         for k in range(lib.density_b200_prot_round_budget()):
             if k:
                 check(lib.density_b200_shard_prot_next(self._h, all_words.data_ptr(), world, table.data_ptr(), stream), "next")
-            carry = fold_tables(gather(table), rank).contiguous()
+            carry = fold_tables(gather_rows(table, group), rank).contiguous()
             check(lib.density_b200_shard_prot_transfer(self._h, carry.data_ptr(), transfer.data_ptr(), stream), "transfer")
-            all_transfers = gather(transfer).contiguous()
+            all_transfers = gather_rows(transfer, group).contiguous()
             check(lib.density_b200_shard_prot_settle(self._h, all_transfers.data_ptr(), world, rank, words.data_ptr(), stream), "settle")
-            all_words = gather(words).contiguous()
+            all_words = gather_rows(words, group).contiguous()
         check(lib.density_b200_shard_prot_next(self._h, all_words.data_ptr(), world, None, stream), "next")
         seam = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
         check(lib.density_b200_shard_prot_finish(self._h, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), seam.data_ptr(), stream),
               "finish")
-        return seam_verdict(gather(seam))
+        return seam_verdict(gather_rows(seam, group))
 
     def prot_status(self):
         """density_b200_shard_prot_status after encode_protected (waits for the device): dict with rounds (until settled, 0: not
         settled), settled, in_state ((penalty, start, previous_incompressible) entering the shard, None: left the candidates), esc and
         changed (this shard's blocks whose copy status changed, per round, 16 values)."""
         out = (ctypes.c_uint32 * PROT_STATUS_WORDS)()
-        rc = self._lib.density_b200_shard_prot_status(self._h, out)
-        if rc:
-            raise _lib.DensityB200Error(f"shard_prot_status rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_shard_prot_status(self._h, out), "shard_prot_status")
         v = list(out)
         ins = None if v[2] == 0xFFFFFFFF else (v[2] & 0xFF, (v[2] >> 8) & 0xFF, v[2] >> 16)
         return {"rounds": v[0], "settled": v[1], "in_state": ins, "esc": v[3], "changed": v[4:20]}
@@ -249,24 +256,18 @@ class ShardedChameleonEncoder:
     def encode(self, d_in, d_out, d_size, d_flags, group=None):
         """d_in / d_out: CUDA uint8 tensors (this rank's shard / its output buffer); d_size: int64[1]; d_flags: int32[1].
         Everything is enqueued on torch's current stream; the all_gather is the only collective."""
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rank, world = _rank_world(group)
+        stream = _stream()
         table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=d_in.device)
-        rc = self._lib.density_b200_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), int(rank == world - 1),
-                                                 table.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"shard_phase1 rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), int(rank == world - 1), table.data_ptr(), stream),
+               "shard_phase1")
+        gathered = gather_rows(table, group)
         carry_ptr = None
-        if world > 1:
-            gathered = exchange_tables(table, group)
-            if rank > 0:
-                self._carry = fold_tables(gathered, rank)
-                carry_ptr = self._carry.data_ptr()
-        rc = self._lib.density_b200_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(),
-                                                 d_flags.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"shard_phase2 rc={rc}: {_lib.last_error()}")
+        if rank > 0:
+            self._carry = fold_tables(gathered, rank)
+            carry_ptr = self._carry.data_ptr()
+        _check(self._lib.density_b200_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
+                                                   stream), "shard_phase2")
 
 
 ALGS = {"chameleon": 0, "cheetah": 1, "lion": 2}
@@ -277,21 +278,27 @@ def _alg_id(alg):
     return ALGS[alg] if isinstance(alg, str) else int(alg)
 
 
+def _fold_on_device(gathered, rank, init, fold, what):
+    """carry-in of `rank`: the stream-start state (init) folded with the rows of ranks < rank in order (fold), enqueued on torch's
+    current stream. gathered: CUDA int32 [world, words]."""
+    stream = _stream()
+    carry = torch.empty(gathered.shape[1], dtype=torch.int32, device=gathered.device)
+    rc = init(carry.data_ptr(), stream)
+    for r in range(rank):
+        if rc == 0:
+            rc = fold(carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
+    _check(rc, what)
+    return carry
+
+
 def fold_cl_tables(alg, kind, gathered, rank):
     """carry-in of `rank` for the Cheetah / Lion sharded encode: the stream-start state (density_b200_cl_table_init) folded with the
     tables of ranks < rank in order (density_b200_cl_table_fold). gathered: CUDA int32 [world, words]. Enqueued on torch's current
     stream."""
     lib = _lib.load()
     alg = _alg_id(alg)
-    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    carry = torch.empty(gathered.shape[1], dtype=torch.int32, device=gathered.device)
-    rc = lib.density_b200_cl_table_init(alg, kind, carry.data_ptr(), stream)
-    for r in range(rank):
-        if rc == 0:
-            rc = lib.density_b200_cl_table_fold(alg, kind, carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
-    if rc:
-        raise _lib.DensityB200Error(f"cl_table_init / fold rc={rc}: {_lib.last_error()}")
-    return carry
+    return _fold_on_device(gathered, rank, lambda acc, st: lib.density_b200_cl_table_init(alg, kind, acc, st),
+                           lambda acc, nxt, st: lib.density_b200_cl_table_fold(alg, kind, acc, nxt, st), "cl_table_init / fold")
 
 
 def fold_cheetah_cmap(gathered, rank):
@@ -299,58 +306,29 @@ def fold_cheetah_cmap(gathered, rank):
     the chunk-map transfers of pieces < rank in order (density_b200_cheetah_cmap_fold). gathered: CUDA int32 [world, 3 * 65536].
     Enqueued on torch's current stream."""
     lib = _lib.load()
-    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    carry = torch.empty(gathered.shape[1], dtype=torch.int32, device=gathered.device)
-    rc = lib.density_b200_cheetah_cmap_init(carry.data_ptr(), stream)
-    for r in range(rank):
-        if rc == 0:
-            rc = lib.density_b200_cheetah_cmap_fold(carry.data_ptr(), gathered[r].contiguous().data_ptr(), stream)
-    if rc:
-        raise _lib.DensityB200Error(f"cheetah_cmap_init / fold rc={rc}: {_lib.last_error()}")
-    return carry
+    return _fold_on_device(gathered, rank, lib.density_b200_cheetah_cmap_init, lib.density_b200_cheetah_cmap_fold,
+                           "cheetah_cmap_init / fold")
 
 
-class ShardedCLEncoder:
+class ShardedCLEncoder(_Handle):
     """Sharded Cheetah / Lion encode through the shard phases, with torch.distributed for the exchanges (the phase-level twin of
     ShardedEncoder.encode(..., alg=...)). Rank r's d_in is bytes [o_r, o_r + n_r) of one input; non-final shards are multiples of 256
     bytes. The concatenation of the pieces equals one cheetah_encode / lion_encode call over the whole input when flags == 0."""
 
     def __init__(self, alg):
-        self._lib = _lib.load()
         self.alg = _alg_id(alg)
-        self._h = self._lib.density_b200_cl_shard_create(self.alg)
-        if not self._h:
-            raise _lib.DensityB200Error(_lib.last_error())
+        self._open("density_b200_cl_shard_create", "density_b200_cl_shard_destroy", self.alg)
         self.words_p = self._lib.density_b200_cl_table_words(self.alg, CL_TABLE_P)
         self.words_c = self._lib.density_b200_cl_table_words(self.alg, CL_TABLE_C)
         self.events = None
-
-    def close(self):
-        if self._h:
-            self._lib.density_b200_cl_shard_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _gather(self, t, world, group):
-        if world == 1:
-            return t.view(1, -1)
-        out = torch.empty((world, t.numel()), dtype=t.dtype, device=t.device)
-        dist.all_gather_into_tensor(out.view(-1), t.contiguous(), group=group)
-        return out
 
     def encode(self, d_in, d_out, d_size, group=None, timing=False):
         """d_in: CUDA uint8 tensor (4-byte aligned), this rank's shard; d_out: its output buffer (2-byte aligned); d_size: int64[1].
         Returns seam_verdict's (flags, total, offsets) over all ranks; flags != 0: the pieces are void and the caller encodes on one
         device. timing: record CUDA events around the phases in self.events (phase 1, P exchange + fold, phase 2, C exchange + fold,
         phase 3 + seams)."""
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rank, world = _rank_world(group)
+        stream = _stream()
         dev = d_in.device
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)] if timing else None
         mark = (lambda k: ev[k].record()) if timing else (lambda k: None)
@@ -359,7 +337,7 @@ class ShardedCLEncoder:
         if n >= 4:
             last[0] = 1
             last[1:] = d_in[n // 4 * 4 - 4:n // 4 * 4].clone().view(torch.int32)
-        quads = self._gather(last, world, group)
+        quads = gather_rows(last, group)
         prev = None
         if rank > 0:
             prev = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -367,26 +345,21 @@ class ShardedCLEncoder:
                 prev = torch.where(quads[r, 0] != 0, quads[r, 1:2], prev)
         mark(0)
         tp = torch.empty(self.words_p, dtype=torch.int32, device=dev)
-        rc = self._lib.density_b200_cl_shard_phase1(self._h, d_in.data_ptr(), n, int(rank == world - 1),
-                                                    prev.data_ptr() if prev is not None else None, tp.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"cl_shard_phase1 rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_cl_shard_phase1(self._h, d_in.data_ptr(), n, int(rank == world - 1),
+                                                      prev.data_ptr() if prev is not None else None, tp.data_ptr(), stream), "cl_shard_phase1")
         mark(1)
-        carry_p = fold_cl_tables(self.alg, CL_TABLE_P, self._gather(tp, world, group), rank) if rank > 0 else None
+        carry_p = fold_cl_tables(self.alg, CL_TABLE_P, gather_rows(tp, group), rank) if rank > 0 else None
         mark(2)
         tc = torch.empty(self.words_c, dtype=torch.int32, device=dev)
-        rc = self._lib.density_b200_cl_shard_phase2(self._h, carry_p.data_ptr() if carry_p is not None else None, tc.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"cl_shard_phase2 rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_cl_shard_phase2(self._h, carry_p.data_ptr() if carry_p is not None else None, tc.data_ptr(), stream),
+               "cl_shard_phase2")
         mark(3)
-        carry_c = fold_cl_tables(self.alg, CL_TABLE_C, self._gather(tc, world, group), rank) if rank > 0 else None
+        carry_c = fold_cl_tables(self.alg, CL_TABLE_C, gather_rows(tc, group), rank) if rank > 0 else None
         mark(4)
         words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
-        rc = self._lib.density_b200_cl_shard_phase3(self._h, carry_c.data_ptr() if carry_c is not None else None, d_out.data_ptr(),
-                                                    d_out.numel(), d_size.data_ptr(), words.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"cl_shard_phase3 rc={rc}: {_lib.last_error()}")
-        verdict = seam_verdict(self._gather(words, world, group))
+        _check(self._lib.density_b200_cl_shard_phase3(self._h, carry_c.data_ptr() if carry_c is not None else None, d_out.data_ptr(),
+                                                      d_out.numel(), d_size.data_ptr(), words.data_ptr(), stream), "cl_shard_phase3")
+        verdict = seam_verdict(gather_rows(words, group))
         mark(5)
         self.events = ev
         return verdict
@@ -397,32 +370,17 @@ class ShardedCLEncoder:
         return [self.events[k].elapsed_time(self.events[k + 1]) for k in range(5)]
 
 
-class ShardedChameleonDecoder:
+class ShardedChameleonDecoder(_Handle):
     """Decode of this rank's piece through the shard phases, with torch.distributed for the exchanges (the mirror of
     ShardedChameleonEncoder)."""
 
     def __init__(self):
-        self._lib = _lib.load()
-        self._h = self._lib.density_b200_decode_shard_create()
-        if not self._h:
-            raise _lib.DensityB200Error(_lib.last_error())
-
-    def close(self):
-        if self._h:
-            self._lib.density_b200_decode_shard_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open("density_b200_decode_shard_create", "density_b200_decode_shard_destroy")
 
     def decode(self, d_in, d_out, d_size, group=None):
         """d_in: CUDA uint8 tensor, this rank's piece (2-byte aligned); d_out: uint8 tensor of capacity d_out.numel() (4-byte aligned);
         d_size: int64[1]. Returns seam_verdict's (flags, total, offsets) over all ranks; flags != 0: the pieces are void."""
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        rank, world = _rank_world(group)
         return self._decode_piece(d_in, d_out, d_size, rank == world - 1, group)
 
     def decode_stream(self, d_in, n_range, d_out, d_size, group=None):
@@ -430,83 +388,54 @@ class ShardedChameleonDecoder:
         followed by its halo (stream_ranges gives the layout); d_out, d_size as in decode. Locates the piece (one host synchronisation
         for the maps) and decodes it. Returns (flags, total, offsets, my_offset): seam_verdict's result and where this rank's output
         starts in the original bytes; flags != 0: the pieces are void and the caller decodes the whole stream on one device."""
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rank = _rank_world(group)[0]
         n_halo = d_in.numel() - n_range
         if n_halo < 0:
             raise ValueError("d_in is shorter than its range")
         m = torch.empty(LOCATE_MAP_WORDS, dtype=torch.int64, device=d_in.device)
-        rc = self._lib.density_b200_decode_locate(self._h, d_in.data_ptr(), n_range, n_halo, m.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"decode_locate rc={rc}: {_lib.last_error()}")
-        if world > 1:
-            maps = torch.empty((world, LOCATE_MAP_WORDS), dtype=torch.int64, device=d_in.device)
-            dist.all_gather_into_tensor(maps.view(-1), m, group=group)
-        else:
-            maps = m.view(1, LOCATE_MAP_WORDS)
+        _check(self._lib.density_b200_decode_locate(self._h, d_in.data_ptr(), n_range, n_halo, m.data_ptr(), _stream()), "decode_locate")
+        maps = gather_rows(m, group)
         start, end, _, is_final = locate_piece(maps.cpu().numpy().view(np.uint64), rank)
         flags, total, offsets = self._decode_piece(d_in[start:end], d_out, d_size, bool(is_final), group)
         return flags, total, offsets, int(offsets[rank])
 
     def _decode_piece(self, d_in, d_out, d_size, is_last, group):
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        rank = _rank_world(group)[0]
+        stream = _stream()
         table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=d_in.device)
-        rc = self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last),
-                                                        table.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"decode_shard_phase1 rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last),
+                                                          table.data_ptr(), stream), "decode_shard_phase1")
+        gathered = gather_rows(table, group)
         carry_ptr = None
-        if world > 1:
-            gathered = exchange_tables(table, group)
-            if rank > 0:
-                self._carry = fold_tables(gathered, rank)
-                carry_ptr = self._carry.data_ptr()
+        if rank > 0:
+            self._carry = fold_tables(gathered, rank)
+            carry_ptr = self._carry.data_ptr()
         words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=d_in.device)
-        rc = self._lib.density_b200_decode_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"decode_shard_phase2 rc={rc}: {_lib.last_error()}")
-        return seam_verdict(exchange_seam_words(words, group) if world > 1 else words.view(1, SEAM_WORDS))
+        _check(self._lib.density_b200_decode_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream),
+               "decode_shard_phase2")
+        return seam_verdict(gather_rows(words, group))
 
 
-class _ShardedHandle:
+class _ShardedHandle(_Handle):
     """A `density_b200_sharded` handle: one process per GPU; the library owns its NCCL communicator (the 128-byte id travels once
     through torch.distributed). torch.distributed is only used to hand out the id."""
 
     def __init__(self, device, group=None):
-        self._lib = _lib.load()
-        self.rank = dist.get_rank(group) if dist.is_initialized() else 0
-        self.world = dist.get_world_size(group) if dist.is_initialized() else 1
+        self.rank, self.world = _rank_world(group)
         ident = torch.zeros(128, dtype=torch.uint8)
         if self.world > 1:
             if self.rank == 0:
                 buf = (ctypes.c_uint8 * 128)()
-                rc = self._lib.density_b200_sharded_unique_id(buf)
-                if rc:
-                    raise _lib.DensityB200Error(f"sharded_unique_id rc={rc}: {_lib.last_error()}")
+                _check(_lib.load().density_b200_sharded_unique_id(buf), "sharded_unique_id")
                 ident = torch.tensor(list(buf), dtype=torch.uint8)
             t = ident.to(device) if dist.get_backend(group) == "nccl" else ident
             dist.broadcast(t, src=0, group=group)
             ident = t.cpu()
         self._id = ident.contiguous()
-        self._h = self._lib.density_b200_sharded_create(self._id.data_ptr() if self.world > 1 else None, self.rank, self.world)
-        if not self._h:
-            raise _lib.DensityB200Error(_lib.last_error())
+        self._open("density_b200_sharded_create", "density_b200_sharded_destroy", self._id.data_ptr() if self.world > 1 else None,
+                   self.rank, self.world)
         self.d_total = torch.zeros(1, dtype=torch.int64, device=device)
         self.d_offset = torch.zeros(1, dtype=torch.int64, device=device)
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.density_b200_sharded_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class ShardedEncoder(_ShardedHandle):
@@ -518,35 +447,28 @@ class ShardedEncoder(_ShardedHandle):
         """Enqueue on torch's current stream. d_size int64[1]: this rank's piece; d_flags int32[1]: != 0 -> the stream is not quiet and
         the pieces are void; self.d_total int64[1]: stream length. gather_root >= 0: pieces gathered into d_gather on that rank (blocks).
         alg "cheetah" / "lion" (or their ids): density_b200_encode_sharded_cl, the same contract for those algorithms."""
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         args = (d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(),
-                int(gather_root), d_gather.data_ptr() if d_gather is not None else None, d_gather.numel() if d_gather is not None else 0, stream)
+                int(gather_root), d_gather.data_ptr() if d_gather is not None else None, d_gather.numel() if d_gather is not None else 0, _stream())
         alg = _alg_id(alg)
         if alg == 0:
             rc = self._lib.density_b200_encode_sharded(self._h, *args)
         else:
             rc = self._lib.density_b200_encode_sharded_cl(self._h, alg, *args)
-        if rc:
-            raise _lib.DensityB200Error(f"encode_sharded{'' if alg == 0 else '_cl'} rc={rc}: {_lib.last_error()}")
+        _check(rc, f"encode_sharded{'' if alg == 0 else '_cl'}")
 
     def encode_protected(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None):
         """density_b200_encode_sharded_protected: Chameleon with copy mode, the arguments of encode. d_flags != 0 only when the copy map
         did not settle within the round budget, the automaton left the candidate states, or on an error: the pieces are then void."""
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self._lib.density_b200_encode_sharded_protected(
+        _check(self._lib.density_b200_encode_sharded_protected(
             self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
             self.d_total.data_ptr(), int(gather_root), d_gather.data_ptr() if d_gather is not None else None,
-            d_gather.numel() if d_gather is not None else 0, stream)
-        if rc:
-            raise _lib.DensityB200Error(f"encode_sharded_protected rc={rc}: {_lib.last_error()}")
+            d_gather.numel() if d_gather is not None else 0, _stream()), "encode_sharded_protected")
 
     def profile(self):
         """stage times (ms) of the last encode: Chameleon flag pass, table exchange + fold, carry / resolve / sizes / scan, emit, seams +
         gather; Cheetah / Lion phase 1, P exchange + fold, phase 2 + C exchange + fold, phase 3, seams + gather"""
         out = (ctypes.c_float * 5)()
-        rc = self._lib.density_b200_sharded_profile(self._h, out)
-        if rc:
-            raise _lib.DensityB200Error(f"sharded_profile rc={rc}: {_lib.last_error()}")
+        _check(self._lib.density_b200_sharded_profile(self._h, out), "sharded_profile")
         return [float(x) for x in out]
 
 
@@ -562,12 +484,9 @@ class ShardedDecoder(_ShardedHandle):
         alg = _alg_id(alg)
         if alg not in (0, 1):
             raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         fn = self._lib.density_b200_decode_sharded if alg == 0 else self._lib.density_b200_decode_sharded_cheetah
-        rc = fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
-                self.d_total.data_ptr(), stream)
-        if rc:
-            raise _lib.DensityB200Error(f"decode_sharded{'' if alg == 0 else '_cheetah'} rc={rc}: {_lib.last_error()}")
+        _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
+                  self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}")
 
     def decode_stream(self, d_in, n_range, d_out, d_size, d_flags, alg="chameleon", range_offset=None):
         """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range
@@ -580,11 +499,9 @@ class ShardedDecoder(_ShardedHandle):
         if alg == 1 and range_offset is None:
             raise ValueError("sharded Cheetah stream decode: range_offset is required")
         n_halo = d_in.numel() - n_range
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        tail = (d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), stream)
+        tail = (d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), _stream())
         if alg == 0:
             rc = self._lib.density_b200_decode_sharded_stream(self._h, d_in.data_ptr(), n_range, n_halo, *tail)
         else:
             rc = self._lib.density_b200_decode_sharded_cheetah_stream(self._h, d_in.data_ptr(), n_range, n_halo, int(range_offset), *tail)
-        if rc:
-            raise _lib.DensityB200Error(f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream rc={rc}: {_lib.last_error()}")
+        _check(rc, f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream")

@@ -642,9 +642,11 @@ def test_cheetah_round_trip_1gib_text_parallel_decoder(torch_cuda, codecs):
 
 def test_encode_sharded_cpp_entry_world1(torch_cuda, codecs):
     """density_b200_encode_sharded (C++: phase 1 -> fold kernel -> phase 2 -> seam verdict -> gather) with one rank: the piece and the
-    gathered stream equal the oracle's; a non-quiet shard is reported, not emitted silently."""
+    gathered stream equal the oracle's; a non-quiet shard is reported, not emitted silently. Both calls launch 11 kernels."""
     torch = torch_cuda
+    import density_b200
     from density_b200 import sharded, synth
+    lib = density_b200.load()
     n = 5 * (1 << 20) + 1021
     data = synth.synth_text(n).numpy()
     want = oracle.encode("chameleon", data)
@@ -654,13 +656,17 @@ def test_encode_sharded_cpp_entry_world1(torch_cuda, codecs):
     d_gather = torch.zeros(d_out.numel(), dtype=torch.uint8, device="cuda")
     d_sz = torch.zeros(1, dtype=torch.int64, device="cuda")
     d_fl = torch.ones(1, dtype=torch.int32, device="cuda")
+    before = lib.density_b200_kernel_launches()
     enc.encode(d_in, d_out, d_sz, d_fl, gather_root=0, d_gather=d_gather)
+    assert lib.density_b200_kernel_launches() - before == 11
     torch.cuda.synchronize()
     assert int(d_fl.item()) == 0 and int(d_sz.item()) == want.size == int(enc.d_total.item())
     assert (d_out[:want.size].cpu().numpy() == want).all() and (d_gather[:want.size].cpu().numpy() == want).all()
     bad = payload("random", 1 << 20, 3)
     d_in2 = torch.from_numpy(bad.copy()).cuda()
+    before = lib.density_b200_kernel_launches()
     enc.encode(d_in2, d_out, d_sz, d_fl)
+    assert lib.density_b200_kernel_launches() - before == 11
     torch.cuda.synchronize()
     assert int(d_fl.item()) != 0
     enc.close()

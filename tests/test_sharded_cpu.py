@@ -31,14 +31,14 @@ def _worker(rank, world, port, shards, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from density_b200 import sharded
     table = torch.from_numpy(last_writer_table(shards[rank]))
-    gathered = sharded.exchange_tables(table)
+    gathered = sharded.gather_rows(table)
     carry = sharded.fold_tables(gathered, rank)
     q.put((rank, carry.numpy().copy()))
     dist.barrier()
     dist.destroy_process_group()
 
 
-def test_exchange_and_fold_world2_gloo():
+def test_gather_rows_and_fold_world2_gloo():
     world = 2
     data = payload("text", 2 * 65536, 4)
     shards = [data[:65536], data[65536:]]

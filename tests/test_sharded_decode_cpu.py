@@ -51,14 +51,14 @@ def _worker(rank, world, port, rows, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from density_b200 import sharded
     mine = words(rows[rank])[0]
-    gathered = sharded.exchange_seam_words(mine)
+    gathered = sharded.gather_rows(mine)
     flags, total, offsets = sharded.seam_verdict(gathered)
     q.put((rank, gathered.numpy().copy(), flags, total, offsets.tolist()))
     dist.barrier()
     dist.destroy_process_group()
 
 
-def test_seam_word_exchange_world2_gloo():
+def test_seam_word_gather_rows_world2_gloo():
     world = 2
     rows = [(0, 1, 0, 1, 1 << 20), (1, 0, 0, 1, 4099)]
     ctx = mp.get_context("spawn")

@@ -103,6 +103,7 @@ _SIGS = {
     "density_b200_test_set_stage_rounds": (None, [ctypes.c_int]),
     "density_b200_test_set_decode_rounds": (None, [ctypes.c_int]),
     "density_b200_test_set_prot_rounds": (None, [ctypes.c_int]),
+    "density_b200_test_set_nccl_library": (ctypes.c_int, [ctypes.c_char_p]),
     "density_b200_prot_debug": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_shutdown": (None, []),
     "density_b200_version": (ctypes.c_char_p, []),

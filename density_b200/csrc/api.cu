@@ -1077,26 +1077,34 @@ struct NcclApi {
     const char* (*GetErrorString)(int) = nullptr;
     bool ok = false;
 };
+NcclApi g_nccl;                     // the resolved table
+bool g_nccl_resolved = false;       // false: resolve libnccl.so.2 on the next use
+std::mutex g_nccl_mu;
+std::atomic<int> g_nccl_handles{0}; // live handles with world > 1: the table they use must not change under them
+NcclApi nccl_resolve(void* h) {
+    NcclApi api;
+    auto sym = [&](const char* n) { return dlsym(h, n); };
+    api.GetUniqueId = reinterpret_cast<decltype(api.GetUniqueId)>(sym("ncclGetUniqueId"));
+    api.CommInitRank = reinterpret_cast<decltype(api.CommInitRank)>(sym("ncclCommInitRank"));
+    api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(sym("ncclCommDestroy"));
+    api.AllGather = reinterpret_cast<decltype(api.AllGather)>(sym("ncclAllGather"));
+    api.Send = reinterpret_cast<decltype(api.Send)>(sym("ncclSend"));
+    api.Recv = reinterpret_cast<decltype(api.Recv)>(sym("ncclRecv"));
+    api.GroupStart = reinterpret_cast<decltype(api.GroupStart)>(sym("ncclGroupStart"));
+    api.GroupEnd = reinterpret_cast<decltype(api.GroupEnd)>(sym("ncclGroupEnd"));
+    api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(sym("ncclGetErrorString"));
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.Send && api.Recv && api.GroupStart && api.GroupEnd;
+    return api;
+}
 NcclApi* nccl_api() {
-    static NcclApi api;
-    static std::once_flag once;
-    std::call_once(once, [] {
+    std::lock_guard<std::mutex> lk(g_nccl_mu);
+    if (!g_nccl_resolved) {
+        g_nccl_resolved = true;
         void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);
         if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-        if (!h) return;
-        auto sym = [&](const char* n) { return dlsym(h, n); };
-        api.GetUniqueId = reinterpret_cast<decltype(api.GetUniqueId)>(sym("ncclGetUniqueId"));
-        api.CommInitRank = reinterpret_cast<decltype(api.CommInitRank)>(sym("ncclCommInitRank"));
-        api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(sym("ncclCommDestroy"));
-        api.AllGather = reinterpret_cast<decltype(api.AllGather)>(sym("ncclAllGather"));
-        api.Send = reinterpret_cast<decltype(api.Send)>(sym("ncclSend"));
-        api.Recv = reinterpret_cast<decltype(api.Recv)>(sym("ncclRecv"));
-        api.GroupStart = reinterpret_cast<decltype(api.GroupStart)>(sym("ncclGroupStart"));
-        api.GroupEnd = reinterpret_cast<decltype(api.GroupEnd)>(sym("ncclGroupEnd"));
-        api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(sym("ncclGetErrorString"));
-        api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.Send && api.Recv && api.GroupStart && api.GroupEnd;
-    });
-    return api.ok ? &api : nullptr;
+        if (h) g_nccl = nccl_resolve(h);
+    }
+    return g_nccl.ok ? &g_nccl : nullptr;
 }
 bool nccl_check(int rc, const char* what) {
     if (rc == 0) return true;
@@ -1106,6 +1114,23 @@ bool nccl_check(int rc, const char* what) {
     return false;
 }
 }  // namespace
+
+int density_b200_test_set_nccl_library(const char* path) {
+    g_last_error.clear();
+    std::lock_guard<std::mutex> lk(g_nccl_mu);
+    if (g_nccl_handles.load()) { set_error("test_set_nccl_library: a sharded handle with world > 1 is alive"); return DENSITY_B200_EARG; }
+    if (!path) { g_nccl = NcclApi(); g_nccl_resolved = false; return DENSITY_B200_OK; }
+    void* h = dlopen(path, RTLD_NOW | RTLD_LOCAL);
+    if (!h) { set_error(dlerror()); return DENSITY_B200_EARG; }
+    const NcclApi api = nccl_resolve(h);
+    if (!api.ok || !api.GetErrorString) {
+        dlclose(h);
+        set_error("test_set_nccl_library: the library lacks an NCCL symbol the sharded drivers use");
+        return DENSITY_B200_EARG;
+    }
+    g_nccl = api; g_nccl_resolved = true;      // the library stays loaded: error strings of earlier calls may point into it
+    return DENSITY_B200_OK;
+}
 
 struct density_b200_sharded {
     int rank = 0, world = 1, num_sms = 0;
@@ -1145,6 +1170,7 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
         if (!a || !nccl_unique_id_128) { set_error("NCCL is not available / no unique id"); delete h; return nullptr; }
         nccl_unique_id id; memcpy(id.internal, nccl_unique_id_128, 128);
         if (!nccl_check(a->CommInitRank(&h->comm, world, id, rank), "ncclCommInitRank")) { delete h; return nullptr; }
+        ++g_nccl_handles;
     }
     if (cudaMallocHost(&h->h_offsets, sizeof(uint64_t) * (world + 2)) != cudaSuccess ||
         cudaMallocHost(&h->h_maps, sizeof(uint64_t) * DENSITY_B200_LOCATE_MAP_WORDS * world) != cudaSuccess) {
@@ -1161,7 +1187,7 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
 
 void density_b200_sharded_destroy(density_b200_sharded* h) {
     if (!h) return;
-    if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); }
+    if (h->comm) { NcclApi* a = nccl_api(); if (a) a->CommDestroy(h->comm); --g_nccl_handles; }
     h->aux.release();
     density_b200_shard_destroy(h->enc);
     density_b200_shard_destroy(h->prot);
@@ -1228,19 +1254,23 @@ struct Exchange {
     }
 };
 
-// variable-length gather of the pieces to `gather_root` at their stream offsets (d_offsets: world + 1 prefix sums, on the device); blocks
-static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_offsets, const uint8_t* d_out, int gather_root, uint8_t* d_gather,
-                         size_t gather_cap, cudaStream_t st) {
+// variable-length gather of the pieces to `gather_root` at their stream offsets (d_offsets: world + 1 prefix sums, d_words: the gathered
+// seam words, whose words 6-7 of the root's row hold its gather_cap; both on the device); blocks. The capacity check is collective:
+// every rank reads the root's capacity, so when it is short all of them return DENSITY_B200_ECAPACITY and none posts a send that no
+// receive would ever match.
+static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_offsets, const uint32_t* d_words, const uint8_t* d_out,
+                         int gather_root, uint8_t* d_gather, cudaStream_t st) {
     const size_t W = (size_t)h->world;
     cudaError_t e;
     // variable-length gather of the pieces at their stream offsets (SURVEY §8e step 5): sizes -> host -> grouped send / recv
     e = cudaMemcpyAsync(h->h_offsets, d_offsets, (W + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->h_offsets + W + 1, d_words + 8 * (size_t)gather_root + 6, sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("gather: sizes to host", e); return DENSITY_B200_ECUDA; }
-    const uint64_t total = h->h_offsets[W];
+    const uint64_t total = h->h_offsets[W], root_cap = h->h_offsets[W + 1];
     const uint64_t my_off = h->h_offsets[h->rank], my_size = h->h_offsets[h->rank + 1] - my_off;
+    if (root_cap < total) { set_error("gather buffer too small"); return DENSITY_B200_ECAPACITY; }
     if (h->rank == gather_root) {
-        if (!d_gather || gather_cap < total) { set_error("gather buffer too small"); return DENSITY_B200_ECAPACITY; }
         if (my_size) e = cudaMemcpyAsync(d_gather + my_off, d_out, my_size, cudaMemcpyDeviceToDevice, st);
         if (e != cudaSuccess) { set_error("gather: local piece", e); return DENSITY_B200_ECUDA; }
     }
@@ -1260,19 +1290,26 @@ static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_
 
 // the argument checks of the sharded encoders
 static int encode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, size_t n, const uint8_t* d_out, const uint64_t* d_out_size,
-                               int gather_root) {
+                               int gather_root, const uint8_t* d_gather) {
     if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (h->rank != h->world - 1 && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
     if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
     if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
+    if (h->rank == gather_root && !d_gather) { set_error("null pointer: d_gather on the gather root"); return DENSITY_B200_EARG; }
     return DENSITY_B200_OK;
 }
 
-// the end of every sharded encode: the verdict, the optional gather of the pieces to gather_root, the last stage event
+// the end of every sharded encode: the verdict, the optional gather of the pieces to gather_root, the last stage event. The root's
+// gather_cap travels to every rank in words 6-7 of its seam words (zero otherwise), so that all ranks judge the capacity alike.
 static int encode_sharded_end(const Exchange& x, const uint8_t* d_out, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
                               uint8_t* d_gather, size_t gather_cap) {
+    if (x.h->rank == gather_root) {
+        const uint64_t cap = gather_cap;        // pageable: consumed before cudaMemcpyAsync returns
+        const cudaError_t e = cudaMemcpyAsync(x.my_words() + 6, &cap, sizeof cap, cudaMemcpyHostToDevice, x.st);
+        if (e != cudaSuccess) { set_error("gather capacity to the seam words", e); return DENSITY_B200_ECUDA; }
+    }
     int rc = x.verdict(d_flags, d_total_size, nullptr);
-    if (rc == DENSITY_B200_OK && gather_root >= 0) rc = gather_pieces(x.h, x.a, x.offsets, d_out, gather_root, d_gather, gather_cap, x.st);
+    if (rc == DENSITY_B200_OK && gather_root >= 0) rc = gather_pieces(x.h, x.a, x.offsets, x.words, d_out, gather_root, d_gather, x.st);
     if (rc != DENSITY_B200_OK) return rc;
     cudaEventRecord(x.h->ev[5], x.st);
     x.h->timed = true;
@@ -1285,7 +1322,7 @@ static int encode_sharded_end(const Exchange& x, const uint8_t* d_out, uint32_t*
 int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
     density_b200_shard* s = h->enc;
@@ -1316,7 +1353,7 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
 int density_b200_encode_sharded_cl(density_b200_sharded* h, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                    uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
     if (rc != DENSITY_B200_OK) return rc;
     if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
     density_b200_cl_shard* s = h->cl[alg - ALG_CHEETAH];
@@ -1366,7 +1403,7 @@ int density_b200_encode_sharded_protected(density_b200_sharded* h, const uint8_t
                                           uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap,
                                           void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root);
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
     if (rc != DENSITY_B200_OK) return rc;
     // every argument the later phases check is checked here, before the first collective: a rank that returned EARG half way through
     // would leave the others waiting in an all-gather

@@ -146,6 +146,9 @@ DENSITY_B200_API int density_b200_table_fold(uint32_t* d_acc, const uint32_t* d_
  *                                    blocks across a cut): the pieces are void and the caller encodes on one device instead, or
  *                                    with density_b200_encode_sharded_protected below, which accepts such input.
  *                                    *d_total_size = length of the whole stream, on every rank. gather_root < 0: no gather, nothing blocks.
+ *                                    d_gather NULL on the root: DENSITY_B200_EARG before any collective. The root's gather_cap reaches
+ *                                    every rank with the seam words: when it is below the stream length every rank returns
+ *                                    DENSITY_B200_ECAPACITY and no piece is sent.
  */
 typedef struct density_b200_sharded density_b200_sharded; /* opaque */
 DENSITY_B200_API int density_b200_sharded_unique_id(uint8_t* out128);
@@ -480,6 +483,12 @@ DENSITY_B200_API void density_b200_test_set_decode_rounds(int k);
 /* Test hook: cut the round budget of the sharded copy-map iteration (density_b200_shard_prot_*, density_b200_encode_sharded_protected)
    to k rounds (1..16, default 16) so that its "did not settle" refusal can be exercised. The single-device encoder does not read it. */
 DENSITY_B200_API void density_b200_test_set_prot_rounds(int k);
+/* Test hook: resolve the NCCL entry points of the sharded drivers (ncclGetUniqueId, ncclCommInitRank, ncclCommDestroy, ncclAllGather,
+   ncclSend, ncclRecv, ncclGroupStart, ncclGroupEnd, ncclGetErrorString) from the shared library at `path` instead of libnccl.so.2, e.g.
+   a loopback library that serves several ranks in one process on one device; NULL restores the default lookup. DENSITY_B200_EARG when
+   the library cannot be loaded, lacks one of the nine symbols, or while a density_b200_sharded handle with world > 1 is alive. Call it
+   while no handle is being created. */
+DENSITY_B200_API int density_b200_test_set_nccl_library(const char* path);
 /* Diagnostic: the last copy-map iteration on the current device, per fixed-point round {first block whose copy status changed
    (~0: none), number of such blocks}: 16 rounds x 2 values. Synchronises the device. */
 DENSITY_B200_API int density_b200_prot_debug(uint64_t* out32);

@@ -307,9 +307,9 @@ static int encode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
             }
             e = cham_encode_phase1(d_in, n, c->ws.p, L, nruns, nullptr, stream, &launches, ev);
             if (e == cudaSuccess && path == 4)
-                e = cham_encode_phase2_blocking(d_in, n, c->ws.p, L, nruns, d_out, cap, d_out_size, 12, stream, &launches);
+                e = cham_encode_phase2_blocking(d_in, n, c->ws.p, L, nruns, d_out, cap, d_out_size, 12, c->num_sms, stream, &launches);
             else if (e == cudaSuccess)
-                e = cham_encode_phase2(d_in, n, c->ws.p, L, nruns, nullptr, d_out, cap, d_out_size, path == 0, false, stream, &launches, ev);
+                e = cham_encode_phase2(d_in, n, c->ws.p, L, nruns, nullptr, d_out, cap, d_out_size, path == 0, false, c->num_sms, stream, &launches, ev);
             if (ev != nullptr && e == cudaSuccess) c->prof_count++;
         }
         c->last_was_chameleon_fastpath_capable = (path != 2);
@@ -456,7 +456,7 @@ static size_t chameleon_encode_host_pipelined(DeviceCtx* c, const uint8_t* in, s
         e = cudaStreamWaitEvent(c->stream, evs[i], 0);
         if (e == cudaSuccess) e = cham_encode_phase1(c->stage_in.p + off, len, c->ws.p, L, nruns, d_tab, c->stream, &launches);
         if (e == cudaSuccess) e = cham_encode_phase2(c->stage_in.p + off, len, c->ws.p, L, nruns, i ? d_acc : nullptr, c->stage_out.p + out_off,
-                                                     c->stage_out.bytes - out_off, d_sizes + i, false, i != 0, c->stream, &launches);
+                                                     c->stage_out.bytes - out_off, d_sizes + i, false, i != 0, c->num_sms, c->stream, &launches);
         if (e == cudaSuccess) e = cham_status_accumulate(c->ws.p, L, d_flag, c->stream, &launches);
         if (e == cudaSuccess) e = cham_table_fold(d_acc, d_tab, c->stream, &launches);
         if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_sizes + i, d_sizes + i, sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
@@ -665,7 +665,7 @@ static int shard_phase2_impl(density_b200_shard* s, const uint32_t* d_carry_in, 
                              bool assume_prev_inc, cudaEvent_t* ev, cudaStream_t st) {
     uint64_t launches = 0;
     const cudaError_t e = cham_encode_phase2(s->d_in, s->n, s->ws.p, s->L, s->nruns, d_carry_in, d_out, cap, d_out_size, false,
-                                             assume_prev_inc, st, &launches, ev);
+                                             assume_prev_inc, s->num_sms, st, &launches, ev);
     return step_result(e, launches, "shard phase2");
 }
 int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
@@ -1779,7 +1779,7 @@ static size_t codec_run(density_b200_codec* h, bool encode, const uint8_t* in, s
         bool ok = false;
         if (e == cudaSuccess) e = cham_quads_to_table(quads, d_carry, st, &launches);
         if (e == cudaSuccess) e = cham_encode_phase1(d_in, n, c->ws.p, L, nruns, nullptr, st, &launches);
-        if (e == cudaSuccess) e = cham_encode_phase2_stream(d_in, n, c->ws.p, L, nruns, d_carry, d_out, d_cap, c->d_size, d_tab, 12, st, &launches, &ok);
+        if (e == cudaSuccess) e = cham_encode_phase2_stream(d_in, n, c->ws.p, L, nruns, d_carry, d_out, d_cap, c->d_size, d_tab, 12, c->num_sms, st, &launches, &ok);
         if (e == cudaSuccess && ok) { e = cham_table_into_quads(d_tab, quads, st, &launches); done = true; }
         c->last_was_chameleon_fastpath_capable = 0;
     }

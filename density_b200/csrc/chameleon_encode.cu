@@ -1374,11 +1374,6 @@ static cudaError_t set_smem_attrs_once() {
     return err;
 }
 
-static void launch_flag_pass(uint32_t nruns, cudaStream_t stream, const uint32_t* in, uint64_t nquads, uint32_t ntiles, uint32_t* sigw,
-                             uint2* unres, uint32_t* unres_count, uint32_t* final_tab, const uint8_t* copymap, const Status* gate) {
-    cham_flag_pass6<<<nruns, F6_THREADS, sizeof(Flag6Smem), stream>>>(in, nquads, ntiles, nruns, sigw, unres, unres_count, final_tab, copymap, gate);
-}
-
 static cudaError_t prot_iterate_coop(int ctas, cudaStream_t stream, const uint32_t* sigw, uint64_t nbytes, uint64_t nblocks, uint32_t nseg, Status* st, int it,
                                      uint8_t* inc, uint8_t* cm_old, uint8_t* cm_new, uint32_t* in_state, uint32_t* out_state, uint16_t* ptab) {
     void* args[] = {&sigw, &nbytes, &nblocks, &nseg, &st, &it, &inc, &cm_old, &cm_new, &in_state, &out_state, &ptab};
@@ -1399,35 +1394,90 @@ uint32_t cham_pick_runs(size_t nbytes, int num_sms) {
     return (uint32_t)r;
 }
 
+// One encode call's view of its workspace: the geometry of its `nbytes` and typed pointers to the arrays of ChamLayout. The segment
+// states and candidate tables of the copy-map iteration sit in the seg_state region, in prot_iterate's layout: in_state [nseg + 1],
+// out_state [nseg + 1] (unused by the sharded iteration), then ptab: gin [ngrp + 2] (as u32), T [nseg][PC_NC], GT [ngrp][PC_NC] (u16).
+struct ChamBufs {
+    size_t nbytes; uint64_t nquads, nblocks; uint32_t ntiles, ngroups, nseg, ngrp;
+    Status* st; uint32_t* sigw; uint8_t *copymap, *copymap2, *incb; uint32_t *seg_state, *tile_bytes, *tile_local; uint64_t *group_total, *group_off;
+    uint2* unres; uint32_t *unres_count, *final_tab, *carry;
+    uint32_t *in_state, *out_state, *gin; uint16_t *ptab, *T, *GT;
+    template <class X> static X* at(uint8_t* ws, size_t off) { return reinterpret_cast<X*>(ws + off); }
+    ChamBufs(uint8_t* ws, const ChamLayout& L, size_t n) {
+        nbytes = n; nquads = n / 4; nblocks = (n + 255) / 256;
+        ntiles = (uint32_t)((nblocks + 63) / 64); ngroups = (ntiles + SCAN_G - 1) / SCAN_G;
+        nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG); ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
+        st = at<Status>(ws, L.status); sigw = at<uint32_t>(ws, L.sigw);
+        copymap = ws + L.copymap; copymap2 = ws + L.copymap2; incb = ws + L.incb;
+        seg_state = at<uint32_t>(ws, L.seg_state);
+        tile_bytes = at<uint32_t>(ws, L.tile_bytes); tile_local = at<uint32_t>(ws, L.tile_local);
+        group_total = at<uint64_t>(ws, L.group_total); group_off = at<uint64_t>(ws, L.group_off);
+        unres = at<uint2>(ws, L.unres); unres_count = at<uint32_t>(ws, L.unres_count);
+        final_tab = at<uint32_t>(ws, L.final_tab); carry = at<uint32_t>(ws, L.carry);
+        in_state = seg_state; out_state = seg_state + (nseg + 1);
+        ptab = reinterpret_cast<uint16_t*>(seg_state + 2 * (nseg + 1));
+        gin = reinterpret_cast<uint32_t*>(ptab); T = ptab + 2 * (ngrp + 2); GT = T + (size_t)nseg * PC_NC;
+    }
+};
+
+// ---- the launches that more than one path makes. `gate` (may be nullptr = always): the kernels return at once unless the quiet check
+// failed and the copy map has not settled yet.
+// flags of every run, with the blocks of `copymap` (may be nullptr) hidden from the dictionary
+static void launch_flag_pass(const ChamBufs& B, const uint8_t* d_in, uint32_t nruns, const uint8_t* copymap, const Status* gate, cudaStream_t stream,
+                             uint64_t* launches) {
+    cham_flag_pass6<<<nruns, F6_THREADS, sizeof(Flag6Smem), stream>>>(reinterpret_cast<const uint32_t*>(d_in), B.nquads, B.ntiles, nruns, B.sigw, B.unres,
+                                                                      B.unres_count, B.final_tab, copymap, gate);
+    ++*launches;
+}
+// the table carried into every run (d_carry_in before the first; nullptr = stream start), then the first-touch flags resolved against it
+static void launch_carry_resolve(const ChamBufs& B, uint32_t nruns, const uint32_t* d_carry_in, const Status* gate, cudaStream_t stream,
+                                 uint64_t* launches) {
+    cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(B.final_tab, d_carry_in, 0, nruns, B.carry, nullptr, gate);
+    cham_resolve<<<dim3(32, nruns), 256, 0, stream>>>(B.unres, B.unres_count, B.carry, B.ntiles, nruns, B.sigw, gate);
+    *launches += 2;
+}
+// export: the fold of the runs' last-writer tables with "nothing touched" as the initial state
+static void launch_export_fold(const ChamBufs& B, uint32_t nruns, uint32_t* d_table_out, const Status* gate, cudaStream_t stream, uint64_t* launches) {
+    cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(B.final_tab, nullptr, 1, nruns, nullptr, d_table_out, gate);
+    ++*launches;
+}
+// Sizes under `copymap` (nullptr: the sizes of cham_phase2_begin stand, and no block is copied), scan, emit. use_copymap_if_nonquiet:
+// the map counts only if the quiet check failed (the in-order encode passes 0: its map always counts). The emit kernel that loads 16
+// bytes at a time runs when `al16_ok` and the input is so aligned; the in-order encode has always taken the other one.
+static cudaError_t sizes_scan_emit(const ChamBufs& B, const uint8_t* d_in, const uint8_t* copymap, int use_copymap_if_nonquiet, bool al16_ok,
+                                   uint8_t* d_out, size_t cap, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
+    if (copymap) {
+        cham_tile_sizes<<<(B.ntiles + 7) / 8, 256, 0, stream>>>(B.sigw, copymap, B.nbytes, B.nblocks, B.ntiles, use_copymap_if_nonquiet, 0, 0, B.st, B.tile_bytes);
+        ++*launches;
+    }
+    cudaError_t e = scan_tiles_launch(B.tile_bytes, B.ntiles, B.tile_local, B.group_total, B.group_off, B.ngroups, B.st, (uint64_t)cap, d_out_size, stream);
+    if (e != cudaSuccess) return e;
+    *launches += 2;
+    if (ev) cudaEventRecord(ev[2], stream);
+    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
+    if (al16_ok && (reinterpret_cast<uintptr_t>(d_in) & 15u) == 0)
+        cham_emit<true><<<B.ntiles, EM_THREADS, 0, stream>>>(in32, B.nbytes, B.nblocks, B.sigw, copymap, use_copymap_if_nonquiet, B.st, B.tile_local, B.group_off, d_out);
+    else
+        cham_emit<false><<<B.ntiles, EM_THREADS, 0, stream>>>(in32, B.nbytes, B.nblocks, B.sigw, copymap, use_copymap_if_nonquiet, B.st, B.tile_local, B.group_off, d_out);
+    ++*launches;
+    if (ev) cudaEventRecord(ev[3], stream);
+    return cudaGetLastError();
+}
+
 // Phase 1 of the encode: flag pass over all runs + fold of the last-writer tables.
 cudaError_t cham_encode_phase1(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns,
                                uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
     cudaError_t e = set_smem_attrs_once();
     if (e != cudaSuccess) return e;
-    const uint64_t nquads = nbytes / 4;
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    e = cudaMemsetAsync(st, 0, sizeof(Status), stream);
+    const ChamBufs B(ws, L, nbytes);
+    e = cudaMemsetAsync(B.st, 0, sizeof(Status), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(&B.st->first_nonquiet_block, 0xFF, sizeof(unsigned long long), stream);   // it starts at ~0
     if (e != cudaSuccess) return e;
-    {
-        // first_nonquiet_block starts at ~0
-        e = cudaMemsetAsync(&st->first_nonquiet_block, 0xFF, sizeof(unsigned long long), stream);
-        if (e != cudaSuccess) return e;
-    }
-    if (nblocks == 0) return cudaSuccess;
+    if (B.nblocks == 0) return cudaSuccess;
     if (ev) cudaEventRecord(ev[0], stream);
-    launch_flag_pass(nruns, stream, reinterpret_cast<const uint32_t*>(d_in), nquads, ntiles, reinterpret_cast<uint32_t*>(ws + L.sigw),
-        reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-        reinterpret_cast<uint32_t*>(ws + L.final_tab), nullptr, nullptr);
-    ++*launches;
+    launch_flag_pass(B, d_in, nruns, nullptr, nullptr, stream, launches);
     if (ev) cudaEventRecord(ev[1], stream);
-    if (d_table_out) {
-        // shard export: fold of this shard's runs with "nothing touched" as the initial state
-        cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), nullptr, 1, nruns,
-                                                        nullptr, d_table_out);
-        ++*launches;
-    }
+    if (d_table_out) launch_export_fold(B, nruns, d_table_out, nullptr, stream, launches);   // a shard's table
     return cudaGetLastError();
 }
 
@@ -1440,106 +1490,49 @@ cudaError_t cham_encode_phase1(const uint8_t* d_in, size_t nbytes, uint8_t* ws, 
 //           map has not settled yet); prot_iterate owns 8 grid-barrier slots, so a batch is at most 8 rounds and `reset_barriers`
 //           clears them first
 //   finish: the exact in-order walk if the map still has not settled (optional), sizes under the copy map, scan, emit
-cudaError_t cham_phase2_begin(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in,
-                              bool assume_prev_inc, cudaStream_t stream, uint64_t* launches) {
-    (void)d_in;
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
-    cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), d_carry_in, 0, nruns,
-                                                    reinterpret_cast<uint32_t*>(ws + L.carry), nullptr);
-    cham_resolve<<<dim3(32, nruns), 256, 0, stream>>>(reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-                                                     reinterpret_cast<uint32_t*>(ws + L.carry), ntiles, nruns, sigw);
-    cham_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(sigw, nullptr, nbytes, nblocks, ntiles, 0, 1, assume_prev_inc ? 1 : 0, st,
-                                                          reinterpret_cast<uint32_t*>(ws + L.tile_bytes));
-    *launches += 3;
+static cudaError_t cham_phase2_begin(const ChamBufs& B, uint32_t nruns, const uint32_t* d_carry_in, bool assume_prev_inc, cudaStream_t stream,
+                                     uint64_t* launches) {
+    launch_carry_resolve(B, nruns, d_carry_in, nullptr, stream, launches);
+    cham_tile_sizes<<<(B.ntiles + 7) / 8, 256, 0, stream>>>(B.sigw, nullptr, B.nbytes, B.nblocks, B.ntiles, 0, 1, assume_prev_inc ? 1 : 0, B.st, B.tile_bytes);
+    ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t cham_phase2_rounds(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in,
-                               int it_first, int it_last, bool reset_barriers, cudaStream_t stream, uint64_t* launches) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
-    uint8_t* copymap = ws + L.copymap;
-    uint8_t* copymap2 = ws + L.copymap2;
-    uint32_t* seg_state = reinterpret_cast<uint32_t*>(ws + L.seg_state);
-    uint8_t* incb = ws + L.incb;
-    int num_ctas = 0;
-    { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_ctas, cudaDevAttrMultiProcessorCount, dev); if (num_ctas < 1) num_ctas = 1; }
-    const uint32_t nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG);
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    const uint64_t nquads = nbytes / 4;
+static cudaError_t cham_phase2_rounds(const ChamBufs& B, const uint8_t* d_in, uint32_t nruns, const uint32_t* d_carry_in, int it_first, int it_last,
+                                      bool reset_barriers, int num_sms, cudaStream_t stream, uint64_t* launches) {
+    const int num_ctas = num_sms > 0 ? num_sms : 1;   // one CTA per SM
     if (it_last - it_first >= 8) return cudaErrorInvalidValue;
     if (reset_barriers) {
-        cudaError_t e = cudaMemsetAsync(st->barrier, 0, sizeof(st->barrier), stream);
+        cudaError_t e = cudaMemsetAsync(B.st->barrier, 0, sizeof(B.st->barrier), stream);
         if (e != cudaSuccess) return e;
     }
     for (int it = it_first; it <= it_last; ++it) {
         if (it > 0) {   // flags under the current copy map (copy-mode blocks hidden from the dictionary)
-            launch_flag_pass(nruns, stream, in32, nquads, ntiles, sigw,
-                reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-                reinterpret_cast<uint32_t*>(ws + L.final_tab), copymap, st);
-            cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), d_carry_in, 0, nruns,
-                                                            reinterpret_cast<uint32_t*>(ws + L.carry), nullptr, st);
-            cham_resolve<<<dim3(32, nruns), 256, 0, stream>>>(reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-                                                             reinterpret_cast<uint32_t*>(ws + L.carry), ntiles, nruns, sigw, st);
-            *launches += 3;
+            launch_flag_pass(B, d_in, nruns, B.copymap, B.st, stream, launches);
+            launch_carry_resolve(B, nruns, d_carry_in, B.st, stream, launches);
         }
-        {   // cooperative launch: the software grid barriers need every CTA resident (the runtime checks it instead of a hang)
-            cudaError_t le = prot_iterate_coop(num_ctas, stream, sigw, nbytes, nblocks, nseg, st, it, incb, copymap, copymap2, seg_state, seg_state + (nseg + 1),
-                                               reinterpret_cast<uint16_t*>(seg_state + 2 * (nseg + 1)));
-            if (le != cudaSuccess) return le;
-        }
+        // cooperative launch: the software grid barriers need every CTA resident (the runtime checks it instead of a hang)
+        cudaError_t le = prot_iterate_coop(num_ctas, stream, B.sigw, B.nbytes, B.nblocks, B.nseg, B.st, it, B.incb, B.copymap, B.copymap2, B.in_state,
+                                           B.out_state, B.ptab);
+        if (le != cudaSuccess) return le;
         ++*launches;
     }
     return cudaGetLastError();
 }
 
-cudaError_t cham_phase2_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint8_t* d_out, size_t cap,
-                               uint64_t* d_out_size, bool with_copy_map, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev,
-                               bool inorder_fallback = true) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    const uint32_t ngroups = (ntiles + SCAN_G - 1) / SCAN_G;
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
-    uint8_t* copymap = ws + L.copymap;
-    if (with_copy_map) {
-        // the exact in-order walk if the iteration did not settle; then the sizes again, now with the copy map
-        if (inorder_fallback) { cham_protected_pass<<<1, 1024, sizeof(ProtSmem), stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, st, 1, sigw, copymap); ++*launches; }
-        cham_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(sigw, copymap, nbytes, nblocks, ntiles, 1, 0, 0, st,
-                                                              reinterpret_cast<uint32_t*>(ws + L.tile_bytes));
+static cudaError_t cham_phase2_finish(const ChamBufs& B, const uint8_t* d_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size, bool with_copy_map,
+                                      bool inorder_fallback, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
+    if (with_copy_map && inorder_fallback) {   // the exact in-order walk if the iteration did not settle
+        cham_protected_pass<<<1, 1024, sizeof(ProtSmem), stream>>>(reinterpret_cast<const uint32_t*>(d_in), B.nbytes, B.st, 1, B.sigw, B.copymap);
         ++*launches;
     }
-    scan_groups_local<<<ngroups, SCAN_T, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.tile_bytes), ntiles,
-                                                      reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                      reinterpret_cast<uint64_t*>(ws + L.group_total));
-    scan_group_totals<<<1, SCAN_T, 0, stream>>>(reinterpret_cast<uint64_t*>(ws + L.group_total), ngroups,
-                                                reinterpret_cast<uint64_t*>(ws + L.group_off), st, (uint64_t)cap, d_out_size);
-    *launches += 2;
-    if (ev) cudaEventRecord(ev[2], stream);
-    if ((reinterpret_cast<uintptr_t>(d_in) & 15u) == 0)
-        cham_emit<true><<<ntiles, EM_THREADS, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, nblocks, sigw,
-                                                           with_copy_map ? copymap : nullptr, 1, st,
-                                                           reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                           reinterpret_cast<uint64_t*>(ws + L.group_off), d_out);
-    else
-        cham_emit<false><<<ntiles, EM_THREADS, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, nblocks, sigw,
-                                                            with_copy_map ? copymap : nullptr, 1, st,
-                                                            reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                            reinterpret_cast<uint64_t*>(ws + L.group_off), d_out);
-    ++*launches;
-    if (ev) cudaEventRecord(ev[3], stream);
-    return cudaGetLastError();
+    return sizes_scan_emit(B, d_in, with_copy_map ? B.copymap : nullptr, 1, true, d_out, cap, d_out_size, stream, launches, ev);
 }
 
 // host-visible verdict of the iteration so far (synchronises the stream): 0 quiet or settled, 1 more rounds needed
-cudaError_t cham_phase2_needs_more(uint8_t* ws, const ChamLayout& L, cudaStream_t stream, bool* more) {
+static cudaError_t cham_phase2_needs_more(const ChamBufs& B, cudaStream_t stream, bool* more) {
     Status h;
-    cudaError_t e = cudaMemcpyAsync(&h, ws + L.status, sizeof h, cudaMemcpyDeviceToHost, stream);
+    cudaError_t e = cudaMemcpyAsync(&h, B.st, sizeof h, cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     if (e != cudaSuccess) return e;
     *more = h.nonquiet && !h.converged && !h.error;
@@ -1548,59 +1541,74 @@ cudaError_t cham_phase2_needs_more(uint8_t* ws, const ChamLayout& L, cudaStream_
 
 constexpr int PROT_ITERS = 4;   // rounds 0..4 are always enqueued (they cost ~3 us each when the input is quiet)
 
+// What the callers of phase 2 choose.
+struct Phase2Opts {
+    const uint32_t* d_carry_in = nullptr;   // the dictionary carried in (nullptr = stream start)
+    bool assume_prev_inc = false;           // count the block before the first as incompressible
+    bool iterate = true;                    // run the copy-map iteration; false: no copy map, the sizes of `begin` stand
+    int max_batches = 0;                    // after the standard rounds the host looks at the verdict (synchronising) and keeps iterating in
+                                            // up to this many batches of rounds 8..15
+    bool inorder_walk = true;               // the in-order walk settles a map that the rounds did not
+    bool* give_up = nullptr;                // set: a map still unsettled after the batches means no emit and *give_up = true
+    uint32_t* d_table_out = nullptr;        // set: export the last-writer table under the final copy map
+    cudaEvent_t* ev = nullptr;              // stage events 2 and 3
+};
+
+static cudaError_t cham_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, uint8_t* d_out, size_t cap,
+                               uint64_t* d_out_size, const Phase2Opts& o, int num_sms, cudaStream_t stream, uint64_t* launches) {
+    if (nbytes == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
+    const ChamBufs B(ws, L, nbytes);
+    cudaError_t e = cham_phase2_begin(B, nruns, o.d_carry_in, o.assume_prev_inc, stream, launches);
+    if (e == cudaSuccess && o.iterate) e = cham_phase2_rounds(B, d_in, nruns, o.d_carry_in, 0, PROT_ITERS, false, num_sms, stream, launches);
+    // A caller that leaves the rest to the in-order walk does not look at the verdict after its last batch; one that gives up looks once
+    // more, so that `more` is the verdict of the last batch.
+    bool more = false;
+    const int looks = o.max_batches + (o.give_up ? 1 : 0);
+    for (int batch = 0; e == cudaSuccess && batch < looks; ++batch) {
+        e = cham_phase2_needs_more(B, stream, &more);
+        if (e != cudaSuccess || !more || batch >= o.max_batches) break;
+        e = cham_phase2_rounds(B, d_in, nruns, o.d_carry_in, 8, 15, true, num_sms, stream, launches);
+    }
+    if (e != cudaSuccess) return e;
+    if (o.give_up && more) { *o.give_up = true; return cudaSuccess; }
+    e = cham_phase2_finish(B, d_in, d_out, cap, d_out_size, o.iterate, o.inorder_walk, stream, launches, o.ev);
+    if (e == cudaSuccess && o.d_table_out) {
+        launch_export_fold(B, nruns, o.d_table_out, nullptr, stream, launches);
+        e = cudaGetLastError();
+    }
+    return e;
+}
+
+// Everything enqueued, no host synchronisation: rounds 0..PROT_ITERS, then the in-order walk if they were not enough.
 cudaError_t cham_encode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns,
                                const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                               bool allow_protected_fallback, bool assume_prev_inc, cudaStream_t stream, uint64_t* launches,
+                               bool allow_protected_fallback, bool assume_prev_inc, int num_sms, cudaStream_t stream, uint64_t* launches,
                                cudaEvent_t* ev) {
-    if (nbytes == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
-    cudaError_t e = cham_phase2_begin(d_in, nbytes, ws, L, nruns, d_carry_in, assume_prev_inc, stream, launches);
-    if (e == cudaSuccess && allow_protected_fallback)
-        e = cham_phase2_rounds(d_in, nbytes, ws, L, nruns, d_carry_in, 0, PROT_ITERS, false, stream, launches);
-    if (e == cudaSuccess) e = cham_phase2_finish(d_in, nbytes, ws, L, d_out, cap, d_out_size, allow_protected_fallback, stream, launches, ev);
-    return e;
+    Phase2Opts o;
+    o.d_carry_in = d_carry_in; o.assume_prev_inc = assume_prev_inc; o.iterate = allow_protected_fallback; o.ev = ev;
+    return cham_phase2(d_in, nbytes, ws, L, nruns, d_out, cap, d_out_size, o, num_sms, stream, launches);
 }
 
 // Same result, for callers that may block: after the standard rounds the host looks at the verdict and keeps iterating in batches of 8
 // rounds (up to `max_batches`) before the in-order walk is allowed to take over.
 cudaError_t cham_encode_phase2_blocking(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, uint8_t* d_out,
-                                        size_t cap, uint64_t* d_out_size, int max_batches, cudaStream_t stream, uint64_t* launches) {
-    if (nbytes == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
-    cudaError_t e = cham_phase2_begin(d_in, nbytes, ws, L, nruns, nullptr, false, stream, launches);
-    if (e == cudaSuccess) e = cham_phase2_rounds(d_in, nbytes, ws, L, nruns, nullptr, 0, PROT_ITERS, false, stream, launches);
-    for (int batch = 0; e == cudaSuccess && batch < max_batches; ++batch) {
-        bool more = false;
-        e = cham_phase2_needs_more(ws, L, stream, &more);
-        if (e != cudaSuccess || !more) break;
-        e = cham_phase2_rounds(d_in, nbytes, ws, L, nruns, nullptr, 8, 15, true, stream, launches);
-    }
-    if (e == cudaSuccess) e = cham_phase2_finish(d_in, nbytes, ws, L, d_out, cap, d_out_size, true, stream, launches, nullptr);
-    return e;
+                                        size_t cap, uint64_t* d_out_size, int max_batches, int num_sms, cudaStream_t stream, uint64_t* launches) {
+    Phase2Opts o;
+    o.max_batches = max_batches;
+    return cham_phase2(d_in, nbytes, ws, L, nruns, d_out, cap, d_out_size, o, num_sms, stream, launches);
 }
 
 // Phase 2 for a reused Codec instance: dictionary carried in, copy map by host-resumed iteration; when it does not settle nothing is
 // emitted and *ok = false (the caller runs the in-order kernel on the instance's state instead). On success d_table_out = this call's
 // last-writer table under the final copy map (copy-mode blocks never reach the dictionary, codec.rs:35-37).
 cudaError_t cham_encode_phase2_stream(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in,
-                                      uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_table_out, int max_batches, cudaStream_t stream,
-                                      uint64_t* launches, bool* ok) {
-    *ok = true;
-    if (nbytes == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
-    cudaError_t e = cham_phase2_begin(d_in, nbytes, ws, L, nruns, d_carry_in, false, stream, launches);
-    if (e == cudaSuccess) e = cham_phase2_rounds(d_in, nbytes, ws, L, nruns, d_carry_in, 0, PROT_ITERS, false, stream, launches);
-    bool more = false;
-    for (int batch = 0; e == cudaSuccess; ++batch) {
-        e = cham_phase2_needs_more(ws, L, stream, &more);
-        if (e != cudaSuccess || !more || batch >= max_batches) break;
-        e = cham_phase2_rounds(d_in, nbytes, ws, L, nruns, d_carry_in, 8, 15, true, stream, launches);
-    }
-    if (e != cudaSuccess) return e;
-    if (more) { *ok = false; return cudaSuccess; }
-    e = cham_phase2_finish(d_in, nbytes, ws, L, d_out, cap, d_out_size, true, stream, launches, nullptr, false);
-    if (e == cudaSuccess) {
-        cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), nullptr, 1, nruns, nullptr, d_table_out);
-        ++*launches;
-        e = cudaGetLastError();
-    }
+                                      uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_table_out, int max_batches, int num_sms,
+                                      cudaStream_t stream, uint64_t* launches, bool* ok) {
+    bool gave_up = false;
+    Phase2Opts o;
+    o.d_carry_in = d_carry_in; o.max_batches = max_batches; o.inorder_walk = false; o.give_up = &gave_up; o.d_table_out = d_table_out;
+    const cudaError_t e = cham_phase2(d_in, nbytes, ws, L, nruns, d_out, cap, d_out_size, o, num_sms, stream, launches);
+    *ok = !gave_up;
     return e;
 }
 cudaError_t cham_quads_to_table(const uint32_t* d_quads, uint32_t* d_table, cudaStream_t stream, uint64_t* launches) {
@@ -1620,14 +1628,12 @@ cudaError_t cham_status_accumulate(const uint8_t* ws, const ChamLayout& L, uint3
     return cudaGetLastError();
 }
 cudaError_t prot_iterate_launch(const uint32_t* sigw_or_null, uint64_t nbytes, uint64_t nblocks, uint32_t nseg, Status* st, int it, uint8_t* inc,
-                                uint8_t* cm_old, uint8_t* cm_new, uint32_t* in_state, uint32_t* out_state, int /*block_bytes*/, int num_sms,
-                                cudaStream_t stream) {
+                                uint8_t* cm_old, uint8_t* cm_new, uint32_t* in_state, uint32_t* out_state, int num_sms, cudaStream_t stream) {
     int ctas = num_sms > 0 ? num_sms : 1;
     if ((uint32_t)ctas > nseg) ctas = nseg ? (int)nseg : 1;       // small inputs: cheaper grid barriers
     // the caller's state region is sized by prot_state_bytes(): the candidate tables live behind the 2 (nseg + 1) state words
     return prot_iterate_coop(ctas, stream, sigw_or_null, nbytes, nblocks, nseg, st, it, inc, cm_old, cm_new, in_state, out_state,
                              reinterpret_cast<uint16_t*>(out_state + (nseg + 1)));
-
 }
 cudaError_t scan_tiles_launch(const uint32_t* tile_bytes, uint32_t ntiles, uint32_t* tile_local, uint64_t* group_total, uint64_t* group_off,
                               uint32_t ngroups, Status* st, uint64_t cap, uint64_t* d_out_size, cudaStream_t stream) {
@@ -1668,50 +1674,16 @@ cudaError_t cham_encode_protected_only(const uint8_t* d_in, size_t nbytes, uint8
                                        size_t cap, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches) {
     cudaError_t e = set_smem_attrs_once();
     if (e != cudaSuccess) return e;
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    const uint32_t ngroups = (ntiles + SCAN_G - 1) / SCAN_G;
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
-    uint8_t* copymap = ws + L.copymap;
-    e = cudaMemsetAsync(st, 0, sizeof(Status), stream);
+    const ChamBufs B(ws, L, nbytes);
+    e = cudaMemsetAsync(B.st, 0, sizeof(Status), stream);
     if (e != cudaSuccess) return e;
-    if (nblocks == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
-    cham_protected_pass<<<1, 1024, sizeof(ProtSmem), stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, st, 0, sigw, copymap);
+    if (B.nblocks == 0) return cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), stream);
+    cham_protected_pass<<<1, 1024, sizeof(ProtSmem), stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, B.st, 0, B.sigw, B.copymap);
     ++*launches;
-    cham_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(sigw, copymap, nbytes, nblocks, ntiles, 0, 0, 0, st,
-                                                          reinterpret_cast<uint32_t*>(ws + L.tile_bytes));
-    ++*launches;
-    scan_groups_local<<<ngroups, SCAN_T, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.tile_bytes), ntiles,
-                                                      reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                      reinterpret_cast<uint64_t*>(ws + L.group_total));
-    ++*launches;
-    scan_group_totals<<<1, SCAN_T, 0, stream>>>(reinterpret_cast<uint64_t*>(ws + L.group_total), ngroups,
-                                                reinterpret_cast<uint64_t*>(ws + L.group_off), st, (uint64_t)cap, d_out_size);
-    ++*launches;
-    cham_emit<false><<<ntiles, EM_THREADS, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_in), nbytes, nblocks, sigw, copymap, 0, st,
-                                                        reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                        reinterpret_cast<uint64_t*>(ws + L.group_off), d_out);
-    ++*launches;
-    return cudaGetLastError();
+    return sizes_scan_emit(B, d_in, B.copymap, 0, false, d_out, cap, d_out_size, stream, launches, nullptr);
 }
 
 // ---- sharded copy-map iteration (see cham_prot_start_k) --------------------------------------------------------------------------------
-// The segment states and candidate tables sit in the seg_state region, in prot_iterate's layout: in_state [nseg + 1], out_state [nseg + 1]
-// (unused here), then gin [ngrp + 2] (as u32), T [nseg][PC_NC], GT [ngrp][PC_NC] (u16).
-struct ProtPtrs { uint32_t* in_state; uint32_t* gin; uint16_t* T; uint16_t* GT; };
-static ProtPtrs prot_ptrs(uint8_t* ws, const ChamLayout& L, uint32_t nseg) {
-    uint32_t* seg_state = reinterpret_cast<uint32_t*>(ws + L.seg_state);
-    uint16_t* ptab = reinterpret_cast<uint16_t*>(seg_state + 2 * (nseg + 1));
-    const uint32_t ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
-    ProtPtrs p;
-    p.in_state = seg_state;
-    p.gin = reinterpret_cast<uint32_t*>(ptab);
-    p.T = ptab + 2 * (ngrp + 2);
-    p.GT = p.T + (size_t)nseg * PC_NC;
-    return p;
-}
-
 cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
                             cudaStream_t stream, uint64_t* launches) {
     cham_prot_start_k<<<1, 32, 0, stream>>>(reinterpret_cast<Status*>(ws + L.status), ps, first_block, d_lengths, rank);
@@ -1726,38 +1698,26 @@ cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t*
 
 cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
                                int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    const uint32_t nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG), ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
-    const Status* st = reinterpret_cast<const Status*>(ws + L.status);
-    uint32_t* sigw = reinterpret_cast<uint32_t*>(ws + L.sigw);
-    const ProtPtrs p = prot_ptrs(ws, L, nseg);
-    if (nblocks) {
-        cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), d_carry_in, 0, nruns,
-                                                        reinterpret_cast<uint32_t*>(ws + L.carry), nullptr, st);
-        cham_resolve<<<dim3(32, nruns), 256, 0, stream>>>(reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-                                                         reinterpret_cast<uint32_t*>(ws + L.carry), ntiles, nruns, sigw, st);
-        cham_prot_seg_k<<<nseg < 2048u ? nseg : 2048u, PSEG, 0, stream>>>(sigw, nbytes, nblocks, nseg, st, it, ws + L.incb, ws + L.copymap, ps, p.T);
-        cham_prot_groups_k<<<(ngrp * PC_NC + 255) / 256, 256, 0, stream>>>(nseg, st, p.T, p.GT);
-        *launches += 4;
+    const ChamBufs B(ws, L, nbytes);
+    if (B.nblocks) {
+        launch_carry_resolve(B, nruns, d_carry_in, B.st, stream, launches);
+        cham_prot_seg_k<<<B.nseg < 2048u ? B.nseg : 2048u, PSEG, 0, stream>>>(B.sigw, nbytes, B.nblocks, B.nseg, B.st, it, B.incb, B.copymap, ps, B.T);
+        cham_prot_groups_k<<<(B.ngrp * PC_NC + 255) / 256, 256, 0, stream>>>(B.nseg, B.st, B.T, B.GT);
+        *launches += 2;
     }
-    cham_prot_transfer_k<<<1, 256, 0, stream>>>(nseg, st, p.GT, d_transfer_out);
+    cham_prot_transfer_k<<<1, 256, 0, stream>>>(B.nseg, B.st, B.GT, d_transfer_out);
     ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
                              uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG), ngrp = (nseg + PC_GROUP - 1) / PC_GROUP;
-    const Status* st = reinterpret_cast<const Status*>(ws + L.status);
-    const ProtPtrs p = prot_ptrs(ws, L, nseg);
-    cham_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, nseg, st, p.GT, p.gin, ps, d_words);
+    const ChamBufs B(ws, L, nbytes);
+    cham_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, B.nseg, B.st, B.GT, B.gin, ps, d_words);
     ++*launches;
-    if (nseg) {
-        cham_prot_seams_k<<<(ngrp + 127) / 128, 128, 0, stream>>>(nseg, st, p.T, p.gin, p.in_state);
-        cham_prot_walk_k<<<(nseg + 127) / 128, 128, 0, stream>>>(nblocks, nseg, st, it, ws + L.incb, ws + L.copymap, ws + L.copymap2, p.in_state,
-                                                                 p.gin, ps, d_words);
+    if (B.nseg) {
+        cham_prot_seams_k<<<(B.ngrp + 127) / 128, 128, 0, stream>>>(B.nseg, B.st, B.T, B.gin, B.in_state);
+        cham_prot_walk_k<<<(B.nseg + 127) / 128, 128, 0, stream>>>(B.nblocks, B.nseg, B.st, it, B.incb, B.copymap, B.copymap2, B.in_state, B.gin, ps, d_words);
         *launches += 2;
     }
     return cudaGetLastError();
@@ -1765,26 +1725,20 @@ cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, Pr
 
 cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
                            const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    const uint32_t ntiles = (uint32_t)((nblocks + 63) / 64);
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    if (nblocks) {
-        cham_prot_commit_k<<<(uint32_t)((nblocks + 1023) / 1024 < 1024 ? (nblocks + 1023) / 1024 : 1024), 256, 0, stream>>>(
-            d_all_words, world, nblocks, st, it, ws + L.copymap, ws + L.copymap2);
+    const ChamBufs B(ws, L, nbytes);
+    if (B.nblocks) {
+        cham_prot_commit_k<<<(uint32_t)((B.nblocks + 1023) / 1024 < 1024 ? (B.nblocks + 1023) / 1024 : 1024), 256, 0, stream>>>(
+            d_all_words, world, B.nblocks, B.st, it, B.copymap, B.copymap2);
         ++*launches;
     }
-    cham_prot_verdict_k<<<1, 32, 0, stream>>>(d_all_words, world, st, it, ps);
+    cham_prot_verdict_k<<<1, 32, 0, stream>>>(d_all_words, world, B.st, it, ps);
     ++*launches;
     if (d_table_out) {
-        if (nblocks) {   // round it + 1: flags under the new map (copy-mode blocks hidden from the dictionary) and the shard's table
+        if (B.nblocks) {   // round it + 1: flags under the new map (copy-mode blocks hidden from the dictionary) and the shard's table
             cudaError_t e = set_smem_attrs_once();
             if (e != cudaSuccess) return e;
-            launch_flag_pass(nruns, stream, reinterpret_cast<const uint32_t*>(d_in), nbytes / 4, ntiles, reinterpret_cast<uint32_t*>(ws + L.sigw),
-                             reinterpret_cast<uint2*>(ws + L.unres), reinterpret_cast<uint32_t*>(ws + L.unres_count),
-                             reinterpret_cast<uint32_t*>(ws + L.final_tab), ws + L.copymap, st);
-            cham_carry_scan<<<65536 / 256, 256, 0, stream>>>(reinterpret_cast<uint32_t*>(ws + L.final_tab), nullptr, 1, nruns, nullptr,
-                                                            d_table_out, st);
-            *launches += 2;
+            launch_flag_pass(B, d_in, nruns, B.copymap, B.st, stream, launches);
+            launch_export_fold(B, nruns, d_table_out, B.st, stream, launches);
         } else {
             cudaError_t e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), stream);   // nothing touched
             if (e != cudaSuccess) return e;
@@ -1795,14 +1749,13 @@ cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, cons
 
 cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
                              uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
-    const uint64_t nblocks = (nbytes + 255) / 256;
-    Status* st = reinterpret_cast<Status*>(ws + L.status);
-    cham_prot_finish_k<<<1, 32, 0, stream>>>(st, ps);
+    const ChamBufs B(ws, L, nbytes);
+    cham_prot_finish_k<<<1, 32, 0, stream>>>(B.st, ps);
     ++*launches;
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess && nblocks) e = cham_phase2_finish(d_in, nbytes, ws, L, d_out, cap, d_out_size, true, stream, launches, ev, false);
+    if (e == cudaSuccess && B.nblocks) e = cham_phase2_finish(B, d_in, d_out, cap, d_out_size, true, false, stream, launches, ev);
     if (e != cudaSuccess) return e;
-    cham_prot_seam_words_k<<<1, 32, 0, stream>>>(nblocks, st, d_out_size, d_seam8);
+    cham_prot_seam_words_k<<<1, 32, 0, stream>>>(B.nblocks, B.st, d_out_size, d_seam8);
     ++*launches;
     return cudaGetLastError();
 }

@@ -1,7 +1,6 @@
 // cheetah_encode.cu — run-parallel Cheetah and Lion encode for sm_90a (the Lion kernels start at "Lion (lion.rs:209-271)").
 //
-// Replaces /root/reference/src/algorithms/cheetah/cheetah.rs:121-150 and lion/lion.rs:209-271 (encode_quad) driven by
-// /root/reference/src/codec/codec.rs:34-80, bit-exactly. Cheetah's decomposition (validated against the oracle by
+// Replaces cheetah.rs:121-150 and lion.rs:209-271 (encode_quad) driven by codec.rs:34-80, bit-exactly. Cheetah's decomposition (validated against the oracle by
 // tools/proto_cheetah_runs.py; Lion's differs in step 1 only, see below and tools/proto_lion_runs.py):
 //
 //  1. PREDICTED_i <=> quad_i == the quad that followed the previous occurrence of the same CONTEXT, where the context is the
@@ -885,12 +884,19 @@ size_t chee_tables_bytes(int alg, int region, size_t nbytes, int num_sms) {
     return (size_t)chee_pick_runs(nbytes, num_sms) * 65536 * per;
 }
 
-// pointers into one workspace (chee_layout) and the three run-table regions
-struct CheeBufs {
-    Status* stages; uint32_t *Pb, *Ab, *Bb, *F0, *F1, *F2; uint8_t *cm, *cm2, *incb; uint32_t *seg, *ctx0, *tile_bytes, *tile_local;
+// One encode over `n` bytes cut into `nruns` runs, as every launch below sees it: the geometry, and typed pointers into the workspace
+// (chee_layout) and the three run-table regions. The last four pointers exist only behind a shard's workspace
+// (cl_shard_workspace_bytes): its gate, its emit gate, its pair flag and the epoch of the round it exports.
+struct CheeView {
+    bool lion; const uint32_t* in32; size_t n; uint32_t bbytes, nruns, ntiles, ngroups, run_ctas, nseg; uint64_t nq, nstep, nblk;
+    Status* stages; size_t stages_bytes; uint32_t *Pb, *Ab, *Bb, *F0, *F1, *F2; uint8_t *cm, *cm2, *incb; uint32_t *seg, *ctx0, *tile_bytes, *tile_local;
     uint64_t *group_total, *group_off; uint4* entP; uint32_t* coldP; uint4* entC;
-    CheeBufs(uint8_t* ws, const CheeLayout& L, uint8_t* const tables[3]) {
-        stages = reinterpret_cast<Status*>(ws + L.status);
+    Status *gate, *emit; uint32_t *pair_flag, *epoch_word;
+    CheeView(int alg, const uint8_t* d_in, size_t nbytes, int num_sms, uint8_t* ws, uint8_t* const tables[3]) {
+        lion = alg == ALG_LION; bbytes = lion ? 64 : 128; in32 = reinterpret_cast<const uint32_t*>(d_in);
+        cut(nbytes, chee_pick_runs(nbytes, num_sms));
+        CheeLayout L; chee_layout(nbytes, nruns, &L);
+        stages = reinterpret_cast<Status*>(ws + L.status); stages_bytes = L.Pbits - L.status;
         Pb = reinterpret_cast<uint32_t*>(ws + L.Pbits); Ab = reinterpret_cast<uint32_t*>(ws + L.Abits); Bb = reinterpret_cast<uint32_t*>(ws + L.Bbits);
         F0 = reinterpret_cast<uint32_t*>(ws + L.F0); F1 = reinterpret_cast<uint32_t*>(ws + L.F1); F2 = reinterpret_cast<uint32_t*>(ws + L.F2);
         cm = ws + L.copymap; cm2 = ws + L.copymap2; incb = ws + L.incb;
@@ -899,84 +905,116 @@ struct CheeBufs {
         tile_bytes = reinterpret_cast<uint32_t*>(ws + L.tile_bytes); tile_local = reinterpret_cast<uint32_t*>(ws + L.tile_local);
         group_total = reinterpret_cast<uint64_t*>(ws + L.group_total); group_off = reinterpret_cast<uint64_t*>(ws + L.group_off);
         entP = reinterpret_cast<uint4*>(tables[0]); coldP = reinterpret_cast<uint32_t*>(tables[1]); entC = reinterpret_cast<uint4*>(tables[2]);
+        gate = reinterpret_cast<Status*>(ws + ((L.total + 255) & ~(size_t)255)); emit = gate + 1; pair_flag = reinterpret_cast<uint32_t*>(emit + 1);
+        epoch_word = pair_flag + 1;
+    }
+    // the same buffers for the first `nbytes` of the input cut into `runs` runs (the prefix stages of chee_iterate)
+    CheeView prefix(size_t nbytes, uint32_t runs) const { CheeView v = *this; v.cut(nbytes, runs); return v; }
+private:
+    void cut(size_t nbytes, uint32_t runs) {
+        n = nbytes; nruns = runs; nq = n / 4; nstep = (n + 127) / 128; nblk = (n + bbytes - 1) / bbytes;
+        ntiles = (uint32_t)((nstep + TILE_B - 1) / TILE_B); ngroups = (ntiles + 4095) / 4096; run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
+        nseg = (uint32_t)((nblk + 255) / 256);
     }
 };
+
+// ---- the steps of one round, each the only place where Cheetah and Lion part for that step. `mask`: the copy map in force (nullptr =
+// none), `gate`: the Status block the kernels run under; the carried-in tables are stacks of planes as cl_table_init / cl_rank_fold
+// leave them (nullptr = stream start), of which the fold kernels take the state planes.
+static void launch_ctx0_pass_p(const CheeView& V, const uint8_t* mask, Status* gate, const uint32_t* d_prev_quad, uint32_t epoch, uint32_t* d_epoch_out,
+                               cudaStream_t stream, uint64_t* launches) {
+    if (V.lion) {
+        lion_ctx0<<<(V.nruns + 127) / 128, 128, 0, stream>>>(V.in32, V.nq, mask, V.nruns, V.ntiles, gate, d_prev_quad, epoch, d_epoch_out, V.ctx0);
+        lion_pass_p<<<V.run_ctas, RP_WARPS * 32, 0, stream>>>(V.in32, V.nq, V.nstep, V.nblk, mask, V.nruns, V.ntiles, gate, V.ctx0, V.entP, V.coldP, epoch,
+                                                              V.F0, V.F1, V.F2, V.Pb);
+    } else {
+        chee_ctx0<<<(V.nruns + 127) / 128, 128, 0, stream>>>(V.in32, V.nq, mask, V.nruns, V.ntiles, gate, d_prev_quad, epoch, d_epoch_out, V.ctx0);
+        chee_pass_p<<<V.run_ctas, RP_WARPS * 32, 0, stream>>>(V.in32, V.nq, V.nstep, mask, V.nruns, V.ntiles, gate, V.ctx0, V.entP, epoch, V.Pb);
+    }
+    *launches += 2;
+}
+static void launch_fold_p_pass_c(const CheeView& V, const uint8_t* mask, Status* gate, uint32_t epoch, const uint32_t* d_carry_p, cudaStream_t stream,
+                                 uint64_t* launches) {
+    if (V.lion) {
+        lion_fold_p<<<PL / 128, 128, 0, stream>>>(V.in32, V.nruns, gate, V.entP, V.coldP, epoch, d_carry_p ? d_carry_p + 2 * PL : nullptr, V.F0, V.F1, V.F2, V.Pb);
+        chee_pass_c<2><<<V.run_ctas, RP_WARPS * 32, 0, stream>>>(V.in32, V.nq, V.nstep, V.nblk, mask, V.nruns, V.ntiles, gate, V.Pb, V.entC, epoch, V.Ab, V.Bb);
+    } else {
+        chee_fold_p<<<PL / 128, 128, 0, stream>>>(V.in32, V.nruns, gate, V.entP, epoch, d_carry_p ? d_carry_p + PL : nullptr, V.Pb);
+        chee_pass_c<1><<<V.run_ctas, RP_WARPS * 32, 0, stream>>>(V.in32, V.nq, V.nstep, V.nblk, mask, V.nruns, V.ntiles, gate, V.Pb, V.entC, epoch, V.Ab, V.Bb);
+    }
+    *launches += 2;
+}
+static void launch_fold_c(const CheeView& V, Status* gate, uint32_t epoch, const uint32_t* d_carry_c, cudaStream_t stream, uint64_t* launches) {
+    chee_fold_c<<<PL / 128, 128, 0, stream>>>(V.in32, V.nruns, gate, V.entC, epoch, d_carry_c ? d_carry_c + PL : nullptr, V.Ab, V.Bb);
+    ++*launches;
+}
+// tile sizes and incompressible bits; final_pass: the sizes under a committed map, valid only if `gate` has converged
+static void launch_tile_sizes(const CheeView& V, const uint8_t* mask, int final_pass, Status* gate, cudaStream_t stream, uint64_t* launches) {
+    if (V.lion) lion_tile_sizes<<<(V.ntiles + 7) / 8, 256, 0, stream>>>(V.Pb, V.Ab, V.Bb, mask, V.n, V.nblk, V.ntiles, final_pass, gate, V.incb, V.tile_bytes);
+    else chee_tile_sizes<<<(V.ntiles + 7) / 8, 256, 0, stream>>>(V.Pb, V.Ab, V.Bb, mask, V.n, V.nblk, V.ntiles, final_pass, gate, V.incb, V.tile_bytes);
+    ++*launches;
+}
+// tile offsets from the tile sizes (and the stream's size, checked against `cap`), then emit
+static cudaError_t launch_scan_emit(const CheeView& V, const uint8_t* mask, Status* gate, size_t cap, uint64_t* d_out_size, uint8_t* d_out,
+                                    cudaStream_t stream, uint64_t* launches) {
+    cudaError_t e = scan_tiles_launch(V.tile_bytes, V.ntiles, V.tile_local, V.group_total, V.group_off, V.ngroups, gate, cap, d_out_size, stream);
+    if (e != cudaSuccess) return e;
+    if (V.lion) lion_emit<<<V.ntiles, 256, 0, stream>>>(V.in32, V.n, V.nblk, V.F0, V.F1, V.F2, V.Pb, V.Ab, V.Bb, mask, gate, V.tile_local, V.group_off, 4096, d_out);
+    else chee_emit<<<V.ntiles, 256, 0, stream>>>(V.in32, V.n, V.nblk, V.Pb, V.Ab, V.Bb, mask, gate, V.tile_local, V.group_off, 4096, d_out);
+    *launches += 3;
+    return cudaSuccess;
+}
 
 // The staged copy-map iteration (epochs epoch_base .. epoch_base + 31). *st_out = the Status block of the last stage: converged != 0
 // means the committed copy map (cm) and the flags and run tables of the last round that ran are final; *d_epoch_out (device, may be
 // nullptr) receives that round's epoch.
-static cudaError_t chee_iterate(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* ws, const CheeLayout& L, uint32_t nruns, uint8_t* const tables[3],
-                                uint32_t epoch_base, int num_sms, bool resume, uint32_t* d_epoch_out, cudaStream_t stream, uint64_t* launches,
-                                Status** st_out) {
-    const bool lion = alg == ALG_LION;
-    const uint32_t bbytes = lion ? 64 : 128;
-    const uint32_t ntiles = (uint32_t)(((nbytes + 127) / 128 + TILE_B - 1) / TILE_B);
-    const CheeBufs B(ws, L, tables);
-    Status* const stages = B.stages;
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    uint32_t* Pb = B.Pb; uint32_t* Ab = B.Ab; uint32_t* Bb = B.Bb; uint32_t* F0 = B.F0; uint32_t* F1 = B.F1; uint32_t* F2 = B.F2;
-    uint8_t* cm = B.cm; uint8_t* cm2 = B.cm2; uint8_t* incb = B.incb;
-    uint32_t* seg = B.seg; uint32_t* ctx0 = B.ctx0; uint32_t* tile_bytes = B.tile_bytes;
-    uint4* entP = B.entP; uint32_t* coldP = B.coldP; uint4* entC = B.entC;
-    cudaError_t e = cudaMemsetAsync(ws + L.status, 0, L.Pbits - L.status, stream);     // both status blocks
+static cudaError_t chee_iterate(const CheeView& V, uint32_t epoch_base, int num_sms, bool resume, uint32_t* d_epoch_out, cudaStream_t stream,
+                                uint64_t* launches, Status** st_out) {
+    cudaError_t e = cudaMemsetAsync(V.stages, 0, V.stages_bytes, stream);     // every stage's status block
     if (e != cudaSuccess) return e;
 
-    // one fixed-point round over the first `nb` bytes cut into `runs` runs: flags under the current map, incompressible bits, automaton
-    auto round = [&](Status* st, int it, size_t nb, uint32_t runs, uint32_t epoch) -> cudaError_t {
-        const uint64_t nq = nb / 4, nstep = (nb + 127) / 128, nblk = (nb + bbytes - 1) / bbytes;
-        const uint32_t nt = (uint32_t)((nstep + TILE_B - 1) / TILE_B);
-        const uint32_t nseg = (uint32_t)((nblk + 255) / 256);
-        const uint32_t run_ctas = (runs + RP_WARPS - 1) / RP_WARPS;
-        const uint8_t* mask = it ? cm : nullptr;
-        if (lion) {
-            lion_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, nullptr, epoch, d_epoch_out, ctx0);
-            lion_pass_p<<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, ctx0, entP, coldP, epoch, F0, F1, F2, Pb);
-            lion_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, coldP, epoch, nullptr, F0, F1, F2, Pb);
-            chee_pass_c<2><<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, Pb, entC, epoch, Ab, Bb);
-            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, nullptr, Ab, Bb);
-            lion_tile_sizes<<<(nt + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, mask, nb, nblk, nt, 0, st, incb, tile_bytes);
-        } else {
-            chee_ctx0<<<(runs + 127) / 128, 128, 0, stream>>>(in32, nq, mask, runs, nt, st, nullptr, epoch, d_epoch_out, ctx0);
-            chee_pass_p<<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, mask, runs, nt, st, ctx0, entP, epoch, Pb);
-            chee_fold_p<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entP, epoch, nullptr, Pb);
-            chee_pass_c<1><<<run_ctas, RP_WARPS * 32, 0, stream>>>(in32, nq, nstep, nblk, mask, runs, nt, st, Pb, entC, epoch, Ab, Bb);
-            chee_fold_c<<<65536 / 128, 128, 0, stream>>>(in32, runs, st, entC, epoch, nullptr, Ab, Bb);
-            chee_tile_sizes<<<(nt + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, mask, nb, nblk, nt, 0, st, incb, tile_bytes);
-        }
-        *launches += 7;
-        return prot_iterate_launch(nullptr, nb, nblk, nseg, st, it, incb, cm, cm2, seg, seg + (nseg + 1), (int)bbytes, num_sms, stream);
+    // one fixed-point round over R (the input or a prefix of it): flags under the current map, incompressible bits, automaton
+    auto round = [&](const CheeView& R, Status* st, int it, uint32_t epoch) -> cudaError_t {
+        const uint8_t* mask = it ? R.cm : nullptr;
+        launch_ctx0_pass_p(R, mask, st, nullptr, epoch, d_epoch_out, stream, launches);
+        launch_fold_p_pass_c(R, mask, st, epoch, nullptr, stream, launches);
+        launch_fold_c(R, st, epoch, nullptr, stream, launches);
+        launch_tile_sizes(R, mask, 0, st, stream, launches);
+        ++*launches;
+        return prot_iterate_launch(nullptr, R.n, R.nblk, R.nseg, st, it, R.incb, R.cm, R.cm2, R.seg, R.seg + (R.nseg + 1), num_sms, stream);
     };
 
     // A stage = up to 8 rounds on one Status block (prot_iterate owns 8 grid-barrier slots per block).
     // test hook (density_b200_test_set_stage_rounds): cut every stage to rounds first..k so that the resume path can be exercised
     const int last_it = g_chee_stage_rounds;
-    auto stage = [&](Status* st, const Status* inherit, int first_it, size_t nb, uint32_t runs, uint32_t ep0) -> cudaError_t {
+    auto stage = [&](const CheeView& R, Status* st, const Status* inherit, int first_it, uint32_t ep0) -> cudaError_t {
         chee_chain_gate<<<1, 1, 0, stream>>>(st, inherit); ++*launches;
         for (int it = first_it; it <= last_it; ++it) {
-            cudaError_t err = round(st, it, nb, runs, ep0 + (uint32_t)it);
+            cudaError_t err = round(R, st, it, ep0 + (uint32_t)it);
             if (err != cudaSuccess) return err;
         }
         return cudaSuccess;
     };
+    Status* const stages = V.stages;
     Status* st;
-    if (ntiles > 2 * PREFIX_TILES) {
+    if (V.ntiles > 2 * PREFIX_TILES) {
         // Stages A1, A2: a cold dictionary makes the first blocks incompressible on every input, and settling that takes 4-10 rounds
         // (copied blocks perturb the sizes of their near-threshold neighbours): run them on the first MiB alone (the copy map of a
         // prefix does not depend on what follows). Stages B1, B2 then start from that map and normally confirm it in one round
         // over the whole input.
-        const size_t nbA = (size_t)PREFIX_TILES * TILE_B * 128;
+        const CheeView A = V.prefix((size_t)PREFIX_TILES * TILE_B * 128, PREFIX_TILES);
         if (!resume) {
-            e = cudaMemsetAsync(cm, 0, (size_t)ntiles * TILE_B * 2, stream);
+            e = cudaMemsetAsync(V.cm, 0, (size_t)V.ntiles * TILE_B * 2, stream);
             if (e != cudaSuccess) return e;
-            e = stage(&stages[0], nullptr, 0, nbA, PREFIX_TILES, epoch_base);
-            if (e == cudaSuccess) e = stage(&stages[1], &stages[0], 1, nbA, PREFIX_TILES, epoch_base + 8);
+            e = stage(A, &stages[0], nullptr, 0, epoch_base);
+            if (e == cudaSuccess) e = stage(A, &stages[1], &stages[0], 1, epoch_base + 8);
         }
-        if (e == cudaSuccess) e = stage(&stages[2], nullptr, 1, nbytes, nruns, epoch_base + 16);
-        if (e == cudaSuccess) e = stage(&stages[3], &stages[2], 1, nbytes, nruns, epoch_base + 24);
+        if (e == cudaSuccess) e = stage(V, &stages[2], nullptr, 1, epoch_base + 16);
+        if (e == cudaSuccess) e = stage(V, &stages[3], &stages[2], 1, epoch_base + 24);
         st = &stages[3];
     } else {
-        e = stage(&stages[0], nullptr, resume ? 1 : 0, nbytes, nruns, epoch_base);
-        if (e == cudaSuccess) e = stage(&stages[1], &stages[0], 1, nbytes, nruns, epoch_base + 8);
+        e = stage(V, &stages[0], nullptr, resume ? 1 : 0, epoch_base);
+        if (e == cudaSuccess) e = stage(V, &stages[1], &stages[0], 1, epoch_base + 8);
         st = &stages[1];
     }
     *st_out = st;
@@ -991,32 +1029,16 @@ static cudaError_t chee_iterate(int alg, const uint8_t* d_in, size_t nbytes, uin
 cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* const tables[3],
                                  uint32_t epoch_base, int num_sms, uint64_t* d_out_size, uint32_t* d_converged, bool resume,
                                  cudaStream_t stream, uint64_t* launches) {
-    const bool lion = alg == ALG_LION;
-    const uint32_t bbytes = lion ? 64 : 128;
-    const uint32_t nruns = chee_pick_runs(nbytes, num_sms);
-    CheeLayout L; chee_layout(nbytes, nruns, &L);
-    const uint64_t nblocks = (nbytes + bbytes - 1) / bbytes;
-    const uint32_t ntiles = (uint32_t)(((nbytes + 127) / 128 + TILE_B - 1) / TILE_B);
-    const uint32_t ngroups = (ntiles + 4095) / 4096;
-    const CheeBufs B(ws, L, tables);
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    uint32_t* Pb = B.Pb; uint32_t* Ab = B.Ab; uint32_t* Bb = B.Bb; uint32_t* F0 = B.F0; uint32_t* F1 = B.F1; uint32_t* F2 = B.F2;
-    uint8_t* cm = B.cm; uint8_t* incb = B.incb; uint32_t* tile_bytes = B.tile_bytes;
+    const CheeView V(alg, d_in, nbytes, num_sms, ws, tables);
     Status* st = nullptr;
-    cudaError_t e = chee_iterate(alg, d_in, nbytes, ws, L, nruns, tables, epoch_base, num_sms, resume, nullptr, stream, launches, &st);
+    cudaError_t e = chee_iterate(V, epoch_base, num_sms, resume, nullptr, stream, launches, &st);
     if (e != cudaSuccess) return e;
     // final sizes under the committed copy map (valid only if converged), scan, emit
-    if (lion) lion_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, cm, nbytes, nblocks, ntiles, 1, st, incb, tile_bytes);
-    else chee_tile_sizes<<<(ntiles + 7) / 8, 256, 0, stream>>>(Pb, Ab, Bb, cm, nbytes, nblocks, ntiles, 1, st, incb, tile_bytes);
-    e = scan_tiles_launch(tile_bytes, ntiles, reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                          reinterpret_cast<uint64_t*>(ws + L.group_total), reinterpret_cast<uint64_t*>(ws + L.group_off), ngroups, st, cap, d_out_size, stream);
+    launch_tile_sizes(V, V.cm, 1, st, stream, launches);
+    e = launch_scan_emit(V, V.cm, st, cap, d_out_size, d_out, stream, launches);
     if (e != cudaSuccess) return e;
-    if (lion) lion_emit<<<ntiles, 256, 0, stream>>>(in32, nbytes, nblocks, F0, F1, F2, Pb, Ab, Bb, cm, st, reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                                    reinterpret_cast<uint64_t*>(ws + L.group_off), 4096, d_out);
-    else chee_emit<<<ntiles, 256, 0, stream>>>(in32, nbytes, nblocks, Pb, Ab, Bb, cm, st, reinterpret_cast<uint32_t*>(ws + L.tile_local),
-                                               reinterpret_cast<uint64_t*>(ws + L.group_off), 4096, d_out);
     chee_finish<<<1, 1, 0, stream>>>(st, d_converged, d_out_size);
-    *launches += 5;
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -1033,49 +1055,22 @@ uint32_t cl_shard_epochs() { return CL_SHARD_EPOCHS; }
 uint32_t cl_table_planes(int alg, int kind) { return kind == 1 ? 3u : alg == ALG_LION ? 12u : 2u; }
 size_t cl_shard_workspace_bytes(size_t nbytes, int num_sms) { return ((chee_workspace_bytes(nbytes, num_sms) + 255) & ~(size_t)255) + 1024; }
 
-namespace {
-struct ClShardGeo {
-    bool lion; uint32_t bbytes, nruns, ntiles, ngroups, run_ctas; uint64_t nq, nstep, nblk; CheeLayout L;
-    Status *gate, *emit; uint32_t *pair_flag, *epoch_word;
-    ClShardGeo(int alg, size_t n, int num_sms, uint8_t* ws) {
-        lion = alg == ALG_LION; bbytes = lion ? 64 : 128;
-        nruns = chee_pick_runs(n, num_sms); chee_layout(n, nruns, &L);
-        nq = n / 4; nstep = (n + 127) / 128; nblk = (n + bbytes - 1) / bbytes;
-        ntiles = (uint32_t)((nstep + TILE_B - 1) / TILE_B); ngroups = (ntiles + 4095) / 4096; run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
-        gate = reinterpret_cast<Status*>(ws + ((L.total + 255) & ~(size_t)255)); emit = gate + 1; pair_flag = reinterpret_cast<uint32_t*>(emit + 1);
-        epoch_word = pair_flag + 1;
-    }
-};
-}  // namespace
-
 // Phase 1: the first shard (d_prev_quad == nullptr) runs the copy-map iteration to the end; a later shard runs ctx0 and pass P. Both
 // export their P transfer.
 cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32_t* d_prev_quad, uint8_t* ws, uint8_t* const tables[3],
                             uint32_t epoch_base, int num_sms, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches) {
-    const ClShardGeo G(alg, n, num_sms, ws);
-    const CheeBufs B(ws, G.L, tables);
+    const CheeView V(alg, d_in, n, num_sms, ws, tables);
     const bool first = d_prev_quad == nullptr;
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
     const uint32_t ep = epoch_base + 32;
     Status* iter = nullptr;
     cudaError_t e = cudaSuccess;
-    if (first) e = chee_iterate(alg, d_in, n, ws, G.L, G.nruns, tables, epoch_base, num_sms, false, G.epoch_word, stream, launches, &iter);
+    if (first) e = chee_iterate(V, epoch_base, num_sms, false, V.epoch_word, stream, launches, &iter);
     if (e != cudaSuccess) return e;
-    cl_shard_gates<<<1, 1, 0, stream>>>(G.gate, G.emit, iter, G.pair_flag, G.epoch_word, ep);
+    cl_shard_gates<<<1, 1, 0, stream>>>(V.gate, V.emit, iter, V.pair_flag, V.epoch_word, ep);
     ++*launches;
-    if (!first) {
-        if (G.lion) {
-            lion_ctx0<<<(G.nruns + 127) / 128, 128, 0, stream>>>(in32, G.nq, nullptr, G.nruns, G.ntiles, G.gate, d_prev_quad, ep, nullptr, B.ctx0);
-            lion_pass_p<<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.ctx0, B.entP, B.coldP,
-                                                                  ep, B.F0, B.F1, B.F2, B.Pb);
-        } else {
-            chee_ctx0<<<(G.nruns + 127) / 128, 128, 0, stream>>>(in32, G.nq, nullptr, G.nruns, G.ntiles, G.gate, d_prev_quad, ep, nullptr, B.ctx0);
-            chee_pass_p<<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, nullptr, G.nruns, G.ntiles, G.gate, B.ctx0, B.entP, ep, B.Pb);
-        }
-        *launches += 2;
-    }
-    if (G.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(in32, B.entP, B.coldP, G.nruns, G.epoch_word, d_tab_p);
-    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(B.entP, G.nruns, G.epoch_word, d_tab_p);
+    if (!first) launch_ctx0_pass_p(V, nullptr, V.gate, d_prev_quad, ep, nullptr, stream, launches);
+    if (V.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(V.in32, V.entP, V.coldP, V.nruns, V.epoch_word, d_tab_p);
+    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(V.entP, V.nruns, V.epoch_word, d_tab_p);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1085,20 +1080,9 @@ cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32
 // stream start, and its flags are final already).
 cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, const uint32_t* d_carry_p, uint8_t* ws, uint8_t* const tables[3],
                             uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
-    const ClShardGeo G(alg, n, num_sms, ws);
-    const CheeBufs B(ws, G.L, tables);
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    const uint32_t ep = epoch_base + 32;
-    if (!first && G.lion) {
-        lion_fold_p<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entP, B.coldP, ep, d_carry_p ? d_carry_p + 2 * PL : nullptr, B.F0, B.F1, B.F2, B.Pb);
-        chee_pass_c<2><<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.Pb, B.entC, ep, B.Ab, B.Bb);
-        *launches += 2;
-    } else if (!first) {
-        chee_fold_p<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entP, ep, d_carry_p ? d_carry_p + PL : nullptr, B.Pb);
-        chee_pass_c<1><<<G.run_ctas, RP_WARPS * 32, 0, stream>>>(in32, G.nq, G.nstep, G.nblk, nullptr, G.nruns, G.ntiles, G.gate, B.Pb, B.entC, ep, B.Ab, B.Bb);
-        *launches += 2;
-    }
-    cl_export_c<<<PL / 128, 128, 0, stream>>>(B.entC, G.nruns, G.epoch_word, d_tab_c);
+    const CheeView V(alg, d_in, n, num_sms, ws, tables);
+    if (!first) launch_fold_p_pass_c(V, nullptr, V.gate, epoch_base + 32, d_carry_p, stream, launches);
+    cl_export_c<<<PL / 128, 128, 0, stream>>>(V.entC, V.nruns, V.epoch_word, d_tab_c);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1108,30 +1092,20 @@ cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, 
 cudaError_t cl_shard_phase3(int alg, const uint8_t* d_in, size_t n, bool first, bool is_last, const uint32_t* d_carry_c, uint8_t* ws,
                             uint8_t* const tables[3], uint32_t epoch_base, int num_sms, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                             uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
-    const ClShardGeo G(alg, n, num_sms, ws);
-    const CheeBufs B(ws, G.L, tables);
-    const uint32_t* in32 = reinterpret_cast<const uint32_t*>(d_in);
-    const uint32_t ep = epoch_base + 32;
-    const uint8_t* mask = first ? B.cm : nullptr;
+    const CheeView V(alg, d_in, n, num_sms, ws, tables);
+    const uint8_t* mask = first ? V.cm : nullptr;
+    if (!first) launch_fold_c(V, V.gate, epoch_base + 32, d_carry_c, stream, launches);
+    launch_tile_sizes(V, mask, 0, V.gate, stream, launches);
     if (!first) {
-        chee_fold_c<<<PL / 128, 128, 0, stream>>>(in32, G.nruns, G.gate, B.entC, ep, d_carry_c ? d_carry_c + PL : nullptr, B.Ab, B.Bb);
-        ++*launches;
-    }
-    if (G.lion) lion_tile_sizes<<<(G.ntiles + 7) / 8, 256, 0, stream>>>(B.Pb, B.Ab, B.Bb, mask, n, G.nblk, G.ntiles, 0, G.gate, B.incb, B.tile_bytes);
-    else chee_tile_sizes<<<(G.ntiles + 7) / 8, 256, 0, stream>>>(B.Pb, B.Ab, B.Bb, mask, n, G.nblk, G.ntiles, 0, G.gate, B.incb, B.tile_bytes);
-    ++*launches;
-    if (!first) {
-        const uint64_t want = (G.nblk + 255) / 256;
+        const uint64_t want = (V.nblk + 255) / 256;
         const uint32_t grid = (uint32_t)(want < (uint64_t)num_sms * 8 ? (want ? want : 1) : (uint64_t)num_sms * 8);
-        cl_inc_pairs<<<grid, 256, 0, stream>>>(B.incb, G.nblk, G.pair_flag);
+        cl_inc_pairs<<<grid, 256, 0, stream>>>(V.incb, V.nblk, V.pair_flag);
         ++*launches;
     }
-    cudaError_t e = scan_tiles_launch(B.tile_bytes, G.ntiles, B.tile_local, B.group_total, B.group_off, G.ngroups, G.emit, cap, d_out_size, stream);
+    cudaError_t e = launch_scan_emit(V, mask, V.emit, cap, d_out_size, d_out, stream, launches);
     if (e != cudaSuccess) return e;
-    if (G.lion) lion_emit<<<G.ntiles, 256, 0, stream>>>(in32, n, G.nblk, B.F0, B.F1, B.F2, B.Pb, B.Ab, B.Bb, mask, G.emit, B.tile_local, B.group_off, 4096, d_out);
-    else chee_emit<<<G.ntiles, 256, 0, stream>>>(in32, n, G.nblk, B.Pb, B.Ab, B.Bb, mask, G.emit, B.tile_local, B.group_off, 4096, d_out);
-    cl_seam_words_k<<<1, 1, 0, stream>>>(B.incb, mask, G.nblk, first, is_last, G.emit, first ? nullptr : G.pair_flag, d_out_size, d_seam8);
-    *launches += 4;
+    cl_seam_words_k<<<1, 1, 0, stream>>>(V.incb, mask, V.nblk, first, is_last, V.emit, first ? nullptr : V.pair_flag, d_out_size, d_seam8);
+    ++*launches;
     return cudaGetLastError();
 }
 

@@ -580,8 +580,6 @@ using namespace cheedec;
 struct CheeDecLayout { bounds::BoundsLayout B; size_t cs, flags, K, usym, ctx_in, ctx_out, dirty, run_epoch, rbits, cin, snap0, total; };
 
 static uint32_t cd_pick_runs(size_t nbytes, int num_sms) {
-    const uint64_t maxblocks = nbytes / 8 + 2;
-    (void)maxblocks;
     // a run should decode to >= 64 KiB (512 blocks); the stream is at most 8.5 bytes per block... use the stream size as a proxy
     uint64_t r = nbytes / (48u << 10);
     static const int per_sm = [] { const char* v = getenv("DENSITY_B200_DEC_RUNS_PER_SM"); const int k = v ? atoi(v) : 0; return (k >= 1 && k <= 32) ? k : 8; }();
@@ -614,133 +612,135 @@ size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms) { Che
 // the per-run tables (zeroed at the start of every call): chunk map 16 B, prediction 8 B per run and key
 size_t chee_decode_tables_bytes(size_t nbytes, int num_sms) { return (size_t)cd_pick_runs(nbytes, num_sms) * 65536 * (sizeof(uint4) + sizeof(uint2)); }
 
+// The decoder's view of one call: the run geometry, the boundary layout and typed pointers into the workspace (cd_layout), the per-run
+// tables and the tail's tables (the scalar_codec.cu workspace: Status (256 B) + chunk_a + chunk_b + pred), which receive the folded
+// tables for the tail loop. A piece of a sharded stream keeps more behind the layout in its own workspace: the fallback word and the
+// PieceStatus (256 B), then its tail tables, taken when `tail_ws` is null. `tables` may be null for a caller that only wants addresses
+// inside the workspace.
+struct CheeDecPtrs {
+    uint32_t nruns, run_ctas; int wide; bounds::BoundsLayout B;
+    DecStatus* st; ClStatus* cs; uint64_t* blk_off; uint4* flags; uint16_t* K; uint2* usym;
+    uint32_t *ctx_in, *ctx_out, *dirty_cur, *dirty_next, *run_epoch, *rbits, *snap, *fallback, *chunk_a, *chunk_b, *pred_final;
+    uint2* cin; uint8_t* tables; size_t tables_bytes; uint4* entC; uint2* entP; PieceStatus* pst; uint8_t* tail_ws;
+    CheeDecPtrs(size_t n, size_t cap, int num_sms, uint8_t* ws, uint8_t* tables_, uint8_t* tail_ws_) {
+        nruns = cd_pick_runs(n, num_sms);
+        run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
+        wide = num_sms * 8;
+        CheeDecLayout L; cd_layout(n, cap, nruns, &L);
+        B = L.B;
+        const size_t off = (L.total + 255) & ~(size_t)255;
+        st = reinterpret_cast<DecStatus*>(ws + L.B.status);
+        cs = reinterpret_cast<ClStatus*>(ws + L.cs);
+        blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
+        flags = reinterpret_cast<uint4*>(ws + L.flags);
+        K = reinterpret_cast<uint16_t*>(ws + L.K);
+        usym = reinterpret_cast<uint2*>(ws + L.usym);
+        ctx_in = reinterpret_cast<uint32_t*>(ws + L.ctx_in);
+        ctx_out = reinterpret_cast<uint32_t*>(ws + L.ctx_out);
+        dirty_cur = reinterpret_cast<uint32_t*>(ws + L.dirty);
+        dirty_next = dirty_cur + nruns;
+        run_epoch = reinterpret_cast<uint32_t*>(ws + L.run_epoch);
+        rbits = reinterpret_cast<uint32_t*>(ws + L.rbits);
+        cin = reinterpret_cast<uint2*>(ws + L.cin);
+        snap = reinterpret_cast<uint32_t*>(ws + L.snap0);
+        fallback = reinterpret_cast<uint32_t*>(ws + off);
+        pst = reinterpret_cast<PieceStatus*>(ws + off + 128);
+        tail_ws = tail_ws_ ? tail_ws_ : ws + off + 256;
+        chunk_a = reinterpret_cast<uint32_t*>(tail_ws + 256);
+        chunk_b = chunk_a + PL;
+        pred_final = chunk_a + 2 * PL;
+        tables = tables_; tables_bytes = chee_decode_tables_bytes(n, num_sms);
+        entC = reinterpret_cast<uint4*>(tables);
+        entP = tables ? reinterpret_cast<uint2*>(tables + (size_t)nruns * PL * sizeof(uint4)) : nullptr;
+    }
+};
+
+// ---- the launch sequences that the one-shot decode and the phases of a piece share ------------------------------------------------------
+// the per-run tables and run 0's snapshot (the zero table) start every call as zeros
+static cudaError_t cd_clear_tables(const CheeDecPtrs& p, cudaStream_t stream) {
+    cudaError_t e = cudaMemsetAsync(p.tables, 0, p.tables_bytes, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.snap, 0, (size_t)p.nruns * PL * sizeof(uint32_t), stream);
+    return e;
+}
+// unpack (literals and copy-mode blocks go straight to the output) and the symbolic chunk-map walk
+static void cd_launch_unpack_walk(const CheeDecPtrs& p, const uint8_t* d_in, uint32_t* out32, cudaStream_t stream, uint64_t* launches) {
+    cd_unpack<<<p.wide, 256, 0, stream>>>(d_in, p.blk_off, p.st, p.flags, p.K, out32);
+    cd_cmap_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.entC, out32, p.usym);
+    *launches += 2;
+}
+// the chunk map carried in (d_cmap_carry: nullptr = the stream start), the reads of carried-in slots, the context init
+static void cd_launch_cmap_resolve(const CheeDecPtrs& p, uint32_t* out32, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
+    cd_cmap_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.nruns, p.entC, p.cin, p.chunk_a, p.chunk_b, d_cmap_carry);
+    cd_cmap_resolve<<<p.wide, 256, 0, stream>>>(p.st, p.nruns, p.usym, p.K, p.cin, out32);
+    cd_ctx_init<<<(p.nruns + 127) / 128, 128, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.ctx_in, p.dirty_cur, p.dirty_next, p.run_epoch, p.cs);
+    *launches += 3;
+}
+// a prediction round: walk the dirty runs (run0_snap: run 0 starts from the stream start's zero table) ...
+static void cd_launch_pred_walk(const CheeDecPtrs& p, uint32_t round, uint32_t* out32, uint32_t run0_snap, cudaStream_t stream, uint64_t* launches) {
+    cd_pred_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.cs, p.nruns, round, p.flags, p.K, p.entP, p.snap, p.ctx_in, p.ctx_out, p.dirty_cur,
+                                                           p.dirty_next, p.run_epoch, p.rbits, out32, run0_snap);
+    ++*launches;
+}
+// ... and the snapshots from the table carried into this round (d_pred_carry: nullptr = the stream start's zeros)
+static void cd_launch_pred_fold(const CheeDecPtrs& p, uint32_t round, const uint32_t* d_pred_carry, cudaStream_t stream, uint64_t* launches) {
+    cd_pred_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.cs, p.nruns, round, p.entP, p.snap, p.run_epoch, p.rbits, p.dirty_next, p.pred_final, d_pred_carry);
+    ++*launches;
+}
+// the verdict of the rounds: *d_fallback != 0 afterwards means the in-order kernel must run instead
+static void cd_launch_finish(const CheeDecPtrs& p, uint32_t* d_fallback, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches) {
+    cd_finish<<<1, 1, 0, stream>>>(p.st, p.cs, d_fallback, d_out_size);
+    ++*launches;
+}
+
 // Enqueues the parallel Cheetah decode. The block count of the main loop is only known on the device; the output needs
 // cap >= main_blocks * 128 (checked on the device). *d_fallback != 0 afterwards: the caller's in-order kernel must run instead.
-// `tail` = the scalar workspace (scalar_codec.cu layout): receives the folded tables for the tail loop.
+// `tail_ws` = the scalar workspace (scalar_codec.cu layout): receives the folded tables for the tail loop.
 cudaError_t chee_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
                                  int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches) {
-    const uint32_t nruns = cd_pick_runs(nbytes, num_sms);
-    CheeDecLayout L; cd_layout(nbytes, cap, nruns, &L);
-    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(d_in, nbytes, cap, ws, L.B, stream, launches);
+    const CheeDecPtrs p(nbytes, cap, num_sms, ws, tables, tail_ws);
+    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(d_in, nbytes, cap, ws, p.B, stream, launches);
+    if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e != cudaSuccess) return e;
-    const DecStatus* st = reinterpret_cast<const DecStatus*>(ws + L.B.status);
-    ClStatus* cs = reinterpret_cast<ClStatus*>(ws + L.cs);
-    const uint64_t* blk_off = reinterpret_cast<const uint64_t*>(ws + L.B.blk_off);
-    uint4* flags = reinterpret_cast<uint4*>(ws + L.flags);
-    uint16_t* K = reinterpret_cast<uint16_t*>(ws + L.K);
-    uint2* usym = reinterpret_cast<uint2*>(ws + L.usym);
-    uint32_t* ctx_in = reinterpret_cast<uint32_t*>(ws + L.ctx_in);
-    uint32_t* ctx_out = reinterpret_cast<uint32_t*>(ws + L.ctx_out);
-    uint2* cin = reinterpret_cast<uint2*>(ws + L.cin);
-    uint32_t* snap = reinterpret_cast<uint32_t*>(ws + L.snap0);
-    uint32_t* dirty_cur = reinterpret_cast<uint32_t*>(ws + L.dirty);
-    uint32_t* dirty_next = dirty_cur + nruns;
-    uint32_t* run_epoch = reinterpret_cast<uint32_t*>(ws + L.run_epoch);
-    uint32_t* rbits = reinterpret_cast<uint32_t*>(ws + L.rbits);
-    uint4* entC = reinterpret_cast<uint4*>(tables);
-    uint2* entP = reinterpret_cast<uint2*>(tables + (size_t)nruns * 65536 * sizeof(uint4));
     uint32_t* out32 = reinterpret_cast<uint32_t*>(d_out);
-    // scalar_codec.cu workspace: Status (256 B) + chunk_a + chunk_b + pred
-    uint32_t* chunk_a = reinterpret_cast<uint32_t*>(tail_ws + 256);
-    uint32_t* chunk_b = chunk_a + 65536;
-    uint32_t* pred_final = chunk_a + 2 * 65536;
-    e = cudaMemsetAsync(tables, 0, chee_decode_tables_bytes(nbytes, num_sms), stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(snap, 0, (size_t)nruns * 65536 * sizeof(uint32_t), stream);   // run 0's snapshot: the zero table
-    if (e != cudaSuccess) return e;
-    const int wide = num_sms * 8;
-    const uint32_t run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
-    cd_unpack<<<wide, 256, 0, stream>>>(d_in, blk_off, st, flags, K, out32);
-    cd_cmap_walk<<<run_ctas, RP_WARPS * 32, 0, stream>>>(st, nruns, flags, K, entC, out32, usym);
-    cd_cmap_fold<<<65536 / 128, 128, 0, stream>>>(st, nruns, entC, cin, chunk_a, chunk_b, nullptr);
-    cd_cmap_resolve<<<wide, 256, 0, stream>>>(st, nruns, usym, K, cin, out32);
-    cd_ctx_init<<<(nruns + 127) / 128, 128, 0, stream>>>(st, nruns, flags, K, ctx_in, dirty_cur, dirty_next, run_epoch, cs);
-    *launches += 5;
-    for (int round = 0; round < MAX_ROUNDS; ++round) {
-        cd_pred_walk<<<run_ctas, RP_WARPS * 32, 0, stream>>>(st, cs, nruns, (uint32_t)round, flags, K, entP, snap, ctx_in, ctx_out, dirty_cur, dirty_next, run_epoch, rbits, out32, 1u);
-        cd_pred_fold<<<65536 / 128, 128, 0, stream>>>(st, cs, nruns, (uint32_t)round, entP, snap, run_epoch, rbits, dirty_next, pred_final, nullptr);
-        cd_round_end<<<1, 32, 0, stream>>>(cs, nruns, (uint32_t)round, ctx_in, ctx_out, dirty_cur, dirty_next);
-        *launches += 3;
+    cd_launch_unpack_walk(p, d_in, out32, stream, launches);
+    cd_launch_cmap_resolve(p, out32, nullptr, stream, launches);
+    for (uint32_t round = 0; round < (uint32_t)MAX_ROUNDS; ++round) {
+        cd_launch_pred_walk(p, round, out32, 1u, stream, launches);
+        cd_launch_pred_fold(p, round, nullptr, stream, launches);
+        cd_round_end<<<1, 32, 0, stream>>>(p.cs, p.nruns, round, p.ctx_in, p.ctx_out, p.dirty_cur, p.dirty_next);
+        ++*launches;
     }
-    cd_finish<<<1, 1, 0, stream>>>(st, cs, d_fallback, d_out_size);
-    ++*launches;
+    cd_launch_finish(p, d_fallback, d_out_size, stream, launches);
     return cudaGetLastError();
 }
 
 // device addresses the tail kernel needs (scalar_codec.cu): boundary status + iteration status
 const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** cl_status) {
-    CheeDecLayout L; cd_layout(nbytes, cap, cd_pick_runs(nbytes, num_sms), &L);
-    if (cl_status) *cl_status = ws + L.cs;
-    return ws + L.B.status;
+    const CheeDecPtrs p(nbytes, cap, num_sms, ws, nullptr, nullptr);
+    if (cl_status) *cl_status = p.cs;
+    return p.st;
 }
 
 // ---- sharded decode: one piece, in phases around the exchanges (include/density_b200.h, DESIGN.md section 5) --------------------------
-// Workspace: the layout of the single-device decoder, then the fallback word and the PieceStatus (256 B), then the tail's tables
-// (the scalar_codec.cu layout: Status (256 B) + chunk_a + chunk_b + pred).
-struct CheeShardPtrs {
-    uint32_t nruns, run_ctas;
-    DecStatus* st; ClStatus* cs; uint64_t* blk_off; uint4* flags; uint16_t* K; uint2* usym;
-    uint32_t *ctx_in, *ctx_out, *dirty_cur, *dirty_next, *run_epoch, *rbits, *snap, *fallback, *chunk_a, *chunk_b, *pred_final;
-    uint2* cin; uint4* entC; uint2* entP; PieceStatus* pst; uint8_t* tail_ws;
-};
-static size_t chee_shard_layout(const CheeShardArgs& a, CheeDecLayout* L) {
-    const size_t off = (cd_layout(a.n, a.cap, cd_pick_runs(a.n, a.num_sms), L) + 255) & ~(size_t)255;
-    return off + 256 + scalar_workspace_bytes(ALG_CHEETAH);
-}
-static CheeShardPtrs chee_shard_ptrs(const CheeShardArgs& a) {
-    CheeShardPtrs p;
-    CheeDecLayout L;
-    chee_shard_layout(a, &L);
-    uint8_t* ws = a.ws;
-    const size_t off = (L.total + 255) & ~(size_t)255;
-    p.nruns = cd_pick_runs(a.n, a.num_sms);
-    p.run_ctas = (p.nruns + RP_WARPS - 1) / RP_WARPS;
-    p.st = reinterpret_cast<DecStatus*>(ws + L.B.status);
-    p.cs = reinterpret_cast<ClStatus*>(ws + L.cs);
-    p.blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
-    p.flags = reinterpret_cast<uint4*>(ws + L.flags);
-    p.K = reinterpret_cast<uint16_t*>(ws + L.K);
-    p.usym = reinterpret_cast<uint2*>(ws + L.usym);
-    p.ctx_in = reinterpret_cast<uint32_t*>(ws + L.ctx_in);
-    p.ctx_out = reinterpret_cast<uint32_t*>(ws + L.ctx_out);
-    p.dirty_cur = reinterpret_cast<uint32_t*>(ws + L.dirty);
-    p.dirty_next = p.dirty_cur + p.nruns;
-    p.run_epoch = reinterpret_cast<uint32_t*>(ws + L.run_epoch);
-    p.rbits = reinterpret_cast<uint32_t*>(ws + L.rbits);
-    p.cin = reinterpret_cast<uint2*>(ws + L.cin);
-    p.snap = reinterpret_cast<uint32_t*>(ws + L.snap0);
-    p.fallback = reinterpret_cast<uint32_t*>(ws + off);
-    p.pst = reinterpret_cast<PieceStatus*>(ws + off + 128);
-    p.tail_ws = ws + off + 256;
-    p.chunk_a = reinterpret_cast<uint32_t*>(p.tail_ws + 256);
-    p.chunk_b = p.chunk_a + PL;
-    p.pred_final = p.chunk_a + 2 * PL;
-    p.entC = reinterpret_cast<uint4*>(a.tables);
-    p.entP = reinterpret_cast<uint2*>(a.tables + (size_t)p.nruns * PL * sizeof(uint4));
-    return p;
-}
+static CheeDecPtrs chee_shard_ptrs(const CheeShardArgs& a) { return CheeDecPtrs(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr); }
 
 size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
-    CheeShardArgs a{}; a.n = n; a.cap = cap; a.num_sms = num_sms;
     CheeDecLayout L;
-    return chee_shard_layout(a, &L);
+    const size_t off = (cd_layout(n, cap, cd_pick_runs(n, num_sms), &L) + 255) & ~(size_t)255;
+    return off + 256 + scalar_workspace_bytes(ALG_CHEETAH);
 }
 
 // Phase 1: boundaries (piece 0 may use copy mode: dec_seq_walk from the fresh automaton), the end of the piece, unpack (literals and
 // copy-mode blocks go straight to d_out), the symbolic chunk-map walk and the piece's chunk-map transfer (d_cmap_out, may be null).
 cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches) {
-    const CheeShardPtrs p = chee_shard_ptrs(a);
-    CheeDecLayout L; chee_shard_layout(a, &L);
-    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, L.B, stream, launches);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.tables, 0, chee_decode_tables_bytes(a.n, a.num_sms), stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(p.snap, 0, (size_t)p.nruns * PL * sizeof(uint32_t), stream);
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches);
+    if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
     if (e != cudaSuccess) return e;
-    const int wide = a.num_sms * 8;
-    uint32_t* out32 = reinterpret_cast<uint32_t*>(a.d_out);
-    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, p.st, p.blk_off, L.B.maxblocks, p.pst);
-    cd_unpack<<<wide, 256, 0, stream>>>(a.d_in, p.blk_off, p.st, p.flags, p.K, out32);
-    cd_cmap_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.entC, out32, p.usym);
-    *launches += 3;
+    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
+    ++*launches;
+    cd_launch_unpack_walk(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
     if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
     return cudaGetLastError();
 }
@@ -748,23 +748,17 @@ cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cuda
 // Phase 2: the chunk map carried in (d_cmap_carry: concrete, the left fold of the earlier pieces' transfers over cd_cmap_init_k's state;
 // nullptr = the stream start), the reads of carried-in slots, the context init.
 cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
-    const CheeShardPtrs p = chee_shard_ptrs(a);
-    uint32_t* out32 = reinterpret_cast<uint32_t*>(a.d_out);
-    cd_cmap_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.nruns, p.entC, p.cin, p.chunk_a, p.chunk_b, d_cmap_carry);
-    cd_cmap_resolve<<<a.num_sms * 8, 256, 0, stream>>>(p.st, p.nruns, p.usym, p.K, p.cin, out32);
-    cd_ctx_init<<<(p.nruns + 127) / 128, 128, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.ctx_in, p.dirty_cur, p.dirty_next, p.run_epoch, p.cs);
-    *launches += 3;
+    cd_launch_cmap_resolve(chee_shard_ptrs(a), reinterpret_cast<uint32_t*>(a.d_out), d_cmap_carry, stream, launches);
     return cudaGetLastError();
 }
 
 // A prediction round, first half: walk the dirty runs, export this round's transfer (d_pred_out, may be null) and the 4 round words.
 cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
-    const CheeShardPtrs p = chee_shard_ptrs(a);
-    cd_pred_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.cs, p.nruns, round, p.flags, p.K, p.entP, p.snap, p.ctx_in, p.ctx_out, p.dirty_cur,
-                                                           p.dirty_next, p.run_epoch, p.rbits, reinterpret_cast<uint32_t*>(a.d_out), a.first ? 1u : 0u);
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    cd_launch_pred_walk(p, round, reinterpret_cast<uint32_t*>(a.d_out), a.first ? 1u : 0u, stream, launches);
     if (d_pred_out) { cd_pred_export<<<PL / 128, 128, 0, stream>>>(p.cs, p.nruns, p.entP, p.run_epoch, d_pred_out); ++*launches; }
     cd_round_words<<<1, 256, 0, stream>>>(p.st, p.cs, p.nruns, p.ctx_out, p.dirty_cur, p.dirty_next, d_words);
-    *launches += 2;
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -772,19 +766,18 @@ cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32
 // context sweep from the gathered round words of all `world` pieces.
 cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
                                   uint32_t rank, cudaStream_t stream, uint64_t* launches) {
-    const CheeShardPtrs p = chee_shard_ptrs(a);
-    cd_pred_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.cs, p.nruns, round, p.entP, p.snap, p.run_epoch, p.rbits, p.dirty_next, p.pred_final, d_pred_carry);
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    cd_launch_pred_fold(p, round, d_pred_carry, stream, launches);
     cd_shard_round_end<<<1, 32, 0, stream>>>(p.cs, p.nruns, round, a.first ? 1u : 0u, rank, world, d_all_words, p.ctx_in, p.ctx_out, p.dirty_cur, p.dirty_next);
-    *launches += 2;
+    ++*launches;
     return cudaGetLastError();
 }
 
 // Phase 3: the verdict of the rounds, the final piece's tail from the folded tables (the tail of a non-final piece is empty), the size
 // and the seam words.
 cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
-    const CheeShardPtrs p = chee_shard_ptrs(a);
-    cd_finish<<<1, 1, 0, stream>>>(p.st, p.cs, p.fallback, d_out_size);
-    ++*launches;
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
     cudaError_t e = scalar_decode_tail(ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
     if (e != cudaSuccess) return e;
     cd_seam_words<<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_out_size, d_seam8);

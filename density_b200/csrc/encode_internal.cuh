@@ -6,6 +6,7 @@
 
 namespace dns {
 
+// chameleon_encode.cu
 // byte offsets of the Chameleon encode scratch arrays inside one workspace allocation
 struct ChamLayout {
     size_t status, sigw, copymap, copymap2, seg_state, incb, tile_bytes, tile_local, group_total, group_off, unres, unres_count, final_tab, carry, total;
@@ -17,10 +18,10 @@ cudaError_t cham_encode_phase1(const uint8_t* d_in, size_t nbytes, uint8_t* ws, 
                                uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev = nullptr);
 cudaError_t cham_encode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns,
                                const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                               bool allow_protected_fallback, bool assume_prev_inc, cudaStream_t stream, uint64_t* launches,
+                               bool allow_protected_fallback, bool assume_prev_inc, int num_sms, cudaStream_t stream, uint64_t* launches,
                                cudaEvent_t* ev = nullptr);
 cudaError_t cham_encode_phase2_blocking(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, uint8_t* d_out,
-                                        size_t cap, uint64_t* d_out_size, int max_batches, cudaStream_t stream, uint64_t* launches);
+                                        size_t cap, uint64_t* d_out_size, int max_batches, int num_sms, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_encode_protected_only(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint8_t* d_out,
                                        size_t cap, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches);
 
@@ -30,18 +31,51 @@ cudaError_t cham_encode_protected_only(const uint8_t* d_in, size_t nbytes, uint8
 cudaError_t cham_quads_to_table(const uint32_t* d_quads, uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_table_into_quads(const uint32_t* d_table, uint32_t* d_quads, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_encode_phase2_stream(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in,
-                                      uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_table_out, int max_batches, cudaStream_t stream,
-                                      uint64_t* launches, bool* ok);
+                                      uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_table_out, int max_batches, int num_sms,
+                                      cudaStream_t stream, uint64_t* launches, bool* ok);
+
+// table helpers (sharded API, pipelined host path)
+cudaError_t cham_status_accumulate(const uint8_t* ws, const ChamLayout& L, uint32_t* d_flag, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_table_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_seam_words(const uint8_t* ws, const ChamLayout& L, size_t nbytes, const uint64_t* d_out_size, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_seam_verdict(const uint32_t* d_all_words, uint32_t world, uint32_t rank, uint32_t* d_flags, uint64_t* d_total, uint64_t* d_offsets,
+                              cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_table_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 
 // shared pieces of the encoders (chameleon_encode.cu)
 struct Status;
-size_t prot_state_bytes(uint64_t nseg_max);
-cudaError_t prot_debug_read(unsigned long long* out32);   // diagnostics: per fixed-point round {first changed block, changed blocks}   // segment states + candidate tables of prot_iterate for up to nseg_max segments of 256 blocks
+size_t prot_state_bytes(uint64_t nseg_max);   // segment states + candidate tables of prot_iterate for up to nseg_max segments of 256 blocks
+cudaError_t prot_debug_read(unsigned long long* out32);   // diagnostics: per fixed-point round {first changed block, changed blocks}
 cudaError_t prot_iterate_launch(const uint32_t* sigw_or_null, uint64_t nbytes, uint64_t nblocks, uint32_t nseg, Status* st, int it, uint8_t* inc,
-                                uint8_t* cm_old, uint8_t* cm_new, uint32_t* in_state, uint32_t* out_state, int block_bytes, int num_sms,
-                                cudaStream_t stream);
+                                uint8_t* cm_old, uint8_t* cm_new, uint32_t* in_state, uint32_t* out_state, int num_sms, cudaStream_t stream);
 cudaError_t scan_tiles_launch(const uint32_t* tile_bytes, uint32_t ntiles, uint32_t* tile_local, uint64_t* group_total, uint64_t* group_off,
                               uint32_t ngroups, Status* st, uint64_t cap, uint64_t* d_out_size, cudaStream_t stream);
+
+// sharded copy-map iteration (density_b200_shard_prot_*): one shard of a longer stream. The shard's record lives in device memory.
+struct ProtShard {
+    unsigned long long first_block;   // global index of the shard's first block
+    uint32_t rounds;                  // rounds run until the map settled (0: not settled)
+    uint32_t settled, in_state, esc;  // in_state: pc_encode candidate of the true incoming state of the last round (0xFFFF: PC_ESC)
+    uint32_t changed[16];             // blocks of this shard whose copy status changed, per round
+};
+constexpr uint32_t PROT_TRANSFER_WORDS = 200, PROT_ROUND_WORDS = 4, PROT_MAX_ROUNDS = 16;
+// start: after cham_encode_phase1 (round 0's flags); first_block, or the sum of lengths[0 .. rank) / 256 when d_lengths is set
+cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
+                            cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t* launches);   // *d = v in stream order
+// round `it`: resolve the flags against the carry-in (NULL = stream start), export the transfer (PROT_TRANSFER_WORDS u32)
+cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
+                               int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches);
+// compose the gathered transfers of the shards before `rank`, walk, compare: PROT_ROUND_WORDS u32 to d_words
+cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
+                             uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+// the global commit of round `it` from the gathered round words; with d_table_out, round it + 1's flags under the new map and its table
+cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
+                           const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches);
+// sizes under the copy map, scan, emit, 8 seam words (word 2: refused or error); ev as cham_encode_phase2
+cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
+                             uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev = nullptr);
 
 // cheetah_encode.cu
 extern int g_chee_stage_rounds;
@@ -128,39 +162,5 @@ cudaError_t scalar_decode(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* 
 // runs only if *d_skip_if == 0
 cudaError_t scalar_decode_tail(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, const void* d_bounds_status,
                                const void* d_cl_status, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_skip_if);
-
-// table helpers (sharded API, pipelined host path)
-cudaError_t cham_status_accumulate(const uint8_t* ws, const ChamLayout& L, uint32_t* d_flag, cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_table_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_seam_words(const uint8_t* ws, const ChamLayout& L, size_t nbytes, const uint64_t* d_out_size, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_seam_verdict(const uint32_t* d_all_words, uint32_t world, uint32_t rank, uint32_t* d_flags, uint64_t* d_total, uint64_t* d_offsets,
-                              cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_table_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
-
-// sharded copy-map iteration (density_b200_shard_prot_*): one shard of a longer stream. The shard's record lives in device memory.
-struct ProtShard {
-    unsigned long long first_block;   // global index of the shard's first block
-    uint32_t rounds;                  // rounds run until the map settled (0: not settled)
-    uint32_t settled, in_state, esc;  // in_state: pc_encode candidate of the true incoming state of the last round (0xFFFF: PC_ESC)
-    uint32_t changed[16];             // blocks of this shard whose copy status changed, per round
-};
-constexpr uint32_t PROT_TRANSFER_WORDS = 200, PROT_ROUND_WORDS = 4, PROT_MAX_ROUNDS = 16;
-// start: after cham_encode_phase1 (round 0's flags); first_block, or the sum of lengths[0 .. rank) / 256 when d_lengths is set
-cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
-                            cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t* launches);   // *d = v in stream order
-// round `it`: resolve the flags against the carry-in (NULL = stream start), export the transfer (PROT_TRANSFER_WORDS u32)
-cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
-                               int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches);
-// compose the gathered transfers of the shards before `rank`, walk, compare: PROT_ROUND_WORDS u32 to d_words
-cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
-                             uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
-// the global commit of round `it` from the gathered round words; with d_table_out, round it + 1's flags under the new map and its table
-cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
-                           const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches);
-// sizes under the copy map, scan, emit, 8 seam words (word 2: refused or error); ev as cham_encode_phase2
-cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
-                             uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev = nullptr);
 
 }  // namespace dns

@@ -246,10 +246,11 @@ def test_chameleon_full_size_1gib_text_bit_exact(torch_cuda, codecs):
 
 
 def test_chameleon_beyond_4gib_prefix_and_round_trip(torch_cuda, codecs):
-    """5 GiB of text in one call (byte offsets past 2^32, the per-GPU shard scale of SURVEY.md §8d config 5). Size-independent checks:
-    the stream of a prefix is a prefix of the stream (codec.rs:72-80 walks the blocks in order; a 64 MiB prefix is compared with the
-    oracle), the stream decodes back to the input on the device, and the output size obeys codec.rs:18-21."""
+    """5 GiB of text in one call (byte offsets past 2^32, the per-GPU shard scale of SURVEY.md §8d config 5): the whole stream equals
+    the oracle's (compared on the device), the stream decodes back to the input on the device, and the output size obeys
+    codec.rs:18-21. The stream of text stays below 2^32 bytes; tests/test_gpu_beyond_4gib.py takes streams past it."""
     torch = torch_cuda
+    import big_streams
     import density_b200
     from density_b200 import synth
     C = codecs["chameleon"]
@@ -266,9 +267,12 @@ def test_chameleon_beyond_4gib_prefix_and_round_trip(torch_cuda, codecs):
     torch.cuda.synchronize()
     m = int(d_sz.item())
     assert 0 < m <= C.safe_encode_buffer_size(n)
-    npre = 64 << 20
-    want = oracle.encode("chameleon", d_in[:npre].cpu().numpy())
-    assert (d_out[:want.size].cpu().numpy() == want).all()
+    want, _ = big_streams.oracle_stream("chameleon", d_in.cpu().numpy())
+    assert m == want.size, (m, want.size)
+    d_want = torch.from_numpy(want).cuda()
+    off = big_streams.first_difference(d_out[:m], d_want)
+    assert off is None, f"first difference from the oracle's stream at byte {off}"
+    del d_want, want
     d_dec = torch.empty(n, dtype=torch.uint8, device="cuda")
     density_b200.decode_device("chameleon", d_out, m, d_dec, d_sz)
     torch.cuda.synchronize()

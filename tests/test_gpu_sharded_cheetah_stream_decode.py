@@ -438,6 +438,32 @@ def test_decode_sharded_cheetah_stream_rejects_bad_arguments(torch_cuda, lib):
     h.close()
 
 
+def test_output_offsets_beyond_4gib(torch_cuda, lib):
+    """The 7.5 GiB Cheetah pair corpus of tests/big_streams.py (a stream of more than 2**32 + 2**28 bytes, every block distinct) in two
+    ranges, the second starting past 2**32 bytes of stream: rank 1 locates its piece, carries the chunk map and the prediction rounds
+    across the cut and writes its output above 2**32, and the decoded bytes equal the input."""
+    import big_streams as bs
+    torch = torch_cuda
+    n = bs.SIZE["cheetah"]
+    if torch.cuda.mem_get_info()[0] < 24 * (1 << 30):
+        pytest.skip("needs 24 GiB of free device memory")
+    data = bs.corpus("cheetah", n)
+    stream, _ = bs.oracle_stream("cheetah", data)
+    m = stream.size
+    assert m > bs.STREAM_MIN
+    r0 = ((1 << 32) // RANGE + 1) * RANGE
+    lay = layout(m, [r0, m - r0])
+    got, (flags, total, offsets), canaries, located, status = decode_located(torch, lib, stream, lay, caps=[2 * (r + h) for _, r, h in lay])
+    del stream
+    assert flags == 0 and total == n and canaries
+    assert all(s[1] == 1 for s in status), status
+    assert int(offsets[1]) > (1 << 32) and int(offsets[1]) == 128 * located[1][2]
+    for r in range(2):
+        assert got[r].size == int(offsets[r + 1] - offsets[r])
+        off = bs.first_difference(got[r], data[int(offsets[r]):int(offsets[r + 1])])
+        assert off is None, f"rank {r}: first difference at output byte {int(offsets[r]) + off}"
+
+
 # ---- 6. two ranks over NCCL --------------------------------------------------------------------------------------------------------
 def _nccl_worker(rank, world, port, n, q):
     import os, sys

@@ -382,55 +382,28 @@ def test_decode_sharded_launch_count_unchanged(torch_cuda, lib):
 
 
 def test_output_offsets_beyond_4gib(torch_cuda, lib):
-    """About 4.5 GiB of zeros (about 2.4 GiB compressed) in two ranges: rank 1's output starts above 2**32."""
+    """The 5.5 GiB Chameleon pair corpus of tests/big_streams.py (a stream of more than 2**32 + 2**28 bytes, every block distinct) in
+    two ranges, the second starting past 2**32 bytes of stream: rank 1 locates its piece and writes its output above 2**32, and the
+    decoded bytes equal the input."""
+    import big_streams as bs
     torch = torch_cuda
-    from density_b200 import sharded
-    n = 4 * 1024 * MIB + 512 * MIB + 4
-    d_data = torch.zeros(n, dtype=torch.uint8, device="cuda")
-    cap_enc = lib.chameleon_safe_encode_buffer_size(n)
-    d_enc = torch.empty(cap_enc, dtype=torch.uint8, device="cuda")
-    sz = torch.zeros(1, dtype=torch.int64, device="cuda")
-    assert lib.density_b200_encode_device(0, d_data.data_ptr(), n, d_enc.data_ptr(), cap_enc, sz.data_ptr(), _stream(torch)) == 0
-    torch.cuda.synchronize()
-    del d_data
-    m = int(sz.item())
-    r0 = (m * 15 // 16) // CH * CH
+    n = bs.SIZE["chameleon"]
+    if torch.cuda.mem_get_info()[0] < 24 * (1 << 30):
+        pytest.skip("needs 24 GiB of free device memory")
+    data = bs.corpus("chameleon", n)
+    stream, _ = bs.oracle_stream("chameleon", data)
+    m = stream.size
+    assert m > bs.STREAM_MIN
+    r0 = ((1 << 32) // CH + 1) * CH
     lay = layout(m, [r0, m - r0])
-    decs = [sharded.ShardedChameleonDecoder() for _ in lay]
-    maps = []
-    for d, (o, nr, hl) in zip(decs, lay):
-        mm = torch.empty(266, dtype=torch.int64, device="cuda")
-        assert lib.density_b200_decode_locate(d._h, d_enc[o:].data_ptr(), nr, hl, mm.data_ptr(), _stream(torch)) == 0
-        maps.append(mm)
-    g = torch.stack(maps).cpu().numpy().view(np.uint64)
-    located = [sharded.locate_piece(g, r) for r in range(2)]
-    tables, outs, words, sizes = [], [], torch.zeros((2, 8), dtype=torch.int32, device="cuda"), []
-    for r, (o, nr, hl) in enumerate(lay):
-        start, end, _, fin = located[r]
-        piece = d_enc[o + start:o + end]
-        cap = 2 * (end - start)
-        out = torch.full((cap + 64,), CANARY, dtype=torch.uint8, device="cuda")
-        t = torch.empty(65536, dtype=torch.int32, device="cuda")
-        assert lib.density_b200_decode_shard_phase1(decs[r]._h, piece.data_ptr(), piece.numel(), cap, fin, t.data_ptr(), _stream(torch)) == 0
-        tables.append(t); outs.append((out, cap))
-    gt = torch.stack(tables)
-    for r in range(2):
-        carry = sharded.fold_tables(gt, r) if r else None
-        s_r = torch.zeros(1, dtype=torch.int64, device="cuda")
-        assert lib.density_b200_decode_shard_phase2(decs[r]._h, carry.data_ptr() if carry is not None else None, outs[r][0].data_ptr(),
-                                                    s_r.data_ptr(), words[r].data_ptr(), _stream(torch)) == 0
-        sizes.append(s_r)
-    torch.cuda.synchronize()
-    flags, total, offsets = sharded.seam_verdict(words)
-    assert flags == 0 and total == n
+    got, (flags, total, offsets), canaries, located = decode_located(torch, lib, stream, lay)
+    del stream
+    assert flags == 0 and total == n and canaries
     assert int(offsets[1]) > (1 << 32) and int(offsets[1]) == 256 * located[1][2]
     for r in range(2):
-        out, cap = outs[r]
-        k = int(sizes[r].item())
-        assert k == int(offsets[r + 1] - offsets[r])
-        assert int(torch.count_nonzero(out[:k])) == 0 and bool((out[cap:] == CANARY).all())
-    for d in decs:
-        d.close()
+        assert got[r].size == int(offsets[r + 1] - offsets[r])
+        off = bs.first_difference(got[r], data[int(offsets[r]):int(offsets[r + 1])])
+        assert off is None, f"rank {r}: first difference at output byte {int(offsets[r]) + off}"
 
 
 # ---- 8. two ranks over NCCL --------------------------------------------------------------------------------------------------------

@@ -45,6 +45,14 @@ _SIGS = {
     "density_b200_decode_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
                                                         ctypes.c_void_p]),
     "density_b200_decode_shard_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_u8p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_shard_prot_transfer": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int,
+                                                               ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_shard_prot_phase1": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                             ctypes.c_void_p]),
+    "density_b200_decode_shard_prot_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_u8p, ctypes.c_void_p, ctypes.c_void_p,
+                                                             ctypes.c_void_p]),
+    "density_b200_decode_sharded_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_decode_sharded": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
                                                    ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_decode_locate": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p]),

@@ -892,17 +892,20 @@ int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_
 // ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
 struct density_b200_decode_shard {
     DevBuf ws;
+    DevBuf seed;                    // the incoming automaton state of the prot_* phases (DECODE_PROT_SEED_WORDS)
     const uint8_t* d_in = nullptr;
     size_t n = 0, cap = 0;
     int is_last = 1;
     int num_sms = 0;
     bool phase1_done = false;
+    int prot_stage = 0;             // prot_*: 1 after the transfer, 2 after phase 1
 };
 
 density_b200_decode_shard* density_b200_decode_shard_create(void) { return new_shard<density_b200_decode_shard>(); }
 void density_b200_decode_shard_destroy(density_b200_decode_shard* s) {
     if (!s) return;
     s->ws.release();
+    s->seed.release();
     delete s;
 }
 int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
@@ -935,6 +938,58 @@ int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_
     if (e == cudaSuccess && s->n) e = cham_decode_seam_words(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, s->is_last, d_out_size, d_seam8, st, &launches);
     s->phase1_done = false;     // the decode pass overwrites the run tables: one phase 2 per phase 1
     return step_result(e, launches, "decode shard phase2");
+}
+
+// ---- the same for streams with copy-mode blocks: the piece's protection transfer first, then the two phases from the composed state -----
+int density_b200_decode_shard_prot_transfer(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                            uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_transfer_out)) { set_error("d_in must be 2-byte, d_transfer_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase1_done = false; s->prot_stage = 0;
+    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
+    if (e == cudaSuccess) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    uint64_t launches = 0;
+    e = cham_decode_prot_transfer(d_in, n, cap, s->ws.p, s->num_sms, is_last_shard, d_transfer_out, st, &launches);
+    const int rc = step_result(e, launches, "decode shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->prot_stage = 1;
+    return rc;
+}
+int density_b200_decode_shard_prot_phase1(density_b200_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
+                                          uint32_t* d_table_out, void* stream) {
+    g_last_error.clear();
+    if (!s || s->prot_stage != 1) { set_error("decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers) || !d_table_out) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_table_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    cudaError_t e = cham_decode_prot_enter(d_all_transfers, (uint32_t)rank, seed, st, &launches);
+    if (e == cudaSuccess) {
+        if (s->n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
+        else e = cham_decode_phase1(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, d_table_out, st, &launches, seed);
+    }
+    const int rc = step_result(e, launches, "decode shard prot phase1");
+    s->prot_stage = rc == DENSITY_B200_OK ? 2 : 0;
+    return rc;
+}
+int density_b200_decode_shard_prot_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
+                                          uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s || s->prot_stage != 2) { set_error("decode_shard_prot_phase2: null pointer / phase1 not done"); return DENSITY_B200_EARG; }
+    if ((!d_out && s->cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_out) & 3) { set_error("d_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    cudaError_t e = s->n ? cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches) : cudaSuccess;
+    if (e == cudaSuccess)
+        e = cham_decode_prot_seam_words(s->n, s->cap, s->ws.p, s->num_sms, s->is_last, reinterpret_cast<const uint32_t*>(s->seed.p), d_out_size, d_seam8,
+                                        st, &launches);
+    s->prot_stage = 0;          // one phase 2 per transfer
+    return step_result(e, launches, "decode shard prot phase2");
 }
 
 // ---- sharded Cheetah decode: one piece, its chunk map carried in and its prediction rounds run over all pieces ------------------------
@@ -1141,6 +1196,7 @@ struct density_b200_sharded {
     density_b200_shard* prot = nullptr;                  // density_b200_encode_sharded_protected
     density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion of density_b200_encode_sharded_cl
     density_b200_decode_shard* dec = nullptr;            // density_b200_decode_sharded[_stream]
+    density_b200_decode_shard* pdec = nullptr;           // density_b200_decode_sharded_protected
     density_b200_cheetah_decode_shard* cdec = nullptr;   // density_b200_decode_sharded_cheetah[_stream]
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     uint64_t* h_maps = nullptr;     // pinned, world range maps (the stream decodes)
@@ -1180,7 +1236,7 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
     }
     h->enc = density_b200_shard_create(); h->prot = density_b200_shard_create();
     h->cl[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->cl[1] = density_b200_cl_shard_create(ALG_LION);
-    h->dec = density_b200_decode_shard_create(); h->cdec = density_b200_cheetah_decode_shard_create();
+    h->dec = density_b200_decode_shard_create(); h->pdec = density_b200_decode_shard_create(); h->cdec = density_b200_cheetah_decode_shard_create();
     for (auto& e : h->ev) cudaEventCreate(&e);
     return h;
 }
@@ -1193,6 +1249,7 @@ void density_b200_sharded_destroy(density_b200_sharded* h) {
     density_b200_shard_destroy(h->prot);
     for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
     density_b200_decode_shard_destroy(h->dec);
+    density_b200_decode_shard_destroy(h->pdec);
     density_b200_cheetah_decode_shard_destroy(h->cdec);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     if (h->h_maps) cudaFreeHost(h->h_maps);
@@ -1483,6 +1540,29 @@ int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
     return decode_sharded_piece(x, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr);
+}
+
+// The inverse of density_b200_encode_sharded_protected (any stream): transfer -> transfers exchange -> phase 1 from the composed state ->
+// table exchange -> fold -> phase 2 -> seam words -> verdict. Everything is enqueued on `stream`; nothing blocks.
+int density_b200_decode_sharded_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                          uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, (size_t)h->world * DECODE_PROT_TRANSFER_WORDS * sizeof(uint32_t))) != DENSITY_B200_OK) return rc;
+    density_b200_decode_shard* s = h->pdec;
+    const size_t R = (size_t)h->rank;
+    uint32_t* transfers = reinterpret_cast<uint32_t*>(x.extra);       // [world][DECODE_PROT_TRANSFER_WORDS]
+    if ((rc = density_b200_decode_shard_prot_transfer(s, d_in, n, cap, h->rank == h->world - 1, transfers + R * DECODE_PROT_TRANSFER_WORDS, x.st))
+        != DENSITY_B200_OK) return rc;
+    if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+    if ((rc = density_b200_decode_shard_prot_phase1(s, transfers, h->world, h->rank, x.tables + R * 65536, x.st)) != DENSITY_B200_OK) return rc;
+    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, x.st, &launches);
+    if ((rc = step_result(e, launches, "sharded protected decode fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)) != DENSITY_B200_OK) return rc;
+    return x.verdict(d_flags, d_total_size, nullptr);
 }
 
 // the exchange buffers of decode_sharded_cheetah_piece: gathered chunk-map and prediction transfers, the carries, the round words

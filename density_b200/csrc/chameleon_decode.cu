@@ -416,16 +416,30 @@ __global__ void dec_carry_scan(const uint32_t* __restrict__ final_tab, uint32_t 
 }
 
 // ---- 4. tail loop (codec.rs:102-123), one thread, literal control flow ---------------------------------------------------
+// The automaton state behind the main loop: dec_seq_walk's, or (quiet: penalty 0 throughout) the entry state jumped over the main
+// blocks. Entry state: protection_state.rs:9-16, or the seed of a piece of a sharded stream.
+__device__ __forceinline__ Protection main_end_state(const DecStatus* __restrict__ st) {
+    Protection ps; ps.init();
+    if (st->seeded) { ps.copy_penalty = st->in_penalty; ps.copy_penalty_start = st->in_start; ps.previous_incompressible = st->in_prev; ps.counter = st->in_phase; }
+    if (st->seq) {
+        ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev;
+        ps.counter += st->main_blocks;
+    } else if (st->main_blocks) {
+        const uint64_t k = (ps.counter + st->main_blocks + 15) / 16 - (ps.counter + 15) / 16;
+        if (ps.copy_penalty_start > 1) { const uint32_t sh = k > 8 ? 8u : (uint32_t)k; const uint32_t v = ps.copy_penalty_start >> sh; ps.copy_penalty_start = v ? v : 1u; }
+        ps.counter += st->main_blocks;
+        ps.previous_incompressible = st->last_main_inc;
+    }
+    return ps;
+}
+
 __global__ void dec_tail(const uint8_t* __restrict__ in, uint64_t n, uint8_t* __restrict__ out, uint64_t cap, uint32_t* __restrict__ dict,
                          DecStatus* __restrict__ st, uint64_t* __restrict__ d_out_size) {
     if (threadIdx.x || blockIdx.x) return;
     if (st->nonquiet) { if (d_out_size) *d_out_size = 0; return; }   // gave up: the caller's in-order fallback (queued behind) produces the result
     if (st->error) { st->out_bytes = 0; if (d_out_size) *d_out_size = 0; return; }
     uint64_t idx = st->tail_off, oidx = st->main_blocks * 256;
-    Protection ps; ps.init();
-    ps.counter = st->main_blocks;             // quiet so far: penalty 0, start 1 (protection_state.rs:9-16,38-43)
-    ps.previous_incompressible = st->last_main_inc;
-    if (st->seq) { ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev; }
+    Protection ps = main_end_state(st);
     bool bad = false, overflow = false;
     auto emit = [&](uint32_t q) {
         if (oidx + 4 > cap) { overflow = true; return; }
@@ -497,10 +511,7 @@ template <class F>
 __device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
     TailWalk w; w.blocks = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
     Protection& ps = w.ps;
-    ps.init();
-    ps.counter = st->main_blocks;
-    ps.previous_incompressible = st->last_main_inc;
-    if (st->seq) { ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev; }
+    ps = main_end_state(st);
     uint64_t idx = st->tail_off;
     while (n - idx > 0) {
         ++w.blocks;
@@ -581,6 +592,34 @@ __global__ void dec_seam_words_k(const uint8_t* __restrict__ in, uint64_t n, con
     words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
 }
 
+// ---- 6. sharded decode of a stream with copy-mode blocks (density_b200_decode_shard_prot_*, DESIGN §5) ----------------------------------
+// The incoming state of piece `rank`: the transfers of the pieces before it (dec_prot_transfer) composed from candidate 0, the stream
+// start. A path that meets PT_ESC or PT_NOEND refuses the piece; the kernels then run from the stream-start state, harmlessly.
+__global__ void dec_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t* __restrict__ seed) {
+    if (threadIdx.x || blockIdx.x) return;
+    uint32_t x = 0;
+    for (uint32_t r = 0; r < rank && x < bounds::PT_NCAND; ++r) x = all_transfers[(size_t)r * bounds::PT_NCAND + x];
+    const uint32_t refused = x < bounds::PT_NCAND ? 0u : 1u;
+    const uint32_t s = bounds::pt_state(refused ? 0u : x);
+    seed[0] = s & 0xFFu; seed[1] = (s >> 8) & 0xFFu; seed[2] = (s >> 16) & 1u; seed[3] = s >> 17; seed[4] = refused;
+}
+// The seam words of such a piece, in the layout of dec_seam_words_k. Copy-mode blocks, a pending penalty and incompressible blocks meet
+// at the cuts legally here (the transfers carry the automaton across), so words 0 and 1 stay 0. Word 2: the transfers composed to no
+// state, an error (malformed, output beyond cap), or a non-final piece that does not decode to whole 256-byte blocks. st == nullptr:
+// an empty piece (no blocks, size 0), refused only by its seed.
+__global__ void dec_prot_seam_words_k(const DecStatus* __restrict__ st, const uint32_t* __restrict__ seed, int is_last,
+                                      uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
+    if (threadIdx.x || blockIdx.x) return;
+    uint64_t sz = 0;
+    uint32_t bad = seed[4];
+    if (st) {
+        sz = *d_out_size;
+        if (st->nonquiet || st->error || (!is_last && (sz % 256))) bad = 1;
+    } else *d_out_size = 0;
+    words[0] = 0; words[1] = 0; words[2] = bad; words[3] = st ? 1u : 0u;
+    words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
+}
+
 }  // namespace chamdec
 
 using namespace chamdec;
@@ -609,7 +648,7 @@ static uint32_t dec_pick_runs(const ChamDecLayout& L, int num_sms) {
 // Phase 1 of the parallel decode, which needs no carry-in: boundaries, then the writer pass (each run's last-writer table). With
 // d_table_out it also exports the piece's table (shard format) for the pieces after it.
 cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
-                               cudaStream_t stream, uint64_t* launches) {
+                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed) {
     static bool attr_done = false;
     if (!attr_done) {
         cudaError_t e0 = cudaFuncSetAttribute(cham_decode_pass7<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Dec7Smem));
@@ -620,7 +659,7 @@ cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, u
     ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
     DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.B.status);
     uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
-    cudaError_t e = bounds::bounds_launch<T>(d_in, nbytes, cap, ws, L.B, stream, launches);
+    cudaError_t e = bounds::bounds_launch<T>(d_in, nbytes, cap, ws, L.B, stream, launches, d_seed, d_seed != nullptr);
     if (e != cudaSuccess) return e;
     const uint32_t nruns = dec_pick_runs(L, num_sms);
     uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
@@ -660,6 +699,45 @@ cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t ca
     return cudaGetLastError();
 }
 
+// The protection transfer of a piece (PT_NCAND words to d_transfer): the candidate rows of the boundary walk, then the head walk over them.
+// The rows stay in the workspace for cham_decode_phase1 with a seed.
+cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
+                                      cudaStream_t stream, uint64_t* launches) {
+    static bool attr_done = false;
+    if (!attr_done) {
+        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                    (int)bounds::prot_transfer_smem<T>());
+        if (e0 != cudaSuccess) return e0;
+        attr_done = true;
+    }
+    ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
+    uint32_t* res = reinterpret_cast<uint32_t*>(ws + L.B.res);
+    uint4* gres = reinterpret_cast<uint4*>(ws + L.B.gres);
+    const uint32_t nchunks = (uint32_t)((nbytes + T::CH - 1) / T::CH);
+    const uint32_t ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
+    if (nchunks) {
+        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, nbytes, nchunks, res);
+        bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
+        *launches += 2;
+    }
+    bounds::dec_prot_transfer<T><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(d_in, nbytes, is_last, res, gres, d_transfer);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches) {
+    dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t cham_decode_prot_seam_words(size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint32_t* d_seed, uint64_t* d_out_size,
+                                        uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
+    const DecStatus* st = nullptr;
+    if (nbytes) { ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L); st = reinterpret_cast<const DecStatus*>(ws + L.B.status); }
+    dec_prot_seam_words_k<<<1, 32, 0, stream>>>(st, d_seed, is_last, d_out_size, d_words);
+    ++*launches;
+    return cudaGetLastError();
+}
+
 // The range map of d_in[0 .. n_range + n_halo) (sharded decode of a stream without known cuts): the candidate walks over the range's
 // chunks, with the halo visible to the walks of its last chunk, their composition per group, then over the whole range. The scratch is
 // the res / gres arrays of the boundary layout of n_range + n_halo bytes, where phase 1 puts them too.
@@ -686,7 +764,7 @@ cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
 // in-order kernel instead (copy-mode blocks present, or a pathological tile); d_out_size is only written when it is 0.
 cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms,
                                  uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches) {
-    cudaError_t e = cham_decode_phase1(d_in, nbytes, cap, ws, num_sms, nullptr, stream, launches);
+    cudaError_t e = cham_decode_phase1(d_in, nbytes, cap, ws, num_sms, nullptr, stream, launches, nullptr);
     if (e == cudaSuccess) e = cham_decode_phase2(d_in, nbytes, d_out, cap, ws, num_sms, nullptr, d_out_size, stream, launches);
     if (e != cudaSuccess) return e;
     ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);

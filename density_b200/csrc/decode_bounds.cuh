@@ -47,7 +47,13 @@ struct DecStatus {
     unsigned int nonquiet, error;        // nonquiet bit 0: copy-mode blocks present (cleared again by dec_seq_walk)
     unsigned int last_main_inc, seq;     // seq: the boundaries come from dec_seq_walk, automaton state below is valid
     unsigned int ps_penalty, ps_start, ps_prev, pad;   // protection state after the main loop (protection_state.rs:9-16)
+    // the state the piece of a sharded stream is entered in (seeded = 1; dec_quiet_check copies it from the seed): the main loop and the
+    // tail start from it instead of protection_state.rs:9-16. in_refused: the transfers composed to no state (the piece is refused)
+    unsigned int seeded, in_penalty, in_start, in_prev, in_phase, in_refused;
 };
+// the incoming state of a seeded boundary walk, as density_b200_decode_shard_prot_phase1 composes it: {penalty, start,
+// previous_incompressible, counter mod 16, refused}
+constexpr uint32_t SEED_WORDS = 5;
 
 __device__ __forceinline__ uint32_t ldu16(const uint8_t* p) { return *reinterpret_cast<const uint16_t*>(p); }
 __device__ __forceinline__ uint64_t ldsig(const uint8_t* p) {   // 8 bytes at a 2-byte aligned address
@@ -181,10 +187,17 @@ __global__ void dec_block_offsets(const uint8_t* __restrict__ in, uint64_t n, ui
 }
 
 // ---- 2. quiet check + capacity check -------------------------------------------------------------------------------------------
+// seed (may be null): the incoming state of a piece (SEED_WORDS); the quiet path also needs penalty 0 on entry and no incompressible pair
+// across the entry seam.
 template <class T>
-__global__ void dec_quiet_check(const uint8_t* __restrict__ in, const uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st, uint64_t cap) {
+__global__ void dec_quiet_check(const uint8_t* __restrict__ in, const uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st, uint64_t cap,
+                                const uint32_t* __restrict__ seed) {
     const uint64_t nb = st->main_blocks;
     const uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (seed && b == 0) {
+        st->seeded = 1; st->in_penalty = seed[0]; st->in_start = seed[1]; st->in_prev = seed[2]; st->in_phase = seed[3]; st->in_refused = seed[4];
+        if (seed[0] || (seed[2] && nb && T::consumed(ldsig(in)) >= T::BS)) atomicOr(&st->nonquiet, 1u);
+    }
     // DENSITY_B200_ECAPACITY — unless the count is void because copy-mode blocks were misread as signatures: every block in front of the
     // first copy-mode block is read correctly, and that includes the incompressible pair that started the episode, so the blocks that
     // fit (blk_off holds no more) are enough to find it; dec_seq_walk then recounts and judges the capacity again
@@ -234,6 +247,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
     const uint32_t tid = threadIdx.x;
     const bool al16 = (reinterpret_cast<uintptr_t>(in) & 15u) == 0;
     Protection ps; ps.init();
+    if (st->seeded) { ps.copy_penalty = st->in_penalty; ps.copy_penalty_start = st->in_start; ps.previous_incompressible = st->in_prev; ps.counter = st->in_phase; }
     uint64_t idx = 0, b = 0;        // meaningful in thread 0 only
     uint32_t g_next = 0;            // first group not entered yet (thread 0)
     uint32_t cb = 0, cb_valid = 0;  // staged rows: chunks [cb, cb + cb_valid)
@@ -402,6 +416,180 @@ __global__ void dec_start_row(const DecStatus* __restrict__ st, const uint64_t* 
     out4[0] = range_offset; out4[1] = st ? 1ull : 0ull; out4[2] = ex; out4[3] = nb;
 }
 
+// ---- 4. the protection transfer of a piece of a sharded stream (DESIGN §5) ----------------------------------------------------------
+// A piece starts at a block boundary, in an automaton state and counter phase (revert_to_copy halves the start on every 16th block of
+// the STREAM) that its decoder does not know. A decode candidate is (penalty 0..9, start 1..10, previous_incompressible, counter mod
+// 16): PT_NCAND of them, candidate 0 the stream start. dec_prot_transfer writes, for every candidate, where the boundary walk of
+// codec.rs:88-100, copy-mode blocks included, leaves a non-final piece: the candidate at its end when the walk ends exactly on the cut,
+// PT_ESC when that state is not a candidate, PT_NOEND when it overshoots the cut, stops short of it or reads a malformed block.
+// The walk follows HEADS keyed by (offset, state, phase), not candidates; heads that reach the same key merge for good, each candidate
+// keeps the index of its head. All heads advance chunk by chunk: a head with penalty 0 jumps its group or its chunk in O(1) from the
+// candidate rows (dec_seq_walk's rule), any other head walks the chunk block by block from shared memory, one thread per head. After a
+// chunk step the heads are merged in a shared hash table; at most PT_CAP stay live, the candidates of the others get PT_NOEND (their
+// piece is refused, never decoded wrong). tests/prot_decode_model.py is the CPU twin and measures the head counts.
+constexpr uint32_t PT_NCAND = 3200, PT_ESC = 0xFFFFu, PT_NOEND = 0xFFFEu, PT_CAP = 256, PT_HT = 8192, PT_THREADS = 1024;
+constexpr uint32_t PT_LIVE = 0xFFFFFFFFu, PT_DEAD = 0xFFFFu;
+__host__ __device__ __forceinline__ uint32_t pt_pack(uint32_t pen, uint32_t start, uint32_t prev, uint32_t phase) {
+    return pen | (start << 8) | (prev << 16) | (phase << 17);
+}
+__host__ __device__ __forceinline__ uint32_t pt_cand(uint32_t s) {     // packed state -> candidate, PT_ESC outside the set
+    const uint32_t pen = s & 0xFFu, start = (s >> 8) & 0xFFu, prev = (s >> 16) & 1u, phase = s >> 17;
+    if (pen >= 10u || start < 1u || start > 10u) return PT_ESC;
+    return phase * 200u + (prev * 10u + (start - 1u)) * 10u + pen;
+}
+__host__ __device__ __forceinline__ uint32_t pt_state(uint32_t c) {    // candidate -> packed state
+    const uint32_t pc = c % 200u;
+    return pt_pack(pc % 10u, (pc / 10u) % 10u + 1u, pc / 100u, c / 200u);
+}
+// nb encoded blocks with penalty 0 (sw_jump on a packed state)
+__device__ __forceinline__ uint32_t pt_jump(uint32_t s, uint32_t nb, uint32_t last_inc) {
+    uint32_t start = (s >> 8) & 0xFFu;
+    const uint32_t ph = s >> 17;
+    const uint32_t k = (ph + nb + 15) / 16 - (ph + 15) / 16;
+    if (start > 1) { start >>= (k > 8 ? 8u : k); if (!start) start = 1; }
+    return pt_pack(0, start, last_inc, (ph + nb) & 15u);
+}
+struct PtSmem {
+    unsigned long long off[2][PT_NCAND];    // head offsets in the piece, double-buffered across a merge
+    uint32_t st[2][PT_NCAND];               // packed head states
+    uint32_t end[PT_NCAND];                 // PT_LIVE, PT_LIVE - 1 (walks this chunk block by block), or the head's result
+    uint16_t newid[PT_NCAND];               // merge: the hash slot, then the head's index after the merge (PT_DEAD: dropped)
+    uint16_t cand_head[PT_NCAND];
+    unsigned long long ht_key[PT_HT];
+    uint16_t ht_val[PT_HT];
+    uint32_t nh, nnew, need_win, min_chunk;
+};
+template <class T>
+__global__ void __launch_bounds__(PT_THREADS, 1)
+dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const uint32_t* __restrict__ res, const uint4* __restrict__ gres,
+                  uint32_t* __restrict__ out) {
+    constexpr uint32_t SW_LOAD = T::CH + 16;
+    extern __shared__ __align__(16) unsigned char pt_raw[];
+    uint8_t* win = pt_raw;
+    PtSmem& S = *reinterpret_cast<PtSmem*>(pt_raw + SW_LOAD);
+    const uint32_t tid = threadIdx.x;
+    if (is_last || n == 0) {          // the last piece's transfer is never composed; an empty piece is the identity
+        for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) out[c] = is_last ? PT_NOEND : c;
+        return;
+    }
+    const bool al16 = (reinterpret_cast<uintptr_t>(in) & 15u) == 0;
+    const uint32_t nchunks = (uint32_t)((n + T::CH - 1) / T::CH);
+    for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) { S.off[0][c] = 0; S.st[0][c] = pt_state(c); S.cand_head[c] = (uint16_t)c; }
+    if (tid == 0) S.nh = PT_NCAND;
+    uint32_t cur = 0;
+    __syncthreads();
+    for (uint32_t c = 0; c < nchunks;) {
+        const uint32_t nh = S.nh;
+        const uint64_t cbase = (uint64_t)c * T::CH, cend = cbase + T::CH;
+        if (tid == 0) { S.need_win = 0; S.nnew = 0; S.min_chunk = 0xFFFFFFFFu; }
+        for (uint32_t i = tid; i < PT_HT; i += PT_THREADS) S.ht_key[i] = 0;
+        __syncthreads();
+        // 1. jumps from the group and chunk rows
+        for (uint32_t h = tid; h < nh; h += PT_THREADS) {
+            uint64_t off = S.off[cur][h];
+            uint32_t s = S.st[cur][h], e = PT_LIVE;
+            if (off < cend) {                                  // otherwise a group jump took it past this chunk
+                const uint32_t ent = (uint32_t)(off - cbase) >> 1, prev = (s >> 16) & 1u;
+                bool jumped = false;
+                if ((s & 0xFFu) == 0 && c % GROUP == 0) {
+                    const uint4 gr = gres[(size_t)(c / GROUP) * T::NCAND + ent];
+                    if (gr.x != TERM && !(gr.z & 9u) && !(prev && (gr.z & 2u))) {
+                        s = pt_jump(s, gr.y, (gr.z >> 2) & 1u); off = cbase + (uint64_t)GROUP * T::CH + 2 * gr.x; jumped = true;
+                    }
+                }
+                if (!jumped && (s & 0xFFu) == 0) {
+                    const uint32_t r = res[(size_t)c * T::NCAND + ent];
+                    const uint32_t ex = r & 0xFFu, fl = row_x<T>(r);
+                    if (ex != TERM && !(fl & 1u) && !(prev && (fl & 2u))) {
+                        s = pt_jump(s, row_nb<T>(r), (fl >> 2) & 1u); off = cend + 2 * ex; jumped = true;
+                    }
+                }
+                if (!jumped) { e = PT_LIVE - 1; S.need_win = 1; }
+                else if (off == n) e = pt_cand(s);
+            }
+            S.off[cur][h] = off; S.st[cur][h] = s; S.end[h] = e;
+        }
+        __syncthreads();
+        // 2. the heads that could not jump walk the chunk block by block
+        if (S.need_win) {
+            for (uint32_t i = tid * 16; i < SW_LOAD; i += PT_THREADS * 16) *reinterpret_cast<uint4*>(win + i) = sw_load16(in, cbase + i, n, al16);
+            __syncthreads();
+            for (uint32_t h = tid; h < nh; h += PT_THREADS) {
+                if (S.end[h] != PT_LIVE - 1) continue;
+                uint64_t off = S.off[cur][h];
+                uint32_t s = S.st[cur][h], e = PT_LIVE;
+                uint32_t pen = s & 0xFFu, start = (s >> 8) & 0xFFu, prev = (s >> 16) & 1u, ph = s >> 17;
+                const uint64_t stop = cend < n ? cend : n;
+                while (off < stop) {                           // codec.rs:88-98; every block of a non-final piece is a main-loop block
+                    if (ph == 0 && start > 1) start >>= 1;
+                    ph = (ph + 1) & 15u;
+                    if (pen) {
+                        pen = (pen - 1) & 0xFFu;
+                        if (!pen) start = (start + 1) & 0xFFu;
+                        off += T::BS;
+                    } else {
+                        if (off + T::SIG > n) { e = PT_NOEND; break; }
+                        const uint8_t* p = win + (uint32_t)(off - cbase);
+                        const uint32_t con = T::consumed(ldsig(p));
+                        if (con >= T::BS) { if (prev) pen = start; prev = 1; } else prev = 0;
+                        off += con;
+                    }
+                    if (off > n) { e = PT_NOEND; break; }
+                }
+                s = pt_pack(pen, start, prev, ph);
+                if (e == PT_LIVE && off == n) e = pt_cand(s);
+                S.off[cur][h] = off; S.st[cur][h] = s; S.end[h] = e;
+            }
+        }
+        __syncthreads();
+        // 3. merge: one head per key (offset, state, phase); the winners take the next indices, up to PT_CAP
+        for (uint32_t h = tid; h < nh; h += PT_THREADS) {
+            if (S.end[h] != PT_LIVE) continue;
+            const uint64_t off = S.off[cur][h];
+            const unsigned long long key = (((unsigned long long)(off - cend) << 21) | S.st[cur][h]) + 1ull;
+            uint32_t slot = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> 51) & (PT_HT - 1);
+            while (true) {
+                const unsigned long long was = atomicCAS(&S.ht_key[slot], 0ull, key);
+                if (was == 0ull) { S.ht_val[slot] = (uint16_t)atomicAdd(&S.nnew, 1u); atomicMin(&S.min_chunk, (uint32_t)(off / T::CH)); break; }
+                if (was == key) break;
+                slot = (slot + 1) & (PT_HT - 1);
+            }
+            S.newid[h] = (uint16_t)slot;
+        }
+        __syncthreads();
+        for (uint32_t h = tid; h < nh; h += PT_THREADS) {
+            if (S.end[h] != PT_LIVE) continue;
+            const uint32_t id = S.ht_val[S.newid[h]];
+            S.newid[h] = id < PT_CAP ? (uint16_t)id : (uint16_t)PT_DEAD;
+        }
+        __syncthreads();
+        // the winners move to the next buffer; every candidate follows its head, or takes its result
+        for (uint32_t h = tid; h < nh; h += PT_THREADS) {
+            if (S.end[h] != PT_LIVE) continue;
+            const uint32_t id = S.newid[h];
+            if (id != PT_DEAD) { S.off[cur ^ 1][id] = S.off[cur][h]; S.st[cur ^ 1][id] = S.st[cur][h]; }
+        }
+        for (uint32_t k = tid; k < PT_NCAND; k += PT_THREADS) {
+            const uint32_t h = S.cand_head[k];
+            if (h == PT_DEAD) continue;
+            const uint32_t e = S.end[h];
+            uint32_t nid = PT_DEAD;
+            if (e != PT_LIVE) out[k] = e;
+            else if ((nid = S.newid[h]) == PT_DEAD) out[k] = PT_NOEND;
+            S.cand_head[k] = (uint16_t)nid;
+        }
+        __syncthreads();
+        if (tid == 0) S.nh = S.nnew < PT_CAP ? S.nnew : PT_CAP;
+        cur ^= 1;
+        const uint32_t next = S.min_chunk;
+        __syncthreads();
+        if (S.nh == 0) break;
+        c = next > c + 1 ? next : c + 1;
+    }
+    for (uint32_t k = tid; k < PT_NCAND; k += PT_THREADS) if (S.cand_head[k] != PT_DEAD) out[k] = PT_NOEND;   // cannot happen: the piece ends
+}
+template <class T> constexpr size_t prot_transfer_smem() { return T::CH + 16 + sizeof(PtSmem); }
+
 // ---- host side: workspace layout + launch sequence ---------------------------------------------------------------------------------
 struct BoundsLayout { size_t status, res, gres, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, total; uint64_t maxblocks; };
 
@@ -427,8 +615,11 @@ inline size_t bounds_layout(size_t nbytes, size_t cap, BoundsLayout* L) {
 }
 
 // Enqueues the boundary kernels. Afterwards (on the stream): st->main_blocks / tail_off / protection state, blk_off[0 .. main_blocks).
+// d_seed (may be null): the incoming state of a piece of a sharded stream (SEED_WORDS, read on the device); rows_ready: dec_chunk_walk and
+// dec_group_compose already filled res / gres for this input (dec_prot_transfer needed them first).
 template <class T>
-inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, const BoundsLayout& L, cudaStream_t stream, uint64_t* launches) {
+inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, const BoundsLayout& L, cudaStream_t stream, uint64_t* launches,
+                                 const uint32_t* d_seed = nullptr, bool rows_ready = false) {
     DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.status);
     cudaError_t e = cudaMemsetAsync(st, 0, sizeof(DecStatus), stream);
     if (e != cudaSuccess) return e;
@@ -441,18 +632,21 @@ inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap,
     uint32_t* c_entry = reinterpret_cast<uint32_t*>(ws + L.c_entry);
     uint64_t* c_bb = reinterpret_cast<uint64_t*>(ws + L.c_blockbase);
     uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.blk_off);
-    dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, nbytes, nchunks, res);
-    dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
+    if (!rows_ready) {
+        dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, nbytes, nchunks, res);
+        dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
+        *launches += 2;
+    }
     dec_top_walk<T><<<1, 32, 0, stream>>>(gres, ngroups, nbytes, g_entry, g_bb, st);
     dec_chunk_entries<T><<<(ngroups + 127) / 128, 128, 0, stream>>>(res, nchunks, g_entry, g_bb, ngroups, c_entry, c_bb, nullptr);
     dec_block_offsets<T><<<(nchunks + 127) / 128, 128, 0, stream>>>(d_in, nbytes, nchunks, c_entry, c_bb, blk_off, L.maxblocks, nullptr);
-    dec_quiet_check<T><<<(unsigned)((L.maxblocks + 255) / 256), 256, 0, stream>>>(d_in, blk_off, L.maxblocks, st, cap);
+    dec_quiet_check<T><<<(unsigned)((L.maxblocks + 255) / 256), 256, 0, stream>>>(d_in, blk_off, L.maxblocks, st, cap, d_seed);
     // streams with copy-mode blocks only (the three kernels return at once otherwise): in-order walk, then the entries of the chunks of
     // jumped groups and the offsets of the blocks of jumped chunks
     dec_seq_walk<T><<<1, SW_THREADS, 0, stream>>>(d_in, nbytes, cap, nchunks, res, gres, ngroups, g_entry, g_bb, c_entry, c_bb, blk_off, L.maxblocks, st);
     dec_chunk_entries<T><<<(ngroups + 127) / 128, 128, 0, stream>>>(res, nchunks, g_entry, g_bb, ngroups, c_entry, c_bb, st);
     dec_block_offsets<T><<<(nchunks + 127) / 128, 128, 0, stream>>>(d_in, nbytes, nchunks, c_entry, c_bb, blk_off, L.maxblocks, st);
-    *launches += 9;
+    *launches += 7;
     return cudaGetLastError();
 }
 

@@ -110,12 +110,22 @@ cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
                                  uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches);
 // the same as two phases, for one piece of a sharded stream: phase 1 needs no carry-in and exports the piece's last-writer table
 // (shard format) when d_table_out is set; phase 2 decodes from d_carry_in (NULL: stream start); then the piece's 8 seam words
+// d_seed (may be NULL): the piece's incoming automaton state (cham_decode_prot_enter), after cham_decode_prot_transfer on the same workspace
 cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
-                               cudaStream_t stream, uint64_t* launches);
+                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr);
 cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms, const uint32_t* d_carry_in,
                                uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint64_t* d_out_size,
                                    uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+// a piece of a stream with copy-mode blocks: its protection transfer (DECODE_PROT_TRANSFER_WORDS, fills the candidate rows of the workspace
+// first), its incoming state composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), and its seam words after
+// cham_decode_phase1 with that seed and cham_decode_phase2 (nbytes 0: an empty piece, the workspace is not read)
+constexpr uint32_t DECODE_PROT_TRANSFER_WORDS = 3200, DECODE_PROT_SEED_WORDS = 5;
+cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
+                                      cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_prot_seam_words(size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint32_t* d_seed, uint64_t* d_out_size,
+                                        uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 // the range map of a piece of a stream without known cuts (DENSITY_B200_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`, at least
 // cham_locate_workspace_bytes(n_range + n_halo), which cham_decode_workspace_bytes of the same length covers
 size_t cham_locate_workspace_bytes(size_t nbytes);

@@ -15,7 +15,10 @@ automaton transfer (compose_prot_transfers is its numpy twin) and 4 round words,
 
 Decode is the mirror image: rank r decodes its piece back into its shard with the same table exchange and fold. The decode
 phase 1 (boundaries, writer pass) needs no carry-in and exports the piece's table; phase 2 decodes from the folded carry-in
-and writes 8 seam words, which every rank gathers and judges with `seam_verdict`.
+and writes 8 seam words, which every rank gathers and judges with `seam_verdict`. Pieces with copy-mode blocks decode through
+ShardedChameleonDecoder.decode_protected or ShardedDecoder.decode_protected: every piece first exports its protection transfer
+(where its boundary walk ends for every automaton state and counter phase it may be entered in; compose_decode_prot_transfers is
+the numpy twin of the composition), and phase 1 starts from the composed state.
 
 Cheetah and Lion shard the same way with three phases around two exchanges (ShardedCLEncoder): the last quad of every shard (the
 context of the next shard's first quad), then the shard's prediction transfer (P table), then its chunk-map transfer (C table). A
@@ -145,6 +148,31 @@ def compose_prot_transfers(transfers, rank):
     x = 0
     for r in range(rank):
         if x == PROT_ESC:
+            break
+        x = int(t[r, x])
+    return x
+
+
+DECODE_PROT_TRANSFER_WORDS = 3200   # DENSITY_B200_DECODE_PROT_TRANSFER_WORDS: (candidate state, counter mod 16) of a decode
+DECODE_PROT_NOEND = 0xFFFE          # a decode transfer entry whose boundary walk does not end on the cut
+
+
+def decode_prot_candidate(state, phase):
+    """(penalty, start, previous_incompressible), counter mod 16 -> the candidate index of a decode transfer entry, PROT_ESC outside
+    the set"""
+    c = prot_candidate(state)
+    return PROT_ESC if c == PROT_ESC else phase * PROT_TRANSFER_WORDS + c
+
+
+def compose_decode_prot_transfers(transfers, rank):
+    """The numpy twin of dec_prot_enter_k: the decode candidate entering piece `rank`, the transfers of pieces < rank (int [world,
+    DECODE_PROT_TRANSFER_WORDS], entry c = candidate at the piece end when entered in candidate c, PROT_ESC or DECODE_PROT_NOEND)
+    applied in order to the stream start (candidate 0). The first PROT_ESC / DECODE_PROT_NOEND met is returned: the pieces are
+    refused."""
+    t = np.asarray(transfers).astype(np.int64) & 0xFFFFFFFF
+    x = 0
+    for r in range(rank):
+        if x >= DECODE_PROT_TRANSFER_WORDS:
             break
         x = int(t[r, x])
     return x
@@ -383,6 +411,31 @@ class ShardedChameleonDecoder(_Handle):
         rank, world = _rank_world(group)
         return self._decode_piece(d_in, d_out, d_size, rank == world - 1, group)
 
+    def decode_protected(self, d_in, d_out, d_size, group=None):
+        """Decode of a piece of any stream, copy-mode blocks included (density_b200_decode_shard_prot_*): the arguments of decode. The
+        pieces' protection transfers are exchanged first, then the tables as in decode. Returns seam_verdict's (flags, total, offsets);
+        flags != 0: the pieces are void (a transfer path that does not end on a cut, a malformed piece, output beyond capacity)."""
+        rank, world = _rank_world(group)
+        stream = _stream()
+        dev = d_in.device
+        lib = self._lib
+        transfer = torch.empty(DECODE_PROT_TRANSFER_WORDS, dtype=torch.int32, device=dev)
+        _check(lib.density_b200_decode_shard_prot_transfer(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(rank == world - 1),
+                                                           transfer.data_ptr(), stream), "decode_shard_prot_transfer")
+        self._transfers = gather_rows(transfer, group).contiguous()
+        table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=dev)
+        _check(lib.density_b200_decode_shard_prot_phase1(self._h, self._transfers.data_ptr(), world, rank, table.data_ptr(), stream),
+               "decode_shard_prot_phase1")
+        gathered = gather_rows(table, group)
+        carry_ptr = None
+        if rank > 0:
+            self._carry = fold_tables(gathered, rank)
+            carry_ptr = self._carry.data_ptr()
+        words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
+        _check(lib.density_b200_decode_shard_prot_phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream),
+               "decode_shard_prot_phase2")
+        return seam_verdict(gather_rows(words, group))
+
     def decode_stream(self, d_in, n_range, d_out, d_size, group=None):
         """Decode of a stream without known cuts. d_in: CUDA uint8 tensor (2-byte aligned), this rank's range (its first n_range bytes)
         followed by its halo (stream_ranges gives the layout); d_out, d_size as in decode. Locates the piece (one host synchronisation
@@ -487,6 +540,13 @@ class ShardedDecoder(_ShardedHandle):
         fn = self._lib.density_b200_decode_sharded if alg == 0 else self._lib.density_b200_decode_sharded_cheetah
         _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
                   self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}")
+
+    def decode_protected(self, d_in, d_out, d_size, d_flags):
+        """density_b200_decode_sharded_protected: the Chameleon pieces of any stream, copy-mode blocks included (the inverse of
+        ShardedEncoder.encode_protected), with the arguments of decode. Enqueued on torch's current stream; nothing blocks."""
+        _check(self._lib.density_b200_decode_sharded_protected(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(),
+                                                               d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), _stream()),
+               "decode_sharded_protected")
 
     def decode_stream(self, d_in, n_range, d_out, d_size, d_flags, alg="chameleon", range_offset=None):
         """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range

@@ -303,6 +303,37 @@ DENSITY_B200_API int density_b200_decode_sharded(density_b200_sharded*, const ui
                                 uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
+ * Sharded Chameleon decode of streams with copy-mode blocks (DESIGN.md section 5): the inverse of density_b200_encode_sharded_protected,
+ * and of the slices of a single-call chameleon_encode stream at its pieces' prefix sums, whatever the data. A piece's block boundaries
+ * depend on the protection automaton state it is entered in and on the counter phase (the penalty start halves on every 16th block of
+ * the stream), so every piece first exports its TRANSFER: DENSITY_B200_DECODE_PROT_TRANSFER_WORDS u32, entry c for the decode candidate
+ * c = phase * 200 + (previous_incompressible * 10 + start - 1) * 10 + penalty (penalty 0..9, start 1..10, phase = blocks before the
+ * piece mod 16; candidate 0 is the stream start) = the candidate in which the boundary walk leaves the piece exactly on its end,
+ * 0xFFFF when that state is not a candidate, 0xFFFE when the walk does not end on the cut (overshoots it, stops short of it, a
+ * malformed block, or more distinct walks than the walk keeps). The final piece's transfer is never read (all 0xFFFE).
+ *   transfer  boundary rows of the piece and its transfer; cap = output capacity (as density_b200_decode_shard_phase1)
+ *   phase 1   the transfers of the pieces before `rank` (d_all_transfers: [world][DENSITY_B200_DECODE_PROT_TRANSFER_WORDS], may be NULL
+ *             for rank 0) composed from candidate 0 give the incoming state; boundaries from it, writer pass, and the piece's table
+ *             exported to d_table_out (copy-mode blocks do not enter it)
+ *   phase 2   as density_b200_decode_shard_phase2, seam words in its layout: words 0 and 1 are 0 (incompressible blocks may meet at a
+ *             cut), word 2 is set when the composition met 0xFFFF or 0xFFFE, the piece is malformed or its output exceeds cap, or a
+ *             non-final piece does not decode to whole 256-byte blocks.
+ * One transfer, phase 1 and phase 2 in this order per piece; otherwise DENSITY_B200_EARG. Nothing is written past cap.
+ */
+#define DENSITY_B200_DECODE_PROT_TRANSFER_WORDS 3200
+DENSITY_B200_API int density_b200_decode_shard_prot_transfer(density_b200_decode_shard*, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                            uint32_t* d_transfer_out, void* stream);
+DENSITY_B200_API int density_b200_decode_shard_prot_phase1(density_b200_decode_shard*, const uint32_t* d_all_transfers, int world, int rank,
+                                          uint32_t* d_table_out, void* stream);
+DENSITY_B200_API int density_b200_decode_shard_prot_phase2(density_b200_decode_shard*, const uint32_t* d_carry_in, uint8_t* d_out,
+                                          uint64_t* d_out_size, uint32_t* d_seam8, void* stream);
+/* End to end over NCCL, the arguments and semantics of density_b200_decode_sharded for any stream: transfer -> ncclAllGather(transfers,
+   12.5 KiB) -> phase 1 -> ncclAllGather(tables) -> fold kernel -> phase 2 -> ncclAllGather(seam words) -> seam verdict. Never blocks;
+   uses its own workspace in the handle. */
+DENSITY_B200_API int density_b200_decode_sharded_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                          uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
  * Sharded Cheetah decode (DESIGN.md section 5). Piece r is what rank r of a sharded Cheetah encode produced (density_b200_cl_shard_phase3
  * or density_b200_encode_sharded_cl), or equally the slice of a single-call cheetah_encode stream at the prefix sums of those sizes.
  * Decoding every piece gives back its shard byte for byte whenever the verdict is 0, so the concatenation equals cheetah_decode of the

@@ -71,7 +71,21 @@ _SIGS = {
     "density_b200_cl_table_fold": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_encode_sharded_cl": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
                                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, ctypes.c_void_p]),
-    "density_b200_cheetah_decode_shard_create": (ctypes.c_void_p, []),
+    "density_b200_cl_shard_prot_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_uint64, ctypes.c_int, ctypes.c_void_p,
+                                                         ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_p": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_c": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_transfer": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_settle": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                         ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_next": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_finish": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p,
+                                                         ctypes.c_void_p]),
+    "density_b200_cl_shard_prot_status": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32)]),
+    "density_b200_encode_sharded_cl_protected": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_u8p,
+                                                                ctypes.c_size_t, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_create":(ctypes.c_void_p, []),
     "density_b200_cheetah_decode_shard_destroy": (None, [ctypes.c_void_p]),
     "density_b200_cheetah_decode_round_budget": (ctypes.c_int, []),
     "density_b200_cheetah_cmap_words": (ctypes.c_size_t, []),

@@ -793,11 +793,17 @@ int density_b200_shard_prot_status(density_b200_shard* s, uint32_t* out) {
 struct density_b200_cl_shard {
     int alg = ALG_CHEETAH, num_sms = 0;
     DevBuf ws, tables[3];           // workspace; the epoch-tagged run tables (zero at allocation, one entry format each)
+    uint8_t* tables_p[3] = {};      // their pointers, as the kernels take them
     uint32_t epoch = 0, epoch_base = 0;
     const uint8_t* d_in = nullptr;
     size_t n = 0;
     bool first = true, is_last = true;
     int phase = 0;                  // the last phase done on the current shard
+    // the copy-map iteration of density_b200_cl_shard_prot_*: the shard's device record and where the phases stand
+    DevBuf prot;
+    uint64_t offset = 0;
+    int prot_phase = 0;             // 0 none, 1 ready for a round (phase 1 or a commit), 2 P, 3 C, 4 transfer, 5 settle, 6 finished
+    int round = 0;                  // rounds committed
 };
 
 static bool cl_alg_ok(int alg) { return alg == ALG_CHEETAH || alg == ALG_LION; }
@@ -811,6 +817,7 @@ density_b200_cl_shard* density_b200_cl_shard_create(int alg) {
 void density_b200_cl_shard_destroy(density_b200_cl_shard* s) {
     if (!s) return;
     s->ws.release(); for (auto& t : s->tables) t.release();
+    s->prot.release();
     delete s;
 }
 size_t density_b200_cl_table_words(int alg, int kind) {
@@ -826,6 +833,7 @@ int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, 
     if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_prev_quad) & 3)) { set_error("d_in and d_prev_quad must be 4-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase = 0;
+    s->prot_phase = 0;              // the workspace is this phase's now: the copy-map phases start over with prot_phase1
     cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
     for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
@@ -874,6 +882,139 @@ int density_b200_cl_shard_phase3(density_b200_cl_shard* s, const uint32_t* d_car
     if (rc == DENSITY_B200_OK) s->phase = 3;
     return rc;
 }
+// ---- sharded Cheetah / Lion encode with copy mode: the copy-map iteration carried over the cuts ------------------------------------------
+static ClProtShard cl_prot_args(density_b200_cl_shard* s) {
+    return ClProtShard{s->alg, s->d_in, s->n, s->offset, s->offset == 0 && s->n > 0, s->ws.p, s->tables_p, s->epoch_base, s->num_sms,
+                       reinterpret_cast<ProtShard*>(s->prot.p)};
+}
+// the phase functions below check the order: `want` is the prot_phase the call follows
+static bool cl_prot_order(density_b200_cl_shard* s, int want, const char* what) {
+    if (s && s->prot_phase == want) return true;
+    set_error(what);
+    return false;
+}
+
+int density_b200_cl_shard_prot_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, uint64_t offset, int is_last_shard,
+                                      uint32_t* d_words_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if (offset % 256) { set_error("offset must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if (!al4(d_in) || !al4(d_words_out)) { set_error("d_in and d_words_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase = 0; s->prot_phase = 0;
+    cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
+    for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
+    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    if (s->epoch > 0x0FFFFF00u) {                      // epochs exhausted: start over on cleared tables
+        for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = cudaMemsetAsync(s->tables[rg].p, 0, s->tables[rg].bytes, st);
+        if (e != cudaSuccess) { set_error("cudaMemsetAsync", e); return DENSITY_B200_ECUDA; }
+        s->epoch = 0;
+    }
+    s->epoch_base = s->epoch + 1; s->epoch += cl_prot_epochs();
+    s->d_in = d_in; s->n = n; s->offset = offset; s->is_last = is_last_shard != 0; s->round = 0;
+    for (int rg = 0; rg < 3; ++rg) s->tables_p[rg] = s->tables[rg].p;
+    uint64_t launches = 0;
+    e = cl_prot_phase1(cl_prot_args(s), d_words_out, st, &launches);
+    const int rc = step_result(e, launches, "cl shard prot phase1");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 1;
+    return rc;
+}
+int density_b200_cl_shard_prot_p(density_b200_cl_shard* s, const uint32_t* d_all_words, int world, int rank, uint32_t* d_table_p_out, void* stream) {
+    g_last_error.clear();
+    if (!d_all_words || !d_table_p_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_prot_order(s, 1, "cl_shard_prot_p: call it after prot_phase1 or prot_next")) return DENSITY_B200_EARG;
+    if (s->round >= g_prot_rounds) { set_error("cl_shard_prot_p: the round budget is used up"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_words) || !al4(d_table_p_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_p(cl_prot_args(s), s->round, d_all_words, (uint32_t)rank, d_table_p_out, reinterpret_cast<cudaStream_t>(stream),
+                                    &launches);
+    const int rc = step_result(e, launches, "cl shard prot p");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 2;
+    return rc;
+}
+int density_b200_cl_shard_prot_c(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream) {
+    g_last_error.clear();
+    if (!d_carry_p || !d_table_c_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_prot_order(s, 2, "cl_shard_prot_c: call it after prot_p")) return DENSITY_B200_EARG;
+    if (!al4(d_carry_p) || !al4(d_table_c_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_c(cl_prot_args(s), s->round, d_carry_p, d_table_c_out, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "cl shard prot c");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 3;
+    return rc;
+}
+int density_b200_cl_shard_prot_transfer(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    if (!d_carry_c || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_prot_order(s, 3, "cl_shard_prot_transfer: call it after prot_c")) return DENSITY_B200_EARG;
+    if (!al4(d_carry_c) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_transfer(cl_prot_args(s), s->round, d_carry_c, d_transfer_out, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "cl shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 4;
+    return rc;
+}
+int density_b200_cl_shard_prot_settle(density_b200_cl_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out,
+                                      void* stream) {
+    g_last_error.clear();
+    if (!d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_prot_order(s, 4, "cl_shard_prot_settle: call it after prot_transfer")) return DENSITY_B200_EARG;
+    if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_settle(cl_prot_args(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out,
+                                         reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "cl shard prot settle");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 5;
+    return rc;
+}
+int density_b200_cl_shard_prot_next(density_b200_cl_shard* s, const uint32_t* d_all_words, int world, void* stream) {
+    g_last_error.clear();
+    if (!d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!cl_prot_order(s, 5, "cl_shard_prot_next: call it after prot_settle")) return DENSITY_B200_EARG;
+    if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_words)) { set_error("words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_next(cl_prot_args(s), s->round, d_all_words, (uint32_t)world, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const int rc = step_result(e, launches, "cl shard prot next");
+    if (rc == DENSITY_B200_OK) { s->prot_phase = 1; ++s->round; }
+    return rc;
+}
+// ev_emit (may be NULL): recorded between the scan and the emit
+static int cl_prot_finish_impl(density_b200_cl_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st,
+                               cudaEvent_t ev_emit) {
+    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!s || s->prot_phase != 1 || s->round == 0) { set_error("cl_shard_prot_finish: call it after prot_next"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_out) & 1) || (reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) {
+        set_error("d_out must be 2-byte, d_out_size 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    uint64_t launches = 0;
+    const cudaError_t e = cl_prot_finish(cl_prot_args(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev_emit);
+    const int rc = step_result(e, launches, "cl shard prot finish");
+    if (rc == DENSITY_B200_OK) s->prot_phase = 6;
+    return rc;
+}
+int density_b200_cl_shard_prot_finish(density_b200_cl_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    return cl_prot_finish_impl(s, d_out, cap, d_out_size, d_seam8, reinterpret_cast<cudaStream_t>(stream), nullptr);
+}
+int density_b200_cl_shard_prot_status(density_b200_cl_shard* s, uint32_t* out) {
+    g_last_error.clear();
+    if (!s || !out || s->prot_phase < 1 || s->round == 0) { set_error("cl_shard_prot_status: null pointer / no round committed"); return DENSITY_B200_EARG; }
+    ProtShard h{};
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(&h, s->prot.p, sizeof h, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error("cl_shard_prot_status", e); return DENSITY_B200_ECUDA; }
+    out[0] = h.stage_ok; out[1] = h.rounds; out[3] = h.esc;
+    const uint32_t c = h.in_state;   // pc_encode candidate -> penalty | start << 8 | previous_incompressible << 16
+    out[2] = c >= PROT_TRANSFER_WORDS ? 0xFFFFFFFFu : (c % 10) | (((c / 10) % 10 + 1) << 8) | ((c / 100) << 16);
+    for (int k = 0; k < 16; ++k) out[4 + k] = h.changed[k];
+    return DENSITY_B200_OK;
+}
+
 int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* stream) {
     g_last_error.clear();
     if (!density_b200_cl_table_words(alg, kind) || !d_table) { set_error("cl_table_init: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
@@ -1195,6 +1336,7 @@ struct density_b200_sharded {
     density_b200_shard* enc = nullptr;                   // density_b200_encode_sharded
     density_b200_shard* prot = nullptr;                  // density_b200_encode_sharded_protected
     density_b200_cl_shard* cl[2] = {nullptr, nullptr};   // Cheetah / Lion of density_b200_encode_sharded_cl
+    density_b200_cl_shard* clp[2] = {nullptr, nullptr};  // Cheetah / Lion of density_b200_encode_sharded_cl_protected
     density_b200_decode_shard* dec = nullptr;            // density_b200_decode_sharded[_stream]
     density_b200_decode_shard* pdec = nullptr;           // density_b200_decode_sharded_protected
     density_b200_cheetah_decode_shard* cdec = nullptr;   // density_b200_decode_sharded_cheetah[_stream]
@@ -1236,6 +1378,7 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
     }
     h->enc = density_b200_shard_create(); h->prot = density_b200_shard_create();
     h->cl[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->cl[1] = density_b200_cl_shard_create(ALG_LION);
+    h->clp[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->clp[1] = density_b200_cl_shard_create(ALG_LION);
     h->dec = density_b200_decode_shard_create(); h->pdec = density_b200_decode_shard_create(); h->cdec = density_b200_cheetah_decode_shard_create();
     for (auto& e : h->ev) cudaEventCreate(&e);
     return h;
@@ -1248,6 +1391,7 @@ void density_b200_sharded_destroy(density_b200_sharded* h) {
     density_b200_shard_destroy(h->enc);
     density_b200_shard_destroy(h->prot);
     for (auto* s : h->cl) density_b200_cl_shard_destroy(s);
+    for (auto* s : h->clp) density_b200_cl_shard_destroy(s);
     density_b200_decode_shard_destroy(h->dec);
     density_b200_decode_shard_destroy(h->pdec);
     density_b200_cheetah_decode_shard_destroy(h->cdec);
@@ -1502,6 +1646,72 @@ int density_b200_encode_sharded_protected(density_b200_sharded* h, const uint8_t
     cudaEvent_t pev[4] = {nullptr, nullptr, h->ev[3], h->ev[4]};
     if ((rc = prot_finish_impl(s, d_out, cap, d_out_size, x.my_words(), st, n ? pev : nullptr)) != DENSITY_B200_OK) return rc;
     if (!n) { cudaEventRecord(h->ev[3], st); cudaEventRecord(h->ev[4], st); }
+    return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
+}
+
+// Sharded Cheetah / Lion encode with copy mode over the handle's communicator: the shard lengths (to the host: the shard at the stream start
+// runs the staged iteration) -> phase 1 -> its round words -> the round budget of {P tables -> fold -> C tables -> fold -> transfers ->
+// round words -> commit} -> finish -> seam words -> verdict -> optional gather. Every rank runs the same rounds, so the collectives match.
+int density_b200_encode_sharded_cl_protected(density_b200_sharded* h, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                             uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather,
+                                             size_t gather_cap, void* stream_v) {
+    g_last_error.clear();
+    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl_protected: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
+    // every argument the phases check is checked here, before the first collective (see density_b200_encode_sharded_protected)
+    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || (reinterpret_cast<uintptr_t>(d_total_size) & 7) || !al4(d_flags)) {
+        set_error("d_out_size and d_total_size must be 8-byte, d_flags 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    density_b200_cl_shard* s = h->clp[alg - ALG_CHEETAH];
+    const size_t W = (size_t)h->world, R = (size_t)h->rank;
+    const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
+    const size_t rw = CL_PROT_ROUND_WORDS;
+    Exchange x;
+    if ((rc = x.open(h, stream_v, W * sizeof(uint64_t) + ((W + 1) * (wp + wc) + W * (PROT_TRANSFER_WORDS + rw) + 64) * sizeof(uint32_t))) != DENSITY_B200_OK)
+        return rc;
+    cudaStream_t st = x.st;
+    uint64_t* lengths = reinterpret_cast<uint64_t*>(x.extra);            // [world]
+    uint32_t* tab_p = reinterpret_cast<uint32_t*>(lengths + W);          // [world][wp]
+    uint32_t* carry_p = tab_p + W * wp;
+    uint32_t* tab_c = carry_p + wp;                                       // [world][wc]
+    uint32_t* carry_c = tab_c + W * wc;
+    uint32_t* transfers = carry_c + wc;                                   // [world][PROT_TRANSFER_WORDS]
+    uint32_t* rwords = transfers + W * PROT_TRANSFER_WORDS;              // [world][CL_PROT_ROUND_WORDS]
+    uint64_t launches = 0;
+    cudaEventRecord(h->ev[0], st);
+    // the byte offset of my shard, on the host: whether this shard holds the stream start decides what phase 1 enqueues
+    cudaError_t e = cham_put_u64(lengths + R, (uint64_t)n, st, &launches);
+    if ((rc = step_result(e, launches, "sharded cl protected: length")) != DENSITY_B200_OK) return rc;
+    if (!x.gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
+    e = cudaMemcpyAsync(h->h_offsets, lengths, W * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if ((rc = step_result(e, 0, "sharded cl protected: lengths to host")) != DENSITY_B200_OK) return rc;
+    uint64_t offset = 0;
+    for (size_t r = 0; r < R; ++r) offset += h->h_offsets[r];
+    if ((rc = density_b200_cl_shard_prot_phase1(s, d_in, n, offset, R == W - 1, rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
+    if (!x.gather(rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+    cudaEventRecord(h->ev[1], st);
+    for (int k = 0; k < g_prot_rounds; ++k) {
+        if ((rc = density_b200_cl_shard_prot_p(s, rwords, (int)W, (int)R, tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
+        launches = 0;
+        e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
+        if ((rc = step_result(e, launches, "sharded cl protected: P fold")) != DENSITY_B200_OK) return rc;
+        if (k == 0) cudaEventRecord(h->ev[2], st);
+        if ((rc = density_b200_cl_shard_prot_c(s, carry_p, tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
+        launches = 0;
+        e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_C, tab_c, (uint32_t)R, carry_c, st, &launches);
+        if ((rc = step_result(e, launches, "sharded cl protected: C fold")) != DENSITY_B200_OK) return rc;
+        if ((rc = density_b200_cl_shard_prot_transfer(s, carry_c, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_cl_shard_prot_settle(s, transfers, (int)W, (int)R, rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_cl_shard_prot_next(s, rwords, (int)W, st)) != DENSITY_B200_OK) return rc;
+    }
+    if ((rc = cl_prot_finish_impl(s, d_out, cap, d_out_size, x.my_words(), st, h->ev[3])) != DENSITY_B200_OK) return rc;
+    cudaEventRecord(h->ev[4], st);
     return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
 }
 

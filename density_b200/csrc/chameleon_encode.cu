@@ -1168,16 +1168,19 @@ __global__ void cham_seam_verdict_k(const uint32_t* __restrict__ all_words, uint
 // {blocks whose copy status changed, met PC_ESC, the iteration had settled before this round, 0}. The verdict over all shards' words is
 // the same on every shard: settled when no block changed anywhere and no path met PC_ESC. ps->first_block makes `counter` global:
 // revert_to_copy halves the start on every 16th block of the STREAM, and shards start at any block.
+// The kernels serve every codec: Chameleon refreshes the incompressible bits from its signatures inside cham_prot_seg_k (sigw_g), Cheetah
+// and Lion pass sigw_g == nullptr with the bits already refreshed by their tile-size kernels; blocks are 256, 128 or 64 bytes.
 // ------------------------------------------------------------------------------------------------------
 constexpr uint32_t PROT_REFUSED = 16;   // Status::error of a shard whose iteration did not settle (or met PC_ESC): nothing is emitted
 
 __global__ void cham_put_u64_k(uint64_t* __restrict__ p, uint64_t v) { if (threadIdx.x == 0 && blockIdx.x == 0) *p = v; }
 __global__ void cham_prot_start_k(Status* __restrict__ st, ProtShard* __restrict__ ps, uint64_t first_block, const uint64_t* __restrict__ lengths,
-                                  uint32_t rank) {
+                                  uint32_t rank, uint32_t block_bytes) {
     if (threadIdx.x || blockIdx.x) return;
-    if (lengths) { uint64_t o = 0; for (uint32_t r = 0; r < rank; ++r) o += lengths[r]; first_block = o / 256; }
+    if (lengths) { uint64_t o = 0; for (uint32_t r = 0; r < rank; ++r) o += lengths[r]; first_block = o / block_bytes; }
     *ps = ProtShard{};
     ps->first_block = first_block;
+    ps->stage_ok = 1;
     st->nonquiet = 1;        // the copy map is always in force on this path: every round's kernels run until the global verdict closes them
     st->converged = 0;
 }
@@ -1197,7 +1200,7 @@ cham_prot_seg_k(const uint32_t* __restrict__ sigw_g, uint64_t nbytes, uint64_t n
     const uint32_t nb = (uint32_t)((nblocks - b0 < (uint64_t)PSEG) ? (nblocks - b0) : PSEG);
     if (tid < nb) {
         const uint64_t b = b0 + tid;
-        if (!(it && cm_old[b])) inc[b] = (nbytes - b * 256 >= 256) && (__popc(sigw_g[2 * b]) + __popc(sigw_g[2 * b + 1]) <= 4);
+        if (sigw_g && !(it && cm_old[b])) inc[b] = (nbytes - b * 256 >= 256) && (__popc(sigw_g[2 * b]) + __popc(sigw_g[2 * b + 1]) <= 4);
         s_inc[tid] = inc[b];
     }
     __syncthreads();
@@ -1276,7 +1279,9 @@ __global__ void cham_prot_seams_k(uint32_t nseg, const Status* __restrict__ st, 
     for (uint32_t s = g * PC_GROUP; s < s1; ++s) { in_state[s] = x; x = T[(size_t)s * PC_NC + x]; }
 }
 // settle, 3: every segment walked from its true incoming state writes the new copy map; the blocks whose status changed are counted
-__global__ void cham_prot_walk_k(uint64_t nblocks, uint32_t nseg, const Status* __restrict__ st, int it, const uint8_t* __restrict__ inc,
+// against the committed map, or in round 0 against the empty one unless `warm` (the map the round's flags were computed under is then
+// the committed one from the start)
+__global__ void cham_prot_walk_k(uint64_t nblocks, uint32_t nseg, const Status* __restrict__ st, int it, int warm, const uint8_t* __restrict__ inc,
                                  const uint8_t* __restrict__ cm_old, uint8_t* __restrict__ cm_new, const uint32_t* __restrict__ in_state,
                                  const uint32_t* __restrict__ gin, ProtShard* __restrict__ ps, uint32_t* __restrict__ words) {
     if (!gate_open(st)) return;
@@ -1288,38 +1293,41 @@ __global__ void cham_prot_walk_k(uint64_t nblocks, uint32_t nseg, const Status* 
     p.counter = ps->first_block + b0;
     prot_walk(p, inc, b0, b1, cm_new);
     uint32_t nd = 0;
-    for (uint64_t b = b0; b < b1; ++b) nd += cm_new[b] != (it ? cm_old[b] : 0);
+    for (uint64_t b = b0; b < b1; ++b) nd += cm_new[b] != ((it || warm) ? cm_old[b] : 0);
     if (nd) {
         atomicAdd(&words[0], nd);
         if (it < 16) atomicAdd(&ps->changed[it], nd);
     }
 }
 
-__device__ __forceinline__ void prot_round_verdict(const uint32_t* all_words, uint32_t world, bool& changed, bool& esc) {
+// all_words: [world][stride] round words, {changed, met PC_ESC, ...} at the front of every row
+__device__ __forceinline__ void prot_round_verdict(const uint32_t* all_words, uint32_t world, uint32_t stride, bool& changed, bool& esc) {
     changed = false; esc = false;
-    for (uint32_t r = 0; r < world; ++r) { changed |= all_words[4 * r] != 0; esc |= all_words[4 * r + 1] != 0; }
+    for (uint32_t r = 0; r < world; ++r) { changed |= all_words[stride * r] != 0; esc |= all_words[stride * r + 1] != 0; }
 }
 // the global commit of a round, 1: cm_old <- cm_new unless the map settled (as prot_iterate step 4; round 0 always commits)
-__global__ void cham_prot_commit_k(const uint32_t* __restrict__ all_words, uint32_t world, uint64_t nblocks, const Status* __restrict__ st, int it,
-                                   uint8_t* __restrict__ cm_old, const uint8_t* __restrict__ cm_new) {
+__global__ void cham_prot_commit_k(const uint32_t* __restrict__ all_words, uint32_t world, uint32_t stride, uint64_t nblocks, const Status* __restrict__ st,
+                                   int it, uint8_t* __restrict__ cm_old, const uint8_t* __restrict__ cm_new) {
     if (!gate_open(st)) return;
     bool changed, esc;
-    prot_round_verdict(all_words, world, changed, esc);
+    prot_round_verdict(all_words, world, stride, changed, esc);
     if (esc || !(changed || it == 0)) return;
     for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nblocks; b += (uint64_t)gridDim.x * blockDim.x) cm_old[b] = cm_new[b];
 }
 // 2: the verdict closes the gate of every later kernel when the map has settled, or when a path met PC_ESC (the shard is then refused)
-__global__ void cham_prot_verdict_k(const uint32_t* __restrict__ all_words, uint32_t world, Status* __restrict__ st, int it, ProtShard* __restrict__ ps) {
+__global__ void cham_prot_verdict_k(const uint32_t* __restrict__ all_words, uint32_t world, uint32_t stride, Status* __restrict__ st, int it,
+                                    ProtShard* __restrict__ ps) {
     if (threadIdx.x || blockIdx.x || !gate_open(st)) return;
     bool changed, esc;
-    prot_round_verdict(all_words, world, changed, esc);
+    prot_round_verdict(all_words, world, stride, changed, esc);
     if (esc) { ps->esc = 1; st->converged = 1; }
     else if (!changed) { ps->settled = 1; ps->rounds = (uint32_t)it + 1; st->converged = 1; }
 }
-// finish: a shard whose iteration did not settle is refused (nothing is emitted: cham_emit returns on an error)
+// finish: a shard whose iteration did not settle, or whose own staged iteration did not (Cheetah / Lion: the shard at the stream start), is
+// refused (nothing is emitted: the emit kernels return on an error)
 __global__ void cham_prot_finish_k(Status* __restrict__ st, const ProtShard* __restrict__ ps) {
     if (threadIdx.x || blockIdx.x) return;
-    if (!ps->settled) st->error = PROT_REFUSED;
+    if (!ps->settled || !ps->stage_ok) st->error = PROT_REFUSED;
 }
 // the seam words of the layout of cham_seam_words_k: incompressible blocks may meet at a cut here, so words 0 and 1 stay 0; word 2 = refused
 // or error (the size is then 0)
@@ -1683,10 +1691,71 @@ cudaError_t cham_encode_protected_only(const uint8_t* d_in, size_t nbytes, uint8
     return sizes_scan_emit(B, d_in, B.copymap, 0, false, d_out, cap, d_out_size, stream, launches, nullptr);
 }
 
-// ---- sharded copy-map iteration (see cham_prot_start_k) --------------------------------------------------------------------------------
+// ---- sharded copy-map iteration (see cham_prot_start_k): the launches every codec shares, then Chameleon's phases -----------------------
+ProtSegs prot_segs(Status* st, uint64_t nbytes, uint64_t nblocks, uint8_t* inc, uint8_t* cm, uint8_t* cm2, uint32_t* seg_state) {
+    ProtSegs P;
+    P.st = st; P.nbytes = nbytes; P.nblocks = nblocks; P.inc = inc; P.cm = cm; P.cm2 = cm2;
+    P.nseg = (uint32_t)((nblocks + PSEG - 1) / PSEG); P.ngrp = (P.nseg + PC_GROUP - 1) / PC_GROUP;
+    P.in_state = seg_state;
+    uint16_t* ptab = reinterpret_cast<uint16_t*>(seg_state + 2 * (P.nseg + 1));
+    P.gin = reinterpret_cast<uint32_t*>(ptab); P.T = ptab + 2 * (P.ngrp + 2); P.GT = P.T + (size_t)P.nseg * PC_NC;
+    return P;
+}
+cudaError_t prot_start(const ProtSegs& P, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank, uint32_t block_bytes,
+                       cudaStream_t stream, uint64_t* launches) {
+    cham_prot_start_k<<<1, 32, 0, stream>>>(P.st, ps, first_block, d_lengths, rank, block_bytes);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t prot_transfer(const ProtSegs& P, const uint32_t* sigw, const ProtShard* ps, int it, uint32_t* d_transfer_out, cudaStream_t stream,
+                          uint64_t* launches) {
+    if (P.nblocks) {
+        cham_prot_seg_k<<<P.nseg < 2048u ? P.nseg : 2048u, PSEG, 0, stream>>>(sigw, P.nbytes, P.nblocks, P.nseg, P.st, it, P.inc, P.cm, ps, P.T);
+        cham_prot_groups_k<<<(P.ngrp * PC_NC + 255) / 256, 256, 0, stream>>>(P.nseg, P.st, P.T, P.GT);
+        *launches += 2;
+    }
+    cham_prot_transfer_k<<<1, 256, 0, stream>>>(P.nseg, P.st, P.GT, d_transfer_out);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t prot_settle(const ProtSegs& P, ProtShard* ps, int it, int warm, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words,
+                        cudaStream_t stream, uint64_t* launches) {
+    cham_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, P.nseg, P.st, P.GT, P.gin, ps, d_words);
+    ++*launches;
+    if (P.nseg) {
+        cham_prot_seams_k<<<(P.ngrp + 127) / 128, 128, 0, stream>>>(P.nseg, P.st, P.T, P.gin, P.in_state);
+        cham_prot_walk_k<<<(P.nseg + 127) / 128, 128, 0, stream>>>(P.nblocks, P.nseg, P.st, it, warm, P.inc, P.cm, P.cm2, P.in_state, P.gin, ps, d_words);
+        *launches += 2;
+    }
+    return cudaGetLastError();
+}
+cudaError_t prot_commit(const ProtSegs& P, ProtShard* ps, int it, const uint32_t* d_all_words, uint32_t world, uint32_t stride, cudaStream_t stream,
+                        uint64_t* launches) {
+    if (P.nblocks) {
+        cham_prot_commit_k<<<(uint32_t)((P.nblocks + 1023) / 1024 < 1024 ? (P.nblocks + 1023) / 1024 : 1024), 256, 0, stream>>>(
+            d_all_words, world, stride, P.nblocks, P.st, it, P.cm, P.cm2);
+        ++*launches;
+    }
+    cham_prot_verdict_k<<<1, 32, 0, stream>>>(d_all_words, world, stride, P.st, it, ps);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t prot_refuse_unsettled(Status* st, const ProtShard* ps, cudaStream_t stream, uint64_t* launches) {
+    cham_prot_finish_k<<<1, 32, 0, stream>>>(st, ps);
+    ++*launches;
+    return cudaGetLastError();
+}
+cudaError_t prot_seam_words(uint64_t nblocks, Status* st, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
+    cham_prot_seam_words_k<<<1, 32, 0, stream>>>(nblocks, st, d_out_size, d_seam8);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+static ProtSegs cham_prot_segs(const ChamBufs& B) { return prot_segs(B.st, B.nbytes, B.nblocks, B.incb, B.copymap, B.copymap2, B.seg_state); }
+
 cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
                             cudaStream_t stream, uint64_t* launches) {
-    cham_prot_start_k<<<1, 32, 0, stream>>>(reinterpret_cast<Status*>(ws + L.status), ps, first_block, d_lengths, rank);
+    cham_prot_start_k<<<1, 32, 0, stream>>>(reinterpret_cast<Status*>(ws + L.status), ps, first_block, d_lengths, rank, 256u);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1699,48 +1768,29 @@ cudaError_t cham_put_u64(uint64_t* d, uint64_t v, cudaStream_t stream, uint64_t*
 cudaError_t cham_prot_transfer(size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, const uint32_t* d_carry_in, const ProtShard* ps,
                                int it, uint32_t* d_transfer_out, cudaStream_t stream, uint64_t* launches) {
     const ChamBufs B(ws, L, nbytes);
-    if (B.nblocks) {
-        launch_carry_resolve(B, nruns, d_carry_in, B.st, stream, launches);
-        cham_prot_seg_k<<<B.nseg < 2048u ? B.nseg : 2048u, PSEG, 0, stream>>>(B.sigw, nbytes, B.nblocks, B.nseg, B.st, it, B.incb, B.copymap, ps, B.T);
-        cham_prot_groups_k<<<(B.ngrp * PC_NC + 255) / 256, 256, 0, stream>>>(B.nseg, B.st, B.T, B.GT);
-        *launches += 2;
-    }
-    cham_prot_transfer_k<<<1, 256, 0, stream>>>(B.nseg, B.st, B.GT, d_transfer_out);
-    ++*launches;
-    return cudaGetLastError();
+    if (B.nblocks) launch_carry_resolve(B, nruns, d_carry_in, B.st, stream, launches);
+    return prot_transfer(cham_prot_segs(B), B.sigw, ps, it, d_transfer_out, stream, launches);
 }
 
 cudaError_t cham_prot_settle(size_t nbytes, uint8_t* ws, const ChamLayout& L, ProtShard* ps, int it, const uint32_t* d_all_transfers, uint32_t rank,
                              uint32_t* d_words, cudaStream_t stream, uint64_t* launches) {
     const ChamBufs B(ws, L, nbytes);
-    cham_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, B.nseg, B.st, B.GT, B.gin, ps, d_words);
-    ++*launches;
-    if (B.nseg) {
-        cham_prot_seams_k<<<(B.ngrp + 127) / 128, 128, 0, stream>>>(B.nseg, B.st, B.T, B.gin, B.in_state);
-        cham_prot_walk_k<<<(B.nseg + 127) / 128, 128, 0, stream>>>(B.nblocks, B.nseg, B.st, it, B.incb, B.copymap, B.copymap2, B.in_state, B.gin, ps, d_words);
-        *launches += 2;
-    }
-    return cudaGetLastError();
+    return prot_settle(cham_prot_segs(B), ps, it, 0, d_all_transfers, rank, d_words, stream, launches);
 }
 
 cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, uint32_t nruns, ProtShard* ps, int it,
                            const uint32_t* d_all_words, uint32_t world, uint32_t* d_table_out, cudaStream_t stream, uint64_t* launches) {
     const ChamBufs B(ws, L, nbytes);
-    if (B.nblocks) {
-        cham_prot_commit_k<<<(uint32_t)((B.nblocks + 1023) / 1024 < 1024 ? (B.nblocks + 1023) / 1024 : 1024), 256, 0, stream>>>(
-            d_all_words, world, B.nblocks, B.st, it, B.copymap, B.copymap2);
-        ++*launches;
-    }
-    cham_prot_verdict_k<<<1, 32, 0, stream>>>(d_all_words, world, B.st, it, ps);
-    ++*launches;
+    cudaError_t e = prot_commit(cham_prot_segs(B), ps, it, d_all_words, world, PROT_ROUND_WORDS, stream, launches);
+    if (e != cudaSuccess) return e;
     if (d_table_out) {
         if (B.nblocks) {   // round it + 1: flags under the new map (copy-mode blocks hidden from the dictionary) and the shard's table
-            cudaError_t e = set_smem_attrs_once();
+            e = set_smem_attrs_once();
             if (e != cudaSuccess) return e;
             launch_flag_pass(B, d_in, nruns, B.copymap, B.st, stream, launches);
             launch_export_fold(B, nruns, d_table_out, B.st, stream, launches);
         } else {
-            cudaError_t e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), stream);   // nothing touched
+            e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), stream);   // nothing touched
             if (e != cudaSuccess) return e;
         }
     }
@@ -1750,14 +1800,10 @@ cudaError_t cham_prot_next(const uint8_t* d_in, size_t nbytes, uint8_t* ws, cons
 cudaError_t cham_prot_finish(const uint8_t* d_in, size_t nbytes, uint8_t* ws, const ChamLayout& L, const ProtShard* ps, uint8_t* d_out, size_t cap,
                              uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches, cudaEvent_t* ev) {
     const ChamBufs B(ws, L, nbytes);
-    cham_prot_finish_k<<<1, 32, 0, stream>>>(B.st, ps);
-    ++*launches;
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = prot_refuse_unsettled(B.st, ps, stream, launches);
     if (e == cudaSuccess && B.nblocks) e = cham_phase2_finish(B, d_in, d_out, cap, d_out_size, true, false, stream, launches, ev);
     if (e != cudaSuccess) return e;
-    cham_prot_seam_words_k<<<1, 32, 0, stream>>>(B.nblocks, B.st, d_out_size, d_seam8);
-    ++*launches;
-    return cudaGetLastError();
+    return prot_seam_words(B.nblocks, B.st, d_out_size, d_seam8, stream, launches);
 }
 
 }  // namespace dns

@@ -699,8 +699,11 @@ __device__ __forceinline__ void chunk_t_compose(uint32_t& T, uint32_t& a, uint32
     else if (a2 != a) { b = a; a = a2; T = 2; }                        // T1 v after T1 w (v != w) or over (a, b) (v != a): (v, a)
 }
 
-// the shard's transfer, composed over its runs in order (the run tables of the round whose tag is *epoch_p)
-__global__ void cl_export_p_chee(const uint4* __restrict__ entP_all, uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+// the shard's transfer, composed over its runs in order (the run tables of the round whose tag is *epoch_p). `gate` (may be nullptr =
+// always): the copy-map rounds of density_b200_cl_shard_prot_* skip the exports once the map has settled, nobody reads them then.
+__global__ void cl_export_p_chee(const uint4* __restrict__ entP_all, uint32_t nruns, const Status* __restrict__ gate, const uint32_t* __restrict__ epoch_p,
+                                 uint32_t* __restrict__ out) {
+    if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
     if (ctx >= PL) return;
     const uint32_t epoch = *epoch_p;
@@ -712,7 +715,8 @@ __global__ void cl_export_p_chee(const uint4* __restrict__ entP_all, uint32_t nr
     out[ctx] = touched; out[PL + ctx] = q;
 }
 __global__ void cl_export_p_lion(const uint32_t* __restrict__ in, const uint4* __restrict__ hot_all, const uint32_t* __restrict__ cold_all,
-                                 uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+                                 uint32_t nruns, const Status* __restrict__ gate, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+    if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t ctx = blockIdx.x * blockDim.x + threadIdx.x;
     if (ctx >= PL) return;
     const uint32_t epoch = *epoch_p;
@@ -731,7 +735,9 @@ __global__ void cl_export_p_lion(const uint32_t* __restrict__ in, const uint4* _
     }
     lion_t_store(out, ctx, x);
 }
-__global__ void cl_export_c(const uint4* __restrict__ entC_all, uint32_t nruns, const uint32_t* __restrict__ epoch_p, uint32_t* __restrict__ out) {
+__global__ void cl_export_c(const uint4* __restrict__ entC_all, uint32_t nruns, const Status* __restrict__ gate, const uint32_t* __restrict__ epoch_p,
+                            uint32_t* __restrict__ out) {
+    if (gate && !(gate->nonquiet && !gate->converged)) return;
     const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= PL) return;
     const uint32_t epoch = *epoch_p;
@@ -778,10 +784,11 @@ __global__ void cl_rank_fold_k(int alg, int kind, const uint32_t* __restrict__ t
     cl_t_init(alg, kind, carry, i);
     for (uint32_t r = 0; r < rank; ++r) cl_t_fold(alg, kind, carry, tables + (size_t)r * planes * PL, i);
 }
-// the context of a shard's first quad comes from the last quad of the nearest earlier shard that has one (words: [world] {has, quad})
-__global__ void cl_prev_quad_k(const uint32_t* __restrict__ words, uint32_t rank, uint32_t* __restrict__ out) {
+// the context of a shard's first quad comes from the last quad of the nearest earlier shard that has one (words: [world][stride], {has,
+// quad} at the front of every row)
+__global__ void cl_prev_quad_k(const uint32_t* __restrict__ words, uint32_t stride, uint32_t rank, uint32_t* __restrict__ out) {
     uint32_t q = 0;
-    for (uint32_t r = 0; r < rank; ++r) if (words[2 * r]) q = words[2 * r + 1];
+    for (uint32_t r = 0; r < rank; ++r) if (words[stride * r]) q = words[stride * r + 1];
     *out = q;
 }
 __global__ void cl_last_quad_k(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t* __restrict__ out) {
@@ -819,6 +826,39 @@ __global__ void cl_seam_words_k(const uint8_t* __restrict__ inc, const uint8_t* 
     const uint64_t sz = *d_out_size;
     words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
 }
+
+// ---- copy mode on every shard (density_b200_cl_shard_prot_*) ---------------------------------------------------------------------------
+// words 4-7 of a shard's round words: {has an encoded quad, the last one, 0, 0} under `cm` (the map the next round uses). With `gate`
+// closed the map has settled, and the record keeps what the round that settled it found. One CTA of 256 threads walks back from the last
+// block; the automaton encodes a block at least every 256 blocks, so it stops within the first chunks.
+__global__ void __launch_bounds__(256)
+cl_prot_quad_k(const uint32_t* __restrict__ in, uint64_t nquads, uint64_t nblocks, uint32_t block_quads, const uint8_t* __restrict__ cm,
+               const Status* __restrict__ gate, ProtShard* __restrict__ ps, uint32_t* __restrict__ words) {
+    __shared__ unsigned long long s_best;               // 1 + the last encoded block that has a quad
+    if (!gate || (gate->nonquiet && !gate->converged)) {
+        if (threadIdx.x == 0) s_best = 0;
+        __syncthreads();
+        for (uint64_t base = 0; base < nblocks; base += blockDim.x) {
+            bool found = false;
+            if (base + threadIdx.x < nblocks) {
+                const uint64_t b = nblocks - 1 - base - threadIdx.x;
+                found = !cm[b] && b * block_quads < nquads;
+                if (found) atomicMax(&s_best, (unsigned long long)b + 1);
+            }
+            if (__syncthreads_or(found)) break;
+        }
+        if (threadIdx.x == 0) {
+            const uint64_t b = s_best;
+            uint64_t qi = b ? b * block_quads - 1 : 0;       // the block's last quad (the stream's last, in a short last block)
+            if (qi >= nquads) qi = nquads - 1;
+            ps->has_quad = b ? 1u : 0u;
+            ps->last_quad = b ? in[qi] : 0u;
+        }
+    }
+    if (threadIdx.x == 0) { words[4] = ps->has_quad; words[5] = ps->last_quad; words[6] = 0; words[7] = 0; }
+}
+// phase 1 of the shard at the stream start: its staged iteration settled or not
+__global__ void cl_prot_stage_k(const Status* __restrict__ iter, ProtShard* __restrict__ ps) { ps->stage_ok = iter->converged ? 1u : 0u; }
 
 }  // namespace chee
 
@@ -886,12 +926,12 @@ size_t chee_tables_bytes(int alg, int region, size_t nbytes, int num_sms) {
 
 // One encode over `n` bytes cut into `nruns` runs, as every launch below sees it: the geometry, and typed pointers into the workspace
 // (chee_layout) and the three run-table regions. The last four pointers exist only behind a shard's workspace
-// (cl_shard_workspace_bytes): its gate, its emit gate, its pair flag and the epoch of the round it exports.
+// (cl_shard_workspace_bytes): its gate, its emit gate, its pair flag, the epoch of the round it exports and the quad before it.
 struct CheeView {
     bool lion; const uint32_t* in32; size_t n; uint32_t bbytes, nruns, ntiles, ngroups, run_ctas, nseg; uint64_t nq, nstep, nblk;
     Status* stages; size_t stages_bytes; uint32_t *Pb, *Ab, *Bb, *F0, *F1, *F2; uint8_t *cm, *cm2, *incb; uint32_t *seg, *ctx0, *tile_bytes, *tile_local;
     uint64_t *group_total, *group_off; uint4* entP; uint32_t* coldP; uint4* entC;
-    Status *gate, *emit; uint32_t *pair_flag, *epoch_word;
+    Status *gate, *emit; uint32_t *pair_flag, *epoch_word, *prev_quad;
     CheeView(int alg, const uint8_t* d_in, size_t nbytes, int num_sms, uint8_t* ws, uint8_t* const tables[3]) {
         lion = alg == ALG_LION; bbytes = lion ? 64 : 128; in32 = reinterpret_cast<const uint32_t*>(d_in);
         cut(nbytes, chee_pick_runs(nbytes, num_sms));
@@ -906,7 +946,7 @@ struct CheeView {
         group_total = reinterpret_cast<uint64_t*>(ws + L.group_total); group_off = reinterpret_cast<uint64_t*>(ws + L.group_off);
         entP = reinterpret_cast<uint4*>(tables[0]); coldP = reinterpret_cast<uint32_t*>(tables[1]); entC = reinterpret_cast<uint4*>(tables[2]);
         gate = reinterpret_cast<Status*>(ws + ((L.total + 255) & ~(size_t)255)); emit = gate + 1; pair_flag = reinterpret_cast<uint32_t*>(emit + 1);
-        epoch_word = pair_flag + 1;
+        epoch_word = pair_flag + 1; prev_quad = epoch_word + 1;
     }
     // the same buffers for the first `nbytes` of the input cut into `runs` runs (the prefix stages of chee_iterate)
     CheeView prefix(size_t nbytes, uint32_t runs) const { CheeView v = *this; v.cut(nbytes, runs); return v; }
@@ -954,10 +994,11 @@ static void launch_tile_sizes(const CheeView& V, const uint8_t* mask, int final_
     else chee_tile_sizes<<<(V.ntiles + 7) / 8, 256, 0, stream>>>(V.Pb, V.Ab, V.Bb, mask, V.n, V.nblk, V.ntiles, final_pass, gate, V.incb, V.tile_bytes);
     ++*launches;
 }
-// tile offsets from the tile sizes (and the stream's size, checked against `cap`), then emit
+// tile offsets from the tile sizes (and the stream's size, checked against `cap`), then emit; ev_emit (may be nullptr) is recorded between
 static cudaError_t launch_scan_emit(const CheeView& V, const uint8_t* mask, Status* gate, size_t cap, uint64_t* d_out_size, uint8_t* d_out,
-                                    cudaStream_t stream, uint64_t* launches) {
+                                    cudaStream_t stream, uint64_t* launches, cudaEvent_t ev_emit = nullptr) {
     cudaError_t e = scan_tiles_launch(V.tile_bytes, V.ntiles, V.tile_local, V.group_total, V.group_off, V.ngroups, gate, cap, d_out_size, stream);
+    if (e == cudaSuccess && ev_emit) e = cudaEventRecord(ev_emit, stream);
     if (e != cudaSuccess) return e;
     if (V.lion) lion_emit<<<V.ntiles, 256, 0, stream>>>(V.in32, V.n, V.nblk, V.F0, V.F1, V.F2, V.Pb, V.Ab, V.Bb, mask, gate, V.tile_local, V.group_off, 4096, d_out);
     else chee_emit<<<V.ntiles, 256, 0, stream>>>(V.in32, V.n, V.nblk, V.Pb, V.Ab, V.Bb, mask, gate, V.tile_local, V.group_off, 4096, d_out);
@@ -1069,8 +1110,8 @@ cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32
     cl_shard_gates<<<1, 1, 0, stream>>>(V.gate, V.emit, iter, V.pair_flag, V.epoch_word, ep);
     ++*launches;
     if (!first) launch_ctx0_pass_p(V, nullptr, V.gate, d_prev_quad, ep, nullptr, stream, launches);
-    if (V.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(V.in32, V.entP, V.coldP, V.nruns, V.epoch_word, d_tab_p);
-    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(V.entP, V.nruns, V.epoch_word, d_tab_p);
+    if (V.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(V.in32, V.entP, V.coldP, V.nruns, nullptr, V.epoch_word, d_tab_p);
+    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(V.entP, V.nruns, nullptr, V.epoch_word, d_tab_p);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1082,7 +1123,7 @@ cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, 
                             uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
     const CheeView V(alg, d_in, n, num_sms, ws, tables);
     if (!first) launch_fold_p_pass_c(V, nullptr, V.gate, epoch_base + 32, d_carry_p, stream, launches);
-    cl_export_c<<<PL / 128, 128, 0, stream>>>(V.entC, V.nruns, V.epoch_word, d_tab_c);
+    cl_export_c<<<PL / 128, 128, 0, stream>>>(V.entC, V.nruns, nullptr, V.epoch_word, d_tab_c);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1130,9 +1171,107 @@ cudaError_t cl_last_quad(const uint8_t* d_in, size_t n, uint32_t* d_out2, cudaSt
     return cudaGetLastError();
 }
 cudaError_t cl_prev_quad(const uint32_t* d_words, uint32_t rank, uint32_t* d_out, cudaStream_t stream, uint64_t* launches) {
-    cl_prev_quad_k<<<1, 1, 0, stream>>>(d_words, rank, d_out);
+    cl_prev_quad_k<<<1, 1, 0, stream>>>(d_words, 2, rank, d_out);
     ++*launches;
     return cudaGetLastError();
+}
+
+// ---- sharded encode with copy mode on every shard (density_b200_cl_shard_prot_*, DESIGN.md section 5) ---------------------------------
+// Round k of the copy-map iteration runs on every shard at once: the context from the quad words of the round before, ctx0 and pass P
+// under the map M_k, fold P and pass C, fold C, sizes and incompressible bits, then the automaton half shared with Chameleon (transfer,
+// settle, commit: prot_*). The shard at the stream start (a.first) runs the staged iteration to the end in phase 1: the map of a prefix
+// does not depend on what follows it, so its map, flags and run tables are final. In the rounds it only re-exports them and walks its
+// blocks again (which changes nothing). A later shard starts from the empty map. Whatever the map the rounds start from, round k leaves a
+// map that agrees with the single call's on one block more than M_k did, and a map that the round leaves unchanged is the single call's.
+// Epochs: epoch_base .. + 31 for the staged iteration, epoch_base + 32 + k for round k; the exports read the epoch of the last round that
+// ran from the ctx0 epoch word. Under the gate of the rounds (V.gate, opened by prot_start) every kernel returns once the map settled.
+constexpr uint32_t CL_PROT_EPOCHS = 32 + PROT_MAX_ROUNDS + 1;
+uint32_t cl_prot_epochs() { return CL_PROT_EPOCHS; }
+
+static ProtSegs cl_prot_segs(const CheeView& V) { return prot_segs(V.gate, V.n, V.nblk, V.incb, V.cm, V.cm2, V.seg); }
+static void launch_prot_quad(const CheeView& V, const uint8_t* cm, const Status* gate, ProtShard* ps, uint32_t* d_words8, cudaStream_t stream,
+                             uint64_t* launches) {
+    cl_prot_quad_k<<<1, 256, 0, stream>>>(V.in32, V.nq, V.nblk, V.bbytes / 4, cm, gate, ps, d_words8);
+    ++*launches;
+}
+
+cudaError_t cl_prot_phase1(const ClProtShard& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    Status* iter = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (a.first) e = chee_iterate(V, a.epoch_base, a.num_sms, false, V.epoch_word, stream, launches, &iter);
+    else if (V.nblk) e = cudaMemsetAsync(V.cm, 0, V.nblk, stream);                 // M_0: nothing copied
+    if (e == cudaSuccess) e = cudaMemsetAsync(V.gate, 0, sizeof(Status), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_words8, 0, CL_PROT_ROUND_WORDS * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    e = prot_start(cl_prot_segs(V), a.ps, a.offset / V.bbytes, nullptr, 0, V.bbytes, stream, launches);
+    if (e != cudaSuccess) return e;
+    if (iter) { cl_prot_stage_k<<<1, 1, 0, stream>>>(iter, a.ps); ++*launches; }
+    launch_prot_quad(V, V.cm, nullptr, a.ps, d_words8, stream, launches);
+    return cudaGetLastError();
+}
+
+cudaError_t cl_prot_p(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
+                      uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    if (!V.nblk) return cudaMemsetAsync(d_tab_p, 0, (size_t)cl_table_planes(a.alg, 0) * PL * sizeof(uint32_t), stream);   // identity
+    if (!a.first) {
+        cl_prev_quad_k<<<1, 1, 0, stream>>>(d_all_words + 4, CL_PROT_ROUND_WORDS, rank, V.prev_quad);
+        ++*launches;
+        launch_ctx0_pass_p(V, V.cm, V.gate, V.prev_quad, a.epoch_base + 32 + (uint32_t)it, V.epoch_word, stream, launches);
+    }
+    if (V.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(V.in32, V.entP, V.coldP, V.nruns, V.gate, V.epoch_word, d_tab_p);
+    else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(V.entP, V.nruns, V.gate, V.epoch_word, d_tab_p);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t cl_prot_c(const ClProtShard& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    if (!V.nblk) return cudaMemsetAsync(d_tab_c, 0, (size_t)cl_table_planes(a.alg, 1) * PL * sizeof(uint32_t), stream);
+    if (!a.first) launch_fold_p_pass_c(V, V.cm, V.gate, a.epoch_base + 32 + (uint32_t)it, d_carry_p, stream, launches);
+    cl_export_c<<<PL / 128, 128, 0, stream>>>(V.entC, V.nruns, V.gate, V.epoch_word, d_tab_c);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t cl_prot_transfer(const ClProtShard& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    if (!a.first && V.nblk) {          // the incompressible bits of the blocks M_k encodes; copied blocks keep those of the round before
+        launch_fold_c(V, V.gate, a.epoch_base + 32 + (uint32_t)it, d_carry_c, stream, launches);
+        launch_tile_sizes(V, V.cm, 0, V.gate, stream, launches);
+    }
+    return prot_transfer(cl_prot_segs(V), nullptr, a.ps, it, d_transfer, stream, launches);
+}
+
+cudaError_t cl_prot_settle(const ClProtShard& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
+                           uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    cudaError_t e = prot_settle(cl_prot_segs(V), a.ps, it, 1, d_all_transfers, rank, d_words8, stream, launches);
+    if (e != cudaSuccess) return e;
+    launch_prot_quad(V, V.cm2, V.gate, a.ps, d_words8, stream, launches);
+    return cudaGetLastError();
+}
+
+cudaError_t cl_prot_next(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    return prot_commit(cl_prot_segs(V), a.ps, it, d_all_words, world, CL_PROT_ROUND_WORDS, stream, launches);
+}
+
+// sizes under the committed map, scan, emit under the gate of the rounds (it has converged when the map settled; the error of an unsettled
+// shard closes it), the seam words
+cudaError_t cl_prot_finish(const ClProtShard& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
+                           uint64_t* launches, cudaEvent_t ev_emit) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    cudaError_t e = prot_refuse_unsettled(V.gate, a.ps, stream, launches);
+    if (e == cudaSuccess && V.nblk) {
+        launch_tile_sizes(V, V.cm, 1, V.gate, stream, launches);
+        e = launch_scan_emit(V, V.cm, V.gate, cap, d_out_size, d_out, stream, launches, ev_emit);
+    } else if (ev_emit) {
+        e = cudaEventRecord(ev_emit, stream);
+    }
+    if (e != cudaSuccess) return e;
+    return prot_seam_words(V.nblk, V.gate, d_out_size, d_seam8, stream, launches);
 }
 
 }  // namespace dns

@@ -58,8 +58,34 @@ struct ProtShard {
     uint32_t rounds;                  // rounds run until the map settled (0: not settled)
     uint32_t settled, in_state, esc;  // in_state: pc_encode candidate of the true incoming state of the last round (0xFFFF: PC_ESC)
     uint32_t changed[16];             // blocks of this shard whose copy status changed, per round
+    uint32_t stage_ok;                // 0: the shard's own staged iteration did not settle (Cheetah / Lion, the shard at the stream start)
+    uint32_t has_quad, last_quad;     // Cheetah / Lion: the shard's last encoded quad under the map of the next round, if it has one
 };
 constexpr uint32_t PROT_TRANSFER_WORDS = 200, PROT_ROUND_WORDS = 4, PROT_MAX_ROUNDS = 16;
+// The launches of the sharded copy-map iteration that every codec shares, on one shard's blocks (nblocks of the codec's size): the
+// incompressible bits `inc`, the committed map `cm`, the next map `cm2`, and the segment states and candidate tables in a region of
+// prot_state_bytes(). Round words are rows of `stride` u32 that start {changed, met PC_ESC, settled before this round, 0}.
+struct ProtSegs {
+    Status* st; uint64_t nbytes, nblocks; uint32_t nseg, ngrp;
+    uint8_t *inc, *cm, *cm2; uint32_t *in_state, *gin; uint16_t *T, *GT;
+};
+ProtSegs prot_segs(Status* st, uint64_t nbytes, uint64_t nblocks, uint8_t* inc, uint8_t* cm, uint8_t* cm2, uint32_t* seg_state);
+// the record of a shard that starts at first_block (or at the sum of d_lengths[0 .. rank) / block_bytes); opens the gate of the rounds
+cudaError_t prot_start(const ProtSegs& P, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank, uint32_t block_bytes,
+                       cudaStream_t stream, uint64_t* launches);
+// the shard's transfer (PROT_TRANSFER_WORDS u32); sigw: Chameleon's signatures, from which the bits are refreshed first (nullptr: as they are)
+cudaError_t prot_transfer(const ProtSegs& P, const uint32_t* sigw, const ProtShard* ps, int it, uint32_t* d_transfer_out, cudaStream_t stream,
+                          uint64_t* launches);
+// the true incoming state from the transfers of the shards before `rank`, the walk into cm2, words 0-3 of d_words. warm: round 0's flags
+// were computed under cm (else under the empty map)
+cudaError_t prot_settle(const ProtSegs& P, ProtShard* ps, int it, int warm, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words,
+                        cudaStream_t stream, uint64_t* launches);
+// the global commit and verdict of round `it` from the gathered round words
+cudaError_t prot_commit(const ProtSegs& P, ProtShard* ps, int it, const uint32_t* d_all_words, uint32_t world, uint32_t stride, cudaStream_t stream,
+                        uint64_t* launches);
+// before the emit: the error of a shard that did not settle; after it: the 8 seam words (word 2: refused or error; the size is then 0)
+cudaError_t prot_refuse_unsettled(Status* st, const ProtShard* ps, cudaStream_t stream, uint64_t* launches);
+cudaError_t prot_seam_words(uint64_t nblocks, Status* st, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches);
 // start: after cham_encode_phase1 (round 0's flags); first_block, or the sum of lengths[0 .. rank) / 256 when d_lengths is set
 cudaError_t cham_prot_start(uint8_t* ws, const ChamLayout& L, ProtShard* ps, uint64_t first_block, const uint64_t* d_lengths, uint32_t rank,
                             cudaStream_t stream, uint64_t* launches);
@@ -103,6 +129,25 @@ cudaError_t cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_
 cudaError_t cl_rank_fold(int alg, int kind, const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
 cudaError_t cl_last_quad(const uint8_t* d_in, size_t n, uint32_t* d_out2, cudaStream_t stream, uint64_t* launches);   // {has a quad, last quad}
 cudaError_t cl_prev_quad(const uint32_t* d_words, uint32_t rank, uint32_t* d_out, cudaStream_t stream, uint64_t* launches);
+// the same with copy-mode blocks anywhere (density_b200_cl_shard_prot_*): the copy-map iteration carried over the cuts, round for round.
+// The shard starts at byte `offset` (first: offset 0 and n > 0, the shard that runs the staged iteration in phase 1); each call takes
+// cl_prot_epochs() fresh epochs from epoch_base. Round words: CL_PROT_ROUND_WORDS u32, {changed, met PC_ESC, settled before, 0, has an
+// encoded quad, that quad, 0, 0}. ps: the shard's record (device).
+constexpr uint32_t CL_PROT_ROUND_WORDS = 8;
+uint32_t cl_prot_epochs();
+struct ClProtShard { int alg; const uint8_t* d_in; size_t n; uint64_t offset; bool first; uint8_t* ws; uint8_t* const* tables; uint32_t epoch_base;
+                     int num_sms; ProtShard* ps; };
+cudaError_t cl_prot_phase1(const ClProtShard& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_p(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
+                      uint64_t* launches);
+cudaError_t cl_prot_c(const ClProtShard& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_transfer(const ClProtShard& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_settle(const ClProtShard& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
+                           uint64_t* launches);
+cudaError_t cl_prot_next(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches);
+// ev_emit (may be nullptr): recorded between the scan and the emit
+cudaError_t cl_prot_finish(const ClProtShard& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
+                           uint64_t* launches, cudaEvent_t ev_emit = nullptr);
 
 // chameleon_decode.cu
 size_t cham_decode_workspace_bytes(size_t nbytes, size_t cap, int nruns_max);

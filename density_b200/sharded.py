@@ -24,7 +24,9 @@ Cheetah and Lion shard the same way with three phases around two exchanges (Shar
 context of the next shard's first quad), then the shard's prediction transfer (P table), then its chunk-map transfer (C table). A
 transfer says what the shard does to the state carried into it; the carry-in of rank r is the stream-start state folded with the
 transfers of ranks < r (density_b200_cl_table_init / _fold, on the device). Only rank 0 may use copy mode; the seam verdict refuses
-what would need it elsewhere.
+what would need it elsewhere. ShardedCLEncoder.encode_protected and ShardedEncoder.encode_protected(..., alg="cheetah" / "lion")
+accept copy mode anywhere: the shard at the stream start settles its own map first, then every round runs the three phases on all
+ranks and exchanges the automaton transfers and 8 round words (which carry each shard's last encoded quad), as Chameleon does.
 
 A sharded Cheetah stream decodes the same way in pieces (ShardedDecoder.decode(..., alg="cheetah"), or the piece phases
 density_b200_cheetah_decode_shard_* with fold_cheetah_cmap and fold_cl_tables for the exchanges): the chunk-map transfers are
@@ -120,6 +122,7 @@ def seam_verdict(words):
 
 PROT_TRANSFER_WORDS = 200  # DENSITY_B200_PROT_TRANSFER_WORDS: candidate states of the protection automaton
 PROT_ROUND_WORDS = 4       # DENSITY_B200_PROT_ROUND_WORDS
+CL_PROT_ROUND_WORDS = 8    # DENSITY_B200_CL_PROT_ROUND_WORDS: the round words of the Cheetah / Lion path, quad words at 4-5
 PROT_STATUS_WORDS = 20     # DENSITY_B200_PROT_STATUS_WORDS
 PROT_ESC = 0xFFFF          # a path that left the candidate states
 _PC_NS, _PC_NP = 10, 10    # candidate starts 1..10, penalties 0..9 (chameleon_encode.cu: PC_NS, PC_NP)
@@ -392,6 +395,55 @@ class ShardedCLEncoder(_Handle):
         self.events = ev
         return verdict
 
+    def encode_protected(self, d_in, d_out, d_size, group=None):
+        """The copy-mode path (density_b200_cl_shard_prot_*): the arguments of encode, any input. The shard at the stream start runs the
+        staged copy-map iteration in phase 1; then the round budget of the iteration runs on all ranks with torch.distributed exchanges
+        (round words, P tables, C tables, transfers) and the device folds. Returns seam_verdict's (flags, total, offsets) over all ranks;
+        flags != 0 only when an iteration did not settle, the automaton left the candidate states, or on an error: the pieces are then
+        void."""
+        rank, world = _rank_world(group)
+        stream = _stream()
+        dev = d_in.device
+        lib = self._lib
+
+        def check(rc, what):
+            _check(rc, f"cl_shard_prot_{what}")
+
+        n = d_in.numel()
+        offset = int(gather_rows(torch.tensor([n], dtype=torch.int64, device=dev), group)[:rank].sum())
+        words = torch.zeros(CL_PROT_ROUND_WORDS, dtype=torch.int32, device=dev)
+        tp = torch.zeros(self.words_p, dtype=torch.int32, device=dev)
+        tc = torch.zeros(self.words_c, dtype=torch.int32, device=dev)
+        transfer = torch.zeros(PROT_TRANSFER_WORDS, dtype=torch.int32, device=dev)
+        check(lib.density_b200_cl_shard_prot_phase1(self._h, d_in.data_ptr(), n, offset, int(rank == world - 1), words.data_ptr(), stream),
+              "phase1")
+        all_words = gather_rows(words, group).contiguous()
+        for _ in range(lib.density_b200_prot_round_budget()):
+            check(lib.density_b200_cl_shard_prot_p(self._h, all_words.data_ptr(), world, rank, tp.data_ptr(), stream), "p")
+            carry_p = fold_cl_tables(self.alg, CL_TABLE_P, gather_rows(tp, group), rank)
+            check(lib.density_b200_cl_shard_prot_c(self._h, carry_p.data_ptr(), tc.data_ptr(), stream), "c")
+            carry_c = fold_cl_tables(self.alg, CL_TABLE_C, gather_rows(tc, group), rank)
+            check(lib.density_b200_cl_shard_prot_transfer(self._h, carry_c.data_ptr(), transfer.data_ptr(), stream), "transfer")
+            all_transfers = gather_rows(transfer, group).contiguous()
+            check(lib.density_b200_cl_shard_prot_settle(self._h, all_transfers.data_ptr(), world, rank, words.data_ptr(), stream), "settle")
+            all_words = gather_rows(words, group).contiguous()
+            check(lib.density_b200_cl_shard_prot_next(self._h, all_words.data_ptr(), world, stream), "next")
+        seam = torch.empty(SEAM_WORDS, dtype=torch.int32, device=dev)
+        check(lib.density_b200_cl_shard_prot_finish(self._h, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), seam.data_ptr(), stream),
+              "finish")
+        return seam_verdict(gather_rows(seam, group))
+
+    def prot_status(self):
+        """density_b200_cl_shard_prot_status after encode_protected (waits for the device): dict with stage_settled (the staged
+        iteration of the shard at the stream start settled; True elsewhere), rounds (until the map settled, 0: not settled), in_state
+        ((penalty, start, previous_incompressible) entering the shard, None: left the candidates), esc and changed (this shard's blocks
+        whose copy status changed, per round, 16 values)."""
+        out = (ctypes.c_uint32 * PROT_STATUS_WORDS)()
+        _check(self._lib.density_b200_cl_shard_prot_status(self._h, out), "cl_shard_prot_status")
+        v = list(out)
+        ins = None if v[2] == 0xFFFFFFFF else (v[2] & 0xFF, (v[2] >> 8) & 0xFF, v[2] >> 16)
+        return {"stage_settled": bool(v[0]), "rounds": v[1], "in_state": ins, "esc": v[3], "changed": v[4:20]}
+
     def phase_ms(self):
         """[phase 1, P exchange + fold, phase 2, C exchange + fold, phase 3 + seams] in ms, of the last encode(timing=True)"""
         torch.cuda.synchronize()
@@ -509,13 +561,19 @@ class ShardedEncoder(_ShardedHandle):
             rc = self._lib.density_b200_encode_sharded_cl(self._h, alg, *args)
         _check(rc, f"encode_sharded{'' if alg == 0 else '_cl'}")
 
-    def encode_protected(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None):
+    def encode_protected(self, d_in, d_out, d_size, d_flags, gather_root=-1, d_gather=None, alg="chameleon"):
         """density_b200_encode_sharded_protected: Chameleon with copy mode, the arguments of encode. d_flags != 0 only when the copy map
-        did not settle within the round budget, the automaton left the candidate states, or on an error: the pieces are then void."""
-        _check(self._lib.density_b200_encode_sharded_protected(
-            self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
-            self.d_total.data_ptr(), int(gather_root), d_gather.data_ptr() if d_gather is not None else None,
-            d_gather.numel() if d_gather is not None else 0, _stream()), "encode_sharded_protected")
+        did not settle within the round budget, the automaton left the candidate states, or on an error: the pieces are then void.
+        alg "cheetah" / "lion" (or their ids): density_b200_encode_sharded_cl_protected, the same contract for those algorithms (the call
+        waits once for the gathered shard lengths)."""
+        args = (d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(),
+                int(gather_root), d_gather.data_ptr() if d_gather is not None else None, d_gather.numel() if d_gather is not None else 0, _stream())
+        alg = _alg_id(alg)
+        if alg == 0:
+            rc = self._lib.density_b200_encode_sharded_protected(self._h, *args)
+        else:
+            rc = self._lib.density_b200_encode_sharded_cl_protected(self._h, alg, *args)
+        _check(rc, f"encode_sharded{'' if alg == 0 else '_cl'}_protected")
 
     def profile(self):
         """stage times (ms) of the last encode: Chameleon flag pass, table exchange + fold, carry / resolve / sizes / scan, emit, seams +

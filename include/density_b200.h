@@ -158,8 +158,8 @@ DENSITY_B200_API int density_b200_encode_sharded(density_b200_sharded*, const ui
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream);
 /* stage times (ms) of the last encode_sharded or encode_sharded_cl call. Chameleon: [0] flag pass, [1] table exchange + fold, [2] carry /
    resolve / sizes / scan, [3] emit, [4] seams + gather. Cheetah / Lion: [0] phase 1, [1] P exchange + fold, [2] phase 2 + C exchange +
-   fold, [3] phase 3, [4] seams + gather. encode_sharded_protected: [0] phase 1, [1] the first table exchange + fold, [2] the rounds, sizes
-   and scan, [3] emit, [4] seams + gather. */
+   fold, [3] phase 3, [4] seams + gather. encode_sharded_protected and encode_sharded_cl_protected: [0] phase 1, [1] the first table
+   exchange + fold, [2] the rounds, sizes and scan, [3] emit, [4] seams + gather. */
 DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* out_ms5);
 
 /*
@@ -193,7 +193,8 @@ DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* 
 #define DENSITY_B200_PROT_TRANSFER_WORDS 200
 #define DENSITY_B200_PROT_ROUND_WORDS 4
 #define DENSITY_B200_PROT_STATUS_WORDS 20
-/* rounds of the iteration (16; density_b200_test_set_prot_rounds lowers it) */
+/* rounds of the iteration (16; density_b200_test_set_prot_rounds lowers it), of this path and of the Cheetah / Lion one
+   (density_b200_cl_shard_prot_*, density_b200_encode_sharded_cl_protected) */
 DENSITY_B200_API int density_b200_prot_round_budget(void);
 /* round 0: flags with unknown carry-in, the last-writer table (as density_b200_shard_phase1) to d_table_out. d_in must stay valid and
    unchanged until prot_finish has been enqueued. */
@@ -272,6 +273,74 @@ DENSITY_B200_API int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_a
 DENSITY_B200_API int density_b200_encode_sharded_cl(density_b200_sharded*, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                    uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather,
                                    size_t gather_cap, void* stream);
+
+/*
+ * Sharded Cheetah / Lion encode with copy mode (DESIGN.md section 5): the path above refuses copy-mode blocks after the first shard,
+ * penalties pending at a cut, incompressible pairs across a cut and an empty first shard; this one accepts them. It runs the copy-map
+ * fixed point of the single-device encoder (flags under the map -> incompressible bits -> automaton -> new map) on all shards at once,
+ * with the prediction tables, the chunk map, the context chain and the automaton state carried over the cuts. Shard r holds bytes
+ * [o_r, o_r + n_r) of one input, every non-final shard a multiple of 256 bytes; its first global block is o_r / 128 (Cheetah) or o_r / 64
+ * (Lion). The shard with o_r == 0 and n_r > 0 holds the stream start: it runs the staged iteration of the single-device encoder to the end
+ * in phase 1 (the map of a prefix does not depend on what follows it, so that map is final); the others start from the empty map. Every
+ * round extends the prefix on which the map agrees with the single call's by at least one block, and a map that a round leaves unchanged
+ * is the single call's. The concatenation of the pieces equals one cheetah_encode / lion_encode call over the whole input, byte for
+ * byte, whenever the verdict is 0. The verdict is non-zero (the pieces are void; nothing is written past `cap`) only when the staged
+ * iteration of the shard at the stream start did not settle, when the rounds did not settle within the budget, when the automaton's true
+ * path left the candidate states, or on an error (capacity).
+ *
+ * Phase API on a density_b200_cl_shard handle (any transport; W shards may run on one GPU): prot_phase1, then per round k = 0, 1, ...:
+ *   P          prot_p: the context of the shard's first encoded quad from the round words of all shards (phase 1's for k = 0, else the
+ *              round before's), ctx0 and pass P under the round's map, the shard's P table.
+ *   exchange   the P tables; the carry-in of shard r is density_b200_cl_table_init folded with the tables of shards < r.
+ *   C          prot_c: fold P from the carry-in, pass C, the shard's C table.
+ *   exchange   the C tables, folded as the P tables.
+ *   transfer   prot_transfer: fold C from the carry-in, sizes and incompressible bits, DENSITY_B200_PROT_TRANSFER_WORDS u32 as
+ *              density_b200_shard_prot_transfer's.
+ *   exchange   the transfers of all shards, in rank order.
+ *   settle     prot_settle: the true incoming state, the shard's next map and DENSITY_B200_CL_PROT_ROUND_WORDS round words {blocks whose
+ *              copy status changed, met 0xFFFF, settled before this round, 0, has an encoded quad, the last encoded quad, 0, 0} under
+ *              the next map (a copied block contributes no quad; a shard without one passes the earlier value on).
+ *   exchange   the round words of all shards, in rank order; then prot_next: the global commit (settled when no shard changed and
+ *              none met 0xFFFF: every later kernel returns at once).
+ * After at least one round, prot_finish emits. Every shard runs the same number of rounds; at most density_b200_prot_round_budget()
+ * (prot_p returns DENSITY_B200_EARG beyond it). Per round and rank that is the P table (0.5 MiB Cheetah, 3 MiB Lion), the C table
+ * (0.75 MiB), 800 bytes of transfer and 32 bytes of round words. Phases called out of order (a quiet density_b200_cl_shard_phase1 on the
+ * handle closes them), misaligned pointers (d_in and tables 4-byte, d_out 2-byte, d_out_size 8-byte), an offset that is not a multiple
+ * of 256 and a non-final shard that is not a multiple of 256 bytes return DENSITY_B200_EARG without enqueuing anything.
+ */
+#define DENSITY_B200_CL_PROT_ROUND_WORDS 8
+/* phase 1: the shard at the stream start (offset 0, n > 0) runs the staged copy-map iteration; the others take the empty map. Writes
+   the shard's round words for round 0 (words 4-5: has an encoded quad, the last one, under that map; the rest 0). d_in must stay valid
+   and unchanged until prot_finish has been enqueued. */
+DENSITY_B200_API int density_b200_cl_shard_prot_phase1(density_b200_cl_shard*, const uint8_t* d_in, size_t n, uint64_t offset, int is_last_shard,
+                                      uint32_t* d_words_out, void* stream);
+/* d_all_words: [world][DENSITY_B200_CL_PROT_ROUND_WORDS], the round words of all shards from phase 1 or the round before */
+DENSITY_B200_API int density_b200_cl_shard_prot_p(density_b200_cl_shard*, const uint32_t* d_all_words, int world, int rank, uint32_t* d_table_p_out,
+                                 void* stream);
+/* d_carry_p / d_carry_c: the P / C state before this shard under the round's map (the stream-start state for the first shard) */
+DENSITY_B200_API int density_b200_cl_shard_prot_c(density_b200_cl_shard*, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream);
+DENSITY_B200_API int density_b200_cl_shard_prot_transfer(density_b200_cl_shard*, const uint32_t* d_carry_c, uint32_t* d_transfer_out, void* stream);
+DENSITY_B200_API int density_b200_cl_shard_prot_settle(density_b200_cl_shard*, const uint32_t* d_all_transfers, int world, int rank,
+                                      uint32_t* d_words_out, void* stream);
+DENSITY_B200_API int density_b200_cl_shard_prot_next(density_b200_cl_shard*, const uint32_t* d_all_words, int world, void* stream);
+/* sizes under the committed map, scan, emit: the piece to d_out, its size to *d_out_size (0 when refused) and 8 seam words in the layout
+   of density_b200_shard_prot_finish's (words 0 and 1 are 0; word 2 = refused or error) */
+DENSITY_B200_API int density_b200_cl_shard_prot_finish(density_b200_cl_shard*, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
+                                      void* stream);
+/* after a commit (waits for the device), DENSITY_B200_PROT_STATUS_WORDS u32: out[0] the staged iteration of the shard at the stream start
+   settled (1 on the other shards), [1] rounds until the map settled (0: not settled), [2] the incoming state of the last round run,
+   penalty | start << 8 | previous_incompressible << 16 (~0: left the candidates), [3] met 0xFFFF, [4 + k] this shard's blocks whose copy
+   status changed in round k (k < 16) */
+DENSITY_B200_API int density_b200_cl_shard_prot_status(density_b200_cl_shard*, uint32_t* out20);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments and gather semantics of density_b200_encode_sharded_cl:
+   ncclAllGather(shard lengths, 8 bytes per rank), which the call waits for (the offsets decide which shard runs the staged iteration)
+   -> phase 1 -> ncclAllGather(round words, 32 bytes) -> the round budget of {P -> ncclAllGather(P tables) -> fold kernel -> C ->
+   ncclAllGather(C tables) -> fold kernel -> transfer -> ncclAllGather(transfers, 800 bytes) -> settle -> ncclAllGather(round words,
+   32 bytes) -> commit} -> finish -> ncclAllGather(seam words) -> verdict -> optional gather. Uses its own workspace in the handle. Bad
+   arguments (those of density_b200_encode_sharded_protected, and alg) return DENSITY_B200_EARG before any collective is enqueued. */
+DENSITY_B200_API int density_b200_encode_sharded_cl_protected(density_b200_sharded*, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out,
+                                             size_t cap, uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
+                                             uint8_t* d_gather, size_t gather_cap, void* stream);
 
 /*
  * Sharded Chameleon decode: the inverse of the sharded encode. Piece r is what shard r of a sharded encode produced (rank r's
@@ -511,8 +580,9 @@ DENSITY_B200_API void density_b200_test_set_stage_rounds(int k);
 /* Test hook: cut the round budget of the sharded Cheetah decode to k rounds (1..40, default 40) so that its "did not settle" refusal
    can be exercised. density_b200_decode_device does not read it. */
 DENSITY_B200_API void density_b200_test_set_decode_rounds(int k);
-/* Test hook: cut the round budget of the sharded copy-map iteration (density_b200_shard_prot_*, density_b200_encode_sharded_protected)
-   to k rounds (1..16, default 16) so that its "did not settle" refusal can be exercised. The single-device encoder does not read it. */
+/* Test hook: cut the round budget of the sharded copy-map iterations (density_b200_shard_prot_*, density_b200_encode_sharded_protected,
+   density_b200_cl_shard_prot_*, density_b200_encode_sharded_cl_protected) to k rounds (1..16, default 16) so that their "did not
+   settle" refusal can be exercised. The single-device encoders do not read it. */
 DENSITY_B200_API void density_b200_test_set_prot_rounds(int k);
 /* Test hook: resolve the NCCL entry points of the sharded drivers (ncclGetUniqueId, ncclCommInitRank, ncclCommDestroy, ncclAllGather,
    ncclSend, ncclRecv, ncclGroupStart, ncclGroupEnd, ncclGetErrorString) from the shared library at `path` instead of libnccl.so.2, e.g.

@@ -48,9 +48,10 @@ static cudaError_t empty_piece_outputs(uint64_t* d_out_size, uint32_t* d_seam8, 
 // grow-only device buffer
 struct DevBuf {
     uint8_t* p = nullptr; size_t bytes = 0;
-    // `stream`: the stream the buffer is about to be used on. The zero fill (the Cheetah / Lion encoder tables rely on starting out
-    // zeroed) is ordered on it; cudaFree of the old buffer synchronises the device, so nothing can still be using it.
-    cudaError_t ensure(size_t need, cudaStream_t stream = nullptr) {
+    // `stream`: the stream that next touches the buffer. The zero fill (the Cheetah / Lion encoder tables rely on starting out
+    // zeroed) is ordered on it; cudaFree of the old buffer synchronises the device, so nothing can still be using it. There is no
+    // default: the library's streams do not order against the legacy default stream, so a fill there could land after the next write.
+    cudaError_t ensure(size_t need, cudaStream_t stream) {
         if (need <= bytes) return cudaSuccess;
         if (p) { cudaFree(p); p = nullptr; bytes = 0; }
         size_t want = need + need / 8 + 4096;
@@ -417,14 +418,23 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
 constexpr size_t PIPE_CHUNK = 64u << 20;
 constexpr size_t PIPE_MIN_BYTES = 96u << 20;
 
+static size_t chameleon_encode_host_pipelined_impl(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap);
+// The pipeline runs on the device's one workspace like every other call: it waits on c->stream for the calls enqueued before it (on
+// whatever stream) and releases the workspace on every exit, the "not quiet" one included (the fallback then acquires it again).
 static size_t chameleon_encode_host_pipelined(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap) {
+    if (!ws_acquire(c, c->stream)) return 0;
+    const size_t r = chameleon_encode_host_pipelined_impl(c, in, n, out, out_cap);
+    ws_release(c, c->stream);
+    return r;
+}
+static size_t chameleon_encode_host_pipelined_impl(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap) {
     const size_t nchunks = (n + PIPE_CHUNK - 1) / PIPE_CHUNK;
     if (nchunks > 4096) return (size_t)-1;
-    cudaError_t e = c->stage_in.ensure(n + 16);
-    if (e == cudaSuccess) e = c->stage_out.ensure(safe_size(ALG_CHAMELEON, n) + 16);
-    if (e == cudaSuccess) e = c->pipe_tables.ensure(2 * 65536 * sizeof(uint32_t) + (nchunks + 1) * sizeof(uint64_t) + 256);
+    cudaError_t e = c->stage_in.ensure(n + 16, c->h2d_stream);
+    if (e == cudaSuccess) e = c->stage_out.ensure(safe_size(ALG_CHAMELEON, n) + 16, c->stream);
+    if (e == cudaSuccess) e = c->pipe_tables.ensure(2 * 65536 * sizeof(uint32_t) + (nchunks + 1) * sizeof(uint64_t) + 256, c->stream);
     ChamLayout L;
-    if (e == cudaSuccess) e = c->ws.ensure(cham_workspace_bytes(PIPE_CHUNK, c->num_sms, &L));
+    if (e == cudaSuccess) e = c->ws.ensure(cham_workspace_bytes(PIPE_CHUNK, c->num_sms, &L), c->stream);
     if (e != cudaSuccess) { set_error("pipeline cudaMalloc", e); return 0; }
     c->layout = L;
     uint32_t* d_acc = reinterpret_cast<uint32_t*>(c->pipe_tables.p);            // dictionary before the current chunk
@@ -509,7 +519,7 @@ static size_t run_sync(bool encode, int alg, const uint8_t* in, size_t n, uint8_
         d_in = c->stage_in.p;
     }
     if (!in_dev && !input_staged) {
-        e = c->stage_in.ensure(n + 16);
+        e = c->stage_in.ensure(n + 16, c->stream);
         if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return 0; }
         e = h2d_any(c->ring_in, c->stage_in.p, in, n, c->stream, is_pageable_host(in));
         if (e != cudaSuccess) { set_error("H2D copy", e); return 0; }
@@ -519,7 +529,7 @@ static size_t run_sync(bool encode, int alg, const uint8_t* in, size_t n, uint8_
         // encode: stage into a full safe-size buffer and check the real size against the caller's capacity afterwards
         // (the reference only fails when the bytes actually written exceed the slice, write_buffer.rs:19)
         d_cap = encode ? safe_size(alg, n) : out_cap;
-        e = c->stage_out.ensure(d_cap + 16);
+        e = c->stage_out.ensure(d_cap + 16, c->stream);
         if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return 0; }
         d_out = c->stage_out.p;
     }

@@ -79,6 +79,15 @@ DENSITY_B200_API size_t lion_safe_encode_buffer_size(size_t size);
  */
 DENSITY_B200_API int density_b200_encode_device(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                uint64_t* d_out_size, void* stream);
+/*
+ * Concurrent callers. The nine symbols above, the stream-ordered calls and the codec instances
+ * on one device share one cached workspace (sharded handles have their own). Calls from
+ * any host thread and on any stream are serialised on it in the order they are enqueued: a
+ * call's device work starts when the previous call's work (on whatever stream) has finished
+ * with the workspace. So a synchronous call (the nine symbols above, the codec instances)
+ * waits for the stream-ordered calls enqueued before it, and returns only after they are done.
+ * density_b200_shutdown must not overlap any other call.
+ */
 /* Test/diagnostic variant: choose the encode path explicitly.
    Chameleon: path 0 = auto (run-parallel fast path, exact protection-aware fallback when needed),
    1 = fast path only (no fallback; out size is only valid if the stream is "quiet"),
@@ -572,7 +581,7 @@ DENSITY_B200_API uint64_t density_b200_kernel_launches(void);
 /* 1 if the last Chameleon encode on this device used the segment-parallel fast path end to end,
    0 if it had to fall back to the sequential protection-aware path. */
 DENSITY_B200_API int density_b200_last_encode_was_fast(void);
-/* Free all cached device workspaces. */
+/* Free all cached device workspaces. No other call may be in progress on any thread; the next call allocates them afresh. */
 DENSITY_B200_API void density_b200_shutdown(void);
 /* Test hook: cut every stage of the Cheetah / Lion copy-map iteration to k rounds (1..7, default 7) so that the host-resumed
    iteration of path 4 can be exercised on ordinary inputs. */

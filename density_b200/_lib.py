@@ -101,6 +101,12 @@ _SIGS = {
     "density_b200_cheetah_cmap_fold": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_decode_sharded_cheetah": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
                                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_prot_transfer": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                       ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_prot_phase1": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                                     ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded_cheetah_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                     ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_cheetah_decode_locate": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint64,
                                                           ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_cheetah_locate_piece": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]),

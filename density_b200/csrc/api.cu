@@ -1148,17 +1148,20 @@ static int g_chee_dec_rounds = 40;    // round budget of the sharded Cheetah dec
 
 struct density_b200_cheetah_decode_shard {
     DevBuf ws, tables;
+    DevBuf seed;                    // the incoming automaton state of the prot_* phases (DECODE_PROT_SEED_WORDS)
     CheeShardArgs a{};
     int num_sms = 0;
     // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2 or a round's fold, 3 a round's walk, 4 phase 3
     int phase = 0;
     uint32_t round = 0;
+    bool transfer_done = false;     // prot_transfer done, prot_phase1 not yet
+    bool prot = false;              // the current piece went through prot_phase1: phase 3 writes the protected seam words
 };
 
 density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void) { return new_shard<density_b200_cheetah_decode_shard>(); }
 void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard* s) {
     if (!s) return;
-    s->ws.release(); s->tables.release();
+    s->ws.release(); s->tables.release(); s->seed.release();
     delete s;
 }
 int density_b200_cheetah_decode_round_budget(void) { return g_chee_dec_rounds; }
@@ -1170,7 +1173,7 @@ int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* 
     if (!s || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0; s->round = 0;
+    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
     CheeShardArgs& a = s->a;
     a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
     cudaError_t e = cudaSuccess;
@@ -1232,11 +1235,58 @@ int density_b200_cheetah_decode_shard_phase3(density_b200_cheetah_decode_shard* 
     if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
-    const cudaError_t e = s->a.n ? chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches) : empty_piece_outputs(d_out_size, d_seam8, st);
+    const uint32_t* seed = s->prot ? reinterpret_cast<const uint32_t*>(s->seed.p) : nullptr;
+    const cudaError_t e = (s->a.n || seed) ? chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches, seed) : empty_piece_outputs(d_out_size, d_seam8, st);
     const int rc = step_result(e, launches, "cheetah decode shard phase3");
     if (rc == DENSITY_B200_OK) s->phase = 4;
     return rc;
 }
+
+// ---- the same for streams with copy-mode blocks: the piece's protection transfer, then phase 1 from the composed state -------------------
+int density_b200_cheetah_decode_shard_prot_transfer(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                                    int is_first, int is_last, uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || (!d_out && cap) || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_transfer_out)) {
+        set_error("d_in must be 2-byte, d_out and d_transfer_out 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
+    CheeShardArgs& a = s->a;
+    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
+    cudaError_t e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
+    if (n) {
+        if (e == cudaSuccess) e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
+        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
+    }
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    a.ws = s->ws.p; a.tables = s->tables.p;
+    uint64_t launches = 0;
+    e = chee_shard_prot_transfer(a, d_transfer_out, st, &launches);
+    const int rc = step_result(e, launches, "cheetah decode shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->transfer_done = true;
+    return rc;
+}
+int density_b200_cheetah_decode_shard_prot_phase1(density_b200_cheetah_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
+                                                  uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s || !s->transfer_done || s->phase != 0) { set_error("cheetah_decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_cmap_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    s->transfer_done = false;   // one phase 1 per transfer
+    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, seed, st, &launches);
+    if (e == cudaSuccess) {
+        if (s->a.n) e = chee_shard_phase1(s->a, d_cmap_out, st, &launches, seed);
+        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    }
+    const int rc = step_result(e, launches, "cheetah decode shard prot phase1");
+    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
+    return rc;
+}
+
 int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard* s, uint32_t* out4) {
     g_last_error.clear();
     if (!s || !out4 || s->phase != 4) { set_error("cheetah_decode_shard_status: null pointer / phase 3 not done"); return DENSITY_B200_EARG; }
@@ -1795,9 +1845,11 @@ static size_t cheetah_piece_extra_bytes(const density_b200_sharded* h) {
 // rank issues the same collectives in the same order whatever its piece holds: an empty piece sends identity transfers and zero words, a
 // refused one keeps exchanging until the verdict. The rounds after the settled one are gated off on the device; their all-gathers still
 // run. first: the piece holds the stream start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output
-// starts, from the verdict's prefix offsets. x is opened with cheetah_piece_extra_bytes.
+// starts, from the verdict's prefix offsets. x is opened with cheetah_piece_extra_bytes. prot: a piece of a stream with copy-mode blocks
+// (density_b200_decode_sharded_cheetah_protected): phase 1 is the protection transfer -> ncclAllGather(transfers) -> prot_phase1, and x
+// holds the gathered transfers behind the buffers of cheetah_piece_extra_bytes.
 static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
-                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) {
+                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot) {
     density_b200_sharded* h = x.h;
     cudaStream_t st = x.st;
     density_b200_cheetah_decode_shard* s = h->cdec;
@@ -1810,7 +1862,17 @@ static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, 
     uint32_t* rwords = carry_p + wp;                                      // [world][4]
     uint64_t launches = 0;
     // the last piece's transfers are never read: it sends what its slot holds
-    int rc = density_b200_cheetah_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, last ? nullptr : tab_c + R * wc, st);
+    uint32_t* cmap_out = last ? nullptr : tab_c + R * wc;
+    int rc;
+    if (prot) {
+        uint32_t* transfers = reinterpret_cast<uint32_t*>(x.extra + cheetah_piece_extra_bytes(h));   // [world][DECODE_PROT_TRANSFER_WORDS]
+        rc = density_b200_cheetah_decode_shard_prot_transfer(s, d_in, n, d_out, cap, first, last, transfers + R * DECODE_PROT_TRANSFER_WORDS, st);
+        if (rc != DENSITY_B200_OK) return rc;
+        if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        rc = density_b200_cheetah_decode_shard_prot_phase1(s, transfers, (int)W, (int)R, cmap_out, st);
+    } else {
+        rc = density_b200_cheetah_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, cmap_out, st);
+    }
     if (rc != DENSITY_B200_OK) return rc;
     if (!x.gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
     cudaError_t e = first ? cudaSuccess : chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
@@ -1837,7 +1899,22 @@ int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* 
     int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h))) != DENSITY_B200_OK) return rc;
-    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr);
+    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
+                                        false);
+}
+
+// The inverse of density_b200_encode_sharded_cl_protected (Cheetah) for any stream: the pieces' protection transfers are exchanged first,
+// then everything runs as density_b200_decode_sharded_cheetah.
+int density_b200_decode_sharded_cheetah_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                                  uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK ||
+        (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h) + (size_t)h->world * DECODE_PROT_TRANSFER_WORDS * sizeof(uint32_t))) != DENSITY_B200_OK)
+        return rc;
+    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
+                                        true);
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
@@ -1984,7 +2061,7 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
     rc = density_b200_cheetah_locate_piece(h->h_maps, h->world, h->rank, piece);
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
     return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
-                                        d_flags, d_total_size, d_out_offset);
+                                        d_flags, d_total_size, d_out_offset, false);
 }
 
 /* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag

@@ -416,30 +416,13 @@ __global__ void dec_carry_scan(const uint32_t* __restrict__ final_tab, uint32_t 
 }
 
 // ---- 4. tail loop (codec.rs:102-123), one thread, literal control flow ---------------------------------------------------
-// The automaton state behind the main loop: dec_seq_walk's, or (quiet: penalty 0 throughout) the entry state jumped over the main
-// blocks. Entry state: protection_state.rs:9-16, or the seed of a piece of a sharded stream.
-__device__ __forceinline__ Protection main_end_state(const DecStatus* __restrict__ st) {
-    Protection ps; ps.init();
-    if (st->seeded) { ps.copy_penalty = st->in_penalty; ps.copy_penalty_start = st->in_start; ps.previous_incompressible = st->in_prev; ps.counter = st->in_phase; }
-    if (st->seq) {
-        ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev;
-        ps.counter += st->main_blocks;
-    } else if (st->main_blocks) {
-        const uint64_t k = (ps.counter + st->main_blocks + 15) / 16 - (ps.counter + 15) / 16;
-        if (ps.copy_penalty_start > 1) { const uint32_t sh = k > 8 ? 8u : (uint32_t)k; const uint32_t v = ps.copy_penalty_start >> sh; ps.copy_penalty_start = v ? v : 1u; }
-        ps.counter += st->main_blocks;
-        ps.previous_incompressible = st->last_main_inc;
-    }
-    return ps;
-}
-
 __global__ void dec_tail(const uint8_t* __restrict__ in, uint64_t n, uint8_t* __restrict__ out, uint64_t cap, uint32_t* __restrict__ dict,
                          DecStatus* __restrict__ st, uint64_t* __restrict__ d_out_size) {
     if (threadIdx.x || blockIdx.x) return;
     if (st->nonquiet) { if (d_out_size) *d_out_size = 0; return; }   // gave up: the caller's in-order fallback (queued behind) produces the result
     if (st->error) { st->out_bytes = 0; if (d_out_size) *d_out_size = 0; return; }
     uint64_t idx = st->tail_off, oidx = st->main_blocks * 256;
-    Protection ps = main_end_state(st);
+    Protection ps = bounds::main_end_state(st);
     bool bad = false, overflow = false;
     auto emit = [&](uint32_t q) {
         if (oidx + 4 > cap) { overflow = true; return; }
@@ -511,7 +494,7 @@ template <class F>
 __device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
     TailWalk w; w.blocks = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
     Protection& ps = w.ps;
-    ps = main_end_state(st);
+    ps = bounds::main_end_state(st);
     uint64_t idx = st->tail_off;
     while (n - idx > 0) {
         ++w.blocks;
@@ -593,16 +576,7 @@ __global__ void dec_seam_words_k(const uint8_t* __restrict__ in, uint64_t n, con
 }
 
 // ---- 6. sharded decode of a stream with copy-mode blocks (density_b200_decode_shard_prot_*, DESIGN §5) ----------------------------------
-// The incoming state of piece `rank`: the transfers of the pieces before it (dec_prot_transfer) composed from candidate 0, the stream
-// start. A path that meets PT_ESC or PT_NOEND refuses the piece; the kernels then run from the stream-start state, harmlessly.
-__global__ void dec_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t* __restrict__ seed) {
-    if (threadIdx.x || blockIdx.x) return;
-    uint32_t x = 0;
-    for (uint32_t r = 0; r < rank && x < bounds::PT_NCAND; ++r) x = all_transfers[(size_t)r * bounds::PT_NCAND + x];
-    const uint32_t refused = x < bounds::PT_NCAND ? 0u : 1u;
-    const uint32_t s = bounds::pt_state(refused ? 0u : x);
-    seed[0] = s & 0xFFu; seed[1] = (s >> 8) & 0xFFu; seed[2] = (s >> 16) & 1u; seed[3] = s >> 17; seed[4] = refused;
-}
+// The incoming state of a piece comes from bounds::dec_prot_enter_k (decode_bounds.cuh).
 // The seam words of such a piece, in the layout of dec_seam_words_k. Copy-mode blocks, a pending penalty and incompressible blocks meet
 // at the cuts legally here (the transfers carry the automaton across), so words 0 and 1 stay 0. Word 2: the transfers composed to no
 // state, an error (malformed, output beyond cap), or a non-final piece that does not decode to whole 256-byte blocks. st == nullptr:
@@ -725,7 +699,7 @@ cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t
     return cudaGetLastError();
 }
 cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches) {
-    dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
+    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
     ++*launches;
     return cudaGetLastError();
 }

@@ -374,24 +374,31 @@ struct PieceStatus { unsigned int refuse, first_inc, last_inc, tail_blocks, pad[
 // The end of the piece, right after the boundary walk. A non-final piece is followed by more stream bytes, so the reference decodes all of
 // its blocks in the main loop (codec.rs:88-100); the blocks the boundary walk left to the tail (those starting in the last 136 bytes) are
 // appended to the block list. Their control flow does not depend on the tables. The final piece keeps its in-order tail; its control flow
-// is walked here for the seam words. Refused (pst->refuse): a piece > 0 that is not quiet (copy mode, two consecutive incompressible
-// blocks); a non-final piece that meets copy mode at its end, ends with a copy penalty pending or inside a copy run, or whose blocks do
-// not end exactly at its last byte.
-__global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, int first, int last, DecStatus* __restrict__ st,
+// is walked here for the seam words. The automaton starts from the state behind the main loop (bounds::main_end_state: the piece's seed
+// carried over its main blocks). Refused (pst->refuse): a non-final piece whose blocks do not end exactly at its last byte or that reads a
+// malformed block; and, unless `prot`, a piece > 0 that is not quiet (copy mode, two consecutive incompressible blocks) or a non-final
+// piece that meets copy mode at its end, ends with a copy penalty pending or inside a copy run. prot: a piece of the protected path
+// (density_b200_cheetah_decode_shard_prot_*), whose seed carries the automaton across the cuts, so the blocks at its end may be copy-mode
+// blocks (appended with BLK_COPY) and it may end in any automaton state.
+__global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, int first, int last, int prot, DecStatus* __restrict__ st,
                              uint64_t* __restrict__ blk_off, uint64_t maxblocks, PieceStatus* __restrict__ pst) {
     if (threadIdx.x || blockIdx.x) return;
     auto sig_at = [&](uint64_t o) { uint64_t s = 0; for (int i = 0; i < 8; ++i) s |= (uint64_t)in[o + i] << (8 * i); return s; };
     if (st->error) { pst->refuse = 1; pst->first_inc = 0; pst->last_inc = 0; pst->tail_blocks = 0; return; }
-    uint32_t refuse = (!first && st->seq) ? 1u : 0u;             // dec_seq_walk ran: two consecutive incompressible blocks in the main loop
-    Protection ps; ps.init();
-    ps.counter = st->main_blocks; ps.previous_incompressible = st->last_main_inc;
-    if (st->seq) { ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev; }
+    uint32_t refuse = (!prot && !first && st->seq) ? 1u : 0u;    // dec_seq_walk ran: two consecutive incompressible blocks in the main loop
+    Protection ps = bounds::main_end_state(st);
     uint64_t idx = st->tail_off, b = st->main_blocks;
     uint32_t tail_first = 0, tail_blocks = 0;
     if (!last) {
         bool bad = false, ends_copy = b > 0 && (blk_off[b - 1] & BLK_COPY);
         while (idx < n) {
-            if (ps.revert_to_copy()) { bad = true; break; }       // copy mode at the end of a non-final piece
+            if (ps.revert_to_copy()) {                             // codec.rs:89-92
+                if (!prot || n - idx < 128) { bad = true; break; } // quiet path: copy mode at the end of a non-final piece
+                if (b < maxblocks) blk_off[b] = idx | BLK_COPY; else st->error = 2;
+                ++b; ++tail_blocks; idx += 128; ends_copy = true;
+                ps.decay();
+                continue;
+            }
             if (n - idx < 8) { bad = true; break; }
             const uint32_t consumed = cld::cheetah_block_bytes(sig_at(idx));
             if (consumed > n - idx) { bad = true; break; }         // the block runs past the piece
@@ -399,9 +406,10 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
             ++b; ++tail_blocks; idx += consumed; ends_copy = false;
             ps.update(consumed >= 128);                            // codec.rs:94-98
         }
-        if (bad || ends_copy || ps.copy_penalty) refuse = 1;
+        if (bad || (!prot && (ends_copy || ps.copy_penalty))) refuse = 1;
         if (!bad) {
             st->main_blocks = b; st->tail_off = idx; st->last_main_inc = ps.previous_incompressible;
+            if (prot) st->seq = 1;                                 // main_end_state reads the state below from now on
             if (st->seq) { st->ps_penalty = ps.copy_penalty; st->ps_start = ps.copy_penalty_start; st->ps_prev = ps.previous_incompressible; }
         }
         if (b * 128 > cap) st->error = 2;
@@ -434,7 +442,7 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
             pair |= inc & ps.previous_incompressible;
             ps.update(inc);
         }
-        if (!first && (copied || pair)) refuse = 1;
+        if (!prot && !first && (copied || pair)) refuse = 1;
     }
     const uint64_t b0 = blk_off[0];
     pst->first_inc = st->main_blocks ? ((!(b0 & BLK_COPY) && cld::cheetah_block_bytes(sig_at(b0)) >= 128) ? 1u : 0u) : tail_first;
@@ -562,14 +570,21 @@ __global__ void cd_shard_round_end(ClStatus* __restrict__ cs, uint32_t nruns, ui
     if (walked == 0) cs->done = 1;
 }
 // the piece's 8 seam words in the layout of the Chameleon decoder's (after the tail): {first block incompressible, previous_incompressible
-// at the end, refused, has blocks, decoded size lo, hi, 0, 0}
+// at the end, refused, has blocks, decoded size lo, hi, 0, 0}. seed (the protected path, nullptr otherwise): the piece's incoming state
+// (bounds::dec_prot_enter_k); words 0 and 1 are then 0, since incompressible blocks may meet at a cut when the transfers carry the
+// automaton across it, and the piece is also refused when the transfers composed to no state. pst == nullptr: an empty piece of the
+// protected path (no blocks, size 0), refused only by its seed.
 __global__ void cd_seam_words(const PieceStatus* __restrict__ pst, const uint32_t* __restrict__ fallback, const Status* __restrict__ tail_status,
-                              int is_last, const uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
+                              int is_last, const uint32_t* __restrict__ seed, uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
     if (threadIdx.x || blockIdx.x) return;
-    const uint64_t sz = *d_out_size;
-    uint32_t bad = (pst->refuse || *fallback || tail_status->error) ? 1u : 0u;
-    if (!is_last && (sz % 128)) bad = 1;
-    words[0] = pst->first_inc; words[1] = pst->last_inc; words[2] = bad; words[3] = 1;
+    uint64_t sz = 0;
+    uint32_t bad = seed ? seed[4] : 0u;
+    if (pst) {
+        sz = *d_out_size;
+        if (pst->refuse || *fallback || tail_status->error) bad = 1;
+        if (!is_last && (sz % 128)) bad = 1;
+    } else *d_out_size = 0;
+    words[0] = pst && !seed ? pst->first_inc : 0u; words[1] = pst && !seed ? pst->last_inc : 0u; words[2] = bad; words[3] = pst ? 1u : 0u;
     words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
 }
 
@@ -732,13 +747,14 @@ size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
 
 // Phase 1: boundaries (piece 0 may use copy mode: dec_seq_walk from the fresh automaton), the end of the piece, unpack (literals and
 // copy-mode blocks go straight to d_out), the symbolic chunk-map walk and the piece's chunk-map transfer (d_cmap_out, may be null).
-cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches) {
+// d_seed (the protected path, nullptr otherwise): the piece's incoming state, after chee_shard_prot_transfer filled the candidate rows.
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed) {
     const CheeDecPtrs p = chee_shard_ptrs(a);
-    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches);
+    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, d_seed != nullptr);
     if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
     if (e != cudaSuccess) return e;
-    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
+    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
     ++*launches;
     cd_launch_unpack_walk(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
     if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
@@ -774,13 +790,51 @@ cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const 
 }
 
 // Phase 3: the verdict of the rounds, the final piece's tail from the folded tables (the tail of a non-final piece is empty), the size
-// and the seam words.
-cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
+// and the seam words (d_seed: the protected path's, see cd_seam_words). An empty piece of the protected path has its seam words only.
+cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                              const uint32_t* d_seed) {
+    if (!a.n) {
+        cd_seam_words<<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+        ++*launches;
+        return cudaGetLastError();
+    }
     const CheeDecPtrs p = chee_shard_ptrs(a);
     cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
     cudaError_t e = scalar_decode_tail(ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
     if (e != cudaSuccess) return e;
-    cd_seam_words<<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_out_size, d_seam8);
+    cd_seam_words<<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// The protected path's first step on a piece (DESIGN.md section 5): the candidate rows of the boundary walk (they stay in the workspace
+// for chee_shard_phase1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing.
+cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    static bool attr_done = false;
+    if (!attr_done) {
+        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                    (int)bounds::prot_transfer_smem<T>());
+        if (e0 != cudaSuccess) return e0;
+        attr_done = true;
+    }
+    uint32_t* res = nullptr;
+    uint4* gres = nullptr;
+    if (a.n) {
+        const CheeDecPtrs p = chee_shard_ptrs(a);
+        res = reinterpret_cast<uint32_t*>(a.ws + p.B.res);
+        gres = reinterpret_cast<uint4*>(a.ws + p.B.gres);
+        const uint32_t nchunks = (uint32_t)((a.n + T::CH - 1) / T::CH);
+        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(a.d_in, a.n, nchunks, res);
+        bounds::dec_group_compose<T><<<(nchunks + bounds::GROUP - 1) / bounds::GROUP, 160, 0, stream>>>(res, nchunks, gres);
+        *launches += 2;
+    }
+    bounds::dec_prot_transfer<T><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(a.d_in, a.n, a.last ? 1 : 0, res, gres, d_transfer);
+    ++*launches;
+    return cudaGetLastError();
+}
+// The incoming state of piece `rank` composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
+cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches) {
+    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
     ++*launches;
     return cudaGetLastError();
 }

@@ -590,6 +590,36 @@ dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const
 }
 template <class T> constexpr size_t prot_transfer_smem() { return T::CH + 16 + sizeof(PtSmem); }
 
+// The incoming state of piece `rank` (SEED_WORDS): the transfers of the pieces before it (dec_prot_transfer, [rank][PT_NCAND]) composed
+// from candidate 0, the stream start. A path that meets PT_ESC or PT_NOEND refuses the piece; the kernels then run from the stream-start
+// state, harmlessly. Static: every decoder's translation unit launches its own copy.
+static __global__ void dec_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t* __restrict__ seed) {
+    if (threadIdx.x || blockIdx.x) return;
+    uint32_t x = 0;
+    for (uint32_t r = 0; r < rank && x < PT_NCAND; ++r) x = all_transfers[(size_t)r * PT_NCAND + x];
+    const uint32_t refused = x < PT_NCAND ? 0u : 1u;
+    const uint32_t s = pt_state(refused ? 0u : x);
+    seed[0] = s & 0xFFu; seed[1] = (s >> 8) & 0xFFu; seed[2] = (s >> 16) & 1u; seed[3] = s >> 17; seed[4] = refused;
+}
+
+// The automaton state behind the main loop: dec_seq_walk's, or (quiet: penalty 0 throughout) the entry state jumped over the main
+// blocks. Entry state: protection_state.rs:9-16, or the seed of a piece of a sharded stream. Unseeded, this is counter = main_blocks,
+// start 1 and the last main block's incompressible bit (or dec_seq_walk's state).
+__device__ __forceinline__ Protection main_end_state(const DecStatus* __restrict__ st) {
+    Protection ps; ps.init();
+    if (st->seeded) { ps.copy_penalty = st->in_penalty; ps.copy_penalty_start = st->in_start; ps.previous_incompressible = st->in_prev; ps.counter = st->in_phase; }
+    if (st->seq) {
+        ps.copy_penalty = st->ps_penalty; ps.copy_penalty_start = st->ps_start; ps.previous_incompressible = st->ps_prev;
+        ps.counter += st->main_blocks;
+    } else if (st->main_blocks) {
+        const uint64_t k = (ps.counter + st->main_blocks + 15) / 16 - (ps.counter + 15) / 16;
+        if (ps.copy_penalty_start > 1) { const uint32_t sh = k > 8 ? 8u : (uint32_t)k; const uint32_t v = ps.copy_penalty_start >> sh; ps.copy_penalty_start = v ? v : 1u; }
+        ps.counter += st->main_blocks;
+        ps.previous_incompressible = st->last_main_inc;
+    }
+    return ps;
+}
+
 // ---- host side: workspace layout + launch sequence ---------------------------------------------------------------------------------
 struct BoundsLayout { size_t status, res, gres, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, total; uint64_t maxblocks; };
 

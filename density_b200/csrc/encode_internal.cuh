@@ -189,12 +189,19 @@ const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int n
 struct CheeShardArgs { const uint8_t* d_in; size_t n; uint8_t* d_out; size_t cap; bool first, last; uint8_t* ws; uint8_t* tables; int num_sms; };
 size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
 uint32_t chee_shard_max_rounds();
-cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches);
+// d_seed (may be NULL): the piece's incoming automaton state (chee_shard_prot_enter), after chee_shard_prot_transfer on the same workspace
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr);
 cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
                                   uint32_t rank, cudaStream_t stream, uint64_t* launches);
-cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches);
+// (d_seed: the same seed, whose seam words do not refuse incompressible blocks at the cuts; n == 0 is allowed there)
+cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                              const uint32_t* d_seed = nullptr);
+// a piece of a stream with copy-mode blocks: its protection transfer (DECODE_PROT_TRANSFER_WORDS; fills the candidate rows of the workspace
+// first) and its incoming state composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), for chee_shard_phase1
+cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches);
 const void* chee_shard_status_ptr(const CheeShardArgs& a);
 cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);

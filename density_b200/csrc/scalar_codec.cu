@@ -8,6 +8,7 @@
 // Stream/driver semantics follow codec/codec.rs:34-126 and codec/protection_state.rs:9-47.
 #include "common.cuh"
 #include "encode_internal.cuh"
+#include "decode_bounds.cuh"
 
 namespace dns {
 namespace scalar {
@@ -246,23 +247,20 @@ __global__ void decode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint8_
     if (last_hash_io) *last_hash_io = D.last_hash;
 }
 
-// the boundary status block of decode_bounds.cuh and the iteration status of cl_decode.cu, as far as the tail needs them
-struct TailBounds { unsigned long long out_bytes, main_blocks, tail_off; unsigned int nonquiet, error, last_main_inc, seq, ps_penalty, ps_start, ps_prev, pad; };
+// the iteration status of cl_decode.cu, as far as the tail needs it
 struct TailIter { unsigned int changed, unknown, done, rounds, final_ctx, gave_up, pad0, pad1; };
 
 // Tail loop only, continuing where the parallel main loop stopped (tables = what the folds left in the workspace).
 template <int ALG>
 __global__ void decode_tail_kernel(const uint8_t* __restrict__ in, uint64_t n, uint8_t* __restrict__ out, uint64_t cap, Tables T,
-                                   Status* __restrict__ status, const TailBounds* __restrict__ tb, const TailIter* __restrict__ ti,
+                                   Status* __restrict__ status, const bounds::DecStatus* __restrict__ tb, const TailIter* __restrict__ ti,
                                    uint64_t* __restrict__ d_out_size, const uint32_t* __restrict__ skip_if) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     if (skip_if && *skip_if != 0) return;   // the parallel decoder gave up: the in-order kernel (queued behind) does everything
     constexpr uint32_t B = ALG == ALG_CHAMELEON ? 256 : ALG == ALG_CHEETAH ? 128 : 64;
     Dec<ALG> D; D.T = T; D.in = in; D.n = n; D.out = out; D.cap = cap;
     D.idx = tb->tail_off; D.oidx = tb->main_blocks * B; D.last_hash = ti->final_ctx;
-    Protection ps; ps.init();
-    ps.counter = tb->main_blocks; ps.previous_incompressible = tb->last_main_inc;   // quiet main loop: penalty 0, start 1
-    if (tb->seq) { ps.copy_penalty = tb->ps_penalty; ps.copy_penalty_start = tb->ps_start; ps.previous_incompressible = tb->ps_prev; }
+    Protection ps = bounds::main_end_state(tb);   // the entry state of a piece of a sharded stream, carried over the main loop
     decode_loops<ALG>(D, ps, false);
     uint64_t res = D.oidx;
     if (D.bad) { status->error = 3; res = 0; }
@@ -326,7 +324,7 @@ cudaError_t scalar_decode_tail(int alg, const uint8_t* d_in, size_t nbytes, uint
     if (alg != ALG_CHEETAH) return cudaErrorInvalidValue;
     scalar::Tables T = carve(alg, ws);   // the folds of cl_decode.cu have filled chunk_a / chunk_b / pred
     Status* st = reinterpret_cast<Status*>(ws);
-    scalar::decode_tail_kernel<ALG_CHEETAH><<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, T, st, reinterpret_cast<const scalar::TailBounds*>(d_bounds_status),
+    scalar::decode_tail_kernel<ALG_CHEETAH><<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, T, st, reinterpret_cast<const bounds::DecStatus*>(d_bounds_status),
                                                                   reinterpret_cast<const scalar::TailIter*>(d_cl_status), d_out_size, d_skip_if);
     ++*launches;
     return cudaGetLastError();

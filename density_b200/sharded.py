@@ -31,6 +31,8 @@ ranks and exchanges the automaton transfers and 8 round words (which carry each 
 A sharded Cheetah stream decodes the same way in pieces (ShardedDecoder.decode(..., alg="cheetah"), or the piece phases
 density_b200_cheetah_decode_shard_* with fold_cheetah_cmap and fold_cl_tables for the exchanges): the chunk-map transfers are
 exchanged once, then every prediction round exchanges each piece's prediction transfer and 4 round words, for a fixed budget of rounds.
+Pieces with copy-mode blocks (ShardedDecoder.decode_protected(..., alg="cheetah"), or density_b200_cheetah_decode_shard_prot_transfer and
+_prot_phase1 in place of phase 1) first exchange their protection transfers, as Chameleon's do.
 
 A stream whose cuts are not known (one chameleon_encode call, the reference library, a file) is cut at byte ranges instead
 (`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
@@ -599,12 +601,17 @@ class ShardedDecoder(_ShardedHandle):
         _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
                   self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}")
 
-    def decode_protected(self, d_in, d_out, d_size, d_flags):
+    def decode_protected(self, d_in, d_out, d_size, d_flags, alg="chameleon"):
         """density_b200_decode_sharded_protected: the Chameleon pieces of any stream, copy-mode blocks included (the inverse of
-        ShardedEncoder.encode_protected), with the arguments of decode. Enqueued on torch's current stream; nothing blocks."""
-        _check(self._lib.density_b200_decode_sharded_protected(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(),
-                                                               d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), _stream()),
-               "decode_sharded_protected")
+        ShardedEncoder.encode_protected), with the arguments of decode. Enqueued on torch's current stream; nothing blocks. alg
+        "cheetah" (or its id): the Cheetah pieces of any stream (density_b200_decode_sharded_cheetah_protected, the inverse of
+        ShardedEncoder.encode_protected(..., alg="cheetah"))."""
+        alg = _alg_id(alg)
+        if alg not in (0, 1):
+            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+        fn = self._lib.density_b200_decode_sharded_protected if alg == 0 else self._lib.density_b200_decode_sharded_cheetah_protected
+        _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
+                  self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}_protected")
 
     def decode_stream(self, d_in, n_range, d_out, d_size, d_flags, alg="chameleon", range_offset=None):
         """Decode of a stream without known cuts (`density_b200_decode_sharded_stream`). d_in: this rank's range (its first n_range

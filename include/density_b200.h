@@ -476,6 +476,33 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah(density_b200_sharded*, 
                                         uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
+ * Sharded Cheetah decode of streams with copy-mode blocks (DESIGN.md section 5): the inverse of density_b200_encode_sharded_cl_protected
+ * (Cheetah), and of the slices of a single-call cheetah_encode stream at its pieces' prefix sums, whatever the data. Copy mode, a pending
+ * penalty, a cut inside a copy run and incompressible blocks on both sides of a cut are all accepted. As for Chameleon
+ * (density_b200_decode_shard_prot_transfer), every piece first exports its TRANSFER, DENSITY_B200_DECODE_PROT_TRANSFER_WORDS u32 in the
+ * same candidate encoding with the same 0xFFFF / 0xFFFE meaning; the final piece's is all 0xFFFE, an empty piece's the identity.
+ *   prot_transfer  boundary rows of the piece and its transfer; the arguments of density_b200_cheetah_decode_shard_phase1 otherwise
+ *   prot_phase1    the transfers of the pieces before `rank` (d_all_transfers: [world][DENSITY_B200_DECODE_PROT_TRANSFER_WORDS], may be
+ *                  NULL for rank 0) composed from candidate 0 give the incoming state; then what density_b200_cheetah_decode_shard_phase1
+ *                  does, from that state, with the chunk-map transfer to d_cmap_out (may be NULL)
+ * The piece then runs phase 2, the rounds and phase 3 of the quiet path unchanged. Its phase 3 writes the seam words in their layout, with
+ * words 0 and 1 = 0 and word 2 set when the composition met 0xFFFF or 0xFFFE, the piece is malformed or its output exceeds cap, the
+ * rounds did not settle, the tail reported an error, or a non-final piece does not decode to whole 128-byte blocks. prot_transfer ->
+ * prot_phase1 -> phase 2 -> rounds -> phase 3 in this order per piece (a quiet phase 1 in between closes the protected sequence);
+ * otherwise DENSITY_B200_EARG. d_in must be 2-byte, d_out and the transfers 4-byte aligned. Nothing is written past cap.
+ */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_prot_transfer(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n,
+                                                    uint8_t* d_out, size_t cap, int is_first, int is_last, uint32_t* d_transfer_out,
+                                                    void* stream);
+DENSITY_B200_API int density_b200_cheetah_decode_shard_prot_phase1(density_b200_cheetah_decode_shard*, const uint32_t* d_all_transfers, int world,
+                                                  int rank, uint32_t* d_cmap_out, void* stream);
+/* End to end over NCCL, the arguments and semantics of density_b200_decode_sharded_cheetah for any stream: prot_transfer ->
+   ncclAllGather(transfers, 12.5 KiB per rank) -> prot_phase1 -> the rest of density_b200_decode_sharded_cheetah. Never blocks; uses its
+   own workspace in the handle. */
+DENSITY_B200_API int density_b200_decode_sharded_cheetah_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out,
+                                                  size_t cap, uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
  * Sharded decode of a stream whose cuts are not known: a stream written by one chameleon_encode call, by the reference library,
  * read from a file, or a gathered sharded stream without its piece sizes. The stream is cut at byte ranges; each rank finds
  * where its piece starts from the stream itself.

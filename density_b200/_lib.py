@@ -113,6 +113,20 @@ _SIGS = {
     "density_b200_decode_sharded_cheetah_stream": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint64, _c_u8p,
                                                                   ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                                                   ctypes.c_void_p]),
+    "density_b200_decode_prot_locate": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_prot_locate": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p,
+                                                               ctypes.c_void_p]),
+    "density_b200_prot_locate_piece": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]),
+    "density_b200_decode_shard_prot_enter": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int,
+                                                            ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_cheetah_decode_shard_prot_enter": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                    ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded_stream_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, _c_u8p,
+                                                                    ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                                                    ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded_cheetah_stream_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, _c_u8p,
+                                                                            ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                                                            ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_codec_create": (ctypes.c_void_p, [ctypes.c_int]),
     "density_b200_codec_destroy": (None, [ctypes.c_void_p]),
     "density_b200_codec_clear_state": (ctypes.c_int, [ctypes.c_void_p]),

@@ -9,6 +9,7 @@
 #include "../../include/density_b200.h"
 #include "common.cuh"
 #include "encode_internal.cuh"
+#include "decode_bounds.cuh"
 
 #include <dlfcn.h>
 
@@ -1109,23 +1110,42 @@ int density_b200_decode_shard_prot_transfer(density_b200_decode_shard* s, const 
     if (rc == DENSITY_B200_OK) s->prot_stage = 1;
     return rc;
 }
+// The protected phase 1 of the piece set up in s, from the seed composed from candidate x0 and the transfers of the pieces before `rank`
+// (prot_phase1: x0 = 0, the rows of prot_transfer ready; prot_enter: a located piece's candidate, no transfers, the rows not computed yet).
+static int decode_prot_phase1_body(density_b200_decode_shard* s, const uint32_t* d_all_transfers, int rank, uint32_t x0, bool rows_ready,
+                                   uint32_t* d_table_out, cudaStream_t st, const char* what) {
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    cudaError_t e = cham_decode_prot_enter(d_all_transfers, (uint32_t)rank, x0, seed, st, &launches);
+    if (e == cudaSuccess) {
+        if (s->n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
+        else e = cham_decode_phase1(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, d_table_out, st, &launches, seed, rows_ready);
+    }
+    const int rc = step_result(e, launches, what);
+    s->prot_stage = rc == DENSITY_B200_OK ? 2 : 0;
+    return rc;
+}
 int density_b200_decode_shard_prot_phase1(density_b200_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
                                           uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
     if (!s || s->prot_stage != 1) { set_error("decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers) || !d_table_out) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
     if (!al4(d_all_transfers) || !al4(d_table_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    return decode_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_table_out, reinterpret_cast<cudaStream_t>(stream), "decode shard prot phase1");
+}
+int density_b200_decode_shard_prot_enter(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                         uint32_t candidate, uint32_t* d_table_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_table_out)) { set_error("d_in must be 2-byte, d_table_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
-    uint64_t launches = 0;
-    cudaError_t e = cham_decode_prot_enter(d_all_transfers, (uint32_t)rank, seed, st, &launches);
-    if (e == cudaSuccess) {
-        if (s->n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
-        else e = cham_decode_phase1(s->d_in, s->n, s->cap, s->ws.p, s->num_sms, d_table_out, st, &launches, seed);
-    }
-    const int rc = step_result(e, launches, "decode shard prot phase1");
-    s->prot_stage = rc == DENSITY_B200_OK ? 2 : 0;
-    return rc;
+    s->phase1_done = false; s->prot_stage = 0;
+    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
+    if (e == cudaSuccess) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    return decode_prot_phase1_body(s, nullptr, 0, candidate, false, d_table_out, st, "decode shard prot enter");
 }
 int density_b200_decode_shard_prot_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
                                           uint32_t* d_seam8, void* stream) {
@@ -1267,24 +1287,50 @@ int density_b200_cheetah_decode_shard_prot_transfer(density_b200_cheetah_decode_
     if (rc == DENSITY_B200_OK) s->transfer_done = true;
     return rc;
 }
+// The protected phase 1 of the piece set up in s->a (see decode_prot_phase1_body)
+static int cheetah_prot_phase1_body(density_b200_cheetah_decode_shard* s, const uint32_t* d_all_transfers, int rank, uint32_t x0, bool rows_ready,
+                                    uint32_t* d_cmap_out, cudaStream_t st, const char* what) {
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    s->transfer_done = false;   // one phase 1 per transfer
+    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, x0, seed, st, &launches);
+    if (e == cudaSuccess) {
+        if (s->a.n) e = chee_shard_phase1(s->a, d_cmap_out, st, &launches, seed, rows_ready);
+        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    }
+    const int rc = step_result(e, launches, what);
+    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
+    return rc;
+}
 int density_b200_cheetah_decode_shard_prot_phase1(density_b200_cheetah_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
                                                   uint32_t* d_cmap_out, void* stream) {
     g_last_error.clear();
     if (!s || !s->transfer_done || s->phase != 0) { set_error("cheetah_decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
     if (!al4(d_all_transfers) || !al4(d_cmap_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
-    uint64_t launches = 0;
-    s->transfer_done = false;   // one phase 1 per transfer
-    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, seed, st, &launches);
-    if (e == cudaSuccess) {
-        if (s->a.n) e = chee_shard_phase1(s->a, d_cmap_out, st, &launches, seed);
-        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    return cheetah_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_cmap_out, reinterpret_cast<cudaStream_t>(stream),
+                                    "cheetah decode shard prot phase1");
+}
+int density_b200_cheetah_decode_shard_prot_enter(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                                 int is_first, int is_last, uint32_t candidate, uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_cmap_out)) {
+        set_error("d_in must be 2-byte, d_out and d_cmap_out 4-byte aligned"); return DENSITY_B200_EARG;
     }
-    const int rc = step_result(e, launches, "cheetah decode shard prot phase1");
-    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
-    return rc;
+    if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("cheetah_decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
+    CheeShardArgs& a = s->a;
+    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
+    cudaError_t e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
+    if (n) {
+        if (e == cudaSuccess) e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
+        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
+    }
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    a.ws = s->ws.p; a.tables = s->tables.p;
+    return cheetah_prot_phase1_body(s, nullptr, 0, candidate, false, d_cmap_out, st, "cheetah decode shard prot enter");
 }
 
 int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard* s, uint32_t* out4) {
@@ -1786,18 +1832,24 @@ static int decode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, siz
 // The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it: phase 1 -> table exchange ->
 // fold -> phase 2 -> seam words -> verdict. is_last: the piece ends the stream (a non-final piece must decode to whole 256-byte blocks).
 // d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
+// cand >= 0: a located piece of a stream with copy-mode blocks (density_b200_decode_sharded_stream_protected), entered in that candidate:
+// prot_enter and prot_phase2 on the handle's protected decode shard take the place of the two phases.
 static int decode_sharded_piece(const Exchange& x, const uint8_t* d_in, size_t n, int is_last, uint8_t* d_out, size_t cap,
-                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) {
-    density_b200_decode_shard* s = x.h->dec;
+                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, int64_t cand = -1) {
+    density_b200_decode_shard* s = cand < 0 ? x.h->dec : x.h->pdec;
+    uint32_t* my_table = x.tables + (size_t)x.h->rank * 65536;
     // phase 1: boundaries and writer pass need no carry-in; the piece's table (runs + tail) lands in my slot of the gather buffer
-    int rc = density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, x.tables + (size_t)x.h->rank * 65536, x.st);
+    int rc = cand < 0 ? density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, my_table, x.st)
+                      : density_b200_decode_shard_prot_enter(s, d_in, n, cap, is_last, (uint32_t)cand, my_table, x.st);
     if (rc != DENSITY_B200_OK) return rc;
     if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
     const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)x.h->rank, x.carry, x.st, &launches);
     if ((rc = step_result(e, launches, "sharded decode fold")) != DENSITY_B200_OK) return rc;
     // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
-    if ((rc = density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)) != DENSITY_B200_OK) return rc;
+    rc = cand < 0 ? density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)
+                  : density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st);
+    if (rc != DENSITY_B200_OK) return rc;
     return x.verdict(d_flags, d_total_size, d_out_offset);
 }
 
@@ -1847,9 +1899,11 @@ static size_t cheetah_piece_extra_bytes(const density_b200_sharded* h) {
 // run. first: the piece holds the stream start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output
 // starts, from the verdict's prefix offsets. x is opened with cheetah_piece_extra_bytes. prot: a piece of a stream with copy-mode blocks
 // (density_b200_decode_sharded_cheetah_protected): phase 1 is the protection transfer -> ncclAllGather(transfers) -> prot_phase1, and x
-// holds the gathered transfers behind the buffers of cheetah_piece_extra_bytes.
+// holds the gathered transfers behind the buffers of cheetah_piece_extra_bytes. cand >= 0 (prot false): a located piece of a stream with
+// copy-mode blocks (density_b200_decode_sharded_cheetah_stream_protected), whose phase 1 is prot_enter from that candidate.
 static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
-                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot) {
+                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot,
+                                        int64_t cand = -1) {
     density_b200_sharded* h = x.h;
     cudaStream_t st = x.st;
     density_b200_cheetah_decode_shard* s = h->cdec;
@@ -1870,6 +1924,8 @@ static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, 
         if (rc != DENSITY_B200_OK) return rc;
         if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
         rc = density_b200_cheetah_decode_shard_prot_phase1(s, transfers, (int)W, (int)R, cmap_out, st);
+    } else if (cand >= 0) {
+        rc = density_b200_cheetah_decode_shard_prot_enter(s, d_in, n, d_out, cap, first, last, (uint32_t)cand, cmap_out, st);
     } else {
         rc = density_b200_cheetah_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, cmap_out, st);
     }
@@ -2062,6 +2118,139 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
     return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
                                         d_flags, d_total_size, d_out_offset, false);
+}
+
+// ---- sharded decode of a stream without known cuts, copy-mode blocks included (DESIGN.md section 5) ----------------------------------
+int density_b200_decode_prot_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map, void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_map)) { set_error("d_in must be 2-byte, d_map 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase1_done = false; s->prot_stage = 0;     // the scratch is phase 1's
+    cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t launches = 0;
+    e = cham_decode_prot_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
+    return step_result(e, launches, "decode prot locate");
+}
+int density_b200_cheetah_decode_prot_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map,
+                                            void* stream) {
+    g_last_error.clear();
+    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_map)) { set_error("d_in must be 2-byte, d_map 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    s->phase = 0; s->transfer_done = false;         // the scratch is phase 1's
+    cudaError_t e = s->ws.ensure(chee_prot_locate_workspace_bytes(n_range + n_halo), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint64_t launches = 0;
+    e = chee_decode_prot_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
+    return step_result(e, launches, "cheetah decode prot locate");
+}
+
+// the message of a prot_locate_walk error code
+static const char* prot_locate_error(int rc) {
+    switch (rc) {
+        case bounds::PL_ERR_MULTIPLE: return "prot_locate_piece: a non-last range is not a multiple of 16384 bytes";
+        case bounds::PL_ERR_HALO: return "prot_locate_piece: a halo is not min(264, the bytes of the later ranges)";
+        case bounds::PL_ERR_OVERFLOW: return "prot_locate_piece: ranges overflow";
+        default: return "prot_locate_piece: bad row in a range map";
+    }
+}
+
+int density_b200_prot_locate_piece(int alg, const uint32_t* h_maps, int world, int rank, uint64_t out6[6]) {
+    g_last_error.clear();
+    if (alg != ALG_CHAMELEON && alg != ALG_CHEETAH) { set_error("prot_locate_piece: alg must be DENSITY_B200_CHAMELEON or DENSITY_B200_CHEETAH"); return DENSITY_B200_EARG; }
+    if (!h_maps || !out6 || world < 1 || rank < 0 || rank >= world) { set_error("prot_locate_piece: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+    const int rc = alg == ALG_CHAMELEON ? bounds::prot_locate_walk<bounds::ChamT::NCAND>(h_maps, world, rank, out6)
+                                        : bounds::prot_locate_walk<bounds::CheeT::NCAND>(h_maps, world, rank, out6);
+    if (rc != bounds::PL_OK) { set_error(prot_locate_error(rc)); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+
+namespace {
+// the refusal of a composition that met 0xFFFF / 0xFFFE: the outputs of a void verdict, without another collective
+__global__ void prot_locate_refused_k(uint32_t* __restrict__ d_flags, uint64_t* __restrict__ d_out_size, uint64_t* __restrict__ d_out_offset,
+                                      uint64_t* __restrict__ d_total_size) {
+    if (threadIdx.x || blockIdx.x) return;
+    *d_flags = 1; *d_out_size = 0;
+    if (d_out_offset) *d_out_offset = 0;
+    if (d_total_size) *d_total_size = 0;
+}
+}  // namespace
+
+// The protected range maps (this rank's already in its slot of `maps`, [world][map words]) to every rank -> the compose kernel -> its 8
+// words to the host: the call's one host synchronisation. piece = {start, end, is_final, is_first, entry candidate, refused}. The layout
+// errors are the same on every rank (the same maps), so is the refusal: a refused rank writes its void outputs and no rank enters
+// another collective.
+static int prot_locate_exchange(const Exchange& x, int alg, uint32_t* maps, uint32_t* d_flags, uint64_t* d_out_size, uint64_t* d_out_offset,
+                                uint64_t* d_total_size, uint64_t piece[6]) {
+    density_b200_sharded* h = x.h;
+    const size_t MW = alg == ALG_CHAMELEON ? DENSITY_B200_PROT_LOCATE_MAP_WORDS : DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS;
+    if (!x.gather(maps, MW, "ncclAllGather(maps)")) return DENSITY_B200_ECUDA;
+    unsigned long long* d_out8 = reinterpret_cast<unsigned long long*>(maps + (size_t)h->world * MW);
+    if (alg == ALG_CHAMELEON) bounds::dec_prot_compose_k<bounds::ChamT::NCAND><<<1, 32, 0, x.st>>>(maps, h->world, h->rank, d_out8);
+    else bounds::dec_prot_compose_k<bounds::CheeT::NCAND><<<1, 32, 0, x.st>>>(maps, h->world, h->rank, d_out8);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->h_maps, d_out8, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, x.st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(x.st);
+    int rc = step_result(e, 1, "protected range maps: compose");
+    if (rc != DENSITY_B200_OK) return rc;
+    if (h->h_maps[6] != bounds::PL_OK) { set_error(prot_locate_error((int)h->h_maps[6])); return DENSITY_B200_EARG; }
+    memcpy(piece, h->h_maps, 6 * sizeof(uint64_t));
+    if (piece[5]) {
+        prot_locate_refused_k<<<1, 32, 0, x.st>>>(d_flags, d_out_size, d_out_offset, d_total_size);
+        rc = step_result(cudaGetLastError(), 1, "protected range maps: refusal");
+    }
+    return rc;
+}
+
+// Sharded decode of a stream without known cuts, copy-mode blocks included: protected range map -> ncclAllGather(maps) -> compose kernel ->
+// one copy to the host and one host synchronisation -> prot_enter on the located piece -> the rest of density_b200_decode_sharded_protected.
+int density_b200_decode_sharded_stream_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* d_out,
+                                                 size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags,
+                                                 uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
+    constexpr size_t MW = DENSITY_B200_PROT_LOCATE_MAP_WORDS;
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, (size_t)h->world * MW * sizeof(uint32_t) + 64)) != DENSITY_B200_OK) return rc;
+    // sized for the whole range + halo: covers the locate scratch and the phases on any piece of it, so that phase 1 does not reallocate
+    const cudaError_t e = h->pdec->ws.ensure(cham_decode_workspace_bytes(n_range + n_halo, cap, h->num_sms), x.st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint32_t* maps = reinterpret_cast<uint32_t*>(x.extra);           // [world][MW], then the 8 words of the composition
+    uint64_t piece[6];
+    if ((rc = density_b200_decode_prot_locate(h->pdec, d_in, n_range, n_halo, maps + (size_t)h->rank * MW, x.st)) != DENSITY_B200_OK ||
+        (rc = prot_locate_exchange(x, ALG_CHAMELEON, maps, d_flags, d_out_size, d_out_offset, d_total_size, piece)) != DENSITY_B200_OK)
+        return rc;
+    if (piece[5]) return DENSITY_B200_OK;    // refused on every rank alike: none enters the collectives below
+    return decode_sharded_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[2], d_out, cap, d_out_size, d_flags,
+                                d_total_size, d_out_offset, (int64_t)piece[4]);
+}
+
+// The same for a Cheetah stream: no range offset is needed, the composition finds the range that holds the stream start.
+int density_b200_decode_sharded_cheetah_stream_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* d_out,
+                                                         size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset, uint32_t* d_flags,
+                                                         uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
+    constexpr size_t MW = DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS;
+    Exchange x;
+    if (rc != DENSITY_B200_OK ||
+        (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h) + (size_t)h->world * MW * sizeof(uint32_t) + 64)) != DENSITY_B200_OK)
+        return rc;
+    // sized for the locate scratch and for the phases on any piece of range + halo, so that phase 1 does not reallocate
+    const size_t locate_bytes = chee_prot_locate_workspace_bytes(n_range + n_halo);
+    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms);
+    const cudaError_t e = h->cdec->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, x.st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    uint32_t* maps = reinterpret_cast<uint32_t*>(x.extra + cheetah_piece_extra_bytes(h));   // [world][MW], then the composition's 8 words
+    uint64_t piece[6];
+    if ((rc = density_b200_cheetah_decode_prot_locate(h->cdec, d_in, n_range, n_halo, maps + (size_t)h->rank * MW, x.st)) != DENSITY_B200_OK ||
+        (rc = prot_locate_exchange(x, ALG_CHEETAH, maps, d_flags, d_out_size, d_out_offset, d_total_size, piece)) != DENSITY_B200_OK)
+        return rc;
+    if (piece[5]) return DENSITY_B200_OK;    // refused on every rank alike: none enters the collectives below
+    return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[3] != 0, piece[2] != 0, d_out, cap, d_out_size,
+                                        d_flags, d_total_size, d_out_offset, false, (int64_t)piece[4]);
 }
 
 /* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag

@@ -622,7 +622,7 @@ static uint32_t dec_pick_runs(const ChamDecLayout& L, int num_sms) {
 // Phase 1 of the parallel decode, which needs no carry-in: boundaries, then the writer pass (each run's last-writer table). With
 // d_table_out it also exports the piece's table (shard format) for the pieces after it.
 cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
-                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed) {
+                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed, bool rows_ready) {
     static bool attr_done = false;
     if (!attr_done) {
         cudaError_t e0 = cudaFuncSetAttribute(cham_decode_pass7<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Dec7Smem));
@@ -633,7 +633,7 @@ cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, u
     ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
     DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.B.status);
     uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.B.blk_off);
-    cudaError_t e = bounds::bounds_launch<T>(d_in, nbytes, cap, ws, L.B, stream, launches, d_seed, d_seed != nullptr);
+    cudaError_t e = bounds::bounds_launch<T>(d_in, nbytes, cap, ws, L.B, stream, launches, d_seed, rows_ready);
     if (e != cudaSuccess) return e;
     const uint32_t nruns = dec_pick_runs(L, num_sms);
     uint32_t* final_tab = reinterpret_cast<uint32_t*>(ws + L.final_tab);
@@ -675,15 +675,22 @@ cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t ca
 
 // The protection transfer of a piece (PT_NCAND words to d_transfer): the candidate rows of the boundary walk, then the head walk over them.
 // The rows stay in the workspace for cham_decode_phase1 with a seed.
-cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
-                                      cudaStream_t stream, uint64_t* launches) {
+static cudaError_t prot_transfer_attr() {
     static bool attr_done = false;
     if (!attr_done) {
-        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                    (int)bounds::prot_transfer_smem<T>());
+        cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)bounds::prot_transfer_smem<T>());
+        if (e0 == cudaSuccess)
+            e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bounds::prot_transfer_smem<T>());
         if (e0 != cudaSuccess) return e0;
         attr_done = true;
     }
+    return cudaSuccess;
+}
+cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
+                                      cudaStream_t stream, uint64_t* launches) {
+    const cudaError_t e0 = prot_transfer_attr();
+    if (e0 != cudaSuccess) return e0;
     ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
     uint32_t* res = reinterpret_cast<uint32_t*>(ws + L.B.res);
     uint4* gres = reinterpret_cast<uint4*>(ws + L.B.gres);
@@ -694,12 +701,14 @@ cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t
         bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
         *launches += 2;
     }
-    bounds::dec_prot_transfer<T><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(d_in, nbytes, is_last, res, gres, d_transfer);
+    bounds::dec_prot_transfer<T, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(d_in, nbytes, nbytes, is_last, res, gres,
+                                                                                                    d_transfer);
     ++*launches;
     return cudaGetLastError();
 }
-cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches) {
-    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
+cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
+                                   uint64_t* launches) {
+    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, x0, d_seed);
     ++*launches;
     return cudaGetLastError();
 }
@@ -732,6 +741,15 @@ cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
     bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(gres, ngroups, n_range, n_halo, reinterpret_cast<unsigned long long*>(d_map));
     ++*launches;
     return cudaGetLastError();
+}
+
+// The protected range map of d_in[0 .. n_range + n_halo) (DENSITY_B200_PROT_LOCATE_MAP_WORDS u32 to d_map); the scratch is
+// cham_locate_workspace_bytes(n_range + n_halo).
+cudaError_t cham_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                    uint64_t* launches) {
+    const cudaError_t e0 = prot_transfer_attr();
+    if (e0 != cudaSuccess) return e0;
+    return bounds::prot_locate_launch<T>(d_in, n_range, n_halo, ws, d_map, stream, launches);
 }
 
 // Enqueues the parallel decode. On return (after the stream drains) *d_nonquiet != 0 means the caller must run the exact

@@ -747,10 +747,11 @@ size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
 
 // Phase 1: boundaries (piece 0 may use copy mode: dec_seq_walk from the fresh automaton), the end of the piece, unpack (literals and
 // copy-mode blocks go straight to d_out), the symbolic chunk-map walk and the piece's chunk-map transfer (d_cmap_out, may be null).
-// d_seed (the protected path, nullptr otherwise): the piece's incoming state, after chee_shard_prot_transfer filled the candidate rows.
-cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed) {
+// d_seed (the protected path, nullptr otherwise): the piece's incoming state; rows_ready: chee_shard_prot_transfer filled the candidate rows.
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
+                              bool rows_ready) {
     const CheeDecPtrs p = chee_shard_ptrs(a);
-    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, d_seed != nullptr);
+    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, rows_ready);
     if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
     if (e != cudaSuccess) return e;
@@ -809,14 +810,21 @@ cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint
 
 // The protected path's first step on a piece (DESIGN.md section 5): the candidate rows of the boundary walk (they stay in the workspace
 // for chee_shard_phase1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing.
-cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+static cudaError_t prot_transfer_attr() {
     static bool attr_done = false;
     if (!attr_done) {
-        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                    (int)bounds::prot_transfer_smem<T>());
+        cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)bounds::prot_transfer_smem<T>());
+        if (e0 == cudaSuccess)
+            e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bounds::prot_transfer_smem<T>());
         if (e0 != cudaSuccess) return e0;
         attr_done = true;
     }
+    return cudaSuccess;
+}
+cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    const cudaError_t e0 = prot_transfer_attr();
+    if (e0 != cudaSuccess) return e0;
     uint32_t* res = nullptr;
     uint4* gres = nullptr;
     if (a.n) {
@@ -828,13 +836,15 @@ cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfe
         bounds::dec_group_compose<T><<<(nchunks + bounds::GROUP - 1) / bounds::GROUP, 160, 0, stream>>>(res, nchunks, gres);
         *launches += 2;
     }
-    bounds::dec_prot_transfer<T><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(a.d_in, a.n, a.last ? 1 : 0, res, gres, d_transfer);
+    bounds::dec_prot_transfer<T, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(a.d_in, a.n, a.n, a.last ? 1 : 0, res, gres,
+                                                                                                    d_transfer);
     ++*launches;
     return cudaGetLastError();
 }
-// The incoming state of piece `rank` composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
-cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches) {
-    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, d_seed);
+// The incoming state of piece `rank` composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
+cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
+                                  uint64_t* launches) {
+    bounds::dec_prot_enter_k<<<1, 32, 0, stream>>>(d_all_transfers, rank, x0, d_seed);
     ++*launches;
     return cudaGetLastError();
 }
@@ -894,6 +904,17 @@ cudaError_t chee_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
                                                    map + 2 + 2 * T::NCAND);
     *launches += 2;
     return cudaGetLastError();
+}
+
+// ---- the protected range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS u32) --------
+// Every range alike, the one with the stream start included: its row (0, 0) is the exact walk from the fresh automaton.
+size_t chee_prot_locate_workspace_bytes(size_t nbytes) { bounds::BoundsLayout B; return bounds::bounds_layout<T>(nbytes, 0, &B); }
+
+cudaError_t chee_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                    uint64_t* launches) {
+    const cudaError_t e0 = prot_transfer_attr();
+    if (e0 != cudaSuccess) return e0;
+    return bounds::prot_locate_launch<T>(d_in, n_range, n_halo, ws, d_map, stream, launches);
 }
 
 }  // namespace dns

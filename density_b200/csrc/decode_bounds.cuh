@@ -419,16 +419,26 @@ __global__ void dec_start_row(const DecStatus* __restrict__ st, const uint64_t* 
 // ---- 4. the protection transfer of a piece of a sharded stream (DESIGN §5) ----------------------------------------------------------
 // A piece starts at a block boundary, in an automaton state and counter phase (revert_to_copy halves the start on every 16th block of
 // the STREAM) that its decoder does not know. A decode candidate is (penalty 0..9, start 1..10, previous_incompressible, counter mod
-// 16): PT_NCAND of them, candidate 0 the stream start. dec_prot_transfer writes, for every candidate, where the boundary walk of
-// codec.rs:88-100, copy-mode blocks included, leaves a non-final piece: the candidate at its end when the walk ends exactly on the cut,
-// PT_ESC when that state is not a candidate, PT_NOEND when it overshoots the cut, stops short of it or reads a malformed block.
+// 16): PT_NCAND of them, candidate 0 the stream start. dec_prot_transfer walks codec.rs:88-100, copy-mode blocks included, from every
+// candidate at once and writes one word per candidate where the walk leaves the piece at its CUT:
+//  * known cuts (LOCATE false, cut == n, one CTA): the candidate at the piece end when the walk ends exactly on the cut, PT_ESC when
+//    that state is not a candidate, PT_NOEND when it overshoots the cut, stops short of it or reads a malformed block;
+//  * the protected range map (LOCATE true, DESIGN §5): in[0 .. n) is a range of `cut` bytes and its halo, and CTA e starts the walks
+//    at the entry offset 2e. Its row of candidate c: the exit index x (the first block start at or after the cut is cut + 2x) and the
+//    candidate there, packed by pt_row; PT_TERM when the main loop ends (fewer than MAXBLK bytes left) in front of the cut; PT_ESC when
+//    the state at the exit is not a candidate; PT_NOEND for a head dropped at the cap. The range map is PT_MAP_HDR header words
+//    {n_range lo, hi, n_halo lo, hi}, then the NCAND x PT_NCAND rows, entry-major.
 // The walk follows HEADS keyed by (offset, state, phase), not candidates; heads that reach the same key merge for good, each candidate
 // keeps the index of its head. All heads advance chunk by chunk: a head with penalty 0 jumps its group or its chunk in O(1) from the
 // candidate rows (dec_seq_walk's rule), any other head walks the chunk block by block from shared memory, one thread per head. After a
 // chunk step the heads are merged in a shared hash table; at most PT_CAP stay live, the candidates of the others get PT_NOEND (their
-// piece is refused, never decoded wrong). tests/prot_decode_model.py is the CPU twin and measures the head counts.
+// piece is refused, never decoded wrong). tests/prot_decode_model.py and tests/prot_locate_model.py are the CPU twins.
 constexpr uint32_t PT_NCAND = 3200, PT_ESC = 0xFFFFu, PT_NOEND = 0xFFFEu, PT_CAP = 256, PT_HT = 8192, PT_THREADS = 1024;
 constexpr uint32_t PT_LIVE = 0xFFFFFFFFu, PT_DEAD = 0xFFFFu;
+constexpr uint32_t PT_TERM = TERM, PT_MAP_HDR = 4;   // a range-map row whose walk reached the stream end; the map's header words
+// a range-map row: exit index (bits 0-7, < NCAND) | exit candidate (bits 8-23). No row equals PT_ESC or PT_NOEND: their low byte
+// would be TERM or 0xFE, and a PT_TERM row is TERM alone.
+__host__ __device__ __forceinline__ uint32_t pt_row(uint32_t exit_idx, uint32_t cand) { return exit_idx | (cand << 8); }
 __host__ __device__ __forceinline__ uint32_t pt_pack(uint32_t pen, uint32_t start, uint32_t prev, uint32_t phase) {
     return pen | (start << 8) | (prev << 16) | (phase << 17);
 }
@@ -449,6 +459,12 @@ __device__ __forceinline__ uint32_t pt_jump(uint32_t s, uint32_t nb, uint32_t la
     if (start > 1) { start >>= (k > 8 ? 8u : k); if (!start) start = 1; }
     return pt_pack(0, start, last_inc, (ph + nb) & 15u);
 }
+// the word of a head that reached off >= cut in state s (see dec_prot_transfer)
+__device__ __forceinline__ uint32_t pt_exit(uint64_t off, uint32_t s, uint64_t cut, int locate) {
+    const uint32_t c = pt_cand(s);
+    if (!locate) return off == cut ? c : PT_NOEND;
+    return c == PT_ESC ? PT_ESC : pt_row((uint32_t)((off - cut) >> 1), c);
+}
 struct PtSmem {
     unsigned long long off[2][PT_NCAND];    // head offsets in the piece, double-buffered across a merge
     uint32_t st[2][PT_NCAND];               // packed head states
@@ -459,22 +475,28 @@ struct PtSmem {
     uint16_t ht_val[PT_HT];
     uint32_t nh, nnew, need_win, min_chunk;
 };
-template <class T>
+template <class T, bool LOCATE>
 __global__ void __launch_bounds__(PT_THREADS, 1)
-dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const uint32_t* __restrict__ res, const uint4* __restrict__ gres,
-                  uint32_t* __restrict__ out) {
+dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, uint64_t cut, int is_last, const uint32_t* __restrict__ res,
+                  const uint4* __restrict__ gres, uint32_t* __restrict__ out) {
+    constexpr int locate = LOCATE ? 1 : 0;
     constexpr uint32_t SW_LOAD = T::CH + 16;
     extern __shared__ __align__(16) unsigned char pt_raw[];
     uint8_t* win = pt_raw;
     PtSmem& S = *reinterpret_cast<PtSmem*>(pt_raw + SW_LOAD);
     const uint32_t tid = threadIdx.x;
-    if (is_last || n == 0) {          // the last piece's transfer is never composed; an empty piece is the identity
-        for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) out[c] = is_last ? PT_NOEND : c;
+    const uint64_t entry = 2ull * blockIdx.x;
+    if (locate) {
+        if (blockIdx.x == 0 && tid < PT_MAP_HDR) out[tid] = (uint32_t)((tid < 2 ? cut : n - cut) >> (32 * (tid & 1)));
+        out += PT_MAP_HDR + (size_t)blockIdx.x * PT_NCAND;
+    }
+    if (is_last || cut == 0) {        // the last piece's transfer is never composed; an empty piece or range is the identity
+        for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) out[c] = is_last ? PT_NOEND : pt_exit(entry, pt_state(c), 0, locate);
         return;
     }
     const bool al16 = (reinterpret_cast<uintptr_t>(in) & 15u) == 0;
-    const uint32_t nchunks = (uint32_t)((n + T::CH - 1) / T::CH);
-    for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) { S.off[0][c] = 0; S.st[0][c] = pt_state(c); S.cand_head[c] = (uint16_t)c; }
+    const uint32_t nchunks = (uint32_t)((cut + T::CH - 1) / T::CH);
+    for (uint32_t c = tid; c < PT_NCAND; c += PT_THREADS) { S.off[0][c] = entry; S.st[0][c] = pt_state(c); S.cand_head[c] = (uint16_t)c; }
     if (tid == 0) S.nh = PT_NCAND;
     uint32_t cur = 0;
     __syncthreads();
@@ -505,7 +527,7 @@ dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const
                     }
                 }
                 if (!jumped) { e = PT_LIVE - 1; S.need_win = 1; }
-                else if (off == n) e = pt_cand(s);
+                else if (off >= cut) e = pt_exit(off, s, cut, locate);
             }
             S.off[cur][h] = off; S.st[cur][h] = s; S.end[h] = e;
         }
@@ -519,8 +541,9 @@ dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const
                 uint64_t off = S.off[cur][h];
                 uint32_t s = S.st[cur][h], e = PT_LIVE;
                 uint32_t pen = s & 0xFFu, start = (s >> 8) & 0xFFu, prev = (s >> 16) & 1u, ph = s >> 17;
-                const uint64_t stop = cend < n ? cend : n;
+                const uint64_t stop = cend < cut ? cend : cut;
                 while (off < stop) {                           // codec.rs:88-98; every block of a non-final piece is a main-loop block
+                    if (locate && off + T::MAXBLK > n) { e = PT_TERM; break; }   // the main loop ends in front of the cut
                     if (ph == 0 && start > 1) start >>= 1;
                     ph = (ph + 1) & 15u;
                     if (pen) {
@@ -537,7 +560,7 @@ dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const
                     if (off > n) { e = PT_NOEND; break; }
                 }
                 s = pt_pack(pen, start, prev, ph);
-                if (e == PT_LIVE && off == n) e = pt_cand(s);
+                if (e == PT_LIVE && off >= cut) e = pt_exit(off, s, cut, locate);
                 S.off[cur][h] = off; S.st[cur][h] = s; S.end[h] = e;
             }
         }
@@ -591,15 +614,74 @@ dec_prot_transfer(const uint8_t* __restrict__ in, uint64_t n, int is_last, const
 template <class T> constexpr size_t prot_transfer_smem() { return T::CH + 16 + sizeof(PtSmem); }
 
 // The incoming state of piece `rank` (SEED_WORDS): the transfers of the pieces before it (dec_prot_transfer, [rank][PT_NCAND]) composed
-// from candidate 0, the stream start. A path that meets PT_ESC or PT_NOEND refuses the piece; the kernels then run from the stream-start
-// state, harmlessly. Static: every decoder's translation unit launches its own copy.
-static __global__ void dec_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t* __restrict__ seed) {
+// from candidate x0 (0, the stream start, for known cuts; a located piece's entry candidate with rank 0). A path that meets PT_ESC or
+// PT_NOEND refuses the piece; the kernels then run from the stream-start state, harmlessly. Static: every decoder's translation unit
+// launches its own copy.
+static __global__ void dec_prot_enter_k(const uint32_t* __restrict__ all_transfers, uint32_t rank, uint32_t x0, uint32_t* __restrict__ seed) {
     if (threadIdx.x || blockIdx.x) return;
-    uint32_t x = 0;
+    uint32_t x = x0;
     for (uint32_t r = 0; r < rank && x < PT_NCAND; ++r) x = all_transfers[(size_t)r * PT_NCAND + x];
     const uint32_t refused = x < PT_NCAND ? 0u : 1u;
     const uint32_t s = pt_state(refused ? 0u : x);
     seed[0] = s & 0xFFu; seed[1] = (s >> 8) & 0xFFu; seed[2] = (s >> 16) & 1u; seed[3] = s >> 17; seed[4] = refused;
+}
+
+// ---- 5. the located piece of a stream without known cuts, from the protected range maps of all ranks (DESIGN §5) --------------------
+// Shared by density_b200_prot_locate_piece (host) and dec_prot_compose_k (device). maps: `world` range maps of PT_MAP_HDR + NC x
+// PT_NCAND u32 (dec_prot_transfer<T, true>) in rank order. Checks the layout (non-last ranges multiples of PL_RANGE_UNIT, each
+// halo min(PL_HALO, the bytes of the later ranges), no overflow) and every row on the path, then walks from (entry 0, candidate 0) of the
+// first non-empty range; an empty range passes the entry on. The walk covers every range, not only those before `rank`, so that a
+// refusal anywhere (a PT_ESC or PT_NOEND row on the path) is known on every rank alike. out6 = {start, end, is_final, is_first, entry
+// candidate, refused}: this rank's piece is d_in[start .. end) entered in that candidate; a refused path zeroes the others.
+enum : int { PL_OK = 0, PL_ERR_MULTIPLE, PL_ERR_HALO, PL_ERR_OVERFLOW, PL_ERR_ROW };
+constexpr uint64_t PL_RANGE_UNIT = 16384, PL_HALO = 264;
+template <uint32_t NC>
+__host__ __device__ inline int prot_locate_walk(const uint32_t* maps, int world, int rank, uint64_t out6[6]) {
+    constexpr uint64_t MW = PT_MAP_HDR + (uint64_t)NC * PT_NCAND;
+    auto hdr = [&](int r, int k) { const uint32_t* m = maps + (size_t)r * MW; return (uint64_t)m[2 * k] | ((uint64_t)m[2 * k + 1] << 32); };
+    uint64_t later = 0;                 // stream bytes behind range r
+    for (int r = world - 1; r >= 0; --r) {
+        const uint64_t nr = hdr(r, 0), nh = hdr(r, 1);
+        if (r < world - 1 && nr % PL_RANGE_UNIT) return PL_ERR_MULTIPLE;
+        if (nh != (later < PL_HALO ? later : PL_HALO)) return PL_ERR_HALO;
+        if (nr > ~later) return PL_ERR_OVERFLOW;
+        later += nr;
+    }
+    for (int k = 0; k < 6; ++k) out6[k] = 0;
+    uint32_t idx = 0, cand = 0;
+    bool started = false, ended = false;     // a non-empty range was passed; a walk reached the stream end
+    for (int r = 0; r < world; ++r) {
+        const uint64_t nr = hdr(r, 0), nh = hdr(r, 1);
+        if (ended || nr == 0) {              // a piece behind the stream end, or an empty range: empty, the entry passes on
+            if (r == rank) out6[2] = ended || nh == 0;
+            continue;
+        }
+        const uint32_t row = maps[(size_t)r * MW + PT_MAP_HDR + (size_t)idx * PT_NCAND + cand];
+        if (row == PT_ESC || row == PT_NOEND) { for (int k = 0; k < 5; ++k) out6[k] = 0; out6[5] = 1; return PL_OK; }
+        const uint32_t x = row & 0xFFu;
+        uint64_t end;
+        if (x == PT_TERM) {
+            if (row != PT_TERM) return PL_ERR_ROW;
+            end = nr + nh; ended = true;
+        } else {
+            if (x >= NC || (row >> 8) >= PT_NCAND) return PL_ERR_ROW;
+            end = nr + 2 * x;
+        }
+        if (2ull * idx > end || end > nr + nh) return PL_ERR_ROW;
+        if (r == rank) { out6[0] = 2ull * idx; out6[1] = end; out6[2] = end == nr + nh; out6[3] = !started; out6[4] = cand; }
+        if (!ended) { idx = x; cand = row >> 8; }
+        started = true;
+    }
+    return PL_OK;
+}
+// the device twin for the NCCL drivers: out8 = {out6, rc, 0}, so that one small copy brings the piece to the host
+template <uint32_t NC>
+__global__ void dec_prot_compose_k(const uint32_t* __restrict__ maps, int world, int rank, unsigned long long* __restrict__ out8) {
+    if (threadIdx.x || blockIdx.x) return;
+    uint64_t o[6];
+    const int rc = prot_locate_walk<NC>(maps, world, rank, o);
+    for (int k = 0; k < 6; ++k) out8[k] = o[k];
+    out8[6] = (unsigned long long)rc; out8[7] = 0;
 }
 
 // The automaton state behind the main loop: dec_seq_walk's, or (quiet: penalty 0 throughout) the entry state jumped over the main
@@ -677,6 +759,27 @@ inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap,
     dec_chunk_entries<T><<<(ngroups + 127) / 128, 128, 0, stream>>>(res, nchunks, g_entry, g_bb, ngroups, c_entry, c_bb, st);
     dec_block_offsets<T><<<(nchunks + 127) / 128, 128, 0, stream>>>(d_in, nbytes, nchunks, c_entry, c_bb, blk_off, L.maxblocks, st);
     *launches += 7;
+    return cudaGetLastError();
+}
+
+// Enqueues the protected range map of d_in[0 .. n_range + n_halo) into d_map (PT_MAP_HDR + T::NCAND x PT_NCAND u32): the candidate rows
+// of the range's chunks (the halo visible to its last chunk's walks), as the quiet locate computes them, then one head walk per entry
+// offset. The scratch is the res / gres arrays of bounds_layout<T>(n_range + n_halo). dec_prot_transfer<T, true> must allow
+// prot_transfer_smem<T>() bytes of dynamic shared memory.
+template <class T>
+inline cudaError_t prot_locate_launch(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                      uint64_t* launches) {
+    BoundsLayout B; bounds_layout<T>(n_range + n_halo, 0, &B);
+    uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
+    uint4* gres = reinterpret_cast<uint4*>(ws + B.gres);
+    const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
+    if (nchunks) {
+        dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
+        dec_group_compose<T><<<(nchunks + GROUP - 1) / GROUP, 160, 0, stream>>>(res, nchunks, gres);
+        *launches += 2;
+    }
+    dec_prot_transfer<T, true><<<T::NCAND, PT_THREADS, prot_transfer_smem<T>(), stream>>>(d_in, n_range + n_halo, n_range, 0, res, gres, d_map);
+    ++*launches;
     return cudaGetLastError();
 }
 

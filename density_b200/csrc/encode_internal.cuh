@@ -155,20 +155,22 @@ cudaError_t cham_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
                                  uint64_t* d_out_size, uint32_t* d_nonquiet, cudaStream_t stream, uint64_t* launches);
 // the same as two phases, for one piece of a sharded stream: phase 1 needs no carry-in and exports the piece's last-writer table
 // (shard format) when d_table_out is set; phase 2 decodes from d_carry_in (NULL: stream start); then the piece's 8 seam words
-// d_seed (may be NULL): the piece's incoming automaton state (cham_decode_prot_enter), after cham_decode_prot_transfer on the same workspace
+// d_seed (may be NULL): the piece's incoming automaton state (cham_decode_prot_enter); rows_ready: cham_decode_prot_transfer on the same
+// workspace filled the candidate rows
 cudaError_t cham_decode_phase1(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, uint32_t* d_table_out,
-                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr);
+                               cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr, bool rows_ready = false);
 cudaError_t cham_decode_phase2(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, int num_sms, const uint32_t* d_carry_in,
                                uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches);
 cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint64_t* d_out_size,
                                    uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 // a piece of a stream with copy-mode blocks: its protection transfer (DECODE_PROT_TRANSFER_WORDS, fills the candidate rows of the workspace
-// first), its incoming state composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), and its seam words after
-// cham_decode_phase1 with that seed and cham_decode_phase2 (nbytes 0: an empty piece, the workspace is not read)
+// first), its incoming state composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), and its seam
+// words after cham_decode_phase1 with that seed and cham_decode_phase2 (nbytes 0: an empty piece, the workspace is not read)
 constexpr uint32_t DECODE_PROT_TRANSFER_WORDS = 3200, DECODE_PROT_SEED_WORDS = 5;
 cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
                                       cudaStream_t stream, uint64_t* launches);
-cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
+                                   uint64_t* launches);
 cudaError_t cham_decode_prot_seam_words(size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint32_t* d_seed, uint64_t* d_out_size,
                                         uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 // the range map of a piece of a stream without known cuts (DENSITY_B200_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`, at least
@@ -176,6 +178,9 @@ cudaError_t cham_decode_prot_seam_words(size_t nbytes, size_t cap, uint8_t* ws, 
 size_t cham_locate_workspace_bytes(size_t nbytes);
 cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint64_t* d_map, cudaStream_t stream,
                                uint64_t* launches);
+// the protected range map (DENSITY_B200_PROT_LOCATE_MAP_WORDS u32 to d_map), the same scratch
+cudaError_t cham_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                    uint64_t* launches);
 
 // cl_decode.cu (run-parallel Cheetah decode)
 size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);
@@ -189,8 +194,10 @@ const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int n
 struct CheeShardArgs { const uint8_t* d_in; size_t n; uint8_t* d_out; size_t cap; bool first, last; uint8_t* ws; uint8_t* tables; int num_sms; };
 size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
 uint32_t chee_shard_max_rounds();
-// d_seed (may be NULL): the piece's incoming automaton state (chee_shard_prot_enter), after chee_shard_prot_transfer on the same workspace
-cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr);
+// d_seed (may be NULL): the piece's incoming automaton state (chee_shard_prot_enter); rows_ready: chee_shard_prot_transfer on the same
+// workspace filled the candidate rows
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr,
+                              bool rows_ready = false);
 cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
@@ -201,7 +208,8 @@ cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint
 // a piece of a stream with copy-mode blocks: its protection transfer (DECODE_PROT_TRANSFER_WORDS; fills the candidate rows of the workspace
 // first) and its incoming state composed from the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), for chee_shard_phase1
 cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
-cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_seed, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
+                                  uint64_t* launches);
 const void* chee_shard_status_ptr(const CheeShardArgs& a);
 cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
@@ -212,6 +220,11 @@ cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_
 size_t chee_locate_workspace_bytes(size_t n_range, size_t n_halo, uint64_t range_offset);
 cudaError_t chee_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset, uint8_t* ws, uint64_t* d_map,
                                cudaStream_t stream, uint64_t* launches);
+// the protected range map of any range (DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS u32 to d_map); scratch chee_prot_locate_workspace_bytes(
+// n_range + n_halo)
+size_t chee_prot_locate_workspace_bytes(size_t nbytes);
+cudaError_t chee_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                    uint64_t* launches);
 
 // scalar_codec.cu (Cheetah / Lion, in-order)
 size_t scalar_workspace_bytes(int alg);

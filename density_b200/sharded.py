@@ -215,6 +215,24 @@ def locate_piece(maps, rank, alg="chameleon"):
     return tuple(int(v) for v in out)
 
 
+PROT_LOCATE_MAP_WORDS = 422404           # DENSITY_B200_PROT_LOCATE_MAP_WORDS: 4 header words + 132 entries x 3200 candidates
+CHEETAH_PROT_LOCATE_MAP_WORDS = 217604   # DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS: 4 + 68 x 3200
+
+
+def prot_locate_piece(maps, rank, alg="chameleon"):
+    """density_b200_prot_locate_piece (host only) on the gathered protected range maps, uint32-compatible [world, map words] in rank
+    order. Returns (start, end, is_final, is_first, entry candidate, refused): this rank's piece is its buffer's bytes [start, end),
+    entered in that decode candidate; refused != 0 on every rank when the composition met 0xFFFF / 0xFFFE anywhere."""
+    alg = _alg_id(alg)
+    if alg not in (0, 1):
+        raise ValueError("prot_locate_piece: alg must be 'chameleon' or 'cheetah'")
+    words = CHEETAH_PROT_LOCATE_MAP_WORDS if alg == 1 else PROT_LOCATE_MAP_WORDS
+    m = np.ascontiguousarray(np.asarray(maps).astype(np.uint32, copy=False).reshape(-1, words))
+    out = (ctypes.c_uint64 * 6)()
+    _check(_lib.load().density_b200_prot_locate_piece(alg, m.ctypes.data, m.shape[0], rank, out), "prot_locate_piece")
+    return tuple(int(v) for v in out)
+
+
 class _Handle:
     """Owns one library handle: made by `create`, freed by `destroy` on close() or when the object is collected."""
 
@@ -506,20 +524,46 @@ class ShardedChameleonDecoder(_Handle):
         flags, total, offsets = self._decode_piece(d_in[start:end], d_out, d_size, bool(is_final), group)
         return flags, total, offsets, int(offsets[rank])
 
-    def _decode_piece(self, d_in, d_out, d_size, is_last, group):
+    def decode_stream_protected(self, d_in, n_range, d_out, d_size, group=None):
+        """decode_stream for any stream, copy-mode blocks included: the protected range map (density_b200_decode_prot_locate), an
+        all_gather of the maps (1.6 MiB per rank), prot_locate_piece on the host, then the located piece from its entry candidate
+        (density_b200_decode_shard_prot_enter, prot_phase2). Returns (flags, total, offsets, my_offset) as decode_stream; a refused
+        composition gives flags 1 on every rank without decoding."""
+        rank, world = _rank_world(group)
+        n_halo = d_in.numel() - n_range
+        if n_halo < 0:
+            raise ValueError("d_in is shorter than its range")
+        m = torch.empty(PROT_LOCATE_MAP_WORDS, dtype=torch.int32, device=d_in.device)
+        _check(self._lib.density_b200_decode_prot_locate(self._h, d_in.data_ptr(), n_range, n_halo, m.data_ptr(), _stream()),
+               "decode_prot_locate")
+        maps = gather_rows(m, group)
+        start, end, is_final, _, cand, refused = prot_locate_piece(maps.cpu().numpy().view(np.uint32), rank)
+        if refused:
+            d_size.zero_()
+            return 1, 0, torch.zeros(world + 1, dtype=torch.int64), 0
+        flags, total, offsets = self._decode_piece(d_in[start:end], d_out, d_size, bool(is_final), group, cand)
+        return flags, total, offsets, int(offsets[rank])
+
+    def _decode_piece(self, d_in, d_out, d_size, is_last, group, cand=None):
+        """cand: a located piece's entry candidate (the protected phases), None: the quiet phases"""
         rank = _rank_world(group)[0]
         stream = _stream()
         table = torch.empty(TABLE_ENTRIES, dtype=torch.int32, device=d_in.device)
-        _check(self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last),
-                                                          table.data_ptr(), stream), "decode_shard_phase1")
+        if cand is None:
+            _check(self._lib.density_b200_decode_shard_phase1(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last),
+                                                              table.data_ptr(), stream), "decode_shard_phase1")
+        else:
+            _check(self._lib.density_b200_decode_shard_prot_enter(self._h, d_in.data_ptr(), d_in.numel(), d_out.numel(), int(is_last), cand,
+                                                                  table.data_ptr(), stream), "decode_shard_prot_enter")
         gathered = gather_rows(table, group)
         carry_ptr = None
         if rank > 0:
             self._carry = fold_tables(gathered, rank)
             carry_ptr = self._carry.data_ptr()
         words = torch.empty(SEAM_WORDS, dtype=torch.int32, device=d_in.device)
-        _check(self._lib.density_b200_decode_shard_phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream),
-               "decode_shard_phase2")
+        phase2 = self._lib.density_b200_decode_shard_phase2 if cand is None else self._lib.density_b200_decode_shard_prot_phase2
+        _check(phase2(self._h, carry_ptr, d_out.data_ptr(), d_size.data_ptr(), words.data_ptr(), stream),
+               "decode_shard_phase2" if cand is None else "decode_shard_prot_phase2")
         return seam_verdict(gather_rows(words, group))
 
 
@@ -630,3 +674,17 @@ class ShardedDecoder(_ShardedHandle):
         else:
             rc = self._lib.density_b200_decode_sharded_cheetah_stream(self._h, d_in.data_ptr(), n_range, n_halo, int(range_offset), *tail)
         _check(rc, f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream")
+
+    def decode_stream_protected(self, d_in, n_range, d_out, d_size, d_flags, alg="chameleon"):
+        """decode_stream for any stream, copy-mode blocks included (density_b200_decode_sharded_stream_protected, or with alg "cheetah"
+        density_b200_decode_sharded_cheetah_stream_protected, which needs no range offset). The arguments and outputs of decode_stream;
+        blocks once, on the composition of the range maps. A refused composition sets d_flags to 1 on every rank."""
+        alg = _alg_id(alg)
+        if alg not in (0, 1):
+            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+        n_halo = d_in.numel() - n_range
+        if n_range < 0 or n_halo < 0:
+            raise ValueError("d_in is shorter than its range")
+        fn = self._lib.density_b200_decode_sharded_stream_protected if alg == 0 else self._lib.density_b200_decode_sharded_cheetah_stream_protected
+        _check(fn(self._h, d_in.data_ptr(), n_range, n_halo, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(),
+                  d_flags.data_ptr(), self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream_protected")

@@ -575,6 +575,64 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah_stream(density_b200_sha
                                                uint64_t* d_out_offset, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
+ * Sharded decode of a stream whose cuts are not known, copy-mode blocks included (DESIGN.md section 5): archives, images, text mixed
+ * with binary, Cheetah's cold start, whatever the data. The input layout of density_b200_decode_sharded_stream: range + halo of
+ * min(264, the bytes of the later ranges), non-last ranges multiples of 16384 bytes; no range offset is needed.
+ *
+ * The PROTECTED RANGE MAP (u32): {n_range lo, n_range hi, n_halo lo, n_halo hi}, then for each entry offset e (2e bytes into the range;
+ * 132 of them for Chameleon, 68 for Cheetah) and each decode candidate c (the encoding of density_b200_decode_shard_prot_transfer,
+ * 3200 of them) one row at [4 + e * 3200 + c]: where the exact boundary walk (codec.rs's main loop with the protection automaton,
+ * copy-mode blocks included) from offset 2e in candidate c leaves the range:
+ *   exit | cand << 8  the first block start at or after n_range is n_range + 2 * exit (exit < 132 / 68), and the walk is in candidate
+ *                     cand there;
+ *   0xFF              the main loop ends (fewer than 264 / 136 bytes left) in front of n_range: the piece ends the stream;
+ *   0xFFFF            the walk leaves the range in a state that is not a candidate;
+ *   0xFFFE            more distinct walks than the walk keeps.
+ * No row of the first two kinds equals 0xFFFF or 0xFFFE.
+ */
+#define DENSITY_B200_PROT_LOCATE_MAP_WORDS 422404
+#define DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS 217604
+/* Enqueue the protected range map of d_in[0 .. n_range + n_halo) (2-byte aligned) into d_map (device, 4-byte aligned): the candidate
+   rows of the quiet locate, then one head walk per entry offset (132 / 68 CTAs). The scratch lives in the shard's workspace, which the
+   next phase 1 overwrites. The layout is checked by density_b200_prot_locate_piece. */
+DENSITY_B200_API int density_b200_decode_prot_locate(density_b200_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                     uint32_t* d_map, void* stream);
+DENSITY_B200_API int density_b200_cheetah_decode_prot_locate(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n_range,
+                                             size_t n_halo, uint32_t* d_map, void* stream);
+/* Host only, needs no device. alg: DENSITY_B200_CHAMELEON or DENSITY_B200_CHEETAH; h_maps: the protected range maps of all `world` ranks
+   in rank order. Checks the layout as density_b200_locate_piece does (DENSITY_B200_EARG, on every rank alike, also for a malformed row on
+   the path) and walks from entry 0, candidate 0 of the first non-empty range through every range; empty ranges pass the entry on.
+   out6 = {start, end, is_final, is_first, entry candidate, refused}: this rank's piece is d_in[start .. end), entered in that candidate,
+   is_final = 1 when no stream byte follows it, is_first = 1 when it holds the stream start. refused = 1 (all the others 0) when the walk
+   met 0xFFFF or 0xFFFE anywhere, so every rank knows it. A piece behind the end of the stream is empty. */
+DENSITY_B200_API int density_b200_prot_locate_piece(int alg, const uint32_t* h_maps, int world, int rank, uint64_t out6[6]);
+/* Phase 1 of a located piece, from its entry candidate (< 3200) instead of composed transfers; the arguments of
+   density_b200_decode_shard_prot_transfer otherwise. Followed by density_b200_decode_shard_prot_phase2, whose seam words it shares. */
+DENSITY_B200_API int density_b200_decode_shard_prot_enter(density_b200_decode_shard*, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
+                                         uint32_t candidate, uint32_t* d_table_out, void* stream);
+/* The same for Cheetah, the arguments of density_b200_cheetah_decode_shard_prot_phase1 with is_first / is_last of the located piece;
+   followed by phase 2, the rounds and phase 3 unchanged. */
+DENSITY_B200_API int density_b200_cheetah_decode_shard_prot_enter(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n,
+                                                 uint8_t* d_out, size_t cap, int is_first, int is_last, uint32_t candidate,
+                                                 uint32_t* d_cmap_out, void* stream);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments of density_b200_decode_sharded_stream: protected range map ->
+   ncclAllGather(maps, 1.6 MiB per rank) -> one compose kernel -> one device-to-host copy of 8 words and ONE host synchronisation ->
+   prot_enter on the located piece -> ncclAllGather(tables) -> fold kernel -> prot_phase2 -> ncclAllGather(seam words) -> verdict. A
+   refused composition is known on every rank from the same maps: each writes *d_flags = 1, *d_out_size = 0 (and 0 to d_out_offset and
+   d_total_size when given) and enters no further collective. cap >= 2 * (n_range + n_halo) is always enough (a copy-mode block decodes to
+   its own length); nothing is written past cap. Uses the handle's protected decode workspace. */
+DENSITY_B200_API int density_b200_decode_sharded_stream_protected(density_b200_sharded*, const uint8_t* d_in, size_t n_range, size_t n_halo,
+                                                 uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint64_t* d_out_offset,
+                                                 uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+/* The same for a Cheetah stream (maps of 0.83 MiB per rank), then the path of density_b200_decode_sharded_cheetah on the located piece
+   with its is_first / is_last: ncclAllGather(chunk-map transfers) -> fold -> phase 2 -> the rounds -> phase 3 -> ncclAllGather(seam
+   words) -> verdict. cap >= 16 * (n_range + n_halo) is always enough. */
+DENSITY_B200_API int density_b200_decode_sharded_cheetah_stream_protected(density_b200_sharded*, const uint8_t* d_in, size_t n_range,
+                                                         size_t n_halo, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                                         uint64_t* d_out_offset, uint32_t* d_flags, uint64_t* d_total_size,
+                                                         void* stream);
+
+/*
  * A reused Codec INSTANCE (streaming continuation). In the reference `encode` / `decode` are methods of an instance
  * (/root/reference/src/codec/codec.rs:16,72,82) whose dictionary survives from call to call until clear_state()
  * (chameleon.rs:148-150, cheetah.rs:198-202, lion.rs:327-331), while the protection state is created inside every call

@@ -141,6 +141,7 @@ _SIGS = {
     "density_b200_last_encode_was_fast": (ctypes.c_int, []),
     "density_b200_decode_status": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_cheetah_decode_rounds": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint32)]),
+    "density_b200_lion_decode_stats": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_encode_status": (ctypes.c_int, [ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_test_set_stage_rounds": (None, [ctypes.c_int]),
     "density_b200_test_set_decode_rounds": (None, [ctypes.c_int]),

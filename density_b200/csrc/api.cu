@@ -214,6 +214,9 @@ struct DeviceCtx {
     // One workspace per device: a call may only start using it when the previous call (on whatever stream) has finished with it.
     // Every enqueue ends with cudaEventRecord(ws_free, its stream) and starts with cudaStreamWaitEvent(its stream, ws_free).
     const void* last_cl_status = nullptr;   // iteration status block of the last parallel Cheetah decode (diagnostics)
+    // the walk counts of the last Lion decode, copied out of the workspace (which later calls reuse and may reallocate) behind the walk;
+    // lion_stats_valid is cleared when a Lion decode runs on the in-order kernel (diagnostics)
+    DevBuf lion_stats; bool lion_stats_valid = false;
     cudaEvent_t ws_free = nullptr;
     bool ws_free_recorded = false;
     std::mutex mu;
@@ -383,28 +386,35 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
             e = scalar_decode(alg, d_in, n, d_out, cap, c->ws.p + pw + 256, d_out_size, stream, &launches, d_nonquiet);
         return step_result(e, launches, "decode launch");
     }
-    if (alg == ALG_CHEETAH && path != 3 && !(reinterpret_cast<uintptr_t>(d_in) & 1) && !(reinterpret_cast<uintptr_t>(d_out) & 3)) {
-        // run-parallel Cheetah decoder (cl_decode.cu) + in-order tail; the exact in-order kernel is queued behind it and only runs if
-        // the context iteration did not settle within its round budget
-        const size_t pw = (chee_decode_workspace_bytes(n, cap, c->num_sms) + 255) & ~(size_t)255;
+    if ((alg == ALG_CHEETAH || alg == ALG_LION) && path != 3 && !(reinterpret_cast<uintptr_t>(d_in) & 1) && !(reinterpret_cast<uintptr_t>(d_out) & 3)) {
+        // run-parallel Cheetah decoder / parallel Lion decoder (cl_decode.cu) + in-order tail; the exact in-order kernel is queued behind
+        // it and only runs on a boundary error or (Cheetah) if the context iteration did not settle within its round budget
+        const bool lion = alg == ALG_LION;
+        const size_t pw = ((lion ? lion_decode_workspace_bytes(n, cap, c->num_sms) : chee_decode_workspace_bytes(n, cap, c->num_sms)) + 255) & ~(size_t)255;
         e = c->ws.ensure(pw + 256 + 2 * ((scalar_workspace_bytes(alg) + 255) & ~(size_t)255), stream);
-        if (e == cudaSuccess) e = c->dec_tables.ensure(chee_decode_tables_bytes(n, c->num_sms) + 256, stream);
+        if (e == cudaSuccess) e = c->dec_tables.ensure(chee_decode_tables_bytes(n, c->num_sms, lion) + 256, stream);
         if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
         uint32_t* d_fallback = reinterpret_cast<uint32_t*>(c->ws.p + pw);
         uint8_t* tail_ws = c->ws.p + pw + 256;
         uint8_t* scalar_ws = tail_ws + ((scalar_workspace_bytes(alg) + 255) & ~(size_t)255);
         e = cudaMemsetAsync(tail_ws, 0, 256, stream);
-        if (e == cudaSuccess) e = chee_decode_parallel(d_in, n, d_out, cap, c->ws.p, c->dec_tables.p, tail_ws, c->num_sms, d_out_size, d_fallback, stream, &launches);
+        if (e == cudaSuccess)
+            e = (lion ? lion_decode_parallel : chee_decode_parallel)(d_in, n, d_out, cap, c->ws.p, c->dec_tables.p, tail_ws, c->num_sms, d_out_size, d_fallback,
+                                                                     stream, &launches);
         if (e == cudaSuccess) {
             const void* cl_st = nullptr;
-            const void* b_st = chee_decode_status_ptr(c->ws.p, n, cap, c->num_sms, &cl_st);
-            c->last_cl_status = cl_st;
+            const void* b_st = (lion ? lion_decode_status_ptr : chee_decode_status_ptr)(c->ws.p, n, cap, c->num_sms, &cl_st);
+            if (!lion) c->last_cl_status = cl_st;
             e = scalar_decode_tail(alg, d_in, n, d_out, cap, tail_ws, b_st, cl_st, d_out_size, stream, &launches, d_fallback);
+            if (lion && e == cudaSuccess) e = c->lion_stats.ensure(64, stream);
+            if (lion && e == cudaSuccess) e = cudaMemcpyAsync(c->lion_stats.p, static_cast<const uint8_t*>(cl_st) + 32, 32, cudaMemcpyDeviceToDevice, stream);
+            if (lion) c->lion_stats_valid = e == cudaSuccess;
         }
         if (e == cudaSuccess && path != 1)
             e = scalar_decode(alg, d_in, n, d_out, cap, scalar_ws, d_out_size, stream, &launches, d_fallback);
         return step_result(e, launches, "decode launch");
     }
+    if (alg == ALG_LION) c->lion_stats_valid = false;
     e = c->ws.ensure(scalar_workspace_bytes(alg), stream);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     e = scalar_decode(alg, d_in, n, d_out, cap, c->ws.p, d_out_size, stream, &launches);
@@ -2351,6 +2361,7 @@ static size_t codec_run(density_b200_codec* h, bool encode, const uint8_t* in, s
     }
     if (e == cudaSuccess && !done) {
         // exact in-order kernel on the instance's state (Cheetah / Lion; Chameleon decode; a Chameleon encode whose copy map did not settle)
+        if (!encode && alg == ALG_LION) c->lion_stats_valid = false;
         e = encode ? scalar_encode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true)
                    : scalar_decode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true);
     }
@@ -2449,7 +2460,7 @@ void density_b200_shutdown(void) {
         DeviceCtx& c = g_ctx[d];
         if (!c.ready) continue;
         cudaSetDevice(d);
-        c.ws.release(); c.stage_in.release(); c.stage_out.release(); c.dec_tables.release(); for (int a2 = 0; a2 < 2; ++a2) for (int rg = 0; rg < 3; ++rg) c.chee_tables[a2][rg].release();
+        c.ws.release(); c.stage_in.release(); c.stage_out.release(); c.dec_tables.release(); c.lion_stats.release(); c.lion_stats_valid = false; for (int a2 = 0; a2 < 2; ++a2) for (int rg = 0; rg < 3; ++rg) c.chee_tables[a2][rg].release();
         c.chee_epoch = 0;
         if (c.d_size) cudaFree(c.d_size);
         if (c.h_size) cudaFreeHost(c.h_size);
@@ -2476,6 +2487,18 @@ int density_b200_cheetah_decode_rounds(uint32_t* out4) {
     if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(raw, c->last_cl_status, sizeof raw, cudaMemcpyDeviceToHost) != cudaSuccess) return DENSITY_B200_ECUDA;
     out4[0] = raw[3]; out4[1] = raw[2] && !raw[5]; out4[2] = raw[6]; out4[3] = chee_shard_max_rounds();   // cl_decode.cu MAX_ROUNDS
     return DENSITY_B200_OK;
+}
+
+/* diagnostic: the prediction walk of the last Lion decode on the current device (synchronises; DENSITY_B200_EARG when that decode ran
+   on the in-order kernel or there was none): out4 = {encoded quads walked, predicted quads, table reads that waited on a predicted quad,
+   rows walked} */
+int density_b200_lion_decode_stats(uint64_t* out4) {
+    DeviceCtx* c = current_ctx();
+    if (!c || !out4) return DENSITY_B200_EARG;
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (cudaDeviceSynchronize() != cudaSuccess) return DENSITY_B200_ECUDA;
+    if (!c->lion_stats_valid) return DENSITY_B200_EARG;
+    return cudaMemcpy(out4, c->lion_stats.p, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost) == cudaSuccess ? DENSITY_B200_OK : DENSITY_B200_ECUDA;
 }
 
 /* test hook: rounds per stage of the Cheetah / Lion copy-map iteration (1..7; 7 = default) */

@@ -26,13 +26,15 @@
 //                       piece's table transfer (cd_pred_export, into cd_pred_fold) and exit context (cd_round_words, into
 //                       cd_shard_round_end); the rounds stop for all pieces at once when none of them walked a run.
 //
-// Lion is NOT decoded here: its 5-deep move-to-front lists make the same iteration advance one run per round (a misplaced
-// operation desynchronises a whole list; measured in tests/cl_model.cpp), so lion_decode stays on the in-order kernel.
+// Lion runs stages 0-2 on its own geometry (64-byte blocks, two per row of 32 quads) and the tail, but not the rounds: its 5-deep
+// move-to-front lists make them advance one run per round (a misplaced operation desynchronises a whole list; measured in
+// tests/cl_model.cpp). Stage 3 is instead one walk in stream order, 32 quads per step (ld_walk, lion_walk.cuh), which never gives up.
 #include <stdlib.h>
 #include "common.cuh"
 #include "encode_internal.cuh"
 #include "decode_bounds.cuh"
 #include "cl_core.cuh"
+#include "lion_walk.cuh"
 
 namespace dns {
 namespace cheedec {
@@ -55,35 +57,51 @@ struct ClStatus {
 __device__ __forceinline__ uint64_t run_step_begin(uint32_t r, uint32_t nruns, uint64_t nsteps) { return (uint64_t)r * nsteps / nruns; }
 
 // ---- 1. unpack ------------------------------------------------------------------------------------------------------------------
-// flags[b] = {predicted, MAP_A, MAP_B, active} bit per quad (LSB-first signature, read_signature.rs:11-16)
+// One warp per row of 32 quads (128 output bytes): one Cheetah block, or two Lion blocks (lanes 0-15 and 16-31), as the Lion encoder
+// lays them out. flags[s] = {predicted, MAP_A, MAP_B, encoded} bit per lane (LSB-first signature, read_signature.rs:11-16); K = the
+// 16-bit hash of a not-predicted quad, the depth (flag - 1, lion.rs:123-186) of a predicted one (0 for Cheetah).
+template <class G> __device__ __forceinline__ uint64_t cd_steps(const DecStatus* st) { return (st->main_blocks * (G::BS / 4) + 31) / 32; }
+
+template <class G>
 __global__ void cd_unpack(const uint8_t* __restrict__ in, const uint64_t* __restrict__ blk_off, const DecStatus* __restrict__ st,
                           uint4* __restrict__ flags, uint16_t* __restrict__ K, uint32_t* __restrict__ out) {
     if (st->error) return;
+    constexpr bool LION = G::BS == 64;
+    constexpr uint32_t QPB = G::BS / 4, FB = LION ? 3 : 2;
     const uint32_t lane = threadIdx.x & 31;
-    const uint64_t nb = st->main_blocks;
-    for (uint64_t b = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); b < nb; b += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const unsigned long long o = blk_off[b];
+    const uint32_t mine = QPB == 32 ? 0xFFFFFFFFu : (lane < 16 ? 0x0000FFFFu : 0xFFFF0000u);   // the lanes of my block
+    const uint64_t nb = st->main_blocks, ns = cd_steps<G>(st);
+    for (uint64_t s = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); s < ns; s += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
+        const uint64_t b = s * (32 / QPB) + lane / QPB;
+        const uint32_t q = lane % QPB;
+        const unsigned long long o = b < nb ? blk_off[b] : BLK_COPY;
+        const bool enc = b < nb && !(o & BLK_COPY);
         const uint8_t* p = in + (o & ~BLK_COPY);
-        if (o & BLK_COPY) {                                        // codec.rs:89-92: 128 raw bytes
-            out[b * 32 + lane] = ldu16(p + 4 * lane) | (ldu16(p + 4 * lane + 2) << 16);
-            if (lane == 0) flags[b] = make_uint4(0, 0, 0, 0);
-            continue;
+        if (b < nb && !enc)                                        // codec.rs:89-92: BS raw bytes
+            out[s * 32 + lane] = ldu16(p + 4 * q) | (ldu16(p + 4 * q + 2) << 16);
+        uint32_t flag = 0, kind = K_PRED;
+        if (enc) {
+            const uint64_t sig = LION ? ((uint64_t)(ldu16(p) | (ldu16(p + 2) << 16)) | ((uint64_t)ldu16(p + 4) << 32)) : bounds::ldsig(p);
+            flag = (uint32_t)(sig >> (FB * q)) & ((1u << FB) - 1u);
+            kind = LION ? lion_kind(flag) : cheetah_kind(flag);
         }
-        const uint32_t slo = ldu16(p) | (ldu16(p + 2) << 16), shi = ldu16(p + 4) | (ldu16(p + 6) << 16);
-        const uint32_t flag = ((lane < 16 ? slo : shi) >> (2 * (lane & 15))) & 3u;
-        const uint32_t plain = __ballot_sync(0xFFFFFFFFu, flag == K_PLAIN);
-        const uint32_t ma = __ballot_sync(0xFFFFFFFFu, flag == K_MAP_A), mb = __ballot_sync(0xFFFFFFFFu, flag == K_MAP_B);
-        const uint8_t* q = p + 8 + 4 * __popc(plain & lanemask_lt()) + 2 * __popc((ma | mb) & lanemask_lt());
+        const uint32_t act = __ballot_sync(0xFFFFFFFFu, enc);
+        const uint32_t plain = __ballot_sync(0xFFFFFFFFu, enc && kind == K_PLAIN);
+        const uint32_t ma = __ballot_sync(0xFFFFFFFFu, enc && kind == K_MAP_A), mb = __ballot_sync(0xFFFFFFFFu, enc && kind == K_MAP_B);
+        const uint32_t lt = lanemask_lt() & mine;
+        const uint8_t* d = p + G::SIG + 4 * __popc(plain & lt) + 2 * __popc((ma | mb) & lt);
         uint32_t k = 0;
-        if (flag == K_PLAIN) { const uint32_t v = ldu16(q) | (ldu16(q + 2) << 16); out[b * 32 + lane] = v; k = hash16(v); }   // cheetah.rs:68-70
-        else if (flag != K_PRED) k = ldu16(q);                                                                                  // cheetah.rs:78,88
-        K[b * 32 + lane] = (uint16_t)k;
-        if (lane == 0) flags[b] = make_uint4(~(plain | ma | mb), ma, mb, 0xFFFFFFFFu);
+        if (enc && kind == K_PLAIN) { const uint32_t v = ldu16(d) | (ldu16(d + 2) << 16); out[s * 32 + lane] = v; k = hash16(v); }   // cheetah.rs:68-70, lion.rs:86-87
+        else if (enc && kind != K_PRED) k = ldu16(d);                                                                                 // cheetah.rs:78,88, lion.rs:100,112
+        else if (LION && enc) k = lion_depth(flag);
+        K[s * 32 + lane] = (uint16_t)k;
+        if (lane == 0) flags[s] = make_uint4(act & ~(plain | ma | mb), ma, mb, act);
     }
 }
 
 // ---- 2. chunk-map values ------------------------------------------------------------------------------------------------------------
 // entry per (run, bucket): {a, b, meta, 0}; meta = epoch << 20 | tags (cl_core.cuh). The tables are zeroed per call: epoch 1 = touched.
+template <class G>
 __global__ void __launch_bounds__(RP_WARPS * 32)
 cd_cmap_walk(const DecStatus* __restrict__ st, uint32_t nruns, const uint4* __restrict__ flags, const uint16_t* __restrict__ K,
              uint4* __restrict__ entC_all, uint32_t* __restrict__ out, uint2* __restrict__ usym /* per block: reads of carried-in slot 0 / slot 1 */) {
@@ -91,7 +109,7 @@ cd_cmap_walk(const DecStatus* __restrict__ st, uint32_t nruns, const uint4* __re
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t r = blockIdx.x * RP_WARPS + (threadIdx.x >> 5);
     if (r >= nruns) return;
-    const uint64_t nsteps = st->main_blocks;
+    const uint64_t nsteps = cd_steps<G>(st);
     const uint64_t s0 = run_step_begin(r, nruns, nsteps), s1 = run_step_begin(r + 1, nruns, nsteps);
     uint4* __restrict__ entC = entC_all + (size_t)r * 65536;
     for (uint64_t s = s0; s < s1; ++s) {
@@ -167,11 +185,12 @@ __device__ __forceinline__ uint32_t run_of_step(uint64_t s, uint32_t nruns, uint
 }
 
 // reads that hit a carried-in slot
+template <class G>
 __global__ void cd_cmap_resolve(const DecStatus* __restrict__ st, uint32_t nruns, const uint2* __restrict__ usym, const uint16_t* __restrict__ K,
                                 const uint2* __restrict__ cin, uint32_t* __restrict__ out) {
     if (st->error) return;
     const uint32_t lane = threadIdx.x & 31;
-    const uint64_t nsteps = st->main_blocks;
+    const uint64_t nsteps = cd_steps<G>(st);
     for (uint64_t s = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); s < nsteps; s += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
         const uint2 u = usym[s];
         if ((u.x | u.y) == 0) continue;
@@ -361,6 +380,49 @@ __global__ void cd_finish(const DecStatus* __restrict__ st, ClStatus* __restrict
     if (!ok && !st->error) cs->gave_up = 1;
     *d_fallback = ok ? 0u : 1u;
     if (!ok && d_out_size) *d_out_size = 0;
+}
+
+// ---- 3'. Lion: the prediction walk ---------------------------------------------------------------------------------------------------
+// lion.rs:50-57,125-186 over every encoded quad in stream order (lion_walk.cuh): one warp, one row of 32 quads per step, the next row's
+// stream data loaded during this row and later rows pulled into L2. The walk never gives up. The table (5 x u32 per context, zeroed per
+// call, lion.rs:70) is the tail's, in the workspace, where the tail continues on it. A CTA whose producer warps fill a shared-memory
+// ring ahead of the walker, and that ring with the table in an 8-CTA cluster's distributed shared memory, measured slower on text and
+// synth_mixed (DESIGN.md section 8).
+// status: a ClStatus prefix (final_ctx for the tail, done for cd_finish) followed by the walk's counts (density_b200_lion_decode_stats).
+struct LionStatus { ClStatus c; unsigned long long quads, pred, dep, rows; };
+constexpr uint32_t LW_PREFETCH = 16;                       // rows ahead whose stream data is pulled into L2 while the walk works
+
+__global__ void __launch_bounds__(32) ld_walk(const DecStatus* __restrict__ st, const uint4* __restrict__ flags, const uint16_t* __restrict__ K,
+                                              uint32_t* __restrict__ out, uint32_t* __restrict__ T, LionStatus* __restrict__ ls) {
+#if defined(__CUDA_ARCH__)                                   // lwalk::Warp / LV are the device lanes only in the device pass
+    if (st->error) return;
+    using namespace lwalk;
+    Warp w{(int)(threadIdx.x & 31)};
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t ns = cd_steps<bounds::LionT>(st);
+    const FlatTable tab{T};
+    WalkCounts cnt{0, 0, 0, 0};
+    uint32_t carry = 0;                                    // lion.rs:67
+    uint4 fl_n = make_uint4(0, 0, 0, 0); uint32_t k_n = 0, v_n = 0;
+    if (ns) { fl_n = flags[0]; k_n = K[lane]; v_n = out[lane]; }
+    for (uint64_t s = 0; s < ns; ++s) {
+        const uint4 fl = fl_n;
+        LV<uint32_t> kh{k_n}, v{v_n};
+        if (s + 1 < ns) { fl_n = flags[s + 1]; k_n = K[(s + 1) * 32 + lane]; v_n = out[(s + 1) * 32 + lane]; }
+        if (s + LW_PREFETCH < ns) {
+            const uint64_t f = s + LW_PREFETCH;
+            if (lane == 0) asm volatile("prefetch.global.L2 [%0];" :: "l"(flags + f));
+            if (lane == 1) asm volatile("prefetch.global.L2 [%0];" :: "l"(K + f * 32));
+            if (lane == 2) asm volatile("prefetch.global.L2 [%0];" :: "l"(out + f * 32));
+        }
+        walk_row(w, fl.x, fl.w, kh, v, tab, carry, cnt);
+        if ((fl.x >> lane) & 1u) out[s * 32 + lane] = v.x;
+    }
+    if (lane == 0) {
+        ls->c.final_ctx = carry; ls->c.done = 1; ls->c.rounds = 1;
+        ls->quads = cnt.quads; ls->pred = cnt.pred; ls->dep = cnt.dep; ls->rows = cnt.rows;
+    }
+#endif
 }
 
 // ---- 5. sharded decode: one piece of a longer stream --------------------------------------------------------------------------------
@@ -604,28 +666,33 @@ static uint32_t cd_pick_runs(size_t nbytes, int num_sms) {
     return (uint32_t)r;
 }
 
-static size_t cd_layout(size_t nbytes, size_t cap, uint32_t nruns, CheeDecLayout* L) {
-    size_t off = bounds::bounds_layout<bounds::CheeT>(nbytes, cap, &L->B);
+// lion: the Lion geometry (two blocks per row) and no prediction-round arrays (the walk replaces the rounds)
+static size_t cd_layout(size_t nbytes, size_t cap, uint32_t nruns, CheeDecLayout* L, bool lion = false) {
+    size_t off = lion ? bounds::bounds_layout<bounds::LionT>(nbytes, cap, &L->B) : bounds::bounds_layout<bounds::CheeT>(nbytes, cap, &L->B);
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const uint64_t mb = L->B.maxblocks;
-    L->cs = take(sizeof(ClStatus));
-    L->flags = take(mb * sizeof(uint4));
-    L->K = take(mb * 32 * sizeof(uint16_t));
-    L->usym = take(mb * sizeof(uint2));
-    L->ctx_in = take((size_t)nruns * 4 + 64);
-    L->ctx_out = take((size_t)nruns * 4 + 64);
-    L->dirty = take((size_t)nruns * 8 + 64);
-    L->run_epoch = take((size_t)nruns * 4 + 64);
-    L->rbits = take((size_t)nruns * 2048 * sizeof(uint32_t));
+    const uint64_t ms = lion ? (L->B.maxblocks + 1) / 2 : L->B.maxblocks;   // rows of 32 quads
+    const size_t rr = lion ? 0 : nruns;                                       // runs with prediction-round arrays
+    L->cs = take(lion ? sizeof(LionStatus) : sizeof(ClStatus));
+    L->flags = take(ms * sizeof(uint4));
+    L->K = take(ms * 32 * sizeof(uint16_t));
+    L->usym = take(ms * sizeof(uint2));
+    L->ctx_in = take(rr * 4 + 64);
+    L->ctx_out = take(rr * 4 + 64);
+    L->dirty = take(rr * 8 + 64);
+    L->run_epoch = take(rr * 4 + 64);
+    L->rbits = take(rr * 2048 * sizeof(uint32_t));
     L->cin = take((size_t)nruns * 65536 * sizeof(uint2));
-    L->snap0 = take((size_t)nruns * 65536 * sizeof(uint32_t));
+    L->snap0 = take(rr * 65536 * sizeof(uint32_t));
     L->total = off;
     return off;
 }
 
 size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms) { CheeDecLayout L; return cd_layout(nbytes, cap, cd_pick_runs(nbytes, num_sms), &L); }
-// the per-run tables (zeroed at the start of every call): chunk map 16 B, prediction 8 B per run and key
-size_t chee_decode_tables_bytes(size_t nbytes, int num_sms) { return (size_t)cd_pick_runs(nbytes, num_sms) * 65536 * (sizeof(uint4) + sizeof(uint2)); }
+// the per-run tables (zeroed at the start of every call): chunk map 16 B, prediction 8 B per run and key (Lion: the chunk map only)
+size_t chee_decode_tables_bytes(size_t nbytes, int num_sms, bool lion) {
+    return (size_t)cd_pick_runs(nbytes, num_sms) * 65536 * (sizeof(uint4) + (lion ? 0 : sizeof(uint2)));
+}
+size_t lion_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms) { CheeDecLayout L; return cd_layout(nbytes, cap, cd_pick_runs(nbytes, num_sms), &L, true); }
 
 // The decoder's view of one call: the run geometry, the boundary layout and typed pointers into the workspace (cd_layout), the per-run
 // tables and the tail's tables (the scalar_codec.cu workspace: Status (256 B) + chunk_a + chunk_b + pred), which receive the folded
@@ -637,11 +704,11 @@ struct CheeDecPtrs {
     DecStatus* st; ClStatus* cs; uint64_t* blk_off; uint4* flags; uint16_t* K; uint2* usym;
     uint32_t *ctx_in, *ctx_out, *dirty_cur, *dirty_next, *run_epoch, *rbits, *snap, *fallback, *chunk_a, *chunk_b, *pred_final;
     uint2* cin; uint8_t* tables; size_t tables_bytes; uint4* entC; uint2* entP; PieceStatus* pst; uint8_t* tail_ws;
-    CheeDecPtrs(size_t n, size_t cap, int num_sms, uint8_t* ws, uint8_t* tables_, uint8_t* tail_ws_) {
+    CheeDecPtrs(size_t n, size_t cap, int num_sms, uint8_t* ws, uint8_t* tables_, uint8_t* tail_ws_, bool lion = false) {
         nruns = cd_pick_runs(n, num_sms);
         run_ctas = (nruns + RP_WARPS - 1) / RP_WARPS;
         wide = num_sms * 8;
-        CheeDecLayout L; cd_layout(n, cap, nruns, &L);
+        CheeDecLayout L; cd_layout(n, cap, nruns, &L, lion);
         B = L.B;
         const size_t off = (L.total + 255) & ~(size_t)255;
         st = reinterpret_cast<DecStatus*>(ws + L.B.status);
@@ -664,9 +731,9 @@ struct CheeDecPtrs {
         chunk_a = reinterpret_cast<uint32_t*>(tail_ws + 256);
         chunk_b = chunk_a + PL;
         pred_final = chunk_a + 2 * PL;
-        tables = tables_; tables_bytes = chee_decode_tables_bytes(n, num_sms);
+        tables = tables_; tables_bytes = chee_decode_tables_bytes(n, num_sms, lion);
         entC = reinterpret_cast<uint4*>(tables);
-        entP = tables ? reinterpret_cast<uint2*>(tables + (size_t)nruns * PL * sizeof(uint4)) : nullptr;
+        entP = tables && !lion ? reinterpret_cast<uint2*>(tables + (size_t)nruns * PL * sizeof(uint4)) : nullptr;
     }
 };
 
@@ -674,21 +741,26 @@ struct CheeDecPtrs {
 // the per-run tables and run 0's snapshot (the zero table) start every call as zeros
 static cudaError_t cd_clear_tables(const CheeDecPtrs& p, cudaStream_t stream) {
     cudaError_t e = cudaMemsetAsync(p.tables, 0, p.tables_bytes, stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(p.snap, 0, (size_t)p.nruns * PL * sizeof(uint32_t), stream);
+    if (e == cudaSuccess && p.entP) e = cudaMemsetAsync(p.snap, 0, (size_t)p.nruns * PL * sizeof(uint32_t), stream);
     return e;
 }
 // unpack (literals and copy-mode blocks go straight to the output) and the symbolic chunk-map walk
+template <class G = bounds::CheeT>
 static void cd_launch_unpack_walk(const CheeDecPtrs& p, const uint8_t* d_in, uint32_t* out32, cudaStream_t stream, uint64_t* launches) {
-    cd_unpack<<<p.wide, 256, 0, stream>>>(d_in, p.blk_off, p.st, p.flags, p.K, out32);
-    cd_cmap_walk<<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.entC, out32, p.usym);
+    cd_unpack<G><<<p.wide, 256, 0, stream>>>(d_in, p.blk_off, p.st, p.flags, p.K, out32);
+    cd_cmap_walk<G><<<p.run_ctas, RP_WARPS * 32, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.entC, out32, p.usym);
     *launches += 2;
 }
-// the chunk map carried in (d_cmap_carry: nullptr = the stream start), the reads of carried-in slots, the context init
+// the chunk map carried in (d_cmap_carry: nullptr = the stream start), the reads of carried-in slots, the context init (Cheetah)
+template <class G = bounds::CheeT>
 static void cd_launch_cmap_resolve(const CheeDecPtrs& p, uint32_t* out32, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
     cd_cmap_fold<<<PL / 128, 128, 0, stream>>>(p.st, p.nruns, p.entC, p.cin, p.chunk_a, p.chunk_b, d_cmap_carry);
-    cd_cmap_resolve<<<p.wide, 256, 0, stream>>>(p.st, p.nruns, p.usym, p.K, p.cin, out32);
-    cd_ctx_init<<<(p.nruns + 127) / 128, 128, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.ctx_in, p.dirty_cur, p.dirty_next, p.run_epoch, p.cs);
-    *launches += 3;
+    cd_cmap_resolve<G><<<p.wide, 256, 0, stream>>>(p.st, p.nruns, p.usym, p.K, p.cin, out32);
+    *launches += 2;
+    if (G::BS == 128) {
+        cd_ctx_init<<<(p.nruns + 127) / 128, 128, 0, stream>>>(p.st, p.nruns, p.flags, p.K, p.ctx_in, p.dirty_cur, p.dirty_next, p.run_epoch, p.cs);
+        ++*launches;
+    }
 }
 // a prediction round: walk the dirty runs (run0_snap: run 0 starts from the stream start's zero table) ...
 static void cd_launch_pred_walk(const CheeDecPtrs& p, uint32_t round, uint32_t* out32, uint32_t run0_snap, cudaStream_t stream, uint64_t* launches) {
@@ -733,6 +805,34 @@ cudaError_t chee_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
 const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** cl_status) {
     const CheeDecPtrs p(nbytes, cap, num_sms, ws, nullptr, nullptr);
     if (cl_status) *cl_status = p.cs;
+    return p.st;
+}
+
+// Enqueues the parallel Lion decode: boundaries, unpack, the chunk-map passes (the Cheetah decoder's kernels on the Lion geometry), the
+// prediction walk on the tail's table, the verdict. *d_fallback != 0 afterwards (a boundary error: malformed stream or capacity): the
+// caller's in-order kernel must run instead. `tail_ws` = the scalar workspace: receives the chunk map and the walked table for the tail.
+cudaError_t lion_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
+                                 int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches) {
+    const CheeDecPtrs p(nbytes, cap, num_sms, ws, tables, tail_ws, true);
+    LionStatus* ls = reinterpret_cast<LionStatus*>(p.cs);
+    cudaError_t e = bounds::bounds_launch<bounds::LionT>(d_in, nbytes, cap, ws, p.B, stream, launches);
+    if (e == cudaSuccess) e = cd_clear_tables(p, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ls, 0, sizeof(LionStatus), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.pred_final, 0, (size_t)5 * PL * sizeof(uint32_t), stream);   // lion.rs:70
+    if (e != cudaSuccess) return e;
+    uint32_t* out32 = reinterpret_cast<uint32_t*>(d_out);
+    cd_launch_unpack_walk<bounds::LionT>(p, d_in, out32, stream, launches);
+    cd_launch_cmap_resolve<bounds::LionT>(p, out32, nullptr, stream, launches);
+    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, out32, p.pred_final, ls);
+    ++*launches;
+    cd_launch_finish(p, d_fallback, d_out_size, stream, launches);
+    return cudaGetLastError();
+}
+
+// device addresses the tail kernel needs: boundary status + walk status (its ClStatus prefix; the counts follow it)
+const void* lion_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** walk_status) {
+    const CheeDecPtrs p(nbytes, cap, num_sms, ws, nullptr, nullptr, true);
+    if (walk_status) *walk_status = p.cs;
     return p.st;
 }
 

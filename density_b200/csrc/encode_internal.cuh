@@ -182,12 +182,18 @@ cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
 cudaError_t cham_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
                                     uint64_t* launches);
 
-// cl_decode.cu (run-parallel Cheetah decode)
+// cl_decode.cu (run-parallel Cheetah decode; parallel Lion decode with the prediction walk)
 size_t chee_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);
-size_t chee_decode_tables_bytes(size_t nbytes, int num_sms);
+size_t chee_decode_tables_bytes(size_t nbytes, int num_sms, bool lion = false);
 cudaError_t chee_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
                                  int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches);
 const void* chee_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** cl_status);
+// Lion: the same workspace contract (tables: chee_decode_tables_bytes(.., true)); the walk status behind *walk_status is a ClStatus prefix
+// followed by 4 u64 counts {encoded quads, predicted quads, table reads that waited on a predicted quad, rows}
+size_t lion_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);
+cudaError_t lion_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
+                                 int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches);
+const void* lion_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** walk_status);
 // sharded Cheetah decode: one piece of a longer stream (first: it holds the stream start; last: no stream byte follows it). ws holds
 // chee_shard_workspace_bytes, tables chee_decode_tables_bytes of the piece. Phase 1, phase 2, then any number of rounds (walk, exchange,
 // fold), then phase 3; every call of one piece gets the same arguments. Chunk-map tables: 3 planes {tags, a, b} of 65536 u32.
@@ -232,9 +238,9 @@ cudaError_t scalar_encode(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* 
                           uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_run_if_zero = nullptr, bool keep_state = false);
 cudaError_t scalar_decode(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws,
                           uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_run_if = nullptr, bool keep_state = false);
-// tail loop only (codec.rs:102-123), continuing from the state the parallel decoder left: tables already in `ws`, boundary status
-// (bounds::DecStatus: tail offset, block count, protection state) and the last hash (cheedec::ClStatus::final_ctx) on the device;
-// runs only if *d_skip_if == 0
+// tail loop only (codec.rs:102-123), Cheetah or Lion, continuing from the state the parallel decoder left: tables already in `ws`,
+// boundary status (bounds::DecStatus: tail offset, block count, protection state) and the last hash (cheedec::ClStatus::final_ctx) on
+// the device; runs only if *d_skip_if == 0
 cudaError_t scalar_decode_tail(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, const void* d_bounds_status,
                                const void* d_cl_status, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_skip_if);
 

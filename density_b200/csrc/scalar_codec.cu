@@ -321,11 +321,13 @@ cudaError_t scalar_decode(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* 
 
 cudaError_t scalar_decode_tail(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, const void* d_bounds_status,
                                const void* d_cl_status, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_skip_if) {
-    if (alg != ALG_CHEETAH) return cudaErrorInvalidValue;
-    scalar::Tables T = carve(alg, ws);   // the folds of cl_decode.cu have filled chunk_a / chunk_b / pred
+    if (alg != ALG_CHEETAH && alg != ALG_LION) return cudaErrorInvalidValue;
+    scalar::Tables T = carve(alg, ws);   // cl_decode.cu has filled chunk_a / chunk_b (the fold) and pred (the Cheetah fold / the Lion walk)
     Status* st = reinterpret_cast<Status*>(ws);
-    scalar::decode_tail_kernel<ALG_CHEETAH><<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, T, st, reinterpret_cast<const bounds::DecStatus*>(d_bounds_status),
-                                                                  reinterpret_cast<const scalar::TailIter*>(d_cl_status), d_out_size, d_skip_if);
+    const bounds::DecStatus* tb = reinterpret_cast<const bounds::DecStatus*>(d_bounds_status);
+    const scalar::TailIter* ti = reinterpret_cast<const scalar::TailIter*>(d_cl_status);
+    if (alg == ALG_CHEETAH) scalar::decode_tail_kernel<ALG_CHEETAH><<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, T, st, tb, ti, d_out_size, d_skip_if);
+    else scalar::decode_tail_kernel<ALG_LION><<<1, 32, 0, stream>>>(d_in, nbytes, d_out, cap, T, st, tb, ti, d_out_size, d_skip_if);
     ++*launches;
     return cudaGetLastError();
 }

@@ -52,9 +52,10 @@ DENSITY_B200_API size_t cheetah_decode(const uint8_t* input, size_t input_size, 
 DENSITY_B200_API size_t cheetah_safe_encode_buffer_size(size_t size);
 
 DENSITY_B200_API size_t lion_encode(const uint8_t* input, size_t input_size, uint8_t* output, size_t output_size);
-/* PERFORMANCE LIMIT: lion_decode runs on the exact in-order device kernel (one thread, ~10-20 MB/s): no parallel formulation of the
-   5-deep move-to-front prediction lists that beats in-order is known (DESIGN.md section 4c). Results are bit-exact; for streams
-   beyond a few MiB the reference's CPU decoder is the faster choice for this one symbol. All other eight symbols run parallel kernels. */
+/* PERFORMANCE LIMIT: lion_decode runs the parallel Lion decoder: boundaries, unpack and chunk-map values in parallel, then one warp
+   walks the 5-deep prediction lists in stream order, 32 quads per step (DESIGN.md section 4c). That walk is serial over the whole
+   stream: 0.05-0.22 GB/s measured on an H100 (README.md), 3.6-7x the in-order kernel but below the reference's CPU decoder, which
+   stays the faster choice for large streams for this one symbol. Results are bit-exact. */
 DENSITY_B200_API size_t lion_decode(const uint8_t* input, size_t input_size, uint8_t* output, size_t output_size);
 DENSITY_B200_API size_t lion_safe_encode_buffer_size(size_t size);
 
@@ -100,9 +101,10 @@ DENSITY_B200_API int density_b200_encode_device(int alg, const uint8_t* d_in, si
    4 = like 0 but may BLOCK: the host reads the verdict and resumes the iteration (up to 12 times) before the in-order kernel. */
 DENSITY_B200_API int density_b200_encode_device_path(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                     uint64_t* d_out_size, void* stream, int path);
-/* Decode counterpart: path 0 = auto (parallel Chameleon decoder, also for streams with copy-mode blocks; the exact in-order
-   kernel is queued behind it as a safety net and for Cheetah / Lion), 1 = parallel decoder only (size 0 if it had to give
-   up), 3 = in-order kernel only. */
+/* Decode counterpart: path 0 = auto (the parallel decoder of each algorithm, also for streams with copy-mode blocks; the exact
+   in-order kernel is queued behind it as a safety net: it runs when the parallel decoder gives up — Cheetah: the context iteration
+   did not settle; all: a malformed stream or a capacity error — and when d_in is not 2-byte or d_out not 4-byte aligned),
+   1 = parallel decoder only (size 0 if it had to give up), 3 = in-order kernel only. */
 DENSITY_B200_API int density_b200_decode_device_path(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                     uint64_t* d_out_size, void* stream, int path);
 /* Diagnostic: status of the last Chameleon encode on the current device (synchronises the device):
@@ -115,6 +117,10 @@ DENSITY_B200_API int density_b200_decode_status(uint64_t* out10);
 /* Diagnostic: the context iteration of the last run-parallel Cheetah decode on the current device (synchronises the device):
    out4 = {rounds used, settled (0: the in-order kernel took over), run walks after round 0, round budget}. */
 DENSITY_B200_API int density_b200_cheetah_decode_rounds(uint32_t* out4);
+/* Diagnostic: the prediction walk of the last Lion decode on the current device (synchronises the device):
+   out4 = {encoded quads walked, predicted quads, table reads that waited on a predicted quad, rows of 32 quads walked}.
+   DENSITY_B200_EARG when that decode ran on the in-order kernel (path 3, misaligned buffers, codec instances) or there was none. */
+DENSITY_B200_API int density_b200_lion_decode_stats(uint64_t* out4);
 /* Same contract for decode; `cap` must be >= the original length. */
 DENSITY_B200_API int density_b200_decode_device(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                uint64_t* d_out_size, void* stream);

@@ -199,9 +199,10 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
     // ---- A
 #pragma unroll
     for (int j = 0; j < F6_QPT; ++j) {
+        // prod_hash / prod_fp written as multiplies, so they issue on the FMA pipe beside the integer ALU work (p is even)
         const uint32_t p = hash_prod(q[j]);
-        h[j] = prod_hash(p);
-        f[j] = prod_fp(p, q[j]);
+        h[j] = __umulhi(p, 0x10000u);
+        f[j] = __umulhi(q[j], 2u) + (p - h[j] * 0x10000u);
         old[j] = S.tab[h[j]];
     }
     uint32_t fmin = f[0];
@@ -228,14 +229,20 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
     // ---- C
     uint32_t clean[F6_QPT], base = 0;
     uint2* __restrict__ myrec = S.rec + warp * F6_WQ;
+    const uint32_t ltmask = lanemask_lt();
 #pragma unroll
     for (int j = 0; j < F6_QPT; ++j) {
-        bool dirty = (missmask >> j) & 1u;
-        if (!dirty) dirty = S.tab[h[j]] != f[j];
+        // straight-line: the re-read and the record store are predicated, the record words are formed whether or not they are stored
+        const bool miss = (missmask >> j) & 1u;
+        uint32_t now = f[j];
+        if (!miss) now = S.tab[h[j]];
+        bool dirty = miss || now != f[j];
         if (GENERIC) dirty = dirty && ((validmask >> j) & 1u);
         const uint32_t db = __ballot_sync(0xFFFFFFFFu, dirty);
         clean[j] = GENERIC ? __ballot_sync(0xFFFFFFFFu, !dirty && ((validmask >> j) & 1u)) : ~db;
-        if (dirty) myrec[base + __popc(db & lanemask_lt())] = make_uint2(h[j] | (f[j] << 16), (pos0 + 32 * j) | (old[j] << 16));
+        const uint2 rv = make_uint2(f[j] * 0x10000u + h[j], old[j] * 0x10000u + (pos0 + 32 * j));
+        const uint32_t k = base + __popc(db & ltmask);
+        if (dirty) myrec[k] = rv;
         base += __popc(db);
     }
     if (lane == 0) {
@@ -251,21 +258,20 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
     uint2 r0 = make_uint2(0, 0);
     bool drop0 = false;
     {
-        uint32_t carry_x = 0, carry_pos = 0;   // record before lane 0's (previous step's lane 31); record 0 has none
         #pragma unroll 1
         for (uint32_t i0 = 0; i0 < base; i0 += 32) {
             const uint32_t i = i0 + lane;
             const bool valid = i < base;
-            uint2 r = make_uint2(0xFFFFFFFFu, 0);
-            if (valid) {
-                r = myrec[i];
-                // "bucket touched before this tile": the pre-tile fingerprint, or the touched bit when that is 0 (stable until phase D)
-                if ((r.y >> 16) != 0 || bit_test(S.vbit, r.x & 0xFFFFu)) r.y |= F6_TOUCHED;
-            }
-            uint32_t px = __shfl_up_sync(0xFFFFFFFFu, r.x, 1), ppos = __shfl_up_sync(0xFFFFFFFFu, r.y & 0xFFFu, 1);
-            if (lane == 0) { px = carry_x; ppos = carry_pos; }
-            const bool drop = valid && i != 0 && px == r.x && ppos + 1 == (r.y & 0xFFFu);
-            carry_x = __shfl_sync(0xFFFFFFFFu, r.x, 31); carry_pos = __shfl_sync(0xFFFFFFFFu, r.y & 0xFFFu, 31);
+            uint2 r = make_uint2(0xFFFFFFFFu, 0), pr = r;   // pr: the record before mine (its x and position are never rewritten)
+            __syncwarp();                               // the previous step's flag writes precede these reads
+            if (valid) r = myrec[i];
+            if (valid && i != 0) pr = myrec[i - 1];
+            __syncwarp();                               // ... and these reads precede this step's flag writes
+            // "bucket touched before this tile": the pre-tile fingerprint, or the touched bit when that is 0 (stable until phase D)
+            uint32_t tch = r.y >> 16;
+            if (valid && tch == 0) tch = S.vbit[(r.x & 0xFFFFu) >> 5] & (1u << (r.x & 31u));
+            if (valid && tch != 0) r.y |= F6_TOUCHED;
+            const bool drop = valid && i != 0 && pr.x == r.x && (((pr.y + 1u) ^ r.y) & 0xFFFu) == 0;
             if (i0 == 0) { r0 = r; drop0 = drop; }
             if (drop) {
                 const uint32_t pos = r.y & 0xFFFu;
@@ -305,18 +311,18 @@ __device__ __forceinline__ void f6_tile(Flag6Smem& S, const uint32_t (&q)[F6_QPT
             const uint32_t myidx = warp * F6_WQ + i;
             bool later = false, hit = false, unres = false;
             if (valid) {
-                const uint32_t n = (S.mbcnt[buf][slot >> 2] >> ((slot & 3u) * 8u)) & 0xFFu;
+                const uint32_t n = (S.mbcnt[buf][slot >> 2] >> ((slot & 3u) * 8u)) & 0xFFu;   // >= 1: my own entry
                 const uint2 e2 = *reinterpret_cast<const uint2*>(&S.mb[slot][0]);
-                const uint32_t me = ((hh >> 12) << 12) | myidx;
-                int best = -1;
-#pragma unroll
-                for (int t = 0; t < F6_MB_CAP; ++t) {
-                    const uint32_t e = ((t & 2) ? e2.y : e2.x) >> ((t & 1) * 16) & 0xFFFFu;
-                    if ((uint32_t)t < n && ((e ^ me) >> 12) == 0) {        // same bucket
-                        if (e < me) best = max(best, (int)(e & 0xFFFu));
-                        later |= e > me;
-                    }
-                }
+                const uint32_t me = (hh & 0xF000u) | myidx;
+                // An entry e of my bucket is earlier than me exactly when me - e - 1 < myidx, and the latest of them has the
+                // smallest such value; it is later exactly when e - me - 1 < 0xFFF - myidx. An entry of another bucket of the slot
+                // meets neither, and an unused entry is replaced by my own, which meets neither.
+                const uint32_t ea = e2.x & 0xFFFFu, eb = n > 1 ? e2.x >> 16 : me, ec = n > 2 ? e2.y & 0xFFFFu : me,
+                               ed = n > 3 ? e2.y >> 16 : me;
+                const uint32_t dmin = min(min(me - ea - 1u, me - eb - 1u), min(me - ec - 1u, me - ed - 1u));
+                const uint32_t umin = min(min(ea - me - 1u, eb - me - 1u), min(ec - me - 1u, ed - me - 1u));
+                int best = dmin < myidx ? (int)(myidx - 1u - dmin) : -1;
+                later = umin < 0xFFFu - myidx;
                 if (n > (uint32_t)F6_MB_CAP) {
                     const uint32_t s2 = slot & (F6_SEC_SLOTS - 1);
                     const uint32_t n2 = S.seccnt[buf][s2];     // <= F6_SEC_CAP here (else the tile overflowed)
@@ -393,28 +399,29 @@ cham_flag_pass6(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles
         nxt[j] = (pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + pos0 + 32 * j) : 0u;
         nxt2[j] = (TILE_Q + pos0 + 32 * j < run_quads) ? ld_stream_u32(rin + TILE_Q + pos0 + 32 * j) : 0u;
     }
+    // The 64-bit addressing and the bounds are set up once: a tile is whole exactly when lt < nfull, and the pointers advance by a tile.
+    const uint32_t nfull = run_quads / TILE_Q;
+    const uint32_t* __restrict__ np = rin + 2 * TILE_Q + pos0;    // my quads of the tile two ahead
+    uint32_t* __restrict__ sp = rsig + tid;                         // my word of the tile's flags
     #pragma unroll 1
-    for (uint32_t lt = 0; lt < ntile_run; ++lt) {
+    for (uint32_t lt = 0; lt < ntile_run; ++lt, np += TILE_Q, sp += TILE_Q / 32) {
         uint32_t q[F6_QPT];
         const uint32_t run_q0 = lt * TILE_Q;
-        const uint32_t left = run_q0 < run_quads ? run_quads - run_q0 : 0u;
         const uint32_t buf = lt & 1u;
 #pragma unroll
         for (int j = 0; j < F6_QPT; ++j) { q[j] = nxt[j]; nxt[j] = nxt2[j]; }
-        {
-            const uint32_t nleft = left > 2u * TILE_Q ? left - 2u * TILE_Q : 0u;
-            const uint32_t* __restrict__ np = rin + run_q0 + 2 * TILE_Q + pos0;
-            if (nleft >= (uint32_t)TILE_Q) {
+        if (lt + 2 < nfull) {
 #pragma unroll
-                for (int j = 0; j < F6_QPT; ++j) nxt2[j] = ld_stream_u32(np + 32 * j);
-            } else {
+            for (int j = 0; j < F6_QPT; ++j) nxt2[j] = ld_stream_u32(np + 32 * j);
+        } else {
+            const uint32_t nleft = run_q0 + 2u * TILE_Q < run_quads ? run_quads - run_q0 - 2u * TILE_Q : 0u;
 #pragma unroll
-                for (int j = 0; j < F6_QPT; ++j) nxt2[j] = (pos0 + 32 * j < nleft) ? ld_stream_u32(np + 32 * j) : 0u;
-            }
+            for (int j = 0; j < F6_QPT; ++j) nxt2[j] = (pos0 + 32 * j < nleft) ? ld_stream_u32(np + 32 * j) : 0u;
         }
-        if (left >= (uint32_t)TILE_Q && !rcm) {
+        if (lt < nfull && !rcm) {
             f6_tile<false>(S, q, (1u << F6_QPT) - 1u, buf, run_q0, unres_run);
         } else {
+            const uint32_t left = run_q0 < run_quads ? run_quads - run_q0 : 0u;
             uint32_t validmask = 0, cp = 0;
             if (rcm) {
 #pragma unroll
@@ -425,7 +432,7 @@ cham_flag_pass6(const uint32_t* __restrict__ in, uint64_t nquads, uint32_t tiles
                 if (pos0 + 32 * j < left && !((cp >> (j >> 1)) & 1u)) validmask |= 1u << j;
             f6_tile<true>(S, q, validmask, buf, run_q0, unres_run);
         }
-        if (tid < TILE_Q / 32) rsig[lt * (TILE_Q / 32) + tid] = S.sigw[buf][tid];
+        if (tid < TILE_Q / 32) *sp = S.sigw[buf][tid];
         if (tid == 0) S.overflow = 0;      // read by everybody before the tile's final barrier; next written after two more barriers
     }
     #pragma unroll 1

@@ -122,6 +122,8 @@ def flag_pass(q, seed=1, stats=None, overlap=False):
             stats["early"] = stats.get("early", 0) + int(early is not None)
             stats["stale"] = stats.get("stale", 0) + nstale
             stats.setdefault("tile_overflow", []).append(overflow)   # per tile, in stream order
+            # records (dropped ones included) of each warp's region: the trip count of the deposit and D loops is ceil(count / 32)
+            stats.setdefault("warp_records", []).append(np.bincount(rec // REGION, minlength=TILE // REGION))
         early = None
         if overflow:
             # replay: restore the pre-tile values of the dirty buckets, walk the dirty members in stream order

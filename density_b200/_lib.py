@@ -107,6 +107,23 @@ _SIGS = {
                                                                      ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_decode_sharded_cheetah_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
                                                                      ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_create": (ctypes.c_void_p, []),
+    "density_b200_lion_decode_shard_destroy": (None, [ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_int,
+                                                             ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_phase2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_walk": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_state_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_phase3": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_prot_transfer": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                    ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_prot_phase1": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                                  ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_lion_decode_shard_stats": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint64)]),
+    "density_b200_decode_sharded_lion": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_void_p,
+                                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_decode_sharded_lion_protected": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t,
+                                                                  ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_cheetah_decode_locate": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint64,
                                                           ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_cheetah_locate_piece": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]),

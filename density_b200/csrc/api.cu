@@ -1370,6 +1370,139 @@ int density_b200_cheetah_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, void
     return step_result(e, l, "cheetah_cmap_fold");
 }
 
+// ---- sharded Lion decode: one piece, its chunk map carried in and the prediction walk's state relayed from the piece before it ---------
+struct density_b200_lion_decode_shard {
+    DevBuf ws, tables;
+    DevBuf seed;                    // the incoming automaton state of the prot_* phases (DECODE_PROT_SEED_WORDS)
+    CheeShardArgs a{};
+    int num_sms = 0;
+    // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2, 3 the walk, 4 phase 3
+    int phase = 0;
+    bool transfer_done = false;     // prot_transfer done, prot_phase1 not yet
+    bool prot = false;              // the current piece went through prot_phase1: phase 3 writes the protected seam words
+};
+static_assert(LION_STATE_WORDS == DENSITY_B200_LION_STATE_WORDS, "the relayed state of the header and of cl_decode.cu");
+
+density_b200_lion_decode_shard* density_b200_lion_decode_shard_create(void) { return new_shard<density_b200_lion_decode_shard>(); }
+void density_b200_lion_decode_shard_destroy(density_b200_lion_decode_shard* s) {
+    if (!s) return;
+    s->ws.release(); s->tables.release(); s->seed.release();
+    delete s;
+}
+// the argument checks and the piece set up in s->a (phase 1 and prot_transfer); DENSITY_B200_OK or the error code, with nothing enqueued
+static int lion_shard_setup(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first,
+                            int is_last, const uint32_t* d_table, bool need_table, bool with_seed, cudaStream_t st) {
+    if (!s || (!d_in && n) || (!d_out && cap) || (need_table && !d_table)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_table)) {
+        set_error("d_in must be 2-byte, d_out and the tables 4-byte aligned"); return DENSITY_B200_EARG;
+    }
+    s->phase = 0; s->transfer_done = false; s->prot = false;
+    CheeShardArgs& a = s->a;
+    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
+    cudaError_t e = with_seed ? s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st) : cudaSuccess;
+    if (n) {
+        if (e == cudaSuccess) e = s->ws.ensure(lion_shard_workspace_bytes(n, cap, s->num_sms), st);
+        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms, true) + 256, st);
+    }
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    a.ws = s->ws.p; a.tables = s->tables.p;
+    return DENSITY_B200_OK;
+}
+int density_b200_lion_decode_shard_phase1(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                          int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    int rc = lion_shard_setup(s, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, false, false, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    uint64_t launches = 0;
+    cudaError_t e = cudaSuccess;
+    if (n) e = lion_shard_phase1(s->a, d_cmap_out, st, &launches);
+    else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    rc = step_result(e, launches, "lion decode shard phase1");
+    if (rc == DENSITY_B200_OK) s->phase = 1;
+    return rc;
+}
+int density_b200_lion_decode_shard_phase2(density_b200_lion_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
+    g_last_error.clear();
+    if (!s || s->phase != 1) { set_error("lion_decode_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
+    if (!al4(d_cmap_carry)) { set_error("d_cmap_carry must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = s->a.n ? lion_shard_phase2(s->a, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;
+    const int rc = step_result(e, launches, "lion decode shard phase2");
+    if (rc == DENSITY_B200_OK) s->phase = 2;
+    return rc;
+}
+int density_b200_lion_decode_shard_walk(density_b200_lion_decode_shard* s, uint32_t* d_state, void* stream) {
+    g_last_error.clear();
+    if (!s || s->phase != 2) { set_error("lion_decode_shard_walk: null pointer / phase 2 not done"); return DENSITY_B200_EARG; }
+    if (!d_state || !al4(d_state)) { set_error("d_state must be a 4-byte aligned pointer"); return DENSITY_B200_EARG; }
+    uint64_t launches = 0;
+    const cudaError_t e = s->a.n ? lion_shard_walk(s->a, d_state, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;  // empty: unchanged
+    const int rc = step_result(e, launches, "lion decode shard walk");
+    if (rc == DENSITY_B200_OK) s->phase = 3;
+    return rc;
+}
+int density_b200_lion_state_init(uint32_t* d_state, void* stream) {
+    g_last_error.clear();
+    if (!d_state || !al4(d_state)) { set_error("d_state must be a 4-byte aligned pointer"); return DENSITY_B200_EARG; }
+    return step_result(lion_state_init(d_state, reinterpret_cast<cudaStream_t>(stream)), 0, "lion_state_init");
+}
+int density_b200_lion_decode_shard_phase3(density_b200_lion_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s || s->phase != 3) { set_error("lion_decode_shard_phase3: null pointer / the walk not done"); return DENSITY_B200_EARG; }
+    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) { set_error("d_out_size must be 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    const uint32_t* seed = s->prot ? reinterpret_cast<const uint32_t*>(s->seed.p) : nullptr;
+    const cudaError_t e = (s->a.n || seed) ? lion_shard_phase3(s->a, d_out_size, d_seam8, st, &launches, seed) : empty_piece_outputs(d_out_size, d_seam8, st);
+    const int rc = step_result(e, launches, "lion decode shard phase3");
+    if (rc == DENSITY_B200_OK) s->phase = 4;
+    return rc;
+}
+int density_b200_lion_decode_shard_prot_transfer(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                                 int is_first, int is_last, uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    int rc = lion_shard_setup(s, d_in, n, d_out, cap, is_first, is_last, d_transfer_out, true, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    uint64_t launches = 0;
+    const cudaError_t e = lion_shard_prot_transfer(s->a, d_transfer_out, st, &launches);
+    rc = step_result(e, launches, "lion decode shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->transfer_done = true;
+    return rc;
+}
+int density_b200_lion_decode_shard_prot_phase1(density_b200_lion_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
+                                               uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s || !s->transfer_done || s->phase != 0) { set_error("lion_decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
+    if (!al4(d_all_transfers) || !al4(d_cmap_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    s->transfer_done = false;   // one phase 1 per transfer
+    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, 0, seed, st, &launches);
+    if (e == cudaSuccess) {
+        if (s->a.n) e = lion_shard_phase1(s->a, d_cmap_out, st, &launches, seed, true);
+        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
+    }
+    const int rc = step_result(e, launches, "lion decode shard prot phase1");
+    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
+    return rc;
+}
+int density_b200_lion_decode_shard_stats(density_b200_lion_decode_shard* s, uint64_t* out4) {
+    g_last_error.clear();
+    if (!s || !out4 || s->phase != 4) { set_error("lion_decode_shard_stats: null pointer / phase 3 not done"); return DENSITY_B200_EARG; }
+    for (int k = 0; k < 4; ++k) out4[k] = 0;
+    if (!s->a.n) return DENSITY_B200_OK;    // an empty piece walks nothing
+    cudaError_t e = cudaDeviceSynchronize();
+    // the counts follow the ClStatus prefix of the walk's status (8 u32)
+    if (e == cudaSuccess) e = cudaMemcpy(out4, static_cast<const uint8_t*>(lion_shard_status_ptr(s->a)) + 32, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error("lion_decode_shard_stats", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon encode across the GPUs of one box (SURVEY §8e): one process per GPU, NCCL over NVLink ---------------------
 // NCCL is resolved at run time from the library that is already in the process (torch loads its bundled libnccl.so.2), else the
 // system one: no link-time dependency, one NCCL per process.
@@ -1456,6 +1589,8 @@ struct density_b200_sharded {
     density_b200_decode_shard* dec = nullptr;            // density_b200_decode_sharded[_stream]
     density_b200_decode_shard* pdec = nullptr;           // density_b200_decode_sharded_protected
     density_b200_cheetah_decode_shard* cdec = nullptr;   // density_b200_decode_sharded_cheetah[_stream]
+    density_b200_lion_decode_shard* ldec = nullptr;      // density_b200_decode_sharded_lion
+    density_b200_lion_decode_shard* lpdec = nullptr;     // density_b200_decode_sharded_lion_protected
     uint64_t* h_offsets = nullptr;  // pinned, world + 1
     uint64_t* h_maps = nullptr;     // pinned, world range maps (the stream decodes)
     cudaEvent_t ev[6] = {};         // stage timing of the last call: start, flag pass, exchange, phase 2 up to emit, emit, gather
@@ -1496,6 +1631,7 @@ density_b200_sharded* density_b200_sharded_create(const uint8_t* nccl_unique_id_
     h->cl[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->cl[1] = density_b200_cl_shard_create(ALG_LION);
     h->clp[0] = density_b200_cl_shard_create(ALG_CHEETAH); h->clp[1] = density_b200_cl_shard_create(ALG_LION);
     h->dec = density_b200_decode_shard_create(); h->pdec = density_b200_decode_shard_create(); h->cdec = density_b200_cheetah_decode_shard_create();
+    h->ldec = density_b200_lion_decode_shard_create(); h->lpdec = density_b200_lion_decode_shard_create();
     for (auto& e : h->ev) cudaEventCreate(&e);
     return h;
 }
@@ -1511,6 +1647,8 @@ void density_b200_sharded_destroy(density_b200_sharded* h) {
     density_b200_decode_shard_destroy(h->dec);
     density_b200_decode_shard_destroy(h->pdec);
     density_b200_cheetah_decode_shard_destroy(h->cdec);
+    density_b200_lion_decode_shard_destroy(h->ldec);
+    density_b200_lion_decode_shard_destroy(h->lpdec);
     if (h->h_offsets) cudaFreeHost(h->h_offsets);
     if (h->h_maps) cudaFreeHost(h->h_maps);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
@@ -1981,6 +2119,75 @@ int density_b200_decode_sharded_cheetah_protected(density_b200_sharded* h, const
         return rc;
     return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
                                         true);
+}
+
+// Sharded Lion decode of this rank's piece d_in[0 .. n) over the handle's communicator: [prot: prot_transfer -> ncclAllGather(transfers) ->
+// prot_phase1, else phase 1] -> chunk-map transfers -> fold -> phase 2 -> the relay of the walk's state (receive from rank - 1, walk, send
+// to rank + 1; the receive and the send are separate groups, since one group would send the state from before the walk) -> phase 3 -> seam
+// words -> verdict. Every rank issues the same collectives whatever its piece holds: an empty piece forwards the state unchanged, a
+// refused one keeps exchanging until the verdict. Rank 0 holds the stream start, the last rank its end.
+static int decode_sharded_lion_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                     uint32_t* d_flags, uint64_t* d_total_size, void* stream_v, bool prot) {
+    if (reinterpret_cast<uintptr_t>(d_out_size) & 7) { set_error("d_out_size must be 8-byte aligned"); return DENSITY_B200_EARG; }
+    const size_t W = (size_t)h->world, R = (size_t)h->rank;
+    const size_t wc = density_b200_cheetah_cmap_words();
+    Exchange x;
+    int rc = x.open(h, stream_v, ((W + 1) * wc + DENSITY_B200_LION_STATE_WORDS + (prot ? W * DECODE_PROT_TRANSFER_WORDS : 0) + 64) * sizeof(uint32_t));
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaStream_t st = x.st;
+    density_b200_lion_decode_shard* s = prot ? h->lpdec : h->ldec;
+    const bool first = R == 0, last = R == W - 1;
+    uint32_t* tab_c = reinterpret_cast<uint32_t*>(x.extra);              // [world][wc]
+    uint32_t* carry_c = tab_c + W * wc;
+    uint32_t* state = carry_c + wc;                                       // the walk's state, DENSITY_B200_LION_STATE_WORDS
+    uint32_t* transfers = state + DENSITY_B200_LION_STATE_WORDS;          // [world][DECODE_PROT_TRANSFER_WORDS] (prot)
+    uint32_t* cmap_out = last ? nullptr : tab_c + R * wc;                 // the last piece's transfer is never read
+    if (prot) {
+        rc = density_b200_lion_decode_shard_prot_transfer(s, d_in, n, d_out, cap, first, last, transfers + R * DECODE_PROT_TRANSFER_WORDS, st);
+        if (rc != DENSITY_B200_OK) return rc;
+        if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        rc = density_b200_lion_decode_shard_prot_phase1(s, transfers, (int)W, (int)R, cmap_out, st);
+    } else {
+        rc = density_b200_lion_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, cmap_out, st);
+    }
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!x.gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const cudaError_t e = first ? lion_state_init(state, st) : chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
+    if ((rc = step_result(e, launches, "sharded lion decode: chunk-map fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_lion_decode_shard_phase2(s, first ? nullptr : carry_c, st)) != DENSITY_B200_OK) return rc;
+    if (!first) {
+        if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
+        const bool ok = nccl_check(x.a->Recv(state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R - 1, h->comm, st), "ncclRecv(walk state)");
+        if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
+    }
+    if ((rc = density_b200_lion_decode_shard_walk(s, state, st)) != DENSITY_B200_OK) return rc;
+    if (!last) {
+        if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
+        const bool ok = nccl_check(x.a->Send(state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R + 1, h->comm, st), "ncclSend(walk state)");
+        if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
+    }
+    if ((rc = density_b200_lion_decode_shard_phase3(s, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
+    return x.verdict(d_flags, d_total_size, nullptr);
+}
+
+// The pieces of a sharded Lion encode: rank 0 holds the stream start, the last rank its end.
+int density_b200_decode_sharded_lion(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
+                                     uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    const int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    if (rc != DENSITY_B200_OK) return rc;
+    return decode_sharded_lion_piece(h, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v, false);
+}
+
+// The inverse of density_b200_encode_sharded_cl_protected (Lion) for any stream: the pieces' protection transfers are exchanged first,
+// then everything runs as density_b200_decode_sharded_lion.
+int density_b200_decode_sharded_lion_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                               uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    const int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    if (rc != DENSITY_B200_OK) return rc;
+    return decode_sharded_lion_piece(h, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v, true);
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {

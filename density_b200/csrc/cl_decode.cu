@@ -389,11 +389,14 @@ __global__ void cd_finish(const DecStatus* __restrict__ st, ClStatus* __restrict
 // ring ahead of the walker, and that ring with the table in an 8-CTA cluster's distributed shared memory, measured slower on text and
 // synth_mixed (DESIGN.md section 8).
 // status: a ClStatus prefix (final_ctx for the tail, done for cd_finish) followed by the walk's counts (density_b200_lion_decode_stats).
+// ctx_in (a piece of a sharded stream after the first, nullptr otherwise): the context of the piece's first quad, last_hash behind the
+// pieces before it; ctx_out (a piece of a sharded stream, nullptr otherwise) receives the context behind the piece. They may alias.
 struct LionStatus { ClStatus c; unsigned long long quads, pred, dep, rows; };
 constexpr uint32_t LW_PREFETCH = 16;                       // rows ahead whose stream data is pulled into L2 while the walk works
 
 __global__ void __launch_bounds__(32) ld_walk(const DecStatus* __restrict__ st, const uint4* __restrict__ flags, const uint16_t* __restrict__ K,
-                                              uint32_t* __restrict__ out, uint32_t* __restrict__ T, LionStatus* __restrict__ ls) {
+                                              uint32_t* __restrict__ out, uint32_t* __restrict__ T, LionStatus* __restrict__ ls,
+                                              const uint32_t* ctx_in, uint32_t* ctx_out) {
 #if defined(__CUDA_ARCH__)                                   // lwalk::Warp / LV are the device lanes only in the device pass
     if (st->error) return;
     using namespace lwalk;
@@ -402,7 +405,7 @@ __global__ void __launch_bounds__(32) ld_walk(const DecStatus* __restrict__ st, 
     const uint64_t ns = cd_steps<bounds::LionT>(st);
     const FlatTable tab{T};
     WalkCounts cnt{0, 0, 0, 0};
-    uint32_t carry = 0;                                    // lion.rs:67
+    uint32_t carry = ctx_in ? *ctx_in : 0u;                // lion.rs:67
     uint4 fl_n = make_uint4(0, 0, 0, 0); uint32_t k_n = 0, v_n = 0;
     if (ns) { fl_n = flags[0]; k_n = K[lane]; v_n = out[lane]; }
     for (uint64_t s = 0; s < ns; ++s) {
@@ -421,6 +424,7 @@ __global__ void __launch_bounds__(32) ld_walk(const DecStatus* __restrict__ st, 
     if (lane == 0) {
         ls->c.final_ctx = carry; ls->c.done = 1; ls->c.rounds = 1;
         ls->quads = cnt.quads; ls->pred = cnt.pred; ls->dep = cnt.dep; ls->rows = cnt.rows;
+        if (ctx_out) *ctx_out = carry;
     }
 #endif
 }
@@ -434,18 +438,23 @@ constexpr uint32_t CM_IDENTITY = 1u | (2u << 3);          // chunk-map transfer 
 struct PieceStatus { unsigned int refuse, first_inc, last_inc, tail_blocks, pad[4]; };
 
 // The end of the piece, right after the boundary walk. A non-final piece is followed by more stream bytes, so the reference decodes all of
-// its blocks in the main loop (codec.rs:88-100); the blocks the boundary walk left to the tail (those starting in the last 136 bytes) are
-// appended to the block list. Their control flow does not depend on the tables. The final piece keeps its in-order tail; its control flow
-// is walked here for the seam words. The automaton starts from the state behind the main loop (bounds::main_end_state: the piece's seed
-// carried over its main blocks). Refused (pst->refuse): a non-final piece whose blocks do not end exactly at its last byte or that reads a
-// malformed block; and, unless `prot`, a piece > 0 that is not quiet (copy mode, two consecutive incompressible blocks) or a non-final
-// piece that meets copy mode at its end, ends with a copy penalty pending or inside a copy run. prot: a piece of the protected path
-// (density_b200_cheetah_decode_shard_prot_*), whose seed carries the automaton across the cuts, so the blocks at its end may be copy-mode
-// blocks (appended with BLK_COPY) and it may end in any automaton state.
+// its blocks in the main loop (codec.rs:88-100); the blocks the boundary walk left to the tail (those starting in the last G::MAXBLK bytes)
+// are appended to the block list. Their control flow does not depend on the tables. The final piece keeps its in-order tail; its control
+// flow is walked here for the seam words. The automaton starts from the state behind the main loop (bounds::main_end_state: the piece's
+// seed carried over its main blocks). Refused (pst->refuse): a non-final piece whose blocks do not end exactly at its last byte or that
+// reads a malformed block; and, unless `prot`, a piece > 0 that is not quiet (copy mode, two consecutive incompressible blocks) or a
+// non-final piece that meets copy mode at its end, ends with a copy penalty pending or inside a copy run. prot: a piece of the protected
+// path (density_b200_cheetah_decode_shard_prot_*, density_b200_lion_decode_shard_prot_*), whose seed carries the automaton across the
+// cuts, so the blocks at its end may be copy-mode blocks (appended with BLK_COPY) and it may end in any automaton state. G: the block
+// geometry (bounds::CheeT: 128-byte blocks, 8-byte signatures of 2-bit flags; bounds::LionT: 64-byte blocks, 6-byte signatures of 3-bit
+// flags).
+template <class G>
 __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, int first, int last, int prot, DecStatus* __restrict__ st,
                              uint64_t* __restrict__ blk_off, uint64_t maxblocks, PieceStatus* __restrict__ pst) {
     if (threadIdx.x || blockIdx.x) return;
-    auto sig_at = [&](uint64_t o) { uint64_t s = 0; for (int i = 0; i < 8; ++i) s |= (uint64_t)in[o + i] << (8 * i); return s; };
+    constexpr bool LION = G::BS == 64;
+    constexpr uint32_t FB = LION ? 3 : 2;                          // flag bits per quad
+    auto sig_at = [&](uint64_t o) { uint64_t s = 0; for (uint32_t i = 0; i < G::SIG; ++i) s |= (uint64_t)in[o + i] << (8 * i); return s; };
     if (st->error) { pst->refuse = 1; pst->first_inc = 0; pst->last_inc = 0; pst->tail_blocks = 0; return; }
     uint32_t refuse = (!prot && !first && st->seq) ? 1u : 0u;    // dec_seq_walk ran: two consecutive incompressible blocks in the main loop
     Protection ps = bounds::main_end_state(st);
@@ -455,18 +464,18 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
         bool bad = false, ends_copy = b > 0 && (blk_off[b - 1] & BLK_COPY);
         while (idx < n) {
             if (ps.revert_to_copy()) {                             // codec.rs:89-92
-                if (!prot || n - idx < 128) { bad = true; break; } // quiet path: copy mode at the end of a non-final piece
+                if (!prot || n - idx < G::BS) { bad = true; break; }   // quiet path: copy mode at the end of a non-final piece
                 if (b < maxblocks) blk_off[b] = idx | BLK_COPY; else st->error = 2;
-                ++b; ++tail_blocks; idx += 128; ends_copy = true;
+                ++b; ++tail_blocks; idx += G::BS; ends_copy = true;
                 ps.decay();
                 continue;
             }
-            if (n - idx < 8) { bad = true; break; }
-            const uint32_t consumed = cld::cheetah_block_bytes(sig_at(idx));
+            if (n - idx < G::SIG) { bad = true; break; }
+            const uint32_t consumed = G::consumed(sig_at(idx));
             if (consumed > n - idx) { bad = true; break; }         // the block runs past the piece
             if (b < maxblocks) blk_off[b] = idx; else st->error = 2;
             ++b; ++tail_blocks; idx += consumed; ends_copy = false;
-            ps.update(consumed >= 128);                            // codec.rs:94-98
+            ps.update(consumed >= G::BS);                          // codec.rs:94-98
         }
         if (bad || (!prot && (ends_copy || ps.copy_penalty))) refuse = 1;
         if (!bad) {
@@ -474,7 +483,7 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
             if (prot) st->seq = 1;                                 // main_end_state reads the state below from now on
             if (st->seq) { st->ps_penalty = ps.copy_penalty; st->ps_start = ps.copy_penalty_start; st->ps_prev = ps.previous_incompressible; }
         }
-        if (b * 128 > cap) st->error = 2;
+        if (b * G::BS > cap) st->error = 2;
     } else {
         // the tail loop's control flow (codec.rs:102-123, scalar_codec.cu decode_loops): copy mode or a new incompressible pair there
         // is refused in a piece > 0; malformed input is left to the tail kernel, which reports it
@@ -483,23 +492,24 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
             ++tail_blocks;
             if (ps.revert_to_copy()) {
                 copied = 1;
-                if (n - idx > 128) { idx += 128; ps.decay(); continue; }
+                if (n - idx > G::BS) { idx += G::BS; ps.decay(); continue; }
                 break;
             }
             const uint64_t mark = idx;
-            if (n - idx < 8) break;
+            if (n - idx < G::SIG) break;
             uint64_t sig = sig_at(idx);
-            idx += 8;
+            idx += G::SIG;
             bool end = false;
-            for (int u = 0; u < 32 && !end; ++u) {
-                const uint32_t fl = (uint32_t)(sig & 3u); sig >>= 2;
+            for (uint32_t u = 0; u < G::BS / 4 && !end; ++u) {
+                const uint32_t fl = (uint32_t)(sig & ((1u << FB) - 1u)); sig >>= FB;
+                const uint32_t kind = LION ? lion_kind(fl) : cheetah_kind(fl);
                 const uint64_t rem = n - idx;
-                if (fl == 0 && rem < 4) end = true;                 // decode_partial_unit: the stream ends inside this quad
-                else if (fl == 0) idx += 4;
-                else if (fl != 3) { if (rem < 2) end = true; else idx += 2; }
+                if (kind == K_PLAIN && rem < 4) end = true;        // decode_partial_unit: the stream ends inside this quad
+                else if (kind == K_PLAIN) idx += 4;
+                else if (kind != K_PRED) { if (rem < 2) end = true; else idx += 2; }
             }
             if (end) break;
-            const uint32_t inc = idx - mark >= 128 ? 1u : 0u;
+            const uint32_t inc = idx - mark >= G::BS ? 1u : 0u;
             if (tail_blocks == 1) tail_first = inc;
             pair |= inc & ps.previous_incompressible;
             ps.update(inc);
@@ -507,7 +517,7 @@ __global__ void cd_piece_end(const uint8_t* __restrict__ in, uint64_t n, uint64_
         if (!prot && !first && (copied || pair)) refuse = 1;
     }
     const uint64_t b0 = blk_off[0];
-    pst->first_inc = st->main_blocks ? ((!(b0 & BLK_COPY) && cld::cheetah_block_bytes(sig_at(b0)) >= 128) ? 1u : 0u) : tail_first;
+    pst->first_inc = st->main_blocks ? ((!(b0 & BLK_COPY) && G::consumed(sig_at(b0)) >= G::BS) ? 1u : 0u) : tail_first;
     pst->last_inc = ps.previous_incompressible;
     pst->refuse = refuse;
     pst->tail_blocks = tail_blocks;
@@ -635,7 +645,8 @@ __global__ void cd_shard_round_end(ClStatus* __restrict__ cs, uint32_t nruns, ui
 // at the end, refused, has blocks, decoded size lo, hi, 0, 0}. seed (the protected path, nullptr otherwise): the piece's incoming state
 // (bounds::dec_prot_enter_k); words 0 and 1 are then 0, since incompressible blocks may meet at a cut when the transfers carry the
 // automaton across it, and the piece is also refused when the transfers composed to no state. pst == nullptr: an empty piece of the
-// protected path (no blocks, size 0), refused only by its seed.
+// protected path (no blocks, size 0), refused only by its seed. BS: the block size, of which a non-final piece decodes a whole number.
+template <uint32_t BS>
 __global__ void cd_seam_words(const PieceStatus* __restrict__ pst, const uint32_t* __restrict__ fallback, const Status* __restrict__ tail_status,
                               int is_last, const uint32_t* __restrict__ seed, uint64_t* __restrict__ d_out_size, uint32_t* __restrict__ words) {
     if (threadIdx.x || blockIdx.x) return;
@@ -644,7 +655,7 @@ __global__ void cd_seam_words(const PieceStatus* __restrict__ pst, const uint32_
     if (pst) {
         sz = *d_out_size;
         if (pst->refuse || *fallback || tail_status->error) bad = 1;
-        if (!is_last && (sz % 128)) bad = 1;
+        if (!is_last && (sz % BS)) bad = 1;
     } else *d_out_size = 0;
     words[0] = pst && !seed ? pst->first_inc : 0u; words[1] = pst && !seed ? pst->last_inc : 0u; words[2] = bad; words[3] = pst ? 1u : 0u;
     words[4] = (uint32_t)sz; words[5] = (uint32_t)(sz >> 32); words[6] = 0; words[7] = 0;
@@ -823,7 +834,7 @@ cudaError_t lion_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_
     uint32_t* out32 = reinterpret_cast<uint32_t*>(d_out);
     cd_launch_unpack_walk<bounds::LionT>(p, d_in, out32, stream, launches);
     cd_launch_cmap_resolve<bounds::LionT>(p, out32, nullptr, stream, launches);
-    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, out32, p.pred_final, ls);
+    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, out32, p.pred_final, ls, nullptr, nullptr);
     ++*launches;
     cd_launch_finish(p, d_fallback, d_out_size, stream, launches);
     return cudaGetLastError();
@@ -855,7 +866,7 @@ cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cuda
     if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
     if (e != cudaSuccess) return e;
-    cd_piece_end<<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
+    cd_piece_end<T><<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
     ++*launches;
     cd_launch_unpack_walk(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
     if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
@@ -895,7 +906,7 @@ cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const 
 cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
                               const uint32_t* d_seed) {
     if (!a.n) {
-        cd_seam_words<<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+        cd_seam_words<128><<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
         ++*launches;
         return cudaGetLastError();
     }
@@ -903,43 +914,48 @@ cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint
     cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
     cudaError_t e = scalar_decode_tail(ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
     if (e != cudaSuccess) return e;
-    cd_seam_words<<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+    cd_seam_words<128><<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
     ++*launches;
     return cudaGetLastError();
 }
 
 // The protected path's first step on a piece (DESIGN.md section 5): the candidate rows of the boundary walk (they stay in the workspace
-// for chee_shard_phase1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing.
+// for the phase 1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing. G: the geometry
+// of the piece's algorithm (CheeT or LionT).
+template <class G, bool LOCATE>
 static cudaError_t prot_transfer_attr() {
     static bool attr_done = false;
     if (!attr_done) {
-        cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)bounds::prot_transfer_smem<T>());
-        if (e0 == cudaSuccess)
-            e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bounds::prot_transfer_smem<T>());
+        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<G, LOCATE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                    (int)bounds::prot_transfer_smem<G>());
         if (e0 != cudaSuccess) return e0;
         attr_done = true;
     }
     return cudaSuccess;
 }
-cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr();
+static_assert(bounds::prot_transfer_smem<bounds::LionT>() <= 227u * 1024u, "the Lion head walk's shared memory must fit in one SM");
+template <class G>
+static cudaError_t shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    const cudaError_t e0 = prot_transfer_attr<G, false>();
     if (e0 != cudaSuccess) return e0;
     uint32_t* res = nullptr;
     uint4* gres = nullptr;
     if (a.n) {
-        const CheeDecPtrs p = chee_shard_ptrs(a);
+        const CheeDecPtrs p(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr, G::BS == 64);
         res = reinterpret_cast<uint32_t*>(a.ws + p.B.res);
         gres = reinterpret_cast<uint4*>(a.ws + p.B.gres);
-        const uint32_t nchunks = (uint32_t)((a.n + T::CH - 1) / T::CH);
-        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(a.d_in, a.n, nchunks, res);
-        bounds::dec_group_compose<T><<<(nchunks + bounds::GROUP - 1) / bounds::GROUP, 160, 0, stream>>>(res, nchunks, gres);
+        const uint32_t nchunks = (uint32_t)((a.n + G::CH - 1) / G::CH);
+        bounds::dec_chunk_walk<G><<<nchunks, 160, 0, stream>>>(a.d_in, a.n, nchunks, res);
+        bounds::dec_group_compose<G><<<(nchunks + bounds::GROUP - 1) / bounds::GROUP, 160, 0, stream>>>(res, nchunks, gres);
         *launches += 2;
     }
-    bounds::dec_prot_transfer<T, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(a.d_in, a.n, a.n, a.last ? 1 : 0, res, gres,
-                                                                                                    d_transfer);
+    bounds::dec_prot_transfer<G, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<G>(), stream>>>(a.d_in, a.n, a.n, a.last ? 1 : 0, res,
+                                                                                                    gres, d_transfer);
     ++*launches;
     return cudaGetLastError();
+}
+cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    return shard_prot_transfer<T>(a, d_transfer, stream, launches);
 }
 // The incoming state of piece `rank` composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
 cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
@@ -965,6 +981,88 @@ cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_
     cd_cmap_rank_fold_k<<<PL / 128, 128, 0, stream>>>(d_tables, rank, d_carry); ++*launches; return cudaGetLastError();
 }
 uint32_t chee_shard_max_rounds() { return MAX_ROUNDS; }
+
+// ---- sharded Lion decode: one piece, in phases around the chunk-map exchange and the relay of the walk's state (DESIGN.md section 5) ----
+// Stages 0-2 are the Cheetah piece's on the Lion geometry; the walk continues the state the pieces before it left (one piece after the
+// other), on the tail's table in the workspace.
+static CheeDecPtrs lion_shard_ptrs(const CheeShardArgs& a) { return CheeDecPtrs(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr, true); }
+
+size_t lion_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
+    CheeDecLayout L;
+    const size_t off = (cd_layout(n, cap, cd_pick_runs(n, num_sms), &L, true) + 255) & ~(size_t)255;
+    return off + 256 + scalar_workspace_bytes(ALG_LION);
+}
+
+// Phase 1: boundaries, the end of the piece, unpack, the symbolic chunk-map walk and the chunk-map transfer (d_cmap_out, may be null), as
+// chee_shard_phase1 on the Lion geometry.
+cudaError_t lion_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
+                              bool rows_ready) {
+    const CheeDecPtrs p = lion_shard_ptrs(a);
+    cudaError_t e = bounds::bounds_launch<bounds::LionT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, rows_ready);
+    if (e == cudaSuccess) e = cd_clear_tables(p, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p.cs, 0, sizeof(LionStatus), stream);
+    if (e != cudaSuccess) return e;
+    cd_piece_end<bounds::LionT><<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off,
+                                                      p.B.maxblocks, p.pst);
+    ++*launches;
+    cd_launch_unpack_walk<bounds::LionT>(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
+    if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
+    return cudaGetLastError();
+}
+
+// Phase 2: the chunk map carried in (nullptr = the stream start) and the reads of carried-in slots.
+cudaError_t lion_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
+    cd_launch_cmap_resolve<bounds::LionT>(lion_shard_ptrs(a), reinterpret_cast<uint32_t*>(a.d_out), d_cmap_carry, stream, launches);
+    return cudaGetLastError();
+}
+
+// The walk from the relayed state d_state (LION_STATE_WORDS: the 65536 lists, then last_hash): the lists into the tail's table (the first
+// piece starts from the zero table and context 0, lion.rs:67,70), ld_walk, then the table and the context behind the piece back to d_state.
+cudaError_t lion_shard_walk(const CheeShardArgs& a, uint32_t* d_state, cudaStream_t stream, uint64_t* launches) {
+    const CheeDecPtrs p = lion_shard_ptrs(a);
+    const size_t tb = (size_t)5 * PL * sizeof(uint32_t);
+    uint32_t* ctx = d_state + 5 * PL;
+    cudaError_t e = a.first ? cudaMemsetAsync(p.pred_final, 0, tb, stream) : cudaMemcpyAsync(p.pred_final, d_state, tb, cudaMemcpyDeviceToDevice, stream);
+    if (e != cudaSuccess) return e;
+    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, reinterpret_cast<uint32_t*>(a.d_out), p.pred_final, reinterpret_cast<LionStatus*>(p.cs),
+                                  a.first ? nullptr : ctx, ctx);
+    ++*launches;
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_state, p.pred_final, tb, cudaMemcpyDeviceToDevice, stream);
+    return e;
+}
+
+// the stream-start state of the relay: zero lists, context 0
+cudaError_t lion_state_init(uint32_t* d_state, cudaStream_t stream) {
+    return cudaMemsetAsync(d_state, 0, (size_t)LION_STATE_WORDS * sizeof(uint32_t), stream);
+}
+
+// Phase 3: the verdict of the walk, the final piece's tail from the walked table (the tail of a non-final piece is empty), the size and
+// the seam words (d_seed: the protected path's). An empty piece of the protected path has its seam words only.
+cudaError_t lion_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                              const uint32_t* d_seed) {
+    if (!a.n) {
+        cd_seam_words<bounds::LionT::BS><<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+        ++*launches;
+        return cudaGetLastError();
+    }
+    const CheeDecPtrs p = lion_shard_ptrs(a);
+    cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
+    cudaError_t e = scalar_decode_tail(ALG_LION, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
+    if (e != cudaSuccess) return e;
+    cd_seam_words<bounds::LionT::BS><<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed,
+                                                         d_out_size, d_seam8);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t lion_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+    return shard_prot_transfer<bounds::LionT>(a, d_transfer, stream, launches);
+}
+
+// the walk's status of the piece (LionStatus: a ClStatus prefix, then the 4 u64 counts)
+const void* lion_shard_status_ptr(const CheeShardArgs& a) { return lion_shard_ptrs(a).cs; }
 
 // ---- the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64) ---------------------
 // Any range: the candidate walks over its chunks (the halo visible to its last chunk's walks), their composition per group and over the
@@ -1012,7 +1110,7 @@ size_t chee_prot_locate_workspace_bytes(size_t nbytes) { bounds::BoundsLayout B;
 
 cudaError_t chee_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
                                     uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr();
+    const cudaError_t e0 = prot_transfer_attr<T, true>();
     if (e0 != cudaSuccess) return e0;
     return bounds::prot_locate_launch<T>(d_in, n_range, n_halo, ws, d_map, stream, launches);
 }

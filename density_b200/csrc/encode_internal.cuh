@@ -221,6 +221,20 @@ cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t*
 cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
+// sharded Lion decode: one piece, the arguments of the Cheetah piece (ws: lion_shard_workspace_bytes, tables: chee_decode_tables_bytes(..,
+// true)). Phase 1 (or prot transfer, then phase 1 with the seed of chee_shard_prot_enter), phase 2, the walk, phase 3. The walk's state
+// travels from piece to piece in LION_STATE_WORDS u32: the 65536 five-slot lists (the tail's layout), then last_hash, then padding.
+constexpr uint32_t LION_STATE_WORDS = 5 * 65536 + 8;
+size_t lion_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
+cudaError_t lion_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr,
+                              bool rows_ready = false);
+cudaError_t lion_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
+cudaError_t lion_shard_walk(const CheeShardArgs& a, uint32_t* d_state, cudaStream_t stream, uint64_t* launches);
+cudaError_t lion_state_init(uint32_t* d_state, cudaStream_t stream);
+cudaError_t lion_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                              const uint32_t* d_seed = nullptr);
+cudaError_t lion_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
+const void* lion_shard_status_ptr(const CheeShardArgs& a);
 // the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`,
 // at least chee_locate_workspace_bytes of the same arguments
 size_t chee_locate_workspace_bytes(size_t n_range, size_t n_halo, uint64_t range_offset);

@@ -34,6 +34,12 @@ exchanged once, then every prediction round exchanges each piece's prediction tr
 Pieces with copy-mode blocks (ShardedDecoder.decode_protected(..., alg="cheetah"), or density_b200_cheetah_decode_shard_prot_transfer and
 _prot_phase1 in place of phase 1) first exchange their protection transfers, as Chameleon's do.
 
+A sharded Lion stream decodes in pieces too (ShardedLionDecoder, or the piece phases density_b200_lion_decode_shard_* with
+fold_cheetah_cmap for the one exchange of chunk-map transfers). Lion has no prediction rounds: each piece's walk starts from the
+prediction lists and context the piece before it left, so the walk's state (DENSITY_B200_LION_STATE_WORDS u32, 1.25 MiB) is relayed
+from rank to rank and the pieces walk one after the other. Pieces with copy-mode blocks (ShardedLionDecoder.decode_protected) first
+exchange their protection transfers, as Cheetah's do.
+
 A stream whose cuts are not known (one chameleon_encode call, the reference library, a file) is cut at byte ranges instead
 (`stream_ranges`): rank r holds its range and a halo of the next 264 bytes, computes the range map of every possible entry offset
 (density_b200_decode_locate), and after an all_gather of the maps `locate_piece` gives every rank the exact offset where its
@@ -637,10 +643,10 @@ class ShardedDecoder(_ShardedHandle):
         """Enqueue on torch's current stream; nothing blocks. d_in: this rank's piece (2-byte aligned); d_out: capacity d_out.numel()
         (4-byte aligned); d_size int64[1]: the decoded size; d_flags int32[1]: != 0 -> the pieces are void and the caller decodes the
         gathered stream on one device; self.d_total int64[1]: the original length. alg "cheetah" (or its id): the pieces of a sharded
-        Cheetah stream (density_b200_decode_sharded_cheetah); Lion has no parallel decoder to shard."""
+        Cheetah stream (density_b200_decode_sharded_cheetah). Lion pieces decode through ShardedLionDecoder."""
         alg = _alg_id(alg)
         if alg not in (0, 1):
-            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion pieces decode through ShardedLionDecoder)")
         fn = self._lib.density_b200_decode_sharded if alg == 0 else self._lib.density_b200_decode_sharded_cheetah
         _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
                   self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}")
@@ -652,7 +658,7 @@ class ShardedDecoder(_ShardedHandle):
         ShardedEncoder.encode_protected(..., alg="cheetah"))."""
         alg = _alg_id(alg)
         if alg not in (0, 1):
-            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+            raise ValueError("sharded decode: alg must be 'chameleon' or 'cheetah' (Lion pieces decode through ShardedLionDecoder)")
         fn = self._lib.density_b200_decode_sharded_protected if alg == 0 else self._lib.density_b200_decode_sharded_cheetah_protected
         _check(fn(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), d_flags.data_ptr(),
                   self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}_protected")
@@ -664,7 +670,7 @@ class ShardedDecoder(_ShardedHandle):
         (density_b200_decode_sharded_cheetah_stream); range_offset, where this rank's range starts in the stream, is then required."""
         alg = _alg_id(alg)
         if alg not in (0, 1):
-            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion streams without known cuts are decoded on one device)")
         if alg == 1 and range_offset is None:
             raise ValueError("sharded Cheetah stream decode: range_offset is required")
         n_halo = d_in.numel() - n_range
@@ -681,10 +687,31 @@ class ShardedDecoder(_ShardedHandle):
         blocks once, on the composition of the range maps. A refused composition sets d_flags to 1 on every rank."""
         alg = _alg_id(alg)
         if alg not in (0, 1):
-            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion is decoded in order on one device)")
+            raise ValueError("sharded stream decode: alg must be 'chameleon' or 'cheetah' (Lion streams without known cuts are decoded on one device)")
         n_halo = d_in.numel() - n_range
         if n_range < 0 or n_halo < 0:
             raise ValueError("d_in is shorter than its range")
         fn = self._lib.density_b200_decode_sharded_stream_protected if alg == 0 else self._lib.density_b200_decode_sharded_cheetah_stream_protected
         _check(fn(self._h, d_in.data_ptr(), n_range, n_halo, d_out.data_ptr(), d_out.numel(), d_size.data_ptr(), self.d_offset.data_ptr(),
                   d_flags.data_ptr(), self.d_total.data_ptr(), _stream()), f"decode_sharded{'' if alg == 0 else '_cheetah'}_stream_protected")
+
+
+class ShardedLionDecoder(_ShardedHandle):
+    """The C++ multi-GPU Lion decode (`density_b200_decode_sharded_lion`): the inverse of ShardedEncoder.encode(..., alg="lion") without
+    a gather. Boundaries, unpack and the chunk map run on every rank at once; the prediction walk is relayed from rank to rank, so the
+    pieces walk one after the other and the whole decode takes about as long as decoding the stream on one device."""
+
+    def decode(self, d_in, d_out, d_size, d_flags):
+        """Enqueue on torch's current stream; nothing blocks. d_in: this rank's piece (2-byte aligned); d_out: capacity d_out.numel()
+        (4-byte aligned); d_size int64[1]: the decoded size; d_flags int32[1]: != 0 -> the pieces are void and the caller decodes the
+        gathered stream on one device; self.d_total int64[1]: the original length."""
+        _check(self._lib.density_b200_decode_sharded_lion(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(),
+                                                          d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), _stream()),
+               "decode_sharded_lion")
+
+    def decode_protected(self, d_in, d_out, d_size, d_flags):
+        """density_b200_decode_sharded_lion_protected: the Lion pieces of any stream, copy-mode blocks included (the inverse of
+        ShardedEncoder.encode_protected(..., alg="lion")), with the arguments of decode."""
+        _check(self._lib.density_b200_decode_sharded_lion_protected(self._h, d_in.data_ptr(), d_in.numel(), d_out.data_ptr(), d_out.numel(),
+                                                                    d_size.data_ptr(), d_flags.data_ptr(), self.d_total.data_ptr(), _stream()),
+               "decode_sharded_lion_protected")

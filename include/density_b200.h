@@ -427,8 +427,8 @@ DENSITY_B200_API int density_b200_decode_sharded_protected(density_b200_sharded*
  *   - a non-final piece's blocks do not end exactly at its last byte, or meet copy mode there;
  *   - the prediction rounds did not settle within the round budget (density_b200_cheetah_decode_round_budget);
  *   - a piece is malformed, its output exceeds `cap`, or a non-final piece does not decode to whole 128-byte blocks.
- * Only the first piece may use copy mode: it holds the stream start, where every Cheetah stream has copy-mode blocks. Lion streams and
- * streams without known cuts are not decoded this way (density_b200_decode_sharded_cheetah_stream locates their pieces first). d_in must
+ * Only the first piece may use copy mode: it holds the stream start, where every Cheetah stream has copy-mode blocks. Lion streams
+ * (density_b200_decode_sharded_lion) and streams without known cuts are not decoded this way (density_b200_decode_sharded_cheetah_stream locates their pieces first). d_in must
  * be 2-byte and d_out 4-byte aligned; nothing is written past `cap`.
  *
  * Phase API of one piece (any transport; W pieces may run on one GPU): phase 1 -> exchange of the chunk-map transfers -> phase 2 -> rounds
@@ -507,6 +507,65 @@ DENSITY_B200_API int density_b200_cheetah_decode_shard_prot_phase1(density_b200_
    own workspace in the handle. */
 DENSITY_B200_API int density_b200_decode_sharded_cheetah_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out,
                                                   size_t cap, uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+
+/*
+ * Sharded Lion decode (DESIGN.md section 5): the inverse of density_b200_encode_sharded_cl (Lion), and with the prot_* first step of
+ * density_b200_encode_sharded_cl_protected (Lion), and of the slices of a single-call lion_encode stream at their pieces' prefix sums.
+ * Boundaries, unpack and the chunk map run on every piece at once, as for Cheetah (Lion's chunk map is Cheetah's). The prediction walk
+ * cannot: each piece's walk starts from the lists and the context the walk of the piece before it left, so the pieces walk one after the
+ * other and a sharded Lion decode takes about as long as decoding the whole stream on one device. Decoding every piece gives back its
+ * shard byte for byte whenever the verdict is 0. The quiet path refuses what Cheetah's refuses (copy mode or two consecutive
+ * incompressible blocks in a later piece, a cut inside a copy run or with a penalty pending, incompressible blocks on both sides of a cut,
+ * a non-final piece whose blocks do not end at its last byte); the protected path accepts all of these, with the transfers of
+ * density_b200_cheetah_decode_shard_prot_transfer. d_in must be 2-byte, d_out and the tables 4-byte, d_out_size 8-byte aligned; nothing
+ * is written past `cap`.
+ *
+ * Phase API of one piece (any transport; W pieces may run on one GPU), in this order per piece: phase 1 (or prot_transfer -> exchange
+ * of the transfers -> prot_phase1) -> exchange of the chunk-map transfers -> phase 2 -> walk -> phase 3 -> seam words -> verdict (the
+ * rule of density_b200_decode_shard_phase2's words). A call out of order, a misaligned or a null pointer returns DENSITY_B200_EARG and
+ * enqueues nothing.
+ *   chunk map     the format of density_b200_cheetah_cmap_words, folded with density_b200_cheetah_cmap_init / _fold
+ *   walk state    DENSITY_B200_LION_STATE_WORDS u32: the 65536 prediction lists (5 u32 each, context-major), then last_hash, then
+ *                 padding. The state in front of the first piece is density_b200_lion_state_init's.
+ */
+#define DENSITY_B200_LION_STATE_WORDS (5 * 65536 + 8)
+typedef struct density_b200_lion_decode_shard density_b200_lion_decode_shard; /* opaque */
+DENSITY_B200_API density_b200_lion_decode_shard* density_b200_lion_decode_shard_create(void);
+DENSITY_B200_API void density_b200_lion_decode_shard_destroy(density_b200_lion_decode_shard*);
+/* phase 1: boundaries (the first piece from the fresh protection automaton, copy mode allowed), the end of the piece, unpack, the
+   symbolic chunk-map walk and the piece's chunk-map transfer to d_cmap_out (may be NULL: no export). is_first: the piece holds the
+   stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3. */
+DENSITY_B200_API int density_b200_lion_decode_shard_phase1(density_b200_lion_decode_shard*, const uint8_t* d_in, size_t n, uint8_t* d_out,
+                                          size_t cap, int is_first, int is_last, uint32_t* d_cmap_out, void* stream);
+/* phase 2: d_cmap_carry = the chunk map before this piece (NULL = stream start). Resolves the reads of carried-in chunk-map slots. */
+DENSITY_B200_API int density_b200_lion_decode_shard_phase2(density_b200_lion_decode_shard*, const uint32_t* d_cmap_carry, void* stream);
+/* the prediction walk: on entry d_state is the walk's state in front of the piece (the first piece starts from the stream-start state
+   whatever it holds), on return the state behind it. An empty piece leaves it unchanged. */
+DENSITY_B200_API int density_b200_lion_decode_shard_walk(density_b200_lion_decode_shard*, uint32_t* d_state, void* stream);
+/* the stream-start walk state: zero lists, context 0 */
+DENSITY_B200_API int density_b200_lion_state_init(uint32_t* d_state, void* stream);
+/* phase 3: the tail of the final piece, the decoded size to *d_out_size (0 when the piece is refused) and the 8 seam words to d_seam8 in
+   the layout of density_b200_cheetah_decode_shard_phase3 (non-final pieces decode to whole 64-byte blocks). */
+DENSITY_B200_API int density_b200_lion_decode_shard_phase3(density_b200_lion_decode_shard*, uint64_t* d_out_size, uint32_t* d_seam8, void* stream);
+/* the protected first step, with the arguments and semantics of density_b200_cheetah_decode_shard_prot_transfer / _prot_phase1 on the
+   Lion geometry (35 entry offsets per 4 KiB chunk, the same 3200 candidates, 0xFFFF / 0xFFFE). Phase 2, the walk and phase 3 follow. */
+DENSITY_B200_API int density_b200_lion_decode_shard_prot_transfer(density_b200_lion_decode_shard*, const uint8_t* d_in, size_t n, uint8_t* d_out,
+                                                 size_t cap, int is_first, int is_last, uint32_t* d_transfer_out, void* stream);
+DENSITY_B200_API int density_b200_lion_decode_shard_prot_phase1(density_b200_lion_decode_shard*, const uint32_t* d_all_transfers, int world,
+                                               int rank, uint32_t* d_cmap_out, void* stream);
+/* Diagnostic, after phase 3 (synchronises the device): the walk counts of this piece, the four values of density_b200_lion_decode_stats. */
+DENSITY_B200_API int density_b200_lion_decode_shard_stats(density_b200_lion_decode_shard*, uint64_t* out4);
+/* End to end over NCCL on a density_b200_sharded handle, with the arguments and semantics of density_b200_decode_sharded_cheetah: phase 1
+   -> ncclAllGather(chunk-map transfers, 0.75 MiB per rank) -> one fold kernel -> phase 2 -> ncclRecv(walk state from rank - 1, on
+   ranks > 0) -> walk -> ncclSend(walk state to rank + 1, on all but the last rank; 1.25 MiB) -> phase 3 -> ncclAllGather(seam words) ->
+   verdict. The receive and the send are separate groups. Empty and refused pieces still receive and forward the state. Never blocks,
+   has no gather, uses its own workspace in the handle. */
+DENSITY_B200_API int density_b200_decode_sharded_lion(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                     uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
+/* The same for any stream: prot_transfer -> ncclAllGather(transfers, 12.5 KiB per rank) -> prot_phase1 -> the rest of
+   density_b200_decode_sharded_lion. */
+DENSITY_B200_API int density_b200_decode_sharded_lion_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                               uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream);
 
 /*
  * Sharded decode of a stream whose cuts are not known: a stream written by one chameleon_encode call, by the reference library,

@@ -12,6 +12,7 @@ from conftest import splitmix_bytes
 from test_gpu_sharded_cl_encode import encode_shards, even_cuts, text
 
 pytestmark = pytest.mark.gpu
+CANARY = 0xA5
 
 MIB = 1 << 20
 
@@ -41,7 +42,7 @@ def _ptr(t):
 def decode_pieces(torch, lib, enc, cuts, caps=None):
     """Every phase of every piece enc[cuts[r]:cuts[r + 1]] on one device, the exchanges replaced by stacking the transfers and folding them
     with the library's init / fold entry points, for the whole round budget. Returns (decoded pieces, (flags, total, offsets), seam
-    words [world][8], status [world][4])."""
+    words [world][8], status [world][4]). Checks that nothing is written past any piece's cap."""
     from density_b200 import sharded
     world = len(cuts) - 1
     st = _stream(torch)
@@ -51,13 +52,13 @@ def decode_pieces(torch, lib, enc, cuts, caps=None):
     for r in range(world):
         d_in = torch.from_numpy(np.ascontiguousarray(enc[cuts[r]:cuts[r + 1]])).cuda()
         cap = caps[r] if caps is not None else 16 * d_in.numel() + 256
-        d_out = torch.zeros(max(cap, 1), dtype=torch.uint8, device="cuda")
+        d_out = torch.full((max(cap, 1) + 64,), CANARY, dtype=torch.uint8, device="cuda")
         h = lib.density_b200_cheetah_decode_shard_create()
         assert h
         rc = lib.density_b200_cheetah_decode_shard_phase1(h, _ptr(d_in), d_in.numel(), d_out.data_ptr(), cap, int(r == 0), int(r == world - 1),
                                                           tc[r].data_ptr(), st)
         assert rc == 0, lib.density_b200_last_error()
-        hs.append(h); ins.append(d_in); outs.append(d_out)
+        hs.append(h); ins.append(d_in); outs.append((d_out, cap))
     for r in range(world):
         carry = sharded.fold_cheetah_cmap(tc, r) if r > 0 else None
         assert lib.density_b200_cheetah_decode_shard_phase2(hs[r], carry.data_ptr() if carry is not None else None, st) == 0
@@ -82,8 +83,10 @@ def decode_pieces(torch, lib, enc, cuts, caps=None):
         assert lib.density_b200_cheetah_decode_shard_status(hs[r], s4) == 0
         status.append(list(s4))
         lib.density_b200_cheetah_decode_shard_destroy(hs[r])
+    for r, (d_out, cap) in enumerate(outs):
+        assert bool((d_out[cap:] == CANARY).all()), f"piece {r} written past cap"
     verdict = sharded.seam_verdict(seam)
-    pieces = [outs[r][:int(sizes[r].item())].cpu().numpy() for r in range(world)]
+    pieces = [outs[r][0][:int(sizes[r].item())].cpu().numpy() for r in range(world)]
     return pieces, verdict, seam.cpu().numpy(), status
 
 

@@ -1051,6 +1051,29 @@ int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_
     return step_result(e, l, "cl_table_fold");
 }
 
+// ---- the argument rule of the sharded decode pieces and drivers (include/density_b200.h): d_in 2-byte, d_out and every table,
+// transfer, carry and word buffer 4-byte, d_out_size 8-byte, d_seam8 4-byte aligned. Each helper returns DENSITY_B200_EARG with the
+// error set, or DENSITY_B200_OK.
+static bool al8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+// the input and the output of a piece; either may be null when its length is 0
+static int decode_in_args(const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap) {
+    if ((!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_out)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+// tables, transfers, carries and words, null where the entry allows it (the caller checks that)
+static int decode_table_args(std::initializer_list<const void*> tables) {
+    for (const void* t : tables)
+        if (!al4(t)) { set_error("tables, transfers, carries and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+// the size and the seam words a piece writes
+static int decode_out_args(const uint64_t* d_out_size, const uint32_t* d_seam8) {
+    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!al8(d_out_size) || !al4(d_seam8)) { set_error("d_out_size must be 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
 struct density_b200_decode_shard {
     DevBuf ws;
@@ -1070,29 +1093,46 @@ void density_b200_decode_shard_destroy(density_b200_decode_shard* s) {
     s->seed.release();
     delete s;
 }
+// the piece set up in s (phase 1, prot_transfer and prot_enter): phase 2 waits for the next phase 1 (with_seed, a protected entry: the
+// protected sequence starts over), the workspace and with_seed the seed are ensured, the piece is stored
+static int decode_piece_setup(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last, bool with_seed, cudaStream_t st) {
+    s->phase1_done = false;
+    if (with_seed) s->prot_stage = 0;
+    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
+    if (e == cudaSuccess && with_seed) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last;
+    return DENSITY_B200_OK;
+}
 int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
                                      uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_in) & 1) { set_error("d_in must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase1_done = false;
-    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    int rc = decode_in_args(d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table_out});
+    if (rc == DENSITY_B200_OK) rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, false, st);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    if (n == 0) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
-    else e = cham_decode_phase1(d_in, n, cap, s->ws.p, s->num_sms, d_table_out, st, &launches);
-    const int rc = step_result(e, launches, "decode shard phase1");
+    const cudaError_t e = n ? cham_decode_phase1(d_in, n, cap, s->ws.p, s->num_sms, d_table_out, st, &launches)
+                            : cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
+    rc = step_result(e, launches, "decode shard phase1");
     if (rc == DENSITY_B200_OK) s->phase1_done = true;
     return rc;
+}
+// the arguments of both phase-2 entries
+static int decode_phase2_args(const density_b200_decode_shard* s, const uint32_t* d_carry_in, const uint8_t* d_out, const uint64_t* d_out_size,
+                              const uint32_t* d_seam8) {
+    int rc = decode_in_args(nullptr, 0, d_out, s->cap);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_carry_in});
+    return rc == DENSITY_B200_OK ? decode_out_args(d_out_size, d_seam8) : rc;
 }
 int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
                                      uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
     if (!s || !s->phase1_done) { set_error("decode_shard_phase2: phase1 not done"); return DENSITY_B200_EARG; }
-    if ((!d_out && s->cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_out) & 3) { set_error("d_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    const int rc = decode_phase2_args(s, d_carry_in, d_out, d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
     cudaError_t e = s->n ? cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches)
@@ -1106,17 +1146,15 @@ int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_
 int density_b200_decode_shard_prot_transfer(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
                                             uint32_t* d_transfer_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_transfer_out)) { set_error("d_in must be 2-byte, d_transfer_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase1_done = false; s->prot_stage = 0;
-    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
-    if (e == cudaSuccess) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    int rc = decode_in_args(d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_transfer_out});
+    if (rc == DENSITY_B200_OK) rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    e = cham_decode_prot_transfer(d_in, n, cap, s->ws.p, s->num_sms, is_last_shard, d_transfer_out, st, &launches);
-    const int rc = step_result(e, launches, "decode shard prot transfer");
+    const cudaError_t e = cham_decode_prot_transfer(d_in, n, cap, s->ws.p, s->num_sms, is_last_shard, d_transfer_out, st, &launches);
+    rc = step_result(e, launches, "decode shard prot transfer");
     if (rc == DENSITY_B200_OK) s->prot_stage = 1;
     return rc;
 }
@@ -1140,29 +1178,28 @@ int density_b200_decode_shard_prot_phase1(density_b200_decode_shard* s, const ui
     g_last_error.clear();
     if (!s || s->prot_stage != 1) { set_error("decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers) || !d_table_out) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_table_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    const int rc = decode_table_args({d_all_transfers, d_table_out});
+    if (rc != DENSITY_B200_OK) return rc;
     return decode_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_table_out, reinterpret_cast<cudaStream_t>(stream), "decode shard prot phase1");
 }
 int density_b200_decode_shard_prot_enter(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
                                          uint32_t candidate, uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_table_out)) { set_error("d_in must be 2-byte, d_table_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
+    if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase1_done = false; s->prot_stage = 0;
-    cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
-    if (e == cudaSuccess) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->cap = cap; s->is_last = is_last_shard;
+    int rc = decode_in_args(d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table_out});
+    if (rc != DENSITY_B200_OK) return rc;
+    if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
+    if ((rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, true, st)) != DENSITY_B200_OK) return rc;
     return decode_prot_phase1_body(s, nullptr, 0, candidate, false, d_table_out, st, "decode shard prot enter");
 }
 int density_b200_decode_shard_prot_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
                                           uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
     if (!s || s->prot_stage != 2) { set_error("decode_shard_prot_phase2: null pointer / phase1 not done"); return DENSITY_B200_EARG; }
-    if ((!d_out && s->cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_out) & 3) { set_error("d_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    const int rc = decode_phase2_args(s, d_carry_in, d_out, d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
     cudaError_t e = s->n ? cham_decode_phase2(s->d_in, s->n, d_out, s->cap, s->ws.p, s->num_sms, d_carry_in, d_out_size, st, &launches) : cudaSuccess;
@@ -1173,66 +1210,148 @@ int density_b200_decode_shard_prot_phase2(density_b200_decode_shard* s, const ui
     return step_result(e, launches, "decode shard prot phase2");
 }
 
-// ---- sharded Cheetah decode: one piece, its chunk map carried in and its prediction rounds run over all pieces ------------------------
+// ---- sharded Cheetah and Lion decode: one piece, its chunk map carried in, then Cheetah's prediction rounds run over all pieces or Lion's
+// prediction walk continued from the state the piece before it left ----------------------------------------------------------------------
 static int g_chee_dec_rounds = 40;    // round budget of the sharded Cheetah decode (density_b200_test_set_decode_rounds)
 
-struct density_b200_cheetah_decode_shard {
+// the phase object of one piece; a.lion: a Lion piece
+struct ClDecodePiece {
     DevBuf ws, tables;
     DevBuf seed;                    // the incoming automaton state of the prot_* phases (DECODE_PROT_SEED_WORDS)
     CheeShardArgs a{};
     int num_sms = 0;
-    // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2 or a round's fold, 3 a round's walk, 4 phase 3
+    // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2 or (Cheetah) a round's fold, 3 a round's walk (Cheetah) or
+    // the walk (Lion), 4 phase 3
     int phase = 0;
-    uint32_t round = 0;
+    uint32_t round = 0;             // Cheetah: the rounds folded
     bool transfer_done = false;     // prot_transfer done, prot_phase1 not yet
-    bool prot = false;              // the current piece went through prot_phase1: phase 3 writes the protected seam words
+    bool prot = false;              // the current piece went through prot_phase1 or prot_enter: phase 3 writes the protected seam words
+    ~ClDecodePiece() { ws.release(); tables.release(); seed.release(); }
 };
+struct density_b200_cheetah_decode_shard : ClDecodePiece {};
+struct density_b200_lion_decode_shard : ClDecodePiece {};
+static_assert(LION_STATE_WORDS == DENSITY_B200_LION_STATE_WORDS, "the relayed state of the header and of cl_decode.cu");
 
 density_b200_cheetah_decode_shard* density_b200_cheetah_decode_shard_create(void) { return new_shard<density_b200_cheetah_decode_shard>(); }
-void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard* s) {
-    if (!s) return;
-    s->ws.release(); s->tables.release(); s->seed.release();
-    delete s;
-}
+density_b200_lion_decode_shard* density_b200_lion_decode_shard_create(void) { return new_shard<density_b200_lion_decode_shard>(); }
+void density_b200_cheetah_decode_shard_destroy(density_b200_cheetah_decode_shard* s) { delete s; }
+void density_b200_lion_decode_shard_destroy(density_b200_lion_decode_shard* s) { delete s; }
 int density_b200_cheetah_decode_round_budget(void) { return g_chee_dec_rounds; }
 size_t density_b200_cheetah_cmap_words(void) { return 3 * 65536; }
 
-int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                             int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
-    g_last_error.clear();
-    if (!s || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+// the argument checks and the piece set up in s->a (phase 1, prot_transfer and prot_enter): the piece's state reset, its workspace and
+// tables (with_seed: and the seed) ensured for its geometry. d_table: the chunk-map or protection transfer out (need_table: not null).
+// DENSITY_B200_OK, or the error code with nothing enqueued.
+static int cl_piece_setup(ClDecodePiece* s, bool lion, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
+                          const uint32_t* d_table, bool need_table, bool with_seed, cudaStream_t st) {
+    if (!s || (need_table && !d_table)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = decode_in_args(d_in, n, d_out, cap);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table});
+    if (rc != DENSITY_B200_OK) return rc;
     s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
     CheeShardArgs& a = s->a;
-    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
-    cudaError_t e = cudaSuccess;
+    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.lion = lion; a.num_sms = s->num_sms;
+    cudaError_t e = with_seed ? s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st) : cudaSuccess;
     if (n) {
-        e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
-        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
-        if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        if (e == cudaSuccess) e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms, lion), st);
+        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms, lion) + 256, st);
     }
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     a.ws = s->ws.p; a.tables = s->tables.p;
+    return DENSITY_B200_OK;
+}
+// phase 1 of the piece set up in s->a (d_seed, rows_ready: chee_shard_phase1's); an empty piece passes the chunk map on unchanged
+static cudaError_t cl_piece_phase1_launch(const ClDecodePiece* s, uint32_t* d_cmap_out, cudaStream_t st, uint64_t* launches,
+                                          const uint32_t* d_seed = nullptr, bool rows_ready = false) {
+    if (s->a.n) return chee_shard_phase1(s->a, d_cmap_out, st, launches, d_seed, rows_ready);
+    return d_cmap_out ? chee_cmap_identity(d_cmap_out, st, launches) : cudaSuccess;
+}
+static int cl_piece_phase1(ClDecodePiece* s, bool lion, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
+                           uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    int rc = cl_piece_setup(s, lion, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, false, false, st);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    if (n) e = chee_shard_phase1(a, d_cmap_out, st, &launches);
-    else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
-    const int rc = step_result(e, launches, "cheetah decode shard phase1");
+    const cudaError_t e = cl_piece_phase1_launch(s, d_cmap_out, st, &launches);
+    rc = step_result(e, launches, "cl decode shard phase1");
     if (rc == DENSITY_B200_OK) s->phase = 1;
     return rc;
 }
-int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
+static int cl_piece_phase2(ClDecodePiece* s, const uint32_t* d_cmap_carry, void* stream) {
     g_last_error.clear();
-    if (!s || s->phase != 1) { set_error("cheetah_decode_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
+    if (!s || s->phase != 1) { set_error("cl decode shard phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
+    int rc = decode_table_args({d_cmap_carry});
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
     const cudaError_t e = s->a.n ? chee_shard_phase2(s->a, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;
-    const int rc = step_result(e, launches, "cheetah decode shard phase2");
+    rc = step_result(e, launches, "cl decode shard phase2");
     if (rc == DENSITY_B200_OK) s->phase = 2;
     return rc;
+}
+// ready: the step before phase 3 is done (the wrappers' rule)
+static int cl_piece_phase3(ClDecodePiece* s, bool ready, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
+    g_last_error.clear();
+    if (!s || !ready) { set_error("cl decode shard phase3: null pointer / the step before it not done"); return DENSITY_B200_EARG; }
+    int rc = decode_out_args(d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint64_t launches = 0;
+    const uint32_t* seed = s->prot ? reinterpret_cast<const uint32_t*>(s->seed.p) : nullptr;
+    const cudaError_t e = (s->a.n || seed) ? chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches, seed) : empty_piece_outputs(d_out_size, d_seam8, st);
+    rc = step_result(e, launches, "cl decode shard phase3");
+    if (rc == DENSITY_B200_OK) s->phase = 4;
+    return rc;
+}
+
+// ---- the same for streams with copy-mode blocks: the piece's protection transfer, then phase 1 from the composed state -------------------
+static int cl_piece_prot_transfer(ClDecodePiece* s, bool lion, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
+                                  uint32_t* d_transfer_out, void* stream) {
+    g_last_error.clear();
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    int rc = cl_piece_setup(s, lion, d_in, n, d_out, cap, is_first, is_last, d_transfer_out, true, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    uint64_t launches = 0;
+    const cudaError_t e = chee_shard_prot_transfer(s->a, d_transfer_out, st, &launches);
+    rc = step_result(e, launches, "cl decode shard prot transfer");
+    if (rc == DENSITY_B200_OK) s->transfer_done = true;
+    return rc;
+}
+// The protected phase 1 of the piece set up in s->a (see decode_prot_phase1_body)
+static int cl_piece_prot_phase1_body(ClDecodePiece* s, const uint32_t* d_all_transfers, int rank, uint32_t x0, bool rows_ready,
+                                     uint32_t* d_cmap_out, cudaStream_t st, const char* what) {
+    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
+    uint64_t launches = 0;
+    s->transfer_done = false;   // one phase 1 per transfer
+    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, x0, seed, st, &launches);
+    if (e == cudaSuccess) e = cl_piece_phase1_launch(s, d_cmap_out, st, &launches, seed, rows_ready);
+    const int rc = step_result(e, launches, what);
+    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
+    return rc;
+}
+static int cl_piece_prot_phase1(ClDecodePiece* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_cmap_out, void* stream) {
+    g_last_error.clear();
+    if (!s || !s->transfer_done || s->phase != 0) { set_error("cl decode shard prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
+    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
+    const int rc = decode_table_args({d_all_transfers, d_cmap_out});
+    if (rc != DENSITY_B200_OK) return rc;
+    return cl_piece_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_cmap_out, reinterpret_cast<cudaStream_t>(stream), "cl decode shard prot phase1");
+}
+
+// ---- the Cheetah piece: the phases above, the prediction rounds between phase 2 and phase 3, and the entry of a located piece ------------
+int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                                             int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
+    return cl_piece_phase1(s, false, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, stream);
+}
+int density_b200_cheetah_decode_shard_phase2(density_b200_cheetah_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
+    return cl_piece_phase2(s, d_cmap_carry, stream);
 }
 int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_shard* s, uint32_t* d_pred_out, uint32_t* d_words4, void* stream) {
     g_last_error.clear();
     if (!s || s->phase != 2) { set_error("cheetah_decode_shard_round_walk: null pointer / phase 2 or the previous round's fold not done"); return DENSITY_B200_EARG; }
     if (!d_words4) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = decode_table_args({d_pred_out, d_words4});
+    if (rc != DENSITY_B200_OK) return rc;
     if (s->round >= (uint32_t)g_chee_dec_rounds) { set_error("cheetah_decode_shard_round_walk: round budget used up"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
@@ -1242,7 +1361,7 @@ int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_sha
         e = cudaMemsetAsync(d_words4, 0, 4 * sizeof(uint32_t), st);
         if (e == cudaSuccess && d_pred_out) e = cudaMemsetAsync(d_pred_out, 0, 2 * 65536 * sizeof(uint32_t), st);
     }
-    const int rc = step_result(e, launches, "cheetah decode shard round walk");
+    rc = step_result(e, launches, "cheetah decode shard round walk");
     if (rc == DENSITY_B200_OK) s->phase = 3;
     return rc;
 }
@@ -1251,96 +1370,35 @@ int density_b200_cheetah_decode_shard_round_fold(density_b200_cheetah_decode_sha
     g_last_error.clear();
     if (!s || s->phase != 3) { set_error("cheetah_decode_shard_round_fold: null pointer / the round's walk not done"); return DENSITY_B200_EARG; }
     if (!d_all_words || world < 1 || rank < 0 || rank >= world) { set_error("cheetah_decode_shard_round_fold: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
+    int rc = decode_table_args({d_pred_carry, d_all_words});
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
     const cudaError_t e = s->a.n ? chee_shard_round_fold(s->a, s->round, d_pred_carry, d_all_words, (uint32_t)world, (uint32_t)rank,
                                                          reinterpret_cast<cudaStream_t>(stream), &launches)
                                  : cudaSuccess;
-    const int rc = step_result(e, launches, "cheetah decode shard round fold");
+    rc = step_result(e, launches, "cheetah decode shard round fold");
     if (rc == DENSITY_B200_OK) { s->phase = 2; ++s->round; }
     return rc;
 }
 int density_b200_cheetah_decode_shard_phase3(density_b200_cheetah_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
-    g_last_error.clear();
-    if (!s || s->phase != 2) { set_error("cheetah_decode_shard_phase3: null pointer / phase 2 or the last round's fold not done"); return DENSITY_B200_EARG; }
-    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    uint64_t launches = 0;
-    const uint32_t* seed = s->prot ? reinterpret_cast<const uint32_t*>(s->seed.p) : nullptr;
-    const cudaError_t e = (s->a.n || seed) ? chee_shard_phase3(s->a, d_out_size, d_seam8, st, &launches, seed) : empty_piece_outputs(d_out_size, d_seam8, st);
-    const int rc = step_result(e, launches, "cheetah decode shard phase3");
-    if (rc == DENSITY_B200_OK) s->phase = 4;
-    return rc;
+    return cl_piece_phase3(s, s && s->phase == 2, d_out_size, d_seam8, stream);     // after phase 2 or the last round's fold
 }
-
-// ---- the same for streams with copy-mode blocks: the piece's protection transfer, then phase 1 from the composed state -------------------
 int density_b200_cheetah_decode_shard_prot_transfer(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                                     int is_first, int is_last, uint32_t* d_transfer_out, void* stream) {
-    g_last_error.clear();
-    if (!s || (!d_in && n) || (!d_out && cap) || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_transfer_out)) {
-        set_error("d_in must be 2-byte, d_out and d_transfer_out 4-byte aligned"); return DENSITY_B200_EARG;
-    }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
-    CheeShardArgs& a = s->a;
-    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
-    cudaError_t e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
-    if (n) {
-        if (e == cudaSuccess) e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
-        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
-    }
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    a.ws = s->ws.p; a.tables = s->tables.p;
-    uint64_t launches = 0;
-    e = chee_shard_prot_transfer(a, d_transfer_out, st, &launches);
-    const int rc = step_result(e, launches, "cheetah decode shard prot transfer");
-    if (rc == DENSITY_B200_OK) s->transfer_done = true;
-    return rc;
-}
-// The protected phase 1 of the piece set up in s->a (see decode_prot_phase1_body)
-static int cheetah_prot_phase1_body(density_b200_cheetah_decode_shard* s, const uint32_t* d_all_transfers, int rank, uint32_t x0, bool rows_ready,
-                                    uint32_t* d_cmap_out, cudaStream_t st, const char* what) {
-    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
-    uint64_t launches = 0;
-    s->transfer_done = false;   // one phase 1 per transfer
-    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, x0, seed, st, &launches);
-    if (e == cudaSuccess) {
-        if (s->a.n) e = chee_shard_phase1(s->a, d_cmap_out, st, &launches, seed, rows_ready);
-        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
-    }
-    const int rc = step_result(e, launches, what);
-    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
-    return rc;
+    return cl_piece_prot_transfer(s, false, d_in, n, d_out, cap, is_first, is_last, d_transfer_out, stream);
 }
 int density_b200_cheetah_decode_shard_prot_phase1(density_b200_cheetah_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
                                                   uint32_t* d_cmap_out, void* stream) {
-    g_last_error.clear();
-    if (!s || !s->transfer_done || s->phase != 0) { set_error("cheetah_decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
-    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_cmap_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    return cheetah_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_cmap_out, reinterpret_cast<cudaStream_t>(stream),
-                                    "cheetah decode shard prot phase1");
+    return cl_piece_prot_phase1(s, d_all_transfers, world, rank, d_cmap_out, stream);
 }
 int density_b200_cheetah_decode_shard_prot_enter(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                                  int is_first, int is_last, uint32_t candidate, uint32_t* d_cmap_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_cmap_out)) {
-        set_error("d_in must be 2-byte, d_out and d_cmap_out 4-byte aligned"); return DENSITY_B200_EARG;
-    }
     if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("cheetah_decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
-    CheeShardArgs& a = s->a;
-    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
-    cudaError_t e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
-    if (n) {
-        if (e == cudaSuccess) e = s->ws.ensure(chee_shard_workspace_bytes(n, cap, s->num_sms), st);
-        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms) + 256, st);
-    }
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    a.ws = s->ws.p; a.tables = s->tables.p;
-    return cheetah_prot_phase1_body(s, nullptr, 0, candidate, false, d_cmap_out, st, "cheetah decode shard prot enter");
+    const int rc = cl_piece_setup(s, false, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, false, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    return cl_piece_prot_phase1_body(s, nullptr, 0, candidate, false, d_cmap_out, st, "cheetah decode shard prot enter");
 }
 
 int density_b200_cheetah_decode_shard_status(density_b200_cheetah_decode_shard* s, uint32_t* out4) {
@@ -1370,67 +1428,13 @@ int density_b200_cheetah_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, void
     return step_result(e, l, "cheetah_cmap_fold");
 }
 
-// ---- sharded Lion decode: one piece, its chunk map carried in and the prediction walk's state relayed from the piece before it ---------
-struct density_b200_lion_decode_shard {
-    DevBuf ws, tables;
-    DevBuf seed;                    // the incoming automaton state of the prot_* phases (DECODE_PROT_SEED_WORDS)
-    CheeShardArgs a{};
-    int num_sms = 0;
-    // the last step done on the current piece: 0 none, 1 phase 1, 2 phase 2, 3 the walk, 4 phase 3
-    int phase = 0;
-    bool transfer_done = false;     // prot_transfer done, prot_phase1 not yet
-    bool prot = false;              // the current piece went through prot_phase1: phase 3 writes the protected seam words
-};
-static_assert(LION_STATE_WORDS == DENSITY_B200_LION_STATE_WORDS, "the relayed state of the header and of cl_decode.cu");
-
-density_b200_lion_decode_shard* density_b200_lion_decode_shard_create(void) { return new_shard<density_b200_lion_decode_shard>(); }
-void density_b200_lion_decode_shard_destroy(density_b200_lion_decode_shard* s) {
-    if (!s) return;
-    s->ws.release(); s->tables.release(); s->seed.release();
-    delete s;
-}
-// the argument checks and the piece set up in s->a (phase 1 and prot_transfer); DENSITY_B200_OK or the error code, with nothing enqueued
-static int lion_shard_setup(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first,
-                            int is_last, const uint32_t* d_table, bool need_table, bool with_seed, cudaStream_t st) {
-    if (!s || (!d_in && n) || (!d_out && cap) || (need_table && !d_table)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3) || !al4(d_table)) {
-        set_error("d_in must be 2-byte, d_out and the tables 4-byte aligned"); return DENSITY_B200_EARG;
-    }
-    s->phase = 0; s->transfer_done = false; s->prot = false;
-    CheeShardArgs& a = s->a;
-    a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.num_sms = s->num_sms;
-    cudaError_t e = with_seed ? s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st) : cudaSuccess;
-    if (n) {
-        if (e == cudaSuccess) e = s->ws.ensure(lion_shard_workspace_bytes(n, cap, s->num_sms), st);
-        if (e == cudaSuccess) e = s->tables.ensure(chee_decode_tables_bytes(n, s->num_sms, true) + 256, st);
-    }
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    a.ws = s->ws.p; a.tables = s->tables.p;
-    return DENSITY_B200_OK;
-}
+// ---- the Lion piece: the phases above and the prediction walk between phase 2 and phase 3 ----------------------------------------------
 int density_b200_lion_decode_shard_phase1(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                           int is_first, int is_last, uint32_t* d_cmap_out, void* stream) {
-    g_last_error.clear();
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = lion_shard_setup(s, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, false, false, st);
-    if (rc != DENSITY_B200_OK) return rc;
-    uint64_t launches = 0;
-    cudaError_t e = cudaSuccess;
-    if (n) e = lion_shard_phase1(s->a, d_cmap_out, st, &launches);
-    else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
-    rc = step_result(e, launches, "lion decode shard phase1");
-    if (rc == DENSITY_B200_OK) s->phase = 1;
-    return rc;
+    return cl_piece_phase1(s, true, d_in, n, d_out, cap, is_first, is_last, d_cmap_out, stream);
 }
 int density_b200_lion_decode_shard_phase2(density_b200_lion_decode_shard* s, const uint32_t* d_cmap_carry, void* stream) {
-    g_last_error.clear();
-    if (!s || s->phase != 1) { set_error("lion_decode_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
-    if (!al4(d_cmap_carry)) { set_error("d_cmap_carry must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    uint64_t launches = 0;
-    const cudaError_t e = s->a.n ? lion_shard_phase2(s->a, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;
-    const int rc = step_result(e, launches, "lion decode shard phase2");
-    if (rc == DENSITY_B200_OK) s->phase = 2;
-    return rc;
+    return cl_piece_phase2(s, d_cmap_carry, stream);
 }
 int density_b200_lion_decode_shard_walk(density_b200_lion_decode_shard* s, uint32_t* d_state, void* stream) {
     g_last_error.clear();
@@ -1448,48 +1452,15 @@ int density_b200_lion_state_init(uint32_t* d_state, void* stream) {
     return step_result(lion_state_init(d_state, reinterpret_cast<cudaStream_t>(stream)), 0, "lion_state_init");
 }
 int density_b200_lion_decode_shard_phase3(density_b200_lion_decode_shard* s, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
-    g_last_error.clear();
-    if (!s || s->phase != 3) { set_error("lion_decode_shard_phase3: null pointer / the walk not done"); return DENSITY_B200_EARG; }
-    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) { set_error("d_out_size must be 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    uint64_t launches = 0;
-    const uint32_t* seed = s->prot ? reinterpret_cast<const uint32_t*>(s->seed.p) : nullptr;
-    const cudaError_t e = (s->a.n || seed) ? lion_shard_phase3(s->a, d_out_size, d_seam8, st, &launches, seed) : empty_piece_outputs(d_out_size, d_seam8, st);
-    const int rc = step_result(e, launches, "lion decode shard phase3");
-    if (rc == DENSITY_B200_OK) s->phase = 4;
-    return rc;
+    return cl_piece_phase3(s, s && s->phase == 3, d_out_size, d_seam8, stream);     // after the walk
 }
 int density_b200_lion_decode_shard_prot_transfer(density_b200_lion_decode_shard* s, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                                  int is_first, int is_last, uint32_t* d_transfer_out, void* stream) {
-    g_last_error.clear();
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = lion_shard_setup(s, d_in, n, d_out, cap, is_first, is_last, d_transfer_out, true, true, st);
-    if (rc != DENSITY_B200_OK) return rc;
-    uint64_t launches = 0;
-    const cudaError_t e = lion_shard_prot_transfer(s->a, d_transfer_out, st, &launches);
-    rc = step_result(e, launches, "lion decode shard prot transfer");
-    if (rc == DENSITY_B200_OK) s->transfer_done = true;
-    return rc;
+    return cl_piece_prot_transfer(s, true, d_in, n, d_out, cap, is_first, is_last, d_transfer_out, stream);
 }
 int density_b200_lion_decode_shard_prot_phase1(density_b200_lion_decode_shard* s, const uint32_t* d_all_transfers, int world, int rank,
                                                uint32_t* d_cmap_out, void* stream) {
-    g_last_error.clear();
-    if (!s || !s->transfer_done || s->phase != 0) { set_error("lion_decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
-    if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_cmap_out)) { set_error("transfers and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    uint32_t* seed = reinterpret_cast<uint32_t*>(s->seed.p);
-    uint64_t launches = 0;
-    s->transfer_done = false;   // one phase 1 per transfer
-    cudaError_t e = chee_shard_prot_enter(d_all_transfers, (uint32_t)rank, 0, seed, st, &launches);
-    if (e == cudaSuccess) {
-        if (s->a.n) e = lion_shard_phase1(s->a, d_cmap_out, st, &launches, seed, true);
-        else if (d_cmap_out) e = chee_cmap_identity(d_cmap_out, st, &launches);    // an empty piece passes the chunk map on unchanged
-    }
-    const int rc = step_result(e, launches, "lion decode shard prot phase1");
-    if (rc == DENSITY_B200_OK) { s->phase = 1; s->prot = true; }
-    return rc;
+    return cl_piece_prot_phase1(s, d_all_transfers, world, rank, d_cmap_out, stream);
 }
 int density_b200_lion_decode_shard_stats(density_b200_lion_decode_shard* s, uint64_t* out4) {
     g_last_error.clear();
@@ -1498,7 +1469,7 @@ int density_b200_lion_decode_shard_stats(density_b200_lion_decode_shard* s, uint
     if (!s->a.n) return DENSITY_B200_OK;    // an empty piece walks nothing
     cudaError_t e = cudaDeviceSynchronize();
     // the counts follow the ClStatus prefix of the walk's status (8 u32)
-    if (e == cudaSuccess) e = cudaMemcpy(out4, static_cast<const uint8_t*>(lion_shard_status_ptr(s->a)) + 32, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(out4, static_cast<const uint8_t*>(chee_shard_status_ptr(s->a)) + 32, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) { set_error("lion_decode_shard_stats", e); return DENSITY_B200_ECUDA; }
     return DENSITY_B200_OK;
 }
@@ -1972,9 +1943,9 @@ int density_b200_encode_sharded_cl_protected(density_b200_sharded* h, int alg, c
 // the argument checks of the sharded decoders; n: the bytes of d_in
 static int decode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap, const uint64_t* d_out_size,
                                const uint32_t* d_flags) {
-    if (!h || (!d_in && n) || (!d_out && cap) || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_out) & 3)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    return DENSITY_B200_OK;
+    if (!h || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!al8(d_out_size)) { set_error("d_out_size must be 8-byte aligned"); return DENSITY_B200_EARG; }
+    return decode_in_args(d_in, n, d_out, cap);
 }
 
 // The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it: phase 1 -> table exchange ->
@@ -2035,165 +2006,143 @@ int density_b200_decode_sharded_protected(density_b200_sharded* h, const uint8_t
     return x.verdict(d_flags, d_total_size, nullptr);
 }
 
-// the exchange buffers of decode_sharded_cheetah_piece: gathered chunk-map and prediction transfers, the carries, the round words
-static size_t cheetah_piece_extra_bytes(const density_b200_sharded* h) {
-    return (((size_t)h->world + 1) * (density_b200_cheetah_cmap_words() + 2 * 65536) + 4 * (size_t)h->world + 64) * sizeof(uint32_t);
+// The exchange buffers of decode_sharded_cl_piece behind Exchange::extra (extra: nullptr for the size alone), in this order: the gathered
+// chunk-map transfers [world][cmap words] and the carry; Cheetah: the gathered prediction transfers [world][2 * 65536], their carry and
+// the round words [world][4]; Lion: the walk state (DENSITY_B200_LION_STATE_WORDS); then with prot the gathered protection transfers
+// [world][DECODE_PROT_TRANSFER_WORDS], with map_words the range maps [world][map_words] and the composition's 8 u64 words.
+struct ClPieceBufs {
+    uint32_t *tab_c, *carry_c, *tab_p, *carry_p, *rwords, *state, *transfers, *maps;
+    size_t bytes;
+};
+static ClPieceBufs cl_piece_bufs(int alg, size_t world, bool prot, size_t map_words, uint8_t* extra = nullptr) {
+    ClPieceBufs b{};
+    size_t off = 0;    // u32 words
+    auto take = [&](size_t words) { uint32_t* p = extra ? reinterpret_cast<uint32_t*>(extra) + off : nullptr; off += words; return p; };
+    const size_t wc = density_b200_cheetah_cmap_words(), wp = 2 * 65536;
+    b.tab_c = take(world * wc);
+    b.carry_c = take(wc);
+    if (alg == ALG_CHEETAH) {
+        b.tab_p = take(world * wp);
+        b.carry_p = take(wp);
+        b.rwords = take(4 * world);
+    } else {
+        b.state = take(DENSITY_B200_LION_STATE_WORDS);
+    }
+    if (prot) b.transfers = take(world * DECODE_PROT_TRANSFER_WORDS);
+    if (map_words) b.maps = take(world * map_words + 16);
+    b.bytes = (off + 64) * sizeof(uint32_t);
+    return b;
 }
 
-// Sharded Cheetah decode of this rank's piece d_in[0 .. n) over the handle's communicator: phase 1 -> chunk-map transfers -> fold ->
-// phase 2 -> every round of the budget (walk -> prediction transfers + round words -> fold) -> phase 3 -> seam words -> verdict. Every
-// rank issues the same collectives in the same order whatever its piece holds: an empty piece sends identity transfers and zero words, a
-// refused one keeps exchanging until the verdict. The rounds after the settled one are gated off on the device; their all-gathers still
-// run. first: the piece holds the stream start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output
-// starts, from the verdict's prefix offsets. x is opened with cheetah_piece_extra_bytes. prot: a piece of a stream with copy-mode blocks
-// (density_b200_decode_sharded_cheetah_protected): phase 1 is the protection transfer -> ncclAllGather(transfers) -> prot_phase1, and x
-// holds the gathered transfers behind the buffers of cheetah_piece_extra_bytes. cand >= 0 (prot false): a located piece of a stream with
-// copy-mode blocks (density_b200_decode_sharded_cheetah_stream_protected), whose phase 1 is prot_enter from that candidate.
-static int decode_sharded_cheetah_piece(const Exchange& x, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
-                                        uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot,
-                                        int64_t cand = -1) {
+// Sharded Cheetah or Lion decode of this rank's piece d_in[0 .. n) over the handle's communicator; x is opened with
+// cl_piece_bufs(alg, world, prot, ..).bytes.
+//   head    [prot: prot_transfer -> ncclAllGather(transfers) -> prot_phase1 | cand >= 0: prot_enter from that candidate (a located piece of
+//           a Cheetah stream with copy-mode blocks, density_b200_decode_sharded_cheetah_stream_protected) | phase 1] -> chunk-map transfers
+//           -> fold -> phase 2
+//   middle  Cheetah: every round of the budget (walk -> prediction transfers + round words -> fold); the rounds after the settled one are
+//           gated off on the device, their all-gathers still run. Lion: the relay of the walk's state (receive from rank - 1, walk, send
+//           to rank + 1).
+//   tail    phase 3 -> seam words -> verdict
+// Every rank issues the same collectives in the same order whatever its piece holds: an empty piece sends identity transfers and zero
+// words and forwards the walk's state unchanged, a refused one keeps exchanging until the verdict. first: the piece holds the stream
+// start; last: no stream byte follows it. d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
+static int decode_sharded_cl_piece(const Exchange& x, int alg, const uint8_t* d_in, size_t n, bool first, bool last, uint8_t* d_out, size_t cap,
+                                   uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot,
+                                   int64_t cand = -1) {
     density_b200_sharded* h = x.h;
     cudaStream_t st = x.st;
-    density_b200_cheetah_decode_shard* s = h->cdec;
+    const bool lion = alg == ALG_LION;
+    density_b200_lion_decode_shard* ls = prot ? h->lpdec : h->ldec;
+    ClDecodePiece* s = lion ? static_cast<ClDecodePiece*>(ls) : h->cdec;
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wc = density_b200_cheetah_cmap_words(), wp = 2 * 65536;
-    uint32_t* tab_c = reinterpret_cast<uint32_t*>(x.extra);              // [world][wc]
-    uint32_t* carry_c = tab_c + W * wc;
-    uint32_t* tab_p = carry_c + wc;                                       // [world][wp]
-    uint32_t* carry_p = tab_p + W * wp;
-    uint32_t* rwords = carry_p + wp;                                      // [world][4]
-    uint64_t launches = 0;
+    const ClPieceBufs b = cl_piece_bufs(alg, W, prot, 0, x.extra);
     // the last piece's transfers are never read: it sends what its slot holds
-    uint32_t* cmap_out = last ? nullptr : tab_c + R * wc;
+    uint32_t* cmap_out = last ? nullptr : b.tab_c + R * wc;
     int rc;
     if (prot) {
-        uint32_t* transfers = reinterpret_cast<uint32_t*>(x.extra + cheetah_piece_extra_bytes(h));   // [world][DECODE_PROT_TRANSFER_WORDS]
-        rc = density_b200_cheetah_decode_shard_prot_transfer(s, d_in, n, d_out, cap, first, last, transfers + R * DECODE_PROT_TRANSFER_WORDS, st);
+        rc = cl_piece_prot_transfer(s, lion, d_in, n, d_out, cap, first, last, b.transfers + R * DECODE_PROT_TRANSFER_WORDS, st);
         if (rc != DENSITY_B200_OK) return rc;
-        if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
-        rc = density_b200_cheetah_decode_shard_prot_phase1(s, transfers, (int)W, (int)R, cmap_out, st);
+        if (!x.gather(b.transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        rc = cl_piece_prot_phase1(s, b.transfers, (int)W, (int)R, cmap_out, st);
     } else if (cand >= 0) {
-        rc = density_b200_cheetah_decode_shard_prot_enter(s, d_in, n, d_out, cap, first, last, (uint32_t)cand, cmap_out, st);
+        rc = density_b200_cheetah_decode_shard_prot_enter(h->cdec, d_in, n, d_out, cap, first, last, (uint32_t)cand, cmap_out, st);
     } else {
-        rc = density_b200_cheetah_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, cmap_out, st);
+        rc = cl_piece_phase1(s, lion, d_in, n, d_out, cap, first, last, cmap_out, st);
     }
     if (rc != DENSITY_B200_OK) return rc;
-    if (!x.gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
-    cudaError_t e = first ? cudaSuccess : chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
-    if ((rc = step_result(e, launches, "sharded cheetah decode: chunk-map fold")) != DENSITY_B200_OK) return rc;
-    if ((rc = density_b200_cheetah_decode_shard_phase2(s, first ? nullptr : carry_c, st)) != DENSITY_B200_OK) return rc;
-    for (int k = 0; k < g_chee_dec_rounds; ++k) {
-        rc = density_b200_cheetah_decode_shard_round_walk(s, last ? nullptr : tab_p + R * wp, rwords + 4 * R, st);
-        if (rc != DENSITY_B200_OK) return rc;
-        if (!x.gather(tab_p, wp, "ncclAllGather(prediction transfers)") || !x.gather(rwords, 4, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
-        launches = 0;
-        if (!first) e = cl_rank_fold(ALG_CHEETAH, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
-        if ((rc = step_result(e, launches, "sharded cheetah decode: prediction fold")) != DENSITY_B200_OK) return rc;
-        rc = density_b200_cheetah_decode_shard_round_fold(s, first ? nullptr : carry_p, rwords, (int)W, (int)R, st);
-        if (rc != DENSITY_B200_OK) return rc;
+    if (!x.gather(b.tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
+    // the first piece has nothing to fold; Lion's relay starts from the stream-start state there
+    uint64_t launches = 0;
+    cudaError_t e = !first ? chee_cmap_rank_fold(b.tab_c, (uint32_t)R, b.carry_c, st, &launches) : lion ? lion_state_init(b.state, st) : cudaSuccess;
+    if ((rc = step_result(e, launches, "sharded cl decode: chunk-map fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = cl_piece_phase2(s, first ? nullptr : b.carry_c, st)) != DENSITY_B200_OK) return rc;
+    if (!lion) {
+        for (int k = 0; k < g_chee_dec_rounds; ++k) {
+            rc = density_b200_cheetah_decode_shard_round_walk(h->cdec, last ? nullptr : b.tab_p + R * wp, b.rwords + 4 * R, st);
+            if (rc != DENSITY_B200_OK) return rc;
+            if (!x.gather(b.tab_p, wp, "ncclAllGather(prediction transfers)") || !x.gather(b.rwords, 4, "ncclAllGather(round words)"))
+                return DENSITY_B200_ECUDA;
+            launches = 0;
+            e = first ? cudaSuccess : cl_rank_fold(ALG_CHEETAH, DENSITY_B200_CL_TABLE_P, b.tab_p, (uint32_t)R, b.carry_p, st, &launches);
+            if ((rc = step_result(e, launches, "sharded cheetah decode: prediction fold")) != DENSITY_B200_OK) return rc;
+            rc = density_b200_cheetah_decode_shard_round_fold(h->cdec, first ? nullptr : b.carry_p, b.rwords, (int)W, (int)R, st);
+            if (rc != DENSITY_B200_OK) return rc;
+        }
+    } else {
+        // the receive and the send are separate groups, since one group would send the state from before the walk
+        if (!first) {
+            if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
+            const bool ok = nccl_check(x.a->Recv(b.state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R - 1, h->comm, st), "ncclRecv(walk state)");
+            if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
+        }
+        if ((rc = density_b200_lion_decode_shard_walk(ls, b.state, st)) != DENSITY_B200_OK) return rc;
+        if (!last) {
+            if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
+            const bool ok = nccl_check(x.a->Send(b.state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R + 1, h->comm, st), "ncclSend(walk state)");
+            if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
+        }
     }
-    if ((rc = density_b200_cheetah_decode_shard_phase3(s, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
+    rc = lion ? density_b200_lion_decode_shard_phase3(ls, d_out_size, x.my_words(), st)
+              : density_b200_cheetah_decode_shard_phase3(h->cdec, d_out_size, x.my_words(), st);
+    if (rc != DENSITY_B200_OK) return rc;
     return x.verdict(d_flags, d_total_size, d_out_offset);
 }
 
-// The pieces of a sharded Cheetah encode: rank 0 holds the stream start, the last rank its end.
+// The pieces of a sharded Cheetah or Lion encode, rank 0 holding the stream start and the last rank its end. prot: the inverse of
+// density_b200_encode_sharded_cl_protected for any stream, whose pieces exchange their protection transfers first.
+static int decode_sharded_cl(density_b200_sharded* h, int alg, bool prot, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
+                             uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
+    g_last_error.clear();
+    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
+    Exchange x;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cl_piece_bufs(alg, (size_t)h->world, prot, 0).bytes)) != DENSITY_B200_OK) return rc;
+    return decode_sharded_cl_piece(x, alg, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
+                                   prot);
+}
 int density_b200_decode_sharded_cheetah(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                         uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
-    Exchange x;
-    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h))) != DENSITY_B200_OK) return rc;
-    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
-                                        false);
+    return decode_sharded_cl(h, ALG_CHEETAH, false, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v);
 }
-
-// The inverse of density_b200_encode_sharded_cl_protected (Cheetah) for any stream: the pieces' protection transfers are exchanged first,
-// then everything runs as density_b200_decode_sharded_cheetah.
 int density_b200_decode_sharded_cheetah_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                                   uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
-    Exchange x;
-    if (rc != DENSITY_B200_OK ||
-        (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h) + (size_t)h->world * DECODE_PROT_TRANSFER_WORDS * sizeof(uint32_t))) != DENSITY_B200_OK)
-        return rc;
-    return decode_sharded_cheetah_piece(x, d_in, n, h->rank == 0, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr,
-                                        true);
+    return decode_sharded_cl(h, ALG_CHEETAH, true, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v);
 }
-
-// Sharded Lion decode of this rank's piece d_in[0 .. n) over the handle's communicator: [prot: prot_transfer -> ncclAllGather(transfers) ->
-// prot_phase1, else phase 1] -> chunk-map transfers -> fold -> phase 2 -> the relay of the walk's state (receive from rank - 1, walk, send
-// to rank + 1; the receive and the send are separate groups, since one group would send the state from before the walk) -> phase 3 -> seam
-// words -> verdict. Every rank issues the same collectives whatever its piece holds: an empty piece forwards the state unchanged, a
-// refused one keeps exchanging until the verdict. Rank 0 holds the stream start, the last rank its end.
-static int decode_sharded_lion_piece(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                                     uint32_t* d_flags, uint64_t* d_total_size, void* stream_v, bool prot) {
-    if (reinterpret_cast<uintptr_t>(d_out_size) & 7) { set_error("d_out_size must be 8-byte aligned"); return DENSITY_B200_EARG; }
-    const size_t W = (size_t)h->world, R = (size_t)h->rank;
-    const size_t wc = density_b200_cheetah_cmap_words();
-    Exchange x;
-    int rc = x.open(h, stream_v, ((W + 1) * wc + DENSITY_B200_LION_STATE_WORDS + (prot ? W * DECODE_PROT_TRANSFER_WORDS : 0) + 64) * sizeof(uint32_t));
-    if (rc != DENSITY_B200_OK) return rc;
-    cudaStream_t st = x.st;
-    density_b200_lion_decode_shard* s = prot ? h->lpdec : h->ldec;
-    const bool first = R == 0, last = R == W - 1;
-    uint32_t* tab_c = reinterpret_cast<uint32_t*>(x.extra);              // [world][wc]
-    uint32_t* carry_c = tab_c + W * wc;
-    uint32_t* state = carry_c + wc;                                       // the walk's state, DENSITY_B200_LION_STATE_WORDS
-    uint32_t* transfers = state + DENSITY_B200_LION_STATE_WORDS;          // [world][DECODE_PROT_TRANSFER_WORDS] (prot)
-    uint32_t* cmap_out = last ? nullptr : tab_c + R * wc;                 // the last piece's transfer is never read
-    if (prot) {
-        rc = density_b200_lion_decode_shard_prot_transfer(s, d_in, n, d_out, cap, first, last, transfers + R * DECODE_PROT_TRANSFER_WORDS, st);
-        if (rc != DENSITY_B200_OK) return rc;
-        if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
-        rc = density_b200_lion_decode_shard_prot_phase1(s, transfers, (int)W, (int)R, cmap_out, st);
-    } else {
-        rc = density_b200_lion_decode_shard_phase1(s, d_in, n, d_out, cap, first, last, cmap_out, st);
-    }
-    if (rc != DENSITY_B200_OK) return rc;
-    if (!x.gather(tab_c, wc, "ncclAllGather(chunk-map transfers)")) return DENSITY_B200_ECUDA;
-    uint64_t launches = 0;
-    const cudaError_t e = first ? lion_state_init(state, st) : chee_cmap_rank_fold(tab_c, (uint32_t)R, carry_c, st, &launches);
-    if ((rc = step_result(e, launches, "sharded lion decode: chunk-map fold")) != DENSITY_B200_OK) return rc;
-    if ((rc = density_b200_lion_decode_shard_phase2(s, first ? nullptr : carry_c, st)) != DENSITY_B200_OK) return rc;
-    if (!first) {
-        if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
-        const bool ok = nccl_check(x.a->Recv(state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R - 1, h->comm, st), "ncclRecv(walk state)");
-        if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
-    }
-    if ((rc = density_b200_lion_decode_shard_walk(s, state, st)) != DENSITY_B200_OK) return rc;
-    if (!last) {
-        if (!nccl_check(x.a->GroupStart(), "ncclGroupStart")) return DENSITY_B200_ECUDA;
-        const bool ok = nccl_check(x.a->Send(state, DENSITY_B200_LION_STATE_WORDS, NCCL_UINT32, (int)R + 1, h->comm, st), "ncclSend(walk state)");
-        if (!nccl_check(x.a->GroupEnd(), "ncclGroupEnd") || !ok) return DENSITY_B200_ECUDA;
-    }
-    if ((rc = density_b200_lion_decode_shard_phase3(s, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
-    return x.verdict(d_flags, d_total_size, nullptr);
-}
-
-// The pieces of a sharded Lion encode: rank 0 holds the stream start, the last rank its end.
 int density_b200_decode_sharded_lion(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                      uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    const int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
-    if (rc != DENSITY_B200_OK) return rc;
-    return decode_sharded_lion_piece(h, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v, false);
+    return decode_sharded_cl(h, ALG_LION, false, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v);
 }
-
-// The inverse of density_b200_encode_sharded_cl_protected (Lion) for any stream: the pieces' protection transfers are exchanged first,
-// then everything runs as density_b200_decode_sharded_lion.
 int density_b200_decode_sharded_lion_protected(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, void* stream_v) {
-    g_last_error.clear();
-    const int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
-    if (rc != DENSITY_B200_OK) return rc;
-    return decode_sharded_lion_piece(h, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v, true);
+    return decode_sharded_cl(h, ALG_LION, true, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v);
 }
 
 int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_map) & 7)) { set_error("d_in must be 2-byte, d_map 8-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    const int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase1_done = false;     // the scratch is phase 1's
     cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
@@ -2278,8 +2227,10 @@ int density_b200_cheetah_locate_piece(const uint64_t* h_maps, int world, int ran
 int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset,
                                        uint64_t* d_map, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_map) & 7)) { set_error("d_in must be 2-byte, d_map 8-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    const int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase = 0;               // the scratch is phase 1's
     cudaError_t e = s->ws.ensure(chee_locate_workspace_bytes(n_range, n_halo, range_offset), st);
@@ -2320,10 +2271,10 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
     g_last_error.clear();
     int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
     Exchange x;
-    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h))) != DENSITY_B200_OK) return rc;
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cl_piece_bufs(ALG_CHEETAH, (size_t)h->world, false, 0).bytes)) != DENSITY_B200_OK) return rc;
     // sized for the locate scratch and for the phases on any piece of range + halo, so that phase 1 does not reallocate
     const size_t locate_bytes = chee_locate_workspace_bytes(n_range, n_halo, range_offset);
-    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms);
+    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms, false);
     const cudaError_t e = h->cdec->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, x.st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     constexpr size_t MW = DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS;    // the map slots hold DENSITY_B200_LOCATE_MAP_WORDS >= MW words per rank
@@ -2333,15 +2284,17 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
     uint64_t piece[5];
     rc = density_b200_cheetah_locate_piece(h->h_maps, h->world, h->rank, piece);
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
-    return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap, d_out_size,
-                                        d_flags, d_total_size, d_out_offset, false);
+    return decode_sharded_cl_piece(x, ALG_CHEETAH, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[4] != 0, piece[3] != 0, d_out, cap,
+                                   d_out_size, d_flags, d_total_size, d_out_offset, false);
 }
 
 // ---- sharded decode of a stream without known cuts, copy-mode blocks included (DESIGN.md section 5) ----------------------------------
 int density_b200_decode_prot_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_map)) { set_error("d_in must be 2-byte, d_map 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_map});
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase1_done = false; s->prot_stage = 0;     // the scratch is phase 1's
     cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
@@ -2353,8 +2306,10 @@ int density_b200_decode_prot_locate(density_b200_decode_shard* s, const uint8_t*
 int density_b200_cheetah_decode_prot_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map,
                                             void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n_range + n_halo) || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_map)) { set_error("d_in must be 2-byte, d_map 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_map});
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->phase = 0; s->transfer_done = false;         // the scratch is phase 1's
     cudaError_t e = s->ws.ensure(chee_prot_locate_workspace_bytes(n_range + n_halo), st);
@@ -2452,22 +2407,21 @@ int density_b200_decode_sharded_cheetah_stream_protected(density_b200_sharded* h
     int rc = decode_sharded_args(h, d_in, n_range + n_halo, d_out, cap, d_out_size, d_flags);
     constexpr size_t MW = DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS;
     Exchange x;
-    if (rc != DENSITY_B200_OK ||
-        (rc = x.open(h, stream_v, cheetah_piece_extra_bytes(h) + (size_t)h->world * MW * sizeof(uint32_t) + 64)) != DENSITY_B200_OK)
+    if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, cl_piece_bufs(ALG_CHEETAH, (size_t)h->world, false, MW).bytes)) != DENSITY_B200_OK)
         return rc;
     // sized for the locate scratch and for the phases on any piece of range + halo, so that phase 1 does not reallocate
     const size_t locate_bytes = chee_prot_locate_workspace_bytes(n_range + n_halo);
-    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms);
+    const size_t piece_bytes = chee_shard_workspace_bytes(n_range + n_halo, cap, h->num_sms, false);
     const cudaError_t e = h->cdec->ws.ensure(locate_bytes > piece_bytes ? locate_bytes : piece_bytes, x.st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint32_t* maps = reinterpret_cast<uint32_t*>(x.extra + cheetah_piece_extra_bytes(h));   // [world][MW], then the composition's 8 words
+    uint32_t* maps = cl_piece_bufs(ALG_CHEETAH, (size_t)h->world, false, MW, x.extra).maps;
     uint64_t piece[6];
     if ((rc = density_b200_cheetah_decode_prot_locate(h->cdec, d_in, n_range, n_halo, maps + (size_t)h->rank * MW, x.st)) != DENSITY_B200_OK ||
         (rc = prot_locate_exchange(x, ALG_CHEETAH, maps, d_flags, d_out_size, d_out_offset, d_total_size, piece)) != DENSITY_B200_OK)
         return rc;
     if (piece[5]) return DENSITY_B200_OK;    // refused on every rank alike: none enters the collectives below
-    return decode_sharded_cheetah_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[3] != 0, piece[2] != 0, d_out, cap, d_out_size,
-                                        d_flags, d_total_size, d_out_offset, false, (int64_t)piece[4]);
+    return decode_sharded_cl_piece(x, ALG_CHEETAH, d_in + piece[0], (size_t)(piece[1] - piece[0]), piece[3] != 0, piece[2] != 0, d_out, cap,
+                                   d_out_size, d_flags, d_total_size, d_out_offset, false, (int64_t)piece[4]);
 }
 
 /* stage times of the last density_b200_encode_sharded or density_b200_encode_sharded_cl call (waits for it). Chameleon: out_ms[0] flag

@@ -848,35 +848,48 @@ const void* lion_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int n
 }
 
 // ---- sharded decode: one piece, in phases around the exchanges (include/density_b200.h, DESIGN.md section 5) --------------------------
-static CheeDecPtrs chee_shard_ptrs(const CheeShardArgs& a) { return CheeDecPtrs(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr); }
+// One piece protocol for both run-parallel decoders: a.lion picks the geometry (bounds::CheeT or bounds::LionT) of every step below.
+// Between phase 2 and phase 3 Cheetah runs the prediction rounds (chee_shard_round_walk / _fold), Lion the walk on the state the pieces
+// before it left (lion_shard_walk).
+static CheeDecPtrs chee_shard_ptrs(const CheeShardArgs& a) { return CheeDecPtrs(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr, a.lion); }
 
-size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
+size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms, bool lion) {
     CheeDecLayout L;
-    const size_t off = (cd_layout(n, cap, cd_pick_runs(n, num_sms), &L) + 255) & ~(size_t)255;
-    return off + 256 + scalar_workspace_bytes(ALG_CHEETAH);
+    const size_t off = (cd_layout(n, cap, cd_pick_runs(n, num_sms), &L, lion) + 255) & ~(size_t)255;
+    return off + 256 + scalar_workspace_bytes(lion ? ALG_LION : ALG_CHEETAH);
 }
 
 // Phase 1: boundaries (piece 0 may use copy mode: dec_seq_walk from the fresh automaton), the end of the piece, unpack (literals and
 // copy-mode blocks go straight to d_out), the symbolic chunk-map walk and the piece's chunk-map transfer (d_cmap_out, may be null).
 // d_seed (the protected path, nullptr otherwise): the piece's incoming state; rows_ready: chee_shard_prot_transfer filled the candidate rows.
-cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
-                              bool rows_ready) {
+template <class G>
+static cudaError_t shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
+                                bool rows_ready) {
     const CheeDecPtrs p = chee_shard_ptrs(a);
-    cudaError_t e = bounds::bounds_launch<bounds::CheeT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, rows_ready);
+    cudaError_t e = bounds::bounds_launch<G>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, rows_ready);
     if (e == cudaSuccess) e = cd_clear_tables(p, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
+    if (e == cudaSuccess && a.lion) e = cudaMemsetAsync(p.cs, 0, sizeof(LionStatus), stream);
     if (e != cudaSuccess) return e;
-    cd_piece_end<T><<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
+    cd_piece_end<G><<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off, p.B.maxblocks, p.pst);
     ++*launches;
-    cd_launch_unpack_walk(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
+    cd_launch_unpack_walk<G>(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
     if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
     return cudaGetLastError();
 }
+cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
+                              bool rows_ready) {
+    return a.lion ? shard_phase1<bounds::LionT>(a, d_cmap_out, stream, launches, d_seed, rows_ready)
+                  : shard_phase1<T>(a, d_cmap_out, stream, launches, d_seed, rows_ready);
+}
 
 // Phase 2: the chunk map carried in (d_cmap_carry: concrete, the left fold of the earlier pieces' transfers over cd_cmap_init_k's state;
-// nullptr = the stream start), the reads of carried-in slots, the context init.
+// nullptr = the stream start), the reads of carried-in slots, the context init (Cheetah).
 cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
-    cd_launch_cmap_resolve(chee_shard_ptrs(a), reinterpret_cast<uint32_t*>(a.d_out), d_cmap_carry, stream, launches);
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    uint32_t* out32 = reinterpret_cast<uint32_t*>(a.d_out);
+    if (a.lion) cd_launch_cmap_resolve<bounds::LionT>(p, out32, d_cmap_carry, stream, launches);
+    else cd_launch_cmap_resolve<T>(p, out32, d_cmap_carry, stream, launches);
     return cudaGetLastError();
 }
 
@@ -901,22 +914,51 @@ cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const 
     return cudaGetLastError();
 }
 
-// Phase 3: the verdict of the rounds, the final piece's tail from the folded tables (the tail of a non-final piece is empty), the size
-// and the seam words (d_seed: the protected path's, see cd_seam_words). An empty piece of the protected path has its seam words only.
-cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
-                              const uint32_t* d_seed) {
+// The walk from the relayed state d_state (LION_STATE_WORDS: the 65536 lists, then last_hash): the lists into the tail's table (the first
+// piece starts from the zero table and context 0, lion.rs:67,70), ld_walk, then the table and the context behind the piece back to d_state.
+cudaError_t lion_shard_walk(const CheeShardArgs& a, uint32_t* d_state, cudaStream_t stream, uint64_t* launches) {
+    const CheeDecPtrs p = chee_shard_ptrs(a);
+    const size_t tb = (size_t)5 * PL * sizeof(uint32_t);
+    uint32_t* ctx = d_state + 5 * PL;
+    cudaError_t e = a.first ? cudaMemsetAsync(p.pred_final, 0, tb, stream) : cudaMemcpyAsync(p.pred_final, d_state, tb, cudaMemcpyDeviceToDevice, stream);
+    if (e != cudaSuccess) return e;
+    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, reinterpret_cast<uint32_t*>(a.d_out), p.pred_final, reinterpret_cast<LionStatus*>(p.cs),
+                                  a.first ? nullptr : ctx, ctx);
+    ++*launches;
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_state, p.pred_final, tb, cudaMemcpyDeviceToDevice, stream);
+    return e;
+}
+
+// the stream-start state of the relay: zero lists, context 0
+cudaError_t lion_state_init(uint32_t* d_state, cudaStream_t stream) {
+    return cudaMemsetAsync(d_state, 0, (size_t)LION_STATE_WORDS * sizeof(uint32_t), stream);
+}
+
+// Phase 3: the verdict of the rounds (Lion: of the walk), the final piece's tail from the folded (walked) tables (the tail of a non-final
+// piece is empty), the size and the seam words (d_seed: the protected path's, see cd_seam_words). An empty piece of the protected path has
+// its seam words only.
+template <class G>
+static cudaError_t shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                                const uint32_t* d_seed) {
     if (!a.n) {
-        cd_seam_words<128><<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+        cd_seam_words<G::BS><<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
         ++*launches;
         return cudaGetLastError();
     }
     const CheeDecPtrs p = chee_shard_ptrs(a);
     cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
-    cudaError_t e = scalar_decode_tail(ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
+    cudaError_t e = scalar_decode_tail(a.lion ? ALG_LION : ALG_CHEETAH, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream,
+                                       launches, p.fallback);
     if (e != cudaSuccess) return e;
-    cd_seam_words<128><<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
+    cd_seam_words<G::BS><<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
     ++*launches;
     return cudaGetLastError();
+}
+cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
+                              const uint32_t* d_seed) {
+    return a.lion ? shard_phase3<bounds::LionT>(a, d_out_size, d_seam8, stream, launches, d_seed)
+                  : shard_phase3<T>(a, d_out_size, d_seam8, stream, launches, d_seed);
 }
 
 // The protected path's first step on a piece (DESIGN.md section 5): the candidate rows of the boundary walk (they stay in the workspace
@@ -941,7 +983,7 @@ static cudaError_t shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_trans
     uint32_t* res = nullptr;
     uint4* gres = nullptr;
     if (a.n) {
-        const CheeDecPtrs p(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr, G::BS == 64);
+        const CheeDecPtrs p = chee_shard_ptrs(a);
         res = reinterpret_cast<uint32_t*>(a.ws + p.B.res);
         gres = reinterpret_cast<uint4*>(a.ws + p.B.gres);
         const uint32_t nchunks = (uint32_t)((a.n + G::CH - 1) / G::CH);
@@ -955,7 +997,7 @@ static cudaError_t shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_trans
     return cudaGetLastError();
 }
 cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
-    return shard_prot_transfer<T>(a, d_transfer, stream, launches);
+    return a.lion ? shard_prot_transfer<bounds::LionT>(a, d_transfer, stream, launches) : shard_prot_transfer<T>(a, d_transfer, stream, launches);
 }
 // The incoming state of piece `rank` composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
 cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
@@ -965,7 +1007,7 @@ cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank
     return cudaGetLastError();
 }
 
-// the diagnostic words of the piece's iteration (ClStatus, 8 x u32)
+// the diagnostic words of the piece's iteration (ClStatus, 8 x u32; Lion: the walk's LionStatus, a ClStatus prefix, then the 4 u64 counts)
 const void* chee_shard_status_ptr(const CheeShardArgs& a) { return chee_shard_ptrs(a).cs; }
 
 cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches) {
@@ -981,88 +1023,6 @@ cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_
     cd_cmap_rank_fold_k<<<PL / 128, 128, 0, stream>>>(d_tables, rank, d_carry); ++*launches; return cudaGetLastError();
 }
 uint32_t chee_shard_max_rounds() { return MAX_ROUNDS; }
-
-// ---- sharded Lion decode: one piece, in phases around the chunk-map exchange and the relay of the walk's state (DESIGN.md section 5) ----
-// Stages 0-2 are the Cheetah piece's on the Lion geometry; the walk continues the state the pieces before it left (one piece after the
-// other), on the tail's table in the workspace.
-static CheeDecPtrs lion_shard_ptrs(const CheeShardArgs& a) { return CheeDecPtrs(a.n, a.cap, a.num_sms, a.ws, a.tables, nullptr, true); }
-
-size_t lion_shard_workspace_bytes(size_t n, size_t cap, int num_sms) {
-    CheeDecLayout L;
-    const size_t off = (cd_layout(n, cap, cd_pick_runs(n, num_sms), &L, true) + 255) & ~(size_t)255;
-    return off + 256 + scalar_workspace_bytes(ALG_LION);
-}
-
-// Phase 1: boundaries, the end of the piece, unpack, the symbolic chunk-map walk and the chunk-map transfer (d_cmap_out, may be null), as
-// chee_shard_phase1 on the Lion geometry.
-cudaError_t lion_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed,
-                              bool rows_ready) {
-    const CheeDecPtrs p = lion_shard_ptrs(a);
-    cudaError_t e = bounds::bounds_launch<bounds::LionT>(a.d_in, a.n, a.cap, a.ws, p.B, stream, launches, d_seed, rows_ready);
-    if (e == cudaSuccess) e = cd_clear_tables(p, stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(p.tail_ws, 0, 256, stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(p.cs, 0, sizeof(LionStatus), stream);
-    if (e != cudaSuccess) return e;
-    cd_piece_end<bounds::LionT><<<1, 32, 0, stream>>>(a.d_in, a.n, a.cap, a.first ? 1 : 0, a.last ? 1 : 0, d_seed ? 1 : 0, p.st, p.blk_off,
-                                                      p.B.maxblocks, p.pst);
-    ++*launches;
-    cd_launch_unpack_walk<bounds::LionT>(p, a.d_in, reinterpret_cast<uint32_t*>(a.d_out), stream, launches);
-    if (d_cmap_out) { cd_cmap_export<<<PL / 256, 256, 0, stream>>>(p.st, p.nruns, p.entC, d_cmap_out); ++*launches; }
-    return cudaGetLastError();
-}
-
-// Phase 2: the chunk map carried in (nullptr = the stream start) and the reads of carried-in slots.
-cudaError_t lion_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches) {
-    cd_launch_cmap_resolve<bounds::LionT>(lion_shard_ptrs(a), reinterpret_cast<uint32_t*>(a.d_out), d_cmap_carry, stream, launches);
-    return cudaGetLastError();
-}
-
-// The walk from the relayed state d_state (LION_STATE_WORDS: the 65536 lists, then last_hash): the lists into the tail's table (the first
-// piece starts from the zero table and context 0, lion.rs:67,70), ld_walk, then the table and the context behind the piece back to d_state.
-cudaError_t lion_shard_walk(const CheeShardArgs& a, uint32_t* d_state, cudaStream_t stream, uint64_t* launches) {
-    const CheeDecPtrs p = lion_shard_ptrs(a);
-    const size_t tb = (size_t)5 * PL * sizeof(uint32_t);
-    uint32_t* ctx = d_state + 5 * PL;
-    cudaError_t e = a.first ? cudaMemsetAsync(p.pred_final, 0, tb, stream) : cudaMemcpyAsync(p.pred_final, d_state, tb, cudaMemcpyDeviceToDevice, stream);
-    if (e != cudaSuccess) return e;
-    ld_walk<<<1, 32, 0, stream>>>(p.st, p.flags, p.K, reinterpret_cast<uint32_t*>(a.d_out), p.pred_final, reinterpret_cast<LionStatus*>(p.cs),
-                                  a.first ? nullptr : ctx, ctx);
-    ++*launches;
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_state, p.pred_final, tb, cudaMemcpyDeviceToDevice, stream);
-    return e;
-}
-
-// the stream-start state of the relay: zero lists, context 0
-cudaError_t lion_state_init(uint32_t* d_state, cudaStream_t stream) {
-    return cudaMemsetAsync(d_state, 0, (size_t)LION_STATE_WORDS * sizeof(uint32_t), stream);
-}
-
-// Phase 3: the verdict of the walk, the final piece's tail from the walked table (the tail of a non-final piece is empty), the size and
-// the seam words (d_seed: the protected path's). An empty piece of the protected path has its seam words only.
-cudaError_t lion_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
-                              const uint32_t* d_seed) {
-    if (!a.n) {
-        cd_seam_words<bounds::LionT::BS><<<1, 1, 0, stream>>>(nullptr, nullptr, nullptr, a.last ? 1 : 0, d_seed, d_out_size, d_seam8);
-        ++*launches;
-        return cudaGetLastError();
-    }
-    const CheeDecPtrs p = lion_shard_ptrs(a);
-    cd_launch_finish(p, p.fallback, d_out_size, stream, launches);
-    cudaError_t e = scalar_decode_tail(ALG_LION, a.d_in, a.n, a.d_out, a.cap, p.tail_ws, p.st, p.cs, d_out_size, stream, launches, p.fallback);
-    if (e != cudaSuccess) return e;
-    cd_seam_words<bounds::LionT::BS><<<1, 1, 0, stream>>>(p.pst, p.fallback, reinterpret_cast<const Status*>(p.tail_ws), a.last ? 1 : 0, d_seed,
-                                                         d_out_size, d_seam8);
-    ++*launches;
-    return cudaGetLastError();
-}
-
-cudaError_t lion_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
-    return shard_prot_transfer<bounds::LionT>(a, d_transfer, stream, launches);
-}
-
-// the walk's status of the piece (LionStatus: a ClStatus prefix, then the 4 u64 counts)
-const void* lion_shard_status_ptr(const CheeShardArgs& a) { return lion_shard_ptrs(a).cs; }
 
 // ---- the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64) ---------------------
 // Any range: the candidate walks over its chunks (the halo visible to its last chunk's walks), their composition per group and over the

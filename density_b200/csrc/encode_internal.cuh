@@ -194,20 +194,17 @@ size_t lion_decode_workspace_bytes(size_t nbytes, size_t cap, int num_sms);
 cudaError_t lion_decode_parallel(const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, uint8_t* tables, uint8_t* tail_ws,
                                  int num_sms, uint64_t* d_out_size, uint32_t* d_fallback, cudaStream_t stream, uint64_t* launches);
 const void* lion_decode_status_ptr(uint8_t* ws, size_t nbytes, size_t cap, int num_sms, const void** walk_status);
-// sharded Cheetah decode: one piece of a longer stream (first: it holds the stream start; last: no stream byte follows it). ws holds
-// chee_shard_workspace_bytes, tables chee_decode_tables_bytes of the piece. Phase 1, phase 2, then any number of rounds (walk, exchange,
-// fold), then phase 3; every call of one piece gets the same arguments. Chunk-map tables: 3 planes {tags, a, b} of 65536 u32.
-struct CheeShardArgs { const uint8_t* d_in; size_t n; uint8_t* d_out; size_t cap; bool first, last; uint8_t* ws; uint8_t* tables; int num_sms; };
-size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
-uint32_t chee_shard_max_rounds();
+// sharded Cheetah and Lion decode: one piece of a longer stream (first: it holds the stream start; last: no stream byte follows it; lion:
+// the Lion geometry). ws holds chee_shard_workspace_bytes, tables chee_decode_tables_bytes of the piece. Phase 1 (or prot transfer, then
+// phase 1 with the seed of chee_shard_prot_enter), phase 2, then Cheetah: any number of rounds (walk, exchange, fold); Lion: the walk; then
+// phase 3. Every call of one piece gets the same arguments. Chunk-map tables: 3 planes {tags, a, b} of 65536 u32.
+struct CheeShardArgs { const uint8_t* d_in; size_t n; uint8_t* d_out; size_t cap; bool first, last, lion; uint8_t* ws; uint8_t* tables; int num_sms; };
+size_t chee_shard_workspace_bytes(size_t n, size_t cap, int num_sms, bool lion);
 // d_seed (may be NULL): the piece's incoming automaton state (chee_shard_prot_enter); rows_ready: chee_shard_prot_transfer on the same
 // workspace filled the candidate rows
 cudaError_t chee_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr,
                               bool rows_ready = false);
 cudaError_t chee_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
-cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
-cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
-                                  uint32_t rank, cudaStream_t stream, uint64_t* launches);
 // (d_seed: the same seed, whose seam words do not refuse incompressible blocks at the cuts; n == 0 is allowed there)
 cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
                               const uint32_t* d_seed = nullptr);
@@ -217,24 +214,20 @@ cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfe
 cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
                                   uint64_t* launches);
 const void* chee_shard_status_ptr(const CheeShardArgs& a);
+// Cheetah: the prediction rounds
+uint32_t chee_shard_max_rounds();
+cudaError_t chee_shard_round_walk(const CheeShardArgs& a, uint32_t round, uint32_t* d_pred_out, uint32_t* d_words, cudaStream_t stream, uint64_t* launches);
+cudaError_t chee_shard_round_fold(const CheeShardArgs& a, uint32_t round, const uint32_t* d_pred_carry, const uint32_t* d_all_words, uint32_t world,
+                                  uint32_t rank, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_identity(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_init(uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_fold(uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 cudaError_t chee_cmap_rank_fold(const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
-// sharded Lion decode: one piece, the arguments of the Cheetah piece (ws: lion_shard_workspace_bytes, tables: chee_decode_tables_bytes(..,
-// true)). Phase 1 (or prot transfer, then phase 1 with the seed of chee_shard_prot_enter), phase 2, the walk, phase 3. The walk's state
-// travels from piece to piece in LION_STATE_WORDS u32: the 65536 five-slot lists (the tail's layout), then last_hash, then padding.
+// Lion: the walk's state travels from piece to piece in LION_STATE_WORDS u32: the 65536 five-slot lists (the tail's layout), then
+// last_hash, then padding.
 constexpr uint32_t LION_STATE_WORDS = 5 * 65536 + 8;
-size_t lion_shard_workspace_bytes(size_t n, size_t cap, int num_sms);
-cudaError_t lion_shard_phase1(const CheeShardArgs& a, uint32_t* d_cmap_out, cudaStream_t stream, uint64_t* launches, const uint32_t* d_seed = nullptr,
-                              bool rows_ready = false);
-cudaError_t lion_shard_phase2(const CheeShardArgs& a, const uint32_t* d_cmap_carry, cudaStream_t stream, uint64_t* launches);
 cudaError_t lion_shard_walk(const CheeShardArgs& a, uint32_t* d_state, cudaStream_t stream, uint64_t* launches);
 cudaError_t lion_state_init(uint32_t* d_state, cudaStream_t stream);
-cudaError_t lion_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches,
-                              const uint32_t* d_seed = nullptr);
-cudaError_t lion_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
-const void* lion_shard_status_ptr(const CheeShardArgs& a);
 // the range map of a piece of a Cheetah stream without known cuts (DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS u64 to d_map); scratch in `ws`,
 // at least chee_locate_workspace_bytes of the same arguments
 size_t chee_locate_workspace_bytes(size_t n_range, size_t n_halo, uint64_t range_offset);

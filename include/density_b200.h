@@ -358,13 +358,20 @@ DENSITY_B200_API int density_b200_encode_sharded_cl_protected(density_b200_shard
                                              uint8_t* d_gather, size_t gather_cap, void* stream);
 
 /*
+ * Sharded decode. Every entry of the phase APIs of a Chameleon, Cheetah or Lion piece below, and every density_b200_decode_sharded*
+ * driver, takes its pointers by one rule: d_in 2-byte aligned; d_out and every table, transfer, carry, word and walk-state buffer
+ * 4-byte aligned; d_out_size 8-byte and d_seam8 4-byte aligned. d_in and d_out may be NULL only when their length is 0, an optional
+ * table only where the entry says so. A misaligned or a missing pointer, or a phase called out of order, returns DENSITY_B200_EARG and
+ * enqueues nothing: there is no in-order fallback on these paths.
+ */
+
+/*
  * Sharded Chameleon decode: the inverse of the sharded encode. Piece r is what shard r of a sharded encode produced (rank r's
  * d_out[0 .. d_out_size)), or equally the slice of a single-call stream at the prefix sums of those sizes. Decoding piece r with the
  * dictionary carried in from pieces < r gives back shard r byte for byte, so the concatenation equals chameleon_decode of the whole
  * stream. Quiet streams only, as for encode: the verdict is non-zero when a piece holds a copy-mode block, a seam joins two
  * incompressible blocks, a non-final piece does not decode to whole 256-byte blocks, or a piece is malformed or its output exceeds
  * `cap`. The decoded pieces are then void and the caller decodes the gathered stream on one device. Nothing is written past `cap`.
- * d_in must be 2-byte and d_out 4-byte aligned (there is no in-order fallback on this path); otherwise DENSITY_B200_EARG.
  */
 typedef struct density_b200_decode_shard density_b200_decode_shard; /* opaque */
 DENSITY_B200_API density_b200_decode_shard* density_b200_decode_shard_create(void);
@@ -428,8 +435,8 @@ DENSITY_B200_API int density_b200_decode_sharded_protected(density_b200_sharded*
  *   - the prediction rounds did not settle within the round budget (density_b200_cheetah_decode_round_budget);
  *   - a piece is malformed, its output exceeds `cap`, or a non-final piece does not decode to whole 128-byte blocks.
  * Only the first piece may use copy mode: it holds the stream start, where every Cheetah stream has copy-mode blocks. Lion streams
- * (density_b200_decode_sharded_lion) and streams without known cuts are not decoded this way (density_b200_decode_sharded_cheetah_stream locates their pieces first). d_in must
- * be 2-byte and d_out 4-byte aligned; nothing is written past `cap`.
+ * (density_b200_decode_sharded_lion) and streams without known cuts are not decoded this way (density_b200_decode_sharded_cheetah_stream locates their pieces first).
+ * Nothing is written past `cap`.
  *
  * Phase API of one piece (any transport; W pieces may run on one GPU): phase 1 -> exchange of the chunk-map transfers -> phase 2 -> rounds
  * (round_walk -> exchange of the prediction transfers and the round words -> round_fold), as many as the round budget -> phase 3 -> seam
@@ -495,7 +502,7 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah(density_b200_sharded*, 
  * words 0 and 1 = 0 and word 2 set when the composition met 0xFFFF or 0xFFFE, the piece is malformed or its output exceeds cap, the
  * rounds did not settle, the tail reported an error, or a non-final piece does not decode to whole 128-byte blocks. prot_transfer ->
  * prot_phase1 -> phase 2 -> rounds -> phase 3 in this order per piece (a quiet phase 1 in between closes the protected sequence);
- * otherwise DENSITY_B200_EARG. d_in must be 2-byte, d_out and the transfers 4-byte aligned. Nothing is written past cap.
+ * otherwise DENSITY_B200_EARG. Nothing is written past cap.
  */
 DENSITY_B200_API int density_b200_cheetah_decode_shard_prot_transfer(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n,
                                                     uint8_t* d_out, size_t cap, int is_first, int is_last, uint32_t* d_transfer_out,
@@ -517,13 +524,11 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah_protected(density_b200_
  * shard byte for byte whenever the verdict is 0. The quiet path refuses what Cheetah's refuses (copy mode or two consecutive
  * incompressible blocks in a later piece, a cut inside a copy run or with a penalty pending, incompressible blocks on both sides of a cut,
  * a non-final piece whose blocks do not end at its last byte); the protected path accepts all of these, with the transfers of
- * density_b200_cheetah_decode_shard_prot_transfer. d_in must be 2-byte, d_out and the tables 4-byte, d_out_size 8-byte aligned; nothing
- * is written past `cap`.
+ * density_b200_cheetah_decode_shard_prot_transfer. Nothing is written past `cap`.
  *
  * Phase API of one piece (any transport; W pieces may run on one GPU), in this order per piece: phase 1 (or prot_transfer -> exchange
  * of the transfers -> prot_phase1) -> exchange of the chunk-map transfers -> phase 2 -> walk -> phase 3 -> seam words -> verdict (the
- * rule of density_b200_decode_shard_phase2's words). A call out of order, a misaligned or a null pointer returns DENSITY_B200_EARG and
- * enqueues nothing.
+ * rule of density_b200_decode_shard_phase2's words).
  *   chunk map     the format of density_b200_cheetah_cmap_words, folded with density_b200_cheetah_cmap_init / _fold
  *   walk state    DENSITY_B200_LION_STATE_WORDS u32: the 65536 prediction lists (5 u32 each, context-major), then last_hash, then
  *                 padding. The state in front of the first piece is density_b200_lion_state_init's.

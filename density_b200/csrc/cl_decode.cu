@@ -403,15 +403,22 @@ __global__ void __launch_bounds__(32) ld_walk(const DecStatus* __restrict__ st, 
     Warp w{(int)(threadIdx.x & 31)};
     const uint32_t lane = threadIdx.x & 31;
     const uint64_t ns = cd_steps<bounds::LionT>(st);
+    // quads of the main loop: with an odd block count the last row has one block, and lanes 16-31 of it would read past the main loop's
+    // output (past cap when the tail is shorter than a block); they are inactive, so they load 0. K holds whole rows (cd_unpack writes
+    // all 32 lanes), so its guard only keeps the two loads alike.
+    const uint64_t nq = st->main_blocks * 16;
     const FlatTable tab{T};
     WalkCounts cnt{0, 0, 0, 0};
     uint32_t carry = ctx_in ? *ctx_in : 0u;                // lion.rs:67
     uint4 fl_n = make_uint4(0, 0, 0, 0); uint32_t k_n = 0, v_n = 0;
-    if (ns) { fl_n = flags[0]; k_n = K[lane]; v_n = out[lane]; }
+    if (ns) { fl_n = flags[0]; if (lane < nq) { k_n = K[lane]; v_n = out[lane]; } }
     for (uint64_t s = 0; s < ns; ++s) {
         const uint4 fl = fl_n;
         LV<uint32_t> kh{k_n}, v{v_n};
-        if (s + 1 < ns) { fl_n = flags[s + 1]; k_n = K[(s + 1) * 32 + lane]; v_n = out[(s + 1) * 32 + lane]; }
+        if (s + 1 < ns) {
+            const uint64_t i = (s + 1) * 32 + lane;
+            fl_n = flags[s + 1]; k_n = i < nq ? K[i] : 0u; v_n = i < nq ? out[i] : 0u;
+        }
         if (s + LW_PREFETCH < ns) {
             const uint64_t f = s + LW_PREFETCH;
             if (lane == 0) asm volatile("prefetch.global.L2 [%0];" :: "l"(flags + f));

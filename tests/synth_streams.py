@@ -24,13 +24,15 @@ import planted
 import protection as P
 from planted import FP0_HASHES, quad_of, twin
 
-ALGS = ("chameleon", "cheetah")
-BS = {"chameleon": 256, "cheetah": 128}
-SIG = 8
-QPB = {"chameleon": 64, "cheetah": 32}              # quads per block
-FB = {"chameleon": 1, "cheetah": 2}                 # flag bits
+ALGS = ("chameleon", "cheetah", "lion")
+BS = {"chameleon": 256, "cheetah": 128, "lion": 64}
+SIG = {"chameleon": 8, "cheetah": 8, "lion": 6}     # signature bytes (lion.rs:325)
+QPB = {"chameleon": 64, "cheetah": 32, "lion": 16}  # quads per block
+FB = {"chameleon": 1, "cheetah": 2, "lion": 3}      # flag bits
 PLAIN, MAP, MAP_A, MAP_B, PRED = 0, 1, 1, 2, 3      # Chameleon: 0 PLAIN, 1 MAP; Cheetah: 0 PLAIN, 1 MAP_A, 2 MAP_B, 3 PREDICTED
 NBYTES = {0: 4, 1: 2, 2: 2, 3: 0}
+L_PA, L_PB, L_PC, L_PD, L_PE, L_MAP_A, L_MAP_B = 1, 2, 3, 4, 5, 6, 7   # Lion (lion.rs:18-27): 0 PLAIN, 1-5 PREDICTED_A..E, 6 MAP_A, 7 MAP_B
+PAYLOAD = {"chameleon": (4, 2, 2, 0), "cheetah": (4, 2, 2, 0), "lion": (4, 0, 0, 0, 0, 0, 2, 2)}   # payload bytes per flag
 M32 = 0xFFFFFFFF
 TILE_BLOCKS = 64                                    # chameleon_decode.cu: a tile is 4096 quads = 64 blocks
 MIN_BLOCK = {"chameleon": 136, "cheetah": 8}        # decode_bounds.cuh bounds_layout: smallest encoded block
@@ -60,8 +62,18 @@ def cheetah_dec_runs(stream_bytes, main_blocks, num_sms=planted.H100_SMS):
     return cds.cd_runs(stream_bytes, main_blocks, num_sms)
 
 
+def lion_dec_runs(stream_bytes, main_blocks, num_sms=planted.H100_SMS):
+    """First main-loop block of every run of the Lion decoder's chunk-map passes: run r starts at row r * nrows // nruns of the rows of
+    two blocks (cd_pick_runs, run_step_begin on cd_steps<LionT>)"""
+    import cl_decode_seams as cds
+    nruns, nrows = cds.pick_runs(stream_bytes, num_sms), (main_blocks + 1) // 2
+    return [2 * (r * nrows // nruns) for r in range(nruns)]
+
+
 def seam_blocks(alg, stream_bytes, cap, main_blocks, num_sms=planted.H100_SMS):
     """First block of every decoder run after the first."""
+    if alg == "lion":
+        return sorted(set(lion_dec_runs(stream_bytes, main_blocks, num_sms)[1:]))
     if alg == "chameleon":
         return sorted({t0 * TILE_BLOCKS for t0, _ in cham_dec_runs(stream_bytes, cap, main_blocks, num_sms)[1:]})
     return sorted(set(cheetah_dec_runs(stream_bytes, main_blocks, num_sms)[1:]))
@@ -69,17 +81,18 @@ def seam_blocks(alg, stream_bytes, cap, main_blocks, num_sms=planted.H100_SMS):
 
 # ---- the plain in-order decoder -------------------------------------------------------------------------------------------------
 def decode_reference(alg, stream, cap, state=None, prot=None):
-    """codec.rs:82-126 with chameleon.rs / cheetah.rs, quad by quad. Returns the decoded bytes (empty on a malformed stream or when
+    """codec.rs:82-126 with chameleon.rs / cheetah.rs / lion.rs, quad by quad. Returns the decoded bytes (empty on a malformed stream or when
     the output would pass `cap`, as the C ABI maps both to 0). `state` (a dict, optional) is the codec instance's dictionary carried
     in and updated, as `Codec::decode` on a reused instance (codec.rs:16,82). `prot` (penalty, start, previous_incompressible,
     counter): the automaton to start from instead of protection_state.rs:9-16 (to decode the tail behind a known main loop)."""
     s = bytes(stream)
     n, idx = len(s), 0
-    bs, qpb, fb = BS[alg], QPB[alg], FB[alg]
+    bs, qpb, fb, sb = BS[alg], QPB[alg], FB[alg], SIG[alg]
     st = state if state is not None else {}
     cm = st.setdefault("a", [0] * 65536)
-    cb = st.setdefault("b", [0] * 65536) if alg == "cheetah" else None
+    cb = st.setdefault("b", [0] * 65536) if alg != "chameleon" else None
     pred = st.setdefault("pred", [0] * 65536) if alg == "cheetah" else None
+    lists = st.setdefault("lists", {}) if alg == "lion" else None       # context -> [next_a .. next_e] (lion.rs:41-48), absent: zeros
     out = bytearray()
     ps = _Prot(*prot) if prot is not None else _Prot()
 
@@ -102,6 +115,8 @@ def decode_reference(alg, stream, cap, state=None, prot=None):
                 cm[hash16(q)] = q
                 return q
             return cm[rd(2)]
+        if alg == "lion":
+            return lion(flag)
         if flag == PLAIN:
             q = rd(4); h = hash16(q)
             cb[h] = cm[h]; cm[h] = q
@@ -118,9 +133,32 @@ def decode_reference(alg, stream, cap, state=None, prot=None):
         st["last"] = h
         return q
 
+    def lion(flag):
+        """lion.rs:84-186 and :286: the list of the context last_hash, then last_hash = the quad's hash (explicit for MAP_A / MAP_B)"""
+        last = st.get("last", 0)
+        L = lists.get(last, [0] * 5)
+        if flag == PLAIN:
+            q = rd(4); h = hash16(q)
+            cb[h] = cm[h]; cm[h] = q
+            L = [q] + L[:4]                                         # shift_predictions
+        elif flag == L_MAP_A:
+            h = rd(2); q = cm[h]
+            L = [q] + L[:4]
+        elif flag == L_MAP_B:
+            h = rd(2); q = cb[h]
+            cb[h] = cm[h]; cm[h] = q
+            L = [q] + L[:4]
+        else:                                                       # PREDICTED_A..E: slot k to the front
+            k = flag - 1
+            q = L[k]; h = hash16(q)
+            L = [q] + L[:k] + L[k + 1:]
+        lists[last] = L
+        st["last"] = h
+        return q
+
     def block(tail):
         """one encoded block; True when the stream ended inside it (decode_partial_unit)"""
-        sig = rd(SIG)
+        sig = rd(sb)
         unit = 8 if alg == "chameleon" else 4
         for _ in range(qpb * 4 // unit):
             full = not tail or n - idx >= unit
@@ -136,7 +174,7 @@ def decode_reference(alg, stream, cap, state=None, prot=None):
         return False
 
     try:
-        while n - idx >= SIG + bs:
+        while n - idx >= sb + bs:
             mark = idx
             if ps.step_copy():
                 out.extend(s[idx:idx + bs]); idx += bs
@@ -189,20 +227,28 @@ def walk(alg, stream):
     """The main loop of `stream` (codec.rs:88-100): block starts, copy-mode blocks, tail offset and the automaton state behind it, and
     the automaton state in front of every block (penalty, start, previous_incompressible, counter % 16)."""
     s = np.asarray(stream, np.uint8)
-    n, bs, fb = s.size, BS[alg], FB[alg]
+    n, bs, fb, sb = s.size, BS[alg], FB[alg], SIG[alg]
     size_of = {f: NBYTES[f] if alg == "cheetah" else (4 if f == 0 else 2) for f in range(4)}
+    if alg == "lion":                                                # payload bytes of 4 flags (12 signature bits) at once
+        f4 = (np.arange(4096)[:, None] >> (3 * np.arange(4))[None, :]) & 7
+        by12 = np.array(PAYLOAD["lion"])[f4].sum(axis=1).tolist()
+        buf = s.tobytes()
     ps = _Prot()
     starts, copy, before = [], [], []
     idx = 0
-    while n - idx >= SIG + bs:
+    while n - idx >= sb + bs:
         before.append((ps.penalty, ps.start, ps.prev, ps.counter & 15))
         starts.append(idx)
         if ps.step_copy():
             copy.append(True)
             idx += bs
             continue
-        sig = int.from_bytes(s[idx:idx + SIG].tobytes(), "little")
-        sz = SIG + sum(size_of[(sig >> (fb * k)) & ((1 << fb) - 1)] for k in range(QPB[alg]))
+        if alg == "lion":
+            sig = int.from_bytes(buf[idx:idx + sb], "little")
+            sz = sb + by12[sig & 4095] + by12[(sig >> 12) & 4095] + by12[(sig >> 24) & 4095] + by12[sig >> 36]
+        else:
+            sig = int.from_bytes(s[idx:idx + sb].tobytes(), "little")
+            sz = sb + sum(size_of[(sig >> (fb * k)) & ((1 << fb) - 1)] for k in range(QPB[alg]))
         copy.append(False)
         idx += sz
         ps.step_update(sz >= bs)
@@ -251,6 +297,13 @@ class _Gen:
             k = rng.integers(p.get("min_plain", 0), p.get("max_plain", 59) + 1, nb)
             rank = np.argsort(rng.random((nb, q)), axis=1).argsort(axis=1)
             F = np.where(rank < k[:, None], PLAIN, MAP).astype(np.int8)
+        elif alg == "lion":
+            pp = p.get("p_pred", 0.5)
+            u = rng.random((nb, q))
+            plain_share = rng.random(nb)[:, None] * 0.6
+            depth = rng.integers(L_PA, L_PE + 1, (nb, q))
+            F = np.where(u < pp, depth, np.where(rng.random((nb, q)) < plain_share, PLAIN,
+                                                 np.where(rng.random((nb, q)) < 0.5, L_MAP_A, L_MAP_B))).astype(np.int8)
         else:
             pp = p.get("p_pred", 0.5)
             u = rng.random((nb, q))
@@ -261,7 +314,8 @@ class _Gen:
         flat_f, flat_v = F.reshape(-1), V.reshape(-1)
         pl = np.flatnonzero(flat_f == PLAIN)
         flat_v[pl] = self._random_quads(pl.size)
-        mp = np.flatnonzero((flat_f == MAP) | (flat_f == MAP_B)) if alg == "cheetah" else np.flatnonzero(flat_f == MAP)
+        mp = np.flatnonzero((flat_f == MAP) | (flat_f == MAP_B)) if alg == "cheetah" else \
+            np.flatnonzero(flat_f >= L_MAP_A) if alg == "lion" else np.flatnonzero(flat_f == MAP)
         # a MAP names, with probability 0.6, the bucket of one of the last 64 PLAIN quads (in-tile readers of a written bucket), otherwise
         # any bucket random content may use
         k = np.searchsorted(pl, mp) - rng.integers(1, 65, mp.size)
@@ -288,8 +342,8 @@ class _Gen:
         return F, V
 
     def sizes(self, F):
-        nbytes = np.array([NBYTES[0], 2, 2, 0], np.int64)
-        return SIG + nbytes[F.astype(np.int64)].sum(axis=1)
+        nbytes = np.array(PAYLOAD[self.alg], np.int64)
+        return SIG[self.alg] + nbytes[F.astype(np.int64)].sum(axis=1)
 
     def force(self, F, b, inc):
         """make block b incompressible (all PLAIN) or not (all MAP / MAP_A), planted quads kept"""
@@ -298,7 +352,7 @@ class _Gen:
         if inc:
             row[~keep] = PLAIN
         else:
-            row[~keep & (row == PLAIN)] = MAP
+            row[~keep & (row == PLAIN)] = L_MAP_A if self.alg == "lion" else MAP
 
     def layout(self, tail_spec):
         """-> (stream bytes, copy flags per block, block offsets, automaton after the last block)"""
@@ -314,10 +368,12 @@ class _Gen:
                 vl[fresh] = self._random_quads(len(fresh))
             else:
                 idx = [i for i in range(b * q, (b + 1) * q) if i not in self.planted]
-                if alg == "cheetah":
-                    fl[idx] = MAP_A
+                if alg != "chameleon":
+                    fl[idx] = L_MAP_A if alg == "lion" else MAP_A
                 vl[idx] = self.free_h[self.rng.integers(0, self.free_h.size, len(idx))].astype(np.uint32)
         sz = self.sizes(F)
+        if alg == "lion":
+            self._lion_blocks(F, V, sz, tail_spec)
         if self.plan.get("quiet", True):
             inc = sz >= bs
             for b in np.flatnonzero(inc[1:] & inc[:-1]) + 1:          # no two incompressible blocks in a row: no copy mode
@@ -326,7 +382,7 @@ class _Gen:
                     cand = [k for k in range(q) if row[k] == PLAIN and (b * q + k) not in self.planted]
                     while sz[b] >= bs and cand:
                         k = cand.pop()
-                        row[k] = MAP_A
+                        row[k] = L_MAP_A if alg == "lion" else MAP_A
                         V[b, k] = self.free_h[0]
                         sz[b] -= 2
                     inc[b] = sz[b] >= bs
@@ -343,17 +399,17 @@ class _Gen:
         body = np.zeros(int(off[-1]), np.uint8)
         # signatures
         enc = ~copy
-        fb = FB[alg]
+        fb, sb = FB[alg], SIG[alg]
         sig = np.zeros(nb, np.uint64)
         for k in range(q):
             sig |= F[:, k].astype(np.uint64) << np.uint64(fb * k)
         so = off[:-1][enc]
-        for i in range(8):
+        for i in range(sb):
             body[so + i] = ((sig[enc] >> np.uint64(8 * i)) & np.uint64(0xFF)).astype(np.uint8)
         # payloads
-        nbytes = np.array([4, 2, 2, 0], np.int64)[F.astype(np.int64)]
+        nbytes = np.array(PAYLOAD[alg], np.int64)[F.astype(np.int64)]
         nbytes[copy] = 0
-        qoff = off[:-1, None] + SIG + np.cumsum(nbytes, axis=1) - nbytes
+        qoff = off[:-1, None] + sb + np.cumsum(nbytes, axis=1) - nbytes
         for width in (4, 2):
             m = nbytes == width
             o, val = qoff[m], V[m].astype(np.uint64)
@@ -365,8 +421,72 @@ class _Gen:
             raw = self.rng.integers(0, 256, (cb.size, bs), dtype=np.uint8)
             body[(off[cb][:, None] + np.arange(bs)).reshape(-1)] = raw.reshape(-1)
         self.F_final, self.V_final, self.copy = F, V, copy
-        tail, tcls = self._tail(tail_spec, ps)
+        tail, tcls = self._tail_lion(tail_spec, ps) if alg == "lion" else self._tail(tail_spec, ps)
         return np.concatenate([body, tail]), copy, off, tcls
+
+    def _lion_blocks(self, F, V, sz, tail_spec):
+        """Lion: no block outside forced_inc is incompressible, so copy mode sits only where the plan forces it and plantings cannot move
+        it; the last block is long enough that, with a tail of 6 .. 69 bytes behind it, it stays in the main loop (codec.rs:88), so the
+        last main-loop quad is the last generated one"""
+        q, nb = self.q, self.nb
+        for b in np.flatnonzero(sz >= BS["lion"]):
+            if b in self.forced_inc:
+                continue
+            for k in range(q):
+                if sz[b] < BS["lion"]:
+                    break
+                if F[b, k] == PLAIN and (b * q + k) not in self.planted:
+                    F[b, k] = L_MAP_A; V[b, k] = self.free_h[0]; sz[b] -= 2
+        L = tail_spec[0]
+        b = nb - 1
+        if SIG["lion"] <= L < SIG["lion"] + BS["lion"] and b not in self.forced_inc:
+            for k in range(q):
+                if sz[b] >= SIG["lion"] + BS["lion"] - L:
+                    break
+                if F[b, k] != PLAIN and (b * q + k) not in self.planted:
+                    sz[b] += 4 - PAYLOAD["lion"][F[b, k]]
+                    F[b, k] = PLAIN; V[b, k] = self._random_quads(1)[0]
+
+    def _tail_lion(self, spec, ps):
+        """_tail for Lion: one block of 16 quads whose first quad is PREDICTED_A where it fits (it reads the list of the main loop's last
+        context), then
+        PLAIN, MAP_A / MAP_B and PREDICTED_A..E quads in random order, and the end asked for"""
+        L, end = spec
+        rng, q, sb = self.rng, self.q, SIG["lion"]
+        if L == 0:
+            return np.zeros(0, np.uint8), "tail_empty"
+        if ps.penalty > 0:
+            return rng.integers(0, 256, L, dtype=np.uint8), "tail_copy_pending"
+        if L < sb:
+            return rng.integers(0, 256, L, dtype=np.uint8), "tail_short_signature"
+        r_end = {"clean": 0, "plain_end": 0, "raw1": 1, "raw2": 2, "raw3": 3, "map0": 0, "map1": 1}[end]
+        term = {"clean": None, "plain_end": PLAIN, "raw1": PLAIN, "raw2": PLAIN, "raw3": PLAIN, "map0": L_MAP_A, "map1": L_MAP_B}[end]
+        D = L - sb - r_end
+        slots = q if term is None else q - 1
+        lead = D // 2 - (slots - 1) <= D // 4                         # room for the leading PREDICTED_A (not in the longest tails)
+        slots -= lead
+        lo, hi = max(0, D // 2 - slots), D // 4
+        if D % 2 or lo > hi:
+            raise ValueError(f"tail {L} {end} does not fit one block")
+        p = int(rng.integers(lo, hi + 1))
+        m = D // 2 - 2 * p
+        npred = slots - p - m if term is None else int(rng.integers(0, slots - p - m + 1))
+        body = [PLAIN] * p + [int(f) for f in rng.integers(L_MAP_A, L_MAP_B + 1, m)] + [int(f) for f in rng.integers(L_PA, L_PE + 1, npred)]
+        rng.shuffle(body)
+        flags = [L_PA] * lead + body
+        if term is not None:
+            flags.append(term)
+            flags += [int(f) for f in rng.integers(0, 8, q - len(flags))]
+        sig = sum(f << (3 * k) for k, f in enumerate(flags))
+        out = bytearray(sig.to_bytes(sb, "little"))
+        for f in body:
+            if f == PLAIN:
+                out += int(self._random_quads(1)[0]).to_bytes(4, "little")
+            elif f >= L_MAP_A:
+                out += int(rng.integers(0, 65536)).to_bytes(2, "little")
+        out += rng.integers(0, 256, r_end, dtype=np.uint8).tobytes()
+        assert len(out) == L, (L, end, len(out))
+        return np.frombuffer(bytes(out), np.uint8), "tail_" + end
 
     def _tail(self, spec, ps):
         """spec = (length, end): the bytes after the main loop. end: "clean" (the last quad's payload ends the stream), "plain_end" (a
@@ -378,9 +498,9 @@ class _Gen:
             return np.zeros(0, np.uint8), "tail_empty"
         if ps.penalty > 0:
             return rng.integers(0, 256, L, dtype=np.uint8), "tail_copy_pending"
-        if L < SIG:
+        if L < SIG[alg]:
             return rng.integers(0, 256, L, dtype=np.uint8), "tail_short_signature"
-        D = L - SIG
+        D = L - SIG[alg]
         r_end = {"clean": 0, "plain_end": 0, "raw1": 1, "raw2": 2, "raw3": 3, "map0": 0, "map1": 1}[end]
         term = {"clean": None, "plain_end": PLAIN, "raw1": PLAIN, "raw2": PLAIN, "raw3": PLAIN, "map0": MAP_A, "map1": MAP_A}[end]
         D -= r_end
@@ -414,7 +534,7 @@ class _Gen:
         if alg == "chameleon" and term is not None:
             flags = [MAP if f == MAP_A else f for f in flags]
         sig = sum(int(f) << (FB[alg] * k) for k, f in enumerate(flags))
-        out = bytearray(sig.to_bytes(SIG, "little"))
+        out = bytearray(sig.to_bytes(SIG[alg], "little"))
         used = 0
         for f in flags:
             if used == D:
@@ -543,6 +663,317 @@ class _Planter:
             g.note("pred_chain_through_context0", qi, None)
 
 
+# ---- Lion plantings -----------------------------------------------------------------------------------------------------------------
+LION_CLASSES = ("map_unwritten_ctx", "mapb_written_once", "mapb_twice", "pred_unwritten_depth_k", "pred_short_list", "pred_duplicates",
+                "six_pushes_then_pred", "self_span_after_depth_k", "pred_chain_context0")
+LION_PLACES = ("lane_0", "lane_15", "lane_16", "lane_31", "copy_row_lane_16", "after_copy_row_lane_0", "run_first", "run_last",
+               "piece_first", "piece_last", "after_copy")
+
+
+def lion_class(name):
+    """the class a noted Lion quad belongs to (its variant suffix dropped)"""
+    return next((c for c in LION_CLASSES if name.startswith(c)), name)
+
+
+def _lion_sim(seq, st):
+    """The values of a planted Lion sequence [(flag, payload)]: every bucket and context it names is fresh (never touched by random
+    content), so lion.rs decodes it from empty state. The context in front of the sequence, and context 0 (random content reads and pushes
+    it), are unknown: a predicted read there is None. st ({"cm": {h: [a, b]}, "lists": {ctx: list}}) carries state between sequences."""
+    cm, lists = st.setdefault("cm", {}), st.setdefault("lists", {})
+    ctx, out = None, []
+    for flag, pay in seq:
+        L = lists.get(ctx, [0] * 5) if ctx else None
+        if flag == PLAIN:
+            q = pay; h = hash16(q)
+            a, _ = cm.get(h, (0, 0)); cm[h] = (q, a)
+        elif flag == L_MAP_A:
+            h = pay; q = cm.get(h, (0, 0))[0]
+        elif flag == L_MAP_B:
+            h = pay; a, b = cm.get(h, (0, 0)); q = b; cm[h] = (b, a)
+        else:
+            k = flag - 1
+            if L is None:
+                out.append(None); ctx = None
+                continue
+            q = L[k]; h = hash16(q)
+            lists[ctx] = [q] + L[:k] + L[k + 1:]
+            out.append(q); ctx = h
+            continue
+        if L is not None:
+            lists[ctx] = [q] + L[:4]
+        out.append(q); ctx = h
+    return out
+
+
+class _LionPlanter:
+    """The Lion classes as sealed sequences: a MAP_A at a fresh bucket in front (its value 0 goes to the random context before it) and one
+    behind (the random quad after the sequence pushes into a fresh context), so random content never reads or writes the lists and chunk
+    map slots a sequence uses, and _lion_sim gives every value. A sequence runs over consecutive encoded quads: copy-mode blocks between
+    them leave last_hash as it is (codec.rs:89-92)."""
+
+    def __init__(self, g, runs_q, cuts_q, copy):
+        self.g, self.runs_q, self.cuts_q, self.copy = g, runs_q, cuts_q, copy
+        self.turn = collections.Counter()                             # per class: plantings placed (cycles its variants)
+        self.miss = collections.Counter()                             # per class: plantings that did not fit (moves on to other variants)
+
+    def free(self, qs):
+        """in the main loop, not planted, not copy mode"""
+        g = self.g
+        return all(0 <= x < g.nb * g.q and x not in g.planted and not self.copy[x // g.q] for x in qs)
+
+    def keeps_forced(self, pos, flags):
+        """the blocks forced compressible stay compressible (at most 10 PLAIN quads planted in one), the blocks forced incompressible stay
+        incompressible (the planted quads carry at most 6 payload bytes less than PLAIN quads: 70 - 6 = 64 bytes)"""
+        g, q = self.g, self.g.q
+        new = collections.defaultdict(list)
+        for x, f in zip(pos, flags):
+            if (x // q) in g.forced_inc:
+                new[x // q].append(f)
+        for b, fs in new.items():
+            fs = fs + [g.planted[b * q + k][0] for k in range(q) if (b * q + k) in g.planted]
+            if g.forced_inc[b] and sum(4 - PAYLOAD["lion"][f] for f in fs) > 6:
+                return False
+            if not g.forced_inc[b] and sum(f == PLAIN for f in fs) > 10:
+                return False
+        return True
+
+    def span(self, e, nb, na):
+        """nb encoded quads in front of e, e and na behind it (copy-mode blocks skipped), or None"""
+        g, pos = self.g, []
+        x = e
+        while len(pos) < nb:
+            x -= 1
+            if x < 0:
+                return None
+            if not self.copy[x // g.q]:
+                pos.insert(0, x)
+        pos.append(e)
+        x = e
+        while len(pos) < nb + 1 + na:
+            x += 1
+            if x >= g.nb * g.q:
+                return None
+            if not self.copy[x // g.q]:
+                pos.append(x)
+        return pos
+
+    def seal(self):
+        return (L_MAP_A, self.g.fresh(), None)
+
+    def place(self, seq, k0, e, pre=None):
+        """seq = [(flag, payload, note or None)] with seq[k0] at quad e; pre = (sequence, first quad): an earlier sequence (a chunk-map
+        write) that must end in front of seq. Returns the positions or None when a quad is taken or a forced block would change."""
+        pos = self.span(e, k0, len(seq) - 1 - k0)
+        if pos is None or not self.free(pos) or not self.keeps_forced(pos, [f for f, _, _ in seq]):
+            return None
+        st = {}
+        if pre is not None:
+            pseq, w = pre
+            ppos = self.span(w, 0, len(pseq) - 1) if w >= 0 else None
+            if ppos is None or ppos[-1] >= pos[0] or not self.free(ppos) or \
+                    not self.keeps_forced(ppos + pos, [f for f, _, _ in pseq] + [f for f, _, _ in seq]):
+                return None
+            for x, (f, v, _) in zip(ppos, pseq):
+                self.g.put(x, f, v)
+            _lion_sim([(f, v) for f, v, _ in pseq], st)
+        vals = self.vals = _lion_sim([(f, v) for f, v, _ in seq], st)
+        for x, (f, v, note), val in zip(pos, seq, vals):
+            self.g.put(x, f, 0 if v is None else v)
+            if note:
+                self.g.note(note, x, val)
+        return pos
+
+    def earlier(self, s0, how):
+        """the first quad of a chunk-map write in front of quad s0: in its row, an earlier row, an earlier chunk-map run or an earlier
+        piece; -> (quad, where), an earlier row where the asked one does not exist"""
+        if how == "same_row" and s0 % 32 >= 5:
+            return s0 - s0 % 32, how
+        if how == "earlier_run":
+            prev = [r for r in self.runs_q if r <= s0]
+            if len(prev) >= 2:
+                return prev[-2] + 37, how
+        if how == "earlier_piece":
+            prev = [c for c in self.cuts_q if c <= s0]
+            if prev:
+                return prev[-1] - 97, how                            # clear of the classes planted on the cut's two sides
+        return s0 - 32 - 7, "earlier_row"
+
+    def plant(self, cls, e, at_read=False):
+        """plant `cls` with its key quad at e (at_read: for the MAP classes, the predicted read behind the MAP at e); True when it was
+        placed"""
+        g, t = self.g, self.turn[cls] + self.miss[cls]
+        fresh = g.fresh
+        val = lambda: quad_of(fresh(), g.fp())
+        if cls == "map_unwritten_ctx":                               # the next quad's context is the explicit hash, not hash16(0)
+            h, y = fresh(), val()
+            if t % 2 == 0:
+                seq = [self.seal(), (L_MAP_A, h, None), (PLAIN, y, None), (L_MAP_A, h, "map_unwritten_ctx_mapa")]
+            else:
+                seq = [self.seal(), (PLAIN, quad_of(h, g.fp()), None), (PLAIN, y, None), (L_MAP_B, h, "map_unwritten_ctx_mapb_once")]
+            ok = self.place(seq + [(L_PA, None, "map_unwritten_ctx_next"), self.seal()], 3 + at_read, e)
+        elif cls in ("mapb_written_once", "mapb_twice"):
+            h, y = fresh(), val()
+            x = quad_of(h, g.fp())
+            write = [self.seal(), (PLAIN, x, None), (PLAIN, y, None), self.seal()]
+            if cls == "mapb_written_once":
+                seq, km = [(L_MAP_B, h, None), (L_PA, None, "mapb_written_once_next"), self.seal()], 0
+            else:
+                seq, km = [(L_MAP_B, h, None), (L_MAP_B, h, None), (L_PB, None, "mapb_twice_next"), self.seal()], 1
+            k0 = km + at_read
+            pos = self.span(e, k0, 0)
+            if pos is None:
+                return False
+            ok = None
+            for j in range(4):                                       # the variant asked for, else the others in turn
+                w, how = self.earlier(pos[0], ("same_row", "earlier_row", "earlier_run", "earlier_piece")[(t + j) % 4])
+                seq[km] = (L_MAP_B, h, cls + "_" + how)
+                ok = self.place(seq, k0, e, (write, w))
+                if ok:
+                    break
+        elif cls == "pred_unwritten_depth_k":
+            ok = self.place([self.seal(), (L_PB + t % 4, None, cls), (L_PA, None, None), self.seal()], 1, e)
+        elif cls == "pred_short_list":                               # depth k, j <= k pushes
+            k = 1 + t % 4
+            c, seq = fresh(), []
+            seq.append((L_MAP_A, c, None))
+            for _ in range(1 + (t // 4) % k):
+                seq += [(PLAIN, val(), None), (L_MAP_A, c, None)]
+            seq.append((L_PA + k, None, cls))
+            ok = self.place(seq + [self.seal()], len(seq) - 1, e)
+        elif cls == "pred_duplicates":                               # MAP_A of bucket c at context c: pushes its value, keeps context c
+            c = fresh()
+            x, z = quad_of(c, g.fp()), quad_of(c, g.fp() ^ 0x5A5A)
+            seq = [self.seal(), (PLAIN, x, None), (L_MAP_A, c, None), (L_MAP_A, c, None), (PLAIN, z, None),     # list c: z x x
+                   (L_PC, None, "pred_duplicates_c"), (L_MAP_A, c, None), (L_PD, None, "pred_duplicates_d"), (L_MAP_A, c, None),
+                   (L_PE, None, "pred_duplicates_e"), self.seal()]
+            ok = self.place(seq, 5, e)
+        elif cls == "six_pushes_then_pred":                          # quads of bucket c keep the context at c
+            c, n = fresh(), 6 + t % 2
+            seq = [(L_MAP_A, c, None)] + [(PLAIN, quad_of(c, 1 + 97 * j + t % 89), None) for j in range(n)]
+            seq.append((L_PC + t % 3, None, cls))
+            ok = self.place(seq + [self.seal()], n + 1, e)
+        elif cls == "self_span_after_depth_k":                       # x at depth k of context hash16(x), read, then PREDICTED_A on x
+            k, R = 1 + t % 4, (2, 5, 14, 30)[(t // 4) % 4]
+            c = fresh()
+            x = quad_of(c, g.fp())
+            seq = [self.seal(), (PLAIN, x, None), (PLAIN, x, None)]
+            for _ in range(k):
+                seq += [(PLAIN, val(), None), (L_MAP_A, c, None)]
+            k0 = len(seq)
+            seq.append((L_PA + k, None, cls))
+            seq += [(L_PA, None, "self_span_run")] * R + [(L_PB, None, "self_span_then_depth_1"), self.seal()]
+            ok = self.place(seq, k0, e)
+            if ok:
+                for i in range(k0, k0 + R + 1):                     # where the run crosses a block, a row or a copy-mode block
+                    a, b = ok[i], ok[i + 1]
+                    where = "cut_by_copy" if b - a > 1 else "cross_15_16" if a % 32 == 15 else "cross_row" if a % 32 == 31 else None
+                    if where:
+                        g.note("self_span_" + where, b, self.vals[i + 1])
+        elif cls == "pred_chain_context0":                           # the context after an unwritten read is 0
+            ok = self.place([self.seal(), (L_PB + t % 4, None, "pred_chain_context0"), (L_PA, None, "pred_chain_context0_after"),
+                             (L_PC, None, "pred_chain_context0_after"), self.seal()], 1, e)
+        else:
+            raise ValueError(cls)
+        if ok:
+            self.turn[cls] += 1
+        else:
+            self.miss[cls] += 1
+        return bool(ok)
+
+    def copy_episode(self, b, a):
+        """blocks b - 2 and b - 1 (forced incompressible, in front of the copy-mode blocks b .. a - 1) planted with quads of one bucket c
+        behind a MAP_A at c: the context stays c and its list holds the last five; the last quad in front of the copy run, PREDICTED_E,
+        reads one of them (hash c: a self-map) and the first quads behind it continue the span across the copy-mode blocks. -> True when
+        it was placed"""
+        g, q = self.g, self.g.q
+        lo, e = (b - 2) * q - 1, a * q
+        if b < 3 or not all(g.forced_inc.get(x) is True for x in (b - 2, b - 1)) or not self.free([lo]) or \
+                any((x in g.planted) for x in range(lo, b * q)) or not self.free(range(e, e + 4)):
+            return None
+        c = g.fresh()
+        xs = [quad_of(c, 1 + 131 * j) for j in range(2 * q - 1)]
+        seq = [(L_MAP_A, c)] + [(PLAIN, x) for x in xs] + [(L_PE, None), (L_PA, None), (L_PA, None), (L_PB, None), (L_MAP_A, g.fresh())]
+        pos = list(range(lo, b * q)) + [e, e + 1, e + 2, e + 3]
+        if not self.keeps_forced(pos, [f for f, _ in seq]):
+            return False
+        vals = _lion_sim(seq, {})
+        for x, (f, v), val, note in zip(pos, seq, vals, [None] * (2 * q) + ["self_span_cut_by_copy_depth_4", "self_span_cut_by_copy",
+                                                                           "self_span_cut_by_copy", "self_span_then_depth_1", None]):
+            g.put(x, f, 0 if v is None else v)
+            if note:
+                g.note(note, x, val)
+        return True
+
+    def stream_start(self):
+        """predicted quads at the stream start: context 0 with empty lists, so they decode to 0"""
+        if self.free(range(4)):
+            for x, f in enumerate((L_PA, L_PC, L_PE)):
+                self.g.put(x, f, 0); self.g.note("pred_chain_context0_stream_start", x, 0)
+            self.g.put(3, L_MAP_A, self.g.fresh())
+
+    def main_end(self, nb):
+        """the last main-loop quad a MAP_A at a never-written bucket h whose list holds y: the tail's first quad (PREDICTED_A) reads y
+        from the walk's last context h (not hash16(0)). -> (quad of the tail's first quad, y) or None"""
+        g = self.g
+        h, y = g.fresh(), quad_of(g.fresh(), g.fp())
+        e = nb * g.q - 1
+        if self.place([self.seal(), (L_MAP_A, h, None), (PLAIN, y, None), (L_MAP_A, h, "map_unwritten_ctx_main_last")], 3, e):
+            return e + 1, y
+        return None
+
+
+def _plant_lion(g, run_blocks, cut_blocks, copy, main_blocks, tail_spec):
+    """the Lion classes, each in turn on every placement kind (rows' lanes 0, 15, 16 and 31, rows with one copy-mode block, chunk-map run
+    edges, piece edges, behind copy-mode episodes); -> ({quad: placements}, tail expectation or None)"""
+    q, nb = g.q, g.nb
+    pl = _LionPlanter(g, [b * q for b in run_blocks], [b * q for b in cut_blocks], copy)
+    kinds = {k: [] for k in LION_PLACES if "copy" not in k}
+    nrows = (nb + 1) // 2
+    for li, lane in enumerate((0, 15, 16, 31)):
+        for j in range(48):
+            kinds[f"lane_{lane}"].append(min(nrows - 1, (j * nrows) // 48 + 3 + 7 * li) * 32 + lane)
+    for b in run_blocks[1:]:
+        kinds["run_first"].append(b * q); kinds["run_last"].append(b * q - 1)
+    for b in cut_blocks:
+        kinds["piece_first"].append(b * q); kinds["piece_last"].append(b * q - 1)
+    place = {}
+    for k, qs in kinds.items():
+        for x in qs:
+            place.setdefault(x, set()).add(k)
+    pl.stream_start()
+    tail = None
+    if main_blocks == nb and SIG["lion"] <= tail_spec[0] <= SIG["lion"] + 4 * (q - 1):             # a tail with a leading PREDICTED_A
+        tail = pl.main_end(nb)
+    ci = collections.Counter({k: nb for k in LION_PLACES})              # streams start the classes at different turns
+    for i in range(max(len(v) for v in kinds.values())):
+        order = list(kinds)[i % len(kinds):] + list(kinds)[:i % len(kinds)]
+        if i % 2:                                                    # the two sides of a seam take turns at coming first
+            order = [k.replace("_first", "_x").replace("_last", "_first").replace("_x", "_last") for k in order]
+        for k in order:
+            if i < len(kinds[k]) and 0 < kinds[k][i] < nb * q - 48:
+                if pl.plant(LION_CLASSES[ci[k] % len(LION_CLASSES)], kinds[k][i]):
+                    ci[k] += 1
+    # copy-mode episodes: the first quad behind one (lane 16 of a row whose first block is copy mode, lane 0 of a row behind one whose
+    # second block is) takes its context from the walk's carry across the copy-mode blocks. It holds a class's key quad (for the MAP
+    # classes the predicted read behind the MAP, which is the last quad in front of the copy run), or, at every third episode, a
+    # self-map span across the copy-mode blocks.
+    for k, b in enumerate(np.flatnonzero(copy[1:] & ~copy[:-1]) + 1):
+        a = int(b)
+        while a < nb and copy[a]:
+            a += 1
+        if a + 2 >= nb:
+            continue
+        where = ("after_copy", "copy_row_lane_16" if (a - 1) % 2 == 0 else "after_copy_row_lane_0")
+        if k % 3 == 2:
+            ok = pl.copy_episode(int(b), a)
+        else:
+            ok = pl.plant(LION_CLASSES[ci[where[1]] % len(LION_CLASSES)], a * q, at_read=True)
+            ci[where[1]] += ok
+        if ok:
+            place.setdefault(a * q, set()).update(where)
+    return place, tail
+
+
 def _drive_automaton(g, seams, nblocks):
     """force incompressible / compressible blocks so that the automaton is in a chosen state in front of chosen blocks: a state at every
     decoder run seam, then every reachable state once; each word (protection.word_to) follows 64 compressible blocks that take the
@@ -638,22 +1069,29 @@ def _geometry(alg, nbytes, cap, main_blocks, num_sms):
     if alg == "chameleon":
         runs = cham_dec_runs(nbytes, cap, main_blocks, num_sms)
         return [t0 * TILE_BLOCKS for t0, _ in runs], runs
+    if alg == "lion":
+        return lion_dec_runs(nbytes, main_blocks, num_sms), None
     return cheetah_dec_runs(nbytes, main_blocks, num_sms), None
 
 
 def build(alg, plan, seed):
     """A stream of `plan["nbytes"]` bytes or so. plan keys: quiet (default True: no two incompressible blocks in a row, no copy mode),
-    p_pred (Cheetah: share of PREDICTED flags), tail = (length, end) (see _Gen._tail), copy_every (force an incompressible pair every
+    p_pred (Cheetah, Lion: share of PREDICTED flags), tail = (length, end) (see _Gen._tail), copy_every (force an incompressible pair every
     that many blocks), prot_states (drive the automaton into every reachable state at chosen blocks, decoder run seams included),
-    cuts (fractions of the block count: piece cuts whose edges get plantings), plant (default True), num_sms.
+    cuts (fractions of the block count: piece cuts whose edges get plantings), plant (default True), num_sms, odd (Lion: the parity of
+    the block count).
     The plantings sit on the decoder's runs at the capacity the stream decodes to (decoded_size: the tests decode with it, one byte
     and one block less, which give the same runs). Returns (stream, manifest): manifest = {main_blocks, tail_off, state, starts,
     copy_blocks, cut_blocks, run_blocks (first block of every decoder run), decoded_size, classes: [(class, block, quad, expected value
-    or None)], placements: {edge kind: [quads that carry a class]}, prot_targets: [(block, state)], tail_class}."""
+    or None)], placements: {edge kind: [quads that carry a class]}, prot_targets: [(block, state)], tail_class, tail_expect (Lion: the
+    first tail quad and the value it decodes to, a predicted read of the main loop's last context)}."""
     num_sms = plan.get("num_sms", planted.H100_SMS)
     q = QPB[alg]
-    avg = {"chameleon": 8 + 128 + 59, "cheetah": 8 + 0.3 * 32 * 4 * (1 - plan.get("p_pred", 0.5)) + 0.7 * 32 * 2 * (1 - plan.get("p_pred", 0.5))}
+    avg = {"chameleon": 8 + 128 + 59, "cheetah": 8 + 0.3 * 32 * 4 * (1 - plan.get("p_pred", 0.5)) + 0.7 * 32 * 2 * (1 - plan.get("p_pred", 0.5)),
+           "lion": 6 + 0.3 * 16 * 4 * (1 - plan.get("p_pred", 0.5)) + 0.7 * 16 * 2 * (1 - plan.get("p_pred", 0.5))}
     nblocks = max(4, int(plan["nbytes"] / avg[alg]))
+    if "odd" in plan:                                                # Lion: the parity of the block count (a last row of one block)
+        nblocks += nblocks % 2 != plan["odd"]
     tail = plan.get("tail", (0, "clean"))
     geo = None                                                       # decoder run seams the plantings are placed at
     for _ in range(6):
@@ -667,11 +1105,14 @@ def build(alg, plan, seed):
             g.forced_inc[nblocks - 2] = g.forced_inc[nblocks - 1] = True
         if plan.get("prot_states") and geo is not None:
             prot_targets = _drive_automaton(g, geo[1:], nblocks)
-        place = {}
+        place, tail_expect = {}, None
         if geo is not None and plan.get("plant", True):
             stream, copy, _, _ = g.layout(tail)
             w = walk(alg, stream)
-            place = _plant(g, alg, geo, cut_blocks, copy, stream.size, decoded_size(alg, stream, w), w["main_blocks"], num_sms)
+            if alg == "lion":
+                place, tail_expect = _plant_lion(g, geo, cut_blocks, copy, w["main_blocks"], tail)
+            else:
+                place = _plant(g, alg, geo, cut_blocks, copy, stream.size, decoded_size(alg, stream, w), w["main_blocks"], num_sms)
         stream, copy, off, tcls = g.layout(tail)
         w = walk(alg, stream)
         size = decoded_size(alg, stream, w)
@@ -694,34 +1135,36 @@ def build(alg, plan, seed):
                     "copy_blocks": copy_blocks, "cut_blocks": cut_blocks, "classes": classes, "prot_targets": prot_targets,
                     "tail_class": tcls, "block_offsets": off[:-1], "nblocks": nblocks, "decoded_size": size,
                     "run_blocks": geo if geo is not None else new, "placements": placements,
-                    "planted_flags": {qi: fl for qi, (fl, _) in g.planted.items()}}
+                    "planted_flags": {qi: fl for qi, (fl, _) in g.planted.items()}, "tail_expect": tail_expect}
 
 
 def flags_of(alg, stream, manifest, block):
     """the flags of an encoded main-loop block"""
     o = manifest["starts"][block]
-    sig = int.from_bytes(np.asarray(stream[o:o + SIG]).tobytes(), "little")
+    sig = int.from_bytes(np.asarray(stream[o:o + SIG[alg]]).tobytes(), "little")
     fb = FB[alg]
     return [(sig >> (fb * k)) & ((1 << fb) - 1) for k in range(QPB[alg])]
 
 
 def _fits(alg, L, end):
-    if L < SIG:
+    if L < SIG[alg]:
         return True
-    D = L - SIG - {"clean": 0, "plain_end": 0, "raw1": 1, "raw2": 2, "raw3": 3, "map0": 0, "map1": 1}[end]
+    D = L - SIG[alg] - {"clean": 0, "plain_end": 0, "raw1": 1, "raw2": 2, "raw3": 3, "map0": 0, "map1": 1}[end]
     if D % 2 or D < 0:
         return False
     q = QPB[alg]
+    if alg == "lion":
+        return D // 2 - (q - (end != "clean")) <= D // 4
     if end == "clean":
         return (2 * q <= D <= 4 * q) if alg == "chameleon" else D <= 4 * q
     return D // 2 - (q - 1) <= D // 4
 
 
 def tail_lengths(alg):
-    """every tail length 0 .. SIG + BS - 1, each with an end that fits it (the ends in turn)"""
+    """every tail length 0 .. SIG[alg] + BS - 1, each with an end that fits it (the ends in turn)"""
     ends = ("clean", "plain_end", "raw1", "raw2", "raw3", "map0", "map1")
     out = []
-    for L in range(SIG + BS[alg]):
+    for L in range(SIG[alg] + BS[alg]):
         ok = [e for e in ends if _fits(alg, L, e)] or ["clean"]
         out.append((L, ok[(L // 2) % len(ok)]))
     return out

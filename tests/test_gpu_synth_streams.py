@@ -23,7 +23,7 @@ import test_gpu_sharded_stream_protected_decode as prot_located
 pytestmark = pytest.mark.gpu
 CANARY = 0xA5
 MIB = 1 << 20
-ALG_ID = {"chameleon": 0, "cheetah": 1}
+ALG_ID = {"chameleon": 0, "cheetah": 1, "lion": 2}
 
 
 @pytest.fixture(scope="module")
@@ -224,7 +224,7 @@ def test_cheetah_paths(torch_cuda, lib, sms, model, name):
             assert got_m == 0, (name, cap)
 
 
-@pytest.mark.parametrize("alg", ss.ALGS)
+@pytest.mark.parametrize("alg", ["chameleon", "cheetah"])      # Lion: tests/test_gpu_lion_synth_streams.py
 def test_reference_symbols_host_and_device(torch_cuda, lib, alg):
     torch = torch_cuda
     for name in [k for k in PLANS if PLANS[k][0] == alg and PLANS[k][1]["nbytes"] <= 4 * MIB and k not in MALFORMED][:2] + \

@@ -1,7 +1,9 @@
-"""Synthesized Chameleon and Cheetah streams (tests/synth_streams.py) on the CPU: every stream parses back to its manifest and every class
+"""Synthesized Chameleon, Cheetah and Lion streams (tests/synth_streams.py) on the CPU: every stream parses back to its manifest and every class
 is where the manifest says, with the flag it was planted with and the value it must decode to; the plain in-order decoder and the oracle
 agree on every stream at every capacity the GPU tests use; the CPU formulations of the parallel decoders (the decode-pass model, the
-Cheetah round model, the range maps of the located paths) give the oracle's answer on them."""
+Cheetah round model, the range maps of the located paths) give the oracle's answer on them. The Lion walk models
+(tests/lion_walk_model.cpp, tests/lion_piece_model.cpp), which compile density_b200/csrc/lion_walk.cuh itself, are checked against the
+plain decoder, which shares no code with them."""
 import collections
 
 import numpy as np
@@ -23,7 +25,14 @@ SMALL = [
     ("cheetah", {"nbytes": 100000, "p_pred": 0.9, "tail": (100, "plain_end")}, 7),
     ("cheetah", {"nbytes": 80000, "p_pred": 0.99, "tail": (9, "map1")}, 8),
     ("cheetah", {"nbytes": 2000000, "p_pred": 0.3, "quiet": False, "prot_states": True}, 9),
+    ("lion", {"nbytes": 400000, "p_pred": 0.5, "cuts": tuple(k / 25 for k in range(1, 25)), "odd": True, "tail": (40, "raw2")}, 51),
+    ("lion", {"nbytes": 300000, "p_pred": 0.3, "quiet": False, "copy_every": 41, "odd": False, "tail": (30, "clean")}, 52),
+    ("lion", {"nbytes": 150000, "p_pred": 0.9, "cuts": (0.2, 0.45, 0.7), "odd": False, "tail": (26, "plain_end")}, 53),
+    ("lion", {"nbytes": 1500000, "p_pred": 0.3, "quiet": False, "prot_states": True, "cuts": tuple(k / 10 for k in range(1, 10)),
+              "tail": (63, "raw3")}, 54),
+    ("lion", {"nbytes": 100000, "p_pred": 0.99, "odd": True, "tail": (9, "map1")}, 55),
 ]
+LION = [i for i, c in enumerate(SMALL) if c[0] == "lion"]
 CHAM_CLASSES = {"map_unwritten", "map_unwritten_fixed", "map_bucket0_before_write", "map_bucket0_after_write", "bucket0_write",
                 "plain_same_value", "plain_same_value_reader", "plain_twin", "plain_twin_reader", "map_fp0_written_same_tile",
                 "map_fp0_written_earlier_tile", "map_fp0_written_earlier_run", "map_fp0_written_earlier_piece", "pileup_4", "pileup_5",
@@ -99,6 +108,54 @@ def test_every_class_is_present_at_every_placement():
         assert PLACES[alg] <= places[alg], (alg, PLACES[alg] - places[alg])
 
 
+# the lane (quad index mod 32) of a row, or of a block (mod 16), every quad of a placement sits on
+LION_LANES = {"lane_0": (32, 0), "lane_15": (32, 15), "lane_16": (32, 16), "lane_31": (32, 31), "copy_row_lane_16": (32, 16),
+              "after_copy_row_lane_0": (32, 0), "after_copy": (16, 0), "run_first": (16, 0), "run_last": (16, 15), "piece_first": (16, 0),
+              "piece_last": (16, 15)}
+
+
+def lion_coverage(streams):
+    """{placement: Lion classes planted on it} and every class name noted, over (stream, manifest) pairs; every quad of a placement sits
+    on its lane, and the quads behind copy-mode episodes follow the last copy-mode block"""
+    on, names = collections.defaultdict(set), set()
+    for _, m in streams:
+        at = collections.defaultdict(set)
+        for c, _, qi, _ in m["classes"]:
+            at[qi].add(ss.lion_class(c)); names.add(c)
+        copy = set(m["copy_blocks"])
+        for k, v in m["placements"].items():
+            mod, lane = LION_LANES[k]
+            for x in v:
+                assert x % mod == lane, (k, x)
+                if "copy" in k:
+                    assert x // 16 - 1 in copy and x // 16 not in copy, (k, x)
+                    assert (k == "copy_row_lane_16") == ((x // 16 - 1) % 2 == 0) or k == "after_copy", (k, x)
+                on[k] |= at[x]
+    return on, names
+
+
+def test_every_lion_class_is_on_every_placement():
+    """every Lion class on the rows' lanes 0, 15, 16 and 31, lane 16 of a row whose first block is copy mode, lane 0 of a row behind one
+    whose second block is, chunk-map run and piece edges and behind copy-mode episodes; the variants of the chunk-map writes, the self-map
+    spans across a block, a row and copy-mode blocks, the stream start, and the predicted first tail quad behind a MAP at an unwritten
+    bucket"""
+    on, names = lion_coverage([stream(i) for i in LION])
+    for k in ss.LION_PLACES:
+        assert set(ss.LION_CLASSES) <= on[k], (k, set(ss.LION_CLASSES) - on[k])
+    for cls in ("mapb_written_once", "mapb_twice"):
+        assert {f"{cls}_{w}" for w in ("same_row", "earlier_row", "earlier_run", "earlier_piece")} <= names, cls
+    assert {"map_unwritten_ctx_mapa", "map_unwritten_ctx_mapb_once", "map_unwritten_ctx_main_last", "self_span_cross_15_16",
+            "self_span_cross_row", "self_span_cut_by_copy", "self_span_then_depth_1", "pred_chain_context0_stream_start"} <= names
+    assert {SMALL[i][1]["odd"] for i in LION if "odd" in SMALL[i][1]} == {True, False}
+    assert {stream(i)[1]["main_blocks"] % 2 for i in LION} == {0, 1}
+    for i in LION:
+        s, m = stream(i)
+        out = oracle.decode("lion", s, 64 * s.size + 4096)
+        if m["tail_expect"] is not None and out.size:                  # (not behind a malformed tail)
+            q, want = m["tail_expect"]
+            assert q == m["main_blocks"] * 16 and int(out[4 * q:4 * q + 4].view("<u4")[0]) == want, i
+
+
 @pytest.mark.parametrize("i", range(len(SMALL)))
 def test_plantings_sit_on_the_runs_of_the_decoding_capacity(i):
     """the decoder's runs at the capacities the streams are decoded with that are not capacity errors (the decoded size, one byte and
@@ -111,6 +168,8 @@ def test_plantings_sit_on_the_runs_of_the_decoding_capacity(i):
     for cap in (size, size - 1, size - ss.BS[alg]):
         if alg == "chameleon":
             runs = [ss.TILE_BLOCKS * t0 for t0, _ in ss.cham_dec_runs(s.size, cap, m["main_blocks"])]
+        elif alg == "lion":
+            runs = ss.lion_dec_runs(s.size, m["main_blocks"])
         else:
             runs = ss.cheetah_dec_runs(s.size, m["main_blocks"])
         assert runs == m["run_blocks"], cap
@@ -121,7 +180,7 @@ def test_plantings_sit_on_the_runs_of_the_decoding_capacity(i):
 
 def test_prot_targets_cover_every_reachable_state():
     import protection as P
-    for i in (2, 8):
+    for i in (2, 8, LION[3]):
         _, m = stream(i)
         assert {st for _, st in m["prot_targets"]} == P.reachable_states()
 
@@ -186,7 +245,7 @@ def test_decode_pass_model():
                 continue
             keep.append(b)
             fl = ss.flags_of("chameleon", s, m, b)
-            o = m["starts"][b] + ss.SIG
+            o = m["starts"][b] + ss.SIG["chameleon"]
             for f in fl:
                 is_plain.append(f == ss.PLAIN)
                 n = 4 if f == ss.PLAIN else 2
@@ -221,3 +280,77 @@ def test_cheetah_round_model(cl_model, i):
             assert st["settled"], st
         if st["settled"]:
             assert out.size == want.size and (out == want).all(), (nruns, st)
+
+
+# ---- Lion: the walk models against the plain decoder ------------------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def lion_walk_model(tmp_path_factory):
+    import lion_streams as ls
+    return ls.build_model(tmp_path_factory.mktemp("lion_walk"))
+
+
+@pytest.mark.parametrize("i", LION)
+def test_lion_walk_model_equals_the_plain_decoder(lion_walk_model, i):
+    """tests/lion_walk_model.cpp (boundaries, unpack, chunk map, the walk of lion_walk.cuh, the tail) gives the plain decoder's bytes at the
+    decoded size and every capacity below it is refused; its counts are the ones lion_streams.walk_counts reads off the stream"""
+    import lion_streams as ls
+    s, m = stream(i)
+    if s.size > 3 * (1 << 19):
+        s = s[:m["starts"][int(np.searchsorted(m["starts"], 1 << 20))]]
+    size = m["decoded_size"] if s.size == stream(i)[0].size else 64 * s.size
+    want = ss.decode_reference("lion", s, size)
+    n, got, c = ls.run_model(lion_walk_model, s, size)
+    assert n == len(want) and got.tobytes() == want, (i, n, len(want))
+    if n:
+        assert c == ls.walk_counts(s, got), (c, ls.walk_counts(s, got))
+        for cap in (n - 1, n - 64):
+            assert ls.run_model(lion_walk_model, s, cap)[0] == 0
+    else:                                                            # a malformed tail: the main loop alone
+        main = s[:m["tail_off"]]
+        want = ss.decode_reference("lion", main, 64 * s.size)
+        n, got, c = ls.run_model(lion_walk_model, main, len(want))
+        assert n == len(want) > 0 and got.tobytes() == want and c == ls.walk_counts(main, got)
+
+
+@pytest.fixture(scope="module")
+def lion_piece_model(tmp_path_factory):
+    import ctypes
+    import os
+    import subprocess
+    so = os.path.join(str(tmp_path_factory.mktemp("lion_piece")), "lion_piece_model.so")
+    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++",
+                           os.path.join(os.path.dirname(os.path.abspath(__file__)), "lion_piece_model.cpp"), "-o", so])
+    L = ctypes.CDLL(so)
+    L.lion_piece_model_check.restype = ctypes.c_long
+    L.lion_piece_model_check.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]
+    return L
+
+
+def lion_cut_sets(m):
+    """the manifest's cuts, chunk-map run seams, each side of planted classes, odd blocks, one-block and empty pieces, the blocks behind
+    copy-mode episodes and automaton targets"""
+    mb = m["main_blocks"]
+    planted_blocks = sorted({b for _, b, _, _ in m["classes"]})
+    pick = lambda xs, f: xs[int(f * (len(xs) - 1))] if xs else mb // 2
+    seams = m["run_blocks"][1:]
+    sets = [list(m["cut_blocks"]), [pick(seams, 0.5)], [pick(seams, 0.2), pick(seams, 0.7)],
+            [pick(planted_blocks, 0.3), pick(planted_blocks, 0.3) + 1, pick(planted_blocks, 0.6)],
+            [mb // 3 | 1, (mb // 2) | 1], [mb // 4, mb // 4 + 1, mb // 4 + 1, mb // 2]]
+    after_copy = [b + 1 for b in m["copy_blocks"] if b + 1 < mb and b + 1 not in m["copy_blocks"]]
+    if after_copy:
+        sets.append(after_copy[1::max(1, len(after_copy) // 5)][:5])
+    if m["prot_targets"]:
+        sets.append([B for B, _ in m["prot_targets"][::max(1, len(m["prot_targets"]) // 7)]][:7])
+    return [sorted(c for c in cs if 0 < c < mb) for cs in sets if cs]
+
+
+@pytest.mark.parametrize("i", LION)
+def test_lion_piece_model_at_the_planted_cuts(lion_piece_model, i):
+    """tests/lion_piece_model.cpp: the walk relayed piece by piece (every piece laid out in rows of its own) equals the whole walk at the
+    manifest's cuts and the cut sets of the GPU tests"""
+    from test_sharded_lion_decode_cpu import walk_pieces
+    s, m = stream(i)
+    for cuts in lion_cut_sets(m):
+        nb, counts = walk_pieces(lion_piece_model, s, [0] + cuts + [m["main_blocks"]])
+        assert nb == m["main_blocks"], (i, cuts)
+        assert counts[0] == counts[4] and counts[1] == counts[5], (i, cuts, counts)

@@ -1084,6 +1084,7 @@ struct density_b200_decode_shard {
     int num_sms = 0;
     bool phase1_done = false;
     int prot_stage = 0;             // prot_*: 1 after the transfer, 2 after phase 1
+    void reset() { phase1_done = false; prot_stage = 0; }     // no step of any piece done
 };
 
 density_b200_decode_shard* density_b200_decode_shard_create(void) { return new_shard<density_b200_decode_shard>(); }
@@ -1093,11 +1094,10 @@ void density_b200_decode_shard_destroy(density_b200_decode_shard* s) {
     s->seed.release();
     delete s;
 }
-// the piece set up in s (phase 1, prot_transfer and prot_enter): phase 2 waits for the next phase 1 (with_seed, a protected entry: the
-// protected sequence starts over), the workspace and with_seed the seed are ensured, the piece is stored
+// the piece set up in s (phase 1, prot_transfer and prot_enter): every step of the piece before it void, the workspace and with_seed the
+// seed ensured, the piece stored
 static int decode_piece_setup(density_b200_decode_shard* s, const uint8_t* d_in, size_t n, size_t cap, int is_last, bool with_seed, cudaStream_t st) {
-    s->phase1_done = false;
-    if (with_seed) s->prot_stage = 0;
+    s->reset();
     cudaError_t e = s->ws.ensure(cham_decode_workspace_bytes(n, cap, s->num_sms), st);
     if (e == cudaSuccess && with_seed) e = s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
@@ -1153,7 +1153,7 @@ int density_b200_decode_shard_prot_transfer(density_b200_decode_shard* s, const 
     if (rc == DENSITY_B200_OK) rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, true, st);
     if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    const cudaError_t e = cham_decode_prot_transfer(d_in, n, cap, s->ws.p, s->num_sms, is_last_shard, d_transfer_out, st, &launches);
+    const cudaError_t e = cham_decode_prot_transfer(d_in, n, s->ws.p, is_last_shard, d_transfer_out, st, &launches);
     rc = step_result(e, launches, "decode shard prot transfer");
     if (rc == DENSITY_B200_OK) s->prot_stage = 1;
     return rc;
@@ -1226,6 +1226,7 @@ struct ClDecodePiece {
     uint32_t round = 0;             // Cheetah: the rounds folded
     bool transfer_done = false;     // prot_transfer done, prot_phase1 not yet
     bool prot = false;              // the current piece went through prot_phase1 or prot_enter: phase 3 writes the protected seam words
+    void reset() { phase = 0; round = 0; transfer_done = false; prot = false; }     // no step of any piece done
     ~ClDecodePiece() { ws.release(); tables.release(); seed.release(); }
 };
 struct density_b200_cheetah_decode_shard : ClDecodePiece {};
@@ -1248,7 +1249,7 @@ static int cl_piece_setup(ClDecodePiece* s, bool lion, const uint8_t* d_in, size
     int rc = decode_in_args(d_in, n, d_out, cap);
     if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table});
     if (rc != DENSITY_B200_OK) return rc;
-    s->phase = 0; s->round = 0; s->transfer_done = false; s->prot = false;
+    s->reset();
     CheeShardArgs& a = s->a;
     a.d_in = d_in; a.n = n; a.d_out = d_out; a.cap = cap; a.first = is_first != 0; a.last = is_last != 0; a.lion = lion; a.num_sms = s->num_sms;
     cudaError_t e = with_seed ? s->seed.ensure(DECODE_PROT_SEED_WORDS * sizeof(uint32_t), st) : cudaSuccess;
@@ -1948,26 +1949,41 @@ static int decode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, siz
     return decode_in_args(d_in, n, d_out, cap);
 }
 
-// The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it: phase 1 -> table exchange ->
-// fold -> phase 2 -> seam words -> verdict. is_last: the piece ends the stream (a non-final piece must decode to whole 256-byte blocks).
-// d_out_offset (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
-// cand >= 0: a located piece of a stream with copy-mode blocks (density_b200_decode_sharded_stream_protected), entered in that candidate:
-// prot_enter and prot_phase2 on the handle's protected decode shard take the place of the two phases.
+// The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it:
+//   head  [prot: prot_transfer -> ncclAllGather(transfers) -> prot_phase1 | cand >= 0: prot_enter from that candidate (a located piece of a
+//         stream with copy-mode blocks, density_b200_decode_sharded_stream_protected) | phase 1]
+//   tail  table exchange -> fold -> phase 2 (prot_phase2 after either protected head) -> seam words -> verdict
+// The protected heads run on the handle's protected decode shard; prot: x is opened with [world][DECODE_PROT_TRANSFER_WORDS] u32 of extra
+// bytes for the transfers. is_last: the piece ends the stream (a non-final piece must decode to whole 256-byte blocks). d_out_offset
+// (may be NULL): where the piece's output starts, from the verdict's prefix offsets.
 static int decode_sharded_piece(const Exchange& x, const uint8_t* d_in, size_t n, int is_last, uint8_t* d_out, size_t cap,
-                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, int64_t cand = -1) {
-    density_b200_decode_shard* s = cand < 0 ? x.h->dec : x.h->pdec;
-    uint32_t* my_table = x.tables + (size_t)x.h->rank * 65536;
+                                uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset, bool prot,
+                                int64_t cand = -1) {
+    const bool seeded = prot || cand >= 0;
+    density_b200_decode_shard* s = seeded ? x.h->pdec : x.h->dec;
+    const size_t R = (size_t)x.h->rank;
+    uint32_t* my_table = x.tables + R * 65536;
     // phase 1: boundaries and writer pass need no carry-in; the piece's table (runs + tail) lands in my slot of the gather buffer
-    int rc = cand < 0 ? density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, my_table, x.st)
-                      : density_b200_decode_shard_prot_enter(s, d_in, n, cap, is_last, (uint32_t)cand, my_table, x.st);
+    int rc;
+    if (prot) {
+        uint32_t* transfers = reinterpret_cast<uint32_t*>(x.extra);
+        rc = density_b200_decode_shard_prot_transfer(s, d_in, n, cap, is_last, transfers + R * DECODE_PROT_TRANSFER_WORDS, x.st);
+        if (rc != DENSITY_B200_OK) return rc;
+        if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        rc = density_b200_decode_shard_prot_phase1(s, transfers, x.h->world, (int)R, my_table, x.st);
+    } else if (cand >= 0) {
+        rc = density_b200_decode_shard_prot_enter(s, d_in, n, cap, is_last, (uint32_t)cand, my_table, x.st);
+    } else {
+        rc = density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, my_table, x.st);
+    }
     if (rc != DENSITY_B200_OK) return rc;
     if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
-    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)x.h->rank, x.carry, x.st, &launches);
+    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, x.st, &launches);
     if ((rc = step_result(e, launches, "sharded decode fold")) != DENSITY_B200_OK) return rc;
     // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
-    rc = cand < 0 ? density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)
-                  : density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st);
+    rc = seeded ? density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)
+                : density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st);
     if (rc != DENSITY_B200_OK) return rc;
     return x.verdict(d_flags, d_total_size, d_out_offset);
 }
@@ -1980,7 +1996,7 @@ int density_b200_decode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
-    return decode_sharded_piece(x, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr);
+    return decode_sharded_piece(x, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr, false);
 }
 
 // The inverse of density_b200_encode_sharded_protected (any stream): transfer -> transfers exchange -> phase 1 from the composed state ->
@@ -1991,19 +2007,7 @@ int density_b200_decode_sharded_protected(density_b200_sharded* h, const uint8_t
     int rc = decode_sharded_args(h, d_in, n, d_out, cap, d_out_size, d_flags);
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v, (size_t)h->world * DECODE_PROT_TRANSFER_WORDS * sizeof(uint32_t))) != DENSITY_B200_OK) return rc;
-    density_b200_decode_shard* s = h->pdec;
-    const size_t R = (size_t)h->rank;
-    uint32_t* transfers = reinterpret_cast<uint32_t*>(x.extra);       // [world][DECODE_PROT_TRANSFER_WORDS]
-    if ((rc = density_b200_decode_shard_prot_transfer(s, d_in, n, cap, h->rank == h->world - 1, transfers + R * DECODE_PROT_TRANSFER_WORDS, x.st))
-        != DENSITY_B200_OK) return rc;
-    if (!x.gather(transfers, DECODE_PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
-    if ((rc = density_b200_decode_shard_prot_phase1(s, transfers, h->world, h->rank, x.tables + R * 65536, x.st)) != DENSITY_B200_OK) return rc;
-    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-    uint64_t launches = 0;
-    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, x.st, &launches);
-    if ((rc = step_result(e, launches, "sharded protected decode fold")) != DENSITY_B200_OK) return rc;
-    if ((rc = density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)) != DENSITY_B200_OK) return rc;
-    return x.verdict(d_flags, d_total_size, nullptr);
+    return decode_sharded_piece(x, d_in, n, h->rank == h->world - 1, d_out, cap, d_out_size, d_flags, d_total_size, nullptr, true);
 }
 
 // The exchange buffers of decode_sharded_cl_piece behind Exchange::extra (extra: nullptr for the size alone), in this order: the gathered
@@ -2137,19 +2141,31 @@ int density_b200_decode_sharded_lion_protected(density_b200_sharded* h, const ui
     return decode_sharded_cl(h, ALG_LION, true, d_in, n, d_out, cap, d_out_size, d_flags, d_total_size, stream_v);
 }
 
-int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
+// The body of the four locate entries: the argument checks (d_map: the u64 range maps 8-byte, the u32 protected range maps 4-byte
+// aligned), then every step of the piece s held void (the locate scratch is phase 1's), ws_bytes of workspace ensured, and
+// launch(workspace, stream, &launches) enqueued.
+extern "C++" {
+template <class S, class M, class F>
+static int locate_entry(S* s, const uint8_t* d_in, size_t n, const M* d_map, size_t ws_bytes, void* stream, const char* what, F launch) {
     g_last_error.clear();
     if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    const int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
+    int rc = decode_in_args(d_in, n, nullptr, 0);
     if (rc != DENSITY_B200_OK) return rc;
-    if (!al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
+    if (sizeof(M) == 8 && !al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
+    if ((rc = decode_table_args({d_map})) != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase1_done = false;     // the scratch is phase 1's
-    cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
+    s->reset();
+    cudaError_t e = s->ws.ensure(ws_bytes, st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     uint64_t launches = 0;
-    e = cham_decode_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
-    return step_result(e, launches, "decode locate");
+    e = launch(s->ws.p, st, &launches);
+    return step_result(e, launches, what);
+}
+}
+
+int density_b200_decode_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t* d_map, void* stream) {
+    return locate_entry(s, d_in, n_range + n_halo, d_map, cham_locate_workspace_bytes(n_range + n_halo), stream, "decode locate",
+                        [&](uint8_t* ws, cudaStream_t st, uint64_t* l) { return cham_decode_locate(d_in, n_range, n_halo, ws, d_map, st, l); });
 }
 
 // The layout checks and the walk from the stream start shared by density_b200_locate_piece (Chameleon) and
@@ -2226,18 +2242,8 @@ int density_b200_cheetah_locate_piece(const uint64_t* h_maps, int world, int ran
 
 int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint64_t range_offset,
                                        uint64_t* d_map, void* stream) {
-    g_last_error.clear();
-    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    const int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
-    if (rc != DENSITY_B200_OK) return rc;
-    if (!al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0;               // the scratch is phase 1's
-    cudaError_t e = s->ws.ensure(chee_locate_workspace_bytes(n_range, n_halo, range_offset), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t launches = 0;
-    e = chee_decode_locate(d_in, n_range, n_halo, range_offset, s->ws.p, d_map, st, &launches);
-    return step_result(e, launches, "cheetah decode locate");
+    return locate_entry(s, d_in, n_range + n_halo, d_map, chee_locate_workspace_bytes(n_range, n_halo, range_offset), stream, "cheetah decode locate",
+                        [&](uint8_t* ws, cudaStream_t st, uint64_t* l) { return chee_decode_locate(d_in, n_range, n_halo, range_offset, ws, d_map, st, l); });
 }
 
 // Sharded decode of a stream without known cuts: this rank holds its range + halo (include/density_b200.h). Locates the piece (one
@@ -2259,7 +2265,7 @@ int density_b200_decode_sharded_stream(density_b200_sharded* h, const uint8_t* d
     rc = density_b200_locate_piece(h->h_maps, h->world, h->rank, piece);
     if (rc != DENSITY_B200_OK) return rc;    // the same verdict on every rank: none enters the collectives below
     return decode_sharded_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[3], d_out, cap, d_out_size, d_flags,
-                                d_total_size, d_out_offset);
+                                d_total_size, d_out_offset, false);
 }
 
 // Sharded decode of a Cheetah stream without known cuts: this rank holds its range + halo at range_offset (include/density_b200.h).
@@ -2290,33 +2296,13 @@ int density_b200_decode_sharded_cheetah_stream(density_b200_sharded* h, const ui
 
 // ---- sharded decode of a stream without known cuts, copy-mode blocks included (DESIGN.md section 5) ----------------------------------
 int density_b200_decode_prot_locate(density_b200_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map, void* stream) {
-    g_last_error.clear();
-    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_map});
-    if (rc != DENSITY_B200_OK) return rc;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase1_done = false; s->prot_stage = 0;     // the scratch is phase 1's
-    cudaError_t e = s->ws.ensure(cham_locate_workspace_bytes(n_range + n_halo), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t launches = 0;
-    e = cham_decode_prot_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
-    return step_result(e, launches, "decode prot locate");
+    return locate_entry(s, d_in, n_range + n_halo, d_map, cham_locate_workspace_bytes(n_range + n_halo), stream, "decode prot locate",
+                        [&](uint8_t* ws, cudaStream_t st, uint64_t* l) { return cham_decode_prot_locate(d_in, n_range, n_halo, ws, d_map, st, l); });
 }
 int density_b200_cheetah_decode_prot_locate(density_b200_cheetah_decode_shard* s, const uint8_t* d_in, size_t n_range, size_t n_halo, uint32_t* d_map,
                                             void* stream) {
-    g_last_error.clear();
-    if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    int rc = decode_in_args(d_in, n_range + n_halo, nullptr, 0);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_map});
-    if (rc != DENSITY_B200_OK) return rc;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0; s->transfer_done = false;         // the scratch is phase 1's
-    cudaError_t e = s->ws.ensure(chee_prot_locate_workspace_bytes(n_range + n_halo), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    uint64_t launches = 0;
-    e = chee_decode_prot_locate(d_in, n_range, n_halo, s->ws.p, d_map, st, &launches);
-    return step_result(e, launches, "cheetah decode prot locate");
+    return locate_entry(s, d_in, n_range + n_halo, d_map, chee_prot_locate_workspace_bytes(n_range + n_halo), stream, "cheetah decode prot locate",
+                        [&](uint8_t* ws, cudaStream_t st, uint64_t* l) { return chee_decode_prot_locate(d_in, n_range, n_halo, ws, d_map, st, l); });
 }
 
 // the message of a prot_locate_walk error code
@@ -2396,7 +2382,7 @@ int density_b200_decode_sharded_stream_protected(density_b200_sharded* h, const 
         return rc;
     if (piece[5]) return DENSITY_B200_OK;    // refused on every rank alike: none enters the collectives below
     return decode_sharded_piece(x, d_in + piece[0], (size_t)(piece[1] - piece[0]), (int)piece[2], d_out, cap, d_out_size, d_flags,
-                                d_total_size, d_out_offset, (int64_t)piece[4]);
+                                d_total_size, d_out_offset, false, (int64_t)piece[4]);
 }
 
 // The same for a Cheetah stream: no range offset is needed, the composition finds the range that holds the stream start.

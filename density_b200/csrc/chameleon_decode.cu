@@ -675,36 +675,9 @@ cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t ca
 
 // The protection transfer of a piece (PT_NCAND words to d_transfer): the candidate rows of the boundary walk, then the head walk over them.
 // The rows stay in the workspace for cham_decode_phase1 with a seed.
-static cudaError_t prot_transfer_attr() {
-    static bool attr_done = false;
-    if (!attr_done) {
-        cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)bounds::prot_transfer_smem<T>());
-        if (e0 == cudaSuccess)
-            e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bounds::prot_transfer_smem<T>());
-        if (e0 != cudaSuccess) return e0;
-        attr_done = true;
-    }
-    return cudaSuccess;
-}
-cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
-                                      cudaStream_t stream, uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr();
-    if (e0 != cudaSuccess) return e0;
-    ChamDecLayout L; dec_layout(nbytes, cap, num_sms, &L);
-    uint32_t* res = reinterpret_cast<uint32_t*>(ws + L.B.res);
-    uint4* gres = reinterpret_cast<uint4*>(ws + L.B.gres);
-    const uint32_t nchunks = (uint32_t)((nbytes + T::CH - 1) / T::CH);
-    const uint32_t ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
-    if (nchunks) {
-        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, nbytes, nchunks, res);
-        bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
-        *launches += 2;
-    }
-    bounds::dec_prot_transfer<T, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<T>(), stream>>>(d_in, nbytes, nbytes, is_last, res, gres,
-                                                                                                    d_transfer);
-    ++*launches;
-    return cudaGetLastError();
+cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, uint8_t* ws, int is_last, uint32_t* d_transfer, cudaStream_t stream,
+                                      uint64_t* launches) {
+    return bounds::prot_transfer_launch<T>(d_in, nbytes, is_last, ws, d_transfer, stream, launches);
 }
 cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
                                    uint64_t* launches) {
@@ -728,18 +701,7 @@ size_t cham_locate_workspace_bytes(size_t nbytes) { bounds::BoundsLayout B; retu
 
 cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint64_t* d_map, cudaStream_t stream,
                                uint64_t* launches) {
-    bounds::BoundsLayout B; bounds::bounds_layout<T>(n_range + n_halo, 0, &B);
-    uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
-    uint4* gres = reinterpret_cast<uint4*>(ws + B.gres);
-    const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
-    const uint32_t ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
-    if (nchunks) {
-        bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
-        bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
-        *launches += 2;
-    }
-    bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(gres, ngroups, n_range, n_halo, reinterpret_cast<unsigned long long*>(d_map));
-    ++*launches;
+    bounds::range_map_launch<T>(d_in, n_range, n_halo, ws, reinterpret_cast<unsigned long long*>(d_map), stream, launches);
     return cudaGetLastError();
 }
 
@@ -747,8 +709,6 @@ cudaError_t cham_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
 // cham_locate_workspace_bytes(n_range + n_halo).
 cudaError_t cham_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
                                     uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr();
-    if (e0 != cudaSuccess) return e0;
     return bounds::prot_locate_launch<T>(d_in, n_range, n_halo, ws, d_map, stream, launches);
 }
 

@@ -969,42 +969,10 @@ cudaError_t chee_shard_phase3(const CheeShardArgs& a, uint64_t* d_out_size, uint
 }
 
 // The protected path's first step on a piece (DESIGN.md section 5): the candidate rows of the boundary walk (they stay in the workspace
-// for the phase 1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing. G: the geometry
-// of the piece's algorithm (CheeT or LionT).
-template <class G, bool LOCATE>
-static cudaError_t prot_transfer_attr() {
-    static bool attr_done = false;
-    if (!attr_done) {
-        const cudaError_t e0 = cudaFuncSetAttribute(bounds::dec_prot_transfer<G, LOCATE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                    (int)bounds::prot_transfer_smem<G>());
-        if (e0 != cudaSuccess) return e0;
-        attr_done = true;
-    }
-    return cudaSuccess;
-}
-static_assert(bounds::prot_transfer_smem<bounds::LionT>() <= 227u * 1024u, "the Lion head walk's shared memory must fit in one SM");
-template <class G>
-static cudaError_t shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr<G, false>();
-    if (e0 != cudaSuccess) return e0;
-    uint32_t* res = nullptr;
-    uint4* gres = nullptr;
-    if (a.n) {
-        const CheeDecPtrs p = chee_shard_ptrs(a);
-        res = reinterpret_cast<uint32_t*>(a.ws + p.B.res);
-        gres = reinterpret_cast<uint4*>(a.ws + p.B.gres);
-        const uint32_t nchunks = (uint32_t)((a.n + G::CH - 1) / G::CH);
-        bounds::dec_chunk_walk<G><<<nchunks, 160, 0, stream>>>(a.d_in, a.n, nchunks, res);
-        bounds::dec_group_compose<G><<<(nchunks + bounds::GROUP - 1) / bounds::GROUP, 160, 0, stream>>>(res, nchunks, gres);
-        *launches += 2;
-    }
-    bounds::dec_prot_transfer<G, false><<<1, bounds::PT_THREADS, bounds::prot_transfer_smem<G>(), stream>>>(a.d_in, a.n, a.n, a.last ? 1 : 0, res,
-                                                                                                    gres, d_transfer);
-    ++*launches;
-    return cudaGetLastError();
-}
+// for the phase 1 with a seed), then the head walk over them, PT_NCAND words to d_transfer. An empty piece reads nothing.
 cudaError_t chee_shard_prot_transfer(const CheeShardArgs& a, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
-    return a.lion ? shard_prot_transfer<bounds::LionT>(a, d_transfer, stream, launches) : shard_prot_transfer<T>(a, d_transfer, stream, launches);
+    return a.lion ? bounds::prot_transfer_launch<bounds::LionT>(a.d_in, a.n, a.last ? 1 : 0, a.ws, d_transfer, stream, launches)
+                  : bounds::prot_transfer_launch<T>(a.d_in, a.n, a.last ? 1 : 0, a.ws, d_transfer, stream, launches);
 }
 // The incoming state of piece `rank` composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS to d_seed).
 cudaError_t chee_shard_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
@@ -1047,27 +1015,20 @@ cudaError_t chee_decode_locate(const uint8_t* d_in, size_t n_range, size_t n_hal
                                cudaStream_t stream, uint64_t* launches) {
     const bool start = chee_locate_has_start(n_range, range_offset);
     bounds::BoundsLayout B; bounds::bounds_layout<T>(n_range + n_halo, start ? ~(size_t)0 : 0, &B);
-    const uint4* gres = reinterpret_cast<const uint4*>(ws + B.gres);
     unsigned long long* map = reinterpret_cast<unsigned long long*>(d_map);
-    uint32_t ngroups = 0;
     if (start) {
         const cudaError_t e = bounds::bounds_launch<T>(d_in, n_range + n_halo, ~(size_t)0, ws, B, stream, launches);
         if (e != cudaSuccess) return e;
+        // no group folded: the identity rows
+        bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(reinterpret_cast<const uint4*>(ws + B.gres), 0, n_range, n_halo, map);
+        ++*launches;
     } else {
-        uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
-        const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
-        ngroups = (nchunks + bounds::GROUP - 1) / bounds::GROUP;
-        if (nchunks) {
-            bounds::dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
-            bounds::dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, reinterpret_cast<uint4*>(ws + B.gres));
-            *launches += 2;
-        }
+        bounds::range_map_launch<T>(d_in, n_range, n_halo, ws, map, stream, launches);
     }
-    bounds::dec_range_compose<T><<<1, bounds::RC_THREADS, 0, stream>>>(gres, ngroups, n_range, n_halo, map);
     bounds::dec_start_row<T><<<1, 32, 0, stream>>>(start ? reinterpret_cast<const DecStatus*>(ws + B.status) : nullptr,
                                                    reinterpret_cast<const uint64_t*>(ws + B.blk_off), n_range, range_offset,
                                                    map + 2 + 2 * T::NCAND);
-    *launches += 2;
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -1077,8 +1038,6 @@ size_t chee_prot_locate_workspace_bytes(size_t nbytes) { bounds::BoundsLayout B;
 
 cudaError_t chee_decode_prot_locate(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
                                     uint64_t* launches) {
-    const cudaError_t e0 = prot_transfer_attr<T, true>();
-    if (e0 != cudaSuccess) return e0;
     return bounds::prot_locate_launch<T>(d_in, n_range, n_halo, ws, d_map, stream, launches);
 }
 

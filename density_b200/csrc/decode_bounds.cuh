@@ -726,6 +726,22 @@ inline size_t bounds_layout(size_t nbytes, size_t cap, BoundsLayout* L) {
     return off;
 }
 
+// Enqueues the candidate rows of the chunks of d_in[0 .. n_walk) into the res / gres arrays of L: dec_chunk_walk, whose walks see
+// n_visible >= n_walk bytes (a range map's halo is visible to the walks of the range's last chunk), then dec_group_compose. Nothing for
+// an empty walk. Returns the number of groups.
+template <class T>
+inline uint32_t rows_launch(const uint8_t* d_in, size_t n_walk, size_t n_visible, uint8_t* ws, const BoundsLayout& L, cudaStream_t stream,
+                            uint64_t* launches) {
+    const uint32_t nchunks = (uint32_t)((n_walk + T::CH - 1) / T::CH);
+    const uint32_t ngroups = (nchunks + GROUP - 1) / GROUP;
+    if (!nchunks) return 0;
+    uint32_t* res = reinterpret_cast<uint32_t*>(ws + L.res);
+    dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_visible, nchunks, res);
+    dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, reinterpret_cast<uint4*>(ws + L.gres));
+    *launches += 2;
+    return ngroups;
+}
+
 // Enqueues the boundary kernels. Afterwards (on the stream): st->main_blocks / tail_off / protection state, blk_off[0 .. main_blocks).
 // d_seed (may be null): the incoming state of a piece of a sharded stream (SEED_WORDS, read on the device); rows_ready: dec_chunk_walk and
 // dec_group_compose already filled res / gres for this input (dec_prot_transfer needed them first).
@@ -744,11 +760,7 @@ inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap,
     uint32_t* c_entry = reinterpret_cast<uint32_t*>(ws + L.c_entry);
     uint64_t* c_bb = reinterpret_cast<uint64_t*>(ws + L.c_blockbase);
     uint64_t* blk_off = reinterpret_cast<uint64_t*>(ws + L.blk_off);
-    if (!rows_ready) {
-        dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, nbytes, nchunks, res);
-        dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, gres);
-        *launches += 2;
-    }
+    if (!rows_ready) rows_launch<T>(d_in, nbytes, nbytes, ws, L, stream, launches);
     dec_top_walk<T><<<1, 32, 0, stream>>>(gres, ngroups, nbytes, g_entry, g_bb, st);
     dec_chunk_entries<T><<<(ngroups + 127) / 128, 128, 0, stream>>>(res, nchunks, g_entry, g_bb, ngroups, c_entry, c_bb, nullptr);
     dec_block_offsets<T><<<(nchunks + 127) / 128, 128, 0, stream>>>(d_in, nbytes, nchunks, c_entry, c_bb, blk_off, L.maxblocks, nullptr);
@@ -762,23 +774,67 @@ inline cudaError_t bounds_launch(const uint8_t* d_in, size_t nbytes, size_t cap,
     return cudaGetLastError();
 }
 
-// Enqueues the protected range map of d_in[0 .. n_range + n_halo) into d_map (PT_MAP_HDR + T::NCAND x PT_NCAND u32): the candidate rows
-// of the range's chunks (the halo visible to its last chunk's walks), as the quiet locate computes them, then one head walk per entry
-// offset. The scratch is the res / gres arrays of bounds_layout<T>(n_range + n_halo). dec_prot_transfer<T, true> must allow
-// prot_transfer_smem<T>() bytes of dynamic shared memory.
+// Enqueues the range map of d_in[0 .. n_range + n_halo) into map (DENSITY_B200_LOCATE_MAP_WORDS u64 for ChamT): the candidate rows of the
+// range's chunks, then their composition over the whole range. The scratch is the res / gres arrays of bounds_layout<T>(n_range + n_halo).
 template <class T>
-inline cudaError_t prot_locate_launch(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
-                                      uint64_t* launches) {
+inline void range_map_launch(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, unsigned long long* map, cudaStream_t stream,
+                             uint64_t* launches) {
     BoundsLayout B; bounds_layout<T>(n_range + n_halo, 0, &B);
-    uint32_t* res = reinterpret_cast<uint32_t*>(ws + B.res);
-    uint4* gres = reinterpret_cast<uint4*>(ws + B.gres);
-    const uint32_t nchunks = (uint32_t)((n_range + T::CH - 1) / T::CH);
-    if (nchunks) {
-        dec_chunk_walk<T><<<nchunks, 160, 0, stream>>>(d_in, n_range + n_halo, nchunks, res);
-        dec_group_compose<T><<<(nchunks + GROUP - 1) / GROUP, 160, 0, stream>>>(res, nchunks, gres);
-        *launches += 2;
+    const uint32_t ngroups = rows_launch<T>(d_in, n_range, n_range + n_halo, ws, B, stream, launches);
+    dec_range_compose<T><<<1, RC_THREADS, 0, stream>>>(reinterpret_cast<const uint4*>(ws + B.gres), ngroups, n_range, n_halo, map);
+    ++*launches;
+}
+
+// The dynamic shared memory of dec_prot_transfer<T, LOCATE>, allowed once per process. Static, as are the two launchers that call it: the
+// build has no relocatable device code, so every translation unit that launches dec_prot_transfer has its own copy of the kernel, whose
+// attribute it must set itself.
+template <class T, bool LOCATE>
+static cudaError_t prot_transfer_attr() {
+    static_assert(prot_transfer_smem<T>() <= 227u * 1024u, "the head walk's shared memory must fit in one SM");
+    static bool attr_done = false;
+    if (!attr_done) {
+        const cudaError_t e = cudaFuncSetAttribute(dec_prot_transfer<T, LOCATE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)prot_transfer_smem<T>());
+        if (e != cudaSuccess) return e;
+        attr_done = true;
     }
-    dec_prot_transfer<T, true><<<T::NCAND, PT_THREADS, prot_transfer_smem<T>(), stream>>>(d_in, n_range + n_halo, n_range, 0, res, gres, d_map);
+    return cudaSuccess;
+}
+
+// Enqueues the protection transfer of the piece d_in[0 .. n) (PT_NCAND words to d_transfer): the candidate rows of its chunks, which
+// stay in the res / gres arrays of bounds_layout<T>(n) for the seeded bounds_launch (rows_ready), then the head walk over them. An empty
+// piece reads nothing.
+template <class T>
+static cudaError_t prot_transfer_launch(const uint8_t* d_in, size_t n, int is_last, uint8_t* ws, uint32_t* d_transfer, cudaStream_t stream,
+                                        uint64_t* launches) {
+    const cudaError_t e = prot_transfer_attr<T, false>();
+    if (e != cudaSuccess) return e;
+    uint32_t* res = nullptr;
+    uint4* gres = nullptr;
+    if (n) {
+        BoundsLayout B; bounds_layout<T>(n, 0, &B);
+        res = reinterpret_cast<uint32_t*>(ws + B.res);
+        gres = reinterpret_cast<uint4*>(ws + B.gres);
+        rows_launch<T>(d_in, n, n, ws, B, stream, launches);
+    }
+    dec_prot_transfer<T, false><<<1, PT_THREADS, prot_transfer_smem<T>(), stream>>>(d_in, n, n, is_last, res, gres, d_transfer);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+// Enqueues the protected range map of d_in[0 .. n_range + n_halo) into d_map (PT_MAP_HDR + T::NCAND x PT_NCAND u32): the candidate rows
+// of the range's chunks, as range_map_launch computes them, then one head walk per entry offset. The scratch is the res / gres arrays of
+// bounds_layout<T>(n_range + n_halo).
+template <class T>
+static cudaError_t prot_locate_launch(const uint8_t* d_in, size_t n_range, size_t n_halo, uint8_t* ws, uint32_t* d_map, cudaStream_t stream,
+                                      uint64_t* launches) {
+    const cudaError_t e = prot_transfer_attr<T, true>();
+    if (e != cudaSuccess) return e;
+    BoundsLayout B; bounds_layout<T>(n_range + n_halo, 0, &B);
+    rows_launch<T>(d_in, n_range, n_range + n_halo, ws, B, stream, launches);
+    dec_prot_transfer<T, true><<<T::NCAND, PT_THREADS, prot_transfer_smem<T>(), stream>>>(d_in, n_range + n_halo, n_range, 0,
+                                                                                          reinterpret_cast<uint32_t*>(ws + B.res),
+                                                                                          reinterpret_cast<uint4*>(ws + B.gres), d_map);
     ++*launches;
     return cudaGetLastError();
 }

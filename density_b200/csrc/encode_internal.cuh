@@ -167,8 +167,8 @@ cudaError_t cham_decode_seam_words(const uint8_t* d_in, size_t nbytes, size_t ca
 // first), its incoming state composed from candidate x0 and the transfers of the pieces before it (DECODE_PROT_SEED_WORDS), and its seam
 // words after cham_decode_phase1 with that seed and cham_decode_phase2 (nbytes 0: an empty piece, the workspace is not read)
 constexpr uint32_t DECODE_PROT_TRANSFER_WORDS = 3200, DECODE_PROT_SEED_WORDS = 5;
-cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, uint32_t* d_transfer,
-                                      cudaStream_t stream, uint64_t* launches);
+cudaError_t cham_decode_prot_transfer(const uint8_t* d_in, size_t nbytes, uint8_t* ws, int is_last, uint32_t* d_transfer, cudaStream_t stream,
+                                      uint64_t* launches);
 cudaError_t cham_decode_prot_enter(const uint32_t* d_all_transfers, uint32_t rank, uint32_t x0, uint32_t* d_seed, cudaStream_t stream,
                                    uint64_t* launches);
 cudaError_t cham_decode_prot_seam_words(size_t nbytes, size_t cap, uint8_t* ws, int num_sms, int is_last, const uint32_t* d_seed, uint64_t* d_out_size,

@@ -377,7 +377,8 @@ typedef struct density_b200_decode_shard density_b200_decode_shard; /* opaque */
 DENSITY_B200_API density_b200_decode_shard* density_b200_decode_shard_create(void);
 DENSITY_B200_API void density_b200_decode_shard_destroy(density_b200_decode_shard*);
 /* phase 1: boundaries and writer pass; exports the piece's last-writer table (shard format, as density_b200_shard_phase1) to
-   d_table_out, including the PLAIN quads of the tail. cap = output capacity (sizes the boundary layout). */
+   d_table_out, including the PLAIN quads of the tail. cap = output capacity (sizes the boundary layout). Ends any piece in progress on
+   the shard, protected steps included. */
 DENSITY_B200_API int density_b200_decode_shard_phase1(density_b200_decode_shard*, const uint8_t* d_in, size_t n, size_t cap, int is_last_shard,
                                      uint32_t* d_table_out, void* stream);
 /* phase 2: d_carry_in = dictionary before this piece (the left fold of the earlier pieces' tables over density_b200_table_init's
@@ -460,7 +461,8 @@ DENSITY_B200_API int density_b200_cheetah_decode_round_budget(void);
 DENSITY_B200_API size_t density_b200_cheetah_cmap_words(void);
 /* phase 1: boundaries (the first piece from the fresh protection automaton, copy mode allowed), the end of the piece, unpack (literals and
    copy-mode blocks go to d_out at once), the symbolic chunk-map walk, and the piece's chunk-map transfer to d_cmap_out (may be NULL: no
-   export). is_first: the piece holds the stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3. */
+   export). is_first: the piece holds the stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3.
+   Ends any piece in progress on the shard, protected steps included. */
 DENSITY_B200_API int density_b200_cheetah_decode_shard_phase1(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n, uint8_t* d_out,
                                              size_t cap, int is_first, int is_last, uint32_t* d_cmap_out, void* stream);
 /* phase 2: d_cmap_carry = the chunk map before this piece (NULL = stream start). Resolves the chunk-map reads, initialises the contexts. */
@@ -539,7 +541,8 @@ DENSITY_B200_API density_b200_lion_decode_shard* density_b200_lion_decode_shard_
 DENSITY_B200_API void density_b200_lion_decode_shard_destroy(density_b200_lion_decode_shard*);
 /* phase 1: boundaries (the first piece from the fresh protection automaton, copy mode allowed), the end of the piece, unpack, the
    symbolic chunk-map walk and the piece's chunk-map transfer to d_cmap_out (may be NULL: no export). is_first: the piece holds the
-   stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3. */
+   stream start; is_last: no stream byte follows it. d_in and d_out must stay valid until phase 3. Ends any piece in progress on the
+   shard, protected steps included. */
 DENSITY_B200_API int density_b200_lion_decode_shard_phase1(density_b200_lion_decode_shard*, const uint8_t* d_in, size_t n, uint8_t* d_out,
                                           size_t cap, int is_first, int is_last, uint32_t* d_cmap_out, void* stream);
 /* phase 2: d_cmap_carry = the chunk map before this piece (NULL = stream start). Resolves the reads of carried-in chunk-map slots. */
@@ -588,7 +591,7 @@ DENSITY_B200_API int density_b200_decode_sharded_lion_protected(density_b200_sha
  */
 #define DENSITY_B200_LOCATE_MAP_WORDS 266
 /* Enqueues the range map of d_in[0 .. n_range + n_halo) into d_map (device, 8-byte aligned). The scratch lives in the handle's
-   workspace, which the next phase 1 overwrites. The layout is not checked here but by density_b200_locate_piece, which every rank
+   workspace, which the next phase 1 overwrites, so the call ends any piece in progress on the shard, protected steps included. The layout is not checked here but by density_b200_locate_piece, which every rank
    runs on the same gathered maps. */
 DENSITY_B200_API int density_b200_decode_locate(density_b200_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
                                 uint64_t* d_map, void* stream);
@@ -623,8 +626,8 @@ DENSITY_B200_API int density_b200_decode_sharded_stream(density_b200_sharded*, c
 #define DENSITY_B200_CHEETAH_LOCATE_MAP_WORDS 142
 /* Enqueues the range map of d_in[0 .. n_range + n_halo) into d_map (device, 8-byte aligned). Kernels: 4 on a range without the stream
    start (2 when it is empty), 11 on the range with it (the 9 boundary kernels of the exact walk, the identity rows, the start row).
-   The scratch lives in the handle's workspace, which the next phase 1 overwrites; on the start range it holds one offset per 8 stream
-   bytes. The layout is checked by density_b200_cheetah_locate_piece. */
+   The scratch lives in the handle's workspace, which the next phase 1 overwrites, so the call ends any piece in progress on the shard,
+   protected steps included; on the start range it holds one offset per 8 stream bytes. The layout is checked by density_b200_cheetah_locate_piece. */
 DENSITY_B200_API int density_b200_cheetah_decode_locate(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
                                         uint64_t range_offset, uint64_t* d_map, void* stream);
 /* Host only, needs no device. h_maps: the Cheetah range maps of all `world` ranks in rank order. Checks the layout as
@@ -664,7 +667,7 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah_stream(density_b200_sha
 #define DENSITY_B200_CHEETAH_PROT_LOCATE_MAP_WORDS 217604
 /* Enqueue the protected range map of d_in[0 .. n_range + n_halo) (2-byte aligned) into d_map (device, 4-byte aligned): the candidate
    rows of the quiet locate, then one head walk per entry offset (132 / 68 CTAs). The scratch lives in the shard's workspace, which the
-   next phase 1 overwrites. The layout is checked by density_b200_prot_locate_piece. */
+   next phase 1 overwrites, so the call ends any piece in progress on the shard, protected steps included. The layout is checked by density_b200_prot_locate_piece. */
 DENSITY_B200_API int density_b200_decode_prot_locate(density_b200_decode_shard*, const uint8_t* d_in, size_t n_range, size_t n_halo,
                                      uint32_t* d_map, void* stream);
 DENSITY_B200_API int density_b200_cheetah_decode_prot_locate(density_b200_cheetah_decode_shard*, const uint8_t* d_in, size_t n_range,

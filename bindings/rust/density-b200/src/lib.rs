@@ -33,6 +33,9 @@ unsafe extern "C" {
     // device-resident, stream-ordered
     pub fn density_b200_encode_device(alg: c_int, d_in: *const u8, n: usize, d_out: *mut u8, cap: usize, d_out_size: *mut u64, stream: *mut c_void) -> c_int;
     pub fn density_b200_decode_device(alg: c_int, d_in: *const u8, n: usize, d_out: *mut u8, cap: usize, d_out_size: *mut u64, stream: *mut c_void) -> c_int;
+    // the length a stream decodes to, without decoding it: {size, verdict} to d_result (device) / DENSITY_B200_OK with *out_size
+    pub fn density_b200_decoded_size_device(alg: c_int, d_in: *const u8, n: usize, d_result: *mut u64, stream: *mut c_void) -> c_int;
+    pub fn density_b200_decoded_size(alg: c_int, input: *const u8, n: usize, out_size: *mut u64) -> c_int;
     // a reused Codec instance (codec.rs:16,72,82)
     pub fn density_b200_codec_create(alg: c_int) -> *mut RawCodec;
     pub fn density_b200_codec_destroy(codec: *mut RawCodec);
@@ -74,6 +77,13 @@ macro_rules! algorithm {
             pub fn decode(input: &[u8], output: &mut [u8]) -> Result<usize, DecodeError> {
                 let n = unsafe { $dec(input.as_ptr(), input.len(), output.as_mut_ptr(), output.len()) };
                 if n == 0 && !input.is_empty() { Err(DecodeError {}) } else { Ok(n) }
+            }
+            /// The output capacity `decode` needs for `input`: the bytes it decodes to, from the block boundaries without decoding.
+            /// `Err` where `decode` fails at any capacity (a malformed stream) or the library could not run.
+            pub fn decoded_size(input: &[u8]) -> Result<usize, DecodeError> {
+                let mut size: u64 = 0;
+                let rc = unsafe { density_b200_decoded_size($id, input.as_ptr(), input.len(), &mut size) };
+                if rc == 0 { usize::try_from(size).map_err(|_| DecodeError {}) } else { Err(DecodeError {}) }
             }
         }
         impl Drop for $name {

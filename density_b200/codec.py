@@ -15,6 +15,7 @@ import numpy as np
 from . import _lib
 
 ALG_IDS = {"chameleon": 0, "cheetah": 1, "lion": 2}
+_EMALFORMED = 3     # DENSITY_B200_EMALFORMED
 
 
 class EncodeError(Exception):
@@ -97,6 +98,19 @@ class _Codec:
             raise DecodeError(_lib.last_error() or "decode failed")
         return r
 
+    @classmethod
+    def decoded_size(cls, input):
+        """The number of bytes `decode` writes for `input` (host buffer or torch CUDA tensor), found from the block boundaries without
+        decoding. Raises DecodeError when the stream is malformed (decode would fail at any capacity)."""
+        ip, n, k1 = _ptr_len(input)
+        size = ctypes.c_uint64(0)
+        rc = _lib.load().density_b200_decoded_size(ALG_IDS[cls.NAME], ip, n, ctypes.byref(size))
+        if rc == _EMALFORMED:
+            raise DecodeError(_lib.last_error() or "malformed stream")
+        if rc != 0:
+            raise _lib.DensityB200Error(f"density_b200_decoded_size rc={rc}: {_lib.last_error()}")
+        return size.value
+
     # convenience: bytes in, bytes out
     @classmethod
     def encode_bytes(cls, data):
@@ -106,8 +120,11 @@ class _Codec:
         return out[:n].tobytes()
 
     @classmethod
-    def decode_bytes(cls, data, original_size):
+    def decode_bytes(cls, data, original_size=None):
+        """original_size None: the size comes from decoded_size (an extra pass over the block boundaries)."""
         a = np.frombuffer(bytes(data), dtype=np.uint8) if not isinstance(data, np.ndarray) else data
+        if original_size is None:
+            original_size = cls.decoded_size(a)
         out = np.empty(max(1, original_size), dtype=np.uint8)
         n = cls.decode(a, out)
         return out[:n].tobytes()
@@ -197,3 +214,13 @@ def decode_device(alg, d_in, n_in, d_out, d_out_size, stream=None, path=0):
                                            d_out_size.data_ptr(), _stream_handle(stream), path)
     if rc != 0:
         raise DecodeError(f"density_b200_decode_device rc={rc}: {_lib.last_error()}")
+
+
+def decoded_size_device(alg, d_in, n_in, d_result, stream=None):
+    """Enqueue the decoded-size query of the first `n_in` bytes of CUDA uint8 tensor `d_in` on `stream` (default: torch's current
+    stream). `d_result` is a CUDA int64/uint64 tensor of two elements that receives {decoded size, verdict}, verdict 0 or 3
+    (DENSITY_B200_EMALFORMED, size 0). No synchronisation."""
+    L = _lib.load()
+    rc = L.density_b200_decoded_size_device(ALG_IDS[alg], d_in.data_ptr(), n_in, d_result.data_ptr(), _stream_handle(stream))
+    if rc != 0:
+        raise DecodeError(f"density_b200_decoded_size_device rc={rc}: {_lib.last_error()}")

@@ -626,6 +626,72 @@ int density_b200_decode_device_path(int alg, const uint8_t* d_in, size_t n, uint
     return device_entry(false, alg, d_in, n, d_out, cap, d_out_size, stream, path);
 }
 
+// ---- decoded size (decoded_size.cu) -------------------------------------------------------------------------------------------
+// n > 0, d_in 2-byte aligned; on the device's workspace like decode_device
+static int decoded_size_locked(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint64_t* d_result, cudaStream_t stream) {
+    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    cudaError_t e = c->ws.ensure(decoded_size_workspace_bytes(alg, n), stream);
+    if (e != cudaSuccess) { ws_release(c, stream); set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    e = decoded_size_launch(alg, d_in, n, c->ws.p, d_result, stream, &launches);
+    ws_release(c, stream);
+    return step_result(e, launches, "decoded size launch");
+}
+
+int density_b200_decoded_size_device(int alg, const uint8_t* d_in, size_t n, uint64_t* d_result, void* stream) {
+    g_last_error.clear();
+    if (alg < 0 || alg > 2) { set_error("bad algorithm id"); return DENSITY_B200_EARG; }
+    if (!d_result || (!d_in && n)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_result) & 7)) {
+        set_error("decoded_size_device: d_in must be 2-byte and d_result 8-byte aligned");
+        return DENSITY_B200_EARG;
+    }
+    DeviceCtx* c = current_ctx();
+    if (!c) return DENSITY_B200_ECUDA;
+    std::lock_guard<std::mutex> lk(c->mu);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (n == 0) {      // codec.rs:102: an empty stream decodes to nothing; no kernel
+        const cudaError_t e = cudaMemsetAsync(d_result, 0, 2 * sizeof(uint64_t), s);
+        if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
+        return DENSITY_B200_OK;
+    }
+    return decoded_size_locked(c, alg, d_in, n, d_result, s);
+}
+
+int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t* out_size) {
+    g_last_error.clear();
+    if (alg < 0 || alg > 2) { set_error("bad algorithm id"); return DENSITY_B200_EARG; }
+    if (!out_size || (!input && n)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (n == 0) { *out_size = 0; return DENSITY_B200_OK; }
+    DeviceCtx* c = current_ctx();
+    if (!c) return DENSITY_B200_ECUDA;
+    std::lock_guard<std::mutex> lk(c->mu);
+    const bool in_dev = is_device_pointer(input);
+    cudaError_t e;
+    if (in_dev) {
+        // synchronous, and it cannot know which stream produced the buffer: wait for all of them (as run_sync)
+        e = cudaDeviceSynchronize();
+        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return DENSITY_B200_ECUDA; }
+    }
+    const uint8_t* d_in = input;
+    if (!in_dev || (reinterpret_cast<uintptr_t>(input) & 1)) {     // host buffers, and device buffers at an odd address, go through stage_in
+        e = c->stage_in.ensure(n + 16, c->stream);
+        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        e = in_dev ? cudaMemcpyAsync(c->stage_in.p, input, n, cudaMemcpyDeviceToDevice, c->stream)
+                   : h2d_any(c->ring_in, c->stage_in.p, input, n, c->stream, is_pageable_host(input));
+        if (e != cudaSuccess) { set_error("input copy", e); return DENSITY_B200_ECUDA; }
+        d_in = c->stage_in.p;
+    }
+    const int rc = decoded_size_locked(c, alg, d_in, n, c->d_size, c->stream);
+    if (rc != DENSITY_B200_OK) { cudaStreamSynchronize(c->stream); return rc; }
+    e = cudaMemcpyAsync(c->h_size, c->d_size, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) { set_error("stream sync", e); return DENSITY_B200_ECUDA; }
+    if (c->h_size[1] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
+    *out_size = c->h_size[0];
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon encode ------------------------------------------------------------------------
 struct density_b200_shard {
     DevBuf ws;

@@ -482,62 +482,9 @@ __global__ void dec_tail(const uint8_t* __restrict__ in, uint64_t n, uint8_t* __
 }
 
 // ---- 5. sharded decode: a piece's exported table and its seam words ----------------------------------------------------------
-// The tail's blocks as dec_tail goes through them, without output: plain(q) sees every PLAIN quad in stream order. The control flow
-// does not depend on the dictionary, so this runs before the carry-in is known.
-struct TailWalk {
-    uint64_t blocks;        // blocks the tail loop entered (copy-mode, encoded, partial)
-    uint32_t first_inc;     // the first tail block is a complete incompressible block
-    uint32_t copied, bad;   // a copy-mode block; a malformed block
-    Protection ps;          // protection state when the tail loop stops
-};
-template <class F>
-__device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
-    TailWalk w; w.blocks = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
-    Protection& ps = w.ps;
-    ps = bounds::main_end_state(st);
-    uint64_t idx = st->tail_off;
-    while (n - idx > 0) {
-        ++w.blocks;
-        if (ps.revert_to_copy()) {
-            w.copied = 1;
-            const uint64_t rem = n - idx;
-            idx += rem > 256 ? 256 : rem;
-            if (rem <= 256) break;
-            ps.decay();
-            continue;
-        }
-        const uint64_t mark = idx;
-        if (n - idx < 8) { w.bad = 1; break; }
-        uint64_t sig = 0;
-        for (int i = 0; i < 8; ++i) sig |= (uint64_t)in[idx + i] << (8 * i);
-        idx += 8;
-        bool end = false;
-        for (int u = 0; u < 32 && !end && !w.bad; ++u) {
-            const bool checked = (n - idx) < 8;
-            for (int k = 0; k < 2 && !end; ++k) {
-                const uint32_t fl = (uint32_t)(sig & 1); sig >>= 1;
-                if (checked && fl == 0) {
-                    const uint64_t rem = n - idx;
-                    if (rem == 0) { end = true; break; }
-                    if (rem < 4) { idx = n; end = true; break; }
-                }
-                if (fl) {
-                    if (n - idx < 2) { w.bad = 1; break; }
-                    idx += 2;
-                } else {
-                    if (n - idx < 4) { w.bad = 1; break; }
-                    plain(in[idx] | (in[idx + 1] << 8) | (in[idx + 2] << 16) | ((uint32_t)in[idx + 3] << 24));
-                    idx += 4;
-                }
-            }
-        }
-        if (end || w.bad) break;
-        const bool inc = idx - mark >= 256;
-        if (w.blocks == 1) w.first_inc = inc ? 1u : 0u;
-        ps.update(inc);
-    }
-    return w;
-}
+// The tail's control flow: bounds::tail_walk (decode_bounds.cuh).
+using bounds::TailWalk;
+using bounds::tail_walk;
 
 // The piece's exported table: the left fold of its run tables (writer pass) ...
 __global__ void dec_export_fold(const uint32_t* __restrict__ final_tab, uint32_t nruns, uint32_t* __restrict__ table_out) {

@@ -702,6 +702,66 @@ __device__ __forceinline__ Protection main_end_state(const DecStatus* __restrict
     return ps;
 }
 
+// Chameleon's tail loop (codec.rs:102-123, chameleon_decode.cu dec_tail) as it goes through the tail's blocks, without output: plain(q)
+// sees every PLAIN quad in stream order, `out` counts the bytes dec_tail writes. The control flow does not depend on the dictionary, so
+// this runs before the carry-in is known (sharded decode) or without any dictionary at all (the decoded-size query).
+struct TailWalk {
+    uint64_t blocks;        // blocks the tail loop entered (copy-mode, encoded, partial)
+    uint64_t out;           // bytes the tail decodes to (meaningless when bad)
+    uint32_t first_inc;     // the first tail block is a complete incompressible block
+    uint32_t copied, bad;   // a copy-mode block; a malformed block
+    Protection ps;          // protection state when the tail loop stops
+};
+template <class F>
+__device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
+    TailWalk w; w.blocks = 0; w.out = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
+    Protection& ps = w.ps;
+    ps = main_end_state(st);
+    uint64_t idx = st->tail_off;
+    while (n - idx > 0) {
+        ++w.blocks;
+        if (ps.revert_to_copy()) {
+            w.copied = 1;
+            const uint64_t rem = n - idx, len = rem > 256 ? 256 : rem;
+            idx += len; w.out += len;
+            if (rem <= 256) break;
+            ps.decay();
+            continue;
+        }
+        const uint64_t mark = idx;
+        if (n - idx < 8) { w.bad = 1; break; }
+        uint64_t sig = 0;
+        for (int i = 0; i < 8; ++i) sig |= (uint64_t)in[idx + i] << (8 * i);
+        idx += 8;
+        bool end = false;
+        for (int u = 0; u < 32 && !end && !w.bad; ++u) {
+            const bool checked = (n - idx) < 8;
+            for (int k = 0; k < 2 && !end; ++k) {
+                const uint32_t fl = (uint32_t)(sig & 1); sig >>= 1;
+                if (checked && fl == 0) {
+                    const uint64_t rem = n - idx;
+                    if (rem == 0) { end = true; break; }
+                    if (rem < 4) { idx = n; w.out += rem; end = true; break; }
+                }
+                if (fl) {
+                    if (n - idx < 2) { w.bad = 1; break; }
+                    idx += 2;
+                } else {
+                    if (n - idx < 4) { w.bad = 1; break; }
+                    plain(in[idx] | (in[idx + 1] << 8) | (in[idx + 2] << 16) | ((uint32_t)in[idx + 3] << 24));
+                    idx += 4;
+                }
+                w.out += 4;
+            }
+        }
+        if (end || w.bad) break;
+        const bool inc = idx - mark >= 256;
+        if (w.blocks == 1) w.first_inc = inc ? 1u : 0u;
+        ps.update(inc);
+    }
+    return w;
+}
+
 // ---- host side: workspace layout + launch sequence ---------------------------------------------------------------------------------
 struct BoundsLayout { size_t status, res, gres, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, total; uint64_t maxblocks; };
 

@@ -251,4 +251,10 @@ cudaError_t scalar_decode(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* 
 cudaError_t scalar_decode_tail(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* d_out, size_t cap, uint8_t* ws, const void* d_bounds_status,
                                const void* d_cl_status, uint64_t* d_out_size, cudaStream_t stream, uint64_t* launches, const uint32_t* d_skip_if);
 
+// decoded_size.cu: the length a stream decodes to, without decoding it; d_in 2-byte aligned, nbytes > 0. Writes {size, 0} or
+// {0, DENSITY_B200_EMALFORMED} to d_result (2 x u64) in stream order; 4 kernels; scratch in `ws`, decoded_size_workspace_bytes(alg, nbytes)
+size_t decoded_size_workspace_bytes(int alg, size_t nbytes);
+cudaError_t decoded_size_launch(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* ws, uint64_t* d_result, cudaStream_t stream,
+                                uint64_t* launches);
+
 }  // namespace dns

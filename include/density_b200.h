@@ -124,6 +124,23 @@ DENSITY_B200_API int density_b200_lion_decode_stats(uint64_t* out4);
 /* Same contract for decode; `cap` must be >= the original length. */
 DENSITY_B200_API int density_b200_decode_device(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                uint64_t* d_out_size, void* stream);
+/*
+ * Decoded size: the number of bytes X::decode writes for a stream (the original length of an encoded input), found from the block
+ * boundaries without decoding it. A stream does not record its length; this gives every decode entry point above the capacity it needs
+ * for streams whose length the caller did not keep. Equivalent to decode for every byte string, whether or not an encoder wrote it:
+ * a size s means decode with cap = s writes s bytes (and with cap = s - 1 writes 0); DENSITY_B200_EMALFORMED means decode writes 0 at
+ * any capacity (the stream ends inside a block). A non-empty stream may decode to 0 bytes, hence the separate verdict.
+ * Workspace: the boundary rows of the stream (3-7 % of n), independent of the decoded size; no output buffer.
+ * Both calls use the device's shared workspace (see "Concurrent callers" above).
+ *
+ * Stream-ordered: d_in device, 2-byte aligned; d_result device, 8-byte aligned, receives two u64 {decoded size, verdict}, verdict 0 or
+ * DENSITY_B200_EMALFORMED (then the size word is 0). n > 0: 4 kernels (the candidate rows, the in-order block walk, the tail); n == 0:
+ * no kernel, {0, 0} by a memset. DENSITY_B200_EARG (a bad algorithm id, a NULL pointer, a misaligned d_in or d_result) enqueues nothing.
+ */
+DENSITY_B200_API int density_b200_decoded_size_device(int alg, const uint8_t* d_in, size_t n, uint64_t* d_result, void* stream);
+/* Synchronous; host or device pointer of any alignment, like the nine reference symbols. DENSITY_B200_OK with *out_size set,
+   DENSITY_B200_EMALFORMED, DENSITY_B200_EARG or DENSITY_B200_ECUDA. */
+DENSITY_B200_API int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t* out_size);
 
 /*
  * Sharded Chameleon encode (one bit-exact stream cut across several GPUs / calls; SURVEY §8e).

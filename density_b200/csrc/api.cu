@@ -692,19 +692,76 @@ int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t*
     return DENSITY_B200_OK;
 }
 
+// ---- the argument rule of the sharded entries (include/density_b200.h, "Sharded encode" and "Sharded decode"). Each helper returns
+// DENSITY_B200_EARG with the error set, or DENSITY_B200_OK.
+static bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+static bool al8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+// the input and the output of a shard or a piece; either may be null when its length is 0. Decode: d_in 2-byte, d_out 4-byte aligned.
+// Encode: d_in 4-byte, d_out 2-byte aligned, and a shard that does not end the stream (!is_last) a multiple of 256 bytes.
+static int in_args(bool encode, const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap, bool is_last = true) {
+    if ((!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (encode && !is_last && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_in), out = reinterpret_cast<uintptr_t>(d_out);
+    if (encode && ((in & 3) || (out & 1))) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (!encode && ((in & 1) || (out & 3))) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+// tables, transfers, carries, words and flags, null where the entry allows it (the caller checks that)
+static int table_args(std::initializer_list<const void*> tables) {
+    for (const void* t : tables)
+        if (!al4(t)) { set_error("tables, transfers, carries, words and flags must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+// the sizes an entry writes: d_out_size (not null) and d_total_size (null where the entry allows it), both 8-byte aligned
+static int size_args(const uint64_t* d_out_size, const uint64_t* d_total_size = nullptr) {
+    if (!d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!al8(d_out_size) || !al8(d_total_size)) { set_error("d_out_size and d_total_size must be 8-byte aligned"); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+// the size and the seam words a shard or a piece writes
+static int out_args(const uint64_t* d_out_size, const uint32_t* d_seam8) {
+    if (!d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    const int rc = size_args(d_out_size);
+    return rc == DENSITY_B200_OK ? table_args({d_seam8}) : rc;
+}
+// the order rule of every sharded encode entry: s is not null, its stage is one of `stages` and it has committed at least min_round
+// rounds; otherwise the error `what`
+extern "C++" {
+template <class S> static bool in_stage(const S* s, std::initializer_list<int> stages, const char* what, int min_round = 0) {
+    if (s && s->round >= min_round)
+        for (int k : stages) if (s->stage == k) return true;
+    set_error(what);
+    return false;
+}
+}
+// after a commit (waits for the device): words 2 .. 19 of the status of a shard's copy-map iteration from its device record, which
+// lands in *h for the caller's words 0 and 1
+static int prot_status_read(const DevBuf& rec, uint32_t* out, ProtShard* h, const char* what) {
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(h, rec.p, sizeof *h, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error(what, e); return DENSITY_B200_ECUDA; }
+    out[3] = h->esc;
+    const uint32_t c = h->in_state;   // pc_encode candidate -> penalty | start << 8 | previous_incompressible << 16
+    out[2] = c >= PROT_TRANSFER_WORDS ? 0xFFFFFFFFu : (c % 10) | (((c / 10) % 10 + 1) << 8) | ((c / 100) << 16);
+    for (int k = 0; k < 16; ++k) out[4 + k] = h->changed[k];
+    return DENSITY_B200_OK;
+}
+
 // ---- sharded Chameleon encode ------------------------------------------------------------------------
 struct density_b200_shard {
+    // PHASE1: the quiet phase 1 done (phase 2 may follow, any number of times). The copy-map iteration of density_b200_shard_prot_*:
+    // FLAGS after prot_phase1 or prot_next with a table, then TRANSFER, SETTLED, COMMITTED (prot_next without a table), FINISHED.
+    enum { NONE, PHASE1, FLAGS, TRANSFER, SETTLED, COMMITTED, FINISHED };
     DevBuf ws;
+    DevBuf prot;                    // the device record of the copy-map iteration (ProtShard)
     ChamLayout L{};
     const uint8_t* d_in = nullptr;
     size_t n = 0;
     uint32_t nruns = 0;
     int num_sms = 0;
-    bool phase1_done = false;
-    // the copy-map iteration of density_b200_shard_prot_*: the shard's device record and where the phases stand
-    DevBuf prot;
-    int prot_phase = 0;             // 0 none, 1 flags ready (phase 1 / next with a table), 2 transfer, 3 settle, 4 committed, 5 finished
-    int round = 0;
+    int stage = NONE;
+    int round = 0;                  // the rounds of the copy-map iteration that went on to the next
+    ~density_b200_shard() { ws.release(); prot.release(); }
 };
 
 // a phase object of the sharded API for the current device (NULL, with the error set, without one)
@@ -719,31 +776,31 @@ template <class S> static S* new_shard() {
 }
 }
 density_b200_shard* density_b200_shard_create(void) { return new_shard<density_b200_shard>(); }
-void density_b200_shard_destroy(density_b200_shard* s) {
-    if (!s) return;
-    s->ws.release();
-    s->prot.release();
-    delete s;
+void density_b200_shard_destroy(density_b200_shard* s) { delete s; }
+
+// the shard d_in[0 .. n) set up in s (phase 1 and prot_phase1): every step of the shard before it void, the workspace and with_prot the
+// iteration's record ensured, the shard stored
+static int cham_shard_setup(density_b200_shard* s, const uint8_t* d_in, size_t n, bool with_prot, cudaStream_t st) {
+    s->stage = density_b200_shard::NONE;
+    cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);
+    if (e == cudaSuccess && with_prot) e = s->prot.ensure(sizeof(ProtShard), st);
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    s->d_in = d_in; s->n = n; s->nruns = cham_pick_runs(n, s->num_sms);
+    return DENSITY_B200_OK;
 }
 int density_b200_shard_phase1(density_b200_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_in) & 3) { set_error("d_in must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->prot_phase = 0;              // the workspace is this phase's now: the copy-map phases start over with prot_phase1
-    size_t need = cham_workspace_bytes(n, s->num_sms, &s->L);
-    cudaError_t e = s->ws.ensure(need, st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->nruns = cham_pick_runs(n, s->num_sms);
+    int rc = in_args(true, d_in, n, nullptr, 0, is_last_shard);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_table_out});
+    if (rc == DENSITY_B200_OK) rc = cham_shard_setup(s, d_in, n, false, st);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    if (n == 0) {
-        e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
-    } else {
-        e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, d_table_out, st, &launches);
-    }
-    const int rc = step_result(e, launches, "shard phase1");
-    if (rc == DENSITY_B200_OK) s->phase1_done = true;
+    const cudaError_t e = n ? cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, d_table_out, st, &launches)
+                            : cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);  // nothing touched
+    rc = step_result(e, launches, "shard phase1");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_shard::PHASE1;
     return rc;
 }
 // phase 2 on the shard's workspace: carry-in, first-touch flags, sizes, scan, emit. assume_prev_inc: the block before the shard counts
@@ -758,10 +815,13 @@ static int shard_phase2_impl(density_b200_shard* s, const uint32_t* d_carry_in, 
 int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                               uint32_t* d_flags, void* stream) {
     g_last_error.clear();
-    if (!s || !s->phase1_done || !d_out_size) { set_error("shard_phase2: phase1 not done / null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_shard::PHASE1}, "shard_phase2: null pointer / phase1 not done")) return DENSITY_B200_EARG;
+    int rc = in_args(true, nullptr, 0, d_out, 0);       // d_out's alignment; phase 2 takes a NULL d_out at any capacity
+    if (rc == DENSITY_B200_OK) rc = table_args({d_carry_in, d_flags});
+    if (rc == DENSITY_B200_OK) rc = size_args(d_out_size);
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int rc = shard_phase2_impl(s, d_carry_in, d_out, cap, d_out_size, d_carry_in != nullptr, nullptr, st);
+    rc = shard_phase2_impl(s, d_carry_in, d_out, cap, d_out_size, d_carry_in != nullptr, nullptr, st);
     if (rc != DENSITY_B200_OK || !d_flags) return rc;
     const cudaError_t e = s->n ? cudaMemcpyAsync(d_flags, s->ws.p + s->L.status + offsetof(Status, nonquiet), sizeof(uint32_t),
                                                  cudaMemcpyDeviceToDevice, st)
@@ -771,7 +831,6 @@ int density_b200_shard_phase2(density_b200_shard* s, const uint32_t* d_carry_in,
 
 // ---- sharded Chameleon encode with copy mode: the copy-map iteration carried over the cuts ---------------------------------------------
 static int g_prot_rounds = (int)PROT_MAX_ROUNDS;   // round budget (density_b200_test_set_prot_rounds)
-static bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 static ProtShard* prot_rec(density_b200_shard* s) { return reinterpret_cast<ProtShard*>(s->prot.p); }
 
 int density_b200_prot_round_budget(void) { return g_prot_rounds; }
@@ -780,34 +839,31 @@ void density_b200_test_set_prot_rounds(int k) { g_prot_rounds = (k >= 1 && k <= 
 // first_block = ~0: taken from d_lengths (the gathered shard lengths) on the device instead
 static int prot_phase1_impl(density_b200_shard* s, const uint8_t* d_in, size_t n, uint64_t first_block, const uint64_t* d_lengths, int rank,
                             int is_last_shard, uint32_t* d_table_out, cudaStream_t st) {
-    if (!s || (!d_in && n) || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if (!al4(d_in) || !al4(d_table_out)) { set_error("d_in and d_table_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);
-    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    s->d_in = d_in; s->n = n; s->nruns = cham_pick_runs(n, s->num_sms);
-    s->phase1_done = false; s->prot_phase = 0; s->round = 0;
+    if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = in_args(true, d_in, n, nullptr, 0, is_last_shard);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_table_out});
+    if (rc == DENSITY_B200_OK) rc = cham_shard_setup(s, d_in, n, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    s->round = 0;
     uint64_t launches = 0;
-    e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, n ? d_table_out : nullptr, st, &launches);
+    cudaError_t e = cham_encode_phase1(d_in, n, s->ws.p, s->L, s->nruns, n ? d_table_out : nullptr, st, &launches);
     if (e == cudaSuccess && !n) e = cudaMemsetAsync(d_table_out, 0, 65536 * sizeof(uint32_t), st);   // nothing touched
     if (e == cudaSuccess) e = cham_prot_start(s->ws.p, s->L, prot_rec(s), d_lengths ? 0 : first_block, d_lengths, (uint32_t)rank, st, &launches);
-    const int rc = step_result(e, launches, "shard prot phase1");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 1;
+    rc = step_result(e, launches, "shard prot phase1");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_shard::FLAGS;
     return rc;
 }
 // ev (may be NULL): the stage events of cham_encode_phase2
 static int prot_finish_impl(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st,
                             cudaEvent_t* ev) {
-    if (!s || (!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 4) { set_error("shard_prot_finish: call it after prot_next without a table"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_out) & 1) || (reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) {
-        set_error("d_out must be 2-byte, d_out_size 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG;
-    }
+    if (!in_stage(s, {density_b200_shard::COMMITTED}, "shard_prot_finish: call it after prot_next without a table")) return DENSITY_B200_EARG;
+    int rc = in_args(true, nullptr, 0, d_out, cap);
+    if (rc == DENSITY_B200_OK) rc = out_args(d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
     const cudaError_t e = cham_prot_finish(s->d_in, s->n, s->ws.p, s->L, prot_rec(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev);
-    const int rc = step_result(e, launches, "shard prot finish");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 5;
+    rc = step_result(e, launches, "shard prot finish");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_shard::FINISHED;
     return rc;
 }
 
@@ -819,43 +875,43 @@ int density_b200_shard_prot_phase1(density_b200_shard* s, const uint8_t* d_in, s
 }
 int density_b200_shard_prot_transfer(density_b200_shard* s, const uint32_t* d_carry_in, uint32_t* d_transfer_out, void* stream) {
     g_last_error.clear();
-    if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 1) { set_error("shard_prot_transfer: call it after prot_phase1 or prot_next with a table"); return DENSITY_B200_EARG; }
-    if (!al4(d_carry_in) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_shard::FLAGS}, "shard_prot_transfer: call it after prot_phase1 or prot_next with a table")) return DENSITY_B200_EARG;
+    if (!d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (table_args({d_carry_in, d_transfer_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
     const cudaError_t e = cham_prot_transfer(s->n, s->ws.p, s->L, s->nruns, d_carry_in, prot_rec(s), s->round, d_transfer_out,
                                              reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "shard prot transfer");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 2;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_shard::TRANSFER;
     return rc;
 }
 int density_b200_shard_prot_settle(density_b200_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out, void* stream) {
     g_last_error.clear();
-    if (!s || !d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 2) { set_error("shard_prot_settle: call it after prot_transfer"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_shard::TRANSFER}, "shard_prot_settle: call it after prot_transfer")) return DENSITY_B200_EARG;
+    if (!d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (table_args({d_all_transfers, d_words_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
     const cudaError_t e = cham_prot_settle(s->n, s->ws.p, s->L, prot_rec(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out,
                                            reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "shard prot settle");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 3;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_shard::SETTLED;
     return rc;
 }
 int density_b200_shard_prot_next(density_b200_shard* s, const uint32_t* d_all_words, int world, uint32_t* d_table_out, void* stream) {
     g_last_error.clear();
-    if (!s || !d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (s->prot_phase != 3) { set_error("shard_prot_next: call it after prot_settle"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_shard::SETTLED}, "shard_prot_next: call it after prot_settle")) return DENSITY_B200_EARG;
+    if (!d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_words) || !al4(d_table_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (table_args({d_all_words, d_table_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     if (d_table_out && s->round + 1 >= g_prot_rounds) { set_error("shard_prot_next: the round budget is used up"); return DENSITY_B200_EARG; }
     uint64_t launches = 0;
     const cudaError_t e = cham_prot_next(s->d_in, s->n, s->ws.p, s->L, s->nruns, prot_rec(s), s->round, d_all_words, (uint32_t)world,
                                          d_table_out, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "shard prot next");
     if (rc != DENSITY_B200_OK) return rc;
-    if (d_table_out) { ++s->round; s->prot_phase = 1; }
-    else s->prot_phase = 4;
+    if (d_table_out) { ++s->round; s->stage = density_b200_shard::FLAGS; }
+    else s->stage = density_b200_shard::COMMITTED;
     return DENSITY_B200_OK;
 }
 int density_b200_shard_prot_finish(density_b200_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
@@ -864,33 +920,27 @@ int density_b200_shard_prot_finish(density_b200_shard* s, uint8_t* d_out, size_t
 }
 int density_b200_shard_prot_status(density_b200_shard* s, uint32_t* out) {
     g_last_error.clear();
-    if (!s || !out || s->prot_phase < 4) { set_error("shard_prot_status: null pointer / rounds not committed"); return DENSITY_B200_EARG; }
+    if (!out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_shard::COMMITTED, density_b200_shard::FINISHED}, "shard_prot_status: rounds not committed")) return DENSITY_B200_EARG;
     ProtShard h{};
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(&h, s->prot.p, sizeof h, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error("shard_prot_status", e); return DENSITY_B200_ECUDA; }
-    out[0] = h.rounds; out[1] = h.settled; out[3] = h.esc;
-    const uint32_t c = h.in_state;   // pc_encode candidate -> penalty | start << 8 | previous_incompressible << 16
-    out[2] = c >= PROT_TRANSFER_WORDS ? 0xFFFFFFFFu : (c % 10) | (((c / 10) % 10 + 1) << 8) | ((c / 100) << 16);
-    for (int k = 0; k < 16; ++k) out[4 + k] = h.changed[k];
-    return DENSITY_B200_OK;
+    const int rc = prot_status_read(s->prot, out, &h, "shard_prot_status");
+    if (rc == DENSITY_B200_OK) { out[0] = h.rounds; out[1] = h.settled; }
+    return rc;
 }
 
 // ---- sharded Cheetah / Lion encode: one shard of a longer stream in three phases around two table exchanges ---------------------------
 struct density_b200_cl_shard {
-    int alg = ALG_CHEETAH, num_sms = 0;
+    // the quiet phases: PHASE1 -> PHASE2 -> PHASE3, once each. The copy-map iteration of density_b200_cl_shard_prot_*: READY after
+    // prot_phase1 or a commit, then P, C, TRANSFER, SETTLED per round, FINISHED.
+    enum { NONE, PHASE1, PHASE2, PHASE3, READY, P, C, TRANSFER, SETTLED, FINISHED };
     DevBuf ws, tables[3];           // workspace; the epoch-tagged run tables (zero at allocation, one entry format each)
-    uint8_t* tables_p[3] = {};      // their pointers, as the kernels take them
-    uint32_t epoch = 0, epoch_base = 0;
-    const uint8_t* d_in = nullptr;
-    size_t n = 0;
-    bool first = true, is_last = true;
-    int phase = 0;                  // the last phase done on the current shard
-    // the copy-map iteration of density_b200_cl_shard_prot_*: the shard's device record and where the phases stand
-    DevBuf prot;
-    uint64_t offset = 0;
-    int prot_phase = 0;             // 0 none, 1 ready for a round (phase 1 or a commit), 2 P, 3 C, 4 transfer, 5 settle, 6 finished
+    DevBuf prot;                    // the device record of the copy-map iteration (ProtShard)
+    ClShardArgs a{};                // the current shard, as every phase takes it
+    uint32_t epoch = 0;
+    int num_sms = 0;
+    int stage = NONE;
     int round = 0;                  // rounds committed
+    ~density_b200_cl_shard() { ws.release(); for (auto& t : tables) t.release(); prot.release(); }
 };
 
 static bool cl_alg_ok(int alg) { return alg == ALG_CHEETAH || alg == ALG_LION; }
@@ -898,190 +948,173 @@ static bool cl_alg_ok(int alg) { return alg == ALG_CHEETAH || alg == ALG_LION; }
 density_b200_cl_shard* density_b200_cl_shard_create(int alg) {
     if (!cl_alg_ok(alg)) { set_error("cl_shard_create: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return nullptr; }
     density_b200_cl_shard* s = new_shard<density_b200_cl_shard>();
-    if (s) s->alg = alg;
+    if (s) s->a.alg = alg;
     return s;
 }
-void density_b200_cl_shard_destroy(density_b200_cl_shard* s) {
-    if (!s) return;
-    s->ws.release(); for (auto& t : s->tables) t.release();
-    s->prot.release();
-    delete s;
-}
+void density_b200_cl_shard_destroy(density_b200_cl_shard* s) { delete s; }
 size_t density_b200_cl_table_words(int alg, int kind) {
     if (!cl_alg_ok(alg) || (kind != DENSITY_B200_CL_TABLE_P && kind != DENSITY_B200_CL_TABLE_C)) return 0;
     return (size_t)cl_table_planes(alg, kind) * 65536;
 }
 
-int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, const uint32_t* d_prev_quad,
-                                 uint32_t* d_table_p_out, void* stream) {
-    g_last_error.clear();
-    if (!s || (!d_in && n) || !d_table_p_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_prev_quad) & 3)) { set_error("d_in and d_prev_quad must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0;
-    s->prot_phase = 0;              // the workspace is this phase's now: the copy-map phases start over with prot_phase1
+// the shard d_in[0 .. n) set up in s->a (phase 1 and prot_phase1): every step of the shard before it void, the workspace, the tables and
+// with_prot the iteration's record ensured, the shard's epochs taken (cl_prot_epochs() with_prot, else cl_shard_epochs())
+static int cl_shard_setup(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, uint64_t offset, bool first, int is_last, bool with_prot,
+                          cudaStream_t st) {
+    s->stage = density_b200_cl_shard::NONE;
+    ClShardArgs& a = s->a;
     cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
-    for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
+    for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(a.alg, rg, n, s->num_sms) + 256, st);
+    if (e == cudaSuccess && with_prot) e = s->prot.ensure(sizeof(ProtShard), st);
     if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     if (s->epoch > 0x0FFFFF00u) {                      // epochs exhausted: start over on cleared tables
         for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = cudaMemsetAsync(s->tables[rg].p, 0, s->tables[rg].bytes, st);
         if (e != cudaSuccess) { set_error("cudaMemsetAsync", e); return DENSITY_B200_ECUDA; }
         s->epoch = 0;
     }
-    s->epoch_base = s->epoch + 1; s->epoch += cl_shard_epochs();
-    s->d_in = d_in; s->n = n; s->first = d_prev_quad == nullptr; s->is_last = is_last_shard != 0;
+    a.epoch_base = s->epoch + 1; s->epoch += with_prot ? cl_prot_epochs() : cl_shard_epochs();
+    a.d_in = d_in; a.n = n; a.offset = offset; a.first = first; a.last = is_last != 0;
+    a.ws = s->ws.p; for (int rg = 0; rg < 3; ++rg) a.tables[rg] = s->tables[rg].p;
+    a.num_sms = s->num_sms; a.ps = reinterpret_cast<ProtShard*>(s->prot.p);
+    return DENSITY_B200_OK;
+}
+
+int density_b200_cl_shard_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, int is_last_shard, const uint32_t* d_prev_quad,
+                                 uint32_t* d_table_p_out, void* stream) {
+    g_last_error.clear();
+    if (!s || !d_table_p_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    int rc = in_args(true, d_in, n, nullptr, 0, is_last_shard);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_prev_quad, d_table_p_out});
+    if (rc == DENSITY_B200_OK) rc = cl_shard_setup(s, d_in, n, 0, d_prev_quad == nullptr, is_last_shard, false, st);
+    if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
-    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    if (n == 0) e = cudaMemsetAsync(d_table_p_out, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_P) * sizeof(uint32_t), st);   // identity
-    else e = cl_shard_phase1(s->alg, d_in, n, d_prev_quad, s->ws.p, tabs, s->epoch_base, s->num_sms, d_table_p_out, st, &launches);
-    const int rc = step_result(e, launches, "cl shard phase1");
-    if (rc == DENSITY_B200_OK) s->phase = 1;
+    // an empty shard exports the identity
+    const cudaError_t e = n ? cl_shard_phase1(s->a, d_prev_quad, d_table_p_out, st, &launches)
+                            : cudaMemsetAsync(d_table_p_out, 0, density_b200_cl_table_words(s->a.alg, DENSITY_B200_CL_TABLE_P) * sizeof(uint32_t), st);
+    rc = step_result(e, launches, "cl shard phase1");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::PHASE1;
     return rc;
 }
 int density_b200_cl_shard_phase2(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream) {
     g_last_error.clear();
-    if (!s || s->phase != 1) { set_error("cl_shard_phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_cl_shard::PHASE1}, "cl_shard_phase2: null pointer / phase 1 not done")) return DENSITY_B200_EARG;
     if (!d_table_c_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    int rc = table_args({d_carry_p, d_table_c_out});
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
-    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    cudaError_t e;
-    if (s->n == 0) e = cudaMemsetAsync(d_table_c_out, 0, density_b200_cl_table_words(s->alg, DENSITY_B200_CL_TABLE_C) * sizeof(uint32_t), st);
-    else e = cl_shard_phase2(s->alg, s->d_in, s->n, s->first, d_carry_p, s->ws.p, tabs, s->epoch_base, s->num_sms, d_table_c_out, st, &launches);
-    const int rc = step_result(e, launches, "cl shard phase2");
-    if (rc == DENSITY_B200_OK) s->phase = 2;
+    const cudaError_t e = s->a.n ? cl_shard_phase2(s->a, d_carry_p, d_table_c_out, st, &launches)
+                                 : cudaMemsetAsync(d_table_c_out, 0, density_b200_cl_table_words(s->a.alg, DENSITY_B200_CL_TABLE_C) * sizeof(uint32_t), st);
+    rc = step_result(e, launches, "cl shard phase2");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::PHASE2;
     return rc;
 }
 int density_b200_cl_shard_phase3(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                  uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
-    if (!s || s->phase != 2) { set_error("cl_shard_phase3: null pointer / phase 2 not done"); return DENSITY_B200_EARG; }
-    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (reinterpret_cast<uintptr_t>(d_out) & 1) { set_error("d_out must be 2-byte aligned"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_cl_shard::PHASE2}, "cl_shard_phase3: null pointer / phase 2 not done")) return DENSITY_B200_EARG;
+    int rc = in_args(true, nullptr, 0, d_out, cap);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_carry_c});
+    if (rc == DENSITY_B200_OK) rc = out_args(d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
-    uint8_t* const tabs[3] = {s->tables[0].p, s->tables[1].p, s->tables[2].p};
-    const cudaError_t e = s->n ? cl_shard_phase3(s->alg, s->d_in, s->n, s->first, s->is_last, d_carry_c, s->ws.p, tabs, s->epoch_base, s->num_sms, d_out,
-                                                 cap, d_out_size, d_seam8, st, &launches)
-                               : empty_piece_outputs(d_out_size, d_seam8, st);
-    const int rc = step_result(e, launches, "cl shard phase3");
-    if (rc == DENSITY_B200_OK) s->phase = 3;
+    const cudaError_t e = s->a.n ? cl_shard_phase3(s->a, d_carry_c, d_out, cap, d_out_size, d_seam8, st, &launches)
+                                 : empty_piece_outputs(d_out_size, d_seam8, st);
+    rc = step_result(e, launches, "cl shard phase3");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::PHASE3;
     return rc;
 }
 // ---- sharded Cheetah / Lion encode with copy mode: the copy-map iteration carried over the cuts ------------------------------------------
-static ClProtShard cl_prot_args(density_b200_cl_shard* s) {
-    return ClProtShard{s->alg, s->d_in, s->n, s->offset, s->offset == 0 && s->n > 0, s->ws.p, s->tables_p, s->epoch_base, s->num_sms,
-                       reinterpret_cast<ProtShard*>(s->prot.p)};
-}
-// the phase functions below check the order: `want` is the prot_phase the call follows
-static bool cl_prot_order(density_b200_cl_shard* s, int want, const char* what) {
-    if (s && s->prot_phase == want) return true;
-    set_error(what);
-    return false;
-}
-
 int density_b200_cl_shard_prot_phase1(density_b200_cl_shard* s, const uint8_t* d_in, size_t n, uint64_t offset, int is_last_shard,
                                       uint32_t* d_words_out, void* stream) {
     g_last_error.clear();
-    if (!s || (!d_in && n) || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!is_last_shard && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
+    if (!s || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (offset % 256) { set_error("offset must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if (!al4(d_in) || !al4(d_words_out)) { set_error("d_in and d_words_out must be 4-byte aligned"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    s->phase = 0; s->prot_phase = 0;
-    cudaError_t e = s->ws.ensure(cl_shard_workspace_bytes(n, s->num_sms), st);
-    for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = s->tables[rg].ensure(chee_tables_bytes(s->alg, rg, n, s->num_sms) + 256, st);
-    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
-    if (s->epoch > 0x0FFFFF00u) {                      // epochs exhausted: start over on cleared tables
-        for (int rg = 0; rg < 3 && e == cudaSuccess; ++rg) e = cudaMemsetAsync(s->tables[rg].p, 0, s->tables[rg].bytes, st);
-        if (e != cudaSuccess) { set_error("cudaMemsetAsync", e); return DENSITY_B200_ECUDA; }
-        s->epoch = 0;
-    }
-    s->epoch_base = s->epoch + 1; s->epoch += cl_prot_epochs();
-    s->d_in = d_in; s->n = n; s->offset = offset; s->is_last = is_last_shard != 0; s->round = 0;
-    for (int rg = 0; rg < 3; ++rg) s->tables_p[rg] = s->tables[rg].p;
+    int rc = in_args(true, d_in, n, nullptr, 0, is_last_shard);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_words_out});
+    if (rc == DENSITY_B200_OK) rc = cl_shard_setup(s, d_in, n, offset, offset == 0 && n > 0, is_last_shard, true, st);
+    if (rc != DENSITY_B200_OK) return rc;
+    s->round = 0;
     uint64_t launches = 0;
-    e = cl_prot_phase1(cl_prot_args(s), d_words_out, st, &launches);
-    const int rc = step_result(e, launches, "cl shard prot phase1");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 1;
+    const cudaError_t e = cl_prot_phase1(s->a, d_words_out, st, &launches);
+    rc = step_result(e, launches, "cl shard prot phase1");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::READY;
     return rc;
 }
 int density_b200_cl_shard_prot_p(density_b200_cl_shard* s, const uint32_t* d_all_words, int world, int rank, uint32_t* d_table_p_out, void* stream) {
     g_last_error.clear();
     if (!d_all_words || !d_table_p_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!cl_prot_order(s, 1, "cl_shard_prot_p: call it after prot_phase1 or prot_next")) return DENSITY_B200_EARG;
+    if (!in_stage(s, {density_b200_cl_shard::READY}, "cl_shard_prot_p: call it after prot_phase1 or prot_next")) return DENSITY_B200_EARG;
     if (s->round >= g_prot_rounds) { set_error("cl_shard_prot_p: the round budget is used up"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_words) || !al4(d_table_p_out)) { set_error("words and tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (table_args({d_all_words, d_table_p_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_p(cl_prot_args(s), s->round, d_all_words, (uint32_t)rank, d_table_p_out, reinterpret_cast<cudaStream_t>(stream),
-                                    &launches);
+    const cudaError_t e = cl_prot_p(s->a, s->round, d_all_words, (uint32_t)rank, d_table_p_out, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "cl shard prot p");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 2;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::P;
     return rc;
 }
 int density_b200_cl_shard_prot_c(density_b200_cl_shard* s, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream) {
     g_last_error.clear();
     if (!d_carry_p || !d_table_c_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!cl_prot_order(s, 2, "cl_shard_prot_c: call it after prot_p")) return DENSITY_B200_EARG;
-    if (!al4(d_carry_p) || !al4(d_table_c_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_cl_shard::P}, "cl_shard_prot_c: call it after prot_p")) return DENSITY_B200_EARG;
+    if (table_args({d_carry_p, d_table_c_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_c(cl_prot_args(s), s->round, d_carry_p, d_table_c_out, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const cudaError_t e = cl_prot_c(s->a, s->round, d_carry_p, d_table_c_out, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "cl shard prot c");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 3;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::C;
     return rc;
 }
 int density_b200_cl_shard_prot_transfer(density_b200_cl_shard* s, const uint32_t* d_carry_c, uint32_t* d_transfer_out, void* stream) {
     g_last_error.clear();
     if (!d_carry_c || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!cl_prot_order(s, 3, "cl_shard_prot_transfer: call it after prot_c")) return DENSITY_B200_EARG;
-    if (!al4(d_carry_c) || !al4(d_transfer_out)) { set_error("tables must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (!in_stage(s, {density_b200_cl_shard::C}, "cl_shard_prot_transfer: call it after prot_c")) return DENSITY_B200_EARG;
+    if (table_args({d_carry_c, d_transfer_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_transfer(cl_prot_args(s), s->round, d_carry_c, d_transfer_out, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const cudaError_t e = cl_prot_transfer(s->a, s->round, d_carry_c, d_transfer_out, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "cl shard prot transfer");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 4;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::TRANSFER;
     return rc;
 }
 int density_b200_cl_shard_prot_settle(density_b200_cl_shard* s, const uint32_t* d_all_transfers, int world, int rank, uint32_t* d_words_out,
                                       void* stream) {
     g_last_error.clear();
     if (!d_all_transfers || !d_words_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!cl_prot_order(s, 4, "cl_shard_prot_settle: call it after prot_transfer")) return DENSITY_B200_EARG;
+    if (!in_stage(s, {density_b200_cl_shard::TRANSFER}, "cl_shard_prot_settle: call it after prot_transfer")) return DENSITY_B200_EARG;
     if (world < 1 || rank < 0 || rank >= world) { set_error("bad rank / world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_transfers) || !al4(d_words_out)) { set_error("transfers and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (table_args({d_all_transfers, d_words_out}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_settle(cl_prot_args(s), s->round, d_all_transfers, (uint32_t)rank, d_words_out,
-                                         reinterpret_cast<cudaStream_t>(stream), &launches);
+    const cudaError_t e = cl_prot_settle(s->a, s->round, d_all_transfers, (uint32_t)rank, d_words_out, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "cl shard prot settle");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 5;
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::SETTLED;
     return rc;
 }
 int density_b200_cl_shard_prot_next(density_b200_cl_shard* s, const uint32_t* d_all_words, int world, void* stream) {
     g_last_error.clear();
     if (!d_all_words) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!cl_prot_order(s, 5, "cl_shard_prot_next: call it after prot_settle")) return DENSITY_B200_EARG;
+    if (!in_stage(s, {density_b200_cl_shard::SETTLED}, "cl_shard_prot_next: call it after prot_settle")) return DENSITY_B200_EARG;
     if (world < 1) { set_error("bad world"); return DENSITY_B200_EARG; }
-    if (!al4(d_all_words)) { set_error("words must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    if (table_args({d_all_words}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_next(cl_prot_args(s), s->round, d_all_words, (uint32_t)world, reinterpret_cast<cudaStream_t>(stream), &launches);
+    const cudaError_t e = cl_prot_next(s->a, s->round, d_all_words, (uint32_t)world, reinterpret_cast<cudaStream_t>(stream), &launches);
     const int rc = step_result(e, launches, "cl shard prot next");
-    if (rc == DENSITY_B200_OK) { s->prot_phase = 1; ++s->round; }
+    if (rc == DENSITY_B200_OK) { s->stage = density_b200_cl_shard::READY; ++s->round; }
     return rc;
 }
 // ev_emit (may be NULL): recorded between the scan and the emit
 static int cl_prot_finish_impl(density_b200_cl_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t st,
                                cudaEvent_t ev_emit) {
-    if ((!d_out && cap) || !d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!s || s->prot_phase != 1 || s->round == 0) { set_error("cl_shard_prot_finish: call it after prot_next"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_out) & 1) || (reinterpret_cast<uintptr_t>(d_out_size) & 7) || !al4(d_seam8)) {
-        set_error("d_out must be 2-byte, d_out_size 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG;
-    }
+    int rc = in_args(true, nullptr, 0, d_out, cap);
+    if (rc == DENSITY_B200_OK) rc = out_args(d_out_size, d_seam8);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (!in_stage(s, {density_b200_cl_shard::READY}, "cl_shard_prot_finish: call it after prot_next", 1)) return DENSITY_B200_EARG;
     uint64_t launches = 0;
-    const cudaError_t e = cl_prot_finish(cl_prot_args(s), d_out, cap, d_out_size, d_seam8, st, &launches, ev_emit);
-    const int rc = step_result(e, launches, "cl shard prot finish");
-    if (rc == DENSITY_B200_OK) s->prot_phase = 6;
+    const cudaError_t e = cl_prot_finish(s->a, d_out, cap, d_out_size, d_seam8, st, &launches, ev_emit);
+    rc = step_result(e, launches, "cl shard prot finish");
+    if (rc == DENSITY_B200_OK) s->stage = density_b200_cl_shard::FINISHED;
     return rc;
 }
 int density_b200_cl_shard_prot_finish(density_b200_cl_shard* s, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
@@ -1090,21 +1123,19 @@ int density_b200_cl_shard_prot_finish(density_b200_cl_shard* s, uint8_t* d_out, 
 }
 int density_b200_cl_shard_prot_status(density_b200_cl_shard* s, uint32_t* out) {
     g_last_error.clear();
-    if (!s || !out || s->prot_phase < 1 || s->round == 0) { set_error("cl_shard_prot_status: null pointer / no round committed"); return DENSITY_B200_EARG; }
+    if (!out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    using S = density_b200_cl_shard;
+    if (!in_stage(s, {S::READY, S::P, S::C, S::TRANSFER, S::SETTLED, S::FINISHED}, "cl_shard_prot_status: no round committed", 1)) return DENSITY_B200_EARG;
     ProtShard h{};
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(&h, s->prot.p, sizeof h, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error("cl_shard_prot_status", e); return DENSITY_B200_ECUDA; }
-    out[0] = h.stage_ok; out[1] = h.rounds; out[3] = h.esc;
-    const uint32_t c = h.in_state;   // pc_encode candidate -> penalty | start << 8 | previous_incompressible << 16
-    out[2] = c >= PROT_TRANSFER_WORDS ? 0xFFFFFFFFu : (c % 10) | (((c / 10) % 10 + 1) << 8) | ((c / 100) << 16);
-    for (int k = 0; k < 16; ++k) out[4 + k] = h.changed[k];
-    return DENSITY_B200_OK;
+    const int rc = prot_status_read(s->prot, out, &h, "cl_shard_prot_status");
+    if (rc == DENSITY_B200_OK) { out[0] = h.stage_ok; out[1] = h.rounds; }
+    return rc;
 }
 
 int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* stream) {
     g_last_error.clear();
     if (!density_b200_cl_table_words(alg, kind) || !d_table) { set_error("cl_table_init: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
+    if (table_args({d_table}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t l = 0;
     const cudaError_t e = cl_table_init(alg, kind, d_table, reinterpret_cast<cudaStream_t>(stream), &l);
     return step_result(e, l, "cl_table_init");
@@ -1112,32 +1143,10 @@ int density_b200_cl_table_init(int alg, int kind, uint32_t* d_table, void* strea
 int density_b200_cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, void* stream) {
     g_last_error.clear();
     if (!density_b200_cl_table_words(alg, kind) || !d_acc || !d_next) { set_error("cl_table_fold: bad algorithm / kind or null pointer"); return DENSITY_B200_EARG; }
+    if (table_args({d_acc, d_next}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t l = 0;
     const cudaError_t e = cl_table_fold(alg, kind, d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
     return step_result(e, l, "cl_table_fold");
-}
-
-// ---- the argument rule of the sharded decode pieces and drivers (include/density_b200.h): d_in 2-byte, d_out and every table,
-// transfer, carry and word buffer 4-byte, d_out_size 8-byte, d_seam8 4-byte aligned. Each helper returns DENSITY_B200_EARG with the
-// error set, or DENSITY_B200_OK.
-static bool al8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
-// the input and the output of a piece; either may be null when its length is 0
-static int decode_in_args(const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap) {
-    if ((!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || !al4(d_out)) { set_error("d_in must be 2-byte, d_out 4-byte aligned"); return DENSITY_B200_EARG; }
-    return DENSITY_B200_OK;
-}
-// tables, transfers, carries and words, null where the entry allows it (the caller checks that)
-static int decode_table_args(std::initializer_list<const void*> tables) {
-    for (const void* t : tables)
-        if (!al4(t)) { set_error("tables, transfers, carries and words must be 4-byte aligned"); return DENSITY_B200_EARG; }
-    return DENSITY_B200_OK;
-}
-// the size and the seam words a piece writes
-static int decode_out_args(const uint64_t* d_out_size, const uint32_t* d_seam8) {
-    if (!d_out_size || !d_seam8) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (!al8(d_out_size) || !al4(d_seam8)) { set_error("d_out_size must be 8-byte, d_seam8 4-byte aligned"); return DENSITY_B200_EARG; }
-    return DENSITY_B200_OK;
 }
 
 // ---- sharded Chameleon decode: one piece of a sharded stream, decoded with the dictionary carried in from the pieces before it ------
@@ -1175,8 +1184,8 @@ int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t
     g_last_error.clear();
     if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = decode_in_args(d_in, n, nullptr, 0);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table_out});
+    int rc = in_args(false, d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_table_out});
     if (rc == DENSITY_B200_OK) rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, false, st);
     if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
@@ -1189,9 +1198,9 @@ int density_b200_decode_shard_phase1(density_b200_decode_shard* s, const uint8_t
 // the arguments of both phase-2 entries
 static int decode_phase2_args(const density_b200_decode_shard* s, const uint32_t* d_carry_in, const uint8_t* d_out, const uint64_t* d_out_size,
                               const uint32_t* d_seam8) {
-    int rc = decode_in_args(nullptr, 0, d_out, s->cap);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_carry_in});
-    return rc == DENSITY_B200_OK ? decode_out_args(d_out_size, d_seam8) : rc;
+    int rc = in_args(false, nullptr, 0, d_out, s->cap);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_carry_in});
+    return rc == DENSITY_B200_OK ? out_args(d_out_size, d_seam8) : rc;
 }
 int density_b200_decode_shard_phase2(density_b200_decode_shard* s, const uint32_t* d_carry_in, uint8_t* d_out, uint64_t* d_out_size,
                                      uint32_t* d_seam8, void* stream) {
@@ -1214,8 +1223,8 @@ int density_b200_decode_shard_prot_transfer(density_b200_decode_shard* s, const 
     g_last_error.clear();
     if (!s || !d_transfer_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = decode_in_args(d_in, n, nullptr, 0);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_transfer_out});
+    int rc = in_args(false, d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_transfer_out});
     if (rc == DENSITY_B200_OK) rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, true, st);
     if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
@@ -1244,7 +1253,7 @@ int density_b200_decode_shard_prot_phase1(density_b200_decode_shard* s, const ui
     g_last_error.clear();
     if (!s || s->prot_stage != 1) { set_error("decode_shard_prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers) || !d_table_out) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
-    const int rc = decode_table_args({d_all_transfers, d_table_out});
+    const int rc = table_args({d_all_transfers, d_table_out});
     if (rc != DENSITY_B200_OK) return rc;
     return decode_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_table_out, reinterpret_cast<cudaStream_t>(stream), "decode shard prot phase1");
 }
@@ -1253,8 +1262,8 @@ int density_b200_decode_shard_prot_enter(density_b200_decode_shard* s, const uin
     g_last_error.clear();
     if (!s || !d_table_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    int rc = decode_in_args(d_in, n, nullptr, 0);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table_out});
+    int rc = in_args(false, d_in, n, nullptr, 0);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_table_out});
     if (rc != DENSITY_B200_OK) return rc;
     if (candidate >= DECODE_PROT_TRANSFER_WORDS) { set_error("decode_shard_prot_enter: candidate >= 3200"); return DENSITY_B200_EARG; }
     if ((rc = decode_piece_setup(s, d_in, n, cap, is_last_shard, true, st)) != DENSITY_B200_OK) return rc;
@@ -1312,8 +1321,8 @@ size_t density_b200_cheetah_cmap_words(void) { return 3 * 65536; }
 static int cl_piece_setup(ClDecodePiece* s, bool lion, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, int is_first, int is_last,
                           const uint32_t* d_table, bool need_table, bool with_seed, cudaStream_t st) {
     if (!s || (need_table && !d_table)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    int rc = decode_in_args(d_in, n, d_out, cap);
-    if (rc == DENSITY_B200_OK) rc = decode_table_args({d_table});
+    int rc = in_args(false, d_in, n, d_out, cap);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_table});
     if (rc != DENSITY_B200_OK) return rc;
     s->reset();
     CheeShardArgs& a = s->a;
@@ -1348,7 +1357,7 @@ static int cl_piece_phase1(ClDecodePiece* s, bool lion, const uint8_t* d_in, siz
 static int cl_piece_phase2(ClDecodePiece* s, const uint32_t* d_cmap_carry, void* stream) {
     g_last_error.clear();
     if (!s || s->phase != 1) { set_error("cl decode shard phase2: null pointer / phase 1 not done"); return DENSITY_B200_EARG; }
-    int rc = decode_table_args({d_cmap_carry});
+    int rc = table_args({d_cmap_carry});
     if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
     const cudaError_t e = s->a.n ? chee_shard_phase2(s->a, d_cmap_carry, reinterpret_cast<cudaStream_t>(stream), &launches) : cudaSuccess;
@@ -1360,7 +1369,7 @@ static int cl_piece_phase2(ClDecodePiece* s, const uint32_t* d_cmap_carry, void*
 static int cl_piece_phase3(ClDecodePiece* s, bool ready, uint64_t* d_out_size, uint32_t* d_seam8, void* stream) {
     g_last_error.clear();
     if (!s || !ready) { set_error("cl decode shard phase3: null pointer / the step before it not done"); return DENSITY_B200_EARG; }
-    int rc = decode_out_args(d_out_size, d_seam8);
+    int rc = out_args(d_out_size, d_seam8);
     if (rc != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint64_t launches = 0;
@@ -1400,7 +1409,7 @@ static int cl_piece_prot_phase1(ClDecodePiece* s, const uint32_t* d_all_transfer
     g_last_error.clear();
     if (!s || !s->transfer_done || s->phase != 0) { set_error("cl decode shard prot_phase1: null pointer / transfer not done"); return DENSITY_B200_EARG; }
     if (world < 1 || rank < 0 || rank >= world || (rank > 0 && !d_all_transfers)) { set_error("bad rank / world or null pointer"); return DENSITY_B200_EARG; }
-    const int rc = decode_table_args({d_all_transfers, d_cmap_out});
+    const int rc = table_args({d_all_transfers, d_cmap_out});
     if (rc != DENSITY_B200_OK) return rc;
     return cl_piece_prot_phase1_body(s, d_all_transfers, rank, 0, true, d_cmap_out, reinterpret_cast<cudaStream_t>(stream), "cl decode shard prot phase1");
 }
@@ -1417,7 +1426,7 @@ int density_b200_cheetah_decode_shard_round_walk(density_b200_cheetah_decode_sha
     g_last_error.clear();
     if (!s || s->phase != 2) { set_error("cheetah_decode_shard_round_walk: null pointer / phase 2 or the previous round's fold not done"); return DENSITY_B200_EARG; }
     if (!d_words4) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    int rc = decode_table_args({d_pred_out, d_words4});
+    int rc = table_args({d_pred_out, d_words4});
     if (rc != DENSITY_B200_OK) return rc;
     if (s->round >= (uint32_t)g_chee_dec_rounds) { set_error("cheetah_decode_shard_round_walk: round budget used up"); return DENSITY_B200_EARG; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1437,7 +1446,7 @@ int density_b200_cheetah_decode_shard_round_fold(density_b200_cheetah_decode_sha
     g_last_error.clear();
     if (!s || s->phase != 3) { set_error("cheetah_decode_shard_round_fold: null pointer / the round's walk not done"); return DENSITY_B200_EARG; }
     if (!d_all_words || world < 1 || rank < 0 || rank >= world) { set_error("cheetah_decode_shard_round_fold: null pointer / bad rank or world"); return DENSITY_B200_EARG; }
-    int rc = decode_table_args({d_pred_carry, d_all_words});
+    int rc = table_args({d_pred_carry, d_all_words});
     if (rc != DENSITY_B200_OK) return rc;
     uint64_t launches = 0;
     const cudaError_t e = s->a.n ? chee_shard_round_fold(s->a, s->round, d_pred_carry, d_all_words, (uint32_t)world, (uint32_t)rank,
@@ -1728,6 +1737,30 @@ struct Exchange {
         return h->world == 1 || nccl_check(a->AllGather(buf + (size_t)h->rank * n, buf, n, NCCL_UINT32, h->comm, st), what);
     }
     uint32_t* my_words() const { return words + 8 * (size_t)h->rank; }
+    // this rank's Chameleon table (its slot of `tables`) to every rank, then one fold kernel: `carry` = the dictionary before this rank
+    int fold_tables(const char* what) const {
+        if (!gather(tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
+        uint64_t launches = 0;
+        const cudaError_t e = cham_rank_fold(tables, (uint32_t)h->rank, carry, st, &launches);
+        return step_result(e, launches, what);
+    }
+    // this rank's Cheetah / Lion table of `kind` (its slot of tabs, [world][table words]) to every rank, then one fold kernel: *carry =
+    // the state before this rank
+    int fold_cl_tables(int alg, int kind, uint32_t* tabs, uint32_t* carry_out, const char* what) const {
+        const bool p = kind == DENSITY_B200_CL_TABLE_P;
+        if (!gather(tabs, density_b200_cl_table_words(alg, kind), p ? "ncclAllGather(P tables)" : "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
+        uint64_t launches = 0;
+        const cudaError_t e = cl_rank_fold(alg, kind, tabs, (uint32_t)h->rank, carry_out, st, &launches);
+        return step_result(e, launches, what);
+    }
+    // this rank's shard length n to every rank: lengths[world] u64
+    int exchange_lengths(uint64_t* lengths, size_t n, const char* what) const {
+        uint64_t launches = 0;
+        const cudaError_t e = cham_put_u64(lengths + h->rank, (uint64_t)n, st, &launches);
+        const int rc = step_result(e, launches, what);
+        if (rc != DENSITY_B200_OK) return rc;
+        return gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)") ? DENSITY_B200_OK : DENSITY_B200_ECUDA;
+    }
     // this rank's seam words (my_words) to every rank -> the verdict over all pieces; *d_out_offset (may be NULL) = where this rank's
     // output starts
     int verdict(uint32_t* d_flags, uint64_t* d_total_size, uint64_t* d_out_offset) const {
@@ -1781,12 +1814,17 @@ static int gather_pieces(density_b200_sharded* h, NcclApi* a, const uint64_t* d_
     return DENSITY_B200_OK;
 }
 
-// the argument checks of the sharded encoders
-static int encode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, size_t n, const uint8_t* d_out, const uint64_t* d_out_size,
-                               int gather_root, const uint8_t* d_gather) {
-    if (!h || (!d_in && n) || !d_out || !d_out_size) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if (h->rank != h->world - 1 && (n % 256)) { set_error("non-final shards must be a multiple of 256 bytes"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("d_in must be 4-byte, d_out 2-byte aligned"); return DENSITY_B200_EARG; }
+// the argument checks of the sharded encoders, every one of them before the first collective: a rank that returned EARG half way
+// through would leave the others waiting in an all-gather. cl: a Cheetah / Lion driver, whose alg must be one of those two.
+static int encode_sharded_args(density_b200_sharded* h, bool cl, int alg, const uint8_t* d_in, size_t n, const uint8_t* d_out,
+                               const uint64_t* d_out_size, const uint32_t* d_flags, const uint64_t* d_total_size, int gather_root,
+                               const uint8_t* d_gather) {
+    if (!h || !d_out) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if (cl && !cl_alg_ok(alg)) { set_error("encode_sharded_cl: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
+    int rc = in_args(true, d_in, n, d_out, 0, h->rank == h->world - 1);
+    if (rc == DENSITY_B200_OK) rc = size_args(d_out_size, d_total_size);
+    if (rc == DENSITY_B200_OK) rc = table_args({d_flags});
+    if (rc != DENSITY_B200_OK) return rc;
     if (gather_root >= h->world) { set_error("bad gather root"); return DENSITY_B200_EARG; }
     if (h->rank == gather_root && !d_gather) { set_error("null pointer: d_gather on the gather root"); return DENSITY_B200_EARG; }
     return DENSITY_B200_OK;
@@ -1815,7 +1853,7 @@ static int encode_sharded_end(const Exchange& x, const uint8_t* d_out, uint32_t*
 int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                 uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
+    int rc = encode_sharded_args(h, false, ALG_CHAMELEON, d_in, n, d_out, d_out_size, d_flags, d_total_size, gather_root, d_gather);
     Exchange x;
     if (rc != DENSITY_B200_OK || (rc = x.open(h, stream_v)) != DENSITY_B200_OK) return rc;
     density_b200_shard* s = h->enc;
@@ -1825,20 +1863,48 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
     if (rc != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[1], x.st);
     // the one exchange step of the path: 256 KiB per rank over NVLink, then ONE fold kernel
-    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-    uint64_t launches = 0;
-    cudaError_t e = cham_rank_fold(x.tables, (uint32_t)h->rank, x.carry, x.st, &launches);
-    if ((rc = step_result(e, launches, "sharded fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = x.fold_tables("sharded fold")) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[2], x.st);
     // phase 2: carry-in, first-touch flags, sizes, scan, emit (seams are judged below, exactly, once every shard knows its flags)
     cudaEvent_t pev[4] = {nullptr, nullptr, h->ev[3], h->ev[4]};
     if ((rc = shard_phase2_impl(s, x.carry, d_out, cap, d_out_size, false, n ? pev : nullptr, x.st)) != DENSITY_B200_OK) return rc;
     if (!n) { cudaEventRecord(h->ev[3], x.st); cudaEventRecord(h->ev[4], x.st); }
-    launches = 0;
+    uint64_t launches = 0;
+    cudaError_t e;
     if (n) e = cham_seam_words(s->ws.p, s->L, n, d_out_size, x.my_words(), x.st, &launches);
     else e = cudaMemsetAsync(x.my_words(), 0, 8 * sizeof(uint32_t), x.st);
     if ((rc = step_result(e, launches, "sharded seam words")) != DENSITY_B200_OK) return rc;
     return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
+}
+
+// The exchange buffers of the Cheetah / Lion encode drivers behind Exchange::extra (extra: nullptr for the size alone), in this order:
+// prot: the shard lengths [world] u64; the gathered P tables [world][P words] and their carry, the gathered C tables [world][C words]
+// and their carry; then quiet: the last quads [world][2] and the previous quad (one word of the 64 behind the buffers); prot: the
+// transfers [world][PROT_TRANSFER_WORDS] and the round words [world][CL_PROT_ROUND_WORDS].
+struct ClEncodeBufs {
+    uint64_t* lengths;
+    uint32_t *tab_p, *carry_p, *tab_c, *carry_c, *quads, *prev_quad, *transfers, *rwords;
+    size_t bytes;
+};
+static ClEncodeBufs cl_encode_bufs(int alg, size_t world, bool prot, uint8_t* extra = nullptr) {
+    ClEncodeBufs b{};
+    size_t off = 0;    // u32 words
+    auto take = [&](size_t words) { uint32_t* p = extra ? reinterpret_cast<uint32_t*>(extra) + off : nullptr; off += words; return p; };
+    const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
+    if (prot) b.lengths = reinterpret_cast<uint64_t*>(take(2 * world));
+    b.tab_p = take(world * wp);
+    b.carry_p = take(wp);
+    b.tab_c = take(world * wc);
+    b.carry_c = take(wc);
+    if (prot) {
+        b.transfers = take(world * PROT_TRANSFER_WORDS);
+        b.rwords = take(world * CL_PROT_ROUND_WORDS);
+    } else {
+        b.quads = take(2 * world);
+        b.prev_quad = take(0);
+    }
+    b.bytes = (off + 64) * sizeof(uint32_t);
+    return b;
 }
 
 // Sharded Cheetah / Lion encode over the handle's communicator: last quads -> phase 1 -> P tables -> fold -> phase 2 -> C tables -> fold
@@ -1846,45 +1912,33 @@ int density_b200_encode_sharded(density_b200_sharded* h, const uint8_t* d_in, si
 int density_b200_encode_sharded_cl(density_b200_sharded* h, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                                    uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
+    int rc = encode_sharded_args(h, true, alg, d_in, n, d_out, d_out_size, d_flags, d_total_size, gather_root, d_gather);
     if (rc != DENSITY_B200_OK) return rc;
-    if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
     density_b200_cl_shard* s = h->cl[alg - ALG_CHEETAH];
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
     Exchange x;
-    if ((rc = x.open(h, stream_v, ((W + 1) * (wp + wc) + 2 * W + 64) * sizeof(uint32_t))) != DENSITY_B200_OK) return rc;
+    if ((rc = x.open(h, stream_v, cl_encode_bufs(alg, W, false).bytes)) != DENSITY_B200_OK) return rc;
     cudaStream_t st = x.st;
-    uint32_t* tab_p = reinterpret_cast<uint32_t*>(x.extra);              // [world][wp]
-    uint32_t* carry_p = tab_p + W * wp;
-    uint32_t* tab_c = carry_p + wp;                                       // [world][wc]
-    uint32_t* carry_c = tab_c + W * wc;
-    uint32_t* quads = carry_c + wc;                                       // [world] {has a quad, last quad}
-    uint32_t* prev_quad = quads + 2 * W;
+    const ClEncodeBufs b = cl_encode_bufs(alg, W, false, x.extra);
     uint64_t launches = 0;
     // 0. the context of my first quad: the last quad of the nearest earlier shard that has one
-    cudaError_t e = cl_last_quad(d_in, n, quads + 2 * R, st, &launches);
-    if (e == cudaSuccess && !x.gather(quads, 2, "ncclAllGather(last quads)")) return DENSITY_B200_ECUDA;
-    if (e == cudaSuccess) e = cl_prev_quad(quads, (uint32_t)R, prev_quad, st, &launches);
+    cudaError_t e = cl_last_quad(d_in, n, b.quads + 2 * R, st, &launches);
+    if (e == cudaSuccess && !x.gather(b.quads, 2, "ncclAllGather(last quads)")) return DENSITY_B200_ECUDA;
+    if (e == cudaSuccess) e = cl_prev_quad(b.quads, (uint32_t)R, b.prev_quad, st, &launches);
     if ((rc = step_result(e, launches, "sharded cl: last quads")) != DENSITY_B200_OK) return rc;
     // 1-2. predictions, exchange, fold
     cudaEventRecord(h->ev[0], st);
-    if ((rc = density_b200_cl_shard_phase1(s, d_in, n, R == W - 1, R ? prev_quad : nullptr, tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cl_shard_phase1(s, d_in, n, R == W - 1, R ? b.prev_quad : nullptr, b.tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[1], st);
-    if (!x.gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
-    launches = 0;
-    e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
-    if ((rc = step_result(e, launches, "sharded cl: P fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = x.fold_cl_tables(alg, DENSITY_B200_CL_TABLE_P, b.tab_p, b.carry_p, "sharded cl: P fold")) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[2], st);
     // 3-4. chunk map, exchange, fold
-    if ((rc = density_b200_cl_shard_phase2(s, carry_p, tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
-    if (!x.gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
-    launches = 0;
-    e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_C, tab_c, (uint32_t)R, carry_c, st, &launches);
-    if ((rc = step_result(e, launches, "sharded cl: C fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cl_shard_phase2(s, b.carry_p, b.tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
+    if ((rc = x.fold_cl_tables(alg, DENSITY_B200_CL_TABLE_C, b.tab_c, b.carry_c, "sharded cl: C fold")) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[3], st);
     // 5. emit and seam words, the verdict over all shards, the optional gather
-    if ((rc = density_b200_cl_shard_phase3(s, carry_c, d_out, cap, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
+    if ((rc = density_b200_cl_shard_phase3(s, b.carry_c, d_out, cap, d_out_size, x.my_words(), st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[4], st);
     return encode_sharded_end(x, d_out, d_flags, d_total_size, gather_root, d_gather, gather_cap);
 }
@@ -1896,38 +1950,27 @@ int density_b200_encode_sharded_protected(density_b200_sharded* h, const uint8_t
                                           uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather, size_t gather_cap,
                                           void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
+    int rc = encode_sharded_args(h, false, ALG_CHAMELEON, d_in, n, d_out, d_out_size, d_flags, d_total_size, gather_root, d_gather);
     if (rc != DENSITY_B200_OK) return rc;
-    // every argument the later phases check is checked here, before the first collective: a rank that returned EARG half way through
-    // would leave the others waiting in an all-gather
-    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || (reinterpret_cast<uintptr_t>(d_total_size) & 7) || !al4(d_flags)) {
-        set_error("d_out_size and d_total_size must be 8-byte, d_flags 4-byte aligned"); return DENSITY_B200_EARG;
-    }
     density_b200_shard* s = h->prot;
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     Exchange x;
     if ((rc = x.open(h, stream_v, W * (2 * sizeof(uint64_t) + (PROT_TRANSFER_WORDS + PROT_ROUND_WORDS) * sizeof(uint32_t)))) != DENSITY_B200_OK) return rc;
     cudaStream_t st = x.st;
-    cudaError_t e = s->ws.ensure(cham_workspace_bytes(n, s->num_sms, &s->L), st);      // phase 1 finds them in place
-    if (e == cudaSuccess) e = s->prot.ensure(sizeof(ProtShard), st);
-    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    // the workspace and the record before the first collective (DevBuf::ensure may cudaFree, which waits for the device); phase 1 finds
+    // them in place
+    if ((rc = cham_shard_setup(s, d_in, n, true, st)) != DENSITY_B200_OK) return rc;
     uint64_t* lengths = reinterpret_cast<uint64_t*>(x.extra);                         // [world]
     uint32_t* transfers = reinterpret_cast<uint32_t*>(lengths + W);                   // [world][PROT_TRANSFER_WORDS]
     uint32_t* rwords = transfers + W * PROT_TRANSFER_WORDS;                          // [world][PROT_ROUND_WORDS]
     uint32_t* my_table = x.tables + R * 65536;
-    uint64_t launches = 0;
     cudaEventRecord(h->ev[0], st);
-    e = cham_put_u64(lengths + R, (uint64_t)n, st, &launches);
-    if ((rc = step_result(e, launches, "sharded protected: length")) != DENSITY_B200_OK) return rc;
-    if (!x.gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
+    if ((rc = x.exchange_lengths(lengths, n, "sharded protected: length")) != DENSITY_B200_OK) return rc;
     if ((rc = prot_phase1_impl(s, d_in, n, 0, lengths, (int)R, R == W - 1, my_table, st)) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[1], st);
     for (int k = 0; k < g_prot_rounds; ++k) {
         if (k > 0 && (rc = density_b200_shard_prot_next(s, rwords, (int)W, my_table, st)) != DENSITY_B200_OK) return rc;
-        if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-        launches = 0;
-        e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, st, &launches);
-        if ((rc = step_result(e, launches, "sharded protected: fold")) != DENSITY_B200_OK) return rc;
+        if ((rc = x.fold_tables("sharded protected: fold")) != DENSITY_B200_OK) return rc;
         if (k == 0) cudaEventRecord(h->ev[2], st);
         if ((rc = density_b200_shard_prot_transfer(s, x.carry, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
         if (!x.gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
@@ -1948,59 +1991,38 @@ int density_b200_encode_sharded_cl_protected(density_b200_sharded* h, int alg, c
                                              uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root, uint8_t* d_gather,
                                              size_t gather_cap, void* stream_v) {
     g_last_error.clear();
-    int rc = encode_sharded_args(h, d_in, n, d_out, d_out_size, gather_root, d_gather);
+    int rc = encode_sharded_args(h, true, alg, d_in, n, d_out, d_out_size, d_flags, d_total_size, gather_root, d_gather);
     if (rc != DENSITY_B200_OK) return rc;
-    if (!cl_alg_ok(alg)) { set_error("encode_sharded_cl_protected: alg must be DENSITY_B200_CHEETAH or DENSITY_B200_LION"); return DENSITY_B200_EARG; }
-    // every argument the phases check is checked here, before the first collective (see density_b200_encode_sharded_protected)
-    if ((reinterpret_cast<uintptr_t>(d_out_size) & 7) || (reinterpret_cast<uintptr_t>(d_total_size) & 7) || !al4(d_flags)) {
-        set_error("d_out_size and d_total_size must be 8-byte, d_flags 4-byte aligned"); return DENSITY_B200_EARG;
-    }
     density_b200_cl_shard* s = h->clp[alg - ALG_CHEETAH];
     const size_t W = (size_t)h->world, R = (size_t)h->rank;
     const size_t wp = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_P), wc = density_b200_cl_table_words(alg, DENSITY_B200_CL_TABLE_C);
     const size_t rw = CL_PROT_ROUND_WORDS;
     Exchange x;
-    if ((rc = x.open(h, stream_v, W * sizeof(uint64_t) + ((W + 1) * (wp + wc) + W * (PROT_TRANSFER_WORDS + rw) + 64) * sizeof(uint32_t))) != DENSITY_B200_OK)
-        return rc;
+    if ((rc = x.open(h, stream_v, cl_encode_bufs(alg, W, true).bytes)) != DENSITY_B200_OK) return rc;
     cudaStream_t st = x.st;
-    uint64_t* lengths = reinterpret_cast<uint64_t*>(x.extra);            // [world]
-    uint32_t* tab_p = reinterpret_cast<uint32_t*>(lengths + W);          // [world][wp]
-    uint32_t* carry_p = tab_p + W * wp;
-    uint32_t* tab_c = carry_p + wp;                                       // [world][wc]
-    uint32_t* carry_c = tab_c + W * wc;
-    uint32_t* transfers = carry_c + wc;                                   // [world][PROT_TRANSFER_WORDS]
-    uint32_t* rwords = transfers + W * PROT_TRANSFER_WORDS;              // [world][CL_PROT_ROUND_WORDS]
-    uint64_t launches = 0;
+    const ClEncodeBufs b = cl_encode_bufs(alg, W, true, x.extra);
     cudaEventRecord(h->ev[0], st);
     // the byte offset of my shard, on the host: whether this shard holds the stream start decides what phase 1 enqueues
-    cudaError_t e = cham_put_u64(lengths + R, (uint64_t)n, st, &launches);
-    if ((rc = step_result(e, launches, "sharded cl protected: length")) != DENSITY_B200_OK) return rc;
-    if (!x.gather(reinterpret_cast<uint32_t*>(lengths), 2, "ncclAllGather(lengths)")) return DENSITY_B200_ECUDA;
-    e = cudaMemcpyAsync(h->h_offsets, lengths, W * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+    if ((rc = x.exchange_lengths(b.lengths, n, "sharded cl protected: length")) != DENSITY_B200_OK) return rc;
+    cudaError_t e = cudaMemcpyAsync(h->h_offsets, b.lengths, W * sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if ((rc = step_result(e, 0, "sharded cl protected: lengths to host")) != DENSITY_B200_OK) return rc;
     uint64_t offset = 0;
     for (size_t r = 0; r < R; ++r) offset += h->h_offsets[r];
-    if ((rc = density_b200_cl_shard_prot_phase1(s, d_in, n, offset, R == W - 1, rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
-    if (!x.gather(rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+    if ((rc = density_b200_cl_shard_prot_phase1(s, d_in, n, offset, R == W - 1, b.rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
+    if (!x.gather(b.rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
     cudaEventRecord(h->ev[1], st);
     for (int k = 0; k < g_prot_rounds; ++k) {
-        if ((rc = density_b200_cl_shard_prot_p(s, rwords, (int)W, (int)R, tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
-        if (!x.gather(tab_p, wp, "ncclAllGather(P tables)")) return DENSITY_B200_ECUDA;
-        launches = 0;
-        e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_P, tab_p, (uint32_t)R, carry_p, st, &launches);
-        if ((rc = step_result(e, launches, "sharded cl protected: P fold")) != DENSITY_B200_OK) return rc;
+        if ((rc = density_b200_cl_shard_prot_p(s, b.rwords, (int)W, (int)R, b.tab_p + R * wp, st)) != DENSITY_B200_OK) return rc;
+        if ((rc = x.fold_cl_tables(alg, DENSITY_B200_CL_TABLE_P, b.tab_p, b.carry_p, "sharded cl protected: P fold")) != DENSITY_B200_OK) return rc;
         if (k == 0) cudaEventRecord(h->ev[2], st);
-        if ((rc = density_b200_cl_shard_prot_c(s, carry_p, tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
-        if (!x.gather(tab_c, wc, "ncclAllGather(C tables)")) return DENSITY_B200_ECUDA;
-        launches = 0;
-        e = cl_rank_fold(alg, DENSITY_B200_CL_TABLE_C, tab_c, (uint32_t)R, carry_c, st, &launches);
-        if ((rc = step_result(e, launches, "sharded cl protected: C fold")) != DENSITY_B200_OK) return rc;
-        if ((rc = density_b200_cl_shard_prot_transfer(s, carry_c, transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
-        if (!x.gather(transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
-        if ((rc = density_b200_cl_shard_prot_settle(s, transfers, (int)W, (int)R, rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
-        if (!x.gather(rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
-        if ((rc = density_b200_cl_shard_prot_next(s, rwords, (int)W, st)) != DENSITY_B200_OK) return rc;
+        if ((rc = density_b200_cl_shard_prot_c(s, b.carry_p, b.tab_c + R * wc, st)) != DENSITY_B200_OK) return rc;
+        if ((rc = x.fold_cl_tables(alg, DENSITY_B200_CL_TABLE_C, b.tab_c, b.carry_c, "sharded cl protected: C fold")) != DENSITY_B200_OK) return rc;
+        if ((rc = density_b200_cl_shard_prot_transfer(s, b.carry_c, b.transfers + R * PROT_TRANSFER_WORDS, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(b.transfers, PROT_TRANSFER_WORDS, "ncclAllGather(transfers)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_cl_shard_prot_settle(s, b.transfers, (int)W, (int)R, b.rwords + R * rw, st)) != DENSITY_B200_OK) return rc;
+        if (!x.gather(b.rwords, rw, "ncclAllGather(round words)")) return DENSITY_B200_ECUDA;
+        if ((rc = density_b200_cl_shard_prot_next(s, b.rwords, (int)W, st)) != DENSITY_B200_OK) return rc;
     }
     if ((rc = cl_prot_finish_impl(s, d_out, cap, d_out_size, x.my_words(), st, h->ev[3])) != DENSITY_B200_OK) return rc;
     cudaEventRecord(h->ev[4], st);
@@ -2012,7 +2034,7 @@ static int decode_sharded_args(density_b200_sharded* h, const uint8_t* d_in, siz
                                const uint32_t* d_flags) {
     if (!h || !d_out_size || !d_flags) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (!al8(d_out_size)) { set_error("d_out_size must be 8-byte aligned"); return DENSITY_B200_EARG; }
-    return decode_in_args(d_in, n, d_out, cap);
+    return in_args(false, d_in, n, d_out, cap);
 }
 
 // The decode of this rank's piece d_in[0 .. n) with the dictionary carried in from the pieces before it:
@@ -2043,10 +2065,7 @@ static int decode_sharded_piece(const Exchange& x, const uint8_t* d_in, size_t n
         rc = density_b200_decode_shard_phase1(s, d_in, n, cap, is_last, my_table, x.st);
     }
     if (rc != DENSITY_B200_OK) return rc;
-    if (!x.gather(x.tables, 65536, "ncclAllGather(tables)")) return DENSITY_B200_ECUDA;
-    uint64_t launches = 0;
-    const cudaError_t e = cham_rank_fold(x.tables, (uint32_t)R, x.carry, x.st, &launches);
-    if ((rc = step_result(e, launches, "sharded decode fold")) != DENSITY_B200_OK) return rc;
+    if ((rc = x.fold_tables("sharded decode fold")) != DENSITY_B200_OK) return rc;
     // phase 2: decode from the carried-in dictionary, then the seam words; the verdict reads them from every rank
     rc = seeded ? density_b200_decode_shard_prot_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st)
                 : density_b200_decode_shard_phase2(s, x.carry, d_out, d_out_size, x.my_words(), x.st);
@@ -2215,10 +2234,10 @@ template <class S, class M, class F>
 static int locate_entry(S* s, const uint8_t* d_in, size_t n, const M* d_map, size_t ws_bytes, void* stream, const char* what, F launch) {
     g_last_error.clear();
     if (!s || !d_map) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    int rc = decode_in_args(d_in, n, nullptr, 0);
+    int rc = in_args(false, d_in, n, nullptr, 0);
     if (rc != DENSITY_B200_OK) return rc;
     if (sizeof(M) == 8 && !al8(d_map)) { set_error("d_map must be 8-byte aligned"); return DENSITY_B200_EARG; }
-    if ((rc = decode_table_args({d_map})) != DENSITY_B200_OK) return rc;
+    if ((rc = table_args({d_map})) != DENSITY_B200_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     s->reset();
     cudaError_t e = s->ws.ensure(ws_bytes, st);
@@ -2597,11 +2616,17 @@ size_t density_b200_codec_encode(density_b200_codec* h, const uint8_t* in, size_
 size_t density_b200_codec_decode(density_b200_codec* h, const uint8_t* in, size_t n, uint8_t* out, size_t cap) { return codec_run(h, false, in, n, out, cap); }
 
 int density_b200_table_init(uint32_t* d_table, void* stream) {
+    g_last_error.clear();
+    if (!d_table) { set_error("table_init: null pointer"); return DENSITY_B200_EARG; }
+    if (table_args({d_table}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t l = 0;
     const cudaError_t e = cham_table_init(d_table, reinterpret_cast<cudaStream_t>(stream), &l);
     return step_result(e, l, "table_init");
 }
 int density_b200_table_fold(uint32_t* d_acc, const uint32_t* d_next, void* stream) {
+    g_last_error.clear();
+    if (!d_acc || !d_next) { set_error("table_fold: null pointer"); return DENSITY_B200_EARG; }
+    if (table_args({d_acc, d_next}) != DENSITY_B200_OK) return DENSITY_B200_EARG;
     uint64_t l = 0;
     const cudaError_t e = cham_table_fold(d_acc, d_next, reinterpret_cast<cudaStream_t>(stream), &l);
     return step_result(e, l, "table_fold");

@@ -1096,20 +1096,18 @@ uint32_t cl_shard_epochs() { return CL_SHARD_EPOCHS; }
 uint32_t cl_table_planes(int alg, int kind) { return kind == 1 ? 3u : alg == ALG_LION ? 12u : 2u; }
 size_t cl_shard_workspace_bytes(size_t nbytes, int num_sms) { return ((chee_workspace_bytes(nbytes, num_sms) + 255) & ~(size_t)255) + 1024; }
 
-// Phase 1: the first shard (d_prev_quad == nullptr) runs the copy-map iteration to the end; a later shard runs ctx0 and pass P. Both
+// Phase 1: the first shard (a.first) runs the copy-map iteration to the end; a later shard runs ctx0 and pass P. Both
 // export their P transfer.
-cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32_t* d_prev_quad, uint8_t* ws, uint8_t* const tables[3],
-                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches) {
-    const CheeView V(alg, d_in, n, num_sms, ws, tables);
-    const bool first = d_prev_quad == nullptr;
-    const uint32_t ep = epoch_base + 32;
+cudaError_t cl_shard_phase1(const ClShardArgs& a, const uint32_t* d_prev_quad, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    const uint32_t ep = a.epoch_base + 32;
     Status* iter = nullptr;
     cudaError_t e = cudaSuccess;
-    if (first) e = chee_iterate(V, epoch_base, num_sms, false, V.epoch_word, stream, launches, &iter);
+    if (a.first) e = chee_iterate(V, a.epoch_base, a.num_sms, false, V.epoch_word, stream, launches, &iter);
     if (e != cudaSuccess) return e;
     cl_shard_gates<<<1, 1, 0, stream>>>(V.gate, V.emit, iter, V.pair_flag, V.epoch_word, ep);
     ++*launches;
-    if (!first) launch_ctx0_pass_p(V, nullptr, V.gate, d_prev_quad, ep, nullptr, stream, launches);
+    if (!a.first) launch_ctx0_pass_p(V, nullptr, V.gate, d_prev_quad, ep, nullptr, stream, launches);
     if (V.lion) cl_export_p_lion<<<PL / 128, 128, 0, stream>>>(V.in32, V.entP, V.coldP, V.nruns, nullptr, V.epoch_word, d_tab_p);
     else cl_export_p_chee<<<PL / 128, 128, 0, stream>>>(V.entP, V.nruns, nullptr, V.epoch_word, d_tab_p);
     ++*launches;
@@ -1119,10 +1117,9 @@ cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32
 // Phase 2: a later shard makes its predictions final from the carried-in P state (planes as cl_table_init / cl_rank_fold leave them;
 // nullptr = stream start) and runs pass C; every shard exports its C transfer. The first shard ignores d_carry_p (its state is the
 // stream start, and its flags are final already).
-cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, const uint32_t* d_carry_p, uint8_t* ws, uint8_t* const tables[3],
-                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
-    const CheeView V(alg, d_in, n, num_sms, ws, tables);
-    if (!first) launch_fold_p_pass_c(V, nullptr, V.gate, epoch_base + 32, d_carry_p, stream, launches);
+cudaError_t cl_shard_phase2(const ClShardArgs& a, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    if (!a.first) launch_fold_p_pass_c(V, nullptr, V.gate, a.epoch_base + 32, d_carry_p, stream, launches);
     cl_export_c<<<PL / 128, 128, 0, stream>>>(V.entC, V.nruns, nullptr, V.epoch_word, d_tab_c);
     ++*launches;
     return cudaGetLastError();
@@ -1130,22 +1127,22 @@ cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, 
 
 // Phase 3: a later shard makes its chunk-map flags final from the carried-in C state (the first shard ignores d_carry_c); then sizes
 // and incompressible bits, scan, emit, the shard's 8 seam words.
-cudaError_t cl_shard_phase3(int alg, const uint8_t* d_in, size_t n, bool first, bool is_last, const uint32_t* d_carry_c, uint8_t* ws,
-                            uint8_t* const tables[3], uint32_t epoch_base, int num_sms, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                            uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches) {
-    const CheeView V(alg, d_in, n, num_sms, ws, tables);
+cudaError_t cl_shard_phase3(const ClShardArgs& a, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
+                            cudaStream_t stream, uint64_t* launches) {
+    const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
+    const bool first = a.first;
     const uint8_t* mask = first ? V.cm : nullptr;
-    if (!first) launch_fold_c(V, V.gate, epoch_base + 32, d_carry_c, stream, launches);
+    if (!first) launch_fold_c(V, V.gate, a.epoch_base + 32, d_carry_c, stream, launches);
     launch_tile_sizes(V, mask, 0, V.gate, stream, launches);
     if (!first) {
         const uint64_t want = (V.nblk + 255) / 256;
-        const uint32_t grid = (uint32_t)(want < (uint64_t)num_sms * 8 ? (want ? want : 1) : (uint64_t)num_sms * 8);
+        const uint32_t grid = (uint32_t)(want < (uint64_t)a.num_sms * 8 ? (want ? want : 1) : (uint64_t)a.num_sms * 8);
         cl_inc_pairs<<<grid, 256, 0, stream>>>(V.incb, V.nblk, V.pair_flag);
         ++*launches;
     }
     cudaError_t e = launch_scan_emit(V, mask, V.emit, cap, d_out_size, d_out, stream, launches);
     if (e != cudaSuccess) return e;
-    cl_seam_words_k<<<1, 1, 0, stream>>>(V.incb, mask, V.nblk, first, is_last, V.emit, first ? nullptr : V.pair_flag, d_out_size, d_seam8);
+    cl_seam_words_k<<<1, 1, 0, stream>>>(V.incb, mask, V.nblk, first, a.last, V.emit, first ? nullptr : V.pair_flag, d_out_size, d_seam8);
     ++*launches;
     return cudaGetLastError();
 }
@@ -1195,7 +1192,7 @@ static void launch_prot_quad(const CheeView& V, const uint8_t* cm, const Status*
     ++*launches;
 }
 
-cudaError_t cl_prot_phase1(const ClProtShard& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches) {
+cudaError_t cl_prot_phase1(const ClShardArgs& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     Status* iter = nullptr;
     cudaError_t e = cudaSuccess;
@@ -1211,7 +1208,7 @@ cudaError_t cl_prot_phase1(const ClProtShard& a, uint32_t* d_words8, cudaStream_
     return cudaGetLastError();
 }
 
-cudaError_t cl_prot_p(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
+cudaError_t cl_prot_p(const ClShardArgs& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
                       uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     if (!V.nblk) return cudaMemsetAsync(d_tab_p, 0, (size_t)cl_table_planes(a.alg, 0) * PL * sizeof(uint32_t), stream);   // identity
@@ -1226,7 +1223,7 @@ cudaError_t cl_prot_p(const ClProtShard& a, int it, const uint32_t* d_all_words,
     return cudaGetLastError();
 }
 
-cudaError_t cl_prot_c(const ClProtShard& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
+cudaError_t cl_prot_c(const ClShardArgs& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     if (!V.nblk) return cudaMemsetAsync(d_tab_c, 0, (size_t)cl_table_planes(a.alg, 1) * PL * sizeof(uint32_t), stream);
     if (!a.first) launch_fold_p_pass_c(V, V.cm, V.gate, a.epoch_base + 32 + (uint32_t)it, d_carry_p, stream, launches);
@@ -1235,7 +1232,7 @@ cudaError_t cl_prot_c(const ClProtShard& a, int it, const uint32_t* d_carry_p, u
     return cudaGetLastError();
 }
 
-cudaError_t cl_prot_transfer(const ClProtShard& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
+cudaError_t cl_prot_transfer(const ClShardArgs& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     if (!a.first && V.nblk) {          // the incompressible bits of the blocks M_k encodes; copied blocks keep those of the round before
         launch_fold_c(V, V.gate, a.epoch_base + 32 + (uint32_t)it, d_carry_c, stream, launches);
@@ -1244,7 +1241,7 @@ cudaError_t cl_prot_transfer(const ClProtShard& a, int it, const uint32_t* d_car
     return prot_transfer(cl_prot_segs(V), nullptr, a.ps, it, d_transfer, stream, launches);
 }
 
-cudaError_t cl_prot_settle(const ClProtShard& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
+cudaError_t cl_prot_settle(const ClShardArgs& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
                            uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     cudaError_t e = prot_settle(cl_prot_segs(V), a.ps, it, 1, d_all_transfers, rank, d_words8, stream, launches);
@@ -1253,14 +1250,14 @@ cudaError_t cl_prot_settle(const ClProtShard& a, int it, const uint32_t* d_all_t
     return cudaGetLastError();
 }
 
-cudaError_t cl_prot_next(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches) {
+cudaError_t cl_prot_next(const ClShardArgs& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     return prot_commit(cl_prot_segs(V), a.ps, it, d_all_words, world, CL_PROT_ROUND_WORDS, stream, launches);
 }
 
 // sizes under the committed map, scan, emit under the gate of the rounds (it has converged when the map settled; the error of an unsettled
 // shard closes it), the seam words
-cudaError_t cl_prot_finish(const ClProtShard& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
+cudaError_t cl_prot_finish(const ClShardArgs& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
                            uint64_t* launches, cudaEvent_t ev_emit) {
     const CheeView V(a.alg, a.d_in, a.n, a.num_sms, a.ws, a.tables);
     cudaError_t e = prot_refuse_unsettled(V.gate, a.ps, stream, launches);

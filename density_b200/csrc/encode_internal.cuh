@@ -111,42 +111,41 @@ cudaError_t chee_encode_parallel(int alg, const uint8_t* d_in, size_t nbytes, ui
                                  uint32_t epoch_base, int num_sms, uint64_t* d_out_size, uint32_t* d_converged, bool resume,
                                  cudaStream_t stream, uint64_t* launches);
 // sharded Cheetah / Lion encode: one shard of a longer stream (non-final shards whole 256-byte multiples). Tables are stacks of
-// cl_table_planes(alg, kind) planes of 65536 u32 (kind 0 = predictions, 1 = chunk map). Each call of phase 1 takes cl_shard_epochs()
-// fresh epochs starting at epoch_base; phases 2 and 3 get the same epoch_base. d_prev_quad: the last quad of the stream before the shard
-// (nullptr = the first shard, which alone may use copy mode); d_carry_*: the carried-in state (nullptr = stream start).
+// cl_table_planes(alg, kind) planes of 65536 u32 (kind 0 = predictions, 1 = chunk map). Every phase of one shard gets the same record:
+// the shard d_in[0 .. n) at byte `offset` of the stream; first: the shard at the stream start, which alone may use copy mode (quiet
+// phases: the shard without a d_prev_quad; prot phases: offset 0 and n > 0); last: no stream byte follows it; ws and the three tables
+// (chee_tables_bytes regions); the epochs from epoch_base; ps: the record of the copy-map iteration (device, prot phases only).
+struct ClShardArgs { int alg; const uint8_t* d_in; size_t n; uint64_t offset; bool first, last; uint8_t* ws; uint8_t* tables[3]; uint32_t epoch_base;
+                     int num_sms; ProtShard* ps; };
+// Each quiet phase 1 takes cl_shard_epochs() fresh epochs; phases 2 and 3 get the same epoch_base. d_prev_quad: the last quad of the
+// stream before the shard (nullptr for the first shard); d_carry_*: the carried-in state (nullptr = stream start).
 uint32_t cl_shard_epochs();
 uint32_t cl_table_planes(int alg, int kind);
 size_t cl_shard_workspace_bytes(size_t nbytes, int num_sms);
-cudaError_t cl_shard_phase1(int alg, const uint8_t* d_in, size_t n, const uint32_t* d_prev_quad, uint8_t* ws, uint8_t* const tables[3],
-                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches);
-cudaError_t cl_shard_phase2(int alg, const uint8_t* d_in, size_t n, bool first, const uint32_t* d_carry_p, uint8_t* ws, uint8_t* const tables[3],
-                            uint32_t epoch_base, int num_sms, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
-cudaError_t cl_shard_phase3(int alg, const uint8_t* d_in, size_t n, bool first, bool is_last, const uint32_t* d_carry_c, uint8_t* ws,
-                            uint8_t* const tables[3], uint32_t epoch_base, int num_sms, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
-                            uint32_t* d_seam8, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_shard_phase1(const ClShardArgs& a, const uint32_t* d_prev_quad, uint32_t* d_tab_p, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_shard_phase2(const ClShardArgs& a, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_shard_phase3(const ClShardArgs& a, const uint32_t* d_carry_c, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8,
+                            cudaStream_t stream, uint64_t* launches);
 cudaError_t cl_table_init(int alg, int kind, uint32_t* d_table, cudaStream_t stream, uint64_t* launches);
 cudaError_t cl_table_fold(int alg, int kind, uint32_t* d_acc, const uint32_t* d_next, cudaStream_t stream, uint64_t* launches);
 cudaError_t cl_rank_fold(int alg, int kind, const uint32_t* d_tables, uint32_t rank, uint32_t* d_carry, cudaStream_t stream, uint64_t* launches);
 cudaError_t cl_last_quad(const uint8_t* d_in, size_t n, uint32_t* d_out2, cudaStream_t stream, uint64_t* launches);   // {has a quad, last quad}
 cudaError_t cl_prev_quad(const uint32_t* d_words, uint32_t rank, uint32_t* d_out, cudaStream_t stream, uint64_t* launches);
 // the same with copy-mode blocks anywhere (density_b200_cl_shard_prot_*): the copy-map iteration carried over the cuts, round for round.
-// The shard starts at byte `offset` (first: offset 0 and n > 0, the shard that runs the staged iteration in phase 1); each call takes
-// cl_prot_epochs() fresh epochs from epoch_base. Round words: CL_PROT_ROUND_WORDS u32, {changed, met PC_ESC, settled before, 0, has an
-// encoded quad, that quad, 0, 0}. ps: the shard's record (device).
+// The first shard runs the staged iteration in phase 1; each prot phase 1 takes cl_prot_epochs() fresh epochs from epoch_base. Round
+// words: CL_PROT_ROUND_WORDS u32, {changed, met PC_ESC, settled before, 0, has an encoded quad, that quad, 0, 0}.
 constexpr uint32_t CL_PROT_ROUND_WORDS = 8;
 uint32_t cl_prot_epochs();
-struct ClProtShard { int alg; const uint8_t* d_in; size_t n; uint64_t offset; bool first; uint8_t* ws; uint8_t* const* tables; uint32_t epoch_base;
-                     int num_sms; ProtShard* ps; };
-cudaError_t cl_prot_phase1(const ClProtShard& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches);
-cudaError_t cl_prot_p(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
+cudaError_t cl_prot_phase1(const ClShardArgs& a, uint32_t* d_words8, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_p(const ClShardArgs& a, int it, const uint32_t* d_all_words, uint32_t rank, uint32_t* d_tab_p, cudaStream_t stream,
                       uint64_t* launches);
-cudaError_t cl_prot_c(const ClProtShard& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
-cudaError_t cl_prot_transfer(const ClProtShard& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
-cudaError_t cl_prot_settle(const ClProtShard& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
+cudaError_t cl_prot_c(const ClShardArgs& a, int it, const uint32_t* d_carry_p, uint32_t* d_tab_c, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_transfer(const ClShardArgs& a, int it, const uint32_t* d_carry_c, uint32_t* d_transfer, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_settle(const ClShardArgs& a, int it, const uint32_t* d_all_transfers, uint32_t rank, uint32_t* d_words8, cudaStream_t stream,
                            uint64_t* launches);
-cudaError_t cl_prot_next(const ClProtShard& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches);
+cudaError_t cl_prot_next(const ClShardArgs& a, int it, const uint32_t* d_all_words, uint32_t world, cudaStream_t stream, uint64_t* launches);
 // ev_emit (may be nullptr): recorded between the scan and the emit
-cudaError_t cl_prot_finish(const ClProtShard& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
+cudaError_t cl_prot_finish(const ClShardArgs& a, uint8_t* d_out, size_t cap, uint64_t* d_out_size, uint32_t* d_seam8, cudaStream_t stream,
                            uint64_t* launches, cudaEvent_t ev_emit = nullptr);
 
 // chameleon_decode.cu

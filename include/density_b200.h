@@ -143,6 +143,16 @@ DENSITY_B200_API int density_b200_decoded_size_device(int alg, const uint8_t* d_
 DENSITY_B200_API int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t* out_size);
 
 /*
+ * Sharded encode. Every entry of the phase APIs of a Chameleon, Cheetah or Lion shard below, density_b200_table_init / _fold,
+ * density_b200_cl_table_init / _fold and every density_b200_encode_sharded* driver takes its pointers by one rule: d_in and d_prev_quad
+ * 4-byte aligned; d_out 2-byte aligned; every table, carry, transfer, word and flag buffer 4-byte aligned; d_out_size and d_total_size
+ * 8-byte and d_seam8 4-byte aligned. A shard that does not end the stream is a multiple of 256 bytes. d_in and d_out may be NULL only
+ * when their length is 0 (phase 2 of a Chameleon shard also takes a NULL d_out), d_flags and d_total_size may be NULL, an optional
+ * table only where the entry says so. A misaligned or a missing pointer, or a phase called out of order, returns DENSITY_B200_EARG and
+ * enqueues nothing; the drivers check every argument before their first collective.
+ */
+
+/*
  * Sharded Chameleon encode (one bit-exact stream cut across several GPUs / calls; SURVEY §8e).
  * The stream is cut at multiples of 256 bytes. Every shard runs phase 1 independently, the
  * 256 KiB last-writer tables are exchanged by the caller (torch.distributed all_gather in
@@ -218,9 +228,7 @@ DENSITY_B200_API int density_b200_sharded_profile(density_b200_sharded*, float* 
  *   exchange   the round words of all shards, in rank order; then prot_next: the global commit (settled when no shard changed and
  *              none met 0xFFFF: every later kernel returns at once), and with a table the next round's flags.
  * After the last round prot_next without a table commits it, and prot_finish emits. Every shard runs the same number of rounds; at
- * most density_b200_prot_round_budget() (prot_next with a table returns DENSITY_B200_EARG beyond it). Phases called out of order,
- * misaligned pointers (d_in and tables 4-byte, d_out 2-byte) and a non-final shard that is not a multiple of 256 bytes return
- * DENSITY_B200_EARG without enqueuing anything.
+ * most density_b200_prot_round_budget() (prot_next with a table returns DENSITY_B200_EARG beyond it).
  */
 #define DENSITY_B200_PROT_TRANSFER_WORDS 200
 #define DENSITY_B200_PROT_ROUND_WORDS 4
@@ -250,9 +258,7 @@ DENSITY_B200_API int density_b200_shard_prot_status(density_b200_shard*, uint32_
 /* End to end over NCCL on a density_b200_sharded handle, with the arguments and gather semantics of density_b200_encode_sharded: an
    ncclAllGather of the shard lengths (the first global block) -> phase 1 -> the round budget of {ncclAllGather(tables) -> fold kernel ->
    transfer -> ncclAllGather(transfers, 800 bytes per rank) -> settle -> ncclAllGather(round words, 16 bytes) -> commit} -> finish ->
-   seam verdict -> optional gather. Uses its own shard state in the handle; nothing blocks unless gather_root >= 0. Bad arguments
-   (d_in 4-byte, d_out 2-byte, d_out_size and d_total_size 8-byte, d_flags 4-byte aligned; a non-final shard a multiple of 256 bytes)
-   return DENSITY_B200_EARG before any collective is enqueued. */
+   seam verdict -> optional gather. Uses its own shard state in the handle; nothing blocks unless gather_root >= 0. */
 DENSITY_B200_API int density_b200_encode_sharded_protected(density_b200_sharded*, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                           uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
                                           uint8_t* d_gather, size_t gather_cap, void* stream);
@@ -283,14 +289,14 @@ DENSITY_B200_API density_b200_cl_shard* density_b200_cl_shard_create(int alg);
 DENSITY_B200_API void density_b200_cl_shard_destroy(density_b200_cl_shard*);
 /* u32 words of one table of `kind` (DENSITY_B200_CL_TABLE_P / _C); 0 for a bad algorithm or kind */
 DENSITY_B200_API size_t density_b200_cl_table_words(int alg, int kind);
-/* phase 1: d_in 4-byte aligned. d_prev_quad: device pointer to the last quad (4 bytes) of the stream before this shard, NULL for the
+/* phase 1: d_prev_quad: device pointer to the last quad (4 bytes) of the stream before this shard, NULL for the
    first shard, which alone runs the copy-map iteration (as the single-device encoder) and exports straight from its settled round.
    Exports the shard's P table. Phases 2 and 3 read d_in again: it must stay valid and unchanged until phase 3 has been enqueued. */
 DENSITY_B200_API int density_b200_cl_shard_phase1(density_b200_cl_shard*, const uint8_t* d_in, size_t n, int is_last_shard,
                                  const uint32_t* d_prev_quad, uint32_t* d_table_p_out, void* stream);
 /* phase 2: d_carry_p = the P state before this shard (NULL = stream start; the first shard ignores it). Exports the shard's C table. */
 DENSITY_B200_API int density_b200_cl_shard_phase2(density_b200_cl_shard*, const uint32_t* d_carry_p, uint32_t* d_table_c_out, void* stream);
-/* phase 3: d_carry_c = the C state before this shard (NULL = stream start; the first shard ignores it). Writes the shard's piece to d_out (2-byte aligned), its size
+/* phase 3: d_carry_c = the C state before this shard (NULL = stream start; the first shard ignores it). Writes the shard's piece to d_out, its size
    to *d_out_size and its 8 seam words to d_seam8 in the layout of density_b200_decode_shard_phase2 ("last block incompressible" =
    previous_incompressible at the shard end; word 2 = this shard is refused). The verdict over all shards is that of the Chameleon
    sharded paths: non-zero when a word 2 is set or a seam joins two incompressible blocks. One phase 3 per phase 1. */
@@ -336,9 +342,8 @@ DENSITY_B200_API int density_b200_encode_sharded_cl(density_b200_sharded*, int a
  *              none met 0xFFFF: every later kernel returns at once).
  * After at least one round, prot_finish emits. Every shard runs the same number of rounds; at most density_b200_prot_round_budget()
  * (prot_p returns DENSITY_B200_EARG beyond it). Per round and rank that is the P table (0.5 MiB Cheetah, 3 MiB Lion), the C table
- * (0.75 MiB), 800 bytes of transfer and 32 bytes of round words. Phases called out of order (a quiet density_b200_cl_shard_phase1 on the
- * handle closes them), misaligned pointers (d_in and tables 4-byte, d_out 2-byte, d_out_size 8-byte), an offset that is not a multiple
- * of 256 and a non-final shard that is not a multiple of 256 bytes return DENSITY_B200_EARG without enqueuing anything.
+ * (0.75 MiB), 800 bytes of transfer and 32 bytes of round words. A quiet density_b200_cl_shard_phase1 on the handle closes the prot
+ * phases; an offset that is not a multiple of 256 returns DENSITY_B200_EARG.
  */
 #define DENSITY_B200_CL_PROT_ROUND_WORDS 8
 /* phase 1: the shard at the stream start (offset 0, n > 0) runs the staged copy-map iteration; the others take the empty map. Writes
@@ -368,8 +373,7 @@ DENSITY_B200_API int density_b200_cl_shard_prot_status(density_b200_cl_shard*, u
    ncclAllGather(shard lengths, 8 bytes per rank), which the call waits for (the offsets decide which shard runs the staged iteration)
    -> phase 1 -> ncclAllGather(round words, 32 bytes) -> the round budget of {P -> ncclAllGather(P tables) -> fold kernel -> C ->
    ncclAllGather(C tables) -> fold kernel -> transfer -> ncclAllGather(transfers, 800 bytes) -> settle -> ncclAllGather(round words,
-   32 bytes) -> commit} -> finish -> ncclAllGather(seam words) -> verdict -> optional gather. Uses its own workspace in the handle. Bad
-   arguments (those of density_b200_encode_sharded_protected, and alg) return DENSITY_B200_EARG before any collective is enqueued. */
+   32 bytes) -> commit} -> finish -> ncclAllGather(seam words) -> verdict -> optional gather. Uses its own workspace in the handle. */
 DENSITY_B200_API int density_b200_encode_sharded_cl_protected(density_b200_sharded*, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out,
                                              size_t cap, uint64_t* d_out_size, uint32_t* d_flags, uint64_t* d_total_size, int gather_root,
                                              uint8_t* d_gather, size_t gather_cap, void* stream);

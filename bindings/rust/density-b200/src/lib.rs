@@ -36,6 +36,9 @@ unsafe extern "C" {
     // the length a stream decodes to, without decoding it: {size, verdict} to d_result (device) / DENSITY_B200_OK with *out_size
     pub fn density_b200_decoded_size_device(alg: c_int, d_in: *const u8, n: usize, d_result: *mut u64, stream: *mut c_void) -> c_int;
     pub fn density_b200_decoded_size(alg: c_int, input: *const u8, n: usize, out_size: *mut u64) -> c_int;
+    // bytes [first, first + len) of what a Chameleon stream decodes to: {written, size, verdict} to d_result (device) / *written
+    pub fn density_b200_chameleon_decode_range_device(d_in: *const u8, n: usize, first: u64, len: u64, d_out: *mut u8, d_result: *mut u64, stream: *mut c_void) -> c_int;
+    pub fn density_b200_chameleon_decode_range(input: *const u8, n: usize, first: u64, output: *mut u8, len: u64, written: *mut u64) -> c_int;
     // a reused Codec instance (codec.rs:16,72,82)
     pub fn density_b200_codec_create(alg: c_int) -> *mut RawCodec;
     pub fn density_b200_codec_destroy(codec: *mut RawCodec);
@@ -112,6 +115,19 @@ macro_rules! algorithm {
 algorithm!(Chameleon, 0, chameleon_encode, chameleon_decode, chameleon_safe_encode_buffer_size, 256, 8, 8); // chameleon.rs:138-147
 algorithm!(Cheetah, 1, cheetah_encode, cheetah_decode, cheetah_safe_encode_buffer_size, 128, 4, 8); // cheetah.rs:188-197
 algorithm!(Lion, 2, lion_encode, lion_decode, lion_safe_encode_buffer_size, 64, 4, 6); // lion.rs:317-326
+
+impl Chameleon {
+    /// Bytes `[first, first + output.len())` of what `input` decodes to, without decoding the bytes in front of them: the bytes written,
+    /// `min(first + output.len(), S) - first`, or 0 when `first >= S` (S: the decoded size). `Err` where `decode` fails at any capacity
+    /// (a malformed stream) or the library could not run.
+    pub fn decode_range(input: &[u8], first: u64, output: &mut [u8]) -> Result<usize, DecodeError> {
+        let mut written: u64 = 0;
+        let rc = unsafe {
+            density_b200_chameleon_decode_range(input.as_ptr(), input.len(), first, output.as_mut_ptr(), output.len() as u64, &mut written)
+        };
+        if rc == 0 { usize::try_from(written).map_err(|_| DecodeError {}) } else { Err(DecodeError {}) }
+    }
+}
 
 #[cfg(test)]
 mod tests {

@@ -7,7 +7,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libdensity_b200.so")
-SOURCES = ["api.cu", "chameleon_encode.cu", "chameleon_decode.cu", "cheetah_encode.cu", "cl_decode.cu", "scalar_codec.cu", "decoded_size.cu"]
+SOURCES = ["api.cu", "chameleon_encode.cu", "chameleon_decode.cu", "cheetah_encode.cu", "cl_decode.cu", "scalar_codec.cu", "decoded_size.cu",
+           "decode_range.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--cudart", "static",

@@ -134,6 +134,21 @@ class Chameleon(_Codec):
     """chameleon.rs:138-147"""
     NAME, _BLOCK, _UNIT, _SIG = "chameleon", 256, 8, 8
 
+    @classmethod
+    def decode_range(cls, input, first, output):
+        """Decode bytes [first, first + len(output)) of what `input` decodes to into `output`, without decoding the bytes in front of
+        them; returns the number of bytes written, min(first + len(output), S) - first or 0 when first >= S (S: the decoded size).
+        Host buffers or torch CUDA tensors of any alignment. Raises DecodeError when the stream is malformed."""
+        ip, n, k1 = _ptr_len(input)
+        op, cap, k2 = _ptr_len(output, writable=True)
+        written = ctypes.c_uint64(0)
+        rc = _lib.load().density_b200_chameleon_decode_range(ip, n, first, op, cap, ctypes.byref(written))
+        if rc == _EMALFORMED:
+            raise DecodeError(_lib.last_error() or "malformed stream")
+        if rc != 0:
+            raise _lib.DensityB200Error(f"density_b200_chameleon_decode_range rc={rc}: {_lib.last_error()}")
+        return written.value
+
 
 class Cheetah(_Codec):
     """cheetah.rs:188-197"""
@@ -224,3 +239,15 @@ def decoded_size_device(alg, d_in, n_in, d_result, stream=None):
     rc = L.density_b200_decoded_size_device(ALG_IDS[alg], d_in.data_ptr(), n_in, d_result.data_ptr(), _stream_handle(stream))
     if rc != 0:
         raise DecodeError(f"density_b200_decoded_size_device rc={rc}: {_lib.last_error()}")
+
+
+def decode_range_device(d_in, n_in, first, d_out, d_result, stream=None):
+    """Enqueue the Chameleon range decode of bytes [first, first + d_out.numel()) of what the first `n_in` bytes of CUDA uint8 tensor
+    `d_in` decode to, into CUDA uint8 tensor `d_out`, on `stream` (default: torch's current stream). `d_result` is a CUDA int64/uint64
+    tensor of three elements that receives {bytes written, decoded size, verdict}, verdict 0 or 3 (DENSITY_B200_EMALFORMED). The call
+    returns once the stream's earlier work and the block-boundary walk are done; the decode itself is left enqueued."""
+    L = _lib.load()
+    rc = L.density_b200_chameleon_decode_range_device(d_in.data_ptr(), n_in, first, d_out.numel(), d_out.data_ptr(), d_result.data_ptr(),
+                                                        _stream_handle(stream))
+    if rc != 0:
+        raise DecodeError(f"density_b200_chameleon_decode_range_device rc={rc}: {_lib.last_error()}")

@@ -692,6 +692,97 @@ int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t*
     return DENSITY_B200_OK;
 }
 
+// ---- Chameleon range decode (decode_range.cu) --------------------------------------------------------------------------------------
+// n > 0, len > 0, d_in 2-byte aligned; on the device's workspace like decode_device. The locate step runs first and the host waits for
+// it on `stream` (the pieces' lengths size the rest); then the pieces are decoded and the w window bytes copied to out: device memory
+// (d_out) or, out_host, host memory (the synchronous entry). *h3 = {w, S, verdict}; d_result receives the same in stream order.
+static int range_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t first, uint64_t len, uint8_t* out, bool out_host,
+                        uint64_t* d_result, cudaStream_t stream, uint64_t h3[3]) {
+    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const char* what = "range decode locate";
+    cudaError_t e = c->ws.ensure(range_locate_workspace_bytes(n), stream);
+    if (e == cudaSuccess) e = range_locate_launch(d_in, n, first, len, c->ws.p, d_result, stream, &launches);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_size, c->ws.p, RANGE_REPORT_WORDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    RangePlan p{};
+    bool planned = false;
+    if (e == cudaSuccess) {
+        for (int k = 0; k < 3; ++k) h3[k] = c->h_size[k];
+        planned = range_plan(c->h_size, n, first, c->num_sms, &p);
+    }
+    if (e == cudaSuccess && planned && p.w) {
+        const uint8_t* window = nullptr;
+        what = "range decode workspace";
+        e = c->ws.ensure(p.ws_bytes, stream);
+        if (e == cudaSuccess) { what = "range decode launch"; e = range_decode_launch(d_in, p, c->ws.p, c->num_sms, stream, &launches, &window); }
+        if (e == cudaSuccess) {
+            what = "range decode window copy";
+            e = out_host ? d2h_any(c->ring_out, out, window, p.w, stream, is_pageable_host(out))
+                         : cudaMemcpyAsync(out, window, p.w, cudaMemcpyDeviceToDevice, stream);
+        }
+    }
+    ws_release(c, stream);
+    const int rc = step_result(e, launches, what);
+    if (rc == DENSITY_B200_OK && !planned) { set_error("range decode: the locate step's report is inconsistent"); return DENSITY_B200_ECUDA; }
+    return rc;
+}
+
+int density_b200_chameleon_decode_range_device(const uint8_t* d_in, size_t n, uint64_t first, uint64_t len, uint8_t* d_out, uint64_t* d_result,
+                                               void* stream) {
+    g_last_error.clear();
+    if (!d_result || (!d_in && n) || (!d_out && len)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_result) & 7)) {
+        set_error("chameleon_decode_range_device: d_in must be 2-byte and d_result 8-byte aligned");
+        return DENSITY_B200_EARG;
+    }
+    DeviceCtx* c = current_ctx();
+    if (!c) return DENSITY_B200_ECUDA;
+    std::lock_guard<std::mutex> lk(c->mu);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (n == 0 || len == 0) {      // nothing to write (codec.rs:102 for an empty stream); no kernel
+        const cudaError_t e = cudaMemsetAsync(d_result, 0, 3 * sizeof(uint64_t), s);
+        if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
+        return DENSITY_B200_OK;
+    }
+    uint64_t h3[3];
+    return range_locked(c, d_in, n, first, len, d_out, false, d_result, s, h3);
+}
+
+int density_b200_chameleon_decode_range(const uint8_t* input, size_t n, uint64_t first, uint8_t* output, uint64_t len, uint64_t* written) {
+    g_last_error.clear();
+    if (!written || (!input && n) || (!output && len)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    *written = 0;
+    if (n == 0 || len == 0) return DENSITY_B200_OK;
+    DeviceCtx* c = current_ctx();
+    if (!c) return DENSITY_B200_ECUDA;
+    std::lock_guard<std::mutex> lk(c->mu);
+    const bool in_dev = is_device_pointer(input), out_dev = is_device_pointer(output);
+    cudaError_t e;
+    if (in_dev || out_dev) {
+        // synchronous, and it cannot know which stream produced or reads the buffers: wait for all of them (as run_sync)
+        e = cudaDeviceSynchronize();
+        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return DENSITY_B200_ECUDA; }
+    }
+    const uint8_t* d_in = input;
+    if (!in_dev || (reinterpret_cast<uintptr_t>(input) & 1)) {     // host buffers, and device buffers at an odd address, go through stage_in
+        e = c->stage_in.ensure(n + 16, c->stream);
+        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        e = in_dev ? cudaMemcpyAsync(c->stage_in.p, input, n, cudaMemcpyDeviceToDevice, c->stream)
+                   : h2d_any(c->ring_in, c->stage_in.p, input, n, c->stream, is_pageable_host(input));
+        if (e != cudaSuccess) { set_error("input copy", e); return DENSITY_B200_ECUDA; }
+        d_in = c->stage_in.p;
+    }
+    uint64_t h3[3] = {0, 0, 0};
+    const int rc = range_locked(c, d_in, n, first, len, output, !out_dev, c->d_size, c->stream, h3);
+    e = cudaStreamSynchronize(c->stream);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (e != cudaSuccess) { set_error("stream sync", e); return DENSITY_B200_ECUDA; }
+    if (h3[2] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
+    *written = h3[0];
+    return DENSITY_B200_OK;
+}
+
 // ---- the argument rule of the sharded entries (include/density_b200.h, "Sharded encode" and "Sharded decode"). Each helper returns
 // DENSITY_B200_EARG with the error set, or DENSITY_B200_OK.
 static bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }

@@ -233,12 +233,35 @@ __device__ __forceinline__ void sw_jump(Protection& ps, uint32_t nb, uint32_t la
     ps.counter += nb;
     ps.previous_incompressible = last_inc;
 }
-template <class T>
+// The stop-and-report mode (STOP = true, the range decode, DESIGN §4g): for the two block indices in `block`, where that block starts
+// and the automaton state in front of it, to out[STOP_WORDS * i ..] = {1, stream offset, penalty | start << 8 | previous_incompressible
+// << 16} when the main loop reaches it (block main_blocks included: the tail loop's start). In this mode the walk jumps no group and no
+// chunk that holds a stop strictly inside, so it meets every stop on a block boundary.
+constexpr uint32_t STOP_WORDS = 4;
+struct WalkStops { uint64_t block[2]; unsigned long long* out; };
+__device__ __forceinline__ unsigned long long stop_state(const Protection& ps) {
+    return ps.copy_penalty | (ps.copy_penalty_start << 8) | ((unsigned long long)ps.previous_incompressible << 16);
+}
+// STOP: the state in front of block b at stream offset i; whether a stop lies strictly inside the nb blocks from block b
+template <bool STOP>
+__device__ __forceinline__ void stop_at(const WalkStops& w, uint64_t b, uint64_t i, const Protection& ps) {
+    if constexpr (STOP)
+        for (int k = 0; k < 2; ++k)
+            if (b == w.block[k]) { unsigned long long* o = w.out + STOP_WORDS * k; o[0] = 1; o[1] = i; o[2] = stop_state(ps); }
+}
+template <bool STOP>
+__device__ __forceinline__ bool stop_inside(const WalkStops& w, uint64_t b, uint32_t nb) {
+    if constexpr (!STOP) return false;
+    const uint64_t e = b + nb;
+    return (w.block[0] > b && w.block[0] < e) || (w.block[1] > b && w.block[1] < e);
+}
+template <class T, bool STOP = false>
 __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, uint32_t nchunks,
                                                            const uint32_t* __restrict__ res, const uint4* __restrict__ gres, uint32_t ngroups,
                                                            uint32_t* __restrict__ g_entry, uint64_t* __restrict__ g_blockbase,
                                                            uint32_t* __restrict__ c_entry, uint64_t* __restrict__ c_blockbase,
-                                                           uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st) {
+                                                           uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st,
+                                                           WalkStops stops = WalkStops{}) {
     if (!(st->nonquiet & 1u)) return;
     constexpr uint32_t SW_LOAD = T::CH + 16;            // + the signature bytes of a block starting at the chunk's last bytes, rounded up to 16
     __shared__ __align__(16) uint8_t win[2][SW_LOAD];   // the chunk being walked + the next one, prefetched during the walk
@@ -256,13 +279,14 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
         if (tid == 0) {
             uint32_t cmd = SW_DONE, c = 0;
             while (n - idx >= T::MAXBLK) {
+                stop_at<STOP>(stops, b, idx, ps);
                 c = (uint32_t)(idx / T::CH);
                 const uint32_t e = (uint32_t)(idx - (uint64_t)c * T::CH) >> 1;          // < NCAND: a block is at most MAXBLK bytes
                 if (c / GROUP == g_next) {
                     // entering a group of 64 chunks: jump over all of it if the automaton provably stays in encoded mode inside
                     const uint32_t g = g_next++;
                     const uint4 gr = gres[(size_t)g * T::NCAND + e];
-                    if (ps.copy_penalty == 0 && gr.x != TERM && !(gr.z & 9u) && !(ps.previous_incompressible && (gr.z & 2u))) {
+                    if (ps.copy_penalty == 0 && gr.x != TERM && !(gr.z & 9u) && !(ps.previous_incompressible && (gr.z & 2u)) && !stop_inside<STOP>(stops, b, gr.y)) {
                         g_entry[g] = e; g_blockbase[g] = b;
                         sw_jump(ps, gr.y, (gr.z >> 2) & 1u);
                         b += gr.y;
@@ -274,7 +298,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
                 if (c < cb || c >= cb + cb_valid) { cmd = SW_ROWS; break; }
                 const uint32_t r = rows[(c - cb) * T::NCAND + e];
                 const uint32_t ex = r & 0xFFu, fl = row_x<T>(r);
-                if (ps.copy_penalty == 0 && ex != TERM && !(fl & 1u) && !(ps.previous_incompressible && (fl & 2u))) {
+                if (ps.copy_penalty == 0 && ex != TERM && !(fl & 1u) && !(ps.previous_incompressible && (fl & 2u)) && !stop_inside<STOP>(stops, b, row_nb<T>(r))) {
                     const uint32_t nb = row_nb<T>(r);
                     c_entry[c] = e; c_blockbase[c] = b;
                     sw_jump(ps, nb, (fl >> 2) & 1u);
@@ -318,6 +342,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
                 const uint64_t wend = wbase + T::CH;
                 c_entry[c] = TERM;                                           // dec_block_offsets leaves this chunk alone
                 while (idx < wend && n - idx >= T::MAXBLK) {
+                    stop_at<STOP>(stops, b, idx, ps);
                     if (ps.revert_to_copy()) {                               // codec.rs:89-92
                         if (b < maxblocks) blk_off[b] = idx | BLK_COPY;
                         ++b; idx += T::BS; ps.decay();
@@ -343,6 +368,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
         for (uint32_t g = s_gnext + tid; g < ngroups; g += SW_THREADS) g_entry[g] = G_SKIP;
     }
     if (tid == 0) {
+        stop_at<STOP>(stops, b, idx, ps);
         st->main_blocks = b; st->tail_off = idx;
         st->ps_penalty = ps.copy_penalty; st->ps_start = ps.copy_penalty_start; st->ps_prev = ps.previous_incompressible;
         st->seq = 1;
@@ -712,13 +738,16 @@ struct TailWalk {
     uint32_t copied, bad;   // a copy-mode block; a malformed block
     Protection ps;          // protection state when the tail loop stops
 };
-template <class F>
-__device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain) {
+// at_block(j, offset, state) sees the tail's block j before the tail loop enters it (the range decode's stops behind the main loop)
+struct NoBlockHook { __device__ void operator()(uint64_t, uint64_t, const Protection&) const {} };
+template <class F, class G = NoBlockHook>
+__device__ TailWalk tail_walk(const uint8_t* __restrict__ in, uint64_t n, const DecStatus* __restrict__ st, F plain, G at_block = G()) {
     TailWalk w; w.blocks = 0; w.out = 0; w.first_inc = 0; w.copied = 0; w.bad = 0;
     Protection& ps = w.ps;
     ps = main_end_state(st);
     uint64_t idx = st->tail_off;
     while (n - idx > 0) {
+        at_block(w.blocks, idx, ps);
         ++w.blocks;
         if (ps.revert_to_copy()) {
             w.copied = 1;
@@ -800,6 +829,27 @@ inline uint32_t rows_launch(const uint8_t* d_in, size_t n_walk, size_t n_visible
     dec_group_compose<T><<<ngroups, 160, 0, stream>>>(res, nchunks, reinterpret_cast<uint4*>(ws + L.gres));
     *launches += 2;
     return ngroups;
+}
+
+// Enqueues the exact in-order main loop of the whole stream d_in[0 .. n), n > 0, with no block offsets stored and no capacity (the
+// decoded-size query and the range decode's locate step): a fresh status with nonquiet bit 0 set, which is dec_seq_walk's gate (the
+// little-endian low byte of the word), the candidate rows, then dec_seq_walk, in stop-and-report mode when STOP. Afterwards (on the
+// stream) st->main_blocks / tail_off and the automaton state behind the main loop. 3 kernels; the scratch is bounds_layout<T>(n, 0).
+template <class T, bool STOP = false>
+inline cudaError_t forced_walk_launch(const uint8_t* d_in, size_t n, uint8_t* ws, const BoundsLayout& L, cudaStream_t stream, uint64_t* launches,
+                                      WalkStops stops = WalkStops{}) {
+    DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.status);
+    cudaError_t e = cudaMemsetAsync(st, 0, sizeof(DecStatus), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(&st->nonquiet, 1, 1, stream);
+    if (e != cudaSuccess) return e;
+    const uint32_t nchunks = (uint32_t)((n + T::CH - 1) / T::CH);
+    const uint32_t ngroups = rows_launch<T>(d_in, n, n, ws, L, stream, launches);
+    dec_seq_walk<T, STOP><<<1, SW_THREADS, 0, stream>>>(
+        d_in, n, ~0ull, nchunks, reinterpret_cast<const uint32_t*>(ws + L.res), reinterpret_cast<const uint4*>(ws + L.gres), ngroups,
+        reinterpret_cast<uint32_t*>(ws + L.g_entry), reinterpret_cast<uint64_t*>(ws + L.g_blockbase), reinterpret_cast<uint32_t*>(ws + L.c_entry),
+        reinterpret_cast<uint64_t*>(ws + L.c_blockbase), nullptr, 0, st, stops);
+    ++*launches;
+    return cudaGetLastError();
 }
 
 // Enqueues the boundary kernels. Afterwards (on the stream): st->main_blocks / tail_off / protection state, blk_off[0 .. main_blocks).

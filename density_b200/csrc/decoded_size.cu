@@ -80,19 +80,10 @@ __global__ void dec_size_tail(const uint8_t* __restrict__ in, uint64_t n, const 
 template <class T>
 static cudaError_t launch(const uint8_t* d_in, size_t n, uint8_t* ws, uint64_t* d_result, cudaStream_t stream, uint64_t* launches) {
     bounds::BoundsLayout L; bounds::bounds_layout<T>(n, 0, &L);
-    DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.status);
-    // a fresh status with nonquiet bit 0 set, which is dec_seq_walk's gate (the little-endian low byte of the word)
-    cudaError_t e = cudaMemsetAsync(st, 0, sizeof(DecStatus), stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(&st->nonquiet, 1, 1, stream);
+    const cudaError_t e = bounds::forced_walk_launch<T>(d_in, n, ws, L, stream, launches);
     if (e != cudaSuccess) return e;
-    const uint32_t nchunks = (uint32_t)((n + T::CH - 1) / T::CH);
-    const uint32_t ngroups = bounds::rows_launch<T>(d_in, n, n, ws, L, stream, launches);
-    bounds::dec_seq_walk<T><<<1, bounds::SW_THREADS, 0, stream>>>(
-        d_in, n, ~0ull, nchunks, reinterpret_cast<const uint32_t*>(ws + L.res), reinterpret_cast<const uint4*>(ws + L.gres), ngroups,
-        reinterpret_cast<uint32_t*>(ws + L.g_entry), reinterpret_cast<uint64_t*>(ws + L.g_blockbase), reinterpret_cast<uint32_t*>(ws + L.c_entry),
-        reinterpret_cast<uint64_t*>(ws + L.c_blockbase), nullptr, 0, st);
-    dec_size_tail<T><<<1, 32, 0, stream>>>(d_in, n, st, reinterpret_cast<unsigned long long*>(d_result));
-    *launches += 2;
+    dec_size_tail<T><<<1, 32, 0, stream>>>(d_in, n, reinterpret_cast<const DecStatus*>(ws + L.status), reinterpret_cast<unsigned long long*>(d_result));
+    ++*launches;
     return cudaGetLastError();
 }
 

@@ -256,4 +256,23 @@ size_t decoded_size_workspace_bytes(int alg, size_t nbytes);
 cudaError_t decoded_size_launch(int alg, const uint8_t* d_in, size_t nbytes, uint8_t* ws, uint64_t* d_result, cudaStream_t stream,
                                 uint64_t* launches);
 
+// decode_range.cu: Chameleon range decode, d_in 2-byte aligned, nbytes > 0, len > 0. The locate step (4 kernels, scratch
+// range_locate_workspace_bytes) writes {w, S, verdict} to d_result (3 x u64) and RANGE_REPORT_WORDS u64 to the workspace's start; the
+// host reads them and range_plan turns them into the pieces (false: the report is inconsistent), whose decode range_decode_launch
+// enqueues on a workspace of plan.ws_bytes (the report may be gone by then): 13 kernels for first < 256, else 26. *d_window: the w
+// window bytes in that workspace, in stream order.
+constexpr uint32_t RANGE_REPORT_WORDS = 8;
+struct RangePlan {
+    uint64_t w, k0, skip, off0, piece_n, stage_cap;    // skip: first - 256 k0, the window's offset in the staging
+    uint32_t cand0;
+    bool final_piece;
+    size_t window_ws, ws_bytes;
+};
+size_t range_locate_workspace_bytes(size_t nbytes);
+cudaError_t range_locate_launch(const uint8_t* d_in, size_t nbytes, uint64_t first, uint64_t len, uint8_t* ws, uint64_t* d_result,
+                                cudaStream_t stream, uint64_t* launches);
+bool range_plan(const uint64_t* report, size_t nbytes, uint64_t first, int num_sms, RangePlan* p);
+cudaError_t range_decode_launch(const uint8_t* d_in, const RangePlan& p, uint8_t* ws, int num_sms, cudaStream_t stream, uint64_t* launches,
+                                const uint8_t** d_window);
+
 }  // namespace dns

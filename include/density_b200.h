@@ -143,6 +143,40 @@ DENSITY_B200_API int density_b200_decoded_size_device(int alg, const uint8_t* d_
 DENSITY_B200_API int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t* out_size);
 
 /*
+ * Chameleon range decode: bytes [first, first + len) of what a stream decodes to, without decoding the bytes in front of them and
+ * without an output buffer of the decoded size. Let D = chameleon_decode(stream) with enough capacity and S = len(D). A range decode
+ *   - writes w = min(first + len, S) - first bytes to d_out, or 0 bytes when first >= S, and those bytes are D[first : first + w];
+ *   - writes nothing outside [d_out, d_out + w); d_out may have any alignment;
+ *   - writes 0 bytes and reports DENSITY_B200_EMALFORMED when the stream is malformed, in the sense of density_b200_decoded_size (decode
+ *     writes 0 at any capacity). The check covers the whole stream, not only the blocks in front of the window, so a window is always
+ *     a slice of what decode returns.
+ * Chameleon's state at a block boundary depends on no decoded value: the dictionary in front of block k holds the last PLAIN quad
+ * before k of each bucket, and the protection automaton reads signatures only. So the call walks the block boundaries of the whole
+ * stream (as density_b200_decoded_size does), rebuilds the dictionary in front of block k0 = first / 256 from the PLAIN quads of the
+ * prefix (no decode pass, no output), and decodes blocks k0 .. k1 (k1: the block of the window's last byte) with the sharded decode's
+ * piece machinery, entered in the located automaton state. Cost: about a boundary walk of the stream plus the prefix's writer pass plus
+ * a decode of the window's blocks.
+ * Scratch (the device's shared workspace): the boundary rows of the stream (3-7 % of n), the workspace of a decode of the blocks up to
+ * k1 (block offsets, run tables) and staging for the window's decoded blocks, (k1 - k0 + 1) x 256 bytes, or S - 256 k0 when the window
+ * ends in the tail loop's blocks (at most two blocks more). Nothing scales with S beyond block k1.
+ * Cheetah and Lion have no range entry: their state at a block is the prediction map, keyed by the contexts of decoded quads, so the
+ * state in front of a window costs a decode of the whole prefix, which would save neither time nor memory over decode itself.
+ *
+ * Stream-ordered: d_in device, 2-byte aligned; d_out device, any alignment; d_result device, 8-byte aligned, receives three u64 {bytes
+ * written w, S, verdict}, verdict 0 or DENSITY_B200_EMALFORMED (then w and S are 0). The call enqueues the boundary walk (4 kernels),
+ * then waits on `stream` for it, because the lengths of the pieces it decodes size their grids: it returns when the work enqueued on
+ * `stream` before it and the walk are done, with the rest enqueued. Then, when w > 0: 13 kernels when first < 256, else 26, and one
+ * copy. n == 0 or len == 0: no kernel, {0, 0, 0} by a memset (S is not computed). DENSITY_B200_EARG (a NULL pointer, a misaligned d_in
+ * or d_result) enqueues nothing. The call uses the device's shared workspace (see "Concurrent callers" above).
+ */
+DENSITY_B200_API int density_b200_chameleon_decode_range_device(const uint8_t* d_in, size_t n, uint64_t first, uint64_t len, uint8_t* d_out,
+                                                                uint64_t* d_result, void* stream);
+/* Synchronous; host or device pointers of any alignment, like the nine reference symbols. DENSITY_B200_OK with *written = w,
+   DENSITY_B200_EMALFORMED (*written = 0), DENSITY_B200_EARG or DENSITY_B200_ECUDA. */
+DENSITY_B200_API int density_b200_chameleon_decode_range(const uint8_t* input, size_t n, uint64_t first, uint8_t* output, uint64_t len,
+                                                         uint64_t* written);
+
+/*
  * Sharded encode. Every entry of the phase APIs of a Chameleon, Cheetah or Lion shard below, density_b200_table_init / _fold,
  * density_b200_cl_table_init / _fold and every density_b200_encode_sharded* driver takes its pointers by one rule: d_in and d_prev_quad
  * 4-byte aligned; d_out 2-byte aligned; every table, carry, transfer, word and flag buffer 4-byte aligned; d_out_size and d_total_size

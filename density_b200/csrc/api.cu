@@ -211,15 +211,30 @@ struct DeviceCtx {
     static constexpr int PROF_RING = 64;
     cudaEvent_t ev[PROF_RING][4] = {};
     uint64_t prof_count = 0;           // encodes recorded since profile_enable(1)
-    // One workspace per device: a call may only start using it when the previous call (on whatever stream) has finished with it.
-    // Every enqueue ends with cudaEventRecord(ws_free, its stream) and starts with cudaStreamWaitEvent(its stream, ws_free).
-    const void* last_cl_status = nullptr;   // iteration status block of the last parallel Cheetah decode (diagnostics)
-    // the walk counts of the last Lion decode, copied out of the workspace (which later calls reuse and may reallocate) behind the walk;
-    // lion_stats_valid is cleared when a Lion decode runs on the in-order kernel (diagnostics)
-    DevBuf lion_stats; bool lion_stats_valid = false;
+    // the diagnostics of the last run-parallel decodes, copied out of the workspace (which later calls reuse and may reallocate) behind
+    // the decode: bytes 0-31 the 8 status words of the last run-parallel Cheetah decode, bytes 32-63 the 4 walk counts of the last Lion
+    // decode. lion_stats_valid is cleared when a Lion decode runs on the in-order kernel
+    DevBuf diag; bool chee_rounds_valid = false, lion_stats_valid = false;
+    // One workspace per device: a call may only start using it when the previous call (on whatever stream) has finished with it (WsLease).
     cudaEvent_t ws_free = nullptr;
     bool ws_free_recorded = false;
     std::mutex mu;
+
+    // frees everything the context owns and resets every flag, so that the next current_ctx() sets it up afresh (device dev is current)
+    void release() {
+        for (DevBuf* b : {&ws, &stage_in, &stage_out, &pipe_tables, &dec_tables, &diag}) b->release();
+        for (auto& tables : chee_tables) for (DevBuf& b : tables) b.release();
+        ring_in.release(); ring_out.release();
+        for (cudaStream_t* s : {&stream, &h2d_stream, &d2h_stream}) { if (*s) cudaStreamDestroy(*s); *s = nullptr; }
+        for (cudaEvent_t* e : {&ev_h2d[0], &ev_h2d[1], &ws_free}) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
+        for (auto& set : ev) for (cudaEvent_t& e : set) { if (e) cudaEventDestroy(e); e = nullptr; }
+        if (d_size) cudaFree(d_size);
+        for (void* p : {(void*)h_size, (void*)h_sizes}) if (p) cudaFreeHost(p);
+        d_size = h_size = h_sizes = nullptr;
+        chee_epoch = 0; layout = ChamLayout{}; last_was_chameleon_fastpath_capable = 0;
+        profile = false; prof_count = 0;
+        chee_rounds_valid = lion_stats_valid = ws_free_recorded = ready = false;
+    }
 };
 
 constexpr int MAX_DEVICES = 64;
@@ -268,30 +283,28 @@ static bool is_device_pointer(const void* p) {
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+// The device's workspace, held by a call on `stream` for the lease's lifetime: the constructor makes the stream wait until the previous
+// holder's work (on whatever stream) is done with it, the destructor records ws_free on the stream. ok is false, with the error set,
+// when the wait could not be enqueued; then nothing is recorded.
+struct WsLease {
+    DeviceCtx* c; cudaStream_t stream; bool ok = true;
+    WsLease(DeviceCtx* c_, cudaStream_t s) : c(c_), stream(s) {
+        if (!c->ws_free_recorded) return;
+        const cudaError_t e = cudaStreamWaitEvent(stream, c->ws_free, 0);
+        if (e != cudaSuccess) { set_error("cudaStreamWaitEvent", e); ok = false; }
+    }
+    ~WsLease() { if (ok && cudaEventRecord(c->ws_free, stream) == cudaSuccess) c->ws_free_recorded = true; }
+    WsLease(const WsLease&) = delete;
+    WsLease& operator=(const WsLease&) = delete;
+};
+
 // path: 0 auto (fast path with exact fallback), 1 fast only (no fallback), 2 protected walk only, 3 scalar kernel
 // path 4 (internal): Chameleon auto path for callers that may block on the stream (the synchronous reference-facing entry points): the
 // copy-map iteration gets up to 12 more batches of 8 rounds before the in-order walk may take over
-static bool ws_acquire(DeviceCtx* c, cudaStream_t stream) {
-    if (!c->ws_free_recorded) return true;
-    cudaError_t e = cudaStreamWaitEvent(stream, c->ws_free, 0);
-    if (e != cudaSuccess) { set_error("cudaStreamWaitEvent", e); return false; }
-    return true;
-}
-static void ws_release(DeviceCtx* c, cudaStream_t stream) {
-    if (cudaEventRecord(c->ws_free, stream) == cudaSuccess) c->ws_free_recorded = true;
-}
-
-static int encode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                     uint64_t* d_out_size, cudaStream_t stream, int path);
 static int encode_device_locked(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                 uint64_t* d_out_size, cudaStream_t stream, int path) {
-    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
-    const int rc = encode_device_locked_impl(c, alg, d_in, n, d_out, cap, d_out_size, stream, path);
-    ws_release(c, stream);
-    return rc;
-}
-static int encode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                     uint64_t* d_out_size, cudaStream_t stream, int path) {
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
     cudaError_t e;
     const bool aligned = !(reinterpret_cast<uintptr_t>(d_in) & 3) && !(reinterpret_cast<uintptr_t>(d_out) & 1);
@@ -361,17 +374,10 @@ static int encode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
 }
 
 // path: 0 auto (parallel decoder with exact in-order fallback), 1 parallel only, 3 in-order kernel only
-static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                     uint64_t* d_out_size, cudaStream_t stream, int path);
 static int decode_device_locked(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                uint64_t* d_out_size, cudaStream_t stream, int path = 0) {
-    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
-    const int rc = decode_device_locked_impl(c, alg, d_in, n, d_out, cap, d_out_size, stream, path);
-    ws_release(c, stream);
-    return rc;
-}
-static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
-                                     uint64_t* d_out_size, cudaStream_t stream, int path) {
+                                uint64_t* d_out_size, cudaStream_t stream, int path) {
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
     cudaError_t e;
     const bool parallel_ok = alg == ALG_CHAMELEON && path != 3 && !(reinterpret_cast<uintptr_t>(d_in) & 1) && !(reinterpret_cast<uintptr_t>(d_out) & 3);
@@ -404,11 +410,11 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
         if (e == cudaSuccess) {
             const void* cl_st = nullptr;
             const void* b_st = (lion ? lion_decode_status_ptr : chee_decode_status_ptr)(c->ws.p, n, cap, c->num_sms, &cl_st);
-            if (!lion) c->last_cl_status = cl_st;
             e = scalar_decode_tail(alg, d_in, n, d_out, cap, tail_ws, b_st, cl_st, d_out_size, stream, &launches, d_fallback);
-            if (lion && e == cudaSuccess) e = c->lion_stats.ensure(64, stream);
-            if (lion && e == cudaSuccess) e = cudaMemcpyAsync(c->lion_stats.p, static_cast<const uint8_t*>(cl_st) + 32, 32, cudaMemcpyDeviceToDevice, stream);
-            if (lion) c->lion_stats_valid = e == cudaSuccess;
+            const size_t at = lion ? 32 : 0;   // Cheetah: the 8 status words at the block's start; Lion: the 4 walk counts at byte 32
+            if (e == cudaSuccess) e = c->diag.ensure(64, stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(c->diag.p + at, static_cast<const uint8_t*>(cl_st) + at, 32, cudaMemcpyDeviceToDevice, stream);
+            (lion ? c->lion_stats_valid : c->chee_rounds_valid) = e == cudaSuccess;
         }
         if (e == cudaSuccess && path != 1)
             e = scalar_decode(alg, d_in, n, d_out, cap, scalar_ws, d_out_size, stream, &launches, d_fallback);
@@ -429,16 +435,11 @@ static int decode_device_locked_impl(DeviceCtx* c, int alg, const uint8_t* d_in,
 constexpr size_t PIPE_CHUNK = 64u << 20;
 constexpr size_t PIPE_MIN_BYTES = 96u << 20;
 
-static size_t chameleon_encode_host_pipelined_impl(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap);
 // The pipeline runs on the device's one workspace like every other call: it waits on c->stream for the calls enqueued before it (on
 // whatever stream) and releases the workspace on every exit, the "not quiet" one included (the fallback then acquires it again).
 static size_t chameleon_encode_host_pipelined(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap) {
-    if (!ws_acquire(c, c->stream)) return 0;
-    const size_t r = chameleon_encode_host_pipelined_impl(c, in, n, out, out_cap);
-    ws_release(c, c->stream);
-    return r;
-}
-static size_t chameleon_encode_host_pipelined_impl(DeviceCtx* c, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap) {
+    const WsLease lease(c, c->stream);
+    if (!lease.ok) return 0;
     const size_t nchunks = (n + PIPE_CHUNK - 1) / PIPE_CHUNK;
     if (nchunks > 4096) return (size_t)-1;
     cudaError_t e = c->stage_in.ensure(n + 16, c->h2d_stream);
@@ -504,61 +505,110 @@ static size_t chameleon_encode_host_pipelined_impl(DeviceCtx* c, const uint8_t* 
     return out_off;
 }
 
+constexpr size_t OWN_OUTPUT = ~(size_t)0;   // SyncCall::run's stage_cap: the entry writes the caller's output itself
+
+// The frame of the synchronous host-or-device entries (the nine symbols, codec instances, decoded size, range decode). Constructing it
+// takes the context and its lock, and synchronises the device when a buffer is on it: the call cannot know which stream produced or
+// reads a device buffer. c is NULL, with the error set, when either fails.
+struct SyncCall {
+    DeviceCtx* c = current_ctx();
+    std::unique_lock<std::mutex> lk;
+    bool in_dev = false, out_dev = false;
+    const uint8_t* staged_in = nullptr;    // the input, when the entry has already put it in stage_in
+    SyncCall(const void* in, const void* out) {
+        if (!c) return;
+        lk = std::unique_lock<std::mutex>(c->mu);
+        in_dev = is_device_pointer(in);
+        out_dev = is_device_pointer(out);
+        const cudaError_t e = in_dev || out_dev ? cudaDeviceSynchronize() : cudaSuccess;
+        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); c = nullptr; }
+    }
+    // Stages the input: a host input through the pinned ring, and with stage_odd a device input at an odd address copied into stage_in
+    // (otherwise the kernels read a device input where it is). A host output is staged in stage_out, stage_cap bytes, unless stage_cap is
+    // OWN_OUTPUT. Then enqueue(d_in, d_out, d_cap) on c->stream, and the k result words at c->d_size are read back into c->h_size. A
+    // staged output gets c->h_size[0] bytes when that is in (0, out_cap]. Returns DENSITY_B200_OK, or an error code with the error set.
+    template <class F>
+    int run(const uint8_t* in, size_t n, bool stage_odd, uint8_t* out, size_t out_cap, size_t stage_cap, int k, F enqueue) {
+        cudaError_t e = cudaSuccess;
+        const uint8_t* d_in = staged_in ? staged_in : in;
+        if (!staged_in && (!in_dev || (stage_odd && (reinterpret_cast<uintptr_t>(in) & 1)))) {
+            e = c->stage_in.ensure(n + 16, c->stream);
+            if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
+            e = in_dev ? cudaMemcpyAsync(c->stage_in.p, in, n, cudaMemcpyDeviceToDevice, c->stream)
+                       : h2d_any(c->ring_in, c->stage_in.p, in, n, c->stream, is_pageable_host(in));
+            if (e != cudaSuccess) { set_error("input copy", e); return DENSITY_B200_ECUDA; }
+            d_in = c->stage_in.p;
+        }
+        const bool stage_out = !out_dev && stage_cap != OWN_OUTPUT;
+        if (stage_out) {
+            e = c->stage_out.ensure(stage_cap + 16, c->stream);
+            if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        }
+        const int rc = stage_out ? enqueue(d_in, c->stage_out.p, stage_cap) : enqueue(d_in, out, out_cap);
+        if (rc != DENSITY_B200_OK) { cudaStreamSynchronize(c->stream); return rc; }
+        e = cudaMemcpyAsync(c->h_size, c->d_size, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        if (e != cudaSuccess) { set_error("stream sync", e); return DENSITY_B200_ECUDA; }
+        const uint64_t produced = c->h_size[0];
+        if (!stage_out || produced == 0 || produced > out_cap) return DENSITY_B200_OK;
+        e = d2h_any(c->ring_out, out, c->stage_out.p, produced, c->stream, is_pageable_host(out));
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        if (e != cudaSuccess) { set_error("D2H copy", e); return DENSITY_B200_ECUDA; }
+        return DENSITY_B200_OK;
+    }
+};
+
+// what a synchronous encode or decode returns: the bytes it wrote (the result word), or 0 with the error set
+static size_t sync_bytes(int rc, const DeviceCtx* c, bool encode, size_t out_cap) {
+    if (rc != DENSITY_B200_OK) return 0;
+    const uint64_t produced = c->h_size[0];
+    if (produced == 0) { set_error(encode ? "encode failed on device (output capacity?)" : "decode failed on device (malformed stream or output capacity)"); return 0; }
+    if (produced > out_cap) { set_error("output buffer too small"); return 0; }
+    return (size_t)produced;
+}
+
 // Synchronous entry point shared by the nine reference-shaped symbols.
 static size_t run_sync(bool encode, int alg, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap) {
     g_last_error.clear();
     if ((!in && n) || (!out && out_cap)) { set_error("null pointer"); return 0; }
     if (n == 0) return 0;  // Codec::encode/decode of an empty slice writes nothing (codec.rs:76,102)
-    DeviceCtx* c = current_ctx();
-    if (!c) return 0;
-    std::lock_guard<std::mutex> lk(c->mu);
-    const bool in_dev = is_device_pointer(in), out_dev = is_device_pointer(out);
-    cudaError_t e;
-    if (in_dev || out_dev) {
-        // the call is synchronous and cannot know which stream produced a device buffer: wait for all of them
-        e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return 0; }
-    }
-    const uint8_t* d_in = in;
-    uint8_t* d_out = out;
-    size_t d_cap = out_cap;
-    bool input_staged = false;
-    if (encode && alg == ALG_CHAMELEON && !in_dev && !out_dev && n >= PIPE_MIN_BYTES) {
-        const size_t r = chameleon_encode_host_pipelined(c, in, n, out, out_cap);
+    SyncCall f(in, out);
+    if (!f.c) return 0;
+    if (encode && alg == ALG_CHAMELEON && !f.in_dev && !f.out_dev && n >= PIPE_MIN_BYTES) {
+        const size_t r = chameleon_encode_host_pipelined(f.c, in, n, out, out_cap);
         if (r != (size_t)-1) return r;
-        input_staged = true;   // not quiet: the whole input is already in stage_in; redo with the protection-aware fallback
-        d_in = c->stage_in.p;
+        f.staged_in = f.c->stage_in.p;   // not quiet: the whole input is already in stage_in; redo with the protection-aware fallback
     }
-    if (!in_dev && !input_staged) {
-        e = c->stage_in.ensure(n + 16, c->stream);
-        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return 0; }
-        e = h2d_any(c->ring_in, c->stage_in.p, in, n, c->stream, is_pageable_host(in));
-        if (e != cudaSuccess) { set_error("H2D copy", e); return 0; }
-        d_in = c->stage_in.p;
+    // encode: stage into a full safe-size buffer and check the real size against the caller's capacity afterwards
+    // (the reference only fails when the bytes actually written exceed the slice, write_buffer.rs:19)
+    const int rc = f.run(in, n, false, out, out_cap, encode ? safe_size(alg, n) : out_cap, 1, [&](const uint8_t* d_in, uint8_t* d_out, size_t d_cap) {
+        return encode ? encode_device_locked(f.c, alg, d_in, n, d_out, d_cap, f.c->d_size, f.c->stream, 4)
+                      : decode_device_locked(f.c, alg, d_in, n, d_out, d_cap, f.c->d_size, f.c->stream, 0);
+    });
+    return sync_bytes(rc, f.c, encode, out_cap);
+}
+
+// The prologue of the stream-ordered entries (encode / decode, decoded size, range decode): the error cleared and the arguments checked
+// (d_in and d_out NULL only when their lengths are 0, d_in in_align-byte aligned, the k result words at d_result not NULL and 8-byte
+// aligned), then the context taken and locked. An empty call zeroes the result words with a memset and launches nothing; otherwise
+// enqueue(c, stream) enqueues the call.
+template <class F>
+static int stream_entry(const uint8_t* d_in, size_t n, const uint8_t* d_out, size_t cap, uint64_t* d_result, int k, uintptr_t in_align,
+                        bool empty, void* stream, F enqueue) {
+    g_last_error.clear();
+    if (!d_result || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & (in_align - 1)) || (reinterpret_cast<uintptr_t>(d_result) & 7)) {
+        set_error("misaligned pointer: d_out_size / d_result must be 8-byte aligned, and d_in 2-byte for decoded size and range decode");
+        return DENSITY_B200_EARG;
     }
-    if (!out_dev) {
-        // encode: stage into a full safe-size buffer and check the real size against the caller's capacity afterwards
-        // (the reference only fails when the bytes actually written exceed the slice, write_buffer.rs:19)
-        d_cap = encode ? safe_size(alg, n) : out_cap;
-        e = c->stage_out.ensure(d_cap + 16, c->stream);
-        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return 0; }
-        d_out = c->stage_out.p;
-    }
-    int rc = encode ? encode_device_locked(c, alg, d_in, n, d_out, d_cap, c->d_size, c->stream, 4)
-                    : decode_device_locked(c, alg, d_in, n, d_out, d_cap, c->d_size, c->stream);
-    if (rc != DENSITY_B200_OK) { cudaStreamSynchronize(c->stream); return 0; }
-    e = cudaMemcpyAsync(c->h_size, c->d_size, sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("stream sync", e); return 0; }
-    const uint64_t produced = *c->h_size;
-    if (produced == 0) { set_error(encode ? "encode failed on device (output capacity?)" : "decode failed on device (malformed stream or output capacity)"); return 0; }
-    if (produced > out_cap) { set_error("output buffer too small"); return 0; }
-    if (!out_dev) {
-        e = d2h_any(c->ring_out, out, d_out, produced, c->stream, is_pageable_host(out));
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) { set_error("D2H copy", e); return 0; }
-    }
-    return (size_t)produced;
+    DeviceCtx* c = current_ctx();
+    if (!c) return DENSITY_B200_ECUDA;
+    std::lock_guard<std::mutex> lk(c->mu);
+    const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (!empty) return enqueue(c, s);
+    const cudaError_t e = cudaMemsetAsync(d_result, 0, k * sizeof(uint64_t), s);
+    if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
 }
 
 }  // namespace dns
@@ -593,20 +643,11 @@ size_t lion_safe_encode_buffer_size(size_t s) { return safe_size(ALG_LION, s); }
 
 static int device_entry(bool encode, int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size,
                         void* stream, int path) {
-    g_last_error.clear();
     if (alg < 0 || alg > 2) { set_error("bad algorithm id"); return DENSITY_B200_EARG; }
-    if (!d_out_size || (!d_in && n) || (!d_out && cap)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    DeviceCtx* c = current_ctx();
-    if (!c) return DENSITY_B200_ECUDA;
-    std::lock_guard<std::mutex> lk(c->mu);
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    if (n == 0) {
-        cudaError_t e = cudaMemsetAsync(d_out_size, 0, sizeof(uint64_t), s);
-        if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
-        return DENSITY_B200_OK;
-    }
-    return encode ? encode_device_locked(c, alg, d_in, n, d_out, cap, d_out_size, s, path)
-                  : decode_device_locked(c, alg, d_in, n, d_out, cap, d_out_size, s, path);
+    return stream_entry(d_in, n, d_out, cap, d_out_size, 1, 1, n == 0, stream, [&](DeviceCtx* c, cudaStream_t s) {
+        return encode ? encode_device_locked(c, alg, d_in, n, d_out, cap, d_out_size, s, path)
+                      : decode_device_locked(c, alg, d_in, n, d_out, cap, d_out_size, s, path);
+    });
 }
 
 int density_b200_encode_device(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap, uint64_t* d_out_size, void* stream) {
@@ -629,33 +670,21 @@ int density_b200_decode_device_path(int alg, const uint8_t* d_in, size_t n, uint
 // ---- decoded size (decoded_size.cu) -------------------------------------------------------------------------------------------
 // n > 0, d_in 2-byte aligned; on the device's workspace like decode_device
 static int decoded_size_locked(DeviceCtx* c, int alg, const uint8_t* d_in, size_t n, uint64_t* d_result, cudaStream_t stream) {
-    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
     cudaError_t e = c->ws.ensure(decoded_size_workspace_bytes(alg, n), stream);
-    if (e != cudaSuccess) { ws_release(c, stream); set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
+    if (e != cudaSuccess) { set_error("workspace cudaMalloc", e); return DENSITY_B200_ECUDA; }
     e = decoded_size_launch(alg, d_in, n, c->ws.p, d_result, stream, &launches);
-    ws_release(c, stream);
     return step_result(e, launches, "decoded size launch");
 }
 
 int density_b200_decoded_size_device(int alg, const uint8_t* d_in, size_t n, uint64_t* d_result, void* stream) {
-    g_last_error.clear();
     if (alg < 0 || alg > 2) { set_error("bad algorithm id"); return DENSITY_B200_EARG; }
-    if (!d_result || (!d_in && n)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_result) & 7)) {
-        set_error("decoded_size_device: d_in must be 2-byte and d_result 8-byte aligned");
-        return DENSITY_B200_EARG;
-    }
-    DeviceCtx* c = current_ctx();
-    if (!c) return DENSITY_B200_ECUDA;
-    std::lock_guard<std::mutex> lk(c->mu);
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    if (n == 0) {      // codec.rs:102: an empty stream decodes to nothing; no kernel
-        const cudaError_t e = cudaMemsetAsync(d_result, 0, 2 * sizeof(uint64_t), s);
-        if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
-        return DENSITY_B200_OK;
-    }
-    return decoded_size_locked(c, alg, d_in, n, d_result, s);
+    // n == 0: an empty stream decodes to nothing (codec.rs:102)
+    return stream_entry(d_in, n, nullptr, 0, d_result, 2, 2, n == 0, stream, [&](DeviceCtx* c, cudaStream_t s) {
+        return decoded_size_locked(c, alg, d_in, n, d_result, s);
+    });
 }
 
 int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t* out_size) {
@@ -663,42 +692,25 @@ int density_b200_decoded_size(int alg, const uint8_t* input, size_t n, uint64_t*
     if (alg < 0 || alg > 2) { set_error("bad algorithm id"); return DENSITY_B200_EARG; }
     if (!out_size || (!input && n)) { set_error("null pointer"); return DENSITY_B200_EARG; }
     if (n == 0) { *out_size = 0; return DENSITY_B200_OK; }
-    DeviceCtx* c = current_ctx();
-    if (!c) return DENSITY_B200_ECUDA;
-    std::lock_guard<std::mutex> lk(c->mu);
-    const bool in_dev = is_device_pointer(input);
-    cudaError_t e;
-    if (in_dev) {
-        // synchronous, and it cannot know which stream produced the buffer: wait for all of them (as run_sync)
-        e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return DENSITY_B200_ECUDA; }
-    }
-    const uint8_t* d_in = input;
-    if (!in_dev || (reinterpret_cast<uintptr_t>(input) & 1)) {     // host buffers, and device buffers at an odd address, go through stage_in
-        e = c->stage_in.ensure(n + 16, c->stream);
-        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
-        e = in_dev ? cudaMemcpyAsync(c->stage_in.p, input, n, cudaMemcpyDeviceToDevice, c->stream)
-                   : h2d_any(c->ring_in, c->stage_in.p, input, n, c->stream, is_pageable_host(input));
-        if (e != cudaSuccess) { set_error("input copy", e); return DENSITY_B200_ECUDA; }
-        d_in = c->stage_in.p;
-    }
-    const int rc = decoded_size_locked(c, alg, d_in, n, c->d_size, c->stream);
-    if (rc != DENSITY_B200_OK) { cudaStreamSynchronize(c->stream); return rc; }
-    e = cudaMemcpyAsync(c->h_size, c->d_size, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("stream sync", e); return DENSITY_B200_ECUDA; }
-    if (c->h_size[1] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
-    *out_size = c->h_size[0];
+    SyncCall f(input, nullptr);
+    if (!f.c) return DENSITY_B200_ECUDA;
+    const int rc = f.run(input, n, true, nullptr, 0, OWN_OUTPUT, 2, [&](const uint8_t* d_in, uint8_t*, size_t) {
+        return decoded_size_locked(f.c, alg, d_in, n, f.c->d_size, f.c->stream);
+    });
+    if (rc != DENSITY_B200_OK) return rc;
+    if (f.c->h_size[1] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
+    *out_size = f.c->h_size[0];
     return DENSITY_B200_OK;
 }
 
 // ---- Chameleon range decode (decode_range.cu) --------------------------------------------------------------------------------------
 // n > 0, len > 0, d_in 2-byte aligned; on the device's workspace like decode_device. The locate step runs first and the host waits for
 // it on `stream` (the pieces' lengths size the rest); then the pieces are decoded and the w window bytes copied to out: device memory
-// (d_out) or, out_host, host memory (the synchronous entry). *h3 = {w, S, verdict}; d_result receives the same in stream order.
+// (d_out) or, out_host, host memory (the synchronous entry). d_result receives {w, S, verdict} in stream order.
 static int range_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t first, uint64_t len, uint8_t* out, bool out_host,
-                        uint64_t* d_result, cudaStream_t stream, uint64_t h3[3]) {
-    if (!ws_acquire(c, stream)) return DENSITY_B200_ECUDA;
+                        uint64_t* d_result, cudaStream_t stream) {
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
     uint64_t launches = 0;
     const char* what = "range decode locate";
     cudaError_t e = c->ws.ensure(range_locate_workspace_bytes(n), stream);
@@ -707,10 +719,7 @@ static int range_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t fi
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     RangePlan p{};
     bool planned = false;
-    if (e == cudaSuccess) {
-        for (int k = 0; k < 3; ++k) h3[k] = c->h_size[k];
-        planned = range_plan(c->h_size, n, first, c->num_sms, &p);
-    }
+    if (e == cudaSuccess) planned = range_plan(c->h_size, n, first, c->num_sms, &p);
     if (e == cudaSuccess && planned && p.w) {
         const uint8_t* window = nullptr;
         what = "range decode workspace";
@@ -722,7 +731,6 @@ static int range_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t fi
                          : cudaMemcpyAsync(out, window, p.w, cudaMemcpyDeviceToDevice, stream);
         }
     }
-    ws_release(c, stream);
     const int rc = step_result(e, launches, what);
     if (rc == DENSITY_B200_OK && !planned) { set_error("range decode: the locate step's report is inconsistent"); return DENSITY_B200_ECUDA; }
     return rc;
@@ -730,23 +738,10 @@ static int range_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t fi
 
 int density_b200_chameleon_decode_range_device(const uint8_t* d_in, size_t n, uint64_t first, uint64_t len, uint8_t* d_out, uint64_t* d_result,
                                                void* stream) {
-    g_last_error.clear();
-    if (!d_result || (!d_in && n) || (!d_out && len)) { set_error("null pointer"); return DENSITY_B200_EARG; }
-    if ((reinterpret_cast<uintptr_t>(d_in) & 1) || (reinterpret_cast<uintptr_t>(d_result) & 7)) {
-        set_error("chameleon_decode_range_device: d_in must be 2-byte and d_result 8-byte aligned");
-        return DENSITY_B200_EARG;
-    }
-    DeviceCtx* c = current_ctx();
-    if (!c) return DENSITY_B200_ECUDA;
-    std::lock_guard<std::mutex> lk(c->mu);
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    if (n == 0 || len == 0) {      // nothing to write (codec.rs:102 for an empty stream); no kernel
-        const cudaError_t e = cudaMemsetAsync(d_result, 0, 3 * sizeof(uint64_t), s);
-        if (e != cudaSuccess) { set_error("memset", e); return DENSITY_B200_ECUDA; }
-        return DENSITY_B200_OK;
-    }
-    uint64_t h3[3];
-    return range_locked(c, d_in, n, first, len, d_out, false, d_result, s, h3);
+    // n == 0 or len == 0: nothing to write (codec.rs:102 for an empty stream)
+    return stream_entry(d_in, n, d_out, len, d_result, 3, 2, n == 0 || len == 0, stream, [&](DeviceCtx* c, cudaStream_t s) {
+        return range_locked(c, d_in, n, first, len, d_out, false, d_result, s);
+    });
 }
 
 int density_b200_chameleon_decode_range(const uint8_t* input, size_t n, uint64_t first, uint8_t* output, uint64_t len, uint64_t* written) {
@@ -754,32 +749,14 @@ int density_b200_chameleon_decode_range(const uint8_t* input, size_t n, uint64_t
     if (!written || (!input && n) || (!output && len)) { set_error("null pointer"); return DENSITY_B200_EARG; }
     *written = 0;
     if (n == 0 || len == 0) return DENSITY_B200_OK;
-    DeviceCtx* c = current_ctx();
-    if (!c) return DENSITY_B200_ECUDA;
-    std::lock_guard<std::mutex> lk(c->mu);
-    const bool in_dev = is_device_pointer(input), out_dev = is_device_pointer(output);
-    cudaError_t e;
-    if (in_dev || out_dev) {
-        // synchronous, and it cannot know which stream produced or reads the buffers: wait for all of them (as run_sync)
-        e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return DENSITY_B200_ECUDA; }
-    }
-    const uint8_t* d_in = input;
-    if (!in_dev || (reinterpret_cast<uintptr_t>(input) & 1)) {     // host buffers, and device buffers at an odd address, go through stage_in
-        e = c->stage_in.ensure(n + 16, c->stream);
-        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
-        e = in_dev ? cudaMemcpyAsync(c->stage_in.p, input, n, cudaMemcpyDeviceToDevice, c->stream)
-                   : h2d_any(c->ring_in, c->stage_in.p, input, n, c->stream, is_pageable_host(input));
-        if (e != cudaSuccess) { set_error("input copy", e); return DENSITY_B200_ECUDA; }
-        d_in = c->stage_in.p;
-    }
-    uint64_t h3[3] = {0, 0, 0};
-    const int rc = range_locked(c, d_in, n, first, len, output, !out_dev, c->d_size, c->stream, h3);
-    e = cudaStreamSynchronize(c->stream);
+    SyncCall f(input, output);
+    if (!f.c) return DENSITY_B200_ECUDA;
+    const int rc = f.run(input, n, true, output, len, OWN_OUTPUT, 3, [&](const uint8_t* d_in, uint8_t* out, size_t) {
+        return range_locked(f.c, d_in, n, first, len, out, !f.out_dev, f.c->d_size, f.c->stream);
+    });
     if (rc != DENSITY_B200_OK) return rc;
-    if (e != cudaSuccess) { set_error("stream sync", e); return DENSITY_B200_ECUDA; }
-    if (h3[2] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
-    *written = h3[0];
+    if (f.c->h_size[2] != 0) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
+    *written = f.c->h_size[0];
     return DENSITY_B200_OK;
 }
 
@@ -2642,66 +2619,44 @@ static size_t codec_run(density_b200_codec* h, bool encode, const uint8_t* in, s
     g_last_error.clear();
     if (!h || (!in && n) || (!out && out_cap)) { set_error("null pointer"); return 0; }
     if (n == 0) return 0;
-    DeviceCtx* c = current_ctx();
-    if (!c) return 0;
-    std::lock_guard<std::mutex> lk(c->mu);
+    SyncCall f(in, out);
+    if (!f.c) return 0;
+    DeviceCtx* c = f.c;
     const int alg = h->alg;
-    const bool in_dev = is_device_pointer(in), out_dev = is_device_pointer(out);
-    cudaError_t e = cudaSuccess;
-    if (in_dev || out_dev) { e = cudaDeviceSynchronize(); if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return 0; } }
-    cudaStream_t st = c->stream;
-    if (!ws_acquire(c, st)) return 0;
-    const uint8_t* d_in = in; uint8_t* d_out = out; size_t d_cap = out_cap;
-    if (!in_dev) {
-        e = c->stage_in.ensure(n + 16, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(c->stage_in.p, in, n, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { set_error("H2D copy", e); return 0; }
-        d_in = c->stage_in.p;
-    }
-    if (!out_dev) {
-        d_cap = encode ? safe_size(alg, n) : out_cap;
-        e = c->stage_out.ensure(d_cap + 16, st);
-        if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return 0; }
-        d_out = c->stage_out.p;
-    }
-    uint64_t launches = 0;
-    uint32_t* quads = reinterpret_cast<uint32_t*>(h->state.p + 256);      // chunk_a = Chameleon's chunk_map
-    bool done = false;
-    if (encode && alg == ALG_CHAMELEON && !(reinterpret_cast<uintptr_t>(d_in) & 3) && !(reinterpret_cast<uintptr_t>(d_out) & 1)) {
-        // run-parallel encoder with the instance's dictionary carried in; the state is only written back when the call succeeded
-        uint32_t* d_carry = reinterpret_cast<uint32_t*>(h->tables.p);
-        uint32_t* d_tab = d_carry + 65536;
-        ChamLayout L;
-        e = c->ws.ensure(cham_workspace_bytes(n, c->num_sms, &L), st);
-        c->layout = L;
-        const uint32_t nruns = cham_pick_runs(n, c->num_sms);
-        bool ok = false;
-        if (e == cudaSuccess) e = cham_quads_to_table(quads, d_carry, st, &launches);
-        if (e == cudaSuccess) e = cham_encode_phase1(d_in, n, c->ws.p, L, nruns, nullptr, st, &launches);
-        if (e == cudaSuccess) e = cham_encode_phase2_stream(d_in, n, c->ws.p, L, nruns, d_carry, d_out, d_cap, c->d_size, d_tab, 12, c->num_sms, st, &launches, &ok);
-        if (e == cudaSuccess && ok) { e = cham_table_into_quads(d_tab, quads, st, &launches); done = true; }
-        c->last_was_chameleon_fastpath_capable = 0;
-    }
-    if (e == cudaSuccess && !done) {
-        // exact in-order kernel on the instance's state (Cheetah / Lion; Chameleon decode; a Chameleon encode whose copy map did not settle)
-        if (!encode && alg == ALG_LION) c->lion_stats_valid = false;
-        e = encode ? scalar_encode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true)
-                   : scalar_decode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true);
-    }
-    g_launches += launches;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_size, c->d_size, sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    ws_release(c, st);
-    if (e != cudaSuccess) { set_error("codec call", e); return 0; }
-    const uint64_t produced = *c->h_size;
-    if (produced == 0) { set_error(encode ? "encode failed on device (output capacity?)" : "decode failed on device (malformed stream or output capacity)"); return 0; }
-    if (produced > out_cap) { set_error("output buffer too small"); return 0; }
-    if (!out_dev) {
-        e = cudaMemcpyAsync(out, d_out, produced, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("D2H copy", e); return 0; }
-    }
-    return (size_t)produced;
+    const int rc = f.run(in, n, false, out, out_cap, encode ? safe_size(alg, n) : out_cap, 1, [&](const uint8_t* d_in, uint8_t* d_out, size_t d_cap) {
+        // the encoders store 2-byte words (encode_device's rule)
+        if (encode && (reinterpret_cast<uintptr_t>(d_out) & 1)) { set_error("codec encode: a device output must be 2-byte aligned"); return DENSITY_B200_EARG; }
+        cudaStream_t st = c->stream;
+        const WsLease lease(c, st);
+        if (!lease.ok) return DENSITY_B200_ECUDA;
+        cudaError_t e = cudaSuccess;
+        uint64_t launches = 0;
+        uint32_t* quads = reinterpret_cast<uint32_t*>(h->state.p + 256);      // chunk_a = Chameleon's chunk_map
+        bool done = false;
+        if (encode && alg == ALG_CHAMELEON && !(reinterpret_cast<uintptr_t>(d_in) & 3) && !(reinterpret_cast<uintptr_t>(d_out) & 1)) {
+            // run-parallel encoder with the instance's dictionary carried in; the state is only written back when the call succeeded
+            uint32_t* d_carry = reinterpret_cast<uint32_t*>(h->tables.p);
+            uint32_t* d_tab = d_carry + 65536;
+            ChamLayout L;
+            e = c->ws.ensure(cham_workspace_bytes(n, c->num_sms, &L), st);
+            c->layout = L;
+            const uint32_t nruns = cham_pick_runs(n, c->num_sms);
+            bool ok = false;
+            if (e == cudaSuccess) e = cham_quads_to_table(quads, d_carry, st, &launches);
+            if (e == cudaSuccess) e = cham_encode_phase1(d_in, n, c->ws.p, L, nruns, nullptr, st, &launches);
+            if (e == cudaSuccess) e = cham_encode_phase2_stream(d_in, n, c->ws.p, L, nruns, d_carry, d_out, d_cap, c->d_size, d_tab, 12, c->num_sms, st, &launches, &ok);
+            if (e == cudaSuccess && ok) { e = cham_table_into_quads(d_tab, quads, st, &launches); done = true; }
+            c->last_was_chameleon_fastpath_capable = 0;
+        }
+        if (e == cudaSuccess && !done) {
+            // exact in-order kernel on the instance's state (Cheetah / Lion; Chameleon decode; a Chameleon encode whose copy map did not settle)
+            if (!encode && alg == ALG_LION) c->lion_stats_valid = false;
+            e = encode ? scalar_encode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true)
+                       : scalar_decode(alg, d_in, n, d_out, d_cap, h->state.p, c->d_size, st, &launches, nullptr, true);
+        }
+        return step_result(e, launches, "codec call");
+    });
+    return sync_bytes(rc, c, encode, out_cap);
 }
 size_t density_b200_codec_encode(density_b200_codec* h, const uint8_t* in, size_t n, uint8_t* out, size_t cap) { return codec_run(h, true, in, n, out, cap); }
 size_t density_b200_codec_decode(density_b200_codec* h, const uint8_t* in, size_t n, uint8_t* out, size_t cap) { return codec_run(h, false, in, n, out, cap); }
@@ -2789,19 +2744,7 @@ void density_b200_shutdown(void) {
         DeviceCtx& c = g_ctx[d];
         if (!c.ready) continue;
         cudaSetDevice(d);
-        c.ws.release(); c.stage_in.release(); c.stage_out.release(); c.dec_tables.release(); c.lion_stats.release(); c.lion_stats_valid = false; for (int a2 = 0; a2 < 2; ++a2) for (int rg = 0; rg < 3; ++rg) c.chee_tables[a2][rg].release();
-        c.chee_epoch = 0;
-        if (c.d_size) cudaFree(c.d_size);
-        if (c.h_size) cudaFreeHost(c.h_size);
-        if (c.stream) cudaStreamDestroy(c.stream);
-        if (c.ws_free) { cudaEventDestroy(c.ws_free); c.ws_free = nullptr; c.ws_free_recorded = false; }
-        if (c.h2d_stream) cudaStreamDestroy(c.h2d_stream);
-        if (c.d2h_stream) cudaStreamDestroy(c.d2h_stream);
-        if (c.h_sizes) cudaFreeHost(c.h_sizes);
-        c.h2d_stream = c.d2h_stream = nullptr; c.h_sizes = nullptr; c.pipe_tables.release();
-        c.ring_in.release(); c.ring_out.release();
-        for (auto& set : c.ev) for (auto& e : set) if (e) { cudaEventDestroy(e); e = nullptr; }
-        c.d_size = nullptr; c.h_size = nullptr; c.stream = nullptr; c.ready = false;
+        c.release();
     }
     if (cur >= 0) cudaSetDevice(cur);
 }
@@ -2810,10 +2753,11 @@ void density_b200_shutdown(void) {
    out4 = {rounds used, settled (0 = the in-order kernel had to take over), run walks after round 0 (of rounds x runs), round budget} */
 int density_b200_cheetah_decode_rounds(uint32_t* out4) {
     DeviceCtx* c = current_ctx();
-    if (!c || !c->last_cl_status || !out4) return DENSITY_B200_EARG;
+    if (!c || !out4) return DENSITY_B200_EARG;
     std::lock_guard<std::mutex> lk(c->mu);
+    if (!c->chee_rounds_valid) return DENSITY_B200_EARG;
     unsigned int raw[8] = {0};
-    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(raw, c->last_cl_status, sizeof raw, cudaMemcpyDeviceToHost) != cudaSuccess) return DENSITY_B200_ECUDA;
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(raw, c->diag.p, sizeof raw, cudaMemcpyDeviceToHost) != cudaSuccess) return DENSITY_B200_ECUDA;
     out4[0] = raw[3]; out4[1] = raw[2] && !raw[5]; out4[2] = raw[6]; out4[3] = chee_shard_max_rounds();   // cl_decode.cu MAX_ROUNDS
     return DENSITY_B200_OK;
 }
@@ -2827,7 +2771,7 @@ int density_b200_lion_decode_stats(uint64_t* out4) {
     std::lock_guard<std::mutex> lk(c->mu);
     if (cudaDeviceSynchronize() != cudaSuccess) return DENSITY_B200_ECUDA;
     if (!c->lion_stats_valid) return DENSITY_B200_EARG;
-    return cudaMemcpy(out4, c->lion_stats.p, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost) == cudaSuccess ? DENSITY_B200_OK : DENSITY_B200_ECUDA;
+    return cudaMemcpy(out4, c->diag.p + 32, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost) == cudaSuccess ? DENSITY_B200_OK : DENSITY_B200_ECUDA;
 }
 
 /* test hook: rounds per stage of the Cheetah / Lion copy-map iteration (1..7; 7 = default) */

@@ -74,9 +74,11 @@ DENSITY_B200_API size_t lion_safe_encode_buffer_size(size_t size);
  * Encode `n` bytes at device pointer d_in (4-byte aligned) into d_out (2-byte aligned,
  * capacity `cap` >= *_safe_encode_buffer_size(n)). All work is enqueued on `stream`
  * (a cudaStream_t passed as void*; NULL = legacy default stream); nothing is synchronised.
- * The encoded size is written to *d_out_size (device memory, 8 bytes) when the stream
- * reaches that point; it is 0 if the device-side capacity check failed.
+ * The encoded size is written to *d_out_size (device memory, 8 bytes, 8-byte aligned) when the
+ * stream reaches that point; it is 0 if the device-side capacity check failed. n == 0: no
+ * kernel, 0 by a memset.
  * Returns DENSITY_B200_OK or an error code for failures detectable at enqueue time.
+ * DENSITY_B200_EARG (a bad algorithm id, a NULL pointer, a misaligned d_out_size) enqueues nothing.
  */
 DENSITY_B200_API int density_b200_encode_device(int alg, const uint8_t* d_in, size_t n, uint8_t* d_out, size_t cap,
                                uint64_t* d_out_size, void* stream);
@@ -769,7 +771,8 @@ DENSITY_B200_API int density_b200_decode_sharded_cheetah_stream_protected(densit
  *   density_b200_codec_encode       = Codec::encode   density_b200_codec_decode      = Codec::decode
  * Synchronous, host or device pointers, bytes written or 0 on error. Chameleon encode runs the run-parallel kernels with the
  * instance's dictionary carried in (buffers larger than HBM can be encoded piecewise, bit-exact with an instance on the CPU);
- * Cheetah / Lion and every decode run the exact in-order kernel on the instance's tables.
+ * Cheetah / Lion and every decode run the exact in-order kernel on the instance's tables. An encode into a device output at
+ * an odd address returns 0, as the nine encode symbols do (the encoders store 2-byte words).
  */
 typedef struct density_b200_codec density_b200_codec; /* opaque */
 DENSITY_B200_API density_b200_codec* density_b200_codec_create(int alg);

@@ -39,6 +39,10 @@ unsafe extern "C" {
     // bytes [first, first + len) of what a Chameleon stream decodes to: {written, size, verdict} to d_result (device) / *written
     pub fn density_b200_chameleon_decode_range_device(d_in: *const u8, n: usize, first: u64, len: u64, d_out: *mut u8, d_result: *mut u64, stream: *mut c_void) -> c_int;
     pub fn density_b200_chameleon_decode_range(input: *const u8, n: usize, first: u64, output: *mut u8, len: u64, written: *mut u64) -> c_int;
+    // the Chameleon seek index: its length bound, its build, and a range decode that reads only the piece between two checkpoints
+    pub fn density_b200_chameleon_index_bytes(n: usize, interval: u64) -> u64;
+    pub fn density_b200_chameleon_index_build(input: *const u8, n: usize, interval: u64, index: *mut u8, index_cap: usize, index_len: *mut u64) -> c_int;
+    pub fn density_b200_chameleon_decode_range_indexed(input: *const u8, n: usize, index: *const u8, index_len: usize, first: u64, output: *mut u8, len: u64, written: *mut u64) -> c_int;
     // a reused Codec instance (codec.rs:16,72,82)
     pub fn density_b200_codec_create(alg: c_int) -> *mut RawCodec;
     pub fn density_b200_codec_destroy(codec: *mut RawCodec);
@@ -124,6 +128,34 @@ impl Chameleon {
         let mut written: u64 = 0;
         let rc = unsafe {
             density_b200_chameleon_decode_range(input.as_ptr(), input.len(), first, output.as_mut_ptr(), output.len() as u64, &mut written)
+        };
+        if rc == 0 { usize::try_from(written).map_err(|_| DecodeError {}) } else { Err(DecodeError {}) }
+    }
+
+    /// The seek index of `input` with a checkpoint every `interval` decoded bytes (a positive multiple of 256): a byte blob that can be
+    /// stored beside the stream. `Err` on a malformed stream, a bad interval, or when the library could not run.
+    pub fn build_index(input: &[u8], interval: u64) -> Result<Vec<u8>, DecodeError> {
+        let bound = unsafe { density_b200_chameleon_index_bytes(input.len(), interval) };
+        let mut index = vec![0u8; usize::try_from(bound).map_err(|_| DecodeError {})?];
+        if index.is_empty() {
+            return Err(DecodeError {});
+        }
+        let mut len: u64 = 0;
+        let rc = unsafe { density_b200_chameleon_index_build(input.as_ptr(), input.len(), interval, index.as_mut_ptr(), index.len(), &mut len) };
+        if rc != 0 {
+            return Err(DecodeError {});
+        }
+        index.truncate(len as usize);
+        Ok(index)
+    }
+
+    /// `decode_range` from the seek index `build_index` returned for `input`: only the stream between the two checkpoints around the
+    /// window is read and decoded. `Err` as `decode_range`, and when the index does not describe `input`.
+    pub fn decode_range_indexed(input: &[u8], index: &[u8], first: u64, output: &mut [u8]) -> Result<usize, DecodeError> {
+        let mut written: u64 = 0;
+        let rc = unsafe {
+            density_b200_chameleon_decode_range_indexed(input.as_ptr(), input.len(), index.as_ptr(), index.len(), first, output.as_mut_ptr(),
+                                                        output.len() as u64, &mut written)
         };
         if rc == 0 { usize::try_from(written).map_err(|_| DecodeError {}) } else { Err(DecodeError {}) }
     }

@@ -5,7 +5,7 @@ this package is the thin host-side mirror of the reference's `Codec` interface p
 for the sharded multi-GPU path.
 """
 from .codec import (CODECS, Chameleon, Cheetah, DecodeError, EncodeError, Lion, decode_device, decode_range_device,  # noqa: F401
-                    decoded_size_device, encode_device)
+                    decode_range_indexed_device, decoded_size_device, encode_device, index_build_device)
 from ._lib import DensityB200Error, SO_PATH, load  # noqa: F401
 
 __version__ = "0.1.0"

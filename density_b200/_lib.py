@@ -25,6 +25,15 @@ _SIGS = {
                                                                    ctypes.c_void_p, ctypes.c_void_p]),
     "density_b200_chameleon_decode_range": (ctypes.c_int, [_c_u8p, ctypes.c_size_t, ctypes.c_uint64, _c_u8p, ctypes.c_uint64,
                                                             ctypes.POINTER(ctypes.c_uint64)]),
+    "density_b200_chameleon_index_bytes": (ctypes.c_uint64, [ctypes.c_size_t, ctypes.c_uint64]),
+    "density_b200_chameleon_index_build_device": (ctypes.c_int, [_c_u8p, ctypes.c_size_t, ctypes.c_uint64, _c_u8p, ctypes.c_size_t,
+                                                                  ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_chameleon_index_build": (ctypes.c_int, [_c_u8p, ctypes.c_size_t, ctypes.c_uint64, _c_u8p, ctypes.c_size_t,
+                                                           ctypes.POINTER(ctypes.c_uint64)]),
+    "density_b200_chameleon_decode_range_indexed_device": (ctypes.c_int, [_c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_uint64,
+                                                                           ctypes.c_uint64, _c_u8p, ctypes.c_void_p, ctypes.c_void_p]),
+    "density_b200_chameleon_decode_range_indexed": (ctypes.c_int, [_c_u8p, ctypes.c_size_t, _c_u8p, ctypes.c_size_t, ctypes.c_uint64, _c_u8p,
+                                                                    ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]),
     "density_b200_shard_create": (ctypes.c_void_p, []),
     "density_b200_shard_destroy": (None, [ctypes.c_void_p]),
     "density_b200_shard_phase1": (ctypes.c_int, [ctypes.c_void_p, _c_u8p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),

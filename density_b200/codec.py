@@ -135,19 +135,52 @@ class Chameleon(_Codec):
     NAME, _BLOCK, _UNIT, _SIG = "chameleon", 256, 8, 8
 
     @classmethod
-    def decode_range(cls, input, first, output):
+    def decode_range(cls, input, first, output, index=None):
         """Decode bytes [first, first + len(output)) of what `input` decodes to into `output`, without decoding the bytes in front of
         them; returns the number of bytes written, min(first + len(output), S) - first or 0 when first >= S (S: the decoded size).
-        Host buffers or torch CUDA tensors of any alignment. Raises DecodeError when the stream is malformed."""
+        Host buffers or torch CUDA tensors of any alignment. Raises DecodeError when the stream is malformed. With `index` (what
+        build_index returned for this stream) only the stream between the two checkpoints around the window is read and decoded; an
+        index that does not describe the stream raises DensityB200Error, one whose stream decodes differently raises DecodeError."""
         ip, n, k1 = _ptr_len(input)
         op, cap, k2 = _ptr_len(output, writable=True)
         written = ctypes.c_uint64(0)
-        rc = _lib.load().density_b200_chameleon_decode_range(ip, n, first, op, cap, ctypes.byref(written))
+        if index is None:
+            name = "density_b200_chameleon_decode_range"
+            rc = _lib.load().density_b200_chameleon_decode_range(ip, n, first, op, cap, ctypes.byref(written))
+        else:
+            xp, xn, k3 = _ptr_len(index)
+            name = "density_b200_chameleon_decode_range_indexed"
+            rc = _lib.load().density_b200_chameleon_decode_range_indexed(ip, n, xp, xn, first, op, cap, ctypes.byref(written))
         if rc == _EMALFORMED:
             raise DecodeError(_lib.last_error() or "malformed stream")
         if rc != 0:
-            raise _lib.DensityB200Error(f"density_b200_chameleon_decode_range rc={rc}: {_lib.last_error()}")
+            raise _lib.DensityB200Error(f"{name} rc={rc}: {_lib.last_error()}")
         return written.value
+
+    @classmethod
+    def build_index(cls, input, interval=16 << 20):
+        """The seek index of stream `input` (include/density_b200.h, "Chameleon seek index"): a checkpoint every `interval` decoded bytes
+        (a positive multiple of 256). Returns bytes for a host input, a CUDA uint8 tensor for a CUDA tensor. Raises DecodeError when
+        the stream is malformed."""
+        ip, n, k1 = _ptr_len(input)
+        L = _lib.load()
+        bound = L.density_b200_chameleon_index_bytes(n, interval)
+        if not bound:
+            raise ValueError("interval must be a positive multiple of 256")
+        try:
+            import torch
+            dev = isinstance(input, torch.Tensor) and input.is_cuda
+        except ImportError:  # pragma: no cover
+            dev = False
+        out = torch.empty(bound, dtype=torch.uint8, device=input.device) if dev else np.empty(bound, dtype=np.uint8)
+        op, _, k2 = _ptr_len(out, writable=True)
+        size = ctypes.c_uint64(0)
+        rc = L.density_b200_chameleon_index_build(ip, n, interval, op, bound, ctypes.byref(size))
+        if rc == _EMALFORMED:
+            raise DecodeError(_lib.last_error() or "malformed stream")
+        if rc != 0:
+            raise _lib.DensityB200Error(f"density_b200_chameleon_index_build rc={rc}: {_lib.last_error()}")
+        return out[:size.value].clone() if dev else out[:size.value].tobytes()
 
 
 class Cheetah(_Codec):
@@ -251,3 +284,27 @@ def decode_range_device(d_in, n_in, first, d_out, d_result, stream=None):
                                                         _stream_handle(stream))
     if rc != 0:
         raise DecodeError(f"density_b200_chameleon_decode_range_device rc={rc}: {_lib.last_error()}")
+
+
+def index_build_device(d_in, n_in, interval, d_index, d_result, stream=None):
+    """Enqueue the Chameleon seek index build of the first `n_in` bytes of CUDA uint8 tensor `d_in` into CUDA uint8 tensor `d_index`
+    (at least density_b200_chameleon_index_bytes(n_in, interval) bytes), on `stream` (default: torch's current stream). `d_result` is a
+    CUDA int64/uint64 tensor of three elements that receives {index bytes, decoded size, verdict}. The call returns once the stream's
+    earlier work and the checkpoint walk are done; the snapshots are left enqueued. Raises DecodeError on a malformed stream (nothing is
+    written to d_index then)."""
+    L = _lib.load()
+    rc = L.density_b200_chameleon_index_build_device(d_in.data_ptr(), n_in, interval, d_index.data_ptr(), d_index.numel(), d_result.data_ptr(),
+                                                       _stream_handle(stream))
+    if rc != 0:
+        raise DecodeError(f"density_b200_chameleon_index_build_device rc={rc}: {_lib.last_error()}")
+
+
+def decode_range_indexed_device(d_in, n_in, d_index, index_len, first, d_out, d_result, stream=None):
+    """decode_range_device from the seek index in the first `index_len` bytes of CUDA uint8 tensor `d_index`: only the stream between the
+    checkpoints around the window is decoded. The call returns once the index's directory has been read (one wait on `stream`), with
+    the decode enqueued. Raises DecodeError when the index does not describe a stream of n_in bytes."""
+    L = _lib.load()
+    rc = L.density_b200_chameleon_decode_range_indexed_device(d_in.data_ptr(), n_in, d_index.data_ptr(), index_len, first, d_out.numel(),
+                                                                d_out.data_ptr(), d_result.data_ptr(), _stream_handle(stream))
+    if rc != 0:
+        raise DecodeError(f"density_b200_chameleon_decode_range_indexed_device rc={rc}: {_lib.last_error()}")

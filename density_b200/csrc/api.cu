@@ -760,6 +760,174 @@ int density_b200_chameleon_decode_range(const uint8_t* input, size_t n, uint64_t
     return DENSITY_B200_OK;
 }
 
+// ---- Chameleon seek index (decode_range.cu) -----------------------------------------------------------------------------------------
+// n > 0, d_in 2-byte aligned, a valid interval. The locate step runs first and the host waits for it (the pieces' lengths size the
+// rest); then, on a well-formed stream, the index is written to `at` (device, 4-byte aligned) and, when out is set, copied from there to
+// out: host memory (out_host) or device memory of any alignment. h3 = {index bytes, S, verdict}; d_result receives the same.
+static int index_build_locked(DeviceCtx* c, const uint8_t* d_in, size_t n, uint64_t interval, uint8_t* at, uint8_t* out, bool out_host,
+                              uint64_t* d_result, cudaStream_t stream, uint64_t h3[3]) {
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const char* what = "index build locate";
+    std::vector<uint64_t> rep(index_report_bytes(index_max_count(n, interval)) / sizeof(uint64_t));
+    cudaError_t e = c->ws.ensure(index_locate_workspace_bytes(n, interval), stream);
+    if (e == cudaSuccess) e = index_locate_launch(d_in, n, interval, c->ws.p, d_result, rep.data(), stream, &launches);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    bool planned = false;
+    if (e == cudaSuccess) {
+        for (int k = 0; k < 3; ++k) h3[k] = rep[k];
+        size_t ws_bytes = 0;
+        planned = index_build_plan(rep.data(), n, c->num_sms, &ws_bytes);
+        if (planned && !rep[2]) {
+            what = "index build workspace";
+            e = c->ws.ensure(ws_bytes, stream);
+            if (e == cudaSuccess) { what = "index build launch"; e = index_build_launch(d_in, rep.data(), c->ws.p, at, c->num_sms, stream, &launches); }
+            if (e == cudaSuccess && out) {
+                what = "index copy";
+                e = out_host ? d2h_any(c->ring_out, out, at, rep[0], stream, is_pageable_host(out))
+                             : cudaMemcpyAsync(out, at, rep[0], cudaMemcpyDeviceToDevice, stream);
+            }
+        }
+    }
+    const int rc = step_result(e, launches, what);
+    if (rc != DENSITY_B200_OK) return rc;
+    if (rep[2]) { set_error("malformed stream: the decoder would read past its end"); return DENSITY_B200_EMALFORMED; }
+    if (!planned) { set_error("index build: the locate step's report is inconsistent"); return DENSITY_B200_ECUDA; }
+    return DENSITY_B200_OK;
+}
+
+// The header and the directory of an index of index_len bytes at `index` (host or device; a device index is read on `stream`, with one
+// wait) into hdr, checked against the stream length. DENSITY_B200_EARG with the error set when they do not describe a valid index.
+static int index_read(const uint8_t* index, bool index_dev, size_t index_len, size_t n, cudaStream_t stream, std::vector<uint64_t>* hdr) {
+    const uint64_t count = index_count_for_bytes(index_len);
+    if (count == ~0ull || count > index_max_count(n, 256)) { set_error("index_len is not the length of an index of this stream"); return DENSITY_B200_EARG; }
+    hdr->assign(cidx_snapshots_at(count) / sizeof(uint64_t), 0);
+    if (index_dev) {
+        cudaError_t e = cudaMemcpyAsync(hdr->data(), index, cidx_snapshots_at(count), cudaMemcpyDeviceToHost, stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+        if (e != cudaSuccess) { set_error("index directory copy", e); return DENSITY_B200_ECUDA; }
+    } else {
+        memcpy(hdr->data(), index, cidx_snapshots_at(count));
+    }
+    if (const char* why = index_check(hdr->data(), n, index_len, count)) { set_error(why); return DENSITY_B200_EARG; }
+    return DENSITY_B200_OK;
+}
+
+// The decode of an indexed piece (d_piece: the piece's first byte, 2-byte aligned) and the checked copy of the window to d_out (device,
+// any alignment), on the device's workspace. snap: the carry-in snapshot, NULL at the stream start; snap_copy: it is in host memory or
+// misaligned, and is staged in the workspace first. With p.w == 0 only the result words {0, S, 0} are written.
+static int range_indexed_locked(DeviceCtx* c, const uint8_t* d_piece, RangePlan p, const uint8_t* snap, bool snap_copy, uint64_t size,
+                                uint8_t* d_out, uint64_t* d_result, cudaStream_t stream) {
+    const WsLease lease(c, stream);
+    if (!lease.ok) return DENSITY_B200_ECUDA;
+    uint64_t launches = 0;
+    const uint8_t* window = nullptr;
+    cudaError_t e = c->ws.ensure(p.ws_bytes, stream);
+    if (e == cudaSuccess && p.w && snap) {
+        p.carry_in = snap_copy ? range_table_slot(c->ws.p) : reinterpret_cast<const uint32_t*>(snap);
+        if (snap_copy) e = cudaMemcpyAsync(range_table_slot(c->ws.p), snap, CIDX_SNAPSHOT_BYTES, cudaMemcpyDefault, stream);
+    }
+    if (e == cudaSuccess && p.w) e = range_decode_launch(d_piece, p, c->ws.p, c->num_sms, stream, &launches, &window);
+    if (e == cudaSuccess) e = index_copy_out_launch(p, window, size, d_out, c->ws.p, d_result, c->num_sms, stream, &launches);
+    return step_result(e, launches, "indexed range decode launch");
+}
+
+// the snapshot an indexed piece starts from (NULL: the stream start)
+static const uint8_t* index_snapshot(const uint8_t* index, const std::vector<uint64_t>& hdr, uint64_t j) {
+    return j ? index + cidx_snapshots_at(hdr[CIDX_COUNT_W]) + (j - 1) * CIDX_SNAPSHOT_BYTES : nullptr;
+}
+
+uint64_t density_b200_chameleon_index_bytes(size_t n, uint64_t interval) {
+    return (interval < 256 || interval % 256) ? 0 : cidx_bytes(index_max_count(n, interval));
+}
+
+int density_b200_chameleon_index_build_device(const uint8_t* d_in, size_t n, uint64_t interval, uint8_t* d_index, size_t index_cap,
+                                              uint64_t* d_result, void* stream) {
+    g_last_error.clear();
+    if (n == 0) { set_error("index build: an empty stream has nothing to index"); return DENSITY_B200_EARG; }
+    if (!density_b200_chameleon_index_bytes(n, interval)) { set_error("index build: interval must be a positive multiple of 256"); return DENSITY_B200_EARG; }
+    if (index_cap < density_b200_chameleon_index_bytes(n, interval)) { set_error("index build: index_cap < density_b200_chameleon_index_bytes(n, interval)"); return DENSITY_B200_EARG; }
+    if (reinterpret_cast<uintptr_t>(d_index) & 3) { set_error("index build: d_index must be 4-byte aligned"); return DENSITY_B200_EARG; }
+    return stream_entry(d_in, n, d_index, index_cap, d_result, 3, 2, false, stream, [&](DeviceCtx* c, cudaStream_t s) {
+        uint64_t h3[3];
+        return index_build_locked(c, d_in, n, interval, d_index, nullptr, false, d_result, s, h3);
+    });
+}
+
+int density_b200_chameleon_index_build(const uint8_t* input, size_t n, uint64_t interval, uint8_t* index, size_t index_cap, uint64_t* index_len) {
+    g_last_error.clear();
+    if (!index_len || !input || !index) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    *index_len = 0;
+    if (n == 0) { set_error("index build: an empty stream has nothing to index"); return DENSITY_B200_EARG; }
+    const uint64_t bound = density_b200_chameleon_index_bytes(n, interval);
+    if (!bound) { set_error("index build: interval must be a positive multiple of 256"); return DENSITY_B200_EARG; }
+    if (index_cap < bound) { set_error("index build: index_cap < density_b200_chameleon_index_bytes(n, interval)"); return DENSITY_B200_EARG; }
+    SyncCall f(input, index);
+    if (!f.c) return DENSITY_B200_ECUDA;
+    uint64_t h3[3] = {0, 0, 0};
+    const int rc = f.run(input, n, true, index, index_cap, OWN_OUTPUT, 3, [&](const uint8_t* d_in, uint8_t* out, size_t) {
+        // a device index that is 4-byte aligned is written in place; any other is built in stage_out and copied
+        const bool direct = f.out_dev && !(reinterpret_cast<uintptr_t>(out) & 3);
+        if (!direct) {
+            const cudaError_t e = f.c->stage_out.ensure(bound, f.c->stream);
+            if (e != cudaSuccess) { set_error("staging cudaMalloc", e); return DENSITY_B200_ECUDA; }
+        }
+        return index_build_locked(f.c, d_in, n, interval, direct ? out : f.c->stage_out.p, direct ? nullptr : out, !f.out_dev, f.c->d_size,
+                                  f.c->stream, h3);
+    });
+    if (rc != DENSITY_B200_OK) return rc;
+    *index_len = h3[0];
+    return DENSITY_B200_OK;
+}
+
+int density_b200_chameleon_decode_range_indexed_device(const uint8_t* d_in, size_t n, const uint8_t* d_index, size_t index_len, uint64_t first,
+                                                       uint64_t len, uint8_t* d_out, uint64_t* d_result, void* stream) {
+    g_last_error.clear();
+    if (!d_index || (reinterpret_cast<uintptr_t>(d_index) & 3)) { set_error("indexed range decode: d_index must be non-NULL and 4-byte aligned"); return DENSITY_B200_EARG; }
+    // n == 0 or len == 0: nothing to write, as density_b200_chameleon_decode_range_device (the index is not read)
+    return stream_entry(d_in, n, d_out, len, d_result, 3, 2, n == 0 || len == 0, stream, [&](DeviceCtx* c, cudaStream_t s) {
+        std::vector<uint64_t> hdr;
+        int rc = index_read(d_index, true, index_len, n, s, &hdr);
+        if (rc != DENSITY_B200_OK) return rc;
+        RangePlan p{};
+        uint64_t j = 0;
+        index_plan(hdr.data(), n, first, len, c->num_sms, &p, &j);
+        return range_indexed_locked(c, d_in + p.piece_off, p, index_snapshot(d_index, hdr, j), false, hdr[CIDX_SIZE_W], d_out, d_result, s);
+    });
+}
+
+int density_b200_chameleon_decode_range_indexed(const uint8_t* input, size_t n, const uint8_t* index, size_t index_len, uint64_t first,
+                                                uint8_t* output, uint64_t len, uint64_t* written) {
+    g_last_error.clear();
+    if (!written || (!input && n) || (!output && len) || !index) { set_error("null pointer"); return DENSITY_B200_EARG; }
+    *written = 0;
+    if (n == 0 || len == 0) return DENSITY_B200_OK;
+    SyncCall f(input, output);
+    if (!f.c) return DENSITY_B200_ECUDA;
+    const bool index_dev = is_device_pointer(index);
+    if (index_dev && !f.in_dev && !f.out_dev) {      // the frame synchronises only for the stream and the output
+        const cudaError_t e = cudaDeviceSynchronize();
+        if (e != cudaSuccess) { set_error("cudaDeviceSynchronize", e); return DENSITY_B200_ECUDA; }
+    }
+    std::vector<uint64_t> hdr;
+    int rc = index_read(index, index_dev, index_len, n, f.c->stream, &hdr);
+    if (rc != DENSITY_B200_OK) return rc;
+    RangePlan p{};
+    uint64_t j = 0;
+    if (!index_plan(hdr.data(), n, first, len, f.c->num_sms, &p, &j)) return DENSITY_B200_OK;     // first >= S
+    // only the piece of the stream is staged (SyncCall stages what it is given), and only snapshot j of the index
+    const uint8_t* snap = index_snapshot(index, hdr, j);
+    const bool snap_copy = !index_dev || (reinterpret_cast<uintptr_t>(snap) & 3);
+    rc = f.run(input + p.piece_off, p.piece_n, true, output, len, p.w, 3, [&](const uint8_t* d_piece, uint8_t* out, size_t) {
+        return range_indexed_locked(f.c, d_piece, p, snap, snap_copy, hdr[CIDX_SIZE_W], out, f.c->d_size, f.c->stream);
+    });
+    if (rc != DENSITY_B200_OK) return rc;
+    if (f.c->h_size[2] != 0) { set_error("indexed range decode: the stream does not decode to what its index describes"); return DENSITY_B200_EMALFORMED; }
+    *written = f.c->h_size[0];
+    return DENSITY_B200_OK;
+}
+
 // ---- the argument rule of the sharded entries (include/density_b200.h, "Sharded encode" and "Sharded decode"). Each helper returns
 // DENSITY_B200_EARG with the error set, or DENSITY_B200_OK.
 static bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }

@@ -255,13 +255,32 @@ __device__ __forceinline__ bool stop_inside(const WalkStops& w, uint64_t b, uint
     const uint64_t e = b + nb;
     return (w.block[0] > b && w.block[0] < e) || (w.block[1] > b && w.block[1] < e);
 }
-template <class T, bool STOP = false>
-__global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, uint32_t nchunks,
-                                                           const uint32_t* __restrict__ res, const uint4* __restrict__ gres, uint32_t ngroups,
-                                                           uint32_t* __restrict__ g_entry, uint64_t* __restrict__ g_blockbase,
-                                                           uint32_t* __restrict__ c_entry, uint64_t* __restrict__ c_blockbase,
-                                                           uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st,
-                                                           WalkStops stops = WalkStops{}) {
+template <bool STOP>
+struct PairStops {      // the walk's view of WalkStops
+    WalkStops w;
+    __device__ __forceinline__ void at(uint64_t b, uint64_t i, const Protection& ps) const { stop_at<STOP>(w, b, i, ps); }
+    __device__ __forceinline__ bool inside(uint64_t b, uint32_t nb) const { return stop_inside<STOP>(w, b, nb); }
+};
+// The stride mode (the Chameleon seek index, DESIGN §4h): in front of every block b = j * every, 1 <= j <= max, out[STRIDE_WORDS (j - 1)
+// ..] = {stream offset, the state as stop_state} when the main loop reaches it (block main_blocks included). As in the stop-and-report
+// mode, the walk jumps no group and no chunk that holds such a block strictly inside.
+constexpr uint32_t STRIDE_WORDS = 2;
+struct StrideStops {
+    uint64_t every, max; unsigned long long* out;
+    __device__ __forceinline__ void at(uint64_t b, uint64_t i, const Protection& ps) const {
+        const uint64_t j = b / every;
+        if (b && j <= max && j * every == b) { unsigned long long* o = out + STRIDE_WORDS * (j - 1); o[0] = i; o[1] = stop_state(ps); }
+    }
+    __device__ __forceinline__ bool inside(uint64_t b, uint32_t nb) const { return nb > 1 && (b + nb - 1) / every > b / every; }
+};
+// The walk of both kernels below. Its pointers carry no __restrict__: the kernels' parameters state it, and restating it here gives the
+// inlined body other alias scopes and dec_seq_walk<T, true> other code.
+template <class T, class Stops>
+__device__ __forceinline__ void seq_walk(const uint8_t* in, uint64_t n, uint64_t cap, uint32_t nchunks,
+                                         const uint32_t* res, const uint4* gres, uint32_t ngroups,
+                                         uint32_t* g_entry, uint64_t* g_blockbase,
+                                         uint32_t* c_entry, uint64_t* c_blockbase,
+                                         uint64_t* blk_off, uint64_t maxblocks, DecStatus* st, Stops stops) {
     if (!(st->nonquiet & 1u)) return;
     constexpr uint32_t SW_LOAD = T::CH + 16;            // + the signature bytes of a block starting at the chunk's last bytes, rounded up to 16
     __shared__ __align__(16) uint8_t win[2][SW_LOAD];   // the chunk being walked + the next one, prefetched during the walk
@@ -279,14 +298,14 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
         if (tid == 0) {
             uint32_t cmd = SW_DONE, c = 0;
             while (n - idx >= T::MAXBLK) {
-                stop_at<STOP>(stops, b, idx, ps);
+                stops.at(b, idx, ps);
                 c = (uint32_t)(idx / T::CH);
                 const uint32_t e = (uint32_t)(idx - (uint64_t)c * T::CH) >> 1;          // < NCAND: a block is at most MAXBLK bytes
                 if (c / GROUP == g_next) {
                     // entering a group of 64 chunks: jump over all of it if the automaton provably stays in encoded mode inside
                     const uint32_t g = g_next++;
                     const uint4 gr = gres[(size_t)g * T::NCAND + e];
-                    if (ps.copy_penalty == 0 && gr.x != TERM && !(gr.z & 9u) && !(ps.previous_incompressible && (gr.z & 2u)) && !stop_inside<STOP>(stops, b, gr.y)) {
+                    if (ps.copy_penalty == 0 && gr.x != TERM && !(gr.z & 9u) && !(ps.previous_incompressible && (gr.z & 2u)) && !stops.inside(b, gr.y)) {
                         g_entry[g] = e; g_blockbase[g] = b;
                         sw_jump(ps, gr.y, (gr.z >> 2) & 1u);
                         b += gr.y;
@@ -298,7 +317,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
                 if (c < cb || c >= cb + cb_valid) { cmd = SW_ROWS; break; }
                 const uint32_t r = rows[(c - cb) * T::NCAND + e];
                 const uint32_t ex = r & 0xFFu, fl = row_x<T>(r);
-                if (ps.copy_penalty == 0 && ex != TERM && !(fl & 1u) && !(ps.previous_incompressible && (fl & 2u)) && !stop_inside<STOP>(stops, b, row_nb<T>(r))) {
+                if (ps.copy_penalty == 0 && ex != TERM && !(fl & 1u) && !(ps.previous_incompressible && (fl & 2u)) && !stops.inside(b, row_nb<T>(r))) {
                     const uint32_t nb = row_nb<T>(r);
                     c_entry[c] = e; c_blockbase[c] = b;
                     sw_jump(ps, nb, (fl >> 2) & 1u);
@@ -342,7 +361,7 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
                 const uint64_t wend = wbase + T::CH;
                 c_entry[c] = TERM;                                           // dec_block_offsets leaves this chunk alone
                 while (idx < wend && n - idx >= T::MAXBLK) {
-                    stop_at<STOP>(stops, b, idx, ps);
+                    stops.at(b, idx, ps);
                     if (ps.revert_to_copy()) {                               // codec.rs:89-92
                         if (b < maxblocks) blk_off[b] = idx | BLK_COPY;
                         ++b; idx += T::BS; ps.decay();
@@ -368,13 +387,30 @@ __global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __rest
         for (uint32_t g = s_gnext + tid; g < ngroups; g += SW_THREADS) g_entry[g] = G_SKIP;
     }
     if (tid == 0) {
-        stop_at<STOP>(stops, b, idx, ps);
+        stops.at(b, idx, ps);
         st->main_blocks = b; st->tail_off = idx;
         st->ps_penalty = ps.copy_penalty; st->ps_start = ps.copy_penalty_start; st->ps_prev = ps.previous_incompressible;
         st->seq = 1;
         st->error = (b * T::BS > cap) ? 2u : 0u;     // the candidate walk's block count was void
         st->nonquiet &= ~1u;
     }
+}
+template <class T, bool STOP = false>
+__global__ void __launch_bounds__(SW_THREADS) dec_seq_walk(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, uint32_t nchunks,
+                                                           const uint32_t* __restrict__ res, const uint4* __restrict__ gres, uint32_t ngroups,
+                                                           uint32_t* __restrict__ g_entry, uint64_t* __restrict__ g_blockbase,
+                                                           uint32_t* __restrict__ c_entry, uint64_t* __restrict__ c_blockbase,
+                                                           uint64_t* __restrict__ blk_off, uint64_t maxblocks, DecStatus* __restrict__ st,
+                                                           WalkStops stops = WalkStops{}) {
+    seq_walk<T>(in, n, cap, nchunks, res, gres, ngroups, g_entry, g_blockbase, c_entry, c_blockbase, blk_off, maxblocks, st, PairStops<STOP>{stops});
+}
+template <class T>
+__global__ void __launch_bounds__(SW_THREADS) dec_seq_walk_stride(const uint8_t* __restrict__ in, uint64_t n, uint64_t cap, uint32_t nchunks,
+                                                                  const uint32_t* __restrict__ res, const uint4* __restrict__ gres, uint32_t ngroups,
+                                                                  uint32_t* __restrict__ g_entry, uint64_t* __restrict__ g_blockbase,
+                                                                  uint32_t* __restrict__ c_entry, uint64_t* __restrict__ c_blockbase,
+                                                                  DecStatus* __restrict__ st, StrideStops stops) {
+    seq_walk<T>(in, n, cap, nchunks, res, gres, ngroups, g_entry, g_blockbase, c_entry, c_blockbase, nullptr, 0, st, stops);
 }
 
 // ---- 3. the map of a whole byte range (sharded decode of a stream whose cuts are not known) ----------------------------------------
@@ -835,19 +871,28 @@ inline uint32_t rows_launch(const uint8_t* d_in, size_t n_walk, size_t n_visible
 // decoded-size query and the range decode's locate step): a fresh status with nonquiet bit 0 set, which is dec_seq_walk's gate (the
 // little-endian low byte of the word), the candidate rows, then dec_seq_walk, in stop-and-report mode when STOP. Afterwards (on the
 // stream) st->main_blocks / tail_off and the automaton state behind the main loop. 3 kernels; the scratch is bounds_layout<T>(n, 0).
-template <class T, bool STOP = false>
+// STRIDE: dec_seq_walk_stride with the stops `stride` instead (the seek index's build).
+template <class T, bool STOP = false, bool STRIDE = false>
 inline cudaError_t forced_walk_launch(const uint8_t* d_in, size_t n, uint8_t* ws, const BoundsLayout& L, cudaStream_t stream, uint64_t* launches,
-                                      WalkStops stops = WalkStops{}) {
+                                      WalkStops stops = WalkStops{}, StrideStops stride = StrideStops{}) {
     DecStatus* st = reinterpret_cast<DecStatus*>(ws + L.status);
     cudaError_t e = cudaMemsetAsync(st, 0, sizeof(DecStatus), stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(&st->nonquiet, 1, 1, stream);
     if (e != cudaSuccess) return e;
     const uint32_t nchunks = (uint32_t)((n + T::CH - 1) / T::CH);
     const uint32_t ngroups = rows_launch<T>(d_in, n, n, ws, L, stream, launches);
-    dec_seq_walk<T, STOP><<<1, SW_THREADS, 0, stream>>>(
-        d_in, n, ~0ull, nchunks, reinterpret_cast<const uint32_t*>(ws + L.res), reinterpret_cast<const uint4*>(ws + L.gres), ngroups,
-        reinterpret_cast<uint32_t*>(ws + L.g_entry), reinterpret_cast<uint64_t*>(ws + L.g_blockbase), reinterpret_cast<uint32_t*>(ws + L.c_entry),
-        reinterpret_cast<uint64_t*>(ws + L.c_blockbase), nullptr, 0, st, stops);
+    const uint32_t* res = reinterpret_cast<const uint32_t*>(ws + L.res);
+    const uint4* gres = reinterpret_cast<const uint4*>(ws + L.gres);
+    uint32_t* g_entry = reinterpret_cast<uint32_t*>(ws + L.g_entry);
+    uint64_t* g_blockbase = reinterpret_cast<uint64_t*>(ws + L.g_blockbase);
+    uint32_t* c_entry = reinterpret_cast<uint32_t*>(ws + L.c_entry);
+    uint64_t* c_blockbase = reinterpret_cast<uint64_t*>(ws + L.c_blockbase);
+    if constexpr (STRIDE)
+        dec_seq_walk_stride<T><<<1, SW_THREADS, 0, stream>>>(d_in, n, ~0ull, nchunks, res, gres, ngroups, g_entry, g_blockbase, c_entry, c_blockbase,
+                                                             st, stride);
+    else
+        dec_seq_walk<T, STOP><<<1, SW_THREADS, 0, stream>>>(d_in, n, ~0ull, nchunks, res, gres, ngroups, g_entry, g_blockbase, c_entry, c_blockbase,
+                                                            nullptr, 0, st, stops);
     ++*launches;
     return cudaGetLastError();
 }

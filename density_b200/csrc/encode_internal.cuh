@@ -267,6 +267,11 @@ struct RangePlan {
     uint32_t cand0;
     bool final_piece;
     size_t window_ws, ws_bytes;
+    // an indexed piece (index_plan): the piece starts piece_off bytes into the stream and has its carry-in, carry_in (NULL: the stream
+    // start); range_decode_launch then takes d_in at the piece and runs no prefix
+    bool indexed;
+    uint64_t piece_off;
+    const uint32_t* carry_in;
 };
 size_t range_locate_workspace_bytes(size_t nbytes);
 cudaError_t range_locate_launch(const uint8_t* d_in, size_t nbytes, uint64_t first, uint64_t len, uint8_t* ws, uint64_t* d_result,
@@ -274,5 +279,39 @@ cudaError_t range_locate_launch(const uint8_t* d_in, size_t nbytes, uint64_t fir
 bool range_plan(const uint64_t* report, size_t nbytes, uint64_t first, int num_sms, RangePlan* p);
 cudaError_t range_decode_launch(const uint8_t* d_in, const RangePlan& p, uint8_t* ws, int num_sms, cudaStream_t stream, uint64_t* launches,
                                 const uint8_t** d_window);
+
+// The Chameleon seek index (DESIGN §4h, include/density_b200.h): a header of CIDX_HEADER_WORDS u64, a directory of C entries {u64 stream
+// offset, u32 decode candidate, u32 0} padded to 256 bytes (with the header), then C snapshots of 65536 u32 in the shard table format.
+constexpr uint64_t CIDX_MAGIC = 0x58444E494D414843ull;   // "CHAMINDX", little-endian
+constexpr uint64_t CIDX_VERSION = 1, CIDX_HEADER_WORDS = 8, CIDX_SNAPSHOT_BYTES = 65536 * sizeof(uint32_t);
+enum : uint32_t { CIDX_MAGIC_W, CIDX_VERSION_W, CIDX_N_W, CIDX_SIZE_W, CIDX_MAIN_BLOCKS_W, CIDX_INTERVAL_W, CIDX_COUNT_W, CIDX_BYTES_W };
+__host__ __device__ inline uint64_t cidx_snapshots_at(uint64_t count) { return (CIDX_HEADER_WORDS * 8 + 16 * count + 255) & ~255ull; }
+__host__ __device__ inline uint64_t cidx_bytes(uint64_t count) { return cidx_snapshots_at(count) + count * CIDX_SNAPSHOT_BYTES; }
+// the most checkpoints an index of an n-byte stream can have at that interval (0 for an interval that is not a positive multiple of 256)
+uint64_t index_max_count(size_t nbytes, uint64_t interval);
+// Build, d_in 2-byte aligned, nbytes > 0: the locate step (4 kernels, scratch index_locate_workspace_bytes) writes {index bytes, S,
+// verdict} to d_result and leaves index_report_bytes(index_max_count) bytes at the body of the workspace: the same three words, then the
+// header and the directory, copied to h_report. The host waits for them; index_build_plan checks them (false: inconsistent) and sizes the
+// workspace of index_build_launch, which writes the index to d_index (4-byte aligned): the header and the directory from h_report, then
+// density_b200_table_init's state and per piece j = 0 .. C - 1 (j > 0: entered at checkpoint j's candidate) phase 1 with its table
+// exported and a fold into snapshot j + 1: 14 C kernels (with the locate step, 4 + 14 C).
+size_t index_report_bytes(uint64_t cmax);
+size_t index_locate_workspace_bytes(size_t nbytes, uint64_t interval);
+cudaError_t index_locate_launch(const uint8_t* d_in, size_t nbytes, uint64_t interval, uint8_t* ws, uint64_t* d_result, uint64_t* h_report,
+                                cudaStream_t stream, uint64_t* launches);
+bool index_build_plan(const uint64_t* report, size_t nbytes, int num_sms, size_t* ws_bytes);
+cudaError_t index_build_launch(const uint8_t* d_in, const uint64_t* report, uint8_t* ws, uint8_t* d_index, int num_sms, cudaStream_t stream,
+                               uint64_t* launches);
+// Indexed range decode. index_count_for_bytes: the C whose layout is index_len bytes long (~0: none). index_check: NULL when the header
+// and directory (host copy) are consistent with the stream length and index_len, else why not. index_plan: the piece of a window
+// (false: first >= S, nothing to decode) and the checkpoint whose snapshot is its carry-in (0: none). range_table_slot: where a snapshot
+// from host memory is staged. index_copy_out_launch: 1 kernel, the checked copy of the window to d_out (NULL: only the check) and the
+// result words.
+uint64_t index_count_for_bytes(uint64_t index_len);
+const char* index_check(const uint64_t* hdr, size_t nbytes, uint64_t index_len, uint64_t count);
+bool index_plan(const uint64_t* hdr, size_t nbytes, uint64_t first, uint64_t len, int num_sms, RangePlan* p, uint64_t* snapshot);
+uint32_t* range_table_slot(uint8_t* ws);
+cudaError_t index_copy_out_launch(const RangePlan& p, const uint8_t* d_window, uint64_t size, uint8_t* d_out, uint8_t* ws, uint64_t* d_result,
+                                  int num_sms, cudaStream_t stream, uint64_t* launches);
 
 }  // namespace dns

@@ -179,6 +179,69 @@ DENSITY_B200_API int density_b200_chameleon_decode_range(const uint8_t* input, s
                                                          uint64_t* written);
 
 /*
+ * Chameleon seek index: the state a range decode needs in front of a window, recorded once per stream at fixed checkpoints, so that a
+ * range decode reads and decodes only the stream between two checkpoints, at the same cost wherever the window is and however long the
+ * stream is. A host-resident stream then sends only that piece over PCIe.
+ *
+ * Format (version 1). One contiguous, position-independent blob with no pointers in it, so it can be stored beside the stream and
+ * loaded again; a pure function of (stream, interval). All fields little-endian.
+ *   - header, 8 x u64: magic "CHAMINDX" (0x58444E494D414843), version 1, n (stream bytes), S (decoded size), main_blocks (the blocks of
+ *     the decoder's main loop), interval (decoded bytes between checkpoints, a positive multiple of 256; I = interval / 256 blocks), C
+ *     (the checkpoint count) and the index's length in bytes;
+ *   - checkpoints at blocks j x I, j = 1 .. C, with C x I < main_blocks (every checkpoint is inside the main loop; the stream start is
+ *     the implicit checkpoint 0);
+ *   - directory, C entries of 16 bytes {u64 stream offset of block j x I, u32 decode candidate (the automaton state in front of it, < 3200,
+ *     as the sharded decode numbers them), u32 0}; the header and the directory together are padded with zeros to a multiple of 256 bytes;
+ *   - snapshots, C x 65536 u32 (256 KiB each) in the shard table format (bit 16 touched, bits 0-15 fingerprint): snapshot j is
+ *     density_b200_table_init's state folded with the last-writer tables of the pieces in front of checkpoint j, the dictionary in front
+ *     of block j x I.
+ * Length: ceil256(64 + 16 C) + 262144 C bytes.
+ */
+/* An upper bound of the index's length for any stream of n bytes at that interval (from n alone: the largest block count n bytes can
+   hold); 0 when the interval is not a positive multiple of 256. */
+DENSITY_B200_API uint64_t density_b200_chameleon_index_bytes(size_t n, uint64_t interval);
+/* Builds the index of d_in[0 .. n) (device, 2-byte aligned, n > 0) into d_index (device, 4-byte aligned, index_cap bytes). d_result
+   (device, 8-byte aligned) receives three u64 {index bytes, S, verdict}. On a malformed stream (in the sense of density_b200_decoded_size)
+   it returns DENSITY_B200_EMALFORMED with d_result = {0, 0, DENSITY_B200_EMALFORMED} and writes nothing to d_index. The call enqueues a
+   boundary walk of the whole stream that stops at every checkpoint (4 kernels) and waits on `stream` for it; then 14 C kernels: per
+   piece between checkpoints, its writer pass and a fold into the next snapshot. DENSITY_B200_EARG (index_cap <
+   density_b200_chameleon_index_bytes(n, interval), n == 0, a bad interval, a NULL or misaligned pointer) enqueues nothing. The call uses
+   the device's shared workspace (see "Concurrent callers" above): the boundary rows of the stream, then a decode workspace for one piece. */
+DENSITY_B200_API int density_b200_chameleon_index_build_device(const uint8_t* d_in, size_t n, uint64_t interval, uint8_t* d_index, size_t index_cap,
+                                                               uint64_t* d_result, void* stream);
+/* Synchronous; host or device pointers of any alignment. DENSITY_B200_OK with *index_len set, DENSITY_B200_EMALFORMED, DENSITY_B200_EARG
+   or DENSITY_B200_ECUDA. */
+DENSITY_B200_API int density_b200_chameleon_index_build(const uint8_t* input, size_t n, uint64_t interval, uint8_t* index, size_t index_cap,
+                                                        uint64_t* index_len);
+/*
+ * Indexed range decode: the contract of density_b200_chameleon_decode_range_device (d_out gets D[first : first + w] and nothing outside
+ * [d_out, d_out + w), d_result = {w, S, verdict}), from the piece of the stream between the checkpoint at or in front of block first / 256
+ * and the first checkpoint behind the window's last block (or the stream end when there is none, or the window reaches the main loop's
+ * end or S). The piece is entered at its checkpoint's candidate with its snapshot as the carry-in, read in place from d_index.
+ *   - The call first copies the header and the directory to the host (one copy, one wait on `stream`) and checks them: the magic, the
+ *     version, n, index_len against the layout for C, the interval, offsets even, strictly increasing and < n, candidates < 3200,
+ *     C x I < main_blocks and 256 main_blocks <= S <= 256 main_blocks + 528. A failure is DENSITY_B200_EARG: no kernel runs and nothing is
+ *     written to d_out or d_result.
+ *   - S and the verdict come from the index: a stream is not walked again. The decoded piece must have the size the index promises for
+ *     it, (c_b - c_a) x interval, or S - 256 c_a I for the final piece; otherwise the call writes {0, S, DENSITY_B200_EMALFORMED} and
+ *     leaves d_out untouched. That catches an index that does not match its stream. An index of another stream with the same structure
+ *     (the same block boundaries and automaton states) is not caught: as with a wrong capacity, that is the caller's error. It never
+ *     makes the call read or write outside the stream, the index, d_out or the workspace.
+ *   - Kernels: 15 whenever w > 0 (the entry, the piece's phase 1 and phase 2, the checked copy), wherever the window is; 1 when first >= S
+ *     (the result words). Workspace: the decode of the piece, at most the window plus 2 x interval of output; nothing grows with n.
+ * Stream-ordered: d_in device, 2-byte aligned; d_index device, 4-byte aligned; d_out device, any alignment; d_result device, 8-byte
+ * aligned. n == 0 or len == 0: no kernel, {0, 0, 0} by a memset (the index is not read).
+ */
+DENSITY_B200_API int density_b200_chameleon_decode_range_indexed_device(const uint8_t* d_in, size_t n, const uint8_t* d_index, size_t index_len,
+                                                                        uint64_t first, uint64_t len, uint8_t* d_out, uint64_t* d_result,
+                                                                        void* stream);
+/* Synchronous; host or device pointers of any alignment for the stream, the index and the output. A host stream is staged only from
+   the piece's first byte to its last; a host index only for its header, its directory and the one snapshot the piece starts from.
+   DENSITY_B200_OK with *written = w, DENSITY_B200_EMALFORMED (*written = 0), DENSITY_B200_EARG or DENSITY_B200_ECUDA. */
+DENSITY_B200_API int density_b200_chameleon_decode_range_indexed(const uint8_t* input, size_t n, const uint8_t* index, size_t index_len,
+                                                                 uint64_t first, uint8_t* output, uint64_t len, uint64_t* written);
+
+/*
  * Sharded encode. Every entry of the phase APIs of a Chameleon, Cheetah or Lion shard below, density_b200_table_init / _fold,
  * density_b200_cl_table_init / _fold and every density_b200_encode_sharded* driver takes its pointers by one rule: d_in and d_prev_quad
  * 4-byte aligned; d_out 2-byte aligned; every table, carry, transfer, word and flag buffer 4-byte aligned; d_out_size and d_total_size
